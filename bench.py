@@ -1,13 +1,13 @@
 #!/usr/bin/env python
-"""bench.py -- pages/sec of the comic-text-detector hot path on N B200s (driver contract).
+"""bench.py -- pages/sec of the comic-text-detector hot path on N H100s.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--batch B]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--batch B] [--dump-outputs DIR]
 
 A "step" = one pass of the WHOLE hot path -- everything `TextDetector.__call__` does (reference
 inference.py:141-178): backbone + seg head + DB head + Detect decode + NMS + mask u8 + DB threshold + connected
 components + text-line boxes/scores (device, one CUDA graph), postprocess_yolo casts + box_thresh + group_output
 (host C++, the engine's worker thread), refine_mask (device, on the resident pages) -- over one batch of B
-synthetic 1024x1024 pages per GPU (BASELINE.json configs[2]/[3]: batch 16 per GPU, fp16 tcgen05 path).
+synthetic 1024x1024 pages per GPU (BASELINE.json configs[2]/[3]: batch 16 per GPU, fp16 tensor-core path).
 
 * value      : whole-job pages/s with the pages already resident in HBM (ctd_submit_full with pages_on_device);
                --engines E (default 2) workspaces per GPU x two batches in flight each; timed with CUDA events on
@@ -17,15 +17,18 @@ synthetic 1024x1024 pages per GPU (BASELINE.json configs[2]/[3]: batch 16 per GP
                timed region; at N > 1 also the NCCL gather of every rank's result arena to rank 0 and rank 0's D2H of
                the gathered arenas.
 * net_only   : the round-1 step (network + NMS + CCL + line boxes, no group_output / refine_mask), for comparison.
-* roofline   : tensor roofline of the tcgen05 convolution kernels: algorithmic conv FLOPs / summed device time of
-               the conv launches (per-op CUDA events, serial order, each kernel timed ALONE at boost clocks ->
-               MEASURED_PEAKS.json bf16_tflops, the burst figure); `whole_step_frac` divides the algorithmic FLOPs
-               by the whole timed net_only step against the same peak.
+* roofline   : tensor roofline of the wgmma convolution kernels: algorithmic conv FLOPs / summed device time of
+               the conv launches (per-op CUDA events, serial order) against the H100 SXM data-sheet dense FP16 rate
+               (989.4 TFLOP/s at 700 W; a power-limited card reaches less); `whole_step_frac` divides the algorithmic
+               FLOPs by the whole timed net_only step against the same peak.
 * config2 / config5 / api_e2e : BASELINE configs[1] (batch 1, fp32-accurate engines) and configs[4] (mixed
                640/1024/1536 stream) and the drop-in Python class, measured on rank 0 at N = 1.
 * cpu_baseline / --impl reference: the oracle restatement of the reference's CPU path for the SAME stages
                (oracle/net_ref.py + oracle/postproc_ref.py + oracle/textblock_ref.py + oracle/pipeline_ref.py: torch
-               CPU fp32 + torchvision + cv2 + numpy, i.e. the reference's own library calls) on this box's host cores.
+               CPU fp32 + torchvision + cv2 + numpy, i.e. the reference's own library calls) on the host's cores.
+* --dump-outputs DIR: after the timed steps, the results of the last timed step (what ctd_submit_full delivers to
+               its caller) as DIR/<name>.npy (float32 values, float64 indices and counts); the two full-page u8 masks as a fixed
+               seeded sample of pixels.
 """
 import argparse
 import json
@@ -41,6 +44,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 GFLOP_PER_PAGE_1024 = 191.414  # BASELINE.md section 2 (2*MAC over the 115 conv/deconv layers)
+H100_FP16_DENSE_TFLOPS = 989.4  # NVIDIA H100 SXM data sheet, dense FP16 tensor rate at 700 W
 
 
 def conv_flops(prog, n, h, w):
@@ -50,10 +54,6 @@ def conv_flops(prog, n, h, w):
         kind = o["kind"]
         if kind == 0:  # stem: 6x6 s2 conv 3 -> cout (algorithmic FLOPs, not the zero-padded tensor-core K)
             out.append(2.0 * (h // 2) * (w // 2) * n * 108 * o["cout"])
-            continue
-        if kind == 10:  # fused Bottleneck: 1x1 c -> c plus 3x3 c -> c on the same pixels
-            down = prog.bufs[o["src_buf"][0]][1]
-            out.append(2.0 * (h // down) * (w // down) * n * 10 * o["cout"] * o["cout"])
             continue
         if kind not in (1, 2, 6, 7):
             out.append(0.0)
@@ -72,7 +72,7 @@ def conv_flops(prog, n, h, w):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -175,9 +175,9 @@ def main():
     ap.add_argument("--engines", type=int, default=2, help="workspaces per GPU; consecutive batches alternate between them")
     ap.add_argument("--sustain-steps", type=int, default=150, help="steps of the seconds-long sustained measurement (0 = skip)")
     ap.add_argument("--api-pages", type=int, default=8, help="pages timed through the TextDetector Python API (0 = skip)")
-    ap.add_argument("--cpu-threads", type=int, default=16,
-                    help="torch intra-op threads of the CPU arm (measured on the B200 host: 16 threads 0.25 s/forward, "
-                         "64 threads 0.48 s, 128 threads 33 s -- more threads only hurt)")
+    ap.add_argument("--cpu-threads", type=int, default=16, help="torch intra-op threads of the CPU arm")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the results of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -199,7 +199,7 @@ def main():
     warm = max(3, args.warmup)
 
     ck = synth.make_checkpoint(0, smooth=True)
-    prog = ctd_b200.compiler.compile_checkpoint(ck, fuse=ctd_b200.compiler.fuse_default(True))
+    prog = ctd_b200.compiler.compile_checkpoint(ck)
     n_eng = max(1, args.engines)
     engs = [ctd_b200.Engine(prog, device=local, max_batch=B, max_h=H, max_w=W, use_graph=True) for _ in range(n_eng)]
     eng = engs[0]
@@ -306,6 +306,9 @@ def main():
         sampler.start()
     ms = timed(step_full, args.steps, drain_full)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        k = state["k"] - 1   # the last timed step; its arena is complete after drain_full
+        dump_outputs(args.dump_outputs, out_arena[k % n_eng][(k // n_eng) & 1].numpy(), lay, B, H, W)
     state["on_device"] = False
     for _ in range(2 * n_eng):
         step_full()
@@ -365,29 +368,12 @@ def main():
     op_ms2, _, _ = eng.profile_forward(dev_ptr=dev_pages.data_ptr(), shape=(B, H, W))
     op_ms = np.minimum(op_ms, op_ms2)
     fl = conv_flops(prog, B, H, W)
-    tc_idx = [i for i, o in enumerate(prog.ops) if o["kind"] in (0, 1, 2, 6, 7, 10)]
+    tc_idx = [i for i, o in enumerate(prog.ops) if o["kind"] in (0, 1, 2, 6, 7)]
     tc_ms = float(sum(op_ms[i] for i in tc_idx))
     tc_flops = float(sum(fl[i] for i in tc_idx))
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    # each conv kernel is timed ALONE between events (sub-millisecond bursts at boost clock) -> burst peak
-    peak_tf = float(peaks.get("bf16_tflops", 1676.8))
-    peak_src = ("MEASURED_PEAKS.json bf16_tflops (burst: kernels timed in isolation)" if peaks
-                else "fallback 1676.8 TFLOP/s burst (B200_PROFILING.md)")
+    peak_tf = H100_FP16_DENSE_TFLOPS
+    peak_src = "H100 SXM data sheet, dense FP16 at 700 W (not a measured rate)"
     achieved = tc_flops / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
-    traffic, traffic_src = None, None
-    for name in ("r02_conv_traffic.json", "r01_conv_traffic.json"):
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", name)))
-            if int(tj.get("batch", 0)) == B:
-                traffic = float(tj["dram_bytes"])
-                traffic_src = "profiles/%s (ncu dram__bytes_read.sum + dram__bytes_write.sum over the %d conv launches of one step)" % (name, int(tj["launches"]))
-                break
-        except Exception:
-            pass
 
     if rank == 0:
         total_pages = B * world * args.steps
@@ -400,29 +386,27 @@ def main():
             "steps": args.steps, "warmup": warm, "ms_per_step": ms / args.steps,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "fp16",
             "data": "synthetic",
-            "config": {"workload": "BASELINE configs[2]: 1024x1024 pages, batch %d per GPU, fp16 tcgen05 path, FULL pipeline of "
+            "config": {"workload": "BASELINE configs[2]: 1024x1024 pages, batch %d per GPU, fp16 wgmma path, FULL pipeline of "
                                    "TextDetector.__call__ (backbone + seg head + DB head + Detect/NMS + mask u8 + DB threshold + CCL + "
                                    "contour boxes/scores on the device, group_output in host C++, refine_mask on the device)" % B,
                        "pages_per_gpu_per_step": B, "page": [H, W], "checkpoint": "synthetic seed 0 (oracle/synth.py)",
-                       "l2": "activations per step (~%.1f GB) exceed the 126 MB L2; no explicit flush" % (
+                       "l2": "activations per step (~%.1f GB) exceed the 50 MB L2; no explicit flush" % (
                            sum(c * (H // d) * (W // d) for c, d in prog.bufs) * 2 * B / 1e9),
                        "cuda_graph": True, "engines_per_gpu": n_eng,
-                       "fused_ops": "5 fused Bottleneck kernels + seg tail as GEMM + col2im (bit-identical / fp32-rounding-equal to the unfused program)",
                        "in_flight": "%d batches per GPU (%d workspaces x 2 slots)" % (2 * n_eng, n_eng),
                        "multi_gpu": ("pages sharded B per rank; one NCCL gather of each rank's complete result arena to rank 0 per step"
                                      if world > 1 else "single GPU")},
             # forward graph (convs + thin ops + NMS / CCL / contour kernels) + copies + the 29 refine_mask launches of a batch
             "gpu_launches": (eng.last_launch_count() + 6 + 29) * args.steps,
             "clocks": clocks,
-            "conv_roofline_frac_of_nominal": net_val / world * GFLOP_PER_PAGE_1024 * 1e9 / 2.25e15,
+            "conv_roofline_frac_of_nominal": net_val / world * GFLOP_PER_PAGE_1024 * 1e9 / (H100_FP16_DENSE_TFLOPS * 1e12),
             "e2e": {"value": e2e_val, "unit": "pages/s", "h2d_bytes_per_step": int(B * H * W * 3), "d2h_bytes_per_step": d2h,
                     "mode": "ctd_submit_full/ctd_collect on %d engine(s) per GPU, two batches in flight per engine, pinned host buffers%s"
                             % (n_eng, "; + NCCL gather of all ranks' arenas and rank 0's D2H of them" if world > 1 else "")},
             "net_only": {"value": net_val, "unit": "pages/s", "ms_per_step": ms_net / args.steps,
                          "what": "round-1 step: network + NMS + CCL + line boxes only (ctd_forward on resident pages), no group_output / refine_mask"},
-            "roofline": {"bound": "tensor", "kernel": "conv_tc / conv_halo / conv_hs / conv_sw / conv_bneck kernels, the tcgen05 implicit-GEMM convolutions (%d launches per step)" % len(tc_idx),
+            "roofline": {"bound": "tensor", "kernel": "conv_tc_kernel, the wgmma implicit-GEMM convolutions (%d ops per step)" % len(tc_idx),
                          "achieved": achieved, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved / peak_tf,
-                         "traffic": traffic, "traffic_unit": "bytes/step", "traffic_source": traffic_src,
                          "peak_source": peak_src, "flops_per_step": tc_flops, "ms_per_step": tc_ms,
                          "share_of_step": tc_ms / float(op_ms.sum() + nms_ms + ccl_ms),
                          "whole_step_frac": (GFLOP_PER_PAGE_1024 * 1e9 * B) / (ms_net / args.steps * 1e-3) / 1e12 / peak_tf,
@@ -454,6 +438,38 @@ def main():
     if dist is not None:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, arena, lay, B, H, W):
+    """The results ctd_submit_full delivered for one batch, as .npy files (at most ~16 MB for B = 16): values in
+    float32, pixel indices and counts in float64 (exact at any batch).  Variable-length lists are zero-padded to their
+    fixed capacity, with the counts stored beside them; the u8 masks are sampled at 1M fixed pixel positions (seed 0)."""
+    from ctd_b200 import multigpu
+    os.makedirs(out_dir, exist_ok=True)
+    a = multigpu.unpack_arena(arena, lay, B, H, W, full=True)
+    f32 = lambda v: np.asarray(v, dtype=np.float32)
+    idx = np.random.default_rng(0).choice(B * H * W, size=min(B * H * W, 1 << 20), replace=False)
+    idx.sort()
+    out = {"mask_u8_sample": a["mask"].reshape(-1)[idx], "mask_refined_sample": a["mask_refined"].reshape(-1)[idx],
+           "mask_sample_index": idx, "n_labels": a["n_labels"]}
+    det = np.zeros((B, 300, 6), np.float32)
+    lbox = np.zeros((B, 1000, 4, 2), np.float32)
+    lsc = np.zeros((B, 1000), np.float32)
+    for i in range(B):
+        det[i, :len(a["det"][i])] = a["det"][i]
+        lbox[i, :len(a["line_boxes"][i])] = a["line_boxes"][i]
+        lsc[i, :len(a["line_scores"][i])] = a["line_scores"][i]
+    out.update(det=det, det_count=[len(d) for d in a["det"]], line_boxes=lbox, line_scores=lsc,
+               line_count=[len(v) for v in a["line_scores"]])
+    nb = max([len(b) for b in a["blocks"]] + [1])
+    blk = np.zeros((B, nb, 7), np.float32)   # x1 y1 x2 y2 vertical angle n_lines
+    for i, bl in enumerate(a["blocks"]):
+        for j, b in enumerate(bl):
+            blk[i, j] = list(b.xyxy[:4]) + [float(bool(b.vertical)), float(b.angle), float(len(b.lines))]
+    out.update(blocks=blk, block_count=[len(b) for b in a["blocks"]])
+    exact = ("mask_sample_index", "n_labels", "det_count", "line_count", "block_count")
+    for name, v in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(v, np.float64) if name in exact else f32(v))
 
 
 def extras(line, args, ck, prog, pages, local):

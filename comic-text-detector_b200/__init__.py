@@ -1,6 +1,6 @@
-"""comic-text-detector_b200: B200-native engine behind the reference's inference path
+"""comic-text-detector_b200: H100-native engine behind the reference's inference path
 (page -> block boxes + text-line map + segmentation mask).  Import as `ctd_b200`
-(the directory name carries a hyphen; /root/repo/ctd_b200.py aliases it)."""
+(the directory name carries a hyphen; ctd_b200.py at the repository root aliases it)."""
 from . import compiler  # noqa: F401
 from .binding import Engine, CtdError, load_library, LIB_PATH  # noqa: F401
 from . import binding, multigpu, textblock  # noqa: F401

@@ -1,4 +1,4 @@
-"""Annotation writer on top of the B200 detector: the on-disk formats of the reference's batch tool
+"""Annotation writer on top of the H100 detector: the on-disk formats of the reference's batch tool
 `model2annotations` (inference.py:19-70) --
 
   <name>.txt        YOLO labels of the text blocks: "1 cx cy w h" per block, normalised, '\\n'-joined without a

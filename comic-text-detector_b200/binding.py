@@ -1,6 +1,6 @@
 """ctypes binding of libctd_b200.so (include/ctd_b200.h).  Thin: numpy arrays in/out, every
 non-zero return code becomes a Python exception carrying ctd_last_error().  There is no CPU
-fallback: if the library is missing or no sm_100 GPU is visible, construction raises."""
+fallback: if the library is missing or no sm_90 GPU is visible, construction raises."""
 import ctypes as C
 import os
 

@@ -16,8 +16,7 @@ import numpy as np
 
 # enum mirrors of include/ctd_b200.h
 (OP_STEM, OP_CONV, OP_DECONV4, OP_AVGPOOL2, OP_SPPF_POOL, OP_UPSAMPLE2, OP_DETECT, OP_SEG_TAIL, OP_DB_TAIL,
- OP_S2D, OP_BNECK) = range(11)
-FUSED_BNECK_CHANNELS = (32, 64)   # c_ the fused Bottleneck kernel (csrc/conv_fuse.cu) is built for
+ OP_S2D) = range(10)
 ACT_NONE, ACT_SILU, ACT_LEAKY, ACT_RELU, ACT_SIGMOID = range(5)
 MAX_SRC = 3
 
@@ -151,19 +150,6 @@ class Program:
         self._op(OP_DECONV4, srcs, dst, ksize=4, stride=2, act=act, **self._pack(wk, b, co))
         return dst
 
-    def bneck(self, src, w1, b1, w2, b2, act, residual):
-        """Fused Bottleneck (common.py:94-104): dst = [src +] act(conv3x3(act(conv1x1(src)))) into a NEW buffer
-        (the fused kernel reads the halo of src while neighbouring tiles write dst).  Blob: W1 [c][c] then W2 [c][9c]
-        (K order (ky, kx, ci)), fp16 and fp32; bias1 | bias2."""
-        c = w1.shape[0]
-        assert w1.shape == (c, c, 1, 1) and w2.shape == (c, c, 3, 3) and src["c"] == c
-        dst = self.tensor(self.newbuf(c, src["down"]), 0, c)
-        wk = np.concatenate([w1.reshape(c, c).reshape(-1), w2.transpose(0, 2, 3, 1).reshape(-1)]).astype(np.float32)
-        bb = np.concatenate([b1, b2]).astype(np.float32)
-        self._op(OP_BNECK, [src], dst, ksize=3, stride=1, act=act, residual=int(residual), cout=c, cout_pad=c,
-                 w16_off=self.add_blob(wk.astype(np.float16)), w32_off=self.add_blob(wk), b_off=self.add_blob(bb))
-        return dst
-
     def detect(self, src, w, b, level, stride, anchors_px):
         co = w.shape[0]
         wk = w.reshape(1, co, -1)
@@ -185,16 +171,8 @@ def fold_bn(w, conv_bias, sd, bn_prefix, eps, transposed=False):
     return wf, (b0 - mu) * scale + beta
 
 
-def fuse_default(fp16_tc):
-    """Whether a caller that builds the fp16 tensor-core engine should ask for fused ops (CTD_FUSE=0 turns it off)."""
-    import os
-    return bool(fp16_tc) and os.environ.get("CTD_FUSE", "1") != "0"
-
-
-def compile_checkpoint(ckpt, head_act="leaky", stem_mode="s2d", fuse=False):
-    """Returns a Program for the full TextDetBase.forward graph (basemodel.py:240-244).  fuse=True emits the
-    Bottlenecks with 32 / 64 channels as ONE op each (OP_BNECK, fp16 tensor-core engine only): same arithmetic and
-    the same fp16 storage points as the two-op form, so the results are bit-identical."""
+def compile_checkpoint(ckpt, head_act="leaky", stem_mode="s2d"):
+    """Returns a Program for the full TextDetBase.forward graph (basemodel.py:240-244)."""
     P = Program()
     cfg = ckpt["blk_det"]["cfg"]
     ysd, ssd, dsd = ckpt["blk_det"]["weights"], ckpt["text_seg"], ckpt["text_det"]
@@ -219,9 +197,6 @@ def compile_checkpoint(ckpt, head_act="leaky", stem_mode="s2d", fuse=False):
         for j in range(n):
             wa, ba = get("%s.m.%d.cv1" % (prefix, j))
             wb, bb = get("%s.m.%d.cv2" % (prefix, j))
-            if fuse and c_ in FUSED_BNECK_CHANNELS and act != ACT_SIGMOID:
-                cur = P.bneck(cur, wa, ba, wb, bb, act, bool(shortcut))
-                continue
             t = P.conv([cur], wa, ba, 1, act)
             # Bottleneck (common.py:103-104): x + cv2(cv1(x)), written in place over x
             P.conv([t], wb, bb, 1, act, dst=cur, residual=bool(shortcut))
@@ -329,7 +304,7 @@ def compile_checkpoint(ckpt, head_act="leaky", stem_mode="s2d", fuse=False):
                 for dx, kx in TAPS[px]:
                     wc[py * 2 + px, dy + 1, dx + 1, :] = w6[:, 0, ky, kx]
     # b_off (the layer has no bias): the same weights as a 1x1 GEMM over the 16 kernel positions, [ky*4+kx][ci] fp16, for the
-    # GEMM + col2im form of the tail (csrc/conv_fuse.cu)
+    # GEMM + col2im form of the tail
     P._op(OP_SEG_TAIL, [u512], None, p_off=P.add_blob(w6.reshape(w6.shape[0], 16).astype(np.float32)),
           w16_off=P.add_blob(wc.reshape(16, 9 * ci6).astype(np.float16)), cout=4, cout_pad=16,
           b_off=P.add_blob(np.ascontiguousarray(w6.reshape(ci6, 16).T).astype(np.float16)))

@@ -1,30 +1,20 @@
-// tcgen05 implicit-GEMM convolutions for sm_100a: four kernels on one skeleton.
+// wgmma implicit-GEMM convolution for sm_90a.
 //
-//   D[128 x N] (fp32, TMEM) += A[128 x 16] * B[N x 16]^T, K-major fp16 operands in 128B/64B/32B-swizzled shared memory
+//   D[128 x BN] (fp32, registers) += A[128 x 16] * B[BN x 16]^T, K-major fp16 operands in 128B/64B/32B-swizzled shared
+//   memory; the 128 rows are a 16x8-pixel tile, the BN columns a slice of output channels
 //
-// Skeleton (all kernels): persistent, one CTA per SM; warp 0 = TMA producer (one elected thread), warp 1 = ONE thread
-// issuing tcgen05.mma cta_group::1 kind::f16 (M=128, K=16) in a straight-line loop (issue_kblock: descriptors are
-// precomputed and advanced with 64-bit adds), warp 2 = TMEM allocator, warps 4-11 = two epilogue warpgroups on
-// alternate tiles (tcgen05.ld 32x32b -> bias + activation (+ residual) -> fp16); mbarrier full/empty rings between
-// the roles, tcgen05.commit frees ring slots and publishes accumulators, a ring of TMEM accumulator stages lets the
-// epilogue of tile i run under the main loop of the following tiles; >= 64-channel slices leave through a swizzled
-// staging tile and one TMA store per 64 channels.  Activations are 4-D TMA boxes over the NHWC buffers: out-of-bounds
-// zero-fill IS the convolution padding, there is no im2col buffer; torch.cat inputs are K-concatenated from up to
-// 3 tensor maps; ConvTranspose 4x4 s2 p1 runs as 4 sub-pixel phases of 2x2 taps.
-//
-//   conv_tc_kernel<BN>    one 16x8-pixel x 64-channel box per (tap, K block) + the matching weight box; stride 2
-//                         through four parity maps; Detect heads decode sigmoid / boxes in the epilogue
-//   conv_halo_kernel<BN>  weights RESIDENT in smem; one halo box per K block, every filter tap is a matrix-descriptor
-//                         view into it (start row (dy+1)*W+(dx+1), SBO = W rows, base_offset 0); 3x3 s1/s2, deconv
-//                         phases, 1x1, the stem (window map over the space-to-depth page) and the seg tail (BN=16)
-//   conv_hs_kernel<BN>    halo activations + weights STREAMED through their own ring (BN = 128 / 256)
-//   conv_sw_kernel        operands swapped for 128 output channels: weights are the M=128 operand, 256 pixels (8x32
-//                         tile, halo views) the N operand; channel-major accumulators, transposed epilogue
+// Persistent, one CTA per SM, 384 threads: warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 =
+// consumers, each issuing wgmma m64nBNk16 for its 64 rows of the tile (4 of the 8 pixel rows) and running the epilogue
+// on its own accumulators.  An mbarrier full/empty ring of operand stages sits between producer and consumers; each
+// consumer keeps one wgmma group in flight and frees the stage of the previous group once that group has retired.
+// Activations are 4-D TMA boxes over the NHWC buffers: out-of-bounds zero-fill IS the convolution padding, there is
+// no im2col buffer; torch.cat inputs are K-concatenated from up to 3 tensor maps; stride 2 reads four parity maps;
+// ConvTranspose 4x4 s2 p1 runs as 4 sub-pixel phases of 2x2 taps; Detect heads decode sigmoid / boxes in the epilogue.
 //
 // Reference semantics: Conv.forward_fuse (models/yolov5/common.py:48-49), Bottleneck add (common.py:104),
-// ConvTranspose2d+BN+ReLU (basemodel.py:26-28), Detect (yolo.py:23-44), UnetHead's final ConvT + Sigmoid
-// (basemodel.py:57-60) + postprocess_mask (inference.py:96-99).
+// ConvTranspose2d+BN+ReLU (basemodel.py:26-28), Detect (yolo.py:23-44).
 #include <cstdlib>
+#include <cstring>
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -35,25 +25,16 @@
 namespace ctd {
 
 constexpr int kTileW = 16, kTileH = 8;  // 128 grid pixels per tile
-constexpr int kThreads = 384;           // warp 0 TMA, warp 1 MMA, warp 2 TMEM alloc, warps 4-11 epilogue
-constexpr int kEpiWarp0 = 4;
+constexpr int kThreads = 384;           // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
 
 template <int BN>
 struct TcCfg {
   static constexpr int kABytes = 128 * 128;  // per stage (worst case 128-byte rows)
   static constexpr int kBBytes = BN * 128;
-  // one persistent CTA per SM.  The streamed-operand layers run at (bytes in flight per SM) / (loaded L2 latency, ~2 us):
-  // the operand ring takes every byte the other regions leave (192 KB: 4 x 48 KB at BN = 256, was 3), which is why the
-  // layout below has no alignment slack (the dynamic shared-memory base is 1024-byte aligned, checked at kernel start)
-  static constexpr int kStages = BN >= 256 ? 4 : (BN >= 128 ? 6 : (BN >= 64 ? 8 : 10));
-  static constexpr int kStoreBytes = BN >= 64 ? 2 * 128 * 128 : 0;      // one 128x64 fp16 staging tile per epilogue warpgroup
-  // TMEM accumulator stages (512 columns per SM): small tiles get a deep ring so that two epilogue warpgroups
-  // can drain two tiles at once while the MMA warp runs ahead
-  static constexpr int kAccStages = BN >= 256 ? 2 : (BN >= 128 ? 4 : 8);
-  static constexpr int kTmemCols = BN * kAccStages < 32 ? 32 : BN * kAccStages;   // power of two >= 32
+  static constexpr int kStages = BN >= 128 ? 6 : (BN >= 64 ? 8 : 10);
   static constexpr int kBiasFloats = 512;
-  // operand ring | store staging (1024-aligned: the ring is a multiple of 1024) | barriers (512 B) | bias
-  static constexpr size_t kSmem = size_t(kStages) * (kABytes + kBBytes) + kStoreBytes + 512 + kBiasFloats * 4;
+  // 1024 bytes of alignment slack | operand ring | barriers (256 B) | bias
+  static constexpr size_t kSmem = 1024 + size_t(kStages) * (kABytes + kBBytes) + 256 + kBiasFloats * 4;
   static_assert(kSmem <= 227 * 1024, "conv_tc_kernel: shared memory");
 };
 
@@ -77,212 +58,80 @@ __device__ __forceinline__ float apply_act_precise(float v) {
   else return v;
 }
 
-// Split-fp16 mode epilogue: `ncols` (multiple of 4, <= 32) accumulator columns -> bias + activation (+ fp32 residual
-// read from the destination) -> FP32 NHWC, 16-byte stores.
-template <int ACT>
-__device__ __forceinline__ void epilogue_chunk_f32(const uint32_t* v, const float* __restrict__ bias_s,
-                                                   float* __restrict__ out, int ncols, bool residual) {
-#pragma unroll
-  for (int q = 0; q < 8; ++q) {
-    if (q * 4 >= ncols) break;
-    const float4 b = *reinterpret_cast<const float4*>(bias_s + q * 4);
-    float4 o;
-    o.x = apply_act_precise<ACT>(__uint_as_float(v[q * 4 + 0]) + b.x);
-    o.y = apply_act_precise<ACT>(__uint_as_float(v[q * 4 + 1]) + b.y);
-    o.z = apply_act_precise<ACT>(__uint_as_float(v[q * 4 + 2]) + b.z);
-    o.w = apply_act_precise<ACT>(__uint_as_float(v[q * 4 + 3]) + b.w);
-    if (residual) {
-      const float4 r = *reinterpret_cast<const float4*>(out + q * 4);
-      o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+template <int BN>
+__device__ __forceinline__ void wgmma_bn(float (&d)[BN / 2], uint64_t ad, uint64_t bd, uint32_t acc) {
+  if constexpr (BN == 128) wgmma_n128(d, ad, bd, acc);
+  else if constexpr (BN == 64) wgmma_n64(d, ad, bd, acc);
+  else if constexpr (BN == 32) wgmma_n32(d, ad, bd, acc);
+  else wgmma_n16(d, ad, bd, acc);
+}
+
+// Epilogue of one accumulator row pair (columns col, col + 1) of an fp16 destination: bias + activation (+ residual)
+// -> fp16.  `out` / `res` point at channel 0 of this tile's N block for the pixel; columns >= ncols are not written.
+template <int ACT, bool RES>
+__device__ __forceinline__ void epi_pair_f16(float v0, float v1, const float* __restrict__ bias_s, int col,
+                                             __half* __restrict__ out, const __half* __restrict__ res, int ncols) {
+  if (col >= ncols) return;
+  float f0 = apply_act<ACT>(v0 + bias_s[col]);
+  float f1 = apply_act<ACT>(v1 + bias_s[col + 1]);
+  if (col + 1 < ncols) {
+    if constexpr (RES) {
+      const float2 r = __half22float2(*reinterpret_cast<const __half2*>(res + col));
+      f0 += r.x;
+      f1 += r.y;
     }
-    *reinterpret_cast<float4*>(out + q * 4) = o;
+    *reinterpret_cast<__half2*>(out + col) = __floats2half2_rn(f0, f1);
+  } else {
+    if constexpr (RES) f0 += __half2float(res[col]);
+    out[col] = __float2half_rn(f0);
+  }
+}
+
+template <int ACT>
+__device__ __forceinline__ void epi_pair_f32(float v0, float v1, const float* __restrict__ bias_s, int col,
+                                             float* __restrict__ out, int ncols, bool residual) {
+  if (col >= ncols) return;
+  float f0 = apply_act_precise<ACT>(v0 + bias_s[col]);
+  float f1 = apply_act_precise<ACT>(v1 + bias_s[col + 1]);
+  if (col + 1 < ncols) {
+    if (residual) {
+      const float2 r = *reinterpret_cast<const float2*>(out + col);
+      f0 += r.x;
+      f1 += r.y;
+    }
+    *reinterpret_cast<float2*>(out + col) = make_float2(f0, f1);
+  } else {
+    if (residual) f0 += out[col];
+    out[col] = f0;
+  }
+}
+
+// The fp16 epilogue over this thread's whole accumulator fragment (two pixels, BN/4 column pairs each).
+template <int BN, int ACT, bool RES>
+__device__ __forceinline__ void epilogue_f16(const float (&acc)[BN / 2], const float* __restrict__ bias_s,
+                                             __half* const (&out)[2], const __half* const (&res)[2], const bool (&valid)[2],
+                                             int ncols, int lane) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (!valid[h]) continue;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j)
+      epi_pair_f16<ACT, RES>(acc[j * 4 + 2 * h], acc[j * 4 + 2 * h + 1], bias_s, j * 8 + (lane & 3) * 2, out[h], res[h],
+                             ncols);
   }
 }
 
 template <int BN, int ACT>
-__device__ __forceinline__ void epilogue_store_f32(uint32_t tmem_row, const float* __restrict__ bias_s,
-                                                   float* __restrict__ out, int cout_left, bool valid, bool residual) {
-  if constexpr (BN >= 32) {
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      uint32_t v0[32];
-      tmem_ld_32x32(tmem_row + uint32_t(c0), v0);
-      tmem_ld_wait();
-      const int left = cout_left - c0;
-      if (valid && left > 0) epilogue_chunk_f32<ACT>(v0, bias_s + c0, out + c0, left < 32 ? left : 32, residual);
-    }
-  } else {
-    uint32_t t16[16];
-    tmem_ld_32x16(tmem_row, t16);
-    tmem_ld_wait();
-    if (valid && cout_left > 0) epilogue_chunk_f32<ACT>(t16, bias_s, out, cout_left < 16 ? cout_left : 16, residual);
-  }
-}
-
-// One 32-column chunk of the accumulator row owned by this thread: bias + activation (+ residual)
-// -> fp16 -> four 16-byte stores.  Straight-line code (no per-element branches), bias from smem.
-template <int ACT, bool RES>
-__device__ __forceinline__ void epilogue_chunk32(const uint32_t (&v)[32], const float* __restrict__ bias_s,
-                                                 __half* __restrict__ out, int ncols) {
-  uint4 r[4];
-  if constexpr (RES) {
+__device__ __forceinline__ void epilogue_f32(const float (&acc)[BN / 2], const float* __restrict__ bias_s,
+                                             float* const (&out)[2], const bool (&valid)[2], int ncols, int lane,
+                                             bool residual) {
 #pragma unroll
-    for (int q = 0; q < 4; ++q)
-      if (q * 8 < ncols) r[q] = *reinterpret_cast<const uint4*>(out + q * 8);
-  }
+  for (int h = 0; h < 2; ++h) {
+    if (!valid[h]) continue;
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    if (q * 8 >= ncols) break;
-    float f[8];
-    const float4 b0 = *reinterpret_cast<const float4*>(bias_s + q * 8);
-    const float4 b1 = *reinterpret_cast<const float4*>(bias_s + q * 8 + 4);
-    f[0] = apply_act<ACT>(__uint_as_float(v[q * 8 + 0]) + b0.x);
-    f[1] = apply_act<ACT>(__uint_as_float(v[q * 8 + 1]) + b0.y);
-    f[2] = apply_act<ACT>(__uint_as_float(v[q * 8 + 2]) + b0.z);
-    f[3] = apply_act<ACT>(__uint_as_float(v[q * 8 + 3]) + b0.w);
-    f[4] = apply_act<ACT>(__uint_as_float(v[q * 8 + 4]) + b1.x);
-    f[5] = apply_act<ACT>(__uint_as_float(v[q * 8 + 5]) + b1.y);
-    f[6] = apply_act<ACT>(__uint_as_float(v[q * 8 + 6]) + b1.z);
-    f[7] = apply_act<ACT>(__uint_as_float(v[q * 8 + 7]) + b1.w);
-    if constexpr (RES) {
-      const __half2* rh = reinterpret_cast<const __half2*>(&r[q]);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 rf = __half22float2(rh[e]);
-        f[2 * e] += rf.x;
-        f[2 * e + 1] += rf.y;
-      }
-    }
-    uint4 o;
-    __half2* oh = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) oh[e] = __floats2half2_rn(f[2 * e], f[2 * e + 1]);
-    *reinterpret_cast<uint4*>(out + q * 8) = o;
-  }
-}
-
-// 32 columns -> bias + activation (+ residual read from global) -> fp16 -> the 128-byte-swizzled staging row of
-// this thread (16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) * 16)); `half` selects chunks 0-3 / 4-7.
-template <int ACT, bool RES>
-__device__ __forceinline__ void epilogue_chunk32_smem(const uint32_t (&v)[32], const float* __restrict__ bias_s,
-                                                      const uint4 (&res)[4], uint32_t stage_row, int row, int half) {
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    float f[8];
-    const float4 b0 = *reinterpret_cast<const float4*>(bias_s + q * 8);
-    const float4 b1 = *reinterpret_cast<const float4*>(bias_s + q * 8 + 4);
-    f[0] = apply_act<ACT>(__uint_as_float(v[q * 8 + 0]) + b0.x);
-    f[1] = apply_act<ACT>(__uint_as_float(v[q * 8 + 1]) + b0.y);
-    f[2] = apply_act<ACT>(__uint_as_float(v[q * 8 + 2]) + b0.z);
-    f[3] = apply_act<ACT>(__uint_as_float(v[q * 8 + 3]) + b0.w);
-    f[4] = apply_act<ACT>(__uint_as_float(v[q * 8 + 4]) + b1.x);
-    f[5] = apply_act<ACT>(__uint_as_float(v[q * 8 + 5]) + b1.y);
-    f[6] = apply_act<ACT>(__uint_as_float(v[q * 8 + 6]) + b1.z);
-    f[7] = apply_act<ACT>(__uint_as_float(v[q * 8 + 7]) + b1.w);
-    if constexpr (RES) {
-      const __half2* rh = reinterpret_cast<const __half2*>(&res[q]);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const float2 rf = __half22float2(rh[e]);
-        f[2 * e] += rf.x;
-        f[2 * e + 1] += rf.y;
-      }
-    }
-    uint32_t w0, w1, w2, w3;
-    {
-      __half2 h0 = __floats2half2_rn(f[0], f[1]), h1 = __floats2half2_rn(f[2], f[3]);
-      __half2 h2 = __floats2half2_rn(f[4], f[5]), h3 = __floats2half2_rn(f[6], f[7]);
-      w0 = *reinterpret_cast<uint32_t*>(&h0); w1 = *reinterpret_cast<uint32_t*>(&h1);
-      w2 = *reinterpret_cast<uint32_t*>(&h2); w3 = *reinterpret_cast<uint32_t*>(&h3);
-    }
-    const int j = half * 4 + q;
-    const uint32_t addr = stage_row + uint32_t(((j ^ (row & 7)) << 4));
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(w0), "r"(w1), "r"(w2), "r"(w3) : "memory");
-  }
-}
-
-// The whole accumulator row owned by this thread, 32 columns at a time.
-template <int BN, int ACT, bool RES>
-__device__ __forceinline__ void epilogue_store(uint32_t tmem_row, const float* __restrict__ bias_s,
-                                               __half* __restrict__ out, int cout_left, bool valid) {
-  if constexpr (BN >= 32) {
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      uint32_t v0[32];
-      tmem_ld_32x32(tmem_row + uint32_t(c0), v0);
-      tmem_ld_wait();
-      if (valid) epilogue_chunk32<ACT, RES>(v0, bias_s + c0, out + c0, cout_left - c0);
-    }
-  } else {
-    uint32_t v0[32];
-    uint32_t t16[16];
-    tmem_ld_32x16(tmem_row, t16);
-    tmem_ld_wait();
-#pragma unroll
-    for (int j = 0; j < 16; ++j) v0[j] = t16[j];
-#pragma unroll
-    for (int j = 16; j < 32; ++j) v0[j] = 0u;
-    if (valid) epilogue_chunk32<ACT, RES>(v0, bias_s, out, cout_left < 16 ? cout_left : 16);
-  }
-}
-
-// TMA-store epilogue for BN >= 64: 64 output channels at a time are staged in the warpgroup's swizzled
-// 128x128-byte buffer and written by ONE bulk tensor store (coalesced 128-byte rows, image-edge clipping by
-// the TMA unit) instead of 128 threads x 8 strided 16-byte stores.
-// Residual rows of one 64-channel chunk (2 x 4 x 16 bytes per thread).  Loaded BEFORE the accumulator wait so the
-// global-memory latency hides under the MMA of the tile.
-struct ResChunk { uint4 lo[4], hi[4]; };
-__device__ __forceinline__ void load_res_chunk(ResChunk& r, const __half* __restrict__ res) {
-#pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    r.lo[q] = *reinterpret_cast<const uint4*>(res + q * 8);
-    r.hi[q] = *reinterpret_cast<const uint4*>(res + 32 + q * 8);
-  }
-}
-
-template <int BN, int ACT, bool RES>
-__device__ __forceinline__ void epilogue_store_tma(uint32_t tmem_row, const float* __restrict__ bias_s,
-                                                   const __half* __restrict__ res, uint32_t stage_base, int row,
-                                                   const CUtensorMap* omap, int n0, int ox0, int oy0, int img,
-                                                   uint32_t bar_id, bool leader, ResChunk& r) {
-  const uint32_t stage_row = stage_base + uint32_t(row) * 128u;
-#pragma unroll 1
-  for (int c0 = 0; c0 < BN; c0 += 64) {
-    // chunk 0 was prefetched by the caller; later chunks load here, eight independent 16-byte loads in flight
-    // under the TMEM read and the barrier below
-    if constexpr (RES) {
-      if (c0 > 0) load_res_chunk(r, res + c0);
-    }
-    // one 32-column half at a time keeps the accumulator registers at 32 (no spills next to the residual)
-    uint32_t v[32];
-    tmem_ld_32x32(tmem_row + uint32_t(c0), v);
-    tmem_ld_wait();
-    // the previous chunk's store must have finished reading the staging buffer
-    if (leader) tma_store_wait_read();
-    named_barrier_sync(bar_id, 128);
-    epilogue_chunk32_smem<ACT, RES>(v, bias_s + c0, r.lo, stage_row, row, 0);
-    tmem_ld_32x32(tmem_row + uint32_t(c0 + 32), v);
-    tmem_ld_wait();
-    epilogue_chunk32_smem<ACT, RES>(v, bias_s + c0 + 32, r.hi, stage_row, row, 1);
-    fence_proxy_async();
-    named_barrier_sync(bar_id, 128);
-    if (leader) {
-      tma_store_4d(omap, stage_base, n0 + c0, ox0, oy0, img);
-      tma_store_commit();
-    }
-  }
-}
-
-// Issue the MMAs of one K block: `ksteps` x (M128 x BN x K16), descriptors advanced by 32 bytes (>>4 = 2) per
-// step.  Straight-line code: the issuing warp's instruction stream is the bottleneck for small tiles, so
-// nothing but the adds and the tcgen05.mma themselves is left in here.
-__device__ __forceinline__ void issue_kblock(uint32_t tmem_d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc0,
-                                             int ksteps) {
-  umma_f16(tmem_d, ad, bd, idesc, acc0);
-  if (ksteps >= 2) umma_f16(tmem_d, ad + 2, bd + 2, idesc, 1u);
-  if (ksteps >= 4) {
-    umma_f16(tmem_d, ad + 4, bd + 4, idesc, 1u);
-    umma_f16(tmem_d, ad + 6, bd + 6, idesc, 1u);
+    for (int j = 0; j < BN / 8; ++j)
+      epi_pair_f32<ACT>(acc[j * 4 + 2 * h], acc[j * 4 + 2 * h + 1], bias_s, j * 8 + (lane & 3) * 2, out[h], ncols,
+                        residual);
   }
 }
 
@@ -290,23 +139,16 @@ template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   using Cfg = TcCfg<BN>;
   extern __shared__ __align__(1024) uint8_t smem_tc[];
-  uint8_t* const smem_raw = smem_tc;
-  const uint32_t smem_base = smem_u32(smem_raw);
-  if (smem_base & 1023u) __trap();   // the layout has no alignment slack
+  // the swizzled operand stages need 1024-byte alignment; the dynamic base is only guaranteed 16
+  const uint32_t raw_base = smem_u32(smem_tc);
+  const uint32_t smem_base = (raw_base + 1023u) & ~1023u;
+  uint8_t* const smem_gen = smem_tc + (smem_base - raw_base);
   const uint32_t a_base = smem_base;
   const uint32_t b_base = a_base + Cfg::kStages * Cfg::kABytes;
-  const uint32_t store_base = b_base + Cfg::kStages * Cfg::kBBytes;
-  const uint32_t bar_base = store_base + Cfg::kStoreBytes;
-  // barriers (8 B each): full[S] | empty[S] | tmem_full[A] | tmem_empty[A] | tmem ptr   (<= 512 bytes)
+  const uint32_t bar_base = b_base + Cfg::kStages * Cfg::kBBytes;
+  // barriers (8 B each): full[S] | empty[S]
   const uint32_t full_bar = bar_base, empty_bar = bar_base + 8 * Cfg::kStages;
-  const uint32_t tmem_full_bar = bar_base + 16 * Cfg::kStages;
-  const uint32_t tmem_empty_bar = tmem_full_bar + 8 * Cfg::kAccStages;
-  const uint32_t tmem_ptr_addr = tmem_empty_bar + 8 * Cfg::kAccStages;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const size_t bar_off = size_t(Cfg::kStages) * (Cfg::kABytes + Cfg::kBBytes) + Cfg::kStoreBytes;
-  volatile uint32_t* tmem_ptr_gen =
-      reinterpret_cast<volatile uint32_t*>(smem_gen + bar_off + 16 * Cfg::kStages + 16 * Cfg::kAccStages);
-  float* bias_s = reinterpret_cast<float*>(smem_gen + bar_off + 512);
+  float* bias_s = reinterpret_cast<float*>(smem_gen + size_t(Cfg::kStages) * (Cfg::kABytes + Cfg::kBBytes) + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const ConvGeom& g = p.g;
@@ -327,24 +169,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     for (int s = 0; s < g.n_src; ++s)
       for (int q = 0; q < (g.in_stride == 2 ? 4 : 1); ++q) prefetch_tensormap(&p.a_map[s][q]);
     prefetch_tensormap(&p.b_map);
-    if (p.use_tma_store)
-      for (int q = 0; q < g.n_phase; ++q) prefetch_tensormap(&p.o_map[q]);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
-    }
-    for (int s = 0; s < Cfg::kAccStages; ++s) {
-      mbar_init(tmem_full_bar + 8 * s, 1);
-      mbar_init(tmem_empty_bar + 8 * s, 128);
+      mbar_init(empty_bar + 8 * s, 2);   // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc(tmem_ptr_addr, Cfg::kTmemCols);
-  for (int i = threadIdx.x; i < g.cout_pad && i < Cfg::kBiasFloats; i += kThreads) bias_s[i] = p.bias[i];
-  tc_fence_before();
+  for (int i = threadIdx.x; i < g.cout_pad && i < Cfg::kBiasFloats; i += kThreads) bias_s[i] = p.bias ? p.bias[i] : 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_gen;
   griddep_launch_dependents();   // successors may begin their prologue as our CTAs retire
   griddep_wait();                // activations / residuals written by the predecessor are visible from here on
 
@@ -376,7 +208,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
           for (int s = 0; s < g.n_src; ++s) {
             for (int cb = 0; cb < p.src_kblocks[s]; ++cb) {
               for (int term = 0; term < n_terms; ++term, ++it) {
-                // term 0: A hi x B hi; 1: A lo x B hi; 2: A hi x B lo (small terms ride in the same accumulator)
+                // term 0: A hi x B hi; 1: A lo x B hi; 2: A hi x B lo
                 const int stage = it % Cfg::kStages;
                 const uint32_t par = ((it / Cfg::kStages) & 1) ^ 1;
                 mbar_wait_relaxed(empty_bar + 8 * stage, par);
@@ -392,978 +224,184 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         }
       }
     }
-  } else if (warp == 1) {
-    // =============================== MMA issuer =================================
-    const uint32_t idesc = make_idesc_f16(BN);
-    const bool leader = elect_one();   // one fixed thread issues every MMA and commit of this CTA
-    const uint64_t a_desc0 = make_kmajor_desc(a_base, row_bytes), b_desc0 = make_kmajor_desc(b_base, row_bytes);
-    const int ksteps = kb / 16;
-    if (leader) {   // the whole loop on the one issuing lane: no per-stage reconvergence
-      int stage = 0, ti = 0;
-      uint32_t full_par = 0;
-      uint64_t ad = a_desc0, bd = b_desc0;
-      if constexpr (BN <= 64) {
-        if (p.split) {
-          // Split-fp16 mode with PROMOTED accumulation.  The tensor core adds into its fp32 accumulator with
-          // truncation: over the K/16 x 3 MMAs of a deep layer the one-sided errors add up to ~K/16 ulps (measured
-          // 3e-5 relative on the 3x3 256->256 layers, 200x a CUDA-core fp32 FMA chain).  So every hi x hi MMA (K = 16)
-          // writes a FRESH accumulator from a ring of kRing TMEM slots and the epilogue threads sum the slots in fp32
-          // registers with round-to-nearest; the small cross terms (lo x hi, hi x lo: 2^-12 of the sum, their
-          // truncation is 2^-36) accumulate in TMEM as usual, in one slot per tile parity (slots 0 / 1).
-          // Each epilogue warpgroup owns its own ring (and cross-term slot): a slot's uses are then consumed by ONE
-          // warpgroup in production order, which the parity protocol needs (a consumer that starts waiting for use u
-          // of a slot before use u-1 has even been produced would see "previous phase complete" and run ahead).
-          constexpr int kRing = (Cfg::kAccStages - 2) / 2;
-          const uint32_t cpt_m = uint32_t(its_per_tile / 3) * uint32_t(ksteps);
-          for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++ti) {
-            const int xs = ti & 1;
-            uint32_t rc = uint32_t(ti >> 1) * cpt_m;   // hi x hi MMAs issued so far for this warpgroup's tiles
-            mbar_wait(tmem_empty_bar + 8 * xs, ((ti >> 1) & 1) ^ 1);
-            tc_fence_after();
-            const uint32_t tmem_x = tmem_base + uint32_t(xs * BN);
-            bool cross_started = false;
-            for (int k_it = 0; k_it < its_per_tile; ++k_it) {
-              mbar_wait(full_bar + 8 * stage, full_par);
-              tc_fence_after();
-              if (k_it % 3 == 0) {
-                for (int ks = 0; ks < ksteps; ++ks, ++rc) {
-                  const uint32_t slot = 2u + uint32_t(xs * kRing) + rc % kRing;
-                  mbar_wait(tmem_empty_bar + 8 * slot, ((rc / kRing) & 1u) ^ 1u);
-                  tc_fence_after();
-                  umma_f16(tmem_base + slot * BN, ad + 2 * ks, bd + 2 * ks, idesc, 0u);
-                  umma_commit(tmem_full_bar + 8 * slot);
-                }
-              } else {
-                issue_kblock(tmem_x, ad, bd, idesc, cross_started ? 1u : 0u, ksteps);
-                cross_started = true;
-              }
-              umma_commit(empty_bar + 8 * stage);
-              if (++stage == Cfg::kStages) {
-                stage = 0; full_par ^= 1u; ad = a_desc0; bd = b_desc0;
-              } else {
-                ad += uint64_t(Cfg::kABytes >> 4); bd += uint64_t(Cfg::kBBytes >> 4);
-              }
-            }
-            umma_commit(tmem_full_bar + 8 * xs);
-          }
-          ti = -1;   // skip the plain loop below
-        }
-      }
-      for (int t = blockIdx.x; ti >= 0 && t < total_tiles; t += gridDim.x, ++ti) {
-        const int as = ti % Cfg::kAccStages;
-        mbar_wait(tmem_empty_bar + 8 * as, ((ti / Cfg::kAccStages) & 1) ^ 1);  // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + uint32_t(as * BN);
+    return;
+  }
+  if (warp < 4) return;
+
+  // =============================== consumers ====================================
+  const int wg = (warp >> 2) - 1;                   // rows [64*wg, 64*wg + 64) of the tile
+  const int wrow = ((warp & 3) << 4) + (lane >> 2);  // this thread's first fragment row within the 64
+  const bool wg_leader = (threadIdx.x & 127) == 0;
+  const uint64_t a_desc0 = make_kmajor_desc(a_base + uint32_t(wg) * 64u * row_bytes, row_bytes);
+  const uint64_t b_desc0 = make_kmajor_desc(b_base, row_bytes);
+  const int ksteps = kb / 16;
+  int stage = 0;
+  uint32_t full_par = 0;
+  constexpr int R = BN / 2;
+
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    int phase, nblk, img, y0, x0;
+    decode(t, phase, nblk, img, y0, x0);
+    float acc[R];
+#pragma unroll
+    for (int i = 0; i < R; ++i) acc[i] = 0.f;
+
+    bool split_done = false;
+    if constexpr (BN <= 64) {
+      if (p.split) {
+        // Split-fp16 mode with PROMOTED accumulation.  The tensor core adds into its fp32 accumulator with
+        // truncation: over the K/16 x 3 MMAs of a deep layer the one-sided errors add up to ~K/16 ulps.  So every
+        // hi x hi MMA (K = 16) writes a FRESH accumulator that is added into `acc` in fp32 registers with
+        // round-to-nearest; the small cross terms (lo x hi, hi x lo: 2^-12 of the sum, their truncation is 2^-36)
+        // accumulate in the tensor core as usual and are added last.
+        float cross[R], tmp[R];
+#pragma unroll
+        for (int i = 0; i < R; ++i) cross[i] = 0.f;
+        bool cross_started = false;
         for (int k_it = 0; k_it < its_per_tile; ++k_it) {
           mbar_wait(full_bar + 8 * stage, full_par);
-          tc_fence_after();
-          issue_kblock(tmem_d, ad, bd, idesc, k_it > 0 ? 1u : 0u, ksteps);
-          umma_commit(empty_bar + 8 * stage);
-          if (k_it == its_per_tile - 1) umma_commit(tmem_full_bar + 8 * as);
-          if (++stage == Cfg::kStages) {
-            stage = 0; full_par ^= 1u; ad = a_desc0; bd = b_desc0;
+          const uint64_t ad = a_desc0 + uint64_t(stage) * (Cfg::kABytes >> 4);
+          const uint64_t bd = b_desc0 + uint64_t(stage) * (Cfg::kBBytes >> 4);
+          if (k_it % 3 == 0) {
+            for (int ks = 0; ks < ksteps; ++ks) {
+              wgmma_fence();
+              wgmma_bn<BN>(tmp, ad + 2 * ks, bd + 2 * ks, 0u);
+              wgmma_commit();
+              wgmma_wait<0>();
+              wgmma_fence_regs(tmp);
+#pragma unroll
+              for (int i = 0; i < R; ++i) acc[i] = __fadd_rn(acc[i], tmp[i]);
+            }
           } else {
-            ad += uint64_t(Cfg::kABytes >> 4); bd += uint64_t(Cfg::kBBytes >> 4);
+            wgmma_fence();
+            for (int ks = 0; ks < ksteps; ++ks)
+              wgmma_bn<BN>(cross, ad + 2 * ks, bd + 2 * ks, (cross_started || ks > 0) ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(cross);
+            cross_started = true;
           }
+          if (wg_leader) mbar_arrive(empty_bar + 8 * stage);
+          if (++stage == Cfg::kStages) { stage = 0; full_par ^= 1u; }
         }
+#pragma unroll
+        for (int i = 0; i < R; ++i) acc[i] = __fadd_rn(acc[i], cross[i]);
+        split_done = true;
       }
     }
-  } else if (warp >= kEpiWarp0) {
-    // =============================== epilogue ====================================
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may read
-    const int group = (warp - kEpiWarp0) >> 2;  // two warpgroups take alternate tiles
-    const int row = quad * 32 + lane;
-    const int py = row / kTileW, px = row - py * kTileW;
-    int ti = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++ti) {
-      if ((ti & 1) != group) continue;
-      int phase, nblk, img, y0, x0;
-      decode(t, phase, nblk, img, y0, x0);
-      const int as = ti % Cfg::kAccStages;
-      const int gy = y0 + py, gx = x0 + px;
-      const bool valid = gy < g.gh && gx < g.gw;
-      const int ph_y = phase >> 1, ph_x = phase & 1;
-      const int oy = gy * g.out_mul + ph_y, ox = gx * g.out_mul + ph_x;
-      __half* out = p.dst == nullptr ? nullptr
-                                     : p.dst + (size_t(img) * g.dst_h * g.dst_w + size_t(valid ? oy : 0) * g.dst_w + (valid ? ox : 0)) * g.dst_cstride +
-                                           g.dst_coff + nblk * BN;
-      ResChunk rc;
-      if constexpr (BN >= 64) {
-        if (p.use_tma_store && g.residual) load_res_chunk(rc, out);
+    if (!split_done) {
+      int prev = -1;
+      for (int k_it = 0; k_it < its_per_tile; ++k_it) {
+        mbar_wait(full_bar + 8 * stage, full_par);
+        const uint64_t ad = a_desc0 + uint64_t(stage) * (Cfg::kABytes >> 4);
+        const uint64_t bd = b_desc0 + uint64_t(stage) * (Cfg::kBBytes >> 4);
+        wgmma_fence();
+        for (int ks = 0; ks < ksteps; ++ks) wgmma_bn<BN>(acc, ad + 2 * ks, bd + 2 * ks, (k_it > 0 || ks > 0) ? 1u : 0u);
+        wgmma_commit();
+        // one group stays in flight: the previous group has retired, its stage goes back to the producer
+        wgmma_wait<1>();
+        if (prev >= 0 && wg_leader) mbar_arrive(empty_bar + 8 * prev);
+        prev = stage;
+        if (++stage == Cfg::kStages) { stage = 0; full_par ^= 1u; }
       }
-      const float* bias_t = bias_s + nblk * BN;
-      if constexpr (BN <= 64) {
-        if (p.split) {
-          // promoted accumulation (see the MMA issuer): sum the hi x hi ring slots of this tile and its cross-term
-          // slot in fp32 registers, then bias / activation / residual -> FP32 destination (or the Detect decode)
-          constexpr int kRing = (Cfg::kAccStages - 2) / 2;       // this warpgroup's ring (see the MMA issuer)
-          const int cpt = (its_per_tile / 3) * (kb / 16);        // hi x hi MMAs per tile
-          const uint32_t lane_off = uint32_t(quad * 32) << 16;
-          float acc[BN];
-#pragma unroll
-          for (int j = 0; j < BN; ++j) acc[j] = 0.f;
-          uint32_t rc = uint32_t(ti >> 1) * uint32_t(cpt);
-          for (int c = 0; c <= cpt; ++c, ++rc) {
-            const bool last = c == cpt;                            // the cross-term slot comes last
-            const uint32_t slot = last ? uint32_t(ti & 1) : 2u + uint32_t((ti & 1) * kRing) + rc % kRing;
-            const uint32_t par = last ? uint32_t((ti >> 1) & 1) : ((rc / kRing) & 1u);
-            mbar_wait_relaxed(tmem_full_bar + 8 * slot, par);
-            tc_fence_after();
-            const uint32_t trow = tmem_base + slot * BN + lane_off;
-            if constexpr (BN >= 32) {
-#pragma unroll
-              for (int c0 = 0; c0 < BN; c0 += 32) {
-                uint32_t v[32];
-                tmem_ld_32x32(trow + uint32_t(c0), v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; ++j) acc[c0 + j] = __fadd_rn(acc[c0 + j], __uint_as_float(v[j]));
-              }
-            } else {
-              uint32_t v[16];
-              tmem_ld_32x16(trow, v);
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 16; ++j) acc[j] = __fadd_rn(acc[j], __uint_as_float(v[j]));
-            }
-            tc_fence_before();
-            mbar_arrive(tmem_empty_bar + 8 * slot);
-          }
-          const uint32_t* accu = reinterpret_cast<const uint32_t*>(acc);
-          if (p.dst != nullptr) {
-            float* out32 = reinterpret_cast<float*>(p.dst) +
-                           (size_t(img) * g.dst_h * g.dst_w + size_t(valid ? oy : 0) * g.dst_w + (valid ? ox : 0)) * g.dst_cstride +
-                           g.dst_coff + nblk * BN;
-            const int cout_left = g.cout - nblk * BN;
-            const bool res = g.residual != 0;
-#pragma unroll
-            for (int c0 = 0; c0 < BN; c0 += 32) {
-              const int left = cout_left - c0;
-              if (!valid || left <= 0) continue;
-              const int nc = left < 32 ? left : 32;
-              switch (g.act) {
-                case CTD_ACT_SILU: epilogue_chunk_f32<CTD_ACT_SILU>(accu + c0, bias_t + c0, out32 + c0, nc, res); break;
-                case CTD_ACT_LEAKY: epilogue_chunk_f32<CTD_ACT_LEAKY>(accu + c0, bias_t + c0, out32 + c0, nc, res); break;
-                case CTD_ACT_RELU: epilogue_chunk_f32<CTD_ACT_RELU>(accu + c0, bias_t + c0, out32 + c0, nc, res); break;
-                case CTD_ACT_SIGMOID: epilogue_chunk_f32<CTD_ACT_SIGMOID>(accu + c0, bias_t + c0, out32 + c0, nc, res); break;
-                default: epilogue_chunk_f32<CTD_ACT_NONE>(accu + c0, bias_t + c0, out32 + c0, nc, res); break;
-              }
-            }
-          } else if (valid) {
-            // Detect decode (yolo.py:36-44): columns = anchor*(5+nc) + o
-            const int no = 5 + p.nc;
-            float* rows = p.blks + (size_t(img) * p.blks_rows_per_img + p.level_row0) * no;
-#pragma unroll
-            for (int j = 0; j < BN; ++j) {
-              const int col = nblk * BN + j;
-              if (col < g.cout) {
-                const int a = col / no, o = col - a * no;
-                const float sg = 1.0f / (1.0f + expf(-(acc[j] + bias_t[j])));
-                float r;
-                if (o == 0) r = (sg * 2.0f - 0.5f + float(gx)) * p.det_stride;
-                else if (o == 1) r = (sg * 2.0f - 0.5f + float(gy)) * p.det_stride;
-                else if (o == 2) r = (sg * 2.0f) * (sg * 2.0f) * p.anchor_wh[2 * a];
-                else if (o == 3) r = (sg * 2.0f) * (sg * 2.0f) * p.anchor_wh[2 * a + 1];
-                else r = sg;
-                rows[(size_t(a) * g.gh * g.gw + size_t(gy) * g.gw + gx) * no + o] = r;
-              }
-            }
-          }
-          continue;
-        }
-      }
-      mbar_wait_relaxed(tmem_full_bar + 8 * as, (ti / Cfg::kAccStages) & 1);
-      tc_fence_after();
-      const uint32_t tmem_row = tmem_base + uint32_t(as * BN) + (uint32_t(quad * 32) << 16);
-      if (p.dst != nullptr) {
-        const int cout_left = g.cout - nblk * BN;
-        bool done_tma = false;
-        if constexpr (BN >= 64) {
-          if (p.use_tma_store) {
-            const uint32_t stage_base = store_base + uint32_t(group) * (128u * 128u);
-            const bool leader = (threadIdx.x & 127) == 0;
-            const CUtensorMap* om = &p.o_map[phase];
-#define CTD_EPT(ACT)                                                                                              \
-  if (g.residual) epilogue_store_tma<BN, ACT, true>(tmem_row, bias_t, out, stage_base, row, om, nblk * BN, x0, y0, img, 1 + group, leader, rc); \
-  else epilogue_store_tma<BN, ACT, false>(tmem_row, bias_t, out, stage_base, row, om, nblk * BN, x0, y0, img, 1 + group, leader, rc);
-            switch (g.act) {
-              case CTD_ACT_SILU: CTD_EPT(CTD_ACT_SILU) break;
-              case CTD_ACT_LEAKY: CTD_EPT(CTD_ACT_LEAKY) break;
-              case CTD_ACT_RELU: CTD_EPT(CTD_ACT_RELU) break;
-              case CTD_ACT_SIGMOID: CTD_EPT(CTD_ACT_SIGMOID) break;
-              default: CTD_EPT(CTD_ACT_NONE) break;
-            }
-#undef CTD_EPT
-            done_tma = true;
-          }
-        }
-        if (!done_tma) {
-#define CTD_EPI(ACT)                                                                              \
-  if (g.residual) epilogue_store<BN, ACT, true>(tmem_row, bias_t, out, cout_left, valid);         \
-  else epilogue_store<BN, ACT, false>(tmem_row, bias_t, out, cout_left, valid);
-        switch (g.act) {
-          case CTD_ACT_SILU: CTD_EPI(CTD_ACT_SILU) break;
-          case CTD_ACT_LEAKY: CTD_EPI(CTD_ACT_LEAKY) break;
-          case CTD_ACT_RELU: CTD_EPI(CTD_ACT_RELU) break;
-          case CTD_ACT_SIGMOID: CTD_EPI(CTD_ACT_SIGMOID) break;
-          default: CTD_EPI(CTD_ACT_NONE) break;
-        }
-#undef CTD_EPI
-        }
-      } else {
-        // Detect decode (yolo.py:36-44): columns = anchor*(5+nc) + o
-        constexpr int kChunk = BN >= 32 ? 32 : 16;
-        const int no = 5 + p.nc;
-        const int no_rcp = 65536 / no + 1;   // col / no == (col * no_rcp) >> 16 for col < 512 (no runtime division per element)
-        float* rows = p.blks + (size_t(img) * p.blks_rows_per_img + p.level_row0) * no;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += kChunk) {
-          uint32_t v[kChunk];
-          if constexpr (kChunk == 32) {
-            tmem_ld_32x32(tmem_row + uint32_t(c0), v);
-          } else {
-            tmem_ld_32x16(tmem_row + uint32_t(c0), reinterpret_cast<uint32_t(&)[16]>(v));
-          }
-          tmem_ld_wait();
-          if (!valid) continue;
-#pragma unroll
-          for (int j = 0; j < kChunk; ++j) {
-            const int col = nblk * BN + c0 + j;
-            if (col < g.cout) {
-              const int a = (col * no_rcp) >> 16, o = col - a * no;
-              const float s = 1.0f / (1.0f + expf(-(__uint_as_float(v[j]) + bias_t[c0 + j])));
-              float r;
-              if (o == 0) r = (s * 2.0f - 0.5f + float(gx)) * p.det_stride;
-              else if (o == 1) r = (s * 2.0f - 0.5f + float(gy)) * p.det_stride;
-              else if (o == 2) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a];
-              else if (o == 3) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a + 1];
-              else r = s;
-              rows[(size_t(a) * g.gh * g.gw + size_t(gy) * g.gw + gx) * no + o] = r;
-            }
-          }
-        }
-      }
-      // all of this thread's tcgen05.ld have completed (wait::ld): hand the accumulator back
-      tc_fence_before();
-      mbar_arrive(tmem_empty_bar + 8 * as);
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && wg_leader) mbar_arrive(empty_bar + 8 * prev);
     }
-    if (p.use_tma_store && (threadIdx.x & 127) == 0) tma_store_wait_all();  // smem must outlive the bulk stores
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
 
-
-// =========================================================================================
-// Halo variant.  For 3x3 stride-1 convolutions (and the 2x2-tap deconvolution phases) with few channels the
-// tap-per-box scheme above is bound by the TMA unit, not by the tensor cores: every tap re-fetches the same
-// 128 pixels (9 boxes of 128 rows per tile, plus 9 weight boxes).  Here
-//   * the weights of the CTA's phase are loaded ONCE and stay resident in shared memory;
-//   * a tile is 8 wide x 16 high, and ONE box per K block brings the tile plus its halo (W x H pixels, lox/loy
-//     of them before the tile); stride-2 convolutions take one such box per parity view of the source;
-//   * filter tap (dy,dx) is the same smem block viewed through a matrix descriptor that starts
-//     (dy+loy)*W + (dx+lox) rows in and steps W rows between 8-row groups (SBO): the 8 pixels of a
-//     tile row are 8 consecutive halo rows, so every 8-row core group stays contiguous.  The 128B/64B swizzle
-//     is a function of the absolute shared-memory address for both TMA (writer) and the MMA (reader), so a
-//     view that starts off the 1024-byte pattern boundary is read consistently with the descriptor's
-//     base_offset left at 0 (measured on B200: setting base_offset = (addr >> 7) & 7 gives wrong results).
-// The CTA -> phase mapping is static (blockIdx.x % n_phase), tiles of that phase are strided over its CTAs.
-constexpr int kHaloTileW = 8, kHaloTileH = 16;
-constexpr int kHaloMaxStages = 8;
-
-template <int BN>
-struct HaloCfg {
-  static constexpr int kAccStages = 8;                      // BN <= 64 -> <= 512 TMEM columns
-  static constexpr int kTmemCols = BN * kAccStages;         // 128 / 256 / 512
-  static constexpr int kStoreBytes = BN >= 64 ? 2 * 128 * 128 : 0;
-  static constexpr int kBiasFloats = 64;
-  static constexpr size_t smem_bytes(int w_bytes, int stages, int stage_bytes) {
-    return 1024 + size_t((w_bytes + 1023) / 1024 * 1024) + size_t(stages) * stage_bytes + 512 + kBiasFloats * 4 + 1024 +
-           kStoreBytes;
-  }
-};
-
-template <int BN>
-__global__ void __launch_bounds__(kThreads, 1) conv_halo_kernel(const __grid_constant__ ConvTcParams p) {
-  using Cfg = HaloCfg<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t w_base = smem_base;
-  const uint32_t w_region = (uint32_t(p.halo_w_bytes) + 1023u) & ~1023u;
-  const uint32_t a_base = w_base + w_region;
-  const int S = p.halo_stages;
-  const uint32_t stage_bytes = uint32_t(p.halo_stage_bytes);
-  const uint32_t bar_base = a_base + uint32_t(S) * stage_bytes;
-  // barriers: full[8] | empty[8] | tmem_full[8] | tmem_empty[8] | weights | tmem ptr
-  const uint32_t full_bar = bar_base, empty_bar = bar_base + 64, tmem_full_bar = bar_base + 128;
-  const uint32_t tmem_empty_bar = bar_base + 192, w_bar = bar_base + 256, tmem_ptr_addr = bar_base + 264;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const size_t bar_off = size_t(w_region) + size_t(S) * stage_bytes;
-  volatile uint32_t* tmem_ptr_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + bar_off + 264);
-  float* bias_s = reinterpret_cast<float*>(smem_gen + bar_off + 512);
-  const uint32_t store_base = (bar_base + 512u + uint32_t(Cfg::kBiasFloats) * 4u + 1023u) & ~1023u;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const ConvGeom& g = p.g;
-  const int kb = p.kb_elems;
-  const uint32_t row_bytes = kb * 2;
-  const int lox = p.halo_lox, loy = p.halo_loy;   // halo pixels before the tile (x / y)
-  const int halo_w = p.halo_w, halo_h = p.halo_h;
-  const uint32_t stage_tx = uint32_t(halo_w * halo_h) * row_bytes;
-  const int n_par = g.in_stride == 2 ? 4 : 1;     // stride-2: one halo box per parity view of the source
-  int kblocks = 0;
-  for (int s = 0; s < g.n_src; ++s) kblocks += p.src_kblocks[s];
-  const int tiles_per_img = p.tiles_x * p.tiles_y;
-  const int spatial_tiles = g.n_img * tiles_per_img;
-  const int phase = int(blockIdx.x) % g.n_phase;
-  const int rank = int(blockIdx.x) / g.n_phase, nrank = int(gridDim.x) / g.n_phase;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < g.n_src; ++s)
-      for (int q = 0; q < n_par; ++q) prefetch_tensormap(&p.a_map[s][q]);
-    prefetch_tensormap(&p.b_map);
-    if (p.use_tma_store) prefetch_tensormap(&p.o_map[phase]);
-    for (int s = 0; s < S; ++s) {
-      mbar_init(full_bar + 8 * s, 1);
-      mbar_init(empty_bar + 8 * s, 1);
-    }
-    for (int s = 0; s < Cfg::kAccStages; ++s) {
-      mbar_init(tmem_full_bar + 8 * s, 1);
-      mbar_init(tmem_empty_bar + 8 * s, 128);
-    }
-    mbar_init(w_bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_ptr_addr, Cfg::kTmemCols);
-  for (int i = threadIdx.x; i < BN; i += kThreads) bias_s[i] = (p.bias != nullptr && i < g.cout_pad) ? p.bias[i] : 0.f;
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_gen;
-  griddep_launch_dependents();   // successors may begin their prologue as our CTAs retire
-  if (warp != 0) griddep_wait(); // the producer waits AFTER issuing the (constant) weight loads, see below
-
-  auto decode = [&](int t, int& img, int& y0, int& x0) {
-    img = t / tiles_per_img;
-    const int trem = t - img * tiles_per_img;
-    const int ty = trem / p.tiles_x;
-    y0 = ty * kHaloTileH;
-    x0 = (trem - ty * p.tiles_x) * kHaloTileW;
-  };
-
-  if (warp == 0) {
-    // =============================== TMA producer ===============================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(w_bar, uint32_t(p.halo_w_bytes));
-      for (int tap = 0; tap < g.taps; ++tap) {
-        int kglob = tap * g.cin_total, kbi = 0;
-        for (int s = 0; s < g.n_src; ++s) {
-          for (int cb = 0; cb < p.src_kblocks[s]; ++cb, ++kbi)
-            tma_load_2d(w_base + uint32_t(tap * kblocks + kbi) * uint32_t(BN) * row_bytes, &p.b_map, w_bar,
-                        kglob + cb * kb, phase * g.cout_pad);
-          kglob += g.src_c[s];
-        }
-      }
-      griddep_wait();   // weights are constant; the activations below are the predecessor's output
-      int it = 0;
-      for (int t = rank; t < spatial_tiles; t += nrank) {
-        int img, y0, x0;
-        decode(t, img, y0, x0);
-        for (int q = 0; q < n_par; ++q)
-          for (int s = 0; s < g.n_src; ++s)
-            for (int cb = 0; cb < p.src_kblocks[s]; ++cb, ++it) {
-              const int stage = it % S;
-              const uint32_t par = ((it / S) & 1) ^ 1;
-              mbar_wait_relaxed(empty_bar + 8 * stage, par);
-              mbar_arrive_expect_tx(full_bar + 8 * stage, stage_tx);
-              tma_load_4d(a_base + uint32_t(stage) * stage_bytes, &p.a_map[s][q], full_bar + 8 * stage, cb * kb,
-                          x0 - lox, y0 - loy, img);
-            }
-      }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer =================================
-    const uint32_t idesc = make_idesc_f16(BN);
-    const uint32_t sbo = uint32_t(halo_w) * row_bytes;
-    const bool leader = elect_one();
-    const int ksteps = kb / 16;
-    // per-tap operand views, relative to the stage / weight base (16-byte units, added to the descriptors)
-    uint32_t tap_a[kMaxTaps], tap_b[kMaxTaps];
-    int tap_q[kMaxTaps];
+    // ---------------------------------------------------------------- epilogue
+    const int ph_y = phase >> 1, ph_x = phase & 1;
+    const float* bias_t = bias_s + nblk * BN;
+    const int ncols = g.cout - nblk * BN;   // columns of this N block that exist
+    int gy[2], gx[2];
+    bool valid[2];
+    size_t pix[2];
 #pragma unroll
-    for (int tap = 0; tap < kMaxTaps; ++tap) {
-      const bool on = tap < g.taps;
-      const int dy = on ? g.tap_dy[phase][tap] : 0, dx = on ? g.tap_dx[phase][tap] : 0;
-      tap_a[tap] = (uint32_t((dy + loy) * halo_w + (dx + lox)) * row_bytes) >> 4;
-      tap_b[tap] = (uint32_t(tap * kblocks) * uint32_t(BN) * row_bytes) >> 4;
-      tap_q[tap] = on ? p.tap_map[phase][tap] : -1;
+    for (int h = 0; h < 2; ++h) {
+      const int row = wg * 64 + wrow + 8 * h;
+      gy[h] = y0 + row / kTileW;
+      gx[h] = x0 + row % kTileW;
+      valid[h] = gy[h] < g.gh && gx[h] < g.gw;
+      const int oy = gy[h] * g.out_mul + ph_y, ox = gx[h] * g.out_mul + ph_x;
+      pix[h] = valid[h] ? size_t(img) * g.dst_h * g.dst_w + size_t(oy) * g.dst_w + ox : 0;
     }
-    const uint64_t a_desc0 = make_kmajor_desc_ex(a_base, row_bytes, sbo, 0u);
-    const uint64_t b_desc0 = make_kmajor_desc(w_base, row_bytes);
-    const uint32_t a_step = stage_bytes >> 4, b_kb_step = (uint32_t(BN) * row_bytes) >> 4;
-    mbar_wait(w_bar, 0);
-    int stage = 0, ti = 0;
-    uint32_t full_par = 0;
-    uint64_t ad_stage = a_desc0;
-    for (int t = rank; t < spatial_tiles; t += nrank, ++ti) {
-      const int as = ti % Cfg::kAccStages;
-      mbar_wait(tmem_empty_bar + 8 * as, ((ti / Cfg::kAccStages) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_base + uint32_t(as * BN);
-      uint32_t acc = 0u;
-      for (int q = 0; q < n_par; ++q) {
-        uint64_t bd_kb = b_desc0;
-        for (int kbi = 0; kbi < kblocks; ++kbi) {
-          mbar_wait(full_bar + 8 * stage, full_par);
-          tc_fence_after();
-          if (leader) {
-#pragma unroll
-            for (int tap = 0; tap < kMaxTaps; ++tap) {
-              if (tap_q[tap] != q) continue;
-              issue_kblock(tmem_d, ad_stage + tap_a[tap], bd_kb + tap_b[tap], idesc, acc, ksteps);
-              acc = 1u;
-            }
-            umma_commit(empty_bar + 8 * stage);
-            if (q == n_par - 1 && kbi == kblocks - 1) umma_commit(tmem_full_bar + 8 * as);
-          }
-          bd_kb += b_kb_step;
-          if (++stage == S) {
-            stage = 0; full_par ^= 1u; ad_stage = a_desc0;
-          } else {
-            ad_stage += a_step;
-          }
-        }
-      }
-    }
-  } else if (warp >= kEpiWarp0) {
-    // =============================== epilogue ====================================
-    const int quad = warp & 3;
-    const int group = (warp - kEpiWarp0) >> 2;
-    const int row = quad * 32 + lane;
-    const int py = row / kHaloTileW, px = row - py * kHaloTileW;
-    int ti = 0;
-    for (int t = rank; t < spatial_tiles; t += nrank, ++ti) {
-      if ((ti & 1) != group) continue;
-      int img, y0, x0;
-      decode(t, img, y0, x0);
-      const int as = ti % Cfg::kAccStages;
-      const int gy = y0 + py, gx = x0 + px;
-      const bool valid = gy < g.gh && gx < g.gw;
-      const int ph_y = phase >> 1, ph_x = phase & 1;
-      const int oy = gy * g.out_mul + ph_y, ox = gx * g.out_mul + ph_x;
-      ResChunk rc;
-      if constexpr (BN >= 64) {
-        if (p.use_tma_store && g.residual)
-          load_res_chunk(rc, p.dst + (size_t(img) * g.dst_h * g.dst_w + size_t(valid ? oy : 0) * g.dst_w + (valid ? ox : 0)) * g.dst_cstride + g.dst_coff);
-      }
-      mbar_wait_relaxed(tmem_full_bar + 8 * as, (ti / Cfg::kAccStages) & 1);
-      tc_fence_after();
-      const uint32_t tmem_row = tmem_base + uint32_t(as * BN) + (uint32_t(quad * 32) << 16);
-      if constexpr (BN == 16) {
-        // seg tail: 4 phase logits per grid pixel -> sigmoid -> 2x2 block of the f32 and u8 masks
-        uint32_t v[16];
-        tmem_ld_32x16(tmem_row, v);
-        tmem_ld_wait();
-        if (valid) {
+    if constexpr (BN == 16) {
+      if (p.seg_f32 != nullptr) {
+        // seg tail: 4 phase logits per grid pixel -> sigmoid -> one row (py2 = the column pair lane & 3) of the
+        // pixel's 2x2 block in the f32 and u8 masks
+        const int py2 = lane & 3;
+        if (py2 < 2) {
           const size_t ow2 = size_t(g.gw) * 2;
-          const size_t o0 = (size_t(img) * g.gh * 2 + size_t(gy) * 2) * ow2 + size_t(gx) * 2;
 #pragma unroll
-          for (int py2 = 0; py2 < 2; ++py2) {
-            const float s0 = 1.0f / (1.0f + expf(-__uint_as_float(v[py2 * 2])));
-            const float s1 = 1.0f / (1.0f + expf(-__uint_as_float(v[py2 * 2 + 1])));
-            *reinterpret_cast<float2*>(p.seg_f32 + o0 + py2 * ow2) = make_float2(s0, s1);
-            *reinterpret_cast<uchar2*>(p.seg_u8 + o0 + py2 * ow2) = make_uchar2((uint8_t)(s0 * 255.0f), (uint8_t)(s1 * 255.0f));
+          for (int h = 0; h < 2; ++h) {
+            if (!valid[h]) continue;
+            const size_t o = (size_t(img) * g.gh * 2 + size_t(gy[h]) * 2 + py2) * ow2 + size_t(gx[h]) * 2;
+            const float s0 = 1.0f / (1.0f + expf(-acc[2 * h]));
+            const float s1 = 1.0f / (1.0f + expf(-acc[2 * h + 1]));
+            *reinterpret_cast<float2*>(p.seg_f32 + o) = make_float2(s0, s1);
+            *reinterpret_cast<uchar2*>(p.seg_u8 + o) = make_uchar2((uint8_t)(s0 * 255.0f), (uint8_t)(s1 * 255.0f));
           }
         }
-        tc_fence_before();
-        mbar_arrive(tmem_empty_bar + 8 * as);
         continue;
       }
-      __half* out = p.dst + (size_t(img) * g.dst_h * g.dst_w + size_t(valid ? oy : 0) * g.dst_w + (valid ? ox : 0)) * g.dst_cstride +
-                    g.dst_coff;
-      bool done_tma = false;
-      if constexpr (BN >= 64) {
-        if (p.use_tma_store) {
-          const uint32_t stage_base = store_base + uint32_t(group) * (128u * 128u);
-          const bool leader = (threadIdx.x & 127) == 0;
-          const CUtensorMap* om = &p.o_map[phase];
-#define CTD_EPT(ACT)                                                                                              \
-  if (g.residual) epilogue_store_tma<BN, ACT, true>(tmem_row, bias_s, out, stage_base, row, om, 0, x0, y0, img, 1 + group, leader, rc); \
-  else epilogue_store_tma<BN, ACT, false>(tmem_row, bias_s, out, stage_base, row, om, 0, x0, y0, img, 1 + group, leader, rc);
-          switch (g.act) {
-            case CTD_ACT_SILU: CTD_EPT(CTD_ACT_SILU) break;
-            case CTD_ACT_LEAKY: CTD_EPT(CTD_ACT_LEAKY) break;
-            case CTD_ACT_RELU: CTD_EPT(CTD_ACT_RELU) break;
-            case CTD_ACT_SIGMOID: CTD_EPT(CTD_ACT_SIGMOID) break;
-            default: CTD_EPT(CTD_ACT_NONE) break;
-          }
-#undef CTD_EPT
-          done_tma = true;
-        }
-      }
-      if (!done_tma) {
-#define CTD_EPI(ACT)                                                                              \
-  if (g.residual) epilogue_store<BN, ACT, true>(tmem_row, bias_s, out, g.cout, valid);            \
-  else epilogue_store<BN, ACT, false>(tmem_row, bias_s, out, g.cout, valid);
-        switch (g.act) {
-          case CTD_ACT_SILU: CTD_EPI(CTD_ACT_SILU) break;
-          case CTD_ACT_LEAKY: CTD_EPI(CTD_ACT_LEAKY) break;
-          case CTD_ACT_RELU: CTD_EPI(CTD_ACT_RELU) break;
-          case CTD_ACT_SIGMOID: CTD_EPI(CTD_ACT_SIGMOID) break;
-          default: CTD_EPI(CTD_ACT_NONE) break;
-        }
-#undef CTD_EPI
-      }
-      tc_fence_before();
-      mbar_arrive(tmem_empty_bar + 8 * as);
     }
-    if (p.use_tma_store && (threadIdx.x & 127) == 0) tma_store_wait_all();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-
-// =========================================================================================
-// Halo activations + streamed weights (BN = 128 / 256).  The wide 3x3 convolutions and deconvolution phases are
-// bound by L2 -> shared-memory operand traffic in conv_tc_kernel (every tap re-fetches its 16 KB activation box).
-// Here the activation halo block of a K block is fetched ONCE (A ring) and viewed per tap exactly as in
-// conv_halo_kernel, while the weights (too large to stay resident) stream through their own ring, one
-// BN x 64-channel box per (K block, tap).  Operand bytes per K block drop from taps*(16 KB + BN*128 B) to
-// 23 KB + taps*BN*128 B.
-template <int BN>
-struct HsCfg {
-  static constexpr int kAStages = BN >= 256 ? 2 : 3;
-  static constexpr int kBStages = BN >= 256 ? 4 : 7;
-  static constexpr int kAStageBytes = 24 * 1024;              // 10 x 18 halo rows of 128 B, 1024-aligned
-  static constexpr int kBBytes = BN * 128;
-  static constexpr int kAccStages = 512 / BN;
-  static constexpr int kTmemCols = 512;
-  static constexpr int kStoreBytes = 2 * 128 * 128;
-  static constexpr int kBiasFloats = 512;
-  static constexpr size_t kSmem = 1024 + size_t(kAStages) * kAStageBytes + size_t(kBStages) * kBBytes + 512 + kBiasFloats * 4 +
-                                  1024 + kStoreBytes;
-};
-
-template <int BN>
-__global__ void __launch_bounds__(kThreads, 1) conv_hs_kernel(const __grid_constant__ ConvTcParams p) {
-  using Cfg = HsCfg<BN>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t a_base = smem_base;
-  const uint32_t b_base = a_base + Cfg::kAStages * Cfg::kAStageBytes;
-  const uint32_t bar_base = b_base + Cfg::kBStages * Cfg::kBBytes;
-  // barriers: a_full[4] | a_empty[4] | b_full[8] | b_empty[8] | tmem_full[4] | tmem_empty[4] | tmem ptr
-  const uint32_t a_full = bar_base, a_empty = bar_base + 32, b_full = bar_base + 64, b_empty = bar_base + 128;
-  const uint32_t tmem_full_bar = bar_base + 192, tmem_empty_bar = bar_base + 224, tmem_ptr_addr = bar_base + 256;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const size_t bar_off = size_t(Cfg::kAStages) * Cfg::kAStageBytes + size_t(Cfg::kBStages) * Cfg::kBBytes;
-  volatile uint32_t* tmem_ptr_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + bar_off + 256);
-  float* bias_s = reinterpret_cast<float*>(smem_gen + bar_off + 512);
-  const uint32_t store_base = (bar_base + 512u + uint32_t(Cfg::kBiasFloats) * 4u + 1023u) & ~1023u;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const ConvGeom& g = p.g;
-  constexpr int kb = 64;
-  constexpr uint32_t row_bytes = 128;
-  const int lox = p.halo_lox, loy = p.halo_loy;
-  const int halo_w = p.halo_w, halo_h = p.halo_h;
-  const uint32_t a_tx = uint32_t(halo_w * halo_h) * row_bytes;
-  constexpr uint32_t b_tx = uint32_t(BN) * row_bytes;
-  int kblocks = 0;
-  for (int s = 0; s < g.n_src; ++s) kblocks += p.src_kblocks[s];
-  const int tiles_per_img = p.tiles_x * p.tiles_y;
-  const int n_nblk = g.cout_pad / BN;
-  const int spatial_tiles = g.n_img * tiles_per_img;
-  const int total_tiles = spatial_tiles * n_nblk * g.n_phase;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < g.n_src; ++s) prefetch_tensormap(&p.a_map[s][0]);
-    prefetch_tensormap(&p.b_map);
-    if (p.use_tma_store)
-      for (int q = 0; q < g.n_phase; ++q) prefetch_tensormap(&p.o_map[q]);
-    for (int s = 0; s < Cfg::kAStages; ++s) { mbar_init(a_full + 8 * s, 1); mbar_init(a_empty + 8 * s, 1); }
-    for (int s = 0; s < Cfg::kBStages; ++s) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, 1); }
-    for (int s = 0; s < Cfg::kAccStages; ++s) { mbar_init(tmem_full_bar + 8 * s, 1); mbar_init(tmem_empty_bar + 8 * s, 128); }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_ptr_addr, Cfg::kTmemCols);
-  for (int i = threadIdx.x; i < g.cout_pad && i < Cfg::kBiasFloats; i += kThreads) bias_s[i] = p.bias[i];
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_gen;
-  griddep_launch_dependents();   // successors may begin their prologue as our CTAs retire
-  griddep_wait();                // activations / residuals written by the predecessor are visible from here on
-
-  // tile index -> (phase, spatial tile, n block), n block fastest (CTAs running together share the halo in L2)
-  auto decode = [&](int t, int& phase, int& nblk, int& img, int& y0, int& x0) {
-    nblk = t % n_nblk;
-    const int r = t / n_nblk;
-    const int sp = r % spatial_tiles;
-    phase = r / spatial_tiles;
-    img = sp / tiles_per_img;
-    const int trem = sp - img * tiles_per_img;
-    const int ty = trem / p.tiles_x;
-    y0 = ty * kHaloTileH;
-    x0 = (trem - ty * p.tiles_x) * kHaloTileW;
-  };
-
-  if (warp == 0) {
-    // =============================== TMA producer ===============================
-    if (elect_one()) {
-      int ia = 0, ib = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-        int phase, nblk, img, y0, x0;
-        decode(t, phase, nblk, img, y0, x0);
-        int kbi = 0;
-        for (int s = 0; s < g.n_src; ++s)
-          for (int cb = 0; cb < p.src_kblocks[s]; ++cb, ++kbi, ++ia) {
-            const int sa = ia % Cfg::kAStages;
-            mbar_wait_relaxed(a_empty + 8 * sa, ((ia / Cfg::kAStages) & 1) ^ 1);
-            mbar_arrive_expect_tx(a_full + 8 * sa, a_tx);
-            tma_load_4d(a_base + sa * Cfg::kAStageBytes, &p.a_map[s][0], a_full + 8 * sa, cb * kb, x0 - lox, y0 - loy, img);
-            for (int tap = 0; tap < g.taps; ++tap, ++ib) {
-              const int sb = ib % Cfg::kBStages;
-              mbar_wait_relaxed(b_empty + 8 * sb, ((ib / Cfg::kBStages) & 1) ^ 1);
-              mbar_arrive_expect_tx(b_full + 8 * sb, b_tx);
-              tma_load_2d(b_base + sb * Cfg::kBBytes, &p.b_map, b_full + 8 * sb, tap * g.cin_total + kbi * kb,
-                          phase * g.cout_pad + nblk * BN);
-            }
-          }
-      }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer =================================
-    const uint32_t idesc = make_idesc_f16(BN);
-    const uint32_t sbo = uint32_t(halo_w) * row_bytes;
-    const bool leader = elect_one();
-    const uint64_t a_desc0 = make_kmajor_desc_ex(a_base, row_bytes, sbo, 0u);
-    const uint64_t b_desc0 = make_kmajor_desc(b_base, row_bytes);
-    // The whole loop runs on the ONE issuing lane (no per-tap reconvergence), with the per-tap operand views of the
-    // tile's phase precomputed into registers: the issuing thread's instruction stream, not the tensor pipe, was the
-    // limiter of this kernel (~70 SASS instructions per tap before, ncu source view).
-    if (leader) {
-      int sa = 0, sb = 0, ti = 0;
-      uint32_t a_par = 0, b_par = 0;
-      uint64_t ad_stage = a_desc0, bd = b_desc0;
-      const int ntaps = g.taps;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++ti) {
-        const int phase = (t / n_nblk) / spatial_tiles;
-        uint32_t tap_a[kMaxTaps];
+    if (p.dst == nullptr) {
+      // Detect decode (yolo.py:36-44): columns = anchor*(5+nc) + o
+      const int no = 5 + p.nc;
+      float* rows = p.blks + (size_t(img) * p.blks_rows_per_img + p.level_row0) * no;
 #pragma unroll
-        for (int tap = 0; tap < kMaxTaps; ++tap) {
-          const int dy = tap < ntaps ? g.tap_dy[phase][tap] : 0, dx = tap < ntaps ? g.tap_dx[phase][tap] : 0;
-          tap_a[tap] = (uint32_t((dy + loy) * halo_w + (dx + lox)) * row_bytes) >> 4;
-        }
-        const int as = ti % Cfg::kAccStages;
-        mbar_wait(tmem_empty_bar + 8 * as, ((ti / Cfg::kAccStages) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + uint32_t(as * BN);
-        uint32_t acc = 0u;
-        for (int kbi = 0; kbi < kblocks; ++kbi) {
-          mbar_wait(a_full + 8 * sa, a_par);
+      for (int h = 0; h < 2; ++h) {
+        if (!valid[h]) continue;
 #pragma unroll
-          for (int tap = 0; tap < kMaxTaps; ++tap) {
-            if (tap >= ntaps) break;
-            mbar_wait(b_full + 8 * sb, b_par);
-            tc_fence_after();
-            issue_kblock(tmem_d, ad_stage + tap_a[tap], bd, idesc, acc, 4);
-            acc = 1u;
-            umma_commit(b_empty + 8 * sb);
-            if (++sb == Cfg::kBStages) { sb = 0; b_par ^= 1u; bd = b_desc0; } else { bd += uint64_t(Cfg::kBBytes >> 4); }
-          }
-          umma_commit(a_empty + 8 * sa);
-          if (kbi == kblocks - 1) umma_commit(tmem_full_bar + 8 * as);
-          if (++sa == Cfg::kAStages) { sa = 0; a_par ^= 1u; ad_stage = a_desc0; } else { ad_stage += uint64_t(Cfg::kAStageBytes >> 4); }
+        for (int i = 0; i < R; ++i) {
+          if (((i >> 1) & 1) != h) continue;
+          const int c = (i >> 2) * 8 + (lane & 3) * 2 + (i & 1);
+          if (c >= ncols) continue;
+          const int col = nblk * BN + c;
+          const int a = col / no, o = col - a * no;
+          const float s = 1.0f / (1.0f + expf(-(acc[i] + bias_t[c])));
+          float r;
+          if (o == 0) r = (s * 2.0f - 0.5f + float(gx[h])) * p.det_stride;
+          else if (o == 1) r = (s * 2.0f - 0.5f + float(gy[h])) * p.det_stride;
+          else if (o == 2) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a];
+          else if (o == 3) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a + 1];
+          else r = s;
+          rows[(size_t(a) * g.gh * g.gw + size_t(gy[h]) * g.gw + gx[h]) * no + o] = r;
         }
       }
-    }
-  } else if (warp >= kEpiWarp0) {
-    // =============================== epilogue ====================================
-    const int quad = warp & 3;
-    const int group = (warp - kEpiWarp0) >> 2;
-    const int row = quad * 32 + lane;
-    const int py = row / kHaloTileW, px = row - py * kHaloTileW;
-    int ti = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++ti) {
-      if ((ti & 1) != group) continue;
-      int phase, nblk, img, y0, x0;
-      decode(t, phase, nblk, img, y0, x0);
-      const int as = ti % Cfg::kAccStages;
-      const int gy = y0 + py, gx = x0 + px;
-      const bool valid = gy < g.gh && gx < g.gw;
-      const int ph_y = phase >> 1, ph_x = phase & 1;
-      const int oy = gy * g.out_mul + ph_y, ox = gx * g.out_mul + ph_x;
-      __half* out = p.dst + (size_t(img) * g.dst_h * g.dst_w + size_t(valid ? oy : 0) * g.dst_w + (valid ? ox : 0)) * g.dst_cstride +
-                    g.dst_coff + nblk * BN;
-      ResChunk rc;
-      if (g.residual) load_res_chunk(rc, out);
-      const float* bias_t = bias_s + nblk * BN;
-      mbar_wait_relaxed(tmem_full_bar + 8 * as, (ti / Cfg::kAccStages) & 1);
-      tc_fence_after();
-      const uint32_t tmem_row = tmem_base + uint32_t(as * BN) + (uint32_t(quad * 32) << 16);
-      const uint32_t stage_base = store_base + uint32_t(group) * (128u * 128u);
-      const bool lead = (threadIdx.x & 127) == 0;
-      const CUtensorMap* om = &p.o_map[phase];
-#define CTD_EPT(ACT)                                                                                              \
-  if (g.residual) epilogue_store_tma<BN, ACT, true>(tmem_row, bias_t, out, stage_base, row, om, nblk * BN, x0, y0, img, 1 + group, lead, rc); \
-  else epilogue_store_tma<BN, ACT, false>(tmem_row, bias_t, out, stage_base, row, om, nblk * BN, x0, y0, img, 1 + group, lead, rc);
+    } else if (p.split) {
+      float* out32[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        out32[h] = reinterpret_cast<float*>(p.dst) + pix[h] * g.dst_cstride + g.dst_coff + nblk * BN;
+      const bool res = g.residual != 0;
       switch (g.act) {
-        case CTD_ACT_SILU: CTD_EPT(CTD_ACT_SILU) break;
-        case CTD_ACT_LEAKY: CTD_EPT(CTD_ACT_LEAKY) break;
-        case CTD_ACT_RELU: CTD_EPT(CTD_ACT_RELU) break;
-        case CTD_ACT_SIGMOID: CTD_EPT(CTD_ACT_SIGMOID) break;
-        default: CTD_EPT(CTD_ACT_NONE) break;
+        case CTD_ACT_SILU: epilogue_f32<BN, CTD_ACT_SILU>(acc, bias_t, out32, valid, ncols, lane, res); break;
+        case CTD_ACT_LEAKY: epilogue_f32<BN, CTD_ACT_LEAKY>(acc, bias_t, out32, valid, ncols, lane, res); break;
+        case CTD_ACT_RELU: epilogue_f32<BN, CTD_ACT_RELU>(acc, bias_t, out32, valid, ncols, lane, res); break;
+        case CTD_ACT_SIGMOID: epilogue_f32<BN, CTD_ACT_SIGMOID>(acc, bias_t, out32, valid, ncols, lane, res); break;
+        default: epilogue_f32<BN, CTD_ACT_NONE>(acc, bias_t, out32, valid, ncols, lane, res); break;
       }
-#undef CTD_EPT
-      tc_fence_before();
-      mbar_arrive(tmem_empty_bar + 8 * as);
-    }
-    if ((threadIdx.x & 127) == 0) tma_store_wait_all();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
-}
-
-
-// =========================================================================================
-// Swapped-operand variant for 128 output channels (conv_sw_kernel).  D^T[128 couts x 256 pixels]: the weight box of a
-// (K block, tap) is the M=128 operand, the activation halo block viewed per tap is the N=256 operand (tile 8 x 32
-// pixels; the same descriptor trick as conv_halo_kernel, SBO = halo width).  One tcgen05.mma therefore covers
-// 256 pixels x 128 channels instead of 128 x 128 -- the issue cost per FLOP halves for the 128-wide layers.
-// Accumulator lanes are CHANNELS, columns are pixels: each epilogue thread owns one channel, adds its bias, applies the
-// activation and writes fp16 into a [pixel][128 channels] staging block (32 pixels = 8 KB at a time, double buffered),
-// which a TMA store (no swizzle, 256-byte rows) scatters into the NHWC destination.
-constexpr int kSwTileW = 8, kSwTileH = 32;
-struct SwCfg {
-  static constexpr int kActStages = 2;
-  static constexpr int kActStageBytes = 44 * 1024;   // (8+2) x (32+2) halo rows of 128 B = 43520, 1024-aligned
-  static constexpr int kWStages = 6;
-  static constexpr int kWBytes = 128 * 128;          // 128 couts x 64 channels
-  static constexpr int kAccStages = 2;               // 2 x 256 TMEM columns
-  static constexpr int kTmemCols = 512;
-  static constexpr int kChunkBytes = 32 * 256;       // 32 pixels x 128 channels fp16
-  static constexpr int kStoreBytes = 2 * 2 * kChunkBytes;   // two epilogue warpgroups x two buffers
-  static constexpr size_t kSmem = size_t(kActStages) * kActStageBytes + size_t(kWStages) * kWBytes + kStoreBytes + 512 + 512;
-};
-
-template <int ACT, bool RES>
-__device__ __forceinline__ void sw_store_chunk(const uint32_t (&v)[32], const unsigned short (&res)[32], float bias, uint32_t buf,
-                                               int co) {
+    } else {
+      __half* out[2];
+      const __half* res[2];   // residual: read from the destination itself (in-place add)
 #pragma unroll
-  for (int j = 0; j < 32; ++j) {
-    float f = apply_act<ACT>(__uint_as_float(v[j]) + bias);
-    if constexpr (RES) f += __half2float(__ushort_as_half(res[j]));
-    const unsigned short bits = __half_as_ushort(__float2half_rn(f));
-    asm volatile("st.shared.b16 [%0], %1;" ::"r"(buf + uint32_t(j) * 256u + uint32_t(co) * 2u), "h"(bits) : "memory");
-  }
-}
-
-__global__ void __launch_bounds__(kThreads, 1) conv_sw_kernel(const __grid_constant__ ConvTcParams p) {
-  using Cfg = SwCfg;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t act_base = smem_base;
-  const uint32_t w_base = act_base + Cfg::kActStages * Cfg::kActStageBytes;
-  const uint32_t store_base = w_base + Cfg::kWStages * Cfg::kWBytes;
-  const uint32_t bar_base = store_base + Cfg::kStoreBytes;
-  // barriers: act_full[4] | act_empty[4] | w_full[8] | w_empty[8] | tmem_full[4] | tmem_empty[4] | tmem ptr
-  const uint32_t act_full = bar_base, act_empty = bar_base + 32, w_full = bar_base + 64, w_empty = bar_base + 128;
-  const uint32_t tmem_full_bar = bar_base + 192, tmem_empty_bar = bar_base + 224, tmem_ptr_addr = bar_base + 256;
-  uint8_t* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-  const size_t bar_off = size_t(Cfg::kActStages) * Cfg::kActStageBytes + size_t(Cfg::kWStages) * Cfg::kWBytes + Cfg::kStoreBytes;
-  volatile uint32_t* tmem_ptr_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + bar_off + 256);
-  float* bias_s = reinterpret_cast<float*>(smem_gen + bar_off + 512);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const ConvGeom& g = p.g;
-  constexpr int kb = 64;
-  constexpr uint32_t row_bytes = 128;
-  const int lox = p.halo_lox, loy = p.halo_loy;
-  const int halo_w = p.halo_w, halo_h = p.halo_h;
-  const uint32_t act_tx = uint32_t(halo_w * halo_h) * row_bytes;
-  constexpr uint32_t w_tx = 128u * row_bytes;
-  int kblocks = 0;
-  for (int s = 0; s < g.n_src; ++s) kblocks += p.src_kblocks[s];
-  const int tiles_per_img = p.tiles_x * p.tiles_y;
-  const int spatial_tiles = g.n_img * tiles_per_img;
-  const int total_tiles = spatial_tiles * g.n_phase;
-
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < g.n_src; ++s) prefetch_tensormap(&p.a_map[s][0]);
-    prefetch_tensormap(&p.b_map);
-    for (int q = 0; q < g.n_phase; ++q) prefetch_tensormap(&p.o_map[q]);
-    for (int s = 0; s < Cfg::kActStages; ++s) { mbar_init(act_full + 8 * s, 1); mbar_init(act_empty + 8 * s, 1); }
-    for (int s = 0; s < Cfg::kWStages; ++s) { mbar_init(w_full + 8 * s, 1); mbar_init(w_empty + 8 * s, 1); }
-    for (int s = 0; s < Cfg::kAccStages; ++s) { mbar_init(tmem_full_bar + 8 * s, 1); mbar_init(tmem_empty_bar + 8 * s, 128); }
-    fence_barrier_init();
-  }
-  if (warp == 2) tmem_alloc(tmem_ptr_addr, Cfg::kTmemCols);
-  for (int i = threadIdx.x; i < 128; i += kThreads) bias_s[i] = i < g.cout_pad ? p.bias[i] : 0.f;
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_gen;
-  griddep_launch_dependents();
-  griddep_wait();
-
-  auto decode = [&](int t, int& phase, int& img, int& y0, int& x0) {
-    const int sp = t % spatial_tiles;
-    phase = t / spatial_tiles;
-    img = sp / tiles_per_img;
-    const int trem = sp - img * tiles_per_img;
-    const int ty = trem / p.tiles_x;
-    y0 = ty * kSwTileH;
-    x0 = (trem - ty * p.tiles_x) * kSwTileW;
-  };
-
-  if (warp == 0) {
-    // =============================== TMA producer ===============================
-    if (elect_one()) {
-      int ia = 0, iw = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-        int phase, img, y0, x0;
-        decode(t, phase, img, y0, x0);
-        int kbi = 0;
-        for (int s = 0; s < g.n_src; ++s)
-          for (int cb = 0; cb < p.src_kblocks[s]; ++cb, ++kbi, ++ia) {
-            const int sa = ia % Cfg::kActStages;
-            mbar_wait_relaxed(act_empty + 8 * sa, ((ia / Cfg::kActStages) & 1) ^ 1);
-            mbar_arrive_expect_tx(act_full + 8 * sa, act_tx);
-            tma_load_4d(act_base + sa * Cfg::kActStageBytes, &p.a_map[s][0], act_full + 8 * sa, cb * kb, x0 - lox, y0 - loy, img);
-            for (int tap = 0; tap < g.taps; ++tap, ++iw) {
-              const int sw = iw % Cfg::kWStages;
-              mbar_wait_relaxed(w_empty + 8 * sw, ((iw / Cfg::kWStages) & 1) ^ 1);
-              mbar_arrive_expect_tx(w_full + 8 * sw, w_tx);
-              tma_load_2d(w_base + sw * Cfg::kWBytes, &p.b_map, w_full + 8 * sw, tap * g.cin_total + kbi * kb, phase * g.cout_pad);
-            }
-          }
+      for (int h = 0; h < 2; ++h) {
+        out[h] = p.dst + pix[h] * g.dst_cstride + g.dst_coff + nblk * BN;
+        res[h] = out[h];
       }
-    }
-  } else if (warp == 1) {
-    // =============================== MMA issuer (one lane) =======================
-    if (elect_one()) {
-      const uint32_t idesc = make_idesc_f16(256);
-      const uint32_t sbo = uint32_t(halo_w) * row_bytes;
-      const uint64_t act_desc0 = make_kmajor_desc_ex(act_base, row_bytes, sbo, 0u);   // N operand: halo views
-      const uint64_t w_desc0 = make_kmajor_desc(w_base, row_bytes);                    // M operand: weight box
-      int sa = 0, sw = 0, ti = 0;
-      uint32_t a_par = 0, w_par = 0;
-      uint64_t act_stage = act_desc0, wd = w_desc0;
-      const int ntaps = g.taps;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++ti) {
-        const int phase = t / spatial_tiles;
-        uint32_t tap_off[kMaxTaps];
-#pragma unroll
-        for (int tap = 0; tap < kMaxTaps; ++tap) {
-          const int dy = tap < ntaps ? g.tap_dy[phase][tap] : 0, dx = tap < ntaps ? g.tap_dx[phase][tap] : 0;
-          tap_off[tap] = (uint32_t((dy + loy) * halo_w + (dx + lox)) * row_bytes) >> 4;
-        }
-        const int as = ti & 1;
-        mbar_wait(tmem_empty_bar + 8 * as, ((ti >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + uint32_t(as * 256);
-        uint32_t acc = 0u;
-        for (int kbi = 0; kbi < kblocks; ++kbi) {
-          mbar_wait(act_full + 8 * sa, a_par);
-#pragma unroll
-          for (int tap = 0; tap < kMaxTaps; ++tap) {
-            if (tap >= ntaps) break;
-            mbar_wait(w_full + 8 * sw, w_par);
-            tc_fence_after();
-            issue_kblock(tmem_d, wd, act_stage + tap_off[tap], idesc, acc, 4);   // A = weights, B = pixels
-            acc = 1u;
-            umma_commit(w_empty + 8 * sw);
-            if (++sw == Cfg::kWStages) { sw = 0; w_par ^= 1u; wd = w_desc0; } else { wd += uint64_t(Cfg::kWBytes >> 4); }
-          }
-          umma_commit(act_empty + 8 * sa);
-          if (kbi == kblocks - 1) umma_commit(tmem_full_bar + 8 * as);
-          if (++sa == Cfg::kActStages) { sa = 0; a_par ^= 1u; act_stage = act_desc0; }
-          else { act_stage += uint64_t(Cfg::kActStageBytes >> 4); }
-        }
+#define CTD_EPI(ACT)                                                                            \
+  if (g.residual) epilogue_f16<BN, ACT, true>(acc, bias_t, out, res, valid, ncols, lane);      \
+  else epilogue_f16<BN, ACT, false>(acc, bias_t, out, res, valid, ncols, lane);
+      switch (g.act) {
+        case CTD_ACT_SILU: CTD_EPI(CTD_ACT_SILU) break;
+        case CTD_ACT_LEAKY: CTD_EPI(CTD_ACT_LEAKY) break;
+        case CTD_ACT_RELU: CTD_EPI(CTD_ACT_RELU) break;
+        case CTD_ACT_SIGMOID: CTD_EPI(CTD_ACT_SIGMOID) break;
+        default: CTD_EPI(CTD_ACT_NONE) break;
       }
+#undef CTD_EPI
     }
-  } else if (warp >= kEpiWarp0) {
-    // =============================== epilogue (channel-major accumulators) ========
-    const int quad = warp & 3;
-    const int group = (warp - kEpiWarp0) >> 2;
-    const int co = quad * 32 + lane;                   // this thread's output channel
-    const float bias = bias_s[co];
-    const bool lead = (threadIdx.x & 127) == 0;
-    const uint32_t buf0 = store_base + uint32_t(group) * (2u * Cfg::kChunkBytes);
-    int ti = 0, nchunk = 0;
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, ++ti) {
-      if ((ti & 1) != group) continue;
-      int phase, img, y0, x0;
-      decode(t, phase, img, y0, x0);
-      const int as = ti & 1;
-      mbar_wait_relaxed(tmem_full_bar + 8 * as, (ti >> 1) & 1);
-      tc_fence_after();
-      const uint32_t tmem_row = tmem_base + uint32_t(as * 256) + (uint32_t(quad * 32) << 16);
-      const CUtensorMap* om = &p.o_map[phase];
-#pragma unroll 1
-      for (int c = 0; c < 8; ++c, ++nchunk) {         // 32 pixels = tile rows 4c .. 4c+3
-        // Bottleneck residual: this thread's channel of the 32 pixels of the chunk (a warp reads 64 contiguous bytes
-        // per pixel), issued before the TMEM read so the loads are in flight under it
-        unsigned short res[32];
-        if (g.residual) {
-          const int ph_y = phase >> 1, ph_x = phase & 1;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int gy = y0 + 4 * c + (j >> 3), gx = x0 + (j & 7);
-            const bool ok = gy < g.gh && gx < g.gw;
-            const size_t off = ((size_t(img) * g.dst_h + size_t(ok ? gy * g.out_mul + ph_y : 0)) * g.dst_w +
-                                size_t(ok ? gx * g.out_mul + ph_x : 0)) * g.dst_cstride + g.dst_coff + co;
-            res[j] = *reinterpret_cast<const unsigned short*>(p.dst + off);
-          }
-        }
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_row + uint32_t(c * 32), v);
-        tmem_ld_wait();
-        const uint32_t buf = buf0 + uint32_t(nchunk & 1) * Cfg::kChunkBytes;
-        if (lead) tma_store_wait_read1();             // the store that used this buffer two chunks ago has drained
-        named_barrier_sync(1 + group, 128);
-#define CTD_SW(ACT)                                                                  \
-  if (g.residual) sw_store_chunk<ACT, true>(v, res, bias, buf, co);                  \
-  else sw_store_chunk<ACT, false>(v, res, bias, buf, co);
-        switch (g.act) {
-          case CTD_ACT_SILU: CTD_SW(CTD_ACT_SILU) break;
-          case CTD_ACT_LEAKY: CTD_SW(CTD_ACT_LEAKY) break;
-          case CTD_ACT_RELU: CTD_SW(CTD_ACT_RELU) break;
-          case CTD_ACT_SIGMOID: CTD_SW(CTD_ACT_SIGMOID) break;
-          default: CTD_SW(CTD_ACT_NONE) break;
-        }
-#undef CTD_SW
-        fence_proxy_async();
-        named_barrier_sync(1 + group, 128);
-        if (lead) {
-          tma_store_4d(om, buf, 0, x0, y0 + 4 * c, img);
-          tma_store_commit();
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(tmem_empty_bar + 8 * as);
-    }
-    if (lead) tma_store_wait_all();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
   }
 }
 
@@ -1381,26 +419,25 @@ static const char* encode_map(PFN_encodeTiled enc, CUtensorMap* m, const void* b
   return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled failed";
 }
 
-static const char* encode_map_noswizzle(PFN_encodeTiled enc, CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims,
-                                        const cuuint64_t* strides_bytes, const cuuint32_t* box) {
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled (no swizzle) failed";
-}
+static int g_num_sms = 132;
+static int g_use_pdl = 0;   // CTD_PDL=1 enables programmatic dependent launch
 
-static int g_num_sms = 148;
-static int g_sw_residual = 0;   // CTD_SW_RESIDUAL=1 routes residual 128-wide layers through conv_sw_kernel too
-static int g_use_pdl = 0;   // CTD_PDL=1 enables programmatic dependent launch (measured: no gain once a second
-                            // workspace fills the tails -- early dependents park on SMs the other batch could use)
-
+// N block: at most 128 output channels, so that a consumer warpgroup's 64 x BN fp32 accumulator fits in registers
+// (64 per thread) next to the epilogue's addresses
 static int pick_block_n(int cout_pad) {
-  if (cout_pad >= 256 && cout_pad % 256 == 0) return 256;
   if (cout_pad >= 128 && cout_pad % 128 == 0) return 128;
   if (cout_pad % 64 == 0) return 64;
   if (cout_pad % 32 == 0) return 32;
   return 16;
+}
+
+static size_t smem_for(int bn) {
+  switch (bn) {
+    case 128: return TcCfg<128>::kSmem;
+    case 64: return TcCfg<64>::kSmem;
+    case 32: return TcCfg<32>::kSmem;
+    default: return TcCfg<16>::kSmem;
+  }
 }
 
 const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
@@ -1462,27 +499,12 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
       }
     }
   int bn = pick_block_n(g.cout_pad);
-  // small grids (the 1/32 and 1/64 layers): a narrower N block spreads the layer over more SMs -- each CTA streams a
-  // quarter of the weights and runs a quarter of the epilogue, which is what the time of a one-tile CTA consists of
+  // small grids (the 1/32 and 1/64 layers): a narrower N block spreads the layer over more SMs
   while (bn > 64 && g.n_img * p.tiles_x * p.tiles_y * (g.cout_pad / bn) * g.n_phase <= g_num_sms / 2) bn /= 2;
-  if (split && bn > 64) bn = 64;   // promoted accumulation keeps a BN-float row per epilogue thread in registers
+  if (split && bn > 64) bn = 64;   // promoted accumulation keeps three BN/2-float fragments per thread in registers
   plan.block_n = bn;
-  p.use_tma_store = 0;
   if (split && ((g.dst_coff % 4) != 0 || (g.dst_cstride % 4) != 0 || (dst != nullptr && g.cout % 4 != 0)))
     return "conv_tc (split): fp32 destination slice must be 16-byte aligned";
-  if (!split && bn >= 64 && dst != nullptr && g.cout % 64 == 0) {
-    // destination slice as a 4-D tensor (channels of this op, x, y, image); deconv phases are parity views
-    const size_t cs = size_t(g.dst_cstride);
-    for (int ph = 0; ph < g.n_phase; ++ph) {
-      const int py = ph >> 1, px = ph & 1;
-      cuuint64_t dims[4] = {cuuint64_t(g.cout), cuuint64_t(g.gw), cuuint64_t(g.gh), cuuint64_t(g.n_img)};
-      cuuint64_t str[3] = {cs * 2 * g.out_mul, cs * 2 * g.dst_w * g.out_mul, cs * 2 * size_t(g.dst_w) * g.dst_h};
-      cuuint32_t box[4] = {64, kTileW, kTileH, 1};
-      const char* base = reinterpret_cast<const char*>(dst) + (size_t(g.dst_coff) + (size_t(py) * g.dst_w + px) * cs) * 2;
-      if (const char* e = encode_map(enc, &p.o_map[ph], base, 4, dims, str, box, 64)) return e;
-    }
-    p.use_tma_store = 1;
-  }
   {
     cuuint64_t dims[2] = {cuuint64_t(g.k_total), cuuint64_t(g.n_phase) * cuuint64_t(g.cout_pad) * n_planes};
     cuuint64_t str[1] = {cuuint64_t(g.k_total) * 2};
@@ -1494,289 +516,8 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
     plan.grid = dim3(unsigned(total_tiles < g_num_sms ? total_tiles : g_num_sms), 1, 1);
   }
   if (g.cout_pad > 512) return "conv_tc: cout_pad > 512 not supported (bias staging)";
-  switch (bn) {
-    case 256: plan.smem_bytes = TcCfg<256>::kSmem; break;
-    case 128: plan.smem_bytes = TcCfg<128>::kSmem; break;
-    case 64: plan.smem_bytes = TcCfg<64>::kSmem; break;
-    case 32: plan.smem_bytes = TcCfg<32>::kSmem; break;
-    default: plan.smem_bytes = TcCfg<16>::kSmem; break;
-  }
+  plan.smem_bytes = smem_for(bn);
   return nullptr;
-}
-
-// shared tail of the halo plans: ring depth, weight map, output maps, launch shape
-static const char* halo_finish(ConvTcPlan& plan, PFN_encodeTiled enc, const void* w16, __half* dst, int kb, int kblocks) {
-  ConvTcParams& p = plan.p;
-  const ConvGeom& g = p.g;
-  const int bn = g.cout_pad;
-  const int row_bytes = kb * 2;
-  const int w_bytes = g.taps * kblocks * bn * row_bytes;
-  const int stage_bytes = (p.halo_w * p.halo_h * row_bytes + 1023) / 1024 * 1024;
-  const size_t fixed = bn == 64 ? HaloCfg<64>::smem_bytes(w_bytes, 0, 0) : HaloCfg<32>::smem_bytes(w_bytes, 0, 0);   // 32 == 16
-  const size_t budget = 227 * 1024;
-  if (fixed + 3 * size_t(stage_bytes) > budget) return "halo: weights do not fit";
-  int stages = int((budget - fixed) / stage_bytes);
-  if (stages > kHaloMaxStages) stages = kHaloMaxStages;
-  p.halo_stages = stages; p.halo_stage_bytes = stage_bytes; p.halo_w_bytes = w_bytes;
-  p.tiles_x = (g.gw + kHaloTileW - 1) / kHaloTileW;
-  p.tiles_y = (g.gh + kHaloTileH - 1) / kHaloTileH;
-  p.use_tma_store = 0;
-  if (bn >= 64 && g.cout % 64 == 0 && dst != nullptr) {
-    const size_t cs = size_t(g.dst_cstride);
-    for (int ph = 0; ph < g.n_phase; ++ph) {
-      const int py = ph >> 1, px = ph & 1;
-      cuuint64_t dims[4] = {cuuint64_t(g.cout), cuuint64_t(g.gw), cuuint64_t(g.gh), cuuint64_t(g.n_img)};
-      cuuint64_t str[3] = {cs * 2 * g.out_mul, cs * 2 * g.dst_w * g.out_mul, cs * 2 * size_t(g.dst_w) * g.dst_h};
-      cuuint32_t box[4] = {64, kHaloTileW, kHaloTileH, 1};
-      const char* base = reinterpret_cast<const char*>(dst) + (size_t(g.dst_coff) + (size_t(py) * g.dst_w + px) * cs) * 2;
-      if (const char* e = encode_map(enc, &p.o_map[ph], base, 4, dims, str, box, 64)) return e;
-    }
-    p.use_tma_store = 1;
-  }
-  {
-    cuuint64_t dims[2] = {cuuint64_t(g.k_total), cuuint64_t(g.n_phase) * cuuint64_t(g.cout_pad)};
-    cuuint64_t str[1] = {cuuint64_t(g.k_total) * 2};
-    cuuint32_t box[2] = {cuuint32_t(kb), cuuint32_t(bn)};
-    if (const char* e = encode_map(enc, &p.b_map, w16, 2, dims, str, box, kb)) return e;
-  }
-  const int spatial_tiles = g.n_img * p.tiles_x * p.tiles_y;
-  int per_phase = g_num_sms / g.n_phase;
-  if (per_phase > spatial_tiles) per_phase = spatial_tiles;
-  if (per_phase < 1) per_phase = 1;
-  plan.grid = dim3(unsigned(per_phase * g.n_phase), 1, 1);
-  plan.block_n = bn;
-  plan.smem_bytes = bn == 64 ? HaloCfg<64>::smem_bytes(w_bytes, stages, stage_bytes) : HaloCfg<32>::smem_bytes(w_bytes, stages, stage_bytes);
-  plan.halo = 1;
-  return nullptr;
-}
-
-const char* conv_halo_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
-                           const int src_coff[], const void* w16, const float* bias, __half* dst, float* seg_f32,
-                           uint8_t* seg_u8) {
-  plan.halo = 0;
-  const bool seg = seg_f32 != nullptr && seg_u8 != nullptr;
-  if (dst == nullptr && !seg) return nullptr;
-  if (seg != (g.cout_pad == 16)) return nullptr;   // BN = 16 exists only with the seg-tail epilogue
-  const bool pw1 = g.in_stride == 1 && g.n_phase == 1 && g.taps == 1;   // 1x1: resident weights, plain 8x16 tile
-  const bool s1 = pw1 || (g.in_stride == 1 && ((g.n_phase == 1 && g.taps == 9) || (g.n_phase == 4 && g.taps == 4)));
-  const bool s2 = g.in_stride == 2 && g.n_phase == 1 && g.taps == 9 && g.src_h % 2 == 0 && g.src_w % 2 == 0;
-  if (!s1 && !s2) return nullptr;
-  if (g.cout_pad != 16 && g.cout_pad != 32 && g.cout_pad != 64) return nullptr;   // one N block per CTA, TMEM ring of 8
-  int kb = 64;
-  for (int s = 0; s < g.n_src; ++s) {
-    if (g.src_c[s] % 64 != 0) kb = 32;
-    if (g.src_c[s] % 32 != 0) return nullptr;
-    if (src_coff[s] % 8 != 0) return nullptr;
-  }
-  if (!seg && ((g.dst_coff % 8) != 0 || (g.dst_cstride % 8) != 0)) return nullptr;
-  for (int ph = 0; ph < g.n_phase; ++ph)
-    for (int t = 0; t < g.taps; ++t)
-      if (g.tap_dy[ph][t] < -1 || g.tap_dy[ph][t] > 1 || g.tap_dx[ph][t] < -1 || g.tap_dx[ph][t] > 1) return nullptr;
-  int kblocks = 0;
-  for (int s = 0; s < g.n_src; ++s) kblocks += g.src_c[s] / kb;
-  {
-    const size_t w_bytes = size_t(g.taps) * kblocks * g.cout_pad * kb * 2;
-    if (w_bytes > 110 * 1024) return nullptr;   // weights must stay resident next to >= 3 activation stages
-  }
-  ConvTcParams& p = plan.p;
-  memset(&p, 0, sizeof(p));
-  p.g = g;
-  p.kb_elems = kb;
-  for (int s = 0; s < g.n_src; ++s) p.src_kblocks[s] = g.src_c[s] / kb;
-  p.dst = dst;
-  p.bias = bias;
-  p.seg_f32 = seg_f32; p.seg_u8 = seg_u8;
-  p.halo_lox = pw1 ? 0 : 1; p.halo_loy = pw1 ? 0 : 1;
-  // stride 1: one pixel either side; stride 2: the parity views only ever reach one pixel back; 1x1: no halo
-  p.halo_w = kHaloTileW + (pw1 ? 0 : (s2 ? 1 : 2));
-  p.halo_h = kHaloTileH + (pw1 ? 0 : (s2 ? 1 : 2));
-  for (int s = 0; s < g.n_src; ++s) {
-    const size_t cs = size_t(g.src_cstride[s]);
-    const char* base = static_cast<const char*>(src_ptr[s]) + size_t(src_coff[s]) * 2;
-    cuuint32_t box[4] = {cuuint32_t(kb), cuuint32_t(p.halo_w), cuuint32_t(p.halo_h), 1};
-    if (!s2) {
-      cuuint64_t dims[4] = {cuuint64_t(g.src_c[s]), cuuint64_t(g.src_w), cuuint64_t(g.src_h), cuuint64_t(g.n_img)};
-      cuuint64_t str[3] = {cs * 2, cs * 2 * g.src_w, cs * 2 * g.src_w * g.src_h};
-      if (const char* e = encode_map(enc, &p.a_map[s][0], base, 4, dims, str, box, kb)) return e;
-    } else {
-      for (int q = 0; q < 4; ++q) {   // parity views: pixel (2*yh+yp, 2*xh+xp)
-        const int yp = q >> 1, xp = q & 1;
-        cuuint64_t dims[4] = {cuuint64_t(g.src_c[s]), cuuint64_t(g.src_w / 2), cuuint64_t(g.src_h / 2), cuuint64_t(g.n_img)};
-        cuuint64_t str[3] = {cs * 2 * 2, cs * 2 * g.src_w * 2, cs * 2 * g.src_w * g.src_h};
-        const char* b2 = base + (size_t(yp) * g.src_w + xp) * cs * 2;
-        if (const char* e = encode_map(enc, &p.a_map[s][q], b2, 4, dims, str, box, kb)) return e;
-      }
-    }
-  }
-  for (int ph = 0; ph < g.n_phase; ++ph)
-    for (int t = 0; t < g.taps; ++t) {
-      if (s2) {
-        // source pixel = 2*o + d, d in {-1,0,1}: d=-1 -> (h=o-1, parity 1); d=0 -> (o,0); d=1 -> (o,1)
-        const int dy = g.tap_dy[ph][t], dx = g.tap_dx[ph][t];
-        p.tap_map[ph][t] = int8_t((dy != 0) * 2 + (dx != 0));
-        p.g.tap_dy[ph][t] = int8_t(dy < 0 ? -1 : 0);
-        p.g.tap_dx[ph][t] = int8_t(dx < 0 ? -1 : 0);
-      } else {
-        p.tap_map[ph][t] = 0;
-      }
-    }
-  const char* e = halo_finish(plan, enc, w16, dst, kb, kblocks);
-  if (e) { plan.halo = 0; return nullptr; }   // not eligible after all: the caller falls back to conv_tc_plan
-  return nullptr;
-}
-
-const char* conv_hs_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
-                         const int src_coff[], const void* w16, const float* bias, __half* dst) {
-  plan.halo = 0;
-  if (dst == nullptr || g.in_stride != 1) return nullptr;
-  if (!((g.n_phase == 1 && g.taps == 9) || (g.n_phase == 4 && g.taps == 4))) return nullptr;
-  int bn = (g.cout_pad % 256 == 0) ? 256 : ((g.cout_pad % 128 == 0) ? 128 : 0);
-  if (bn == 0 || g.cout_pad > 512 || g.cout % 64 != 0) return nullptr;   // TMA-store epilogue only
-  {
-    // small grids (1/64 layers): N = 128 blocks give twice the CTAs, each with half of the weight stream and epilogue
-    const int sp = g.n_img * ((g.gw + kHaloTileW - 1) / kHaloTileW) * ((g.gh + kHaloTileH - 1) / kHaloTileH) * g.n_phase;
-    if (bn == 256 && sp * (g.cout_pad / 256) <= g_num_sms / 2) bn = 128;
-  }
-  for (int s = 0; s < g.n_src; ++s)
-    if (g.src_c[s] % 64 != 0 || src_coff[s] % 8 != 0) return nullptr;
-  if ((g.dst_coff % 8) != 0 || (g.dst_cstride % 8) != 0) return nullptr;
-  for (int ph = 0; ph < g.n_phase; ++ph)
-    for (int t = 0; t < g.taps; ++t)
-      if (g.tap_dy[ph][t] < -1 || g.tap_dy[ph][t] > 1 || g.tap_dx[ph][t] < -1 || g.tap_dx[ph][t] > 1) return nullptr;
-  ConvTcParams& p = plan.p;
-  memset(&p, 0, sizeof(p));
-  p.g = g;
-  p.kb_elems = 64;
-  for (int s = 0; s < g.n_src; ++s) p.src_kblocks[s] = g.src_c[s] / 64;
-  p.dst = dst;
-  p.bias = bias;
-  p.halo_lox = 1; p.halo_loy = 1;
-  p.halo_w = kHaloTileW + 2; p.halo_h = kHaloTileH + 2;
-  p.tiles_x = (g.gw + kHaloTileW - 1) / kHaloTileW;
-  p.tiles_y = (g.gh + kHaloTileH - 1) / kHaloTileH;
-  for (int s = 0; s < g.n_src; ++s) {
-    const size_t cs = size_t(g.src_cstride[s]);
-    const char* base = static_cast<const char*>(src_ptr[s]) + size_t(src_coff[s]) * 2;
-    cuuint64_t dims[4] = {cuuint64_t(g.src_c[s]), cuuint64_t(g.src_w), cuuint64_t(g.src_h), cuuint64_t(g.n_img)};
-    cuuint64_t str[3] = {cs * 2, cs * 2 * g.src_w, cs * 2 * g.src_w * g.src_h};
-    cuuint32_t box[4] = {64, cuuint32_t(p.halo_w), cuuint32_t(p.halo_h), 1};
-    if (const char* e = encode_map(enc, &p.a_map[s][0], base, 4, dims, str, box, 64)) return e;
-  }
-  {
-    const size_t cs = size_t(g.dst_cstride);
-    for (int ph = 0; ph < g.n_phase; ++ph) {
-      const int py = ph >> 1, px = ph & 1;
-      cuuint64_t dims[4] = {cuuint64_t(g.cout), cuuint64_t(g.gw), cuuint64_t(g.gh), cuuint64_t(g.n_img)};
-      cuuint64_t str[3] = {cs * 2 * g.out_mul, cs * 2 * g.dst_w * g.out_mul, cs * 2 * size_t(g.dst_w) * g.dst_h};
-      cuuint32_t box[4] = {64, kHaloTileW, kHaloTileH, 1};
-      const char* base = reinterpret_cast<const char*>(dst) + (size_t(g.dst_coff) + (size_t(py) * g.dst_w + px) * cs) * 2;
-      if (const char* e = encode_map(enc, &p.o_map[ph], base, 4, dims, str, box, 64)) return e;
-    }
-    p.use_tma_store = 1;
-  }
-  {
-    cuuint64_t dims[2] = {cuuint64_t(g.k_total), cuuint64_t(g.n_phase) * cuuint64_t(g.cout_pad)};
-    cuuint64_t str[1] = {cuuint64_t(g.k_total) * 2};
-    cuuint32_t box[2] = {64, cuuint32_t(bn)};
-    if (const char* e = encode_map(enc, &p.b_map, w16, 2, dims, str, box, 64)) return e;
-  }
-  const int total_tiles = g.n_img * p.tiles_x * p.tiles_y * (g.cout_pad / bn) * g.n_phase;
-  plan.grid = dim3(unsigned(total_tiles < g_num_sms ? total_tiles : g_num_sms), 1, 1);
-  plan.block_n = bn;
-  plan.smem_bytes = bn == 256 ? HsCfg<256>::kSmem : HsCfg<128>::kSmem;
-  p.halo_stages = bn == 256 ? HsCfg<256>::kAStages : HsCfg<128>::kAStages;
-  p.hs_b_stages = bn == 256 ? HsCfg<256>::kBStages : HsCfg<128>::kBStages;
-  plan.halo = 2;
-  return nullptr;
-}
-
-const char* conv_sw_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
-                         const int src_coff[], const void* w16, const float* bias, __half* dst) {
-  plan.halo = 0;
-  if (dst == nullptr || g.in_stride != 1) return nullptr;
-  // The kernel handles Bottleneck residuals (tests/test_gpu_kernels.py), but its channel-major 2-byte residual loads
-  // make those layers slower than conv_hs_kernel (measured 6.32 -> 6.44 ms per step): leave them there.
-  if (g.residual && !g_sw_residual) return nullptr;
-  // (1x1 layers were tried here too: without halo reuse the transposed epilogue costs more than the wider MMA saves)
-  if (!((g.n_phase == 1 && g.taps == 9) || (g.n_phase == 4 && g.taps == 4))) return nullptr;
-  if (g.cout_pad != 128 || g.cout != 128) return nullptr;
-  for (int s = 0; s < g.n_src; ++s)
-    if (g.src_c[s] % 64 != 0 || src_coff[s] % 8 != 0) return nullptr;
-  if ((g.dst_coff % 8) != 0 || (g.dst_cstride % 8) != 0) return nullptr;
-  for (int ph = 0; ph < g.n_phase; ++ph)
-    for (int t = 0; t < g.taps; ++t)
-      if (g.tap_dy[ph][t] < -1 || g.tap_dy[ph][t] > 1 || g.tap_dx[ph][t] < -1 || g.tap_dx[ph][t] > 1) return nullptr;
-  ConvTcParams& p = plan.p;
-  memset(&p, 0, sizeof(p));
-  p.g = g;
-  p.kb_elems = 64;
-  for (int s = 0; s < g.n_src; ++s) p.src_kblocks[s] = g.src_c[s] / 64;
-  p.dst = dst;
-  p.bias = bias;
-  p.halo_lox = 1; p.halo_loy = 1;
-  p.halo_w = kSwTileW + 2; p.halo_h = kSwTileH + 2;
-  p.tiles_x = (g.gw + kSwTileW - 1) / kSwTileW;
-  p.tiles_y = (g.gh + kSwTileH - 1) / kSwTileH;
-  for (int s = 0; s < g.n_src; ++s) {
-    const size_t cs = size_t(g.src_cstride[s]);
-    const char* base = static_cast<const char*>(src_ptr[s]) + size_t(src_coff[s]) * 2;
-    cuuint64_t dims[4] = {cuuint64_t(g.src_c[s]), cuuint64_t(g.src_w), cuuint64_t(g.src_h), cuuint64_t(g.n_img)};
-    cuuint64_t str[3] = {cs * 2, cs * 2 * g.src_w, cs * 2 * g.src_w * g.src_h};
-    cuuint32_t box[4] = {64, cuuint32_t(p.halo_w), cuuint32_t(p.halo_h), 1};
-    if (const char* e = encode_map(enc, &p.a_map[s][0], base, 4, dims, str, box, 64)) return e;
-  }
-  {
-    const size_t cs = size_t(g.dst_cstride);
-    for (int ph = 0; ph < g.n_phase; ++ph) {
-      const int py = ph >> 1, px = ph & 1;
-      cuuint64_t dims[4] = {cuuint64_t(g.cout), cuuint64_t(g.gw), cuuint64_t(g.gh), cuuint64_t(g.n_img)};
-      cuuint64_t str[3] = {cs * 2 * g.out_mul, cs * 2 * g.dst_w * g.out_mul, cs * 2 * size_t(g.dst_w) * g.dst_h};
-      cuuint32_t box[4] = {128, kSwTileW, 4, 1};   // one staging chunk: 4 tile rows x 8 pixels x 128 channels
-      const char* base = reinterpret_cast<const char*>(dst) + (size_t(g.dst_coff) + (size_t(py) * g.dst_w + px) * cs) * 2;
-      if (const char* e = encode_map_noswizzle(enc, &p.o_map[ph], base, 4, dims, str, box)) return e;
-    }
-    p.use_tma_store = 1;
-  }
-  {
-    cuuint64_t dims[2] = {cuuint64_t(g.k_total), cuuint64_t(g.n_phase) * cuuint64_t(g.cout_pad)};
-    cuuint64_t str[1] = {cuuint64_t(g.k_total) * 2};
-    cuuint32_t box[2] = {64, 128};
-    if (const char* e = encode_map(enc, &p.b_map, w16, 2, dims, str, box, 64)) return e;
-  }
-  const int total_tiles = g.n_img * p.tiles_x * p.tiles_y * g.n_phase;
-  plan.grid = dim3(unsigned(total_tiles < g_num_sms ? total_tiles : g_num_sms), 1, 1);
-  plan.block_n = 128;
-  plan.smem_bytes = SwCfg::kSmem + 1024;
-  plan.halo = 3;
-  return nullptr;
-}
-
-const char* conv_halo_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void* s2d, int n, int ph, int pw,
-                                const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff, int cout,
-                                int act) {
-  ConvTcParams& p = plan.p;
-  memset(&p, 0, sizeof(p));
-  plan.halo = 0;
-  ConvGeom& g = p.g;
-  const int oh = ph / 2, ow = pw / 2, pitch = ow + 4;
-  g.n_img = n; g.gh = oh; g.gw = ow; g.dst_h = oh; g.dst_w = ow; g.out_mul = 1; g.n_phase = 1;
-  g.taps = 3; g.cin_total = 64; g.k_total = 192; g.n_src = 1; g.src_c[0] = 64; g.src_cstride[0] = 16;
-  g.src_h = oh; g.src_w = ow; g.in_stride = 1;
-  for (int t = 0; t < 3; ++t) { g.tap_dy[0][t] = int8_t(t - 1); g.tap_dx[0][t] = 0; }
-  g.cout = cout; g.cout_pad = 32; g.dst_cstride = dst_cstride; g.dst_coff = dst_coff; g.act = act; g.residual = 0;
-  p.kb_elems = 64;
-  p.src_kblocks[0] = 1;
-  p.dst = dst;
-  p.bias = bias;
-  p.halo_lox = 0; p.halo_loy = 1;   // the 4-pixel window already holds the x neighbours
-  p.halo_w = kHaloTileW; p.halo_h = kHaloTileH + 2;
-  {
-    cuuint64_t dims[4] = {64, cuuint64_t(ow), cuuint64_t(oh), cuuint64_t(n)};
-    cuuint64_t str[3] = {32, cuuint64_t(pitch) * 32, cuuint64_t(pitch) * 32 * oh};
-    cuuint32_t box[4] = {64, cuuint32_t(p.halo_w), cuuint32_t(p.halo_h), 1};
-    if (const char* e = encode_map(enc, &p.a_map[0][0], s2d, 4, dims, str, box, 64)) return e;
-  }
-  return halo_finish(plan, enc, w16, dst, 64, 1);
 }
 
 const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void* s2d, int n, int ph, int pw,
@@ -1823,8 +564,6 @@ cudaError_t conv_tc_init() {
   {
     const char* pdl = getenv("CTD_PDL");
     g_use_pdl = (pdl && pdl[0] == '1') ? 1 : 0;
-    const char* swr = getenv("CTD_SW_RESIDUAL");
-    g_sw_residual = (swr && swr[0] == '1') ? 1 : 0;
   }
   int dev = 0;
   if (cudaGetDevice(&dev) == cudaSuccess) {
@@ -1834,20 +573,8 @@ cudaError_t conv_tc_init() {
 #define CTD_SET(BN)                                                                                   \
   e = cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(TcCfg<BN>::kSmem)); \
   if (e != cudaSuccess) return e;
-  CTD_SET(256) CTD_SET(128) CTD_SET(64) CTD_SET(32) CTD_SET(16)
+  CTD_SET(128) CTD_SET(64) CTD_SET(32) CTD_SET(16)
 #undef CTD_SET
-  e = cudaFuncSetAttribute(conv_halo_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(conv_halo_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(conv_halo_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(conv_sw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(SwCfg::kSmem + 1024));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(conv_hs_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(HsCfg<256>::kSmem));
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(conv_hs_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(HsCfg<128>::kSmem));
-  if (e != cudaSuccess) return e;
   return cudaSuccess;
 }
 
@@ -1868,26 +595,12 @@ static cudaError_t launch_pdl(K kernel, dim3 grid, size_t smem, cudaStream_t s, 
 }
 
 cudaError_t conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s) {
-  if (plan.halo == 3) return launch_pdl(conv_sw_kernel, plan.grid, plan.smem_bytes, s, plan.p);
-  if (plan.halo == 2) {
-    if (plan.block_n == 256) return launch_pdl(conv_hs_kernel<256>, plan.grid, plan.smem_bytes, s, plan.p);
-    else return launch_pdl(conv_hs_kernel<128>, plan.grid, plan.smem_bytes, s, plan.p);
-    return cudaGetLastError();
-  }
-  if (plan.halo) {
-    if (plan.block_n == 64) return launch_pdl(conv_halo_kernel<64>, plan.grid, plan.smem_bytes, s, plan.p);
-    else if (plan.block_n == 32) return launch_pdl(conv_halo_kernel<32>, plan.grid, plan.smem_bytes, s, plan.p);
-    else return launch_pdl(conv_halo_kernel<16>, plan.grid, plan.smem_bytes, s, plan.p);
-    return cudaGetLastError();
-  }
   switch (plan.block_n) {
-    case 256: return launch_pdl(conv_tc_kernel<256>, plan.grid, plan.smem_bytes, s, plan.p); break;
-    case 128: return launch_pdl(conv_tc_kernel<128>, plan.grid, plan.smem_bytes, s, plan.p); break;
-    case 64: return launch_pdl(conv_tc_kernel<64>, plan.grid, plan.smem_bytes, s, plan.p); break;
-    case 32: return launch_pdl(conv_tc_kernel<32>, plan.grid, plan.smem_bytes, s, plan.p); break;
-    default: return launch_pdl(conv_tc_kernel<16>, plan.grid, plan.smem_bytes, s, plan.p); break;
+    case 128: return launch_pdl(conv_tc_kernel<128>, plan.grid, plan.smem_bytes, s, plan.p);
+    case 64: return launch_pdl(conv_tc_kernel<64>, plan.grid, plan.smem_bytes, s, plan.p);
+    case 32: return launch_pdl(conv_tc_kernel<32>, plan.grid, plan.smem_bytes, s, plan.p);
+    default: return launch_pdl(conv_tc_kernel<16>, plan.grid, plan.smem_bytes, s, plan.p);
   }
-  return cudaGetLastError();
 }
 
 }  // namespace ctd

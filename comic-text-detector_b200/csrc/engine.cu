@@ -1,6 +1,6 @@
 // libctd_b200.so: C-ABI engine (see include/ctd_b200.h).  Owns device buffers, the weight blob,
 // per-shape launch plans (tensor maps) and the optional CUDA graph; runs the op list emitted by
-// the Python host "compiler".  No CPU fallback: every entry point fails without an sm_100 GPU.
+// the Python host "compiler".  No CPU fallback: every entry point fails without an sm_90 GPU.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -92,8 +92,8 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= cfg->device)
     return ctd_fail(nullptr, CTD_E_NO_DEVICE, "no CUDA device %d (this engine has no CPU fallback)", cfg->device);
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 10)
-    return ctd_fail(nullptr, CTD_E_NO_DEVICE, "device %d is not sm_100 (compute %d.%d)", cfg->device, prop.major, prop.minor);
+  if (cudaGetDeviceProperties(&prop, cfg->device) != cudaSuccess || prop.major != 9 || prop.minor != 0)
+    return ctd_fail(nullptr, CTD_E_NO_DEVICE, "device %d is not sm_90 (compute %d.%d)", cfg->device, prop.major, prop.minor);
   h = new ctd_handle();
   h->cfg = *cfg;
   h->ops.assign(ops, ops + n_ops);
@@ -119,9 +119,6 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
         if (op.src_buf[k] >= 0 && op.src_buf[k] < n_bufs) needed[op.src_buf[k]] = 1;
       if (op.residual && op.dst_buf >= 0 && op.dst_buf < n_bufs) needed[op.dst_buf] = 1;
     }
-    const char* hm = getenv("CTD_HALO");
-    // bit 0: conv_halo_kernel (resident weights), 1: conv_hs_kernel (streamed), 2: conv_sw_kernel, 3: seg tail as GEMM + col2im
-    h->halo_mode = hm ? atoi(hm) : 15;
     const char* ov = getenv("CTD_OVERLAP");
     h->overlap = have_db && !(ov && ov[0] == '0');
   }
@@ -164,12 +161,6 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
     h->enc = reinterpret_cast<PFN_encodeTiled>(fn);
   }
   CKC(conv_tc_init());
-  CKC(ctd::conv_bneck_init());
-  for (int i = 0; i < n_ops; ++i)
-    if (ops[i].kind == CTD_OP_BNECK && (cfg->precision != CTD_PREC_FP16_TC || !ctd::conv_bneck_supported(ops[i].cout))) {
-      ctd_fail(h, CTD_E_INVALID, "op %d: fused Bottleneck needs CTD_PREC_FP16_TC and 32 or 64 channels", i);
-      return bail(CTD_E_INVALID);
-    }
   h->blob_bytes = blob_bytes;
   CKC(cudaMalloc(&h->d_blob, blob_bytes));
   CKC(cudaMemcpy(h->d_blob, blob, blob_bytes, cudaMemcpyHostToDevice));
@@ -331,28 +322,10 @@ static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
     return CTD_OK;
   }
   if (h->cfg.precision != CTD_PREC_FP16_TC) return CTD_OK;
-  sp.bn.resize(h->ops.size());
   for (size_t i = 0; i < h->ops.size(); ++i) {
     const ctd_op& op = h->ops[i];
-    if (op.kind == CTD_OP_BNECK) {
-      // fused Bottleneck: 1x1 + 3x3 (+ residual) in one kernel, intermediate in shared memory (conv_fuse.cu)
-      const ctd_bufdesc& sb = h->bufs[op.src_buf[0]];
-      const ctd_bufdesc& db = h->bufs[op.dst_buf];
-      if (op.n_src != 1 || op.src_c[0] != op.cout || op.cout != op.cout_pad || sb.down != db.down || op.src_buf[0] == op.dst_buf)
-        return ctd_fail(h, CTD_E_INVALID, "op %zu: malformed fused Bottleneck", i);
-      int nsm = 148;
-      cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, h->cfg.device);
-      const char* e = ctd::conv_bneck_plan(sp.bn[i], h->enc, n, ph / sb.down, pw / sb.down, op.cout, h->d_buf[op.src_buf[0]],
-                                           sb.channels, op.src_coff[0], h->d_blob + op.w16_off,
-                                           reinterpret_cast<const float*>(h->d_blob + op.b_off),
-                                           static_cast<__half*>(h->d_buf[op.dst_buf]), db.channels, op.dst_coff, op.act,
-                                           op.residual, nsm);
-      if (e) return ctd_fail(h, CTD_E_INVALID, "op %zu: %s", i, e);
-      sp.has_tc[i] = 1;
-      continue;
-    }
     if (op.kind == CTD_OP_STEM) {
-      const char* e = ((h->halo_mode & 1) ? conv_halo_plan_stem : conv_tc_plan_stem)(
+      const char* e = conv_tc_plan_stem(
           sp.tc[i], h->enc, h->d_buf[op.src_buf[0]], n, ph, pw, h->d_blob + op.w16_off,
           reinterpret_cast<const float*>(h->d_blob + op.b_off), static_cast<__half*>(h->d_buf[op.dst_buf]),
           h->bufs[op.dst_buf].channels, op.dst_coff, op.cout, op.act);
@@ -360,30 +333,19 @@ static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
       sp.has_tc[i] = 1;
       continue;
     }
-    if (op.kind == CTD_OP_SEG_TAIL && (h->halo_mode & 8) && op.b_off > 0 && op.src_c[0] == 64) {
-      // final ConvT 4x4 s2 (64 -> 1) + sigmoid + u8 mask as one 1x1 GEMM over the 16 kernel positions + col2im epilogue
-      const ctd_bufdesc& sb = h->bufs[op.src_buf[0]];
-      int nsm = 148;
-      cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, h->cfg.device);
-      const char* e = ctd::conv_segtail_plan(sp.seg, h->enc, n, ph / sb.down, pw / sb.down, h->d_buf[op.src_buf[0]], sb.channels,
-                                             op.src_coff[0], h->d_blob + op.b_off, h->d_mask, h->d_mask_u8, nsm);
-      if (e) return ctd_fail(h, CTD_E_INVALID, "seg tail: %s", e);
-      sp.seg_op = int(i);
-      sp.has_tc[i] = 1;
-      continue;
-    }
-    if (op.kind == CTD_OP_SEG_TAIL && (h->halo_mode & 1) && op.w16_off > 0 && op.cout_pad == 16) {
-      // final ConvT 4x4 s2 (C -> 1) + sigmoid + u8 mask as a 3x3 / 4-output halo convolution
+    if (op.kind == CTD_OP_SEG_TAIL && op.w16_off > 0 && op.cout_pad == 16) {
+      // final ConvT 4x4 s2 (C -> 1) + sigmoid + u8 mask as a 3x3 / 4-output convolution with the seg-tail epilogue
       ctd_op c3 = op;
       c3.kind = CTD_OP_CONV; c3.ksize = 3; c3.stride = 1;
       ConvGeom g;
       if (int rc = op_geom(h, c3, n, ph, pw, g)) return rc;
       const void* src[CTD_MAX_SRC] = {h->d_buf[op.src_buf[0]]};
-      int coff[CTD_MAX_SRC] = {op.src_coff[0]};
-      const char* e = conv_halo_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off, nullptr, nullptr, h->d_mask,
-                                     h->d_mask_u8);
+      const int coff[CTD_MAX_SRC] = {op.src_coff[0]};
+      const char* e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off, nullptr, nullptr);
       if (e) return ctd_fail(h, CTD_E_INVALID, "seg tail: %s", e);
-      sp.has_tc[i] = sp.tc[i].halo ? 1 : 0;
+      sp.tc[i].p.seg_f32 = h->d_mask;
+      sp.tc[i].p.seg_u8 = h->d_mask_u8;
+      sp.has_tc[i] = 1;
       continue;
     }
     if (op.kind != CTD_OP_CONV && op.kind != CTD_OP_DECONV4 && op.kind != CTD_OP_DETECT) continue;
@@ -396,20 +358,8 @@ static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
       coff[s] = op.src_coff[s];
     }
     __half* dst = op.kind == CTD_OP_DETECT ? nullptr : static_cast<__half*>(h->d_buf[op.dst_buf]);
-    const char* e = nullptr;
-    sp.tc[i].halo = 0;
-    if ((h->halo_mode & 1) && op.kind != CTD_OP_DETECT)
-      e = conv_halo_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off,
-                         reinterpret_cast<const float*>(h->d_blob + op.b_off), dst);
-    if (!e && !sp.tc[i].halo && (h->halo_mode & 4) && op.kind != CTD_OP_DETECT)
-      e = conv_sw_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off,
-                       reinterpret_cast<const float*>(h->d_blob + op.b_off), dst);
-    if (!e && !sp.tc[i].halo && (h->halo_mode & 2) && op.kind != CTD_OP_DETECT)
-      e = conv_hs_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off,
-                       reinterpret_cast<const float*>(h->d_blob + op.b_off), dst);
-    if (!e && !sp.tc[i].halo)
-      e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off,
-                       reinterpret_cast<const float*>(h->d_blob + op.b_off), dst);
+    const char* e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off,
+                                 reinterpret_cast<const float*>(h->d_blob + op.b_off), dst);
     if (e) return ctd_fail(h, CTD_E_INVALID, "op %zu: %s", i, e);
     if (op.kind == CTD_OP_DETECT) {
       ConvTcParams& p = sp.tc[i].p;
@@ -538,12 +488,7 @@ static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, ShapePlan&
     if (rc) return rc;
     return split_written_slice(h, op, n, ph, pw, cnt);
   }
-  if (op.kind == CTD_OP_BNECK) {
-    if (h->cfg.precision != CTD_PREC_FP16_TC || !sp.has_tc[i])
-      return ctd_fail(h, CTD_E_INVALID, "op %zu: fused Bottleneck ops run on the fp16 tensor-core engine only", i);
-    cudaError_t e = ctd::conv_bneck_launch(sp.bn[i], h->stream);
-    rc = e == cudaSuccess ? CTD_OK : ctd_fail(h, CTD_E_CUDA, "conv_bneck op %zu: %s", i, cudaGetErrorString(e));
-  } else if (op.kind == CTD_OP_STEM && h->cfg.precision == CTD_PREC_FP16_TC) {
+  if (op.kind == CTD_OP_STEM && h->cfg.precision == CTD_PREC_FP16_TC) {
     // tensor-core stem: space-to-depth pre-pass into the padded window buffer, then the implicit GEMM
     cudaError_t e = s2d_launch<__half>(h->d_pages, n, ph, pw, static_cast<__half*>(h->d_buf[op.src_buf[0]]), 16, 0,
                                        pw / 2 + 4, 1, h->stream);
@@ -551,7 +496,7 @@ static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, ShapePlan&
     rc = e == cudaSuccess ? CTD_OK : ctd_fail(h, CTD_E_CUDA, "stem op %zu: %s", i, cudaGetErrorString(e));
     ++*cnt;
   } else if (op.kind == CTD_OP_SEG_TAIL && h->cfg.precision == CTD_PREC_FP16_TC && sp.has_tc[i]) {
-    cudaError_t e = sp.seg_op == int(i) ? ctd::conv_segtail_launch(sp.seg, h->stream) : conv_tc_launch(sp.tc[i], h->stream);
+    cudaError_t e = conv_tc_launch(sp.tc[i], h->stream);
     rc = e == cudaSuccess ? CTD_OK : ctd_fail(h, CTD_E_CUDA, "seg tail op %zu: %s", i, cudaGetErrorString(e));
   } else if (gemm) {
     if (h->cfg.precision == CTD_PREC_FP16_TC) {

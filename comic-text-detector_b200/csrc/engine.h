@@ -16,8 +16,6 @@
 
 #include "kernels.h"
 
-using ctd::BneckPlan;
-using ctd::SegTailPlan;
 using ctd::ConvTcPlan;
 using ctd::NmsWorkspace;
 using ctd::PFN_encodeTiled;
@@ -51,9 +49,6 @@ struct RefineJob {
 struct ShapePlan {
   std::vector<ConvTcPlan> tc;  // index = op index (unused entries default)
   std::vector<char> has_tc;
-  std::vector<BneckPlan> bn;   // fused Bottleneck ops (CTD_OP_BNECK), index = op index
-  SegTailPlan seg;             // seg tail as GEMM + col2im (conv_fuse.cu) when seg_op >= 0
-  int seg_op = -1;
   cudaGraphExec_t graph = nullptr;
   int launches = 0;
 };
@@ -110,7 +105,6 @@ struct ctd_handle {
   bool slot_busy[2] = {false, false};
   // overlapped schedule: post-processing of the DB maps / the Detect rows runs on side streams under the
   // remaining network ops (see run_ops)
-  int halo_mode = 15;  // CTD_HALO bit mask (0 routes every conv through conv_tc_kernel, for A/B measurements)
   bool overlap = false;
   cudaStream_t side = nullptr, side2 = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_fork2 = nullptr, ev_join2 = nullptr;

@@ -40,12 +40,10 @@ struct ConvGeom {
 void fill_conv_geom_taps(ConvGeom& g, int kind, int ksize, int stride);
 
 // ---------------------------------------------------------------------------------------
-// tcgen05 implicit-GEMM convolution (conv_tc.cu)
+// wgmma implicit-GEMM convolution (conv_tc.cu)
 struct alignas(64) ConvTcParams {
   CUtensorMap a_map[CTD_MAX_SRC][4];  // [source][parity]: parity maps only for stride-2 convs
   CUtensorMap b_map;                  // packed weights [n_phase*cout_pad][k_total], K-major
-  CUtensorMap o_map[4];               // destination slice, one map per deconv phase (TMA-store epilogue)
-  int use_tma_store;                  // 1: epilogue stages 64-channel chunks in smem and stores them by TMA
   ConvGeom g;
   int kb_elems;                       // channels per K block: 64 / 32 / 16 (swizzle 128/64/32 B)
   int src_kblocks[CTD_MAX_SRC];
@@ -60,19 +58,12 @@ struct alignas(64) ConvTcParams {
   float det_stride;
   float anchor_wh[6];     // pixels
   int nc;
-  // halo variant (conv_halo_kernel): weights resident in smem, ONE activation box per K block holds the tile
-  // plus its halo and every filter tap is an MMA operand view into it
-  int halo_lox, halo_loy;             // halo pixels before the tile in x / y
-  int halo_w, halo_h;                 // halo block size in pixels (tile 8 x 16 + halo)
-  int halo_stages, halo_stage_bytes;  // activation ring
-  int halo_w_bytes;                   // resident weights of one phase: taps * kblocks * BN * kb * 2
-  int hs_b_stages;                    // conv_hs_kernel: depth of the streamed-weight ring (halo_stages = A ring)
-  // seg-tail epilogue (halo kernel, BN = 16): accumulator columns 0..3 are the sub-pixel phases of the final
-  // ConvT 4x4 s2 (C -> 1); sigmoid -> f32 mask + truncated u8 mask at (2y+py, 2x+px)
+  // seg-tail epilogue (BN = 16, seg_f32 != nullptr): accumulator columns 0..3 are the sub-pixel phases of the final
+  // ConvT 4x4 s2 (C -> 1) computed as a 3x3 convolution; sigmoid -> f32 mask + truncated u8 mask at (2y+py, 2x+px)
   float* seg_f32;
   uint8_t* seg_u8;
-  // split-fp16 mode (CTD_PREC_SPLIT_TC, conv_tc_kernel only): every fp32 operand x is carried as two fp16 planes
-  // hi = fp16(x), lo = fp16(x - hi); a K block issues (hi,hi) + (lo,hi) + (hi,lo) into the same fp32 accumulator
+  // split-fp16 mode (CTD_PREC_SPLIT_TC): every fp32 operand x is carried as two fp16 planes
+  // hi = fp16(x), lo = fp16(x - hi); a K block issues (hi,hi) + (lo,hi) + (hi,lo) into fp32 accumulators
   // (~22 significant bits per operand), and the epilogue writes FP32.  Activation planes: image n_img + i of the
   // same tensor map holds the lo plane of image i; weight lo rows follow the hi rows (row + split_row_off).
   int split;
@@ -82,7 +73,6 @@ struct alignas(64) ConvTcParams {
 
 struct ConvTcPlan {
   ConvTcParams p;
-  int halo = 0;                       // 1: conv_halo_kernel, 2: conv_hs_kernel (halo A, streamed B), 3: conv_sw_kernel
   int block_n;
   dim3 grid;
   size_t smem_bytes;
@@ -102,72 +92,8 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
 const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void* s2d, int n, int ph, int pw,
                               const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff, int cout,
                               int act);
-// Halo variant for stride-1 3x3 convolutions and the 2x2-tap deconvolution phases whose weights fit in shared
-// memory.  Sets plan.halo = 1 when the op is eligible, leaves it 0 (and returns nullptr) when not.
-const char* conv_halo_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
-                           const int src_coff[], const void* w16, const float* bias, __half* dst,
-                           float* seg_f32 = nullptr, uint8_t* seg_u8 = nullptr);
-// Halo activations + STREAMED weights for the wide stride-1 3x3 convolutions / deconvolution phases whose weights
-// do not fit in shared memory (BN = 128 / 256).  Sets plan.halo = 2 when eligible.
-const char* conv_hs_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
-                         const int src_coff[], const void* w16, const float* bias, __half* dst);
-// Swapped operands for the 128-wide stride-1 3x3 convolutions / deconvolution phases: the 128 output channels are the
-// MMA's M (weights = A operand), 256 PIXELS (8 x 32 tile, halo views) are its N, so one instruction does twice the
-// work of the pixel-major form at N = 128; the epilogue transposes through shared memory.  Sets plan.halo = 3.
-const char* conv_sw_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
-                         const int src_coff[], const void* w16, const float* bias, __half* dst);
-// Stem through the halo kernel (window map of conv_tc_plan_stem, halo in y only).
-const char* conv_halo_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void* s2d, int n, int ph, int pw,
-                                const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff, int cout,
-                                int act);
 cudaError_t conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s);
 cudaError_t conv_tc_init();  // sets max dynamic smem attributes once
-
-// ---------------------------------------------------------------------------------------
-// Fused Bottleneck (conv_fuse.cu): y = [x +] act(conv3x3(act(conv1x1(x)))), c -> c -> c channels, c in {32, 64}; the
-// intermediate stays in shared memory.  w16: W1 [c][c] followed by W2 [c][9*c] (K-major fp16, K = (tap, ci));
-// bias: bias1[c] | bias2[c].  Source and destination are different buffers.
-struct alignas(64) BneckParams {
-  CUtensorMap x_map, w1_map, w2_map, o_map;
-  int n_img, gh, gw;
-  int tiles_x, tiles_y;     // 8 x 16-pixel tiles
-  int act, residual;
-  int dst_cstride, dst_coff;
-  __half* dst;
-  const __half* src;        // residual: x re-read per output pixel
-  int src_cstride, src_coff;
-  const float* bias;
-};
-struct BneckPlan {
-  BneckParams p;
-  int c;
-  dim3 grid;
-  size_t smem_bytes;
-};
-bool conv_bneck_supported(int c);
-const char* conv_bneck_plan(BneckPlan& plan, PFN_encodeTiled enc, int n_img, int gh, int gw, int c, const void* src,
-                            int src_cstride, int src_coff, const void* w16, const float* bias, __half* dst,
-                            int dst_cstride, int dst_coff, int act, int residual, int num_sms);
-cudaError_t conv_bneck_init();   // also sets the attributes of conv_segtail_kernel
-
-// Seg tail (conv_fuse.cu): ConvTranspose2d(64 -> 1, 4x4, s2, p1) + sigmoid + u8 mask as ONE 1x1 GEMM over the 16 kernel
-// positions + a col2im epilogue.  w16: [16 = ky*4+kx][64 channels] fp16; source must have exactly 64 channels.
-struct alignas(64) SegTailParams {
-  CUtensorMap x_map, w_map;
-  int n_img, gh, gw;
-  int tiles_x, tiles_y;     // 16 x 12 input pixels per tile
-  float* seg_f32;
-  uint8_t* seg_u8;
-};
-struct SegTailPlan {
-  SegTailParams p;
-  dim3 grid;
-  size_t smem_bytes;
-};
-const char* conv_segtail_plan(SegTailPlan& plan, PFN_encodeTiled enc, int n_img, int gh, int gw, const void* src, int src_cstride,
-                              int src_coff, const void* w16, float* seg_f32, uint8_t* seg_u8, int num_sms);
-cudaError_t conv_segtail_launch(const SegTailPlan& plan, cudaStream_t s);
-cudaError_t conv_bneck_launch(const BneckPlan& plan, cudaStream_t s);
 
 // ---------------------------------------------------------------------------------------
 // CUDA-core kernels (simt.cu): accurate/bisecting path and the thin layers.  T = float | __half.

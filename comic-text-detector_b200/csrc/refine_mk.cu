@@ -10,7 +10,7 @@
 // state record in global memory; per-window scalar decisions are one-CTA-per-window kernels.  Results are bit-identical to
 // refine.cu and to the oracle (tests/test_gpu_refine.py runs all three).
 //
-// The sweeps are instruction-issue bound, not memory bound (ncu, profiles/r02_refine_full_summary.txt), so the binary planes
+// The sweeps are instruction-issue bound, not memory bound, so the binary planes
 // are handled as BIT masks wherever a neighbourhood is involved: warp ballots pack 32 pixels per shared-memory word and one
 // thread per (half) word does the work of 16 - 32 pixels with funnel shifts, ANDs and popcounts -- the erosions of phase 0,
 // the dilation, the run contacts of the labelling and the per-label sums (one update per RUN, not per pixel).

@@ -1,5 +1,5 @@
 // CUDA-core kernels: the fp32-accurate / bisecting convolution path (same op descriptors and
-// weight packing as the tcgen05 path) and the thin layers that are HBM-bound by nature
+// weight packing as the tensor-core path) and the thin layers that are HBM-bound by nature
 // (stem from u8, pools, nearest upsample, the seg/DB tails).  T = float or __half storage,
 // arithmetic always fp32.
 #include <cuda_fp16.h>
@@ -684,7 +684,7 @@ cudaError_t db_tail_launch(const T* src, int n, int h, int w, int cs, const floa
                            uint8_t* bitmap, float db_thresh, cudaStream_t s) {
   const long long total = (long long)n * h * w;
   const long long blocks = (total + 127) / 128;
-  const long long cap = 148LL * 16;   // a few resident CTAs per SM, each looping over its share of the pixels
+  const long long cap = 132LL * 16;   // a few resident CTAs per SM, each looping over its share of the pixels
   db_tail_kernel<T><<<unsigned(blocks < cap ? blocks : cap), 128, 0, s>>>(src, n, h, w, cs, params, lines, bitmap, db_thresh);
   return cudaGetLastError();
 }

@@ -1,4 +1,4 @@
-"""Drop-in `TextDetector` over the B200 engine.
+"""Drop-in `TextDetector` over the H100 engine.
 
 Same constructor and call signature as the reference's `inference.TextDetector`
 (inference.py:116-178): `TextDetector(model_path, input_size=1024, device=..., half=False, nms_thresh=0.35,
@@ -75,8 +75,7 @@ class TextDetector:
         self.backend = 'b200'
         if precision is None:
             precision = PREC_FP16_TC
-        # fused Bottleneck ops exist on the fp16 tensor-core engine only (bit-identical to the two-op form)
-        self.program = compiler.compile_checkpoint(ckpt, head_act=act, fuse=compiler.fuse_default(precision == PREC_FP16_TC))
+        self.program = compiler.compile_checkpoint(ckpt, head_act=act)
         # DB threshold is hard-coded 0.3 in the reference (inference.py:139 ignores mask_thresh)
         self.net = Engine(self.program, device=device_index, precision=precision, max_batch=1, max_h=input_size[0],
                           max_w=input_size[1], conf_thresh=conf_thresh, nms_thresh=nms_thresh, db_thresh=0.3)

@@ -1,5 +1,5 @@
 /*
- * ctd_b200.h -- C ABI of libctd_b200.so, the B200 (sm_100a) engine behind the reference's
+ * ctd_b200.h -- C ABI of libctd_b200.so, the H100 (sm_90a) engine behind the reference's
  * inference path  page -> (block boxes, text-line map, segmentation mask).
  *
  * The reference is pure Python and has no FFI; the seam this library replaces is the
@@ -35,7 +35,7 @@ extern "C" {
 #define CTD_OK 0
 #define CTD_E_INVALID (-1)   /* bad argument / malformed program                            */
 #define CTD_E_CUDA (-2)      /* CUDA runtime/driver error (message has the CUDA string)     */
-#define CTD_E_NO_DEVICE (-3) /* no sm_100 GPU visible: the engine has NO CPU fallback       */
+#define CTD_E_NO_DEVICE (-3) /* no sm_90 GPU visible: the engine has NO CPU fallback       */
 #define CTD_E_SHAPE (-4)     /* page size not a multiple of 64 (basemodel.py:62-78 stride)  */
 #define CTD_E_CAPACITY (-5)  /* batch larger than the reserved workspace                    */
 
@@ -57,12 +57,8 @@ enum ctd_op_kind {
   CTD_OP_SEG_TAIL = 7,  /* ConvT4x4s2 64->1 + sigmoid    (basemodel.py:57-60)               */
   CTD_OP_DB_TAIL = 8,   /* ConvT2x2s2+BN+ReLU -> ConvT2x2s2 -> sigmoid, both branches
                            (basemodel.py:99-103,138-142)                                    */
-  CTD_OP_S2D = 9,       /* u8 BGR page -> /255 -> 2x2 space-to-depth, 12(+4 zero) channels at 1/2 resolution:
+  CTD_OP_S2D = 9        /* u8 BGR page -> /255 -> 2x2 space-to-depth, 12(+4 zero) channels at 1/2 resolution:
                            turns the 6x6 s2 p2 stem conv into a 3x3 s1 p1 conv for the tensor cores       */
-  CTD_OP_BNECK = 10     /* fused Bottleneck (common.py:94-104): dst = [src +] act(conv3x3(act(conv1x1(src)))), c -> c -> c
-                           channels (c = cout in {32, 64}), src and dst in DIFFERENT buffers; w16_off / w32_off: W1 [c][c]
-                           followed by W2 [c][9c] (K = (ky, kx, ci)); b_off: bias1[c] | bias2[c]; residual = the `+ src`.
-                           CTD_PREC_FP16_TC only (the compiler emits it on request, compiler.py fuse=True)              */
 };
 
 enum ctd_act { CTD_ACT_NONE = 0, CTD_ACT_SILU = 1, CTD_ACT_LEAKY = 2, CTD_ACT_RELU = 3, CTD_ACT_SIGMOID = 4 };
@@ -96,10 +92,10 @@ typedef struct ctd_bufdesc {
 } ctd_bufdesc;
 
 enum ctd_precision {
-  CTD_PREC_FP16_TC = 0,   /* fp16 storage, tcgen05 implicit GEMM, fp32 accumulate (default) */
+  CTD_PREC_FP16_TC = 0,   /* fp16 storage, wgmma implicit GEMM, fp32 accumulate (default) */
   CTD_PREC_FP32_SIMT = 1, /* fp32 storage + CUDA-core fp32 kernels ("vs reference fp32" config) */
   CTD_PREC_FP16_SIMT = 2, /* fp16 storage + CUDA-core kernels (bisecting aid)               */
-  CTD_PREC_SPLIT_TC = 3   /* fp32 storage; tcgen05 with every operand split into fp16 hi + lo planes
+  CTD_PREC_SPLIT_TC = 3   /* fp32 storage; wgmma with every operand split into fp16 hi + lo planes
                              (hi*hi + lo*hi + hi*lo, fp32 accumulate: ~22 significant bits) -- the
                              tensor-core path that meets the 1e-3 "vs reference fp32" tolerance  */
 };

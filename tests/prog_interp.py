@@ -54,7 +54,7 @@ class Interp:
             return op["src_buf"][0], op["src_coff"][0] + op["src_c"][0], 3 * op["src_c"][0]
         if op["dst_buf"] < 0:
             return None
-        c = op["cout"] if k in (cc.OP_STEM, cc.OP_CONV, cc.OP_DECONV4, cc.OP_BNECK) else (16 if k == cc.OP_S2D else op["src_c"][0])
+        c = op["cout"] if k in (cc.OP_STEM, cc.OP_CONV, cc.OP_DECONV4) else (16 if k == cc.OP_S2D else op["src_c"][0])
         return op["dst_buf"], op["dst_coff"], c
 
     def step(self, i):
@@ -118,20 +118,6 @@ class Interp:
                 out[..., 2:4] = (y[..., 2:4] * 2) ** 2 * anch.view(1, 3, 1, 1, 2)
                 r0 = sum(3 * (h // (8 << l)) * (w // (8 << l)) for l in range(op["aux"]))
                 self.blks[:, r0:r0 + 3 * ny * nx] = out.reshape(bs, -1, no)
-        elif k == cc.OP_BNECK:
-            # fused Bottleneck: the 1x1 output is rounded to the storage type exactly where the two-op form stores it
-            c = op["cout"]
-            cnt = c * c + 9 * c * c
-            wk = (_blob(prog, op["w16_off"], cnt, np.float16).float() if use_fp16_weights
-                  else _blob(prog, op["w32_off"], cnt, np.float32))
-            w1 = wk[:c * c].view(c, c, 1, 1)
-            w2 = wk[c * c:].view(c, 3, 3, c).permute(0, 3, 1, 2)
-            b = _blob(prog, op["b_off"], 2 * c, np.float32)
-            t = self.q(_act(F.conv2d(srcs[0], w1, b[:c]), op["act"]))
-            y = _act(F.conv2d(t, w2, b[c:], 1, 1), op["act"])
-            if op["residual"]:
-                y = y + srcs[0]
-            bufs[op["dst_buf"]][:, op["dst_coff"]:op["dst_coff"] + c] = self.q(y)
         elif k == cc.OP_DECONV4:
             K = 4 * cin
             wk = (_blob(prog, op["w16_off"], 4 * op["cout_pad"] * K, np.float16).float() if use_fp16_weights

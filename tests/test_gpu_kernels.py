@@ -41,21 +41,20 @@ CONV_CASES = [
     ([128], 64, 1, 1, cc.ACT_RELU, False, 192, 64, 1),
     ([16], 32, 3, 1, cc.ACT_SILU, False, 64, 128, 2),   # 16-channel K blocks (32-byte swizzle): the s2d stem
     ([16], 16, 1, 1, cc.ACT_NONE, False, 64, 64, 1),
-    ([64, 64], 64, 3, 1, cc.ACT_LEAKY, False, 64, 128, 2),   # halo kernel: two K blocks from two sources
-    ([32, 64], 64, 3, 1, cc.ACT_RELU, True, 128, 64, 1),     # halo kernel: 32-channel K blocks (64-byte swizzle)
+    ([64, 64], 64, 3, 1, cc.ACT_LEAKY, False, 64, 128, 2),   # two sources, 64-channel K blocks
+    ([32, 64], 64, 3, 1, cc.ACT_RELU, True, 128, 64, 1),     # 32-channel K blocks (64-byte swizzle)
     ([128], 32, 3, 1, cc.ACT_SILU, False, 64, 192, 1),
-    ([256], 256, 3, 1, cc.ACT_LEAKY, True, 64, 64, 1),       # halo A + streamed weights, BN=256, residual
-    ([128], 128, 3, 1, cc.ACT_SILU, True, 64, 64, 2),        # swapped-operand kernel (128 couts = M) with residual
-    ([64, 64], 128, 3, 1, cc.ACT_RELU, False, 128, 64, 1),   # swapped-operand kernel, two sources
-    ([128, 64], 128, 1, 1, cc.ACT_SILU, False, 64, 192, 1),  # swapped-operand kernel, 1x1 over two sources
-    ([128, 128], 512, 3, 1, cc.ACT_SILU, False, 64, 128, 1),  # same, two sources x two N blocks
+    ([256], 256, 3, 1, cc.ACT_LEAKY, True, 64, 64, 1),       # two 128-wide N blocks, residual
+    ([128], 128, 3, 1, cc.ACT_SILU, True, 64, 64, 2),        # BN = 128 with residual
+    ([64, 64], 128, 3, 1, cc.ACT_RELU, False, 128, 64, 1),   # two sources
+    ([128, 64], 128, 1, 1, cc.ACT_SILU, False, 64, 192, 1),  # 1x1 over two sources
+    ([128, 128], 512, 3, 1, cc.ACT_SILU, False, 64, 128, 1),  # two sources x four N blocks
 ]
 
 
 @pytest.mark.parametrize("prec", [PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT])
 @pytest.mark.parametrize("case", CONV_CASES, ids=lambda c: "c%s_o%d_k%d_s%d_r%d" % ("+".join(map(str, c[0])), c[1], c[2], c[3], int(c[5])))
-def test_conv(case, prec, monkeypatch):
-    monkeypatch.setenv("CTD_SW_RESIDUAL", "1")   # also exercise the residual path of the swapped-operand kernel
+def test_conv(case, prec):
     srcc, cout, k, stride, act, residual, h, w, n = case
     rng = np.random.default_rng(hash((tuple(srcc), cout, k, stride)) % 2**32)
     cin = sum(srcc)

@@ -3,7 +3,7 @@
 engine, only op i runs (ctd_debug_run_ops), and the slice it wrote must match the interpreter's result for op i.
 Nothing is amplified by the (ill-conditioned, random-weight) net, so the tolerances are those of one rounding:
 
-  * CTD_PREC_FP16_TC (the benchmarked tcgen05 engine) vs the fp16-storage emulation: <= 2e-3 relative -- one fp16
+  * CTD_PREC_FP16_TC (the benchmarked wgmma engine) vs the fp16-storage emulation: <= 2e-3 relative -- one fp16
     ulp (2^-10) where a value sits on a rounding boundary and the fp32 accumulation order differs;
   * CTD_PREC_SPLIT_TC (split-fp16 tensor-core engine) and CTD_PREC_FP32_SIMT (CUDA-core fp32 engine) vs the fp32
     interpreter: <= 1e-4 of (|ref| + 1 % of the tensor's scale) -- both sides round differently in fp32 (torch's

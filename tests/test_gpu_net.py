@@ -82,7 +82,7 @@ def test_forward_matches_oracle(prec, smooth):
 
 
 def test_benchmark_config_matches_oracle():
-    """BASELINE configs[2] itself -- 1024x1024, batch 16, fp16 tcgen05 path under a CUDA graph (what bench.py
+    """BASELINE configs[2] itself -- 1024x1024, batch 16, fp16 wgmma path under a CUDA graph (what bench.py
     times) -- against the fp32 oracle on all 16 pages (structured and noise pages alternate)."""
     _check_against_oracle(PREC_FP16_TC, True, 16, 1024, 1024, use_graph=True)
 
@@ -95,7 +95,7 @@ def test_stream_bucket_sizes_match_oracle(prec, size):
 
 
 def test_fp16_engine_tracks_fp16_storage_emulation():
-    """The tcgen05 engine against the CPU emulation of ITS OWN numerics (fp16 weights + fp16 activation storage, fp32
+    """The wgmma engine against the CPU emulation of ITS OWN numerics (fp16 weights + fp16 activation storage, fp32
     accumulate): what is left is accumulation order and one-ulp rounding flips amplified by the net, an order of
     magnitude below the engine's distance to the fp32 reference."""
     import prog_interp
@@ -194,7 +194,7 @@ def test_batch_invariance():
 
 
 def test_tc_layers_track_fp32_engine():
-    """Layer-by-layer: every buffer of the tcgen05 engine (halo / tap-per-box / stem kernels, fp16 storage) against the
+    """Layer-by-layer: every buffer of the wgmma engine (tap-per-box conv and stem, fp16 storage) against the
     same buffer of the fp32 CUDA-core engine on the same page.  fp16 storage noise grows slowly through the net;
     a kernel bug (a wrong tap, a bad border) shows up as an O(1) relative error in the first buffer it touches."""
     ck = get_checkpoint(0, True)
