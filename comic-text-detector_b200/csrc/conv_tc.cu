@@ -252,8 +252,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         // Split-fp16 mode with PROMOTED accumulation.  The tensor core adds into its fp32 accumulator with
         // truncation: over the K/16 x 3 MMAs of a deep layer the one-sided errors add up to ~K/16 ulps.  So every
         // hi x hi MMA (K = 16) writes a FRESH accumulator that is added into `acc` in fp32 registers with
-        // round-to-nearest; the small cross terms (lo x hi, hi x lo: 2^-12 of the sum, their truncation is 2^-36)
-        // accumulate in the tensor core as usual and are added last.
+        // round-to-nearest; the cross terms (lo x hi, hi x lo: lo is stored scaled by kSplitLoScale, so they are
+        // 2^-12 of the sum once unscaled and their truncation is 2^-36) accumulate in the tensor core as usual and
+        // are unscaled and added last.
         float cross[R], tmp[R];
 #pragma unroll
         for (int i = 0; i < R; ++i) cross[i] = 0.f;
@@ -285,7 +286,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
           if (++stage == Cfg::kStages) { stage = 0; full_par ^= 1u; }
         }
 #pragma unroll
-        for (int i = 0; i < R; ++i) acc[i] = __fadd_rn(acc[i], cross[i]);
+        for (int i = 0; i < R; ++i) acc[i] = __fadd_rn(acc[i], cross[i] * kSplitLoUnscale);
         split_done = true;
       }
     }

@@ -178,7 +178,8 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
       CKC(cudaMalloc(&h->d_buf16[i], bytes));
       CKC(cudaMemset(h->d_buf16[i], 0, bytes));
     }
-    // weights: hi rows (the blob's fp16 copy = fp16(w32)) followed by lo rows fp16(w32 - hi), per GEMM op
+    // weights: hi rows (the blob's fp16 copy = fp16(w32)) followed by lo rows fp16((w32 - hi) * kSplitLoScale),
+    // per GEMM op
     h->wsplit_off.assign(size_t(n_ops), 0);
     std::vector<__half> ws;
     const char* hb = static_cast<const char*>(blob);
@@ -202,7 +203,7 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
       for (size_t k = 0; k < cnt; ++k) {
         const __half hi = __float2half_rn(w32[k]);
         ws[base + k] = hi;
-        ws[base + cnt + k] = __float2half_rn(w32[k] - __half2float(hi));
+        ws[base + cnt + k] = __float2half_rn((w32[k] - __half2float(hi)) * kSplitLoScale);
       }
     }
     CKC(cudaMalloc(&h->d_wsplit, ws.size() * 2 + 256));

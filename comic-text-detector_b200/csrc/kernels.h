@@ -10,6 +10,14 @@
 namespace ctd {
 
 constexpr int kMaxTaps = 9;
+
+// Split-fp16 lo planes are stored scaled by 2^11.  x - hi is about 2^-11 |x|; unscaled it falls into the fp16
+// subnormals (step 2^-24) once |x| < 2^-3 and loses a bit per octave below.  Scaled, lo keeps its 11 bits down to
+// |x| ~ 2^-14, so hi + lo holds x to 2^-23 relative (22 significant bits) over the range activations and weights
+// take.  |x - hi| * 2^11 <= 2^4 * 2^11 for any fp16-range x, so the scaled lo never overflows.  Both factors are
+// powers of two: scaling and unscaling are exact.
+constexpr float kSplitLoScale = 2048.0f;
+constexpr float kSplitLoUnscale = 1.0f / 2048.0f;
 constexpr int kMaxPhases = 4;
 
 // Geometry shared by the tensor-core and CUDA-core convolution kernels.  A "grid" pixel is an
@@ -63,9 +71,10 @@ struct alignas(64) ConvTcParams {
   float* seg_f32;
   uint8_t* seg_u8;
   // split-fp16 mode (CTD_PREC_SPLIT_TC): every fp32 operand x is carried as two fp16 planes
-  // hi = fp16(x), lo = fp16(x - hi); a K block issues (hi,hi) + (lo,hi) + (hi,lo) into fp32 accumulators
-  // (~22 significant bits per operand), and the epilogue writes FP32.  Activation planes: image n_img + i of the
-  // same tensor map holds the lo plane of image i; weight lo rows follow the hi rows (row + split_row_off).
+  // hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale); a K block issues (hi,hi) + (lo,hi) + (hi,lo) into fp32
+  // accumulators, the cross terms are merged as cross * kSplitLoUnscale, and the epilogue writes FP32.  Activation
+  // planes: image n_img + i of the same tensor map holds the lo plane of image i; weight lo rows follow the hi rows
+  // (row + split_row_off).
   int split;
   int split_img_off;
   int split_row_off;
@@ -118,7 +127,7 @@ cudaError_t stem_launch(const uint8_t* pages, int n, int h, int w, const float* 
 template <typename T>
 cudaError_t s2d_launch(const uint8_t* pages, int n, int h, int w, T* dst, int dst_cstride, int dst_coff, int pitch_px,
                        int xoff, cudaStream_t s);
-// fp32 NHWC channel slice -> fp16 hi / lo planes (split-fp16 mode): hi = fp16(x), lo = fp16(x - hi).
+// fp32 NHWC channel slice -> fp16 hi / lo planes (split-fp16 mode): hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale).
 // src / hi / lo point at the first channel of the slice; `cstride` elements between pixels (same in all three).
 cudaError_t split_planes_launch(const float* src, __half* hi, __half* lo, size_t npix, int c, int cstride,
                                 cudaStream_t s);

@@ -695,7 +695,8 @@ template cudaError_t db_tail_launch<__half>(const __half*, int, int, int, int, c
 
 
 // ---------------------------------------------------------------------------------------------
-// split-fp16 mode: fp32 NHWC channel slice -> hi = fp16(x), lo = fp16(x - hi) planes (4 channels per thread)
+// split-fp16 mode: fp32 NHWC channel slice -> hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale) planes (4 channels
+// per thread)
 __global__ void split_planes_kernel(const float* __restrict__ src, __half* __restrict__ hi, __half* __restrict__ lo,
                                     size_t npix, int c4, int cstride) {
   const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
@@ -705,8 +706,10 @@ __global__ void split_planes_kernel(const float* __restrict__ src, __half* __res
   const size_t off = pix * size_t(cstride) + size_t(q) * 4;
   const float4 v = *reinterpret_cast<const float4*>(src + off);
   const __half h0 = __float2half_rn(v.x), h1 = __float2half_rn(v.y), h2 = __float2half_rn(v.z), h3 = __float2half_rn(v.w);
-  const __half l0 = __float2half_rn(v.x - __half2float(h0)), l1 = __float2half_rn(v.y - __half2float(h1));
-  const __half l2 = __float2half_rn(v.z - __half2float(h2)), l3 = __float2half_rn(v.w - __half2float(h3));
+  const __half l0 = __float2half_rn((v.x - __half2float(h0)) * kSplitLoScale);
+  const __half l1 = __float2half_rn((v.y - __half2float(h1)) * kSplitLoScale);
+  const __half l2 = __float2half_rn((v.z - __half2float(h2)) * kSplitLoScale);
+  const __half l3 = __float2half_rn((v.w - __half2float(h3)) * kSplitLoScale);
   __half2 hh[2] = {__halves2half2(h0, h1), __halves2half2(h2, h3)};
   __half2 ll[2] = {__halves2half2(l0, l1), __halves2half2(l2, l3)};
   *reinterpret_cast<uint2*>(hi + off) = *reinterpret_cast<uint2*>(hh);

@@ -1,11 +1,14 @@
 """-m gpu: every CUDA kernel against a plain torch fp32 reference of the same op (fp16-rounded
-operands for the fp16 engines, so only accumulation order and the output rounding differ)."""
+operands for the fp16 engines, so only accumulation order and the output rounding differ).  The tensor-core engines
+(fp16 and split-fp16) are also held to the elementwise bound of tests/util.py, so a wrong value at a small output
+fails as well as one at the largest."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
-from util import SingleOp, h16, cc, PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT
+from util import (SingleOp, h16, cc, PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT, PREC_SPLIT_TC, fp16_tc_ab,
+                  split_tc_ab, bound_ratio)
 
 pytestmark = pytest.mark.gpu
 
@@ -49,27 +52,50 @@ CONV_CASES = [
     ([64, 64], 128, 3, 1, cc.ACT_RELU, False, 128, 64, 1),   # two sources
     ([128, 64], 128, 1, 1, cc.ACT_SILU, False, 64, 192, 1),  # 1x1 over two sources
     ([128, 128], 512, 3, 1, cc.ACT_SILU, False, 64, 128, 1),  # two sources x four N blocks
+    # (..., down): sources at 1/down resolution of the page
+    ([64], 64, 3, 1, cc.ACT_SILU, True, 192, 320, 2, 16),      # 12x20 grid: partial tiles in x and y, batch 2
+    ([128, 64], 128, 3, 2, cc.ACT_LEAKY, False, 512, 960, 2, 8),  # 32x60 grid: partial in x
+    ([32], 96, 3, 1, cc.ACT_RELU, False, 192, 320, 3, 16),     # BN 32 x 3 N blocks, partial tiles, batch 3
+    ([64], 128, 1, 1, cc.ACT_SILU, False, 512, 512, 2, 1),     # 4096 tiles: ~31 per persistent CTA
 ]
 
 
-@pytest.mark.parametrize("prec", [PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT])
-@pytest.mark.parametrize("case", CONV_CASES, ids=lambda c: "c%s_o%d_k%d_s%d_r%d" % ("+".join(map(str, c[0])), c[1], c[2], c[3], int(c[5])))
+def _check_bound(prec, got, x, wgt, bias, ref, K, transposed=False, stride=1, pad=1):
+    """Elementwise bound of the tensor-core engines; M = |bias| + conv(|x|, |w|) in float64."""
+    if prec not in (PREC_FP16_TC, PREC_SPLIT_TC):
+        return
+    cf = F.conv_transpose2d if transposed else F.conv2d
+    mag = cf(x.abs(), torch.from_numpy(wgt).double().abs(), torch.from_numpy(bias).double().abs(), stride, pad)
+    a, b = fp16_tc_ab(K) if prec == PREC_FP16_TC else split_tc_ab(K)
+    r = bound_ratio(got, ref, mag.permute(0, 2, 3, 1).numpy(), a, b)
+    assert r.max() <= 1.0, "err/bound %.3g at %s" % (r.max(), np.unravel_index(np.argmax(r), r.shape))
+
+
+def _conv_id(c):
+    i = "c%s_o%d_k%d_s%d_r%d" % ("+".join(map(str, c[0])), c[1], c[2], c[3], int(c[5]))
+    return i if len(c) < 10 else i + "_d%d_n%d_%dx%d" % (c[9], c[8], c[6], c[7])
+
+
+@pytest.mark.parametrize("prec", [PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT, PREC_SPLIT_TC])
+@pytest.mark.parametrize("case", CONV_CASES, ids=_conv_id)
 def test_conv(case, prec):
-    srcc, cout, k, stride, act, residual, h, w, n = case
+    srcc, cout, k, stride, act, residual, h, w, n = case[:9]
+    down = case[9] if len(case) > 9 else 1
     rng = np.random.default_rng(hash((tuple(srcc), cout, k, stride)) % 2**32)
     cin = sum(srcc)
-    so = SingleOp(srcc, down=1, extra_channels=8)
+    so = SingleOp(srcc, down=down, extra_channels=8)
     wgt = _rand(rng, cout, cin, k, k, scale=1.0 / np.sqrt(cin * k * k))
     bias = _rand(rng, cout, scale=0.5)
-    ins = [_rand(rng, n, h, w, c) for c in srcc]
+    sh, sw = h // down, w // down
+    ins = [_rand(rng, n, sh, sw, c) for c in srcc]
     dst = None
     dst_init = None
     if residual:
-        db = so.P.newbuf(cout + 8, stride)
+        db = so.P.newbuf(cout + 8, down * stride)
         dst = so.P.tensor(db, 8, cout)
-        dst_init = _rand(rng, n, h // stride, w // stride, cout + 8)
+        dst_init = _rand(rng, n, sh // stride, sw // stride, cout + 8)
     out_t = so.P.conv(so.srcs, wgt.astype(np.float64), bias.astype(np.float64), stride, act, dst=dst, residual=residual)
-    if prec != PREC_FP32_SIMT:
+    if prec in (PREC_FP16_TC, PREC_FP16_SIMT):
         ins = [h16(a) for a in ins]
         wgt = h16(wgt)
         if dst_init is not None:
@@ -83,30 +109,40 @@ def test_conv(case, prec):
     ref = ref.permute(0, 2, 3, 1).numpy()
     err = np.abs(got - ref).max()
     assert err <= _tol(prec, ref), "max abs err %g (ref max %g)" % (err, np.abs(ref).max())
+    _check_bound(prec, got, x, wgt, bias, ref, cin * k * k, stride=stride, pad=k // 2)
 
 
 DECONV_CASES = [([64], 32, 32, 32, 1), ([128], 64, 64, 64, 1), ([512], 256, 32, 32, 2), ([256], 128, 32, 64, 1),
-                ([96], 64, 96, 32, 2)]
+                ([96], 64, 96, 32, 2),
+                # (..., down): sources at 1/down of the page; 12x20 grid = partial tiles in x and y
+                ([64], 32, 12, 20, 2, 16), ([128], 128, 12, 20, 3, 16), ([64], 64, 128, 128, 2, 2)]
 
 
-@pytest.mark.parametrize("prec", [PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT])
-@pytest.mark.parametrize("case", DECONV_CASES, ids=lambda c: "c%d_o%d_%dx%d" % (c[0][0], c[1], c[2], c[3]))
+def _deconv_id(c):
+    i = "c%d_o%d_%dx%d" % (c[0][0], c[1], c[2], c[3])
+    return i if len(c) < 6 else i + "_d%d_n%d" % (c[5], c[4])
+
+
+@pytest.mark.parametrize("prec", [PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT, PREC_SPLIT_TC])
+@pytest.mark.parametrize("case", DECONV_CASES, ids=_deconv_id)
 def test_deconv4(case, prec):
-    srcc, cout, h, w, n = case
+    srcc, cout, h, w, n = case[:5]
+    down = case[5] if len(case) > 5 else 2
     rng = np.random.default_rng(cout * 7 + h)
     cin = sum(srcc)
-    so = SingleOp(srcc, down=2, extra_channels=0)
+    so = SingleOp(srcc, down=down, extra_channels=0)
     wgt = _rand(rng, cin, cout, 4, 4, scale=1.0 / np.sqrt(cin * 4))
     bias = _rand(rng, cout, scale=0.5)
     ins = [_rand(rng, n, h, w, c) for c in srcc]
     out_t = so.P.deconv4(so.srcs, wgt.astype(np.float64), bias.astype(np.float64), cc.ACT_RELU)
-    if prec != PREC_FP32_SIMT:
+    if prec in (PREC_FP16_TC, PREC_FP16_SIMT):
         ins = [h16(a) for a in ins]
         wgt = h16(wgt)
-    got = so.run(out_t, ins, n, 2 * h, 2 * w, prec)
+    got = so.run(out_t, ins, n, down * h, down * w, prec)
     x = torch.from_numpy(np.concatenate(ins, -1)).permute(0, 3, 1, 2).double()
     ref = F.relu(F.conv_transpose2d(x, torch.from_numpy(wgt).double(), torch.from_numpy(bias).double(), 2, 1))
     ref = ref.permute(0, 2, 3, 1).numpy()
     assert got.shape == ref.shape
     err = np.abs(got - ref).max()
     assert err <= _tol(prec, ref), "max abs err %g (ref max %g)" % (err, np.abs(ref).max())
+    _check_bound(prec, got, x, wgt, bias, ref, 4 * cin, transposed=True, stride=2, pad=1)
