@@ -15,8 +15,8 @@ sources / channel-offset destinations, and emits the flat op list + weight blob 
 import numpy as np
 
 # enum mirrors of include/ctd_b200.h
-(OP_STEM, OP_CONV, OP_DECONV4, OP_AVGPOOL2, OP_SPPF_POOL, OP_UPSAMPLE2, OP_DETECT, OP_SEG_TAIL, OP_DB_TAIL,
- OP_S2D) = range(10)
+OP_STEM, OP_CONV, OP_DECONV4, OP_AVGPOOL2, OP_SPPF_POOL, OP_UPSAMPLE2, OP_DETECT, OP_SEG_TAIL, OP_DB_TAIL = range(9)
+OP_S2D = 9  # reserved value of a retired op kind: never emitted, no engine kernel; the name stays for existing callers
 ACT_NONE, ACT_SILU, ACT_LEAKY, ACT_RELU, ACT_SIGMOID = range(5)
 MAX_SRC = 3
 
@@ -100,7 +100,7 @@ class Program:
         op = dict(kind=kind, n_src=len(srcs), src_buf=[0] * MAX_SRC, src_coff=[0] * MAX_SRC, src_c=[0] * MAX_SRC,
                   dst_buf=-1, dst_coff=0, cout=0, cout_pad=0, ksize=1, stride=1, act=ACT_NONE, residual=0, aux=0,
                   w16_off=0, w32_off=0, b_off=0, p_off=0)
-        assert 1 <= len(srcs) <= MAX_SRC or kind in (OP_S2D,)
+        assert 1 <= len(srcs) <= MAX_SRC
         for i, s in enumerate(srcs):
             op["src_buf"][i], op["src_coff"][i], op["src_c"][i] = s["buf"], s["coff"], s["c"]
         if dst is not None:
@@ -171,7 +171,7 @@ def fold_bn(w, conv_bias, sd, bn_prefix, eps, transposed=False):
     return wf, (b0 - mu) * scale + beta
 
 
-def compile_checkpoint(ckpt, head_act="leaky", stem_mode="s2d"):
+def compile_checkpoint(ckpt, head_act="leaky"):
     """Returns a Program for the full TextDetBase.forward graph (basemodel.py:240-244)."""
     P = Program()
     cfg = ckpt["blk_det"]["cfg"]
@@ -303,11 +303,8 @@ def compile_checkpoint(ckpt, head_act="leaky", stem_mode="s2d"):
             for dy, ky in TAPS[py]:
                 for dx, kx in TAPS[px]:
                     wc[py * 2 + px, dy + 1, dx + 1, :] = w6[:, 0, ky, kx]
-    # b_off (the layer has no bias): the same weights as a 1x1 GEMM over the 16 kernel positions, [ky*4+kx][ci] fp16, for the
-    # GEMM + col2im form of the tail
     P._op(OP_SEG_TAIL, [u512], None, p_off=P.add_blob(w6.reshape(w6.shape[0], 16).astype(np.float32)),
-          w16_off=P.add_blob(wc.reshape(16, 9 * ci6).astype(np.float16)), cout=4, cout_pad=16,
-          b_off=P.add_blob(np.ascontiguousarray(w6.reshape(ci6, 16).T).astype(np.float16)))
+          w16_off=P.add_blob(wc.reshape(16, 9 * ci6).astype(np.float16)), cout=4, cout_pad=16)
 
     # ---- text_det: DBHead.forward (basemodel.py:106-125) ----------------------------------------
     du128 = up_c3(dsd, [f64, u64], "upconv3")

@@ -177,8 +177,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   }
   for (int i = threadIdx.x; i < g.cout_pad && i < Cfg::kBiasFloats; i += kThreads) bias_s[i] = p.bias ? p.bias[i] : 0.f;
   __syncthreads();
-  griddep_launch_dependents();   // successors may begin their prologue as our CTAs retire
-  griddep_wait();                // activations / residuals written by the predecessor are visible from here on
 
   // tile index -> (phase, spatial tile, n block); n block varies fastest so that CTAs running
   // concurrently share the A tile in L2
@@ -421,7 +419,6 @@ static const char* encode_map(PFN_encodeTiled enc, CUtensorMap* m, const void* b
 }
 
 static int g_num_sms = 132;
-static int g_use_pdl = 0;   // CTD_PDL=1 enables programmatic dependent launch
 
 // N block: at most 128 output channels, so that a consumer warpgroup's 64 x BN fp32 accumulator fits in registers
 // (64 per thread) next to the epilogue's addresses
@@ -562,10 +559,6 @@ const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void*
 
 cudaError_t conv_tc_init() {
   cudaError_t e;
-  {
-    const char* pdl = getenv("CTD_PDL");
-    g_use_pdl = (pdl && pdl[0] == '1') ? 1 : 0;
-  }
   int dev = 0;
   if (cudaGetDevice(&dev) == cudaSuccess) {
     int n = 0;
@@ -579,29 +572,14 @@ cudaError_t conv_tc_init() {
   return cudaSuccess;
 }
 
-// All conv kernels are launched as programmatic dependents (see griddep_wait in ptx.cuh).
-template <typename K>
-static cudaError_t launch_pdl(K kernel, dim3 grid, size_t smem, cudaStream_t s, const ConvTcParams& p) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = dim3(kThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = g_use_pdl ? 1 : 0;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, p);
-}
-
 cudaError_t conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s) {
   switch (plan.block_n) {
-    case 128: return launch_pdl(conv_tc_kernel<128>, plan.grid, plan.smem_bytes, s, plan.p);
-    case 64: return launch_pdl(conv_tc_kernel<64>, plan.grid, plan.smem_bytes, s, plan.p);
-    case 32: return launch_pdl(conv_tc_kernel<32>, plan.grid, plan.smem_bytes, s, plan.p);
-    default: return launch_pdl(conv_tc_kernel<16>, plan.grid, plan.smem_bytes, s, plan.p);
+    case 128: conv_tc_kernel<128><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
+    case 64: conv_tc_kernel<64><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
+    case 32: conv_tc_kernel<32><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
+    default: conv_tc_kernel<16><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
   }
+  return cudaGetLastError();
 }
 
 }  // namespace ctd

@@ -41,6 +41,8 @@ int ctd_fail(ctd_handle* h, int code, const char* fmt, ...) {
   } while (0)
 
 static int rows_per_image(int ph, int pw) { return 3 * ((ph / 8) * (pw / 8) + (ph / 16) * (pw / 16) + (ph / 32) * (pw / 32)); }
+// op kinds that are one implicit GEMM over packed weights (conv_tc_kernel or conv_simt_kernel)
+static bool is_gemm(int kind) { return kind == CTD_OP_CONV || kind == CTD_OP_DECONV4 || kind == CTD_OP_DETECT; }
 
 extern "C" const char* ctd_last_error(const ctd_handle* h) { return h ? h->err.c_str() : g_create_error.c_str(); }
 
@@ -119,11 +121,19 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
         if (op.src_buf[k] >= 0 && op.src_buf[k] < n_bufs) needed[op.src_buf[k]] = 1;
       if (op.residual && op.dst_buf >= 0 && op.dst_buf < n_bufs) needed[op.dst_buf] = 1;
     }
-    const char* ov = getenv("CTD_OVERLAP");
-    h->overlap = have_db && !(ov && ov[0] == '0');
+    h->overlap = have_db;
   }
   h->elem = (cfg->precision == CTD_PREC_FP32_SIMT || cfg->precision == CTD_PREC_SPLIT_TC) ? 4 : 2;
   auto bail = [&](int code) { std::string e = h->err; ctd_destroy(h); g_create_error = e; return code; };
+  h->detect_prm.assign(size_t(n_ops), {});
+  for (int i = 0; i < n_ops; ++i) {
+    if (ops[i].kind != CTD_OP_DETECT) continue;
+    if (ops[i].p_off < 0 || size_t(ops[i].p_off) + sizeof(h->detect_prm[0]) > blob_bytes) {
+      ctd_fail(h, CTD_E_INVALID, "op %d: detect parameters outside the blob", i);
+      return bail(CTD_E_INVALID);
+    }
+    memcpy(h->detect_prm[size_t(i)].data(), static_cast<const char*>(blob) + ops[i].p_off, sizeof(h->detect_prm[0]));
+  }
 #define CKC(expr)                                                                                        \
   do {                                                                                                   \
     cudaError_t _e = (expr);                                                                             \
@@ -185,7 +195,7 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
     const char* hb = static_cast<const char*>(blob);
     for (int i = 0; i < n_ops; ++i) {
       const ctd_op& op = ops[i];
-      if (op.kind != CTD_OP_CONV && op.kind != CTD_OP_DECONV4 && op.kind != CTD_OP_DETECT) continue;
+      if (!is_gemm(op.kind)) continue;
       int cin = 0;
       for (int k = 0; k < op.n_src; ++k) cin += op.src_c[k];
       const int taps = op.kind == CTD_OP_DECONV4 ? 4 : op.ksize * op.ksize;
@@ -284,144 +294,90 @@ static int op_geom(ctd_handle* h, const ctd_op& op, int n, int ph, int pw, ConvG
   return CTD_OK;
 }
 
+// DETECT epilogue: the decoded rows of pyramid level op.aux go to d_blks (ConvTcParams and ConvSimtParams)
+template <typename P>
+static void set_detect(const ctd_handle* h, size_t i, int ph, int pw, P& p) {
+  p.blks = h->d_blks;
+  p.blks_rows_per_img = rows_per_image(ph, pw);
+  int row0 = 0;
+  for (int l = 0; l < h->ops[i].aux; ++l) row0 += 3 * (ph / (8 << l)) * (pw / (8 << l));
+  p.level_row0 = row0;
+  p.nc = h->cfg.nc;
+  p.det_stride = h->detect_prm[i][0];
+  for (int k = 0; k < 6; ++k) p.anchor_wh[k] = h->detect_prm[i][1 + k];
+}
+
+// Ops that run conv_tc_kernel; every other op runs on the CUDA cores.
+static bool runs_on_tensor_cores(int precision, int kind) {
+  switch (precision) {
+    case CTD_PREC_SPLIT_TC: return is_gemm(kind);
+    case CTD_PREC_FP16_TC: return is_gemm(kind) || kind == CTD_OP_STEM || kind == CTD_OP_SEG_TAIL;
+    default: return false;
+  }
+}
+
+// tensor-core launch plans of one shape: the only place that picks an op's kernel by precision
 static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
   sp.tc.resize(h->ops.size());
-  sp.has_tc.assign(h->ops.size(), 0);
-  if (h->cfg.precision == CTD_PREC_SPLIT_TC) {
-    // every GEMM-shaped op through conv_tc_kernel in split-fp16 form; stem / tails / thin ops stay on the fp32
-    // CUDA-core kernels (run_one_op)
-    for (size_t i = 0; i < h->ops.size(); ++i) {
-      const ctd_op& op = h->ops[i];
-      if (op.kind != CTD_OP_CONV && op.kind != CTD_OP_DECONV4 && op.kind != CTD_OP_DETECT) continue;
+  const bool split = h->cfg.precision == CTD_PREC_SPLIT_TC;
+  for (size_t i = 0; i < h->ops.size(); ++i) {
+    const ctd_op& op = h->ops[i];
+    if (!runs_on_tensor_cores(h->cfg.precision, op.kind)) continue;
+    const float* bias = reinterpret_cast<const float*>(h->d_blob + op.b_off);
+    const char* e = nullptr;
+    if (op.kind == CTD_OP_STEM) {
+      e = conv_tc_plan_stem(sp.tc[i], h->enc, h->d_buf[op.src_buf[0]], n, ph, pw, h->d_blob + op.w16_off, bias,
+                            static_cast<__half*>(h->d_buf[op.dst_buf]), h->bufs[op.dst_buf].channels, op.dst_coff,
+                            op.cout, op.act);
+    } else {
+      // the seg tail (final ConvT 4x4 s2, C -> 1) is a 3x3 convolution whose 4 output channels are the sub-pixel
+      // phases, with the sigmoid / u8-mask epilogue
+      const bool seg = op.kind == CTD_OP_SEG_TAIL;
+      if (seg && op.cout_pad != 16) return ctd_fail(h, CTD_E_INVALID, "op %zu: seg tail needs cout_pad 16", i);
+      ctd_op gop = op;
+      if (seg) { gop.kind = CTD_OP_CONV; gop.ksize = 3; gop.stride = 1; }
       ConvGeom g;
-      if (int rc = op_geom(h, op, n, ph, pw, g)) return rc;
+      if (int rc = op_geom(h, gop, n, ph, pw, g)) return rc;
       const void* src[CTD_MAX_SRC];
       int coff[CTD_MAX_SRC];
       for (int s = 0; s < op.n_src; ++s) {
-        src[s] = h->d_buf16[op.src_buf[s]];
+        src[s] = (split ? h->d_buf16 : h->d_buf)[op.src_buf[s]];
         coff[s] = op.src_coff[s];
       }
-      __half* dst = op.kind == CTD_OP_DETECT ? nullptr : static_cast<__half*>(h->d_buf[op.dst_buf]);
-      const char* e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, h->d_wsplit + h->wsplit_off[i],
-                                   reinterpret_cast<const float*>(h->d_blob + op.b_off), dst, 1);
-      if (e) return ctd_fail(h, CTD_E_INVALID, "op %zu: %s", i, e);
-      if (op.kind == CTD_OP_DETECT) {
-        ConvTcParams& p = sp.tc[i].p;
-        p.blks = h->d_blks;
-        p.blks_rows_per_img = rows_per_image(ph, pw);
-        int row0 = 0;
-        for (int l = 0; l < op.aux; ++l) row0 += 3 * (ph / (8 << l)) * (pw / (8 << l));
-        p.level_row0 = row0;
-        p.nc = h->cfg.nc;
-        float hp[7];
-        cudaMemcpy(hp, h->d_blob + op.p_off, sizeof(hp), cudaMemcpyDeviceToHost);
-        p.det_stride = hp[0];
-        for (int k = 0; k < 6; ++k) p.anchor_wh[k] = hp[1 + k];
+      const void* w = split ? h->d_wsplit + h->wsplit_off[i] : h->d_blob + op.w16_off;
+      __half* dst = (seg || op.kind == CTD_OP_DETECT) ? nullptr : static_cast<__half*>(h->d_buf[op.dst_buf]);
+      e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, w, seg ? nullptr : bias, dst, split);
+      if (op.kind == CTD_OP_DETECT) set_detect(h, i, ph, pw, sp.tc[i].p);
+      if (seg) {
+        sp.tc[i].p.seg_f32 = h->d_mask;
+        sp.tc[i].p.seg_u8 = h->d_mask_u8;
       }
-      sp.has_tc[i] = 1;
     }
-    return CTD_OK;
-  }
-  if (h->cfg.precision != CTD_PREC_FP16_TC) return CTD_OK;
-  for (size_t i = 0; i < h->ops.size(); ++i) {
-    const ctd_op& op = h->ops[i];
-    if (op.kind == CTD_OP_STEM) {
-      const char* e = conv_tc_plan_stem(
-          sp.tc[i], h->enc, h->d_buf[op.src_buf[0]], n, ph, pw, h->d_blob + op.w16_off,
-          reinterpret_cast<const float*>(h->d_blob + op.b_off), static_cast<__half*>(h->d_buf[op.dst_buf]),
-          h->bufs[op.dst_buf].channels, op.dst_coff, op.cout, op.act);
-      if (e) return ctd_fail(h, CTD_E_INVALID, "stem: %s", e);
-      sp.has_tc[i] = 1;
-      continue;
-    }
-    if (op.kind == CTD_OP_SEG_TAIL && op.w16_off > 0 && op.cout_pad == 16) {
-      // final ConvT 4x4 s2 (C -> 1) + sigmoid + u8 mask as a 3x3 / 4-output convolution with the seg-tail epilogue
-      ctd_op c3 = op;
-      c3.kind = CTD_OP_CONV; c3.ksize = 3; c3.stride = 1;
-      ConvGeom g;
-      if (int rc = op_geom(h, c3, n, ph, pw, g)) return rc;
-      const void* src[CTD_MAX_SRC] = {h->d_buf[op.src_buf[0]]};
-      const int coff[CTD_MAX_SRC] = {op.src_coff[0]};
-      const char* e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off, nullptr, nullptr);
-      if (e) return ctd_fail(h, CTD_E_INVALID, "seg tail: %s", e);
-      sp.tc[i].p.seg_f32 = h->d_mask;
-      sp.tc[i].p.seg_u8 = h->d_mask_u8;
-      sp.has_tc[i] = 1;
-      continue;
-    }
-    if (op.kind != CTD_OP_CONV && op.kind != CTD_OP_DECONV4 && op.kind != CTD_OP_DETECT) continue;
-    ConvGeom g;
-    if (int rc = op_geom(h, op, n, ph, pw, g)) return rc;
-    const void* src[CTD_MAX_SRC];
-    int coff[CTD_MAX_SRC];
-    for (int s = 0; s < op.n_src; ++s) {
-      src[s] = h->d_buf[op.src_buf[s]];
-      coff[s] = op.src_coff[s];
-    }
-    __half* dst = op.kind == CTD_OP_DETECT ? nullptr : static_cast<__half*>(h->d_buf[op.dst_buf]);
-    const char* e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, h->d_blob + op.w16_off,
-                                 reinterpret_cast<const float*>(h->d_blob + op.b_off), dst);
     if (e) return ctd_fail(h, CTD_E_INVALID, "op %zu: %s", i, e);
-    if (op.kind == CTD_OP_DETECT) {
-      ConvTcParams& p = sp.tc[i].p;
-      p.blks = h->d_blks;
-      p.blks_rows_per_img = rows_per_image(ph, pw);
-      int row0 = 0;
-      for (int l = 0; l < op.aux; ++l) row0 += 3 * (ph / (8 << l)) * (pw / (8 << l));
-      p.level_row0 = row0;
-      p.nc = h->cfg.nc;
-      float hp[7];
-      cudaMemcpy(hp, h->d_blob + op.p_off, sizeof(hp), cudaMemcpyDeviceToHost);
-      p.det_stride = hp[0];
-      for (int k = 0; k < 6; ++k) p.anchor_wh[k] = hp[1 + k];
-    }
-    sp.has_tc[i] = 1;
   }
   return CTD_OK;
 }
 
 template <typename T>
-static int run_op_simt(ctd_handle* h, const ctd_op& op, int n, int ph, int pw) {
-  cudaStream_t s = h->stream;
-  const bool f32 = sizeof(T) == 4;
-  switch (op.kind) {
-    case CTD_OP_CONV:
-    case CTD_OP_DECONV4:
-    case CTD_OP_DETECT: {
-      ConvSimtParams p;
-      memset(&p, 0, sizeof(p));
-      if (int rc = op_geom(h, op, n, ph, pw, p.g)) return rc;
-      for (int k = 0; k < op.n_src; ++k)
-        p.src[k] = static_cast<char*>(h->d_buf[op.src_buf[k]]) + size_t(op.src_coff[k]) * sizeof(T);
-      p.w = h->d_blob + (f32 ? op.w32_off : op.w16_off);
-      p.bias = reinterpret_cast<const float*>(h->d_blob + op.b_off);
-      if (op.kind == CTD_OP_DETECT) {
-        p.dst = nullptr;
-        p.blks = h->d_blks;
-        p.blks_rows_per_img = rows_per_image(ph, pw);
-        int row0 = 0;
-        for (int l = 0; l < op.aux; ++l) row0 += 3 * (ph / (8 << l)) * (pw / (8 << l));
-        p.level_row0 = row0;
-        p.nc = h->cfg.nc;
-        float hp[7];
-        cudaMemcpy(hp, h->d_blob + op.p_off, sizeof(hp), cudaMemcpyDeviceToHost);
-        p.det_stride = hp[0];
-        for (int k = 0; k < 6; ++k) p.anchor_wh[k] = hp[1 + k];
-      } else {
-        p.dst = h->d_buf[op.dst_buf];
-      }
-      CK(conv_simt_launch<T>(p, s));
-      return CTD_OK;
-    }
-    default: return ctd_fail(h, CTD_E_INVALID, "run_op_simt: bad kind %d", op.kind);
-  }
+static int run_op_simt(ctd_handle* h, size_t i, int n, int ph, int pw) {
+  const ctd_op& op = h->ops[i];
+  ConvSimtParams p;
+  memset(&p, 0, sizeof(p));
+  if (int rc = op_geom(h, op, n, ph, pw, p.g)) return rc;
+  for (int k = 0; k < op.n_src; ++k)
+    p.src[k] = static_cast<char*>(h->d_buf[op.src_buf[k]]) + size_t(op.src_coff[k]) * sizeof(T);
+  p.w = h->d_blob + (sizeof(T) == 4 ? op.w32_off : op.w16_off);
+  p.bias = reinterpret_cast<const float*>(h->d_blob + op.b_off);
+  if (op.kind == CTD_OP_DETECT) set_detect(h, i, ph, pw, p);
+  else p.dst = h->d_buf[op.dst_buf];
+  CK(conv_simt_launch<T>(p, h->stream));
+  return CTD_OK;
 }
 
 template <typename T>
 static int run_op_thin(ctd_handle* h, const ctd_op& op, int n, int ph, int pw) {
   cudaStream_t s = h->stream;
-  const ctd_bufdesc* sb = (op.kind == CTD_OP_STEM || op.kind == CTD_OP_S2D) ? nullptr : &h->bufs[op.src_buf[0]];
-  (void)sb;
+  const ctd_bufdesc* sb = op.kind == CTD_OP_STEM ? nullptr : &h->bufs[op.src_buf[0]];
   const int sh = sb ? ph / sb->down : ph, sw = sb ? pw / sb->down : pw;
   const T* src = sb ? static_cast<const T*>(h->d_buf[op.src_buf[0]]) + op.src_coff[0] : nullptr;
   switch (op.kind) {
@@ -429,10 +385,6 @@ static int run_op_thin(ctd_handle* h, const ctd_op& op, int n, int ph, int pw) {
       CK(stem_launch<T>(h->d_pages, n, ph, pw, reinterpret_cast<const float*>(h->d_blob + op.w32_off),
                         reinterpret_cast<const float*>(h->d_blob + op.b_off), static_cast<T*>(h->d_buf[op.dst_buf]),
                         h->bufs[op.dst_buf].channels, op.dst_coff, op.cout, op.act, s));
-      return CTD_OK;
-    case CTD_OP_S2D:
-      CK(s2d_launch<T>(h->d_pages, n, ph, pw, static_cast<T*>(h->d_buf[op.dst_buf]), h->bufs[op.dst_buf].channels,
-                       op.dst_coff, pw / 2, 0, s));
       return CTD_OK;
     case CTD_OP_AVGPOOL2:
       CK(avgpool2_launch<T>(src, n, sh, sw, op.src_c[0], sb->channels,
@@ -463,7 +415,6 @@ static int split_written_slice(ctd_handle* h, const ctd_op& op, int n, int ph, i
   int buf = op.dst_buf, coff = op.dst_coff, c = op.cout;
   if (op.kind == CTD_OP_SPPF_POOL) { buf = op.src_buf[0]; coff = op.src_coff[0] + op.src_c[0]; c = 3 * op.src_c[0]; }
   else if (op.kind == CTD_OP_AVGPOOL2 || op.kind == CTD_OP_UPSAMPLE2) c = op.src_c[0];
-  else if (op.kind == CTD_OP_S2D) c = 16;
   if (buf < 0 || c <= 0) return CTD_OK;
   const ctd_bufdesc& b = h->bufs[buf];
   const size_t npix = size_t(n) * (ph / b.down) * (pw / b.down);
@@ -474,51 +425,49 @@ static int split_written_slice(ctd_handle* h, const ctd_op& op, int n, int ph, i
   return CTD_OK;
 }
 
-static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, ShapePlan& sp, int* cnt) {
+static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, const ShapePlan& sp, int* cnt) {
   const ctd_op& op = h->ops[i];
-  const bool gemm = op.kind == CTD_OP_CONV || op.kind == CTD_OP_DECONV4 || op.kind == CTD_OP_DETECT;
+  const ConvTcPlan& tc = sp.tc[i];
   int rc = CTD_OK;
-  if (h->cfg.precision == CTD_PREC_SPLIT_TC) {
-    if (gemm) {
-      cudaError_t e = conv_tc_launch(sp.tc[i], h->stream);
-      rc = e == cudaSuccess ? CTD_OK : ctd_fail(h, CTD_E_CUDA, "conv_tc (split) op %zu: %s", i, cudaGetErrorString(e));
-    } else {
-      rc = run_op_thin<float>(h, op, n, ph, pw);
+  if (tc.block_n) {
+    cudaError_t e = cudaSuccess;
+    if (op.kind == CTD_OP_STEM) {
+      // space-to-depth pre-pass into the padded window buffer the tensor-core stem reads
+      e = s2d_launch(h->d_pages, n, ph, pw, static_cast<__half*>(h->d_buf[op.src_buf[0]]), h->stream);
+      ++*cnt;
     }
-    ++*cnt;
-    if (rc) return rc;
-    return split_written_slice(h, op, n, ph, pw, cnt);
-  }
-  if (op.kind == CTD_OP_STEM && h->cfg.precision == CTD_PREC_FP16_TC) {
-    // tensor-core stem: space-to-depth pre-pass into the padded window buffer, then the implicit GEMM
-    cudaError_t e = s2d_launch<__half>(h->d_pages, n, ph, pw, static_cast<__half*>(h->d_buf[op.src_buf[0]]), 16, 0,
-                                       pw / 2 + 4, 1, h->stream);
-    if (e == cudaSuccess) e = conv_tc_launch(sp.tc[i], h->stream);
-    rc = e == cudaSuccess ? CTD_OK : ctd_fail(h, CTD_E_CUDA, "stem op %zu: %s", i, cudaGetErrorString(e));
-    ++*cnt;
-  } else if (op.kind == CTD_OP_SEG_TAIL && h->cfg.precision == CTD_PREC_FP16_TC && sp.has_tc[i]) {
-    cudaError_t e = conv_tc_launch(sp.tc[i], h->stream);
-    rc = e == cudaSuccess ? CTD_OK : ctd_fail(h, CTD_E_CUDA, "seg tail op %zu: %s", i, cudaGetErrorString(e));
-  } else if (gemm) {
-    if (h->cfg.precision == CTD_PREC_FP16_TC) {
-      cudaError_t e = conv_tc_launch(sp.tc[i], h->stream);
-      rc = e == cudaSuccess ? CTD_OK : ctd_fail(h, CTD_E_CUDA, "conv_tc op %zu: %s", i, cudaGetErrorString(e));
-    } else if (h->cfg.precision == CTD_PREC_FP32_SIMT) {
-      rc = run_op_simt<float>(h, op, n, ph, pw);
-    } else {
-      rc = run_op_simt<__half>(h, op, n, ph, pw);
-    }
+    if (e == cudaSuccess) e = conv_tc_launch(tc, h->stream);
+    if (e != cudaSuccess) rc = ctd_fail(h, CTD_E_CUDA, "conv_tc op %zu: %s", i, cudaGetErrorString(e));
+  } else if (is_gemm(op.kind)) {
+    rc = h->elem == 4 ? run_op_simt<float>(h, i, n, ph, pw) : run_op_simt<__half>(h, i, n, ph, pw);
   } else {
     rc = h->elem == 4 ? run_op_thin<float>(h, op, n, ph, pw) : run_op_thin<__half>(h, op, n, ph, pw);
   }
   ++*cnt;
-  return rc;
+  if (rc || h->d_buf16.empty()) return rc;
+  return split_written_slice(h, op, n, ph, pw, cnt);   // split-fp16 mode: refresh the planes of what the op wrote
 }
 
-static int run_ops(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp, int* launches, bool record = false) {
+// NMS of the Detect rows
+static int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
+  CK(nms_launch(h->d_blks, n, rows_per_image(ph, pw), h->cfg.nc, h->cfg.conf_thresh, h->cfg.nms_thresh, h->nms, h->d_det,
+                h->d_det_count, s));
+  *cnt += kNmsLaunches;
+  return CTD_OK;
+}
+
+// DB post-processing: connected components of the bitmap, then the text-line boxes
+static int launch_db_post(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
+  CK(ccl_launch(h->d_bitmap, n, ph, pw, h->d_labels, h->d_ccl_scratch, h->d_nlabels, s));
+  CK(segrep_launch(h->d_bitmap, h->d_lines, size_t(2) * ph * pw, h->d_ccl_scratch, n, ph, pw, 1000, 1.5f,
+                   h->d_segrep_scratch, h->d_line_boxes, h->d_line_scores, h->d_line_count, s));
+  *cnt += kCclLaunches + kSegrepLaunches;
+  return CTD_OK;
+}
+
+static int run_ops(ctd_handle* h, int n, int ph, int pw, const ShapePlan& sp, int* launches, bool record = false) {
   int cnt = 0;
   size_t evi = 0;
-  const int rows = rows_per_image(ph, pw);
   if (h->overlap && !record && !h->cfg.debug_skip_postproc) {
     // Two-phase order.  Phase 1: every op the DB maps depend on (program order).  Then the DB post-processing
     // (CCL + contour boxes: latency-bound kernels that leave most SMs idle) forks to a side stream and runs
@@ -529,11 +478,8 @@ static int run_ops(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp, int* lau
         if (int rc = run_one_op(h, i, n, ph, pw, sp, &cnt)) return rc;
     CK(cudaEventRecord(h->ev_fork, h->stream));
     CK(cudaStreamWaitEvent(h->side, h->ev_fork, 0));
-    CK(ccl_launch(h->d_bitmap, n, ph, pw, h->d_labels, h->d_ccl_scratch, h->d_nlabels, h->side));
-    CK(segrep_launch(h->d_bitmap, h->d_lines, size_t(2) * ph * pw, h->d_ccl_scratch, n, ph, pw, 1000, 1.5f,
-                     h->d_segrep_scratch, h->d_line_boxes, h->d_line_scores, h->d_line_count, h->side));
+    if (int rc = launch_db_post(h, n, ph, pw, h->side, &cnt)) return rc;
     CK(cudaEventRecord(h->ev_join, h->side));
-    cnt += 23;
     size_t last_detect = h->ops.size();
     for (size_t i = 0; i < h->ops.size(); ++i)
       if (!h->db_ancestor[i] && h->ops[i].kind == CTD_OP_DETECT) last_detect = i;
@@ -544,17 +490,13 @@ static int run_ops(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp, int* lau
       if (i == last_detect) {
         CK(cudaEventRecord(h->ev_fork2, h->stream));
         CK(cudaStreamWaitEvent(h->side2, h->ev_fork2, 0));
-        CK(nms_launch(h->d_blks, n, rows, h->cfg.nc, h->cfg.conf_thresh, h->cfg.nms_thresh, h->nms, h->d_det,
-                      h->d_det_count, h->side2));
+        if (int rc = launch_nms(h, n, ph, pw, h->side2, &cnt)) return rc;
         CK(cudaEventRecord(h->ev_join2, h->side2));
         nms_forked = true;
-        cnt += 5;
       }
     }
     if (!nms_forked) {
-      CK(nms_launch(h->d_blks, n, rows, h->cfg.nc, h->cfg.conf_thresh, h->cfg.nms_thresh, h->nms, h->d_det,
-                    h->d_det_count, h->stream));
-      cnt += 5;
+      if (int rc = launch_nms(h, n, ph, pw, h->stream, &cnt)) return rc;
     } else {
       CK(cudaStreamWaitEvent(h->stream, h->ev_join2, 0));
     }
@@ -570,22 +512,16 @@ static int run_ops(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp, int* lau
   *launches = cnt;
   if (h->cfg.debug_skip_postproc) return CTD_OK;
   // post-processing on the same stream
-  CK(nms_launch(h->d_blks, n, rows, h->cfg.nc, h->cfg.conf_thresh, h->cfg.nms_thresh, h->nms, h->d_det,
-                h->d_det_count, h->stream));
-  cnt += 5;
+  if (int rc = launch_nms(h, n, ph, pw, h->stream, &cnt)) return rc;
   if (record) CK(cudaEventRecord(h->op_events[evi++], h->stream));
-  CK(ccl_launch(h->d_bitmap, n, ph, pw, h->d_labels, h->d_ccl_scratch, h->d_nlabels, h->stream));
-  cnt += 8;
-  CK(segrep_launch(h->d_bitmap, h->d_lines, size_t(2) * ph * pw, h->d_ccl_scratch, n, ph, pw, 1000, 1.5f,
-                   h->d_segrep_scratch, h->d_line_boxes, h->d_line_scores, h->d_line_count, h->stream));
-  cnt += 15;
+  if (int rc = launch_db_post(h, n, ph, pw, h->stream, &cnt)) return rc;
   if (record) CK(cudaEventRecord(h->op_events[evi++], h->stream));
   *launches = cnt;
   return CTD_OK;
 }
 
-// shape checks + plan lookup + (first time) graph capture; the forward itself is enqueue_forward()
-int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out) {
+// shape checks + the launch plans of (n, ph, pw), built on first use
+static int find_plan(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out) {
   if (n < 1 || n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
   if (ph % 64 || pw % 64 || ph > h->cfg.max_h || pw > h->cfg.max_w || ph < 64 || pw < 64)
     return ctd_fail(h, CTD_E_SHAPE, "page %dx%d must be a multiple of 64 and <= %dx%d", ph, pw, h->cfg.max_h, h->cfg.max_w);
@@ -597,20 +533,25 @@ int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan*
     if (int rc = build_plans(h, n, ph, pw, sp)) return rc;
     it = h->plans.emplace(key, std::move(sp)).first;
   }
-  ShapePlan& sp = it->second;
-  if (h->cfg.use_graph && !sp.graph && (h->cfg.precision == CTD_PREC_FP16_TC || h->cfg.precision == CTD_PREC_SPLIT_TC)) {
-    // DETECT params are fetched with a blocking memcpy in the SIMT path: plans are already built, so
-    // capture only sees kernel launches (TC path).  SIMT paths run un-captured.
+  *out = &it->second;
+  return CTD_OK;
+}
+
+// plan lookup + (first time, use_graph) graph capture; the forward itself is enqueue_forward()
+int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out) {
+  ShapePlan* sp = nullptr;
+  if (int rc = find_plan(h, n, ph, pw, &sp)) return rc;
+  if (h->cfg.use_graph && !sp->graph) {
     cudaGraph_t graph;
     CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-    int rc = run_ops(h, n, ph, pw, sp, &sp.launches);
+    int rc = run_ops(h, n, ph, pw, *sp, &sp->launches);
     cudaError_t e = cudaStreamEndCapture(h->stream, &graph);
     if (rc) return rc;
     CK(e);
-    CK(cudaGraphInstantiate(&sp.graph, graph, 0));
+    CK(cudaGraphInstantiate(&sp->graph, graph, 0));
     cudaGraphDestroy(graph);
   }
-  *out = &sp;
+  *out = sp;
   return CTD_OK;
 }
 
@@ -894,25 +835,17 @@ extern "C" int ctd_profile_forward(ctd_handle* h, const uint8_t* pages, int32_t 
   if (!h || !pages || !op_ms) return CTD_E_INVALID;
   const int need = int(h->ops.size()) + 2;
   if (cap < need) return ctd_fail(h, CTD_E_INVALID, "op_ms needs %d entries", need);
-  if (n < 1 || n > h->cfg.max_batch || ph % 64 || pw % 64 || ph > h->cfg.max_h || pw > h->cfg.max_w)
-    return ctd_fail(h, CTD_E_SHAPE, "bad shape");
-  CK(cudaSetDevice(h->cfg.device));
+  ShapePlan* sp = nullptr;
+  if (int rc = find_plan(h, n, ph, pw, &sp)) return rc;
   while (int(h->op_events.size()) < need + 1) {
     cudaEvent_t e;
     CK(cudaEventCreate(&e));
     h->op_events.push_back(e);
   }
-  auto key = std::make_tuple(int(n), int(ph), int(pw));
-  auto it = h->plans.find(key);
-  if (it == h->plans.end()) {
-    ShapePlan sp;
-    if (int rc = build_plans(h, n, ph, pw, sp)) return rc;
-    it = h->plans.emplace(key, std::move(sp)).first;
-  }
   CK(cudaMemcpyAsync(h->d_pages, pages, size_t(n) * ph * pw * 3,
                      pages_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
   int launches = 0;
-  if (int rc = run_ops(h, n, ph, pw, it->second, &launches, true)) return rc;
+  if (int rc = run_ops(h, n, ph, pw, *sp, &launches, true)) return rc;
   CK(cudaStreamSynchronize(h->stream));
   const int nev = h->cfg.debug_skip_postproc ? int(h->ops.size()) : need;
   for (int i = 0; i < need; ++i) op_ms[i] = 0.f;
@@ -999,20 +932,12 @@ extern "C" int ctd_debug_run_ops(ctd_handle* h, const uint8_t* pages, int32_t n,
                                  int32_t last_op) {
   if (!h) return CTD_E_INVALID;
   if (first_op < 0 || last_op >= int(h->ops.size()) || first_op > last_op) return ctd_fail(h, CTD_E_INVALID, "bad op range");
-  if (n < 1 || n > h->cfg.max_batch || ph % 64 || pw % 64 || ph > h->cfg.max_h || pw > h->cfg.max_w || ph < 64 || pw < 64)
-    return ctd_fail(h, CTD_E_SHAPE, "bad shape");
-  CK(cudaSetDevice(h->cfg.device));
-  auto key = std::make_tuple(int(n), int(ph), int(pw));
-  auto it = h->plans.find(key);
-  if (it == h->plans.end()) {
-    ShapePlan sp;
-    if (int rc = build_plans(h, n, ph, pw, sp)) return rc;
-    it = h->plans.emplace(key, std::move(sp)).first;
-  }
+  ShapePlan* sp = nullptr;
+  if (int rc = find_plan(h, n, ph, pw, &sp)) return rc;
   if (pages) CK(cudaMemcpyAsync(h->d_pages, pages, size_t(n) * ph * pw * 3, cudaMemcpyHostToDevice, h->stream));
   int cnt = 0;
   for (int i = first_op; i <= last_op; ++i)
-    if (int rc = run_one_op(h, size_t(i), n, ph, pw, it->second, &cnt)) return rc;
+    if (int rc = run_one_op(h, size_t(i), n, ph, pw, *sp, &cnt)) return rc;
   CK(cudaStreamSynchronize(h->stream));
   h->n = n; h->ph = ph; h->pw = pw;
   h->have_forward = true;

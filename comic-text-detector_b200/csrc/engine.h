@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <array>
 #include <condition_variable>
 #include <deque>
 #include <map>
@@ -47,8 +48,7 @@ struct RefineJob {
 };
 
 struct ShapePlan {
-  std::vector<ConvTcPlan> tc;  // index = op index (unused entries default)
-  std::vector<char> has_tc;
+  std::vector<ConvTcPlan> tc;  // index = op index; block_n == 0: the op runs on the CUDA cores
   cudaGraphExec_t graph = nullptr;
   int launches = 0;
 };
@@ -56,6 +56,7 @@ struct ctd_handle {
   ctd_config cfg{};
   std::vector<ctd_op> ops;
   std::vector<ctd_bufdesc> bufs;
+  std::vector<std::array<float, 7>> detect_prm;   // per op; DETECT: stride, then 3 anchors (w, h) in pixels
   std::string err;
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, tev0 = nullptr, tev1 = nullptr;
@@ -103,8 +104,8 @@ struct ctd_handle {
   cudaEvent_t ev_in_done[2] = {nullptr, nullptr}, ev_in_free[2] = {nullptr, nullptr};
   cudaEvent_t ev_out_ready[2] = {nullptr, nullptr}, ev_out_done[2] = {nullptr, nullptr};
   bool slot_busy[2] = {false, false};
-  // overlapped schedule: post-processing of the DB maps / the Detect rows runs on side streams under the
-  // remaining network ops (see run_ops)
+  // overlapped schedule (programs with a DB tail): post-processing of the DB maps / the Detect rows runs on side
+  // streams under the remaining network ops (see run_ops)
   bool overlap = false;
   cudaStream_t side = nullptr, side2 = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_fork2 = nullptr, ev_join2 = nullptr;

@@ -123,10 +123,10 @@ cudaError_t conv_simt_launch(const ConvSimtParams& p, cudaStream_t s);
 template <typename T>
 cudaError_t stem_launch(const uint8_t* pages, int n, int h, int w, const float* wgt /*[32][108] (ky,kx,c)*/,
                         const float* bias, T* dst, int dst_cstride, int dst_coff, int cout, int act, cudaStream_t s);
-// u8 BGR HWC page -> /255 -> space-to-depth(2): dst[n][h/2][w/2][16], channel = (dy*2+dx)*3 + c, 12..15 = 0
-template <typename T>
-cudaError_t s2d_launch(const uint8_t* pages, int n, int h, int w, T* dst, int dst_cstride, int dst_coff, int pitch_px,
-                       int xoff, cudaStream_t s);
+// Pre-pass of the tensor-core stem: u8 BGR HWC page -> /255 -> space-to-depth(2) into the padded window buffer
+// dst[n][h/2][w/2 + 4][16] fp16 (see conv_tc_plan_stem): pixel x at column x + 1, channel = (dy*2+dx)*3 + c, 12..15 = 0,
+// padding columns zeroed.
+cudaError_t s2d_launch(const uint8_t* pages, int n, int h, int w, __half* dst, cudaStream_t s);
 // fp32 NHWC channel slice -> fp16 hi / lo planes (split-fp16 mode): hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale).
 // src / hi / lo point at the first channel of the slice; `cstride` elements between pixels (same in all three).
 cudaError_t split_planes_launch(const float* src, __half* hi, __half* lo, size_t npix, int c, int cstride,
@@ -161,12 +161,14 @@ struct NmsWorkspace {
 };
 cudaError_t nms_launch(const float* blks, int n, int rows, int nc, float conf, float iou, NmsWorkspace& ws,
                        float* det /*[n][300][6]*/, int* det_count, cudaStream_t s);
+constexpr int kNmsLaunches = 5;   // kernels nms_launch enqueues
 size_t nms_workspace_bytes(int n, int cap);
 void nms_workspace_bind(NmsWorkspace& ws, void* base, int n, int cap);
 
 // 8-connectivity labelling with OpenCV's label numbering; labels i32, n_labels incl. background.
 cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* labels, int32_t* scratch /*3*n*h*w ints*/,
                        int32_t* n_labels, cudaStream_t s);
+constexpr int kCclLaunches = 8;   // kernels and memsets ccl_launch enqueues
 cudaError_t ccl_stats_launch(const int32_t* labels, int h, int w, int32_t* stats, int cap, cudaStream_t s);
 
 // SegDetectorRepresenter.boxes_from_bitmap (segrep.cu).  Lf = foreground union-find roots left in the CCL
@@ -175,6 +177,7 @@ size_t segrep_scratch_bytes(int n, int h, int w, int max_cand);
 cudaError_t segrep_launch(const uint8_t* bitmap, const float* pred, size_t pred_page_stride, const int* Lf, int n, int h,
                           int w, int max_cand, float unclip_ratio, void* scratch, int16_t* boxes, float* scores,
                           int* n_contours, cudaStream_t s);
+constexpr int kSegrepLaunches = 15;   // kernels and memsets segrep_launch enqueues
 cudaError_t binarize_launch(const float* pred, size_t count, float thresh, uint8_t* bitmap, cudaStream_t s);
 
 // refine_mask (refine.cu): one CTA per block window.  d_wins: n_wins x {x1,y1,x2,y2,(int64)pixel offset}

@@ -33,14 +33,6 @@ __device__ __forceinline__ float exp_neg_fast(float v) {
   return y;
 }
 
-// ---------------------------------------------------------------- programmatic dependent launch
-// A kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while its predecessor in the
-// stream is still running: everything before griddep_wait() (barrier init, tensor-map prefetch, bias staging,
-// loads of CONSTANT data such as weights) overlaps the predecessor's tail; griddep_wait() returns once the
-// predecessor grid has completed and its memory is visible.  griddep_launch_dependents() lets the successor start.
-__device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));

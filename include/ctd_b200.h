@@ -47,18 +47,20 @@ extern "C" {
  * weight blob.  The engine owns no architecture knowledge beyond these op kinds.           */
 
 enum ctd_op_kind {
-  CTD_OP_STEM = 0,      /* 6x6 s2 p2 conv on the u8 BGR page (/255 fused), common.py:30-49 cfg L0 */
+  CTD_OP_STEM = 0,      /* 6x6 s2 p2 conv on the u8 BGR page (/255 fused), common.py:30-49 cfg L0;
+                           w32_off: direct form, w16_off: 3x3 window form over the 2x2 space-to-depth page
+                           (tensor cores; src_buf[0] is its padded space-to-depth buffer)  */
   CTD_OP_CONV = 1,      /* k in {1,3}, stride in {1,2}, pad k/2; K-concatenated sources     */
   CTD_OP_DECONV4 = 2,   /* ConvTranspose2d 4x4 s2 p1 (basemodel.py:26) as 4 sub-pixel phases */
   CTD_OP_AVGPOOL2 = 3,  /* AvgPool2d(2,2)                (basemodel.py:38)                  */
   CTD_OP_SPPF_POOL = 4, /* 3 chained MaxPool2d(5,1,2)    (common.py:188-196)                */
   CTD_OP_UPSAMPLE2 = 5, /* nn.Upsample(x2, nearest)      (cfg layers 11,15)                 */
   CTD_OP_DETECT = 6,    /* Detect 1x1 conv + sigmoid + box decode (yolo.py:23-44)           */
-  CTD_OP_SEG_TAIL = 7,  /* ConvT4x4s2 64->1 + sigmoid    (basemodel.py:57-60)               */
-  CTD_OP_DB_TAIL = 8,   /* ConvT2x2s2+BN+ReLU -> ConvT2x2s2 -> sigmoid, both branches
+  CTD_OP_SEG_TAIL = 7,  /* ConvT4x4s2 64->1 + sigmoid    (basemodel.py:57-60); p_off: fp32 [C][4][4],
+                           w16_off: fp16 3x3 conv with the 4 sub-pixel phases as outputs, cout_pad 16 */
+  CTD_OP_DB_TAIL = 8    /* ConvT2x2s2+BN+ReLU -> ConvT2x2s2 -> sigmoid, both branches
                            (basemodel.py:99-103,138-142)                                    */
-  CTD_OP_S2D = 9        /* u8 BGR page -> /255 -> 2x2 space-to-depth, 12(+4 zero) channels at 1/2 resolution:
-                           turns the 6x6 s2 p2 stem conv into a 3x3 s1 p1 conv for the tensor cores       */
+  /* 9 is reserved (a retired op kind)                                                      */
 };
 
 enum ctd_act { CTD_ACT_NONE = 0, CTD_ACT_SILU = 1, CTD_ACT_LEAKY = 2, CTD_ACT_RELU = 3, CTD_ACT_SIGMOID = 4 };
@@ -82,7 +84,7 @@ typedef struct ctd_op {
   int32_t aux;                   /* DETECT: pyramid level (0,1,2)                           */
   int64_t w16_off;               /* blob offset: fp16 weights [phase][cout_pad][taps*Cin] K-major */
   int64_t w32_off;               /* blob offset: fp32 weights, same layout                  */
-  int64_t b_off;                 /* blob offset: fp32 bias[cout_pad] (BN folded)            */
+  int64_t b_off;                 /* blob offset: fp32 bias[cout_pad] (BN folded); STEM, CONV, DECONV4, DETECT */
   int64_t p_off;                 /* blob offset: extra fp32 params (DETECT anchors, tails)  */
 } ctd_op;
 

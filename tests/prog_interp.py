@@ -54,7 +54,7 @@ class Interp:
             return op["src_buf"][0], op["src_coff"][0] + op["src_c"][0], 3 * op["src_c"][0]
         if op["dst_buf"] < 0:
             return None
-        c = op["cout"] if k in (cc.OP_STEM, cc.OP_CONV, cc.OP_DECONV4) else (16 if k == cc.OP_S2D else op["src_c"][0])
+        c = op["cout"] if k in (cc.OP_STEM, cc.OP_CONV, cc.OP_DECONV4) else op["src_c"][0]
         return op["dst_buf"], op["dst_coff"], c
 
     def step(self, i):
@@ -83,13 +83,6 @@ class Interp:
             b = _blob(prog, op["b_off"], op["cout"], np.float32)
             y = _act(F.conv2d(x, wt, b, 2, 2), op["act"])
             bufs[op["dst_buf"]][:, op["dst_coff"]:op["dst_coff"] + op["cout"]] = y
-        elif k == cc.OP_S2D:
-            x = torch.from_numpy(np.ascontiguousarray(pages.transpose(0, 3, 1, 2)).astype(np.float32) / 255)
-            y = torch.zeros(n, 16, h // 2, w // 2)
-            for dy in range(2):
-                for dx in range(2):
-                    y[:, (dy * 2 + dx) * 3:(dy * 2 + dx) * 3 + 3] = x[:, :, dy::2, dx::2]
-            bufs[op["dst_buf"]][:, op["dst_coff"]:op["dst_coff"] + 16] = self.q(y)
         elif k in (cc.OP_CONV, cc.OP_DETECT):
             ks, st = op["ksize"], op["stride"]
             K = ks * ks * cin

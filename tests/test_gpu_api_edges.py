@@ -33,6 +33,17 @@ def test_shape_and_capacity_errors(prog):
         eng.close()
 
 
+@pytest.mark.parametrize("ph", [0, 32])
+def test_profile_forward_rejects_bad_shapes(prog, ph):
+    """the per-op profiler checks the page size like the forward does (at least 64, a multiple of 64)"""
+    eng = ctd_b200.Engine(prog, max_batch=1, max_h=256, max_w=256)
+    try:
+        with pytest.raises(ctd_b200.binding.CtdError, match="multiple of 64"):
+            eng.profile_forward(np.zeros((1, ph, 256, 3), np.uint8))
+    finally:
+        eng.close()
+
+
 @pytest.mark.parametrize("fill", [0, 255])
 def test_blank_pages_through_the_detector(fill):
     det = ctd_b200.TextDetector(get_checkpoint(0, True), input_size=256, act="leaky")

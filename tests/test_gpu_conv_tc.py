@@ -229,8 +229,7 @@ def test_bench_plans_per_op(prec, n, h, w):
         for i, op in enumerate(prog.ops):
             kind = op["kind"]
             gemm = kind in (cc.OP_CONV, cc.OP_DECONV4, cc.OP_DETECT)
-            tc_tail = not split and (kind == cc.OP_STEM or (kind == cc.OP_SEG_TAIL and op["w16_off"] > 0
-                                                             and op["cout_pad"] == 16))
+            tc_tail = not split and kind in (cc.OP_STEM, cc.OP_SEG_TAIL)
             if not (gemm or tc_tail):
                 continue
             srcs = [(op["src_buf"][j], op["src_coff"][j], op["src_c"][j]) for j in range(op["n_src"])]

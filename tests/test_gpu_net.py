@@ -75,10 +75,13 @@ def _check_against_oracle(prec, smooth, n, h, w, use_graph=False, seed=1000):
     return pages, prog, (blks, mask, lines)
 
 
-@pytest.mark.parametrize("prec", [PREC_FP32_SIMT, PREC_FP16_SIMT, PREC_FP16_TC, PREC_SPLIT_TC])
+@pytest.mark.parametrize("prec,use_graph", [
+    pytest.param(p, g, id="%d%s" % (p, "-graph" if g else ""))
+    for p, g in [(PREC_FP32_SIMT, False), (PREC_FP16_SIMT, False), (PREC_FP16_TC, False), (PREC_SPLIT_TC, False),
+                 (PREC_FP32_SIMT, True), (PREC_FP16_SIMT, True)]])
 @pytest.mark.parametrize("smooth", [False, True], ids=["rough", "smooth"])
-def test_forward_matches_oracle(prec, smooth):
-    _check_against_oracle(prec, smooth, 2, 256, 320)
+def test_forward_matches_oracle(prec, use_graph, smooth):
+    _check_against_oracle(prec, smooth, 2, 256, 320, use_graph=use_graph)
 
 
 def test_benchmark_config_matches_oracle():
