@@ -1,11 +1,13 @@
 // wgmma implicit-GEMM convolution for sm_90a.
 //
-//   D[128 x BN] (fp32, registers) += A[128 x 16] * B[BN x 16]^T, K-major fp16 operands in 128B/64B/32B-swizzled shared
-//   memory; the 128 rows are a 16x8-pixel tile, the BN columns a slice of output channels
+//   D[16*TH x BN] (fp32, registers) += A[16*TH x 16] * B[BN x 16]^T, K-major fp16 operands in 128B/64B/32B-swizzled
+//   shared memory; the 16*TH rows are a 16xTH-pixel tile (TH = 8 or 16), the BN columns a slice of output channels
 //
 // Persistent, one CTA per SM, 384 threads: warpgroup 0 = TMA producer (one elected thread), warpgroups 1 and 2 =
-// consumers, each issuing wgmma m64nBNk16 for its 64 rows of the tile (4 of the 8 pixel rows) and running the epilogue
-// on its own accumulators.  An mbarrier full/empty ring of operand stages sits between producer and consumers; each
+// consumers, each owning TH/2 pixel rows of the tile (8*TH accumulator rows): per K = 16 step it issues TH/8 wgmma
+// m64nBNk16 against the same B descriptor, and it runs the epilogue on its own accumulators.  At TH = 16 the producer
+// warpgroup gives registers to the consumers (setmaxnreg 40 / 232: 128 accumulators per thread at BN = 128).  An
+// mbarrier full/empty ring of operand stages sits between producer and consumers; each
 // consumer keeps one wgmma group in flight and frees the stage of the previous group once that group has retired.
 // Activations are 4-D TMA boxes over the NHWC buffers: out-of-bounds zero-fill IS the convolution padding, there is
 // no im2col buffer; torch.cat inputs are K-concatenated from up to 3 tensor maps; stride 2 reads four parity maps;
@@ -24,14 +26,17 @@
 
 namespace ctd {
 
-constexpr int kTileW = 16, kTileH = 8;  // 128 grid pixels per tile
-constexpr int kThreads = 384;           // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
+constexpr int kTileW = 16;     // tile width in grid pixels; the height TH (8 or 16) is a template parameter
+constexpr int kThreads = 384;  // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
 
-template <int BN>
+// Shared memory per (BN, TH): stages x (A box of 16*TH rows + B box of BN rows, 128-byte rows in the worst case).
+//   TH = 8:  BN 128: 6 x 32 KB | 64: 8 x 24 KB | 32: 10 x 20 KB | 16: 10 x 18 KB
+//   TH = 16: BN 128: 4 x 48 KB | 64: 5 x 40 KB | 32:  6 x 36 KB | 16:  6 x 34 KB
+template <int BN, int TH>
 struct TcCfg {
-  static constexpr int kABytes = 128 * 128;  // per stage (worst case 128-byte rows)
+  static constexpr int kABytes = TH * kTileW * 128;  // per stage (worst case 128-byte rows)
   static constexpr int kBBytes = BN * 128;
-  static constexpr int kStages = BN >= 128 ? 6 : (BN >= 64 ? 8 : 10);
+  static constexpr int kStages = TH == 8 ? (BN >= 128 ? 6 : (BN >= 64 ? 8 : 10)) : (BN >= 128 ? 4 : (BN >= 64 ? 5 : 6));
   static constexpr int kBiasFloats = 512;
   // 1024 bytes of alignment slack | operand ring | barriers (256 B) | bias
   static constexpr size_t kSmem = 1024 + size_t(kStages) * (kABytes + kBBytes) + 256 + kBiasFloats * 4;
@@ -135,9 +140,10 @@ __device__ __forceinline__ void epilogue_f32(const float (&acc)[BN / 2], const f
   }
 }
 
-template <int BN>
+template <int BN, int TH>
 __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
-  using Cfg = TcCfg<BN>;
+  using Cfg = TcCfg<BN, TH>;
+  constexpr int MT = TH / 8;   // m64 row blocks per consumer warpgroup
   extern __shared__ __align__(1024) uint8_t smem_tc[];
   // the swizzled operand stages need 1024-byte alignment; the dynamic base is only guaranteed 16
   const uint32_t raw_base = smem_u32(smem_tc);
@@ -155,7 +161,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
 
   const int kb = p.kb_elems;
   const uint32_t row_bytes = kb * 2;
-  const uint32_t stage_tx = 128u * row_bytes + uint32_t(BN) * row_bytes;
+  const uint32_t stage_tx = uint32_t(TH * kTileW) * row_bytes + uint32_t(BN) * row_bytes;
   int kblocks_per_tap = 0;
   for (int s = 0; s < g.n_src; ++s) kblocks_per_tap += p.src_kblocks[s];
   const int n_terms = p.split ? 3 : 1;   // split-fp16 mode: (hi,hi) + (lo,hi) + (hi,lo) per K block
@@ -188,13 +194,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     img = sp / tiles_per_img;
     const int trem = sp - img * tiles_per_img;
     const int ty = trem / p.tiles_x;
-    y0 = ty * kTileH;
+    y0 = ty * TH;
     x0 = (trem - ty * p.tiles_x) * kTileW;
   };
 
-  if (warp == 0) {
-    // =============================== TMA producer ===============================
-    if (elect_one()) {
+  if (warp < 4) {
+    // =============================== TMA producer (warpgroup 0) ===============================
+    if constexpr (TH == 16) setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
       int it = 0;
       for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         int phase, nblk, img, y0, x0;
@@ -224,14 +231,15 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     }
     return;
   }
-  if (warp < 4) return;
 
   // =============================== consumers ====================================
-  const int wg = (warp >> 2) - 1;                   // rows [64*wg, 64*wg + 64) of the tile
-  const int wrow = ((warp & 3) << 4) + (lane >> 2);  // this thread's first fragment row within the 64
+  if constexpr (TH == 16) setmaxnreg_inc<232>();
+  const int wg = (warp >> 2) - 1;                   // rows [64*MT*wg, 64*MT*(wg + 1)) of the tile
+  const int wrow = ((warp & 3) << 4) + (lane >> 2);  // this thread's first fragment row within a 64-row block
   const bool wg_leader = (threadIdx.x & 127) == 0;
-  const uint64_t a_desc0 = make_kmajor_desc(a_base + uint32_t(wg) * 64u * row_bytes, row_bytes);
+  const uint64_t a_desc0 = make_kmajor_desc(a_base + uint32_t(wg * MT) * 64u * row_bytes, row_bytes);
   const uint64_t b_desc0 = make_kmajor_desc(b_base, row_bytes);
+  const uint64_t a_mstep = (64u * row_bytes) >> 4;   // descriptor step from one 64-row block to the next
   const int ksteps = kb / 16;
   int stage = 0;
   uint32_t full_par = 0;
@@ -240,12 +248,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
     int phase, nblk, img, y0, x0;
     decode(t, phase, nblk, img, y0, x0);
-    float acc[R];
+    float acc[MT][R];
 #pragma unroll
-    for (int i = 0; i < R; ++i) acc[i] = 0.f;
+    for (int m = 0; m < MT; ++m)
+#pragma unroll
+      for (int i = 0; i < R; ++i) acc[m][i] = 0.f;
 
     bool split_done = false;
-    if constexpr (BN <= 64) {
+    if constexpr (BN <= 64 && TH == 8) {   // conv_tc_plan keeps split mode at 16x8 tiles
       if (p.split) {
         // Split-fp16 mode with PROMOTED accumulation.  The tensor core adds into its fp32 accumulator with
         // truncation: over the K/16 x 3 MMAs of a deep layer the one-sided errors add up to ~K/16 ulps.  So every
@@ -269,7 +279,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
               wgmma_wait<0>();
               wgmma_fence_regs(tmp);
 #pragma unroll
-              for (int i = 0; i < R; ++i) acc[i] = __fadd_rn(acc[i], tmp[i]);
+              for (int i = 0; i < R; ++i) acc[0][i] = __fadd_rn(acc[0][i], tmp[i]);
             }
           } else {
             wgmma_fence();
@@ -284,7 +294,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
           if (++stage == Cfg::kStages) { stage = 0; full_par ^= 1u; }
         }
 #pragma unroll
-        for (int i = 0; i < R; ++i) acc[i] = __fadd_rn(acc[i], cross[i] * kSplitLoUnscale);
+        for (int i = 0; i < R; ++i) acc[0][i] = __fadd_rn(acc[0][i], cross[i] * kSplitLoUnscale);
         split_done = true;
       }
     }
@@ -295,7 +305,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         const uint64_t ad = a_desc0 + uint64_t(stage) * (Cfg::kABytes >> 4);
         const uint64_t bd = b_desc0 + uint64_t(stage) * (Cfg::kBBytes >> 4);
         wgmma_fence();
-        for (int ks = 0; ks < ksteps; ++ks) wgmma_bn<BN>(acc, ad + 2 * ks, bd + 2 * ks, (k_it > 0 || ks > 0) ? 1u : 0u);
+        // every row block m reads the same B box: an output element's K order does not depend on TH
+        for (int ks = 0; ks < ksteps; ++ks)
+#pragma unroll
+          for (int m = 0; m < MT; ++m)
+            wgmma_bn<BN>(acc[m], ad + m * a_mstep + 2 * ks, bd + 2 * ks, (k_it > 0 || ks > 0) ? 1u : 0u);
         wgmma_commit();
         // one group stays in flight: the previous group has retired, its stage goes back to the producer
         wgmma_wait<1>();
@@ -304,7 +318,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         if (++stage == Cfg::kStages) { stage = 0; full_par ^= 1u; }
       }
       wgmma_wait<0>();
-      wgmma_fence_regs(acc);
+#pragma unroll
+      for (int m = 0; m < MT; ++m) wgmma_fence_regs(acc[m]);
       if (prev >= 0 && wg_leader) mbar_arrive(empty_bar + 8 * prev);
     }
 
@@ -312,94 +327,97 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     const int ph_y = phase >> 1, ph_x = phase & 1;
     const float* bias_t = bias_s + nblk * BN;
     const int ncols = g.cout - nblk * BN;   // columns of this N block that exist
-    int gy[2], gx[2];
-    bool valid[2];
-    size_t pix[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = wg * 64 + wrow + 8 * h;
-      gy[h] = y0 + row / kTileW;
-      gx[h] = x0 + row % kTileW;
-      valid[h] = gy[h] < g.gh && gx[h] < g.gw;
-      const int oy = gy[h] * g.out_mul + ph_y, ox = gx[h] * g.out_mul + ph_x;
-      pix[h] = valid[h] ? size_t(img) * g.dst_h * g.dst_w + size_t(oy) * g.dst_w + ox : 0;
-    }
-    if constexpr (BN == 16) {
-      if (p.seg_f32 != nullptr) {
-        // seg tail: 4 phase logits per grid pixel -> sigmoid -> one row (py2 = the column pair lane & 3) of the
-        // pixel's 2x2 block in the f32 and u8 masks
-        const int py2 = lane & 3;
-        if (py2 < 2) {
-          const size_t ow2 = size_t(g.gw) * 2;
+    for (int m = 0; m < MT; ++m) {
+      int gy[2], gx[2];
+      bool valid[2];
+      size_t pix[2];
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            if (!valid[h]) continue;
-            const size_t o = (size_t(img) * g.gh * 2 + size_t(gy[h]) * 2 + py2) * ow2 + size_t(gx[h]) * 2;
-            const float s0 = 1.0f / (1.0f + expf(-acc[2 * h]));
-            const float s1 = 1.0f / (1.0f + expf(-acc[2 * h + 1]));
-            *reinterpret_cast<float2*>(p.seg_f32 + o) = make_float2(s0, s1);
-            *reinterpret_cast<uchar2*>(p.seg_u8 + o) = make_uchar2((uint8_t)(s0 * 255.0f), (uint8_t)(s1 * 255.0f));
+      for (int h = 0; h < 2; ++h) {
+        const int row = (wg * MT + m) * 64 + wrow + 8 * h;
+        gy[h] = y0 + row / kTileW;
+        gx[h] = x0 + row % kTileW;
+        valid[h] = gy[h] < g.gh && gx[h] < g.gw;
+        const int oy = gy[h] * g.out_mul + ph_y, ox = gx[h] * g.out_mul + ph_x;
+        pix[h] = valid[h] ? size_t(img) * g.dst_h * g.dst_w + size_t(oy) * g.dst_w + ox : 0;
+      }
+      if constexpr (BN == 16) {
+        if (p.seg_f32 != nullptr) {
+          // seg tail: 4 phase logits per grid pixel -> sigmoid -> one row (py2 = the column pair lane & 3) of the
+          // pixel's 2x2 block in the f32 and u8 masks
+          const int py2 = lane & 3;
+          if (py2 < 2) {
+            const size_t ow2 = size_t(g.gw) * 2;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (!valid[h]) continue;
+              const size_t o = (size_t(img) * g.gh * 2 + size_t(gy[h]) * 2 + py2) * ow2 + size_t(gx[h]) * 2;
+              const float s0 = 1.0f / (1.0f + expf(-acc[m][2 * h]));
+              const float s1 = 1.0f / (1.0f + expf(-acc[m][2 * h + 1]));
+              *reinterpret_cast<float2*>(p.seg_f32 + o) = make_float2(s0, s1);
+              *reinterpret_cast<uchar2*>(p.seg_u8 + o) = make_uchar2((uint8_t)(s0 * 255.0f), (uint8_t)(s1 * 255.0f));
+            }
+          }
+          continue;
+        }
+      }
+      if (p.dst == nullptr) {
+        // Detect decode (yolo.py:36-44): columns = anchor*(5+nc) + o
+        const int no = 5 + p.nc;
+        float* rows = p.blks + (size_t(img) * p.blks_rows_per_img + p.level_row0) * no;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!valid[h]) continue;
+#pragma unroll
+          for (int i = 0; i < R; ++i) {
+            if (((i >> 1) & 1) != h) continue;
+            const int c = (i >> 2) * 8 + (lane & 3) * 2 + (i & 1);
+            if (c >= ncols) continue;
+            const int col = nblk * BN + c;
+            const int a = col / no, o = col - a * no;
+            const float s = 1.0f / (1.0f + expf(-(acc[m][i] + bias_t[c])));
+            float r;
+            if (o == 0) r = (s * 2.0f - 0.5f + float(gx[h])) * p.det_stride;
+            else if (o == 1) r = (s * 2.0f - 0.5f + float(gy[h])) * p.det_stride;
+            else if (o == 2) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a];
+            else if (o == 3) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a + 1];
+            else r = s;
+            rows[(size_t(a) * g.gh * g.gw + size_t(gy[h]) * g.gw + gx[h]) * no + o] = r;
           }
         }
-        continue;
-      }
-    }
-    if (p.dst == nullptr) {
-      // Detect decode (yolo.py:36-44): columns = anchor*(5+nc) + o
-      const int no = 5 + p.nc;
-      float* rows = p.blks + (size_t(img) * p.blks_rows_per_img + p.level_row0) * no;
+      } else if (p.split) {
+        float* out32[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!valid[h]) continue;
-#pragma unroll
-        for (int i = 0; i < R; ++i) {
-          if (((i >> 1) & 1) != h) continue;
-          const int c = (i >> 2) * 8 + (lane & 3) * 2 + (i & 1);
-          if (c >= ncols) continue;
-          const int col = nblk * BN + c;
-          const int a = col / no, o = col - a * no;
-          const float s = 1.0f / (1.0f + expf(-(acc[i] + bias_t[c])));
-          float r;
-          if (o == 0) r = (s * 2.0f - 0.5f + float(gx[h])) * p.det_stride;
-          else if (o == 1) r = (s * 2.0f - 0.5f + float(gy[h])) * p.det_stride;
-          else if (o == 2) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a];
-          else if (o == 3) r = (s * 2.0f) * (s * 2.0f) * p.anchor_wh[2 * a + 1];
-          else r = s;
-          rows[(size_t(a) * g.gh * g.gw + size_t(gy[h]) * g.gw + gx[h]) * no + o] = r;
+        for (int h = 0; h < 2; ++h)
+          out32[h] = reinterpret_cast<float*>(p.dst) + pix[h] * g.dst_cstride + g.dst_coff + nblk * BN;
+        const bool res = g.residual != 0;
+        switch (g.act) {
+          case CTD_ACT_SILU: epilogue_f32<BN, CTD_ACT_SILU>(acc[m], bias_t, out32, valid, ncols, lane, res); break;
+          case CTD_ACT_LEAKY: epilogue_f32<BN, CTD_ACT_LEAKY>(acc[m], bias_t, out32, valid, ncols, lane, res); break;
+          case CTD_ACT_RELU: epilogue_f32<BN, CTD_ACT_RELU>(acc[m], bias_t, out32, valid, ncols, lane, res); break;
+          case CTD_ACT_SIGMOID: epilogue_f32<BN, CTD_ACT_SIGMOID>(acc[m], bias_t, out32, valid, ncols, lane, res); break;
+          default: epilogue_f32<BN, CTD_ACT_NONE>(acc[m], bias_t, out32, valid, ncols, lane, res); break;
         }
-      }
-    } else if (p.split) {
-      float* out32[2];
+      } else {
+        __half* out[2];
+        const __half* res[2];   // residual: read from the destination itself (in-place add)
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
-        out32[h] = reinterpret_cast<float*>(p.dst) + pix[h] * g.dst_cstride + g.dst_coff + nblk * BN;
-      const bool res = g.residual != 0;
-      switch (g.act) {
-        case CTD_ACT_SILU: epilogue_f32<BN, CTD_ACT_SILU>(acc, bias_t, out32, valid, ncols, lane, res); break;
-        case CTD_ACT_LEAKY: epilogue_f32<BN, CTD_ACT_LEAKY>(acc, bias_t, out32, valid, ncols, lane, res); break;
-        case CTD_ACT_RELU: epilogue_f32<BN, CTD_ACT_RELU>(acc, bias_t, out32, valid, ncols, lane, res); break;
-        case CTD_ACT_SIGMOID: epilogue_f32<BN, CTD_ACT_SIGMOID>(acc, bias_t, out32, valid, ncols, lane, res); break;
-        default: epilogue_f32<BN, CTD_ACT_NONE>(acc, bias_t, out32, valid, ncols, lane, res); break;
-      }
-    } else {
-      __half* out[2];
-      const __half* res[2];   // residual: read from the destination itself (in-place add)
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        out[h] = p.dst + pix[h] * g.dst_cstride + g.dst_coff + nblk * BN;
-        res[h] = out[h];
-      }
-#define CTD_EPI(ACT)                                                                            \
-  if (g.residual) epilogue_f16<BN, ACT, true>(acc, bias_t, out, res, valid, ncols, lane);      \
-  else epilogue_f16<BN, ACT, false>(acc, bias_t, out, res, valid, ncols, lane);
-      switch (g.act) {
-        case CTD_ACT_SILU: CTD_EPI(CTD_ACT_SILU) break;
-        case CTD_ACT_LEAKY: CTD_EPI(CTD_ACT_LEAKY) break;
-        case CTD_ACT_RELU: CTD_EPI(CTD_ACT_RELU) break;
-        case CTD_ACT_SIGMOID: CTD_EPI(CTD_ACT_SIGMOID) break;
-        default: CTD_EPI(CTD_ACT_NONE) break;
-      }
+        for (int h = 0; h < 2; ++h) {
+          out[h] = p.dst + pix[h] * g.dst_cstride + g.dst_coff + nblk * BN;
+          res[h] = out[h];
+        }
+#define CTD_EPI(ACT)                                                                             \
+  if (g.residual) epilogue_f16<BN, ACT, true>(acc[m], bias_t, out, res, valid, ncols, lane);   \
+  else epilogue_f16<BN, ACT, false>(acc[m], bias_t, out, res, valid, ncols, lane);
+        switch (g.act) {
+          case CTD_ACT_SILU: CTD_EPI(CTD_ACT_SILU) break;
+          case CTD_ACT_LEAKY: CTD_EPI(CTD_ACT_LEAKY) break;
+          case CTD_ACT_RELU: CTD_EPI(CTD_ACT_RELU) break;
+          case CTD_ACT_SIGMOID: CTD_EPI(CTD_ACT_SIGMOID) break;
+          default: CTD_EPI(CTD_ACT_NONE) break;
+        }
 #undef CTD_EPI
+      }
     }
   }
 }
@@ -420,8 +438,8 @@ static const char* encode_map(PFN_encodeTiled enc, CUtensorMap* m, const void* b
 
 static int g_num_sms = 132;
 
-// N block: at most 128 output channels, so that a consumer warpgroup's 64 x BN fp32 accumulator fits in registers
-// (64 per thread) next to the epilogue's addresses
+// N block: at most 128 output channels, so that a consumer warpgroup's 8*TH x BN fp32 accumulator fits in registers
+// (64 per thread at TH = 8, 128 at TH = 16) next to the epilogue's addresses
 static int pick_block_n(int cout_pad) {
   if (cout_pad >= 128 && cout_pad % 128 == 0) return 128;
   if (cout_pad % 64 == 0) return 64;
@@ -429,12 +447,13 @@ static int pick_block_n(int cout_pad) {
   return 16;
 }
 
+template <int TH>
 static size_t smem_for(int bn) {
   switch (bn) {
-    case 128: return TcCfg<128>::kSmem;
-    case 64: return TcCfg<64>::kSmem;
-    case 32: return TcCfg<32>::kSmem;
-    default: return TcCfg<16>::kSmem;
+    case 128: return TcCfg<128, TH>::kSmem;
+    case 64: return TcCfg<64, TH>::kSmem;
+    case 32: return TcCfg<32, TH>::kSmem;
+    default: return TcCfg<16, TH>::kSmem;
   }
 }
 
@@ -458,7 +477,19 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
   p.kb_elems = kb;
   for (int s = 0; s < g.n_src; ++s) p.src_kblocks[s] = g.src_c[s] / kb;
   p.tiles_x = (g.gw + kTileW - 1) / kTileW;
-  p.tiles_y = (g.gh + kTileH - 1) / kTileH;
+  int bn = pick_block_n(g.cout_pad);
+  // small grids (the 1/32 and 1/64 layers): a narrower N block spreads the layer over more SMs
+  const int tiles8 = g.n_img * p.tiles_x * ((g.gh + 7) / 8) * g.n_phase;   // 16x8 tiles per N block
+  while (bn > 64 && tiles8 * (g.cout_pad / bn) <= g_num_sms / 2) bn /= 2;
+  if (split && bn > 64) bn = 64;   // promoted accumulation keeps three BN/2-float fragments per thread in registers
+  // 16x16 tiles (M = 256) read each weight box once per 256 pixels instead of 128.  Used for the fp16 NHWC-store ops
+  // (CONV, DECONV4) whose layer still has a tile per SM at that size; split mode, Detect and the seg tail
+  // (dst == nullptr) stay at 16x8.
+  int th = 8;
+  if (!split && dst != nullptr &&
+      g.n_img * p.tiles_x * ((g.gh + 15) / 16) * g.n_phase * (g.cout_pad / bn) >= g_num_sms)
+    th = 16;
+  p.tiles_y = (g.gh + th - 1) / th;
   p.dst = dst;
   p.bias = bias;
   const int sh = g.src_h, sw = g.src_w;
@@ -468,7 +499,7 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
     if (g.in_stride == 1) {
       cuuint64_t dims[4] = {cuuint64_t(g.src_c[s]), cuuint64_t(sw), cuuint64_t(sh), cuuint64_t(g.n_img * n_planes)};
       cuuint64_t str[3] = {cs * 2, cs * 2 * sw, cs * 2 * sw * sh};
-      cuuint32_t box[4] = {cuuint32_t(kb), kTileW, kTileH, 1};
+      cuuint32_t box[4] = {cuuint32_t(kb), kTileW, cuuint32_t(th), 1};
       if (const char* e = encode_map(enc, &p.a_map[s][0], base, 4, dims, str, box, kb)) return e;
     } else {
       // parity views: pixel (2*yh+yp, 2*xh+xp)
@@ -476,7 +507,7 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
         const int yp = q >> 1, xp = q & 1;
         cuuint64_t dims[4] = {cuuint64_t(g.src_c[s]), cuuint64_t(sw / 2), cuuint64_t(sh / 2), cuuint64_t(g.n_img * n_planes)};
         cuuint64_t str[3] = {cs * 2 * 2, cs * 2 * sw * 2, cs * 2 * sw * sh};
-        cuuint32_t box[4] = {cuuint32_t(kb), kTileW, kTileH, 1};
+        cuuint32_t box[4] = {cuuint32_t(kb), kTileW, cuuint32_t(th), 1};
         const char* b2 = base + (size_t(yp) * sw + xp) * cs * 2;
         if (const char* e = encode_map(enc, &p.a_map[s][q], b2, 4, dims, str, box, kb)) return e;
       }
@@ -496,11 +527,8 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
         p.tap_map[ph][t] = 0;
       }
     }
-  int bn = pick_block_n(g.cout_pad);
-  // small grids (the 1/32 and 1/64 layers): a narrower N block spreads the layer over more SMs
-  while (bn > 64 && g.n_img * p.tiles_x * p.tiles_y * (g.cout_pad / bn) * g.n_phase <= g_num_sms / 2) bn /= 2;
-  if (split && bn > 64) bn = 64;   // promoted accumulation keeps three BN/2-float fragments per thread in registers
   plan.block_n = bn;
+  plan.tile_h = th;
   if (split && ((g.dst_coff % 4) != 0 || (g.dst_cstride % 4) != 0 || (dst != nullptr && g.cout % 4 != 0)))
     return "conv_tc (split): fp32 destination slice must be 16-byte aligned";
   {
@@ -514,7 +542,7 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
     plan.grid = dim3(unsigned(total_tiles < g_num_sms ? total_tiles : g_num_sms), 1, 1);
   }
   if (g.cout_pad > 512) return "conv_tc: cout_pad > 512 not supported (bias staging)";
-  plan.smem_bytes = smem_for(bn);
+  plan.smem_bytes = th == 16 ? smem_for<16>(bn) : smem_for<8>(bn);
   return nullptr;
 }
 
@@ -533,7 +561,7 @@ const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void*
   p.kb_elems = 64;
   p.src_kblocks[0] = 1;
   p.tiles_x = (ow + kTileW - 1) / kTileW;
-  p.tiles_y = (oh + kTileH - 1) / kTileH;
+  p.tiles_y = (oh + 7) / 8;   // 16x8 tiles
   p.dst = dst;
   p.bias = bias;
   {
@@ -541,10 +569,11 @@ const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void*
     // 64 contiguous channels (4 pixels); window x starts at padded pixel x = original pixel x-1
     cuuint64_t dims[4] = {64, cuuint64_t(ow), cuuint64_t(oh), cuuint64_t(n)};
     cuuint64_t str[3] = {32, cuuint64_t(pitch) * 32, cuuint64_t(pitch) * 32 * oh};
-    cuuint32_t box[4] = {64, kTileW, kTileH, 1};
+    cuuint32_t box[4] = {64, kTileW, 8, 1};
     if (const char* e = encode_map(enc, &p.a_map[0][0], s2d, 4, dims, str, box, 64)) return e;
   }
   plan.block_n = 32;
+  plan.tile_h = 8;
   {
     cuuint64_t dims[2] = {192, 32};
     cuuint64_t str[1] = {192 * 2};
@@ -553,7 +582,7 @@ const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void*
   }
   const int total_tiles = n * p.tiles_x * p.tiles_y;
   plan.grid = dim3(unsigned(total_tiles < g_num_sms ? total_tiles : g_num_sms), 1, 1);
-  plan.smem_bytes = TcCfg<32>::kSmem;
+  plan.smem_bytes = TcCfg<32, 8>::kSmem;
   return nullptr;
 }
 
@@ -564,21 +593,29 @@ cudaError_t conv_tc_init() {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) g_num_sms = n;
   }
-#define CTD_SET(BN)                                                                                   \
-  e = cudaFuncSetAttribute(conv_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(TcCfg<BN>::kSmem)); \
+#define CTD_SET(BN, TH)                                                                                       \
+  e = cudaFuncSetAttribute(conv_tc_kernel<BN, TH>, cudaFuncAttributeMaxDynamicSharedMemorySize,               \
+                           int(TcCfg<BN, TH>::kSmem));                                                        \
   if (e != cudaSuccess) return e;
-  CTD_SET(128) CTD_SET(64) CTD_SET(32) CTD_SET(16)
+  CTD_SET(128, 8) CTD_SET(64, 8) CTD_SET(32, 8) CTD_SET(16, 8)
+  CTD_SET(128, 16) CTD_SET(64, 16) CTD_SET(32, 16) CTD_SET(16, 16)
 #undef CTD_SET
   return cudaSuccess;
 }
 
-cudaError_t conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s) {
+template <int TH>
+static void launch_th(const ConvTcPlan& plan, cudaStream_t s) {
   switch (plan.block_n) {
-    case 128: conv_tc_kernel<128><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
-    case 64: conv_tc_kernel<64><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
-    case 32: conv_tc_kernel<32><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
-    default: conv_tc_kernel<16><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
+    case 128: conv_tc_kernel<128, TH><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
+    case 64: conv_tc_kernel<64, TH><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
+    case 32: conv_tc_kernel<32, TH><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
+    default: conv_tc_kernel<16, TH><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p); break;
   }
+}
+
+cudaError_t conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s) {
+  if (plan.tile_h == 16) launch_th<16>(plan, s);
+  else launch_th<8>(plan, s);
   return cudaGetLastError();
 }
 

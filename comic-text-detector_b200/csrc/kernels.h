@@ -55,7 +55,7 @@ struct alignas(64) ConvTcParams {
   ConvGeom g;
   int kb_elems;                       // channels per K block: 64 / 32 / 16 (swizzle 128/64/32 B)
   int src_kblocks[CTD_MAX_SRC];
-  int tiles_x, tiles_y;               // 16x8-pixel tiles per image
+  int tiles_x, tiles_y;               // 16xTH-pixel tiles per image (TH = ConvTcPlan::tile_h)
   int8_t tap_map[kMaxPhases][kMaxTaps];  // parity map index per tap (stride 2), else 0
   __half* dst;
   const float* bias;
@@ -83,6 +83,7 @@ struct alignas(64) ConvTcParams {
 struct ConvTcPlan {
   ConvTcParams p;
   int block_n;
+  int tile_h;   // TH: 8 or 16 pixel rows per tile
   dim3 grid;
   size_t smem_bytes;
 };

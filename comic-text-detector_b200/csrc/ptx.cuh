@@ -22,6 +22,13 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
+// Warpgroup register reallocation (every warp of the warpgroup executes it): a producer warpgroup hands registers
+// back to the pool, consumer warpgroups take them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------- fast activation math
 // e^-v for the fast SiLU / sigmoid epilogues: ONE ex2.approx.ftz.  `__expf` is ex2.approx WITHOUT .ftz, which the compiler
 // wraps in a denormal guard (FSETP + two predicated FMULs per element: a quarter of the epilogue's instructions, ncu
