@@ -54,6 +54,13 @@ class CtdResultsLayout(C.Structure):
 
 MAX_BLOCKS, MAX_BLOCK_DIST = 1300, 8192   # CTD_MAX_BLOCKS / CTD_MAX_BLOCK_DIST
 
+# numpy mirrors of `ctd_region_line` / `ctd_region` (include/ctd_b200.h)
+REGION_LINE_DTYPE = np.dtype([("quad", np.float64, (8,)), ("language", np.int32), ("vertical", np.int32),
+                              ("font_size", np.float64)], align=True)
+REGION_DTYPE = np.dtype([("out_h", np.int32), ("out_w", np.int32), ("rotate", np.int32), ("status", np.int32),
+                         ("offset", np.int64), ("homography", np.float64, (9,)), ("inverse", np.float64, (9,))],
+                        align=True)
+
 EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_get_net_outputs", "ctd_get_mask_u8",
            "ctd_get_detections", "ctd_get_db_components", "ctd_last_forward_ms", "ctd_last_launch_count",
            "ctd_debug_read_buffer", "ctd_debug_write_buffer", "ctd_connected_components", "ctd_nms",
@@ -61,7 +68,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_get_text_lines", "ctd_seg_represent", "ctd_refine_mask", "ctd_submit", "ctd_collect",
            "ctd_results_bytes", "ctd_join", "ctd_forward_resized", "ctd_get_mask_u8_resized",
            "ctd_resize_linear_u8", "ctd_debug_run_ops", "ctd_get_nms_status", "ctd_group_output",
-           "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena"]
+           "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena",
+           "ctd_region_plan", "ctd_transform_regions"]
 
 _lib = None
 
@@ -119,6 +127,8 @@ def load_library():
     lib.ctd_results_layout.argtypes = [vp, C.POINTER(CtdResultsLayout)]
     lib.ctd_submit_full.argtypes = [vp, i32, vp, i32, i32, i32, i32, i32, vp]
     lib.ctd_device_arena.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(vp)]
+    lib.ctd_region_plan.argtypes = [vp, i32, i32, i32, i32, vp, C.POINTER(C.c_size_t)]
+    lib.ctd_transform_regions.argtypes = [vp, vp, i32, i32, i32, vp, i32, vp, C.c_size_t]
     for name in EXPORTS[3:]:
         getattr(lib, name).restype = C.c_int
     lib.ctd_expand_textwindow.restype = None
@@ -128,6 +138,18 @@ def load_library():
 
 def _ptr(a):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def region_plan(lines, im_w, im_h, textheight):
+    """`ctd_region_plan` (host C++, no GPU): lines = REGION_LINE_DTYPE records -> (REGION_DTYPE records, packed bytes)"""
+    lib = load_library()
+    lines = np.ascontiguousarray(lines, REGION_LINE_DTYPE)
+    plan = np.zeros((len(lines),), REGION_DTYPE)
+    total = C.c_size_t()
+    rc = lib.ctd_region_plan(_ptr(lines), len(lines), int(im_w), int(im_h), int(textheight), _ptr(plan), C.byref(total))
+    if rc != 0:
+        raise CtdError("ctd_region_plan failed (%d): page %dx%d, textheight %d" % (rc, im_w, im_h, textheight))
+    return plan, int(total.value)
 
 
 class Engine:
@@ -396,6 +418,26 @@ class Engine:
             pages = np.ascontiguousarray(pages, dtype=np.uint8)
         self._ck(self.lib.ctd_debug_run_ops(self.h, _ptr(pages), n, h, w, first, last))
         self.shape = (n, h, w)
+
+    # ---- text-line crops (ctd_transform_regions) -------------------------------------------
+    def transform_regions(self, page, plan, out=None, page_shape=None):
+        """warp every plan entry with status 0 out of `page` in one launch -> packed u8 bytes (plan layout).
+        page: u8 [ih][iw][3] host array, or a device pointer (int) with page_shape = (ih, iw).  out: optional host
+        u8 buffer of at least the plan's total bytes."""
+        plan = np.ascontiguousarray(plan, REGION_DTYPE)
+        total = int(max((int(r["offset"]) + int(r["out_h"]) * int(r["out_w"]) * 3 for r in plan), default=0))
+        if out is None:
+            out = np.empty((total,), np.uint8)
+        if page_shape is None:
+            page = np.ascontiguousarray(page, np.uint8)
+            ih, iw, c = page.shape
+            assert c == 3
+            ptr, on_dev = _ptr(page), 0
+        else:
+            (ih, iw), ptr, on_dev = page_shape, C.c_void_p(int(page)), 1
+        self._ck(self.lib.ctd_transform_regions(self.h, ptr, int(ih), int(iw), on_dev, _ptr(plan), len(plan), _ptr(out),
+                                                out.nbytes))
+        return out
 
     # ---- stand-alone array kernels --------------------------------------------------------
     def connected_components(self, img, stats_cap=0):

@@ -7,12 +7,15 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden"
 mkdir -p _obj
 pids=()
-for f in engine pipeline conv_tc simt postproc segrep refine refine_mk resize group; do
+for f in engine pipeline conv_tc simt postproc segrep refine refine_mk resize group region_plan region; do
   [ -f $f.cu ] || [ -f $f.cpp ] || continue
   src=$f.cu; [ -f $src ] || src=$f.cpp
+  extra=""
+  # the crop planner restates OpenCV's double arithmetic operation for operation: no contraction into FMAs
+  [ $f = region_plan ] && extra="-Xcompiler -ffp-contract=off"
   if [ ! -f _obj/$f.o ] || [ $src -nt _obj/$f.o ] || [ -n "$(find . -maxdepth 1 \( -name '*.h' -o -name '*.cuh' \) -newer _obj/$f.o)" ] \
      || [ ../../include/ctd_b200.h -nt _obj/$f.o ]; then
-    $NVCC $FLAGS "$@" -c $src -o _obj/$f.o &
+    $NVCC $FLAGS $extra "$@" -c $src -o _obj/$f.o &
     pids+=($!)
   fi
 done

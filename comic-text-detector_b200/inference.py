@@ -16,7 +16,7 @@ import numpy as np
 
 from . import compiler
 from .binding import Engine, PREC_FP16_TC, PREC_FP32_SIMT
-from .textblock import TextBlock, blocks_from_records, group_output, overlap_area  # noqa: F401
+from .textblock import TextBlock, blocks_from_records, group_output, overlap_area, transformed_regions  # noqa: F401
 
 REFINEMASK_INPAINT = 0
 REFINEMASK_ANNOTATION = 1
@@ -92,3 +92,11 @@ class TextDetector:
         mask, mask_refined, rec, lines, dist = self.net.detect_page(img, self.input_size[0], self.input_size[1], refine_mode,
                                                                     keep_undetected_mask)
         return mask, mask_refined, blocks_from_records(rec, lines, dist)
+
+    def get_transformed_regions(self, img, blk_list, textheight):
+        """The OCR crops of every line of every block: per block, a list of u8 arrays in line order, each equal byte
+        for byte to the reference's `blk.get_transformed_region(img, idx, textheight)` (utils/textblock.py:162-194).
+        One host plan (csrc/region_plan.cpp), one page upload, one GPU launch and one copy back for the whole page,
+        on this detector's engine.  img: u8 BGR [h][w][3], the page `blk_list` was detected on.  Raises CtdError,
+        naming the block and the line, before any GPU work if the reference would raise on a line."""
+        return transformed_regions(self.net, img, blk_list, textheight)

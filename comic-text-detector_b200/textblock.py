@@ -1,13 +1,19 @@
-"""`TextBlock` records and the line -> block grouping of the drop-in detector.
+"""`TextBlock` records, the line -> block grouping of the drop-in detector and the text-line crops for OCR.
 
 The grouping itself (`group_output`, reference utils/textblock.py:421-508 and its callees) is native code:
 `ctd_group_output` in libctd_b200.so (csrc/group.cpp, declared in include/ctd_b200.h).  This module only converts
 between the reference's python types -- the `(boxes, cls, conf)` tuple of `postprocess_yolo`, the int32 line quads,
 the `TextBlock` objects callers of `TextDetector.__call__` receive (field names of utils/textblock.py:12-85) -- and the
 flat C arrays of that call.
+
+The crops (`get_transformed_region`, utils/textblock.py:162-194) are native too: `ctd_region_plan` (host C++,
+csrc/region_plan.cpp) computes every line's output shape and cv2-identical homography, `ctd_transform_regions`
+(csrc/region.cu) warps all of them out of the page in one GPU launch.
 """
 import copy
 import ctypes as C
+import numbers
+import threading
 
 import numpy as np
 
@@ -18,8 +24,9 @@ LANGCLS2IDX = {"eng": 0, "ja": 1, "unknown": 2}
 
 
 class TextBlock(object):
-    """Result record with the reference's field names (textblock.py:12-85); the UI/OCR helpers of the
-    reference class (min_rect, get_transformed_region, colours ...) are not part of the detection path."""
+    """Result record with the reference's field names (textblock.py:12-85).  Of the reference class's helpers it has
+    `get_transformed_region`, the per-line OCR crop (on the GPU); the UI helpers (min_rect, alignment, colours ...)
+    are not part of it."""
 
     def __init__(self, xyxy, lines=None, language="unknown", vertical=False, font_size=-1, distance=None, angle=0,
                  vec=None, norm=-1, merged=False, weight=-1, text=None, translation="", fg_r=0, fg_g=0, fg_b=0,
@@ -64,6 +71,17 @@ class TextBlock(object):
 
     def to_dict(self):
         return copy.deepcopy(vars(self))
+
+    def get_transformed_region(self, img, idx, textheight) -> np.ndarray:
+        """Line `idx` cut out of `img` (u8 BGR [h][w][3]) straightened to `textheight` px, equal byte for byte to the
+        reference's method (utils/textblock.py:162-194): horizontal lines come out textheight px high, vertical ones
+        textheight px wide and rotated 90 degrees counter-clockwise.  Runs on a small kernels-only engine that is
+        created on cuda:0 at the first call and kept for the process; every call uploads the whole page, so for
+        several lines use `TextDetector.get_transformed_regions`, which crops all lines of a page in one launch.
+        Raises CtdError where the reference raises (a line whose crop would be 1 px wide or high, a degenerate quad)."""
+        eng, lock = _region_engine()
+        with lock:
+            return transformed_regions(eng, img, [self], textheight, line_index=idx)[0][0]
 
 
 def blocks_from_records(blocks, lines, dist):
@@ -140,6 +158,80 @@ def group_output(blks, lines, im_w, im_h, mask=None, sort_blklist=True):
     if rc != 0:
         raise binding.CtdError("ctd_group_output failed (%d)" % rc)
     return blocks_from_records(rec[:n.value], lout, dout)
+
+
+_REGION_ENGINE = None
+_REGION_LOCK = threading.Lock()
+
+
+def _region_engine():
+    """the process-wide kernels-only engine behind TextBlock.get_transformed_region (no network ops, a 64x64
+    workspace), created on device 0 at first use; its handle is not thread-safe, so calls hold the returned lock"""
+    global _REGION_ENGINE
+    with _REGION_LOCK:
+        if _REGION_ENGINE is None:
+            from . import compiler
+            P = compiler.Program()
+            P.nc = 2
+            P.newbuf(8, 1)
+            _REGION_ENGINE = binding.Engine(P, device=0, max_batch=1, max_h=64, max_w=64, skip_postproc=True)
+    return _REGION_ENGINE, _REGION_LOCK
+
+
+def _check_textheight(textheight):
+    if isinstance(textheight, numbers.Integral) and not isinstance(textheight, bool):
+        return int(textheight)
+    if isinstance(textheight, numbers.Real) and float(textheight).is_integer():
+        return int(textheight)
+    raise ValueError("textheight must be an integer number of pixels, got %r" % (textheight,))
+
+
+def region_lines(blk_list, line_index=None):
+    """REGION_LINE_DTYPE records for every line of every block (or line `line_index` of each), and (block, line) of
+    each record"""
+    keys = []
+    for b, blk in enumerate(blk_list):
+        for i in (range(len(blk.lines)) if line_index is None else [line_index]):
+            keys.append((b, i))
+    rec = np.zeros((len(keys),), binding.REGION_LINE_DTYPE)
+    for r, (b, i) in zip(rec, keys):
+        blk = blk_list[b]
+        r["quad"] = np.asarray(blk.lines[i], np.float64).reshape(8)
+        r["language"] = LANGCLS2IDX["eng"] if blk.language == "eng" else (
+            LANGCLS2IDX["unknown"] if blk.language == "unknown" else LANGCLS2IDX["ja"])
+        r["vertical"] = 1 if blk.vertical else 0
+        r["font_size"] = float(blk.font_size)
+    return rec, keys
+
+
+def transformed_regions(engine, img, blk_list, textheight, line_index=None, page_shape=None):
+    """Crops of every line of every block (or of line `line_index` of each block) as per-block lists of u8 arrays:
+    one plan, one page upload, one launch, one copy back.  img: u8 [h][w][3] host array, or a device pointer (int)
+    with page_shape = (h, w).  Raises CtdError, naming the block and the line, where the reference would raise; that
+    check runs before any GPU work."""
+    textheight = _check_textheight(textheight)
+    if page_shape is None:
+        img = np.ascontiguousarray(img)
+        if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
+            raise ValueError("the page must be uint8 [h][w][3], got %s %s" % (img.dtype, img.shape))
+        im_h, im_w = img.shape[:2]
+    else:
+        im_h, im_w = page_shape
+    rec, keys = region_lines(blk_list, line_index)
+    plan, total = binding.region_plan(rec, im_w, im_h, textheight)
+    for (b, i), st in zip(keys, plan["status"].tolist()):
+        if st != 0:
+            why = "the reference raises on it (crop side of 1 px or a degenerate quad)" if st == 1 else \
+                  "its crop has a side of %d px or more" % 32767
+            raise binding.CtdError("block %d, line %d: no crop at textheight %d: %s" % (b, i, textheight, why))
+    out = np.empty((total,), np.uint8)
+    if len(plan):
+        engine.transform_regions(img, plan, out=out, page_shape=page_shape)
+    res = [[] for _ in blk_list]
+    for (b, _i), r in zip(keys, plan):
+        o, hh, ww = int(r["offset"]), int(r["out_h"]), int(r["out_w"])
+        res[b].append(out[o:o + hh * ww * 3].reshape(hh, ww, 3))
+    return res
 
 
 def overlap_area(a, b):

@@ -361,6 +361,44 @@ CTD_API int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages, i
 /* Device copy of slot `slot`'s complete results (same layout) and the stream its last writes were enqueued on.   */
 CTD_API int ctd_device_arena(ctd_handle* h, int32_t slot, void** base, void** post_stream);
 
+/* ---- text-line crops for OCR (SURVEY 8f row f4) ----------------------------------------------------------------
+ * `TextBlock.get_transformed_region(img, idx, textheight)` (utils/textblock.py:162-194): line `idx` of a block, pushed
+ * out by font_size / 3 for 'eng' (and horizontal 'unknown') blocks and clipped to [0, im_w] x [0, im_h], cut out of the
+ * page with `cv2.findHomography(src, dst, RANSAC, 5.0)` + `cv2.warpPerspective(img, M, (w, h))` (INTER_LINEAR,
+ * BORDER_CONSTANT 0) at a fixed text height (h = textheight for horizontal lines, w = textheight for vertical ones,
+ * the other side from the line's aspect ratio), vertical crops rotated 90 degrees counter-clockwise.
+ *
+ * ctd_region_plan (host C++, no handle, thread-safe, needs no GPU) does the geometry: for every requested line the
+ * output shape, the homography bit-identical to cv2.findHomography's (OpenCV's normalised 4-point DLT with its Jacobi
+ * eigen solver) and the inverse cv2.warpPerspective samples with (cv2.invert, DECOMP_LU), plus the crop's offset in one
+ * packed u8 buffer (*total_bytes = its size).  A line on which the reference raises (findHomography returns None when
+ * w == 1 or h == 1; a zero or non-finite aspect ratio) gets status 1 and no bytes; a crop with a side of 32767 px or more
+ * gets status 2 (OpenCV's 16-bit remap coordinates do not reach it).  When the rounded size is 0 the crop has the page's
+ * shape, as cv2 gives it for an empty dsize.  Returns CTD_E_INVALID for textheight < 2 (unused by any caller: the
+ * reference then either raises or returns that page-sized crop) and for a page side < 1 or >= 32767.               */
+typedef struct ctd_region_line {   /* one requested line: TextBlock.lines[idx] + the block fields the method reads */
+  double quad[8];                  /* x1 y1 .. x4 y4 (TL, TR, BR, BL)                                                 */
+  int32_t language, vertical;      /* LANG_LIST index, TextBlock.vertical                                             */
+  double font_size;                /* TextBlock.font_size (an int, or a float after a merge)                          */
+} ctd_region_line;
+typedef struct ctd_region {
+  int32_t out_h, out_w;            /* shape of the returned array (after the rotation, after the dsize-empty rule)    */
+  int32_t rotate;                  /* 1: vertical direction                                                           */
+  int32_t status;                  /* 0 ok, 1 the reference raises on this line, 2 too large (see above)              */
+  int64_t offset;                  /* byte offset of this crop in the packed output (out_h * out_w * 3 bytes, HWC)    */
+  double homography[9];            /* as cv2.findHomography returns it                                                */
+  double inverse[9];               /* as cv2.invert(M, DECOMP_LU) returns it; what the kernel reads                   */
+} ctd_region;
+CTD_API int ctd_region_plan(const ctd_region_line* lines, int32_t n, int32_t im_w, int32_t im_h, int32_t textheight,
+                            ctd_region* out, size_t* total_bytes);
+/* One launch warps every planned crop (status 0) of the page into `pixels_out` (HOST, the plan's packed layout; bytes
+ * of regions with status != 0 are not written).  page: u8 BGR [ih][iw][3], a HOST pointer, or with page_on_device != 0
+ * a DEVICE pointer on the handle's GPU.  Blocking.  Bit-exact with cv2.warpPerspective(img, M, (w, h)) + cv2.rotate
+ * for the plan's `inverse` (csrc/region.cu).  CTD_E_CAPACITY if pixels_bytes is smaller than the plan's total,
+ * CTD_E_SHAPE for a bad page size, CTD_E_INVALID for a malformed plan entry.                                       */
+CTD_API int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t page_on_device,
+                                  const ctd_region* plan, int32_t n, uint8_t* pixels_out, size_t pixels_bytes);
+
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
  * [rows][5+nc]); output as ctd_get_detections for one page.                                */
 CTD_API int ctd_nms(ctd_handle* h, const float* pred, int32_t rows, float conf_thresh, float iou_thresh, float* det,
