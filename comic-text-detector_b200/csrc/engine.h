@@ -35,13 +35,10 @@ struct PipeJob {
   const uint8_t* pages_dev = nullptr;   // caller's device pages (pages_on_device) or null: the slot's staging copy
 };
 
-// refine windows of one launch (all pages of a batch): RefineWin records + small / large index lists
-struct HostWin { int x1, y1, x2, y2; long long off; int page, pad; };   // = RefineWin (refine.cu / refine_mk.cu)
-struct HostChunk { int win, y0, rows, pad; };                            // = Chunk (refine_mk.cu)
+// refine windows of one launch (all pages of a batch) and the chunks they are cut into
 struct RefineJob {
-  std::vector<HostWin> wins;
-  std::vector<int> idx_small, idx_large;     // cooperative kernels (refine.cu)
-  std::vector<HostChunk> chunks;             // phase-synchronous kernels (refine_mk.cu)
+  std::vector<ctd::RefineWin> wins;
+  std::vector<ctd::RefineChunk> chunks;
   size_t total_px = 0;
   void add(int x1, int y1, int x2, int y2, int page, int iw, int ih);   // python slice semantics; empty windows dropped
   size_t table_bytes() const;

@@ -181,27 +181,29 @@ cudaError_t segrep_launch(const uint8_t* bitmap, const float* pred, size_t pred_
 constexpr int kSegrepLaunches = 15;   // kernels and memsets segrep_launch enqueues
 cudaError_t binarize_launch(const float* pred, size_t count, float thresh, uint8_t* bitmap, cudaStream_t s);
 
-// refine_mask (refine.cu): one CTA per block window.  d_wins: n_wins x {x1,y1,x2,y2,(int64)pixel offset}
 // cv2.resize INTER_LINEAR, uint8, 1 or 3 channels, bit-exact (resize.cu).  src rows are `src_pitch` bytes apart; the
 // dh x dw result is written at the top-left of a canvas_h x canvas_w canvas whose remaining pixels are zeroed.
 cudaError_t resize_linear_u8_launch(const uint8_t* src, int sh, int sw, size_t src_pitch, int channels, uint8_t* dst,
                                     int dh, int dw, int canvas_h, int canvas_w, cudaStream_t s);
+
+// refine_mask (refine_mk.cu): one kernel per phase over the window pixels of all pages of a batch, one CTA per chunk.
+struct RefineWin {
+  int x1, y1, x2, y2;     // window (python slice semantics: rows y1..y2-1, cols x1..x2-1)
+  long long off;          // pixel offset of this window's planes inside each scratch plane (a multiple of 4)
+  int page;               // page of the batch the window belongs to
+};
+// Pixels [i0, i0 + rows * cols) of the window planes, i0 = y0 * rw + x0, cols = min(rw - x0, kRefineChunkPx).  A
+// window of width rw <= kRefineChunkPx is cut into chunks of whole rows (x0 = 0, cols = rw); a wider window into row
+// segments (rows = 1, x0 a multiple of kRefineChunkPx).
+struct RefineChunk { int win, y0, x0, rows; };
+constexpr int kRefineChunkPx = 8192;
+// scratch planes for `total_px` window pixels (the sum of the window areas, each rounded up to 4)
 size_t refine_scratch_bytes(size_t total_px);
-// d_wins: RefineWin records {x1,y1,x2,y2,(int64) plane offset,(int) page,(int) pad} = 32 bytes; idx_small / idx_large:
-// device index lists into d_wins (windows above refine_large_px() pixels are processed by a CTA cluster each).
-cudaError_t refine_launch(const uint8_t* d_img, const uint8_t* d_mask, int H, int W, const void* d_wins, const int* d_idx_small,
-                          int n_small, const int* d_idx_large, int n_large, size_t total_px, void* scratch, int refine_mode,
-                          uint8_t* d_out, cudaStream_t s);
-int refine_large_px();
-size_t refine_win_bytes();
-// phase-synchronous form (refine_mk.cu): one kernel per phase over all window pixels of the batch, windows cut into
-// chunks of whole rows {win, y0, rows, pad} by the host; d_state: refine_mk_state_bytes(n_wins) bytes of per-window state
+// d_state: refine_mk_state_bytes(n_wins) bytes of per-window state
 size_t refine_mk_state_bytes(int n_wins);
-size_t refine_mk_chunk_bytes();
-int refine_mk_chunk_px();
 // the first n_multi_chunks records of d_chunks are the chunks of windows that span more than one chunk
-cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, int H, int W, const void* d_wins, int n_wins,
-                             const void* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
+cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, int H, int W, const RefineWin* d_wins, int n_wins,
+                             const RefineChunk* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
                              void* scratch, int refine_mode, uint8_t* d_out, cudaStream_t s);
 
 }  // namespace ctd

@@ -3,7 +3,7 @@
 //
 //   phase A (device)  forward + NMS + mask u8 + DB threshold + CCL + line boxes           (engine.cu)
 //   phase B (host)    postprocess_yolo casts, box_thresh filter, `group_output` (group.cpp), expand_textwindow
-//   phase C (device)  `refine_mask` on the resident page + mask (refine.cu), optionally refine_undetected_mask
+//   phase C (device)  `refine_mask` on the resident page + mask (refine_mk.cu), optionally refine_undetected_mask
 //
 // ctd_submit_full / ctd_collect run batches of net-sized pages through A -> B -> C with two batches in flight per
 // engine: the caller's thread enqueues phase A, a per-engine worker thread waits for A's small results, runs phase B
@@ -46,20 +46,19 @@ void RefineJob::add(int x1, int y1, int x2, int y2, int page, int iw, int ih) {
   norm_slice(y1, y2, ih);
   const size_t a = (x2 > x1 && y2 > y1) ? size_t(x2 - x1) * (y2 - y1) : 0;
   if (a == 0) return;                                    // empty slice: the reference's loop body is a no-op
-  HostWin w{x1, y1, x2, y2, (long long)total_px, page, 0};
   const int wi = int(wins.size());
-  (a > size_t(refine_large_px()) ? idx_large : idx_small).push_back(wi);
   const int rw = x2 - x1, rh = y2 - y1;
-  int rows_per = std::max(1, refine_mk_chunk_px() / rw);
+  // whole rows per chunk, or one row segment of <= kRefineChunkPx pixels per chunk when a row is longer
+  int rows_per = std::max(1, kRefineChunkPx / rw);
   if (rows_per >= 8) rows_per &= ~3;   // chunk starts on multiples of 4 rows -> 4-byte aligned in the window planes
-  for (int y0 = 0; y0 < rh; y0 += rows_per)   // pad bit 0: aligned start (the labelling kernel then loads 4 pixels per thread)
-    chunks.push_back(HostChunk{wi, y0, std::min(rows_per, rh - y0), ((long long)y0 * rw) % 4 == 0 ? 1 : 0});
-  wins.push_back(w);
+  for (int y0 = 0; y0 < rh; y0 += rows_per)
+    for (int x0 = 0; x0 < rw; x0 += kRefineChunkPx) chunks.push_back(RefineChunk{wi, y0, x0, std::min(rows_per, rh - y0)});
+  wins.push_back(RefineWin{x1, y1, x2, y2, (long long)total_px, page});
   total_px = (total_px + a + 3) / 4 * 4;
 }
 size_t RefineJob::table_bytes() const {
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
-  return al(wins.size() * sizeof(HostWin)) + al((idx_small.size() + idx_large.size()) * 4) + al(chunks.size() * sizeof(HostChunk));
+  return al(wins.size() * sizeof(RefineWin)) + al(chunks.size() * sizeof(RefineChunk));
 }
 
 // uploads the window tables of `job` into the (grown on demand) refine scratch and launches the refine kernels:
@@ -68,13 +67,6 @@ size_t RefineJob::table_bytes() const {
 int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int ih, int iw,
                   int refine_mode, uint8_t* d_out, cudaStream_t st, char* pinned) {
   if (job.wins.empty()) return CTD_OK;
-  static_assert(sizeof(HostWin) == 32 && sizeof(HostChunk) == 16, "RefineWin / Chunk layout");
-  if (refine_win_bytes() != sizeof(HostWin) || refine_mk_chunk_bytes() != sizeof(HostChunk))
-    return ctd_fail(h, CTD_E_INVALID, "RefineWin / Chunk layout mismatch");
-  const char* rf_env = getenv("CTD_REFINE");                   // CTD_REFINE=coop: the cooperative kernels of refine.cu
-  bool coop = rf_env && rf_env[0] == 'c';
-  for (const HostWin& w : job.wins)                            // a window row must fit one chunk of the phase kernels
-    if (w.x2 - w.x1 > refine_mk_chunk_px()) coop = true;
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t tb = job.table_bytes();   // a multiple of 256
   const size_t sb = refine_mk_state_bytes(int(job.wins.size()));
@@ -88,20 +80,16 @@ int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, con
     h->refine_scratch_cap = need + need / 2;
   }
   char* base = static_cast<char*>(h->d_refine_scratch);
-  const size_t wb = al(job.wins.size() * sizeof(HostWin));
-  const size_t ib = al((job.idx_small.size() + job.idx_large.size()) * 4);
+  const size_t wb = al(job.wins.size() * sizeof(RefineWin));
   std::vector<char> local;
   char* stage = pinned;
   if (!stage) { local.resize(tb); stage = local.data(); }
-  memcpy(stage, job.wins.data(), job.wins.size() * sizeof(HostWin));
-  int* hidx = reinterpret_cast<int*>(stage + wb);
-  if (!job.idx_small.empty()) memcpy(hidx, job.idx_small.data(), job.idx_small.size() * 4);
-  if (!job.idx_large.empty()) memcpy(hidx + job.idx_small.size(), job.idx_large.data(), job.idx_large.size() * 4);
+  memcpy(stage, job.wins.data(), job.wins.size() * sizeof(RefineWin));
   // chunk table: the chunks of windows that span SEVERAL chunks first -- only those have chunk borders to unite and
   // chunk-local roots to re-point (k_union_border / k_flat1 run on that prefix); the kernels are order-agnostic
   int n_multi = 0;
   {
-    HostChunk* hc = reinterpret_cast<HostChunk*>(stage + wb + ib);
+    RefineChunk* hc = reinterpret_cast<RefineChunk*>(stage + wb);
     const size_t nc = job.chunks.size();
     size_t tail = nc;
     for (size_t i = 0; i < nc;) {
@@ -117,13 +105,9 @@ int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, con
   }
   CK(cudaMemcpyAsync(base, stage, tb, cudaMemcpyHostToDevice, st));
   if (!pinned) CK(cudaStreamSynchronize(st));   // pageable staging dies with this frame
-  const int* d_idx = reinterpret_cast<const int*>(base + wb);
-  if (coop)
-    CK(refine_launch(d_img, d_mask, ih, iw, base, d_idx, int(job.idx_small.size()), d_idx + job.idx_small.size(),
-                     int(job.idx_large.size()), job.total_px, base + tb + sb, refine_mode, d_out, st));
-  else
-    CK(refine_mk_launch(d_img, d_mask, ih, iw, base, int(job.wins.size()), base + wb + ib, int(job.chunks.size()), n_multi,
-                        base + tb, job.total_px, base + tb + sb, refine_mode, d_out, st));
+  CK(refine_mk_launch(d_img, d_mask, ih, iw, reinterpret_cast<const RefineWin*>(base), int(job.wins.size()),
+                      reinterpret_cast<const RefineChunk*>(base + wb), int(job.chunks.size()), n_multi, base + tb,
+                      job.total_px, base + tb + sb, refine_mode, d_out, st));
   return CTD_OK;
 }
 
@@ -316,9 +300,9 @@ static int ensure_full_pipeline(ctd_handle* h) {
   int lo = 0, hi = 0;
   CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
   CK(cudaStreamCreateWithPriority(&h->post, cudaStreamNonBlocking, hi));
-  // window tables: <= CTD_MAX_BLOCKS windows per page, 32-byte record + 4-byte index
-  // <= CTD_MAX_BLOCKS windows per page (32 + 4 bytes each) and <= area / chunk + rows chunks per window (16 bytes)
-  h->pipe_pinned_cap = size_t(h->cfg.max_batch) * (size_t(CTD_MAX_BLOCKS) * 36 + size_t(CTD_MAX_BLOCKS) * 16 * 8) + (size_t(8) << 20);
+  // window tables: <= CTD_MAX_BLOCKS windows per page (32 bytes each) and <= area / chunk + rows chunks per window
+  // (16 bytes each)
+  h->pipe_pinned_cap = size_t(h->cfg.max_batch) * (size_t(CTD_MAX_BLOCKS) * 32 + size_t(CTD_MAX_BLOCKS) * 16 * 8) + (size_t(8) << 20);
   for (int i = 0; i < 2; ++i) {
     CK(cudaHostAlloc(reinterpret_cast<void**>(&h->pipe_pinned[i]), h->pipe_pinned_cap, cudaHostAllocDefault));
     CK(cudaEventCreateWithFlags(&h->ev_post_done[i], cudaEventDisableTiming));

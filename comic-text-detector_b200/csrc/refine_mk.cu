@@ -1,14 +1,15 @@
 // refine_mask on the GPU, phase-synchronous form (reference utils/textmask.py:159-169 and callees 16-132).
 //
-// csrc/refine.cu runs ONE cooperative kernel with a CTA (or an 8-CTA cluster) per block window and barriers between
-// the phases.  Measured on the synthetic 1024^2 pages: every phase is a latency-bound sweep with one pixel per thread
-// iteration, a 1 Mpx window keeps 8 SMs busy for 15 ms while the other 140 idle, and a batch of 16 pages (~50 Mpx of
-// overlapping windows) cost 29 ms -- 4.5x the network.  Here every phase is its own kernel over ALL window pixels of
-// the batch: the windows are cut into chunks of whole rows (<= kChunkPx pixels, table built by the host, which knows
-// the window sizes), one CTA per chunk, so a giant window is spread over the whole GPU and the kernel boundary is the
-// barrier.  Per-window reductions (histograms, xor sums, the two largest hole areas) go through a small per-window
-// state record in global memory; per-window scalar decisions are one-CTA-per-window kernels.  Results are bit-identical to
-// refine.cu and to the oracle (tests/test_gpu_refine.py runs all three).
+// Why one kernel per phase: a single cooperative kernel with a CTA (or an 8-CTA cluster) per block window and barriers
+// between the phases, measured on the synthetic 1024^2 pages, ran every phase as a latency-bound sweep with one pixel
+// per thread iteration: a 1 Mpx window kept 8 SMs busy for 15 ms while the other 140 idled, and a batch of 16 pages
+// (~50 Mpx of overlapping windows) cost 29 ms -- 4.5x the network.  Here every phase is its own kernel over ALL window
+// pixels of the batch: the windows are cut into chunks (RefineChunk, kernels.h: whole rows of <= kChunkPx pixels, or
+// row segments of <= kChunkPx pixels when a window row is longer; table built by the host, which knows the window
+// sizes), one CTA per chunk, so a giant window is spread over the whole GPU and the kernel boundary is the barrier.
+// Per-window reductions (histograms, xor sums, the two largest hole areas) go through a small per-window state record
+// in global memory; per-window scalar decisions are one-CTA-per-window kernels.  Results are bit-identical to the
+// oracle (tests/test_gpu_refine.py).
 //
 // The sweeps are instruction-issue bound, not memory bound, so the binary planes
 // are handled as BIT masks wherever a neighbourhood is involved: warp ballots pack 32 pixels per shared-memory word and one
@@ -25,13 +26,7 @@ namespace ctd {
 namespace {
 
 constexpr int kThreads = 256;
-
-struct RefineWin {
-  int x1, y1, x2, y2;
-  long long off;
-  int page, pad;
-};
-struct Chunk { int win, y0, rows, pad; };
+constexpr int kChunkPx = kRefineChunkPx;
 
 struct WinState {
   int hist[4][256];               // [0] grey of the eroded-mask pixels, [1..3] B, G, R of the whole window
@@ -47,34 +42,38 @@ struct Ctx {
   const uint8_t* mask_all;
   uint32_t* out_all;
   const RefineWin* wins;
-  const Chunk* chunks;
+  const RefineChunk* chunks;
   WinState* st;
   int H, W, mode;
   // planes (window-pixel indexed)
   int* L;
   int* acc;
-  uint8_t *grey, *cand, *predm, *merged, *tmp;   // cand: unused here (kept: the scratch layout is shared with refine.cu)
+  uint8_t *grey, *predm, *merged, *tmp;
 };
 
+// A chunk's pixels are contiguous in the window planes: chunk pixel k is window pixel i0 + k, at window row
+// y0 + k / cols and column x0 + k % cols.  A chunk is one row (rows == 1) or whole rows (x0 == 0, cols == rw).
 struct View {
   RefineWin win;
-  int w, rw, rh, y0, rows, i0, cnt, aligned;   // aligned: the chunk starts on a 4-byte boundary of the window planes
+  int w, rw, rh, y0, x0, rows, cols, i0, cnt, aligned;   // aligned: the chunk starts on a 4-byte boundary of the planes
   const uint8_t* img;
   const uint8_t* mask;
 };
 
 __device__ __forceinline__ View view_of(const Ctx& c, int chunk) {
   View v;
-  const Chunk ch = c.chunks[chunk];
+  const RefineChunk ch = c.chunks[chunk];
   v.w = ch.win;
   v.win = c.wins[ch.win];
   v.rw = v.win.x2 - v.win.x1;
   v.rh = v.win.y2 - v.win.y1;
   v.y0 = ch.y0;
+  v.x0 = ch.x0;
   v.rows = ch.rows;
-  v.i0 = ch.y0 * v.rw;
-  v.cnt = ch.rows * v.rw;
-  v.aligned = ch.pad & 1;
+  v.cols = min(v.rw - ch.x0, kChunkPx);
+  v.i0 = ch.y0 * v.rw + ch.x0;
+  v.cnt = ch.rows * v.cols;
+  v.aligned = (v.i0 & 3) == 0;   // the window planes start on 4-byte boundaries
   v.img = c.img_all + size_t(v.win.page) * c.H * c.W * 3;
   v.mask = c.mask_all + size_t(v.win.page) * c.H * c.W;
   return v;
@@ -147,22 +146,48 @@ __device__ __forceinline__ void divmod(int i, const DivW& dv, int& q, int& r) {
 
 // ---- phase 0: grey, pred mask (cross erosion > 60), merged = 0, histograms ------------------------------------------
 constexpr int kU = 4;   // pixels per thread and outer iteration: the loads of all kU pixels are issued before the first use
-constexpr int kChunkPxFwd = 8192;                       // = kChunkPx (defined with the labelling kernels below)
-constexpr int kExtWords = (3 * kChunkPxFwd) / 32 + 4;   // chunk (<= kChunkPx) + one halo row above and below
+// Halo rectangle of a chunk: its rows plus one row above and below, its columns plus one column left and right, clipped
+// to the window.  Whole rows: <= 3 * kChunkPx pixels (the rows of a chunk, two halo rows of <= kChunkPx); a row
+// segment: 3 rows of <= kChunkPx + 2 pixels.  3 * (kChunkPx + 2) = 24582 bits = 769 words, read up to one word past
+// the last written one: kExtWords holds both.
+constexpr int kExtWords = (3 * kChunkPx) / 32 + 4;
+static_assert(3 * (kChunkPx + 2) / 32 + 2 < kExtWords, "a row segment's halo rectangle fits the shared bit masks");
+struct Halo {
+  int ystart, xs, ew, ext, off;   // first row / column, width (the row stride of the bit masks), pixels, chunk offset
+};
+__device__ __forceinline__ Halo halo_of(const View& v) {
+  Halo h;
+  h.ystart = v.y0 > 0 ? v.y0 - 1 : 0;
+  h.xs = v.x0 > 0 ? v.x0 - 1 : 0;
+  h.ew = min(v.x0 + v.cols + 1, v.rw) - h.xs;
+  h.ext = (min(v.y0 + v.rows + 1, v.rh) - h.ystart) * h.ew;
+  // chunk pixel k sits at rectangle position k + off: a chunk is one row, or its rows are as wide as the rectangle
+  h.off = (v.y0 - h.ystart) * h.ew + v.x0 - h.xs;
+  return h;
+}
 __device__ __forceinline__ unsigned bits_from(const unsigned* M, int pos) {   // 32 bits starting at pixel `pos` (< 0 reads 0)
   if (pos <= -32) return 0u;
   if (pos < 0) return M[0] << (-pos);
   const int w = pos >> 5, sft = pos & 31;
   return __funnelshift_r(M[w], M[w + 1], sft);
 }
+// 32 pixels of a chunk starting at window column x: the bits whose pixel is the first (rs) / last (re) of its window row
+// (bits past the end of a row segment are not pixels of the chunk)
+__device__ __forceinline__ void row_ends(int x, int rw, unsigned& rs, unsigned& re) {
+  rs = 0u;
+  for (int j = x == 0 ? 0 : rw - x; j < 32; j += rw) rs |= 1u << j;
+  int xe = x + 32;                                  // column of the pixel after the 32
+  if (xe >= rw) xe %= rw;
+  re = (rs >> 1) | (xe == 0 ? 0x80000000u : 0u);
+}
 // The two erosions of the mask crop are threshold tests of a minimum: min over the cross > 60 <=> NO pixel of the cross is
-// <= 60.  So the chunk's rows plus one row above and below are packed into two "bad pixel" bit masks (mask <= 60,
-// mask <= 127) by warp ballots -- ONE mask load per pixel instead of nine bounds-checked ones -- and one thread per
-// 32-pixel word ORs the 5 / 9 shifted views (row ends masked; outside the window reads 0 = not bad = BORDER_CONSTANT +inf).
+// <= 60.  So the chunk's halo rectangle is packed into two "bad pixel" bit masks (mask <= 60, mask <= 127) by warp
+// ballots -- ONE mask load per pixel instead of nine bounds-checked ones -- and one thread per 32-pixel word ORs the
+// 5 / 9 shifted views (window row ends masked; outside the window reads 0 = not bad = BORDER_CONSTANT +inf).
 __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
   __shared__ int sh[4][256];
   __shared__ unsigned N60[kExtWords], N127[kExtWords];
-  __shared__ unsigned F60[kChunkPxFwd / 32 + 1], F127[kChunkPxFwd / 32 + 1];
+  __shared__ unsigned F60[kChunkPx / 32 + 1], F127[kChunkPx / 32 + 1];
   const View v = view_of(c, blockIdx.x);
   for (int i = threadIdx.x; i < 1024; i += kThreads) (&sh[0][0])[i] = 0;
   for (int i = threadIdx.x; i < kExtWords; i += kThreads) { N60[i] = 0u; N127[i] = 0u; }
@@ -170,40 +195,34 @@ __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
   uint8_t* grey = c.grey + v.win.off;
   uint8_t* predm = c.predm + v.win.off;
   uint8_t* merged = c.merged + v.win.off;
-  const DivW dv = make_div(v.rw, 3 * kChunkPxFwd + 1);
-  const int ystart = v.y0 > 0 ? v.y0 - 1 : 0;
-  const int yend = min(v.y0 + v.rows + 1, v.rh);
-  const int ext = (yend - ystart) * v.rw;
-  const int off = (v.y0 - ystart) * v.rw;
-  for (int e0 = 0; e0 < ext; e0 += kThreads) {
+  const Halo hl = halo_of(v);
+  const DivW dv = make_div(hl.ew, 3 * (kChunkPx + 2) + 1);
+  for (int e0 = 0; e0 < hl.ext; e0 += kThreads) {
     const int e = e0 + threadIdx.x;
     int mv = 255;
-    if (e < ext) {
+    if (e < hl.ext) {
       int ye, xe;
       divmod(e, dv, ye, xe);
-      mv = v.mask[size_t(v.win.y1 + ystart + ye) * c.W + v.win.x1 + xe];
+      mv = v.mask[size_t(v.win.y1 + hl.ystart + ye) * c.W + v.win.x1 + hl.xs + xe];
     }
     const unsigned b60 = __ballot_sync(0xffffffffu, mv <= 60), b127 = __ballot_sync(0xffffffffu, mv <= 127);
-    if ((threadIdx.x & 31) == 0) { N60[e >> 5] = b60; N127[e >> 5] = b127; }
+    if ((threadIdx.x & 31) == 0 && e < hl.ext) { N60[e >> 5] = b60; N127[e >> 5] = b127; }
   }
   __syncthreads();
+  const int ew = hl.ew;
   for (int w = threadIdx.x; w * 32 < v.cnt; w += kThreads) {
-    const int k0 = w * 32;
-    int yl, x0;
-    divmod(k0, dv, yl, x0);
-    unsigned rs = 0u;
-    for (int j = x0 == 0 ? 0 : v.rw - x0; j < 32; j += v.rw) rs |= 1u << j;
-    int xe = x0 + 32;
-    if (xe >= v.rw) xe %= v.rw;
-    const unsigned re = (rs >> 1) | (xe == 0 ? 0x80000000u : 0u);
-    const int p = k0 + off;
+    const int p = w * 32 + hl.off;
+    int ye, xe;
+    divmod(p, dv, ye, xe);
+    unsigned rs, re;
+    row_ends(hl.xs + xe, v.rw, rs, re);
     // cross (textmask.py:86-89, MORPH_CROSS 3x3) on the <= 60 mask
-    F60[w] = bits_from(N60, p) | bits_from(N60, p - v.rw) | bits_from(N60, p + v.rw) | (bits_from(N60, p - 1) & ~rs) |
+    F60[w] = bits_from(N60, p) | bits_from(N60, p - ew) | bits_from(N60, p + ew) | (bits_from(N60, p - 1) & ~rs) |
              (bits_from(N60, p + 1) & ~re);
     // full 3x3 (textmask.py:60, the eroded mask of get_topk_color) on the <= 127 mask
-    F127[w] = bits_from(N127, p) | bits_from(N127, p - v.rw) | bits_from(N127, p + v.rw) |
-              ((bits_from(N127, p - 1) | bits_from(N127, p - v.rw - 1) | bits_from(N127, p + v.rw - 1)) & ~rs) |
-              ((bits_from(N127, p + 1) | bits_from(N127, p - v.rw + 1) | bits_from(N127, p + v.rw + 1)) & ~re);
+    F127[w] = bits_from(N127, p) | bits_from(N127, p - ew) | bits_from(N127, p + ew) |
+              ((bits_from(N127, p - 1) | bits_from(N127, p - ew - 1) | bits_from(N127, p + ew - 1)) & ~rs) |
+              ((bits_from(N127, p + 1) | bits_from(N127, p - ew + 1) | bits_from(N127, p + ew + 1)) & ~re);
   }
   __syncthreads();
   const DivW dvw = make_div(v.rw, v.rw * v.rh);
@@ -451,13 +470,14 @@ __global__ void k_decide2(Ctx c, int n_wins) {
 }
 
 // ---- labelling of a source plane: candidate `round` (0..3) or, round == 4, the inverse of `merged` (hole filling) -----
-// Level 1, one CTA per chunk (whole rows, <= kChunkPx pixels), everything in SHARED memory: source pixels (coalesced),
-// run starts by warp ballot, seams between warps and the contacts between the rows of the chunk united in a shared
-// union-find, one root per chunk-local component written to L (tmp = 1 marks those roots: they are the chain nodes of
-// the global forest).  Level 2: only the first row of every chunk issues global unions with the row above it.
-// Level 3: compress from the chain nodes, then every pixel takes its (chunk-local) parent's root.
-constexpr int kChunkPx = 8192;
-static_assert(kChunkPx == kChunkPxFwd, "kChunkPxFwd mirrors kChunkPx");
+// Level 1, one CTA per chunk (<= kChunkPx pixels), everything in SHARED memory: source pixels (coalesced), run starts by
+// warp ballot, seams between warps and the contacts between the rows of the chunk united in a shared union-find, one
+// root per chunk-local component written to L (tmp = 1 marks those roots: they are the chain nodes of the global
+// forest).  Level 2: only the first row of every chunk issues global unions with the row above it, and the first pixel
+// of a row segment with the last pixel of the segment to its left.  Level 3: compress from the chain nodes, then every
+// pixel takes its (chunk-local) parent's root.
+// In the chunk-local passes a chunk pixel k is treated as at column k % rw of row k / rw: right for whole rows, and for
+// a row segment (k < cnt <= kChunkPx < rw) one row whose first pixel starts a run and which has no row above.
 constexpr int kLabelThreads = 512;
 
 __device__ __forceinline__ int suf_find(const int* L, int a) {
@@ -557,7 +577,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
               if (k + j < v.cnt) {
                 int yl, x;
                 divmod(k + j, dv, yl, x);
-                s4 |= unsigned(v.img[(size_t(v.win.y1 + v.y0 + yl) * c.W + v.win.x1 + x) * 3 + (kind - 3)]) << (8 * j);
+                s4 |= unsigned(v.img[(size_t(v.win.y1 + v.y0 + yl) * c.W + v.win.x1 + v.x0 + x) * 3 + (kind - 3)]) << (8 * j);
               }
             }
           }
@@ -625,7 +645,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
           else {
             int yl, x;
             divmod(k, dv, yl, x);
-            raw[u] = v.img[(size_t(v.win.y1 + v.y0 + yl) * c.W + v.win.x1 + x) * 3 + (kind - 3)];
+            raw[u] = v.img[(size_t(v.win.y1 + v.y0 + yl) * c.W + v.win.x1 + v.x0 + x) * 3 + (kind - 3)];
           }
         }
       }
@@ -778,18 +798,23 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     }
   }
 }
-// level 2: the first row of every chunk against the last row of the chunk above
+// level 2: the first row of every chunk against the row above it (x-1, x, x+1, possibly in the neighbouring row
+// segments), and the first pixel of a row segment against the last pixel of the segment to its left
 constexpr int kBorderThreads = 256;  // (64-thread CTAs measured 3x slower: a window row is up to thousands of pixels)
 __global__ void __launch_bounds__(kBorderThreads) k_union_border(Ctx c, int round) {
   const View v = view_of(c, blockIdx.x);
   if (round < 4 && round >= c.st[v.w].nproc) return;
-  if (v.y0 == 0) return;
+  if (v.i0 == 0) return;      // the window's first chunk
   int* L = c.L + v.win.off;   // foreground <=> L >= 0 (written for every pixel by k_label_local)
-  for (int x = threadIdx.x; x < v.rw; x += int(blockDim.x)) {
-    const int i = v.i0 + x;
+  if (v.x0 > 0 && threadIdx.x == 0 && __ldcg(L + v.i0) >= 0 && __ldcg(L + v.i0 - 1) >= 0) uf_union(L, v.i0, v.i0 - 1);
+  if (v.y0 == 0) return;
+  for (int k = threadIdx.x; k < v.cols; k += int(blockDim.x)) {
+    const int i = v.i0 + k, x = v.x0 + k;
     if (__ldcg(L + i) < 0) continue;
     const int up = i - v.rw;
     if (__ldcg(L + up) >= 0) {
+      // only the first pixel of each (run x run above) overlap: the pixels left of it are united with it (in the chunk
+      // or across the segment seam) and so are the ones above
       const bool first = x == 0 || __ldcg(L + i - 1) < 0 || __ldcg(L + up - 1) < 0;
       if (first) uf_union(L, i, up);
     } else {
@@ -854,7 +879,7 @@ __global__ void __launch_bounds__(kThreads) k_top_a(Ctx c) {
       if (rf[u] && L[i] == i) m = max(m, area[i]);
     }
   }
-  if (v.y0 == 0 && threadIdx.x == 0) m = max(m, st.area0);
+  if (v.i0 == 0 && threadIdx.x == 0) m = max(m, st.area0);   // once per window: its first chunk
   for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_down_sync(0xffffffffu, m, o));
   if ((threadIdx.x & 31) == 0 && m >= 0) atomicMax(&st.max1, m);
 }
@@ -881,7 +906,7 @@ __global__ void __launch_bounds__(kThreads) k_top_b(Ctx c) {
       if (rf[u] && L[i] == i) push(area[i]);
     }
   }
-  if (v.y0 == 0 && threadIdx.x == 0) push(st.area0);
+  if (v.i0 == 0 && threadIdx.x == 0) push(st.area0);
   for (int o = 16; o > 0; o >>= 1) {
     m2 = max(m2, __shfl_down_sync(0xffffffffu, m2, o));
     c1 += __shfl_down_sync(0xffffffffu, c1, o);
@@ -936,43 +961,39 @@ __global__ void __launch_bounds__(kThreads) k_mapply(Ctx c, int round) {
 
 // ---- dilate 3x3 (inpaint mode): merged -> tmp; the caller swaps the two planes afterwards -----------------------------
 // `merged` is binary (0 / 255): the 3x3 maximum is an OR of nine shifted copies of the foreground BIT mask.  The chunk's
-// rows plus one row above and below (inside the window) are packed into shared-memory words by warp ballots, one thread
-// per 32-pixel word ORs the nine views (row ends masked), and the bytes are written back coalesced: ~25 instructions per
-// pixel instead of ~120 (nine bounds-checked byte loads).
-constexpr int kDilWords = (3 * kChunkPx) / 32 + 4;   // chunk (<= kChunkPx) + two halo rows (a row is <= kChunkPx pixels)
+// halo rectangle (see k_phase0) is packed into shared-memory words by warp ballots, one thread per 32-pixel word ORs
+// the nine views (window row ends masked), and the bytes are written back coalesced: ~25 instructions per pixel instead
+// of ~120 (nine bounds-checked byte loads).
 __global__ void __launch_bounds__(kThreads) k_dilate(Ctx c) {
-  __shared__ unsigned Mw[kDilWords];
+  __shared__ unsigned Mw[kExtWords];
   __shared__ unsigned Ow[kChunkPx / 32 + 1];
   const View v = view_of(c, blockIdx.x);
   const uint8_t* merged = c.merged + v.win.off;
   uint8_t* tmp = c.tmp + v.win.off;
-  for (int i = threadIdx.x; i < kDilWords; i += kThreads) Mw[i] = 0u;
+  for (int i = threadIdx.x; i < kExtWords; i += kThreads) Mw[i] = 0u;
   __syncthreads();
-  const int ystart = v.y0 > 0 ? v.y0 - 1 : 0;
-  const int yend = min(v.y0 + v.rows + 1, v.rh);
-  const int ext = (yend - ystart) * v.rw;            // pixels of the chunk + halo rows
-  const int off = (v.y0 - ystart) * v.rw;            // chunk pixel k sits at extended position k + off
-  const uint8_t* src = merged + size_t(ystart) * v.rw;
-  for (int e0 = 0; e0 < ext; e0 += kThreads) {
+  const Halo hl = halo_of(v);
+  const int ew = hl.ew;
+  // rectangle position e -> window pixel: contiguous for whole rows (gap 0); a row segment's rectangle has <= 3 rows
+  const int gap = v.rw - ew;
+  const uint8_t* src = merged + size_t(hl.ystart) * v.rw + hl.xs;
+  for (int e0 = 0; e0 < hl.ext; e0 += kThreads) {
     const int e = e0 + threadIdx.x;
-    const unsigned m = __ballot_sync(0xffffffffu, e < ext && src[e] != 0);
-    if ((threadIdx.x & 31) == 0) Mw[e >> 5] = m;
+    const int row = gap == 0 ? 0 : (e >= ew) + (e >= 2 * ew);
+    const unsigned m = __ballot_sync(0xffffffffu, e < hl.ext && src[e + row * gap] != 0);
+    if ((threadIdx.x & 31) == 0 && e < hl.ext) Mw[e >> 5] = m;
   }
   __syncthreads();
-  const DivW dv = make_div(v.rw, kChunkPx + 1);
+  const DivW dv = make_div(ew, 3 * (kChunkPx + 2) + 1);
   for (int w = threadIdx.x; w * 32 < v.cnt; w += kThreads) {
-    const int k0 = w * 32;
-    int yl, x0;
-    divmod(k0, dv, yl, x0);
-    unsigned rs = 0u;                                 // bits whose pixel is the first of its row
-    for (int j = x0 == 0 ? 0 : v.rw - x0; j < 32; j += v.rw) rs |= 1u << j;
-    int xe = x0 + 32;
-    if (xe >= v.rw) xe %= v.rw;
-    const unsigned re = (rs >> 1) | (xe == 0 ? 0x80000000u : 0u);   // ... the last of its row
-    const int p = k0 + off;
-    unsigned o = bits_from(Mw, p) | bits_from(Mw, p - v.rw) | bits_from(Mw, p + v.rw);
-    o |= (bits_from(Mw, p - 1) | bits_from(Mw, p - v.rw - 1) | bits_from(Mw, p + v.rw - 1)) & ~rs;
-    o |= (bits_from(Mw, p + 1) | bits_from(Mw, p - v.rw + 1) | bits_from(Mw, p + v.rw + 1)) & ~re;
+    const int p = w * 32 + hl.off;
+    int ye, xe;
+    divmod(p, dv, ye, xe);
+    unsigned rs, re;
+    row_ends(hl.xs + xe, v.rw, rs, re);
+    unsigned o = bits_from(Mw, p) | bits_from(Mw, p - ew) | bits_from(Mw, p + ew);
+    o |= (bits_from(Mw, p - 1) | bits_from(Mw, p - ew - 1) | bits_from(Mw, p + ew - 1)) & ~rs;
+    o |= (bits_from(Mw, p + 1) | bits_from(Mw, p - ew + 1) | bits_from(Mw, p + ew + 1)) & ~re;
     Ow[w] = o;
   }
   __syncthreads();
@@ -1006,27 +1027,25 @@ __global__ void __launch_bounds__(kThreads) k_or(Ctx c) {
 }  // namespace
 
 size_t refine_mk_state_bytes(int n_wins) { return (size_t(n_wins) * sizeof(WinState) + 255) / 256 * 256; }
-size_t refine_mk_chunk_bytes() { return sizeof(Chunk); }
-int refine_mk_chunk_px() { return kChunkPx; }
+// L (4 B), per-root sums (16 B), grey, predm, merged, tmp (1 B each) per window pixel
+size_t refine_scratch_bytes(size_t total_px) { return total_px * (4 + 16 + 4) + 4096; }
 
-// d_wins: n_wins RefineWin records; d_chunks: n_chunks {win, y0, rows, pad} (whole rows, <= refine_mk_chunk_px() pixels
-// each unless a single row is longer); d_state: refine_mk_state_bytes(n_wins) bytes (zeroed here); scratch planes as in
-// refine_launch.  img / mask / out hold H*W-pixel planes per page.
-cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, int H, int W, const void* d_wins, int n_wins,
-                             const void* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
+// d_wins: n_wins windows; d_chunks: n_chunks chunks (RefineChunk, kernels.h); d_state: refine_mk_state_bytes(n_wins)
+// bytes (zeroed here); scratch: refine_scratch_bytes(total_px) bytes.  img / mask / out hold H*W-pixel planes per page.
+cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, int H, int W, const RefineWin* d_wins, int n_wins,
+                             const RefineChunk* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
                              void* scratch, int refine_mode, uint8_t* d_out, cudaStream_t s) {
   if (n_wins <= 0 || n_chunks <= 0) return cudaSuccess;
   Ctx c;
   c.img_all = d_img; c.mask_all = d_mask; c.out_all = reinterpret_cast<uint32_t*>(d_out);
-  c.wins = static_cast<const RefineWin*>(d_wins);
-  c.chunks = static_cast<const Chunk*>(d_chunks);
+  c.wins = d_wins;
+  c.chunks = d_chunks;
   c.st = static_cast<WinState*>(d_state);
   c.H = H; c.W = W; c.mode = refine_mode;
   char* p = static_cast<char*>(scratch);
   c.L = reinterpret_cast<int*>(p); p += total_px * 4;
   c.acc = reinterpret_cast<int*>(p); p += total_px * 16;
   c.grey = reinterpret_cast<uint8_t*>(p); p += total_px;
-  c.cand = reinterpret_cast<uint8_t*>(p); p += total_px;
   c.predm = reinterpret_cast<uint8_t*>(p); p += total_px;
   c.merged = reinterpret_cast<uint8_t*>(p); p += total_px;
   c.tmp = reinterpret_cast<uint8_t*>(p);
