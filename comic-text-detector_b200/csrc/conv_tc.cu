@@ -12,6 +12,9 @@
 // Activations are 4-D TMA boxes over the NHWC buffers: out-of-bounds zero-fill IS the convolution padding, there is
 // no im2col buffer; torch.cat inputs are K-concatenated from up to 3 tensor maps; stride 2 reads four parity maps;
 // ConvTranspose 4x4 s2 p1 runs as 4 sub-pixel phases of 2x2 taps; Detect heads decode sigmoid / boxes in the epilogue.
+// The fp16 NHWC epilogue (CONV, DECONV4, stem) writes the warpgroup's tile into a swizzled staging buffer with stmatrix
+// and one elected thread stores it with TMA through the destination map, so the store drains while the warpgroup
+// runs the next tile's mainloop; an in-place residual is TMA-loaded into the same buffer at the start of the tile.
 //
 // Reference semantics: Conv.forward_fuse (models/yolov5/common.py:48-49), Bottleneck add (common.py:104),
 // ConvTranspose2d+BN+ReLU (basemodel.py:26-28), Detect (yolo.py:23-44).
@@ -29,18 +32,25 @@ namespace ctd {
 constexpr int kTileW = 16;     // tile width in grid pixels; the height TH (8 or 16) is a template parameter
 constexpr int kThreads = 384;  // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
 
-// Shared memory per (BN, TH): stages x (A box of 16*TH rows + B box of BN rows, 128-byte rows in the worst case).
-//   TH = 8:  BN 128: 6 x 32 KB | 64: 8 x 24 KB | 32: 10 x 20 KB | 16: 10 x 18 KB
-//   TH = 16: BN 128: 4 x 48 KB | 64: 5 x 40 KB | 32:  6 x 36 KB | 16:  6 x 34 KB
+// Shared memory per (BN, TH): stages x (A box of 16*TH rows + B box of BN rows, 128-byte rows in the worst case),
+// then one fp16 staging tile of 8*TH pixels x BN channels per consumer warpgroup.
+//   TH = 8:  BN 128: 5 x 32 KB + 2 x 16 KB | 64: 8 x 24 KB + 2 x 8 KB | 32: 10 x 20 KB + 2 x 4 KB | 16: 10 x 18 KB + 2 x 2 KB
+//   TH = 16: BN 128: 3 x 48 KB + 2 x 32 KB | 64: 4 x 40 KB + 2 x 16 KB | 32: 5 x 36 KB + 2 x 8 KB | 16: 6 x 34 KB + 2 x 4 KB
 template <int BN, int TH>
 struct TcCfg {
   static constexpr int kABytes = TH * kTileW * 128;  // per stage (worst case 128-byte rows)
   static constexpr int kBBytes = BN * 128;
-  static constexpr int kStages = TH == 8 ? (BN >= 128 ? 6 : (BN >= 64 ? 8 : 10)) : (BN >= 128 ? 4 : (BN >= 64 ? 5 : 6));
+  static constexpr int kStages = TH == 8 ? (BN >= 128 ? 5 : (BN >= 64 ? 8 : 10))
+                                         : (BN >= 128 ? 3 : (BN >= 64 ? 4 : (BN >= 32 ? 5 : 6)));
+  // staging: store boxes of kBoxN channels x 16 x TH/2 pixels, rows of kBoxN fp16 in the box's swizzle
+  static constexpr int kBoxN = BN < 64 ? BN : 64;
+  static constexpr int kBoxBytes = 8 * TH * kBoxN * 2;
+  static constexpr int kStgBytes = (BN / kBoxN) * kBoxBytes;   // per consumer warpgroup
   static constexpr int kBiasFloats = 512;
-  // 1024 bytes of alignment slack | operand ring | barriers (256 B) | bias
-  static constexpr size_t kSmem = 1024 + size_t(kStages) * (kABytes + kBBytes) + 256 + kBiasFloats * 4;
+  // 1024 bytes of alignment slack | operand ring | staging (2 warpgroups) | barriers (256 B) | bias
+  static constexpr size_t kSmem = 1024 + size_t(kStages) * (kABytes + kBBytes) + 2 * kStgBytes + 256 + kBiasFloats * 4;
   static_assert(kSmem <= 227 * 1024, "conv_tc_kernel: shared memory");
+  static_assert(kBoxBytes % 1024 == 0, "conv_tc_kernel: store boxes must keep the 1024-byte swizzle alignment");
 };
 
 template <int ACT>
@@ -71,24 +81,44 @@ __device__ __forceinline__ void wgmma_bn(float (&d)[BN / 2], uint64_t ad, uint64
   else wgmma_n16(d, ad, bd, acc);
 }
 
-// Epilogue of one accumulator row pair (columns col, col + 1) of an fp16 destination: bias + activation (+ residual)
-// -> fp16.  `out` / `res` point at channel 0 of this tile's N block for the pixel; columns >= ncols are not written.
-template <int ACT, bool RES>
-__device__ __forceinline__ void epi_pair_f16(float v0, float v1, const float* __restrict__ bias_s, int col,
-                                             __half* __restrict__ out, const __half* __restrict__ res, int ncols) {
-  if (col >= ncols) return;
-  float f0 = apply_act<ACT>(v0 + bias_s[col]);
-  float f1 = apply_act<ACT>(v1 + bias_s[col + 1]);
-  if (col + 1 < ncols) {
-    if constexpr (RES) {
-      const float2 r = __half22float2(*reinterpret_cast<const __half2*>(res + col));
-      f0 += r.x;
-      f1 += r.y;
+// fp16 epilogue of row block m of a consumer warpgroup: bias + activation (+ residual, already loaded into the
+// staging tile) -> fp16, written into the staging tile in place.  One stmatrix x4 covers the 16 rows of this warp
+// and 16 columns: matrix q holds rows 8*(q & 1) .. +7 and the column block j + (q >> 1), which are accumulators
+// acc[4j + 2q], acc[4j + 2q + 1].  Rows of a box are kBoxN fp16 with the 32/64/128-byte swizzle of the tensor map (the
+// 16-byte chunk index XOR address bits 7..9); eight consecutive rows then hit eight distinct chunk columns, so the
+// stores are free of bank conflicts.
+template <int BN, int TH, int ACT, bool RES>
+__device__ __forceinline__ void stage_f16(const float (&acc)[BN / 2], const float* __restrict__ bias_s, uint32_t stg,
+                                          int m, int warp4, int lane) {
+  using Cfg = TcCfg<BN, TH>;
+  constexpr uint32_t kRowBytes = Cfg::kBoxN * 2;
+  const int q = lane >> 3;
+  const uint32_t pixrow = uint32_t(m * 64 + warp4 * 16 + (q & 1) * 8 + (lane & 7));
+#pragma unroll
+  for (int j = 0; j < BN / 8; j += 2) {
+    const int col = (j + (q >> 1)) * 8;   // first column of the matrix this lane addresses
+    const uint32_t off = pixrow * kRowBytes + uint32_t(col % Cfg::kBoxN) * 2;
+    const uint32_t addr = stg + uint32_t(col / Cfg::kBoxN) * Cfg::kBoxBytes +
+                          (off ^ (((off >> 7) & (kRowBytes / 16 - 1)) << 4));
+    uint32_t r[4];
+    if constexpr (RES) ldmatrix_x4(addr, r);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int c = (j + (i >> 1)) * 8 + (lane & 3) * 2;
+      float f0 = apply_act<ACT>(acc[j * 4 + 2 * i] + bias_s[c]);
+      float f1 = apply_act<ACT>(acc[j * 4 + 2 * i + 1] + bias_s[c + 1]);
+      if constexpr (RES) {
+        __half2 h;
+        memcpy(&h, &r[i], 4);
+        const float2 rv = __half22float2(h);
+        // __fadd_rn: never fused with the multiply of the fast division (one rounding each, as in the fp32 reference)
+        f0 = __fadd_rn(f0, rv.x);
+        f1 = __fadd_rn(f1, rv.y);
+      }
+      const __half2 o = __floats2half2_rn(f0, f1);
+      memcpy(&r[i], &o, 4);
     }
-    *reinterpret_cast<__half2*>(out + col) = __floats2half2_rn(f0, f1);
-  } else {
-    if constexpr (RES) f0 += __half2float(res[col]);
-    out[col] = __float2half_rn(f0);
+    stmatrix_x4(addr, r);
   }
 }
 
@@ -108,21 +138,6 @@ __device__ __forceinline__ void epi_pair_f32(float v0, float v1, const float* __
   } else {
     if (residual) f0 += out[col];
     out[col] = f0;
-  }
-}
-
-// The fp16 epilogue over this thread's whole accumulator fragment (two pixels, BN/4 column pairs each).
-template <int BN, int ACT, bool RES>
-__device__ __forceinline__ void epilogue_f16(const float (&acc)[BN / 2], const float* __restrict__ bias_s,
-                                             __half* const (&out)[2], const __half* const (&res)[2], const bool (&valid)[2],
-                                             int ncols, int lane) {
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    if (!valid[h]) continue;
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
-      epi_pair_f16<ACT, RES>(acc[j * 4 + 2 * h], acc[j * 4 + 2 * h + 1], bias_s, j * 8 + (lane & 3) * 2, out[h], res[h],
-                             ncols);
   }
 }
 
@@ -151,10 +166,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   uint8_t* const smem_gen = smem_tc + (smem_base - raw_base);
   const uint32_t a_base = smem_base;
   const uint32_t b_base = a_base + Cfg::kStages * Cfg::kABytes;
-  const uint32_t bar_base = b_base + Cfg::kStages * Cfg::kBBytes;
-  // barriers (8 B each): full[S] | empty[S]
-  const uint32_t full_bar = bar_base, empty_bar = bar_base + 8 * Cfg::kStages;
-  float* bias_s = reinterpret_cast<float*>(smem_gen + size_t(Cfg::kStages) * (Cfg::kABytes + Cfg::kBBytes) + 256);
+  const uint32_t stg_base = b_base + Cfg::kStages * Cfg::kBBytes;
+  const uint32_t bar_base = stg_base + 2 * Cfg::kStgBytes;
+  // barriers (8 B each): full[S] | empty[S] | residual[2] (one per consumer warpgroup)
+  const uint32_t full_bar = bar_base, empty_bar = bar_base + 8 * Cfg::kStages, res_bar0 = bar_base + 16 * Cfg::kStages;
+  float* bias_s = reinterpret_cast<float*>(smem_gen + (bar_base - smem_base) + 256);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const ConvGeom& g = p.g;
@@ -175,10 +191,14 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     for (int s = 0; s < g.n_src; ++s)
       for (int q = 0; q < (g.in_stride == 2 ? 4 : 1); ++q) prefetch_tensormap(&p.a_map[s][q]);
     prefetch_tensormap(&p.b_map);
+    if (p.dst != nullptr && !p.split)
+      for (int ph = 0; ph < g.n_phase; ++ph) prefetch_tensormap(&p.d_map[ph]);
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(full_bar + 8 * s, 1);
       mbar_init(empty_bar + 8 * s, 2);   // one arrival per consumer warpgroup
     }
+    mbar_init(res_bar0, 1);
+    mbar_init(res_bar0 + 8, 1);
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < g.cout_pad && i < Cfg::kBiasFloats; i += kThreads) bias_s[i] = p.bias ? p.bias[i] : 0.f;
@@ -244,10 +264,28 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   int stage = 0;
   uint32_t full_par = 0;
   constexpr int R = BN / 2;
+  // fp16 NHWC destination (CONV, DECONV4, stem): the epilogue stages the warpgroup's 8*TH x BN tile in shared memory
+  // and one elected thread stores it with TMA while the warpgroup goes on to the next tile's mainloop
+  const bool nhwc16 = p.dst != nullptr && !p.split;
+  const bool res16 = nhwc16 && g.residual != 0;
+  const uint32_t stg = stg_base + uint32_t(wg) * Cfg::kStgBytes;
+  const uint32_t res_bar = res_bar0 + 8u * uint32_t(wg);
+  const uint32_t epi_bar = 1 + wg;   // named barrier of this warpgroup's 128 threads (0 is __syncthreads)
+  uint32_t res_par = 0;
 
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
     int phase, nblk, img, y0, x0;
     decode(t, phase, nblk, img, y0, x0);
+    const int sy0 = y0 + wg * (TH / 2);   // first pixel row of this warpgroup's staging tile
+    if (res16 && wg_leader) {
+      // in-place residual: once the previous tile's store has read the staging tile, load this tile's residual box
+      // into it, under the mainloop
+      tma_store_wait_read();
+      mbar_arrive_expect_tx(res_bar, Cfg::kStgBytes);
+#pragma unroll
+      for (int b = 0; b < BN / Cfg::kBoxN; ++b)
+        tma_load_4d(stg + b * Cfg::kBoxBytes, &p.d_map[phase], res_bar, nblk * BN + b * Cfg::kBoxN, x0, sy0, img);
+    }
     float acc[MT][R];
 #pragma unroll
     for (int m = 0; m < MT; ++m)
@@ -324,8 +362,70 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
     }
 
     // ---------------------------------------------------------------- epilogue
-    const int ph_y = phase >> 1, ph_x = phase & 1;
     const float* bias_t = bias_s + nblk * BN;
+    if (nhwc16) {
+      if (res16) {
+        mbar_wait(res_bar, res_par);
+        res_par ^= 1u;
+      } else {
+        if (wg_leader) tma_store_wait_read();   // the previous tile's store has read the staging tile
+        named_barrier_sync(epi_bar, 128);
+      }
+#define CTD_EPI(ACT)                                                                                   \
+  _Pragma("unroll") for (int m = 0; m < MT; ++m) {                                                     \
+    if (res16) stage_f16<BN, TH, ACT, true>(acc[m], bias_t, stg, m, warp & 3, lane);                   \
+    else stage_f16<BN, TH, ACT, false>(acc[m], bias_t, stg, m, warp & 3, lane);                        \
+  }
+      switch (g.act) {
+        case CTD_ACT_SILU: CTD_EPI(CTD_ACT_SILU) break;
+        case CTD_ACT_LEAKY: CTD_EPI(CTD_ACT_LEAKY) break;
+        case CTD_ACT_RELU: CTD_EPI(CTD_ACT_RELU) break;
+        case CTD_ACT_SIGMOID: CTD_EPI(CTD_ACT_SIGMOID) break;
+        default: CTD_EPI(CTD_ACT_NONE) break;
+      }
+#undef CTD_EPI
+      // generic-proxy writes -> visible to the TMA (async proxy) store, then one thread stores the whole tile
+      fence_proxy_async();
+      named_barrier_sync(epi_bar, 128);
+      if (wg_leader) {
+#pragma unroll
+        for (int b = 0; b < BN / Cfg::kBoxN; ++b)
+          tma_store_4d(&p.d_map[phase], stg + b * Cfg::kBoxBytes, nblk * BN + b * Cfg::kBoxN, x0, sy0, img);
+        tma_store_commit();
+      }
+      if (p.dst_map_cols < g.cout && p.dst_map_cols < (nblk + 1) * BN) {
+        // columns [dst_map_cols, cout): within the last 16-byte granule of the slice, which the map leaves out
+#pragma unroll
+        for (int m = 0; m < MT; ++m)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = (wg * MT + m) * 64 + wrow + 8 * h;
+            const int gy = y0 + row / kTileW, gx = x0 + row % kTileW;
+            if (gy >= g.gh || gx >= g.gw) continue;
+            const int oy = gy * g.out_mul + (phase >> 1), ox = gx * g.out_mul + (phase & 1);
+            __half* out = p.dst + (size_t(img) * g.dst_h * g.dst_w + size_t(oy) * g.dst_w + ox) * g.dst_cstride +
+                          g.dst_coff;
+#pragma unroll
+            for (int i = 0; i < R; ++i) {
+              if (((i >> 1) & 1) != h) continue;
+              const int c = (i >> 2) * 8 + (lane & 3) * 2 + (i & 1), col = nblk * BN + c;
+              if (col < p.dst_map_cols || col >= g.cout) continue;
+              float f;
+              switch (g.act) {
+                case CTD_ACT_SILU: f = apply_act<CTD_ACT_SILU>(acc[m][i] + bias_t[c]); break;
+                case CTD_ACT_LEAKY: f = apply_act<CTD_ACT_LEAKY>(acc[m][i] + bias_t[c]); break;
+                case CTD_ACT_RELU: f = apply_act<CTD_ACT_RELU>(acc[m][i] + bias_t[c]); break;
+                case CTD_ACT_SIGMOID: f = apply_act<CTD_ACT_SIGMOID>(acc[m][i] + bias_t[c]); break;
+                default: f = acc[m][i] + bias_t[c]; break;
+              }
+              if (res16) f = __fadd_rn(f, __half2float(out[col]));
+              out[col] = __float2half_rn(f);
+            }
+          }
+      }
+      continue;
+    }
+    const int ph_y = phase >> 1, ph_x = phase & 1;
     const int ncols = g.cout - nblk * BN;   // columns of this N block that exist
 #pragma unroll
     for (int m = 0; m < MT; ++m) {
@@ -385,7 +485,8 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
             rows[(size_t(a) * g.gh * g.gw + size_t(gy[h]) * g.gw + gx[h]) * no + o] = r;
           }
         }
-      } else if (p.split) {
+      } else {
+        // split-fp16 mode: fp32 NHWC destination
         float* out32[2];
 #pragma unroll
         for (int h = 0; h < 2; ++h)
@@ -398,28 +499,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
           case CTD_ACT_SIGMOID: epilogue_f32<BN, CTD_ACT_SIGMOID>(acc[m], bias_t, out32, valid, ncols, lane, res); break;
           default: epilogue_f32<BN, CTD_ACT_NONE>(acc[m], bias_t, out32, valid, ncols, lane, res); break;
         }
-      } else {
-        __half* out[2];
-        const __half* res[2];   // residual: read from the destination itself (in-place add)
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          out[h] = p.dst + pix[h] * g.dst_cstride + g.dst_coff + nblk * BN;
-          res[h] = out[h];
-        }
-#define CTD_EPI(ACT)                                                                             \
-  if (g.residual) epilogue_f16<BN, ACT, true>(acc[m], bias_t, out, res, valid, ncols, lane);   \
-  else epilogue_f16<BN, ACT, false>(acc[m], bias_t, out, res, valid, ncols, lane);
-        switch (g.act) {
-          case CTD_ACT_SILU: CTD_EPI(CTD_ACT_SILU) break;
-          case CTD_ACT_LEAKY: CTD_EPI(CTD_ACT_LEAKY) break;
-          case CTD_ACT_RELU: CTD_EPI(CTD_ACT_RELU) break;
-          case CTD_ACT_SIGMOID: CTD_EPI(CTD_ACT_SIGMOID) break;
-          default: CTD_EPI(CTD_ACT_NONE) break;
-        }
-#undef CTD_EPI
       }
     }
   }
+  // the staging tiles must outlive the last TMA stores that read them
+  if (nhwc16 && wg_leader) tma_store_wait_all();
 }
 
 // =========================================================================================
@@ -434,6 +518,29 @@ static const char* encode_map(PFN_encodeTiled enc, CUtensorMap* m, const void* b
                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   return r == CUDA_SUCCESS ? nullptr : "cuTensorMapEncodeTiled failed";
+}
+
+// fp16 NHWC destination maps of the staged epilogue, one per phase: {cout & ~7, gw, gh, n_img} over the slice, so that
+// TMA clips the padding columns (cout .. cout_pad), the neighbouring channels and the pixels beyond the grid (the
+// innermost dimension is clipped in 16-byte units: the last cout % 8 columns are stored from registers).  A
+// DECONV4 phase map starts at the phase's sub-pixel (ph_y, ph_x) and steps two destination pixels in x and y.  Boxes
+// are min(BN, 64) channels x 16 x TH/2 pixels (one consumer warpgroup's half of the tile) in the swizzle of a K block
+// of the same width.
+static const char* encode_dst_maps(PFN_encodeTiled enc, ConvTcParams& p, const __half* dst, int bn, int th) {
+  const ConvGeom& g = p.g;
+  const int boxn = bn < 64 ? bn : 64;
+  p.dst_map_cols = g.cout & ~7;
+  if (p.dst_map_cols == 0) return "conv_tc: fp16 destination needs at least 8 output channels";
+  const cuuint64_t px = cuuint64_t(g.dst_cstride) * 2;   // bytes per destination pixel
+  for (int ph = 0; ph < g.n_phase; ++ph) {
+    const int ph_y = ph >> 1, ph_x = ph & 1;
+    const char* base = reinterpret_cast<const char*>(dst) + size_t(g.dst_coff) * 2 + (size_t(ph_y) * g.dst_w + ph_x) * px;
+    cuuint64_t dims[4] = {cuuint64_t(p.dst_map_cols), cuuint64_t(g.gw), cuuint64_t(g.gh), cuuint64_t(g.n_img)};
+    cuuint64_t str[3] = {px * g.out_mul, px * g.dst_w * g.out_mul, px * g.dst_w * g.dst_h};
+    cuuint32_t box[4] = {cuuint32_t(boxn), kTileW, cuuint32_t(th / 2), 1};
+    if (const char* e = encode_map(enc, &p.d_map[ph], base, 4, dims, str, box, boxn)) return e;
+  }
+  return nullptr;
 }
 
 static int g_num_sms = 132;
@@ -529,6 +636,8 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
     }
   plan.block_n = bn;
   plan.tile_h = th;
+  if (dst != nullptr && !split)
+    if (const char* e = encode_dst_maps(enc, p, dst, bn, th)) return e;
   if (split && ((g.dst_coff % 4) != 0 || (g.dst_cstride % 4) != 0 || (dst != nullptr && g.cout % 4 != 0)))
     return "conv_tc (split): fp32 destination slice must be 16-byte aligned";
   {
@@ -574,6 +683,7 @@ const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void*
   }
   plan.block_n = 32;
   plan.tile_h = 8;
+  if (const char* e = encode_dst_maps(enc, p, dst, 32, 8)) return e;
   {
     cuuint64_t dims[2] = {192, 32};
     cuuint64_t str[1] = {192 * 2};

@@ -52,12 +52,20 @@ void fill_conv_geom_taps(ConvGeom& g, int kind, int ksize, int stride);
 struct alignas(64) ConvTcParams {
   CUtensorMap a_map[CTD_MAX_SRC][4];  // [source][parity]: parity maps only for stride-2 convs
   CUtensorMap b_map;                  // packed weights [n_phase*cout_pad][k_total], K-major
+  // fp16 NHWC destination [phase]: {cout, gw, gh, n_img} over the slice (base at channel dst_coff; a DECONV4 phase
+  // map starts at its sub-pixel and steps two pixels).  The epilogue stores its staged tile through it, and an
+  // in-place residual is loaded through it; TMA clipping keeps padding columns, neighbouring channels and pixels
+  // beyond the grid unwritten.
+  CUtensorMap d_map[kMaxPhases];
   ConvGeom g;
   int kb_elems;                       // channels per K block: 64 / 32 / 16 (swizzle 128/64/32 B)
   int src_kblocks[CTD_MAX_SRC];
   int tiles_x, tiles_y;               // 16xTH-pixel tiles per image (TH = ConvTcPlan::tile_h)
   int8_t tap_map[kMaxPhases][kMaxTaps];  // parity map index per tap (stride 2), else 0
   __half* dst;
+  // columns [0, dst_map_cols) go through d_map: cout rounded down to 8, since TMA clips the innermost dimension in
+  // 16-byte units; the epilogue stores columns [dst_map_cols, cout) from registers
+  int dst_map_cols;
   const float* bias;
   // DETECT epilogue (dst == nullptr): decoded rows go to blks
   float* blks;
@@ -79,6 +87,7 @@ struct alignas(64) ConvTcParams {
   int split_img_off;
   int split_row_off;
 };
+static_assert(sizeof(ConvTcParams) <= 4096, "ConvTcParams: kernel parameters are limited to 4 KB");
 
 struct ConvTcPlan {
   ConvTcParams p;

@@ -124,6 +124,20 @@ __device__ __forceinline__ void named_barrier_sync(uint32_t id, uint32_t nthread
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// Four 8x8 b16 matrices between registers and shared memory: lanes 8q..8q+7 give the row addresses of matrix q, and
+// thread t holds row t/4, columns 2*(t%4) and 2*(t%4)+1 of every matrix in r[q] (the wgmma accumulator fragment).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+               "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
+
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // D[64 x N] (fp32, registers of the issuing warpgroup) (+)= A[64 x 16] * B[N x 16]^T, both operands K-major fp16 in
 // swizzled shared memory.  Accumulator fragment of thread t of the warpgroup (warp w = t / 32, lane l): d[i] holds

@@ -10,8 +10,10 @@ moves from L2 into shared memory (A = activation boxes, B = weight boxes; every 
 loads one A box and one B box).  The plan is computed here from the same rules as csrc/conv_tc.cu (132 SMs).
 
 With --gpu, the program also runs on cuda:0: each op's device time is the minimum over --runs un-graphed forwards
-(Engine.profile_forward, CUDA events around every op), and the row adds the achieved TFLOP/s and operand TB/s.  The
-card's name and power limit are printed with the table.
+(Engine.profile_forward, CUDA events around every op), and the row adds the achieved TFLOP/s, operand TB/s and HBM
+TB/s (least HBM bytes over time).  The totals end with one line per op kind (1x1 CONV, 3x3 CONV, DECONV4, DETECT,
+stem, seg tail), with ms, TFLOP/s and HBM TB/s under --gpu.  The card's name and power limit are printed with the
+table.
 """
 import argparse
 import json
@@ -167,18 +169,19 @@ def main():
             r["ms"] = ms[r["op"]]
             r["tflops"] = r["gflop"] / r["ms"] if r["ms"] > 0 else 0.0
             r["operand_tbs"] = (r["a_gb"] + r["b_gb"]) / r["ms"] if r["ms"] > 0 else 0.0
+            r["hbm_tbs"] = r["hbm_gb"] / r["ms"] if r["ms"] > 0 else 0.0
     print("conv_tc ops at %d x %d x %d fp16%s" % (n, h, w, ("; " + card) if card else " (CPU model, not measured)"))
     hdr = "%4s %-8s %2s %2s %5s %9s %4s %6s %6s %7s %10s %8s %6s %6s" % (
         "op", "kind", "k", "s", "res", "cin/cout", "BN", "tile", "tiles", "t/CTA", "GFLOP", "HBM GB", "A GB", "B GB")
     if args.gpu:
-        hdr += " %7s %7s %7s" % ("ms", "TFLOP/s", "opTB/s")
+        hdr += " %7s %7s %7s %7s" % ("ms", "TFLOP/s", "opTB/s", "HBMTB/s")
     print(hdr)
     for r in rows:
         line = "%4d %-8s %2d %2d %5d %9s %4d %6s %6d %7d %10.2f %8.3f %6.2f %6.2f" % (
             r["op"], r["kind"], r["k"], r["stride"], r["res"], "%d/%d" % (r["cin"], r["cout"]), r["bn"], r["tile"],
             r["tiles"], r["tiles_per_cta"], r["gflop"], r["hbm_gb"], r["a_gb"], r["b_gb"])
         if args.gpu:
-            line += " %7.3f %7.1f %7.2f" % (r["ms"], r["tflops"], r["operand_tbs"])
+            line += " %7.3f %7.1f %7.2f %7.2f" % (r["ms"], r["tflops"], r["operand_tbs"], r["hbm_tbs"])
         print(line)
     gemm = [r for r in rows if r["kind"] in ("conv", "deconv4", "detect")]
     for name, sel in (("CONV/DECONV4/DETECT (%d ops)" % len(gemm), gemm), ("all %d tensor-core ops" % len(rows), rows)):
@@ -189,10 +192,22 @@ def main():
             ms = sum(r["ms"] for r in sel)
             line += "; %.3f ms, %.1f TFLOP/s, operands %.2f TB/s" % (ms, t["gflop"] / ms, (t["a_gb"] + t["b_gb"]) / ms)
         print(line)
-    for kind in ("conv", "deconv4", "detect"):
-        sel = [r for r in rows if r["kind"] == kind]
-        print("  %-8s %3d ops: operands %.2f GB%s" % (kind, len(sel), sum(r["a_gb"] + r["b_gb"] for r in sel),
-                                                   ", %.3f ms" % sum(r["ms"] for r in sel) if args.gpu else ""))
+    groups = (("1x1 CONV", lambda r: r["kind"] == "conv" and r["k"] == 1),
+              ("3x3 CONV", lambda r: r["kind"] == "conv" and r["k"] == 3),
+              ("DECONV4", lambda r: r["kind"] == "deconv4"), ("DETECT", lambda r: r["kind"] == "detect"),
+              ("stem", lambda r: r["kind"] == "stem"), ("seg tail", lambda r: r["kind"] == "seg_tail"))
+    for name, pick in groups:
+        sel = [r for r in rows if pick(r)]
+        if not sel:
+            continue
+        t = {k: sum(r[k] for r in sel) for k in ("gflop", "hbm_gb", "a_gb", "b_gb")}
+        line = "  %-8s %3d ops: %.3f TFLOP, HBM %.2f GB, operands %.2f GB" % (
+            name, len(sel), t["gflop"] / 1e3, t["hbm_gb"], t["a_gb"] + t["b_gb"])
+        if args.gpu:
+            # HBM TB/s: least HBM bytes over device time
+            ms = sum(r["ms"] for r in sel)
+            line += "; %.3f ms, %.1f TFLOP/s, HBM %.2f TB/s" % (ms, t["gflop"] / ms, t["hbm_gb"] / ms)
+        print(line)
     if args.json:
         with open(args.json, "w") as f:
             json.dump({"shape": [n, h, w], "card": card, "rows": rows}, f, indent=1)
