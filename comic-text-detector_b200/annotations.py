@@ -13,11 +13,12 @@ import glob
 import json
 import os
 import os.path as osp
+from collections import deque
 from pathlib import Path
 
 import numpy as np
 
-from .inference import REFINEMASK_ANNOTATION, TextDetector
+from .inference import REFINEMASK_ANNOTATION, TextDetector, check_page
 
 IMG_EXT = (".bmp", ".jpg", ".png", ".jpeg")
 
@@ -107,16 +108,36 @@ def model2annotations(model_path, img_dir_list, save_dir, save_json=False, detec
     """`model2annotations(model_path, img_dir_list, save_dir, save_json)` of the reference (inference.py:19-70)."""
     if isinstance(img_dir_list, str):
         img_dir_list = [img_dir_list]
-    det = detector if detector is not None else TextDetector(model_path=model_path, input_size=1024, act="leaky")
+    # batches of up to 8 pages (scripts/pages_bench.py: the fastest of the measured batch sizes)
+    det = detector if detector is not None else TextDetector(model_path=model_path, input_size=1024, act="leaky",
+                                                             max_batch=8)
     os.makedirs(save_dir, exist_ok=True)
     try:
         imglist = []
         for d in img_dir_list:
             imglist += find_all_imgs(d, abs_path=True)
-        for img_path in imglist:
-            img = imread(img_path)
-            _mask, mask_refined, blk_list = det(img, refine_mode=REFINEMASK_ANNOTATION, keep_undetected_mask=True)
+        # pages are decoded while the previous batches run on the GPU (TextDetector.detect_stream); results come back
+        # in input order, so each one is written with the page it belongs to.  A page that cannot be read ends the
+        # stream there: every page before it is still written, then the error is raised, as page by page.
+        read, failed = deque(), []
+
+        def pages():
+            for img_path in imglist:
+                img = imread(img_path)
+                try:
+                    check_page(img)
+                except ValueError as ex:
+                    failed.append(ValueError("%s: %s" % (img_path, ex)))
+                    return
+                read.append((img_path, img))
+                yield img
+
+        for _mask, mask_refined, blk_list in det.detect_stream(pages(), refine_mode=REFINEMASK_ANNOTATION,
+                                                                keep_undetected_mask=True):
+            img_path, img = read.popleft()
             write_annotations(save_dir, osp.basename(img_path), img, mask_refined, blk_list, save_json)
+        if failed:
+            raise failed[0]
     finally:
         if detector is None:
             det.close()

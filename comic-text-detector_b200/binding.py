@@ -54,6 +54,11 @@ class CtdResultsLayout(C.Structure):
 
 MAX_BLOCKS, MAX_BLOCK_DIST = 1300, 8192   # CTD_MAX_BLOCKS / CTD_MAX_BLOCK_DIST
 
+# numpy mirror of `ctd_page_entry` (include/ctd_b200.h)
+PAGE_ENTRY_DTYPE = np.dtype([("ih", np.int32), ("iw", np.int32), ("unpad_h", np.int32), ("unpad_w", np.int32),
+                             ("page_off", np.int64), ("mask_off", np.int64), ("refined_off", np.int64),
+                             ("blocks_off", np.int64)], align=True)
+
 # numpy mirrors of `ctd_region_line` / `ctd_region` (include/ctd_b200.h)
 REGION_LINE_DTYPE = np.dtype([("quad", np.float64, (8,)), ("language", np.int32), ("vertical", np.int32),
                               ("font_size", np.float64)], align=True)
@@ -69,7 +74,7 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_results_bytes", "ctd_join", "ctd_forward_resized", "ctd_get_mask_u8_resized",
            "ctd_resize_linear_u8", "ctd_debug_run_ops", "ctd_get_nms_status", "ctd_group_output",
            "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena",
-           "ctd_region_plan", "ctd_transform_regions"]
+           "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages"]
 
 _lib = None
 
@@ -129,6 +134,8 @@ def load_library():
     lib.ctd_device_arena.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(vp)]
     lib.ctd_region_plan.argtypes = [vp, i32, i32, i32, i32, vp, C.POINTER(C.c_size_t)]
     lib.ctd_transform_regions.argtypes = [vp, vp, i32, i32, i32, vp, i32, vp, C.c_size_t]
+    lib.ctd_pages_plan.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.ctd_submit_pages.argtypes = [vp, i32, vp, i32, i32, i32, vp, i32, i32, vp]
     for name in EXPORTS[3:]:
         getattr(lib, name).restype = C.c_int
     lib.ctd_expand_textwindow.restype = None
@@ -150,6 +157,32 @@ def region_plan(lines, im_w, im_h, textheight):
     if rc != 0:
         raise CtdError("ctd_region_plan failed (%d): page %dx%d, textheight %d" % (rc, im_w, im_h, textheight))
     return plan, int(total.value)
+
+
+def pages_plan(shapes, net_h, net_w):
+    """`ctd_pages_plan` (host C++, no GPU): page sizes [(ih, iw), ...] -> (PAGE_ENTRY_DTYPE records, input bytes,
+    results bytes) of one batch for `Engine.submit_pages`."""
+    lib = load_library()
+    pages = np.zeros((len(shapes),), PAGE_ENTRY_DTYPE)
+    for i, (ih, iw) in enumerate(shapes):
+        pages[i]["ih"], pages[i]["iw"] = ih, iw
+    ib, rb = C.c_size_t(), C.c_size_t()
+    rc = lib.ctd_pages_plan(_ptr(pages), len(pages), int(net_h), int(net_w), C.byref(ib), C.byref(rb))
+    if rc != 0:
+        raise CtdError("ctd_pages_plan failed (%d): pages %s do not letterbox into a %dx%d net input"
+                       % (rc, list(shapes), net_h, net_w))
+    return pages, int(ib.value), int(rb.value)
+
+
+def decode_block_section(sec, layout):
+    """One page's block section (u8 bytes, see ctd_results_layout) -> (header i32 [4] = n_blocks, n_lines, n_dist,
+    flags; block records; line quads i32 [MAX_BLOCKS, 8]; distances f64 [MAX_BLOCK_DIST]), views into `sec`."""
+    hdr = sec[:16].view(np.int32)
+    ro, lo, do = layout["blk_records_off"], layout["blk_lines_off"], layout["blk_dist_off"]
+    rec = sec[ro:ro + MAX_BLOCKS * BLOCK_DTYPE.itemsize].view(BLOCK_DTYPE)[:int(hdr[0])]
+    lines = sec[lo:lo + MAX_BLOCKS * 32].view(np.int32).reshape(-1, 8)
+    dist = sec[do:do + MAX_BLOCK_DIST * 8].view(np.float64)
+    return hdr, rec, lines, dist
 
 
 class Engine:
@@ -395,6 +428,51 @@ class Engine:
 
     def collect(self, slot):
         self._ck(self.lib.ctd_collect(self.h, slot))
+
+    def submit_pages(self, slot, pages, net_h, net_w, refine_mode=0, keep_undetected=False):
+        """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages): the pages (u8 [h][w][3]
+        each) are packed into this slot's pinned input buffer, which like the pinned results buffer belongs to the
+        engine and grows on demand.  Collect with collect_pages(slot)."""
+        import torch
+        if not hasattr(self, "_pg_bufs"):
+            self._pg_bufs = [[None, None], [None, None]]   # per slot: pinned input, pinned results
+            self._pg_inflight = [None, None]
+        if self._pg_inflight[slot] is not None:
+            raise CtdError("slot %d has an uncollected submission" % slot)
+        entries, in_bytes, res_bytes = pages_plan([p.shape[:2] for p in pages], net_h, net_w)
+        bufs = self._pg_bufs[slot]
+        for k, need in ((0, in_bytes), (1, res_bytes)):
+            if bufs[k] is None or bufs[k].numel() < need:
+                bufs[k] = torch.empty((max(need, 1) * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        inp = bufs[0].numpy()
+        for e, p in zip(entries, pages):
+            o = int(e["page_off"])
+            np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+        self._ck(self.lib.ctd_submit_pages(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
+                                           C.c_void_p(bufs[0].data_ptr()), int(refine_mode), int(bool(keep_undetected)),
+                                           C.c_void_p(bufs[1].data_ptr())))
+        self._pg_inflight[slot] = entries
+        self.shape = (len(entries), net_h, net_w)
+
+    def collect_pages(self, slot):
+        """blocks until the batch of submit_pages(slot) is done -> per page the 5-tuple detect_page returns
+        (mask, mask_refined, block records, lines, distances), copied out of the slot's pinned buffer."""
+        entries = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
+        if entries is None:
+            raise CtdError("slot %d has no submit_pages batch in flight" % slot)
+        self._pg_inflight[slot] = None
+        self.collect(slot)
+        res = self._pg_bufs[slot][1].numpy()
+        lay = self.results_layout()
+        stride = lay["blocks_stride"]
+        out = []
+        for e in entries:
+            ih, iw = int(e["ih"]), int(e["iw"])
+            mo, ro, bo = int(e["mask_off"]), int(e["refined_off"]), int(e["blocks_off"])
+            _hdr, rec, lines, dist = decode_block_section(res[bo:bo + stride], lay)
+            out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy(), res[ro:ro + ih * iw].reshape(ih, iw).copy(),
+                        rec.copy(), lines.copy(), dist.copy()))
+        return out
 
     def join(self, other):
         """everything enqueued so far on `other`'s stream becomes a dependency of this engine's stream."""

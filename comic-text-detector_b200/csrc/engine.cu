@@ -235,10 +235,8 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
     L.a_bytes = L.lc + al(nb * 4);
     L.refined = L.a_bytes;
     L.blocks = L.refined + al(px);
-    L.rec_off = 64;
-    L.lines_off = L.rec_off + al(size_t(CTD_MAX_BLOCKS) * sizeof(ctd_block));
-    L.dist_off = L.lines_off + al(size_t(CTD_MAX_BLOCKS) * 32);
-    L.blocks_stride = L.dist_off + al(size_t(CTD_MAX_BLOCK_DIST) * 8);
+    const BlockSection bs = block_section_layout();
+    L.rec_off = bs.rec_off; L.lines_off = bs.lines_off; L.dist_off = bs.dist_off; L.blocks_stride = bs.stride;
     L.total = L.blocks + nb * L.blocks_stride;
     h->results_bytes = L.total;
     CKC(cudaMalloc(&h->d_mask_u8, h->results_bytes));

@@ -5,6 +5,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <math.h>
+
+#include <algorithm>
 #include <array>
 #include <condition_variable>
 #include <deque>
@@ -29,10 +32,53 @@ struct ArenaLayout {
   size_t det, cnt, nl, lb, ls, lc, a_bytes, refined, blocks, blocks_stride, rec_off, lines_off, dist_off, total;
 };
 
+// one page's block section (ctd_page_blocks header, ctd_block records, line quads, distances): offsets inside the
+// section and its size, the same for every handle
+struct BlockSection {
+  size_t rec_off, lines_off, dist_off, stride;
+};
+inline BlockSection block_section_layout() {
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  BlockSection b;
+  b.rec_off = 64;
+  b.lines_off = b.rec_off + al(size_t(CTD_MAX_BLOCKS) * sizeof(ctd_block));
+  b.dist_off = b.lines_off + al(size_t(CTD_MAX_BLOCKS) * 32);
+  b.stride = b.dist_off + al(size_t(CTD_MAX_BLOCK_DIST) * 8);
+  return b;
+}
+
+// letterbox(im, (net_h, net_w), auto=False) (imgproc_utils.py:86-117, python round = half to even) and the
+// resize_ratio that maps net coordinates back to the page (inference.py:148).  false: the page does not letterbox into
+// the net input (a side < 1 or an unpadded side of 0).
+struct Letterbox {
+  int unpad_h, unpad_w;
+  float ratio_x, ratio_y;
+};
+inline bool letterbox_of(int ih, int iw, int net_h, int net_w, Letterbox& lb) {
+  if (ih < 1 || iw < 1 || net_h < 1 || net_w < 1) return false;
+  const double r = std::min(double(net_h) / ih, double(net_w) / iw);
+  lb.unpad_w = int(nearbyint(iw * r));
+  lb.unpad_h = int(nearbyint(ih * r));
+  if (lb.unpad_w < 1 || lb.unpad_h < 1 || lb.unpad_w > net_w || lb.unpad_h > net_h) return false;
+  lb.ratio_x = float(double(iw) / double(lb.unpad_w));
+  lb.ratio_y = float(double(ih) / double(lb.unpad_h));
+  return true;
+}
+
+// results of a ctd_submit_pages batch of n pages: the phase-A rows (sized for n pages) at the start of the results
+// buffer, then the packed page masks, the mask_refined planes and the block sections at the ctd_page_entry offsets
+struct PagesHead {
+  size_t det, cnt, lb, ls, lc, masks;
+};
+PagesHead pages_head(int n);
+
 struct PipeJob {
   int slot = 0, n = 0, ph = 0, pw = 0, refine_mode = 0;
   void* results_host = nullptr;
   const uint8_t* pages_dev = nullptr;   // caller's device pages (pages_on_device) or null: the slot's staging copy
+  // ctd_submit_pages: the batch's pages (ph x pw is the net shape), and whether to run refine_undetected_mask
+  std::vector<ctd_page_entry> pages;
+  int keep_undetected = 0;
 };
 
 // refine windows of one launch (all pages of a batch) and the chunks they are cut into
@@ -40,7 +86,8 @@ struct RefineJob {
   std::vector<ctd::RefineWin> wins;
   std::vector<ctd::RefineChunk> chunks;
   size_t total_px = 0;
-  void add(int x1, int y1, int x2, int y2, int page, int iw, int ih);   // python slice semantics; empty windows dropped
+  // window of the iw x ih page whose planes start at pixel page_off; python slice semantics; empty windows dropped
+  void add(int x1, int y1, int x2, int y2, size_t page_off, int iw, int ih);
   size_t table_bytes() const;
 };
 
@@ -124,6 +171,20 @@ struct ctd_handle {
   int pipe_rc[2] = {0, 0};
   std::string pipe_err[2];
   int host_threads = 4;
+  // any-size batches (ctd_submit_pages): per-slot device planes (packed pages | results head, masks, mask_refined |
+  // second refine output and threshold planes of refine_undetected_mask), grown while the slot is idle; per-slot page
+  // tables (pinned + device, max_batch entries); the worker's own connected-components scratch
+  uint8_t* d_pg_in[2] = {nullptr, nullptr};
+  uint8_t* d_pg_res[2] = {nullptr, nullptr};
+  uint8_t* d_pg_aux[2] = {nullptr, nullptr};
+  size_t pg_in_cap[2] = {0, 0}, pg_res_cap[2] = {0, 0}, pg_aux_cap[2] = {0, 0};
+  ctd::PageGeom* h_pg_tab[2] = {nullptr, nullptr};
+  ctd::PageGeom* d_pg_tab[2] = {nullptr, nullptr};
+  void* d_pg_cc = nullptr;
+  size_t pg_cc_cap = 0;
+  // refine scratch of the worker's phase C on the post stream (d_refine_scratch belongs to the caller's stream)
+  void* d_post_refine = nullptr;
+  size_t post_refine_cap = 0;
   // last forward
   int n = 0, ph = 0, pw = 0;
   int last_launches = 0;
@@ -139,7 +200,7 @@ int ensure_io_scratch(ctd_handle* h, size_t bytes);
 // connected components + stats of a DEVICE u8 image on the engine stream (grow-on-demand scratch): *d_stats points at
 // [stats_cap][5] ints on the device, *n_labels is read back (synchronises the stream)
 int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap, int32_t** d_stats, int32_t* n_labels);
-int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int ih, int iw,
-                  int refine_mode, uint8_t* d_out, cudaStream_t st, char* pinned);
+int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int refine_mode,
+                  uint8_t* d_out, cudaStream_t st, void** scratch, size_t* cap, char* pinned);
 int ctd_collect_full(ctd_handle* h, int slot);
 void ctd_pipeline_shutdown(ctd_handle* h);

@@ -194,12 +194,27 @@ cudaError_t binarize_launch(const float* pred, size_t count, float thresh, uint8
 // dh x dw result is written at the top-left of a canvas_h x canvas_w canvas whose remaining pixels are zeroed.
 cudaError_t resize_linear_u8_launch(const uint8_t* src, int sh, int sw, size_t src_pitch, int channels, uint8_t* dst,
                                     int dh, int dw, int canvas_h, int canvas_w, cudaStream_t s);
+// One page of a batch of pages of different sizes (ctd_submit_pages): u8 BGR source at byte `src_off` of the packed
+// pages, letterboxed to unpad_h x unpad_w; its page-sized mask starts at byte `dst_off` of the packed mask planes and
+// owns rows [row0, row0 + ih) of the batch's stacked mask rows.
+struct PageGeom {
+  long long src_off, dst_off;
+  int ih, iw, unpad_h, unpad_w, row0, pad;
+};
+// The same resize as resize_linear_u8_launch for every page of a batch in one launch each: the letterbox of page p
+// into dst[p] (n x net_h x net_w x 3), and the back-projection of mask[p][:unpad_h, :unpad_w] (n x net_h x net_w u8)
+// to ih x iw at dst + dst_off.  total_rows = the sum of ih.
+cudaError_t letterbox_batch_launch(const uint8_t* src, const PageGeom* d_tab, int n, uint8_t* dst, int net_h, int net_w,
+                                   cudaStream_t s);
+cudaError_t backproject_batch_launch(const uint8_t* mask, int net_h, int net_w, const PageGeom* d_tab, int n,
+                                     int total_rows, uint8_t* dst, cudaStream_t s);
 
 // refine_mask (refine_mk.cu): one kernel per phase over the window pixels of all pages of a batch, one CTA per chunk.
 struct RefineWin {
   int x1, y1, x2, y2;     // window (python slice semantics: rows y1..y2-1, cols x1..x2-1)
   long long off;          // pixel offset of this window's planes inside each scratch plane (a multiple of 4)
-  int page;               // page of the batch the window belongs to
+  long long page_off;     // pixel offset of the window's page in the mask / mask_refined planes (x3 in the image)
+  int pitch;              // width of that page = its row pitch in pixels
 };
 // Pixels [i0, i0 + rows * cols) of the window planes, i0 = y0 * rw + x0, cols = min(rw - x0, kRefineChunkPx).  A
 // window of width rw <= kRefineChunkPx is cut into chunks of whole rows (x0 = 0, cols = rw); a wider window into row
@@ -210,8 +225,9 @@ constexpr int kRefineChunkPx = 8192;
 size_t refine_scratch_bytes(size_t total_px);
 // d_state: refine_mk_state_bytes(n_wins) bytes of per-window state
 size_t refine_mk_state_bytes(int n_wins);
-// the first n_multi_chunks records of d_chunks are the chunks of windows that span more than one chunk
-cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, int H, int W, const RefineWin* d_wins, int n_wins,
+// the first n_multi_chunks records of d_chunks are the chunks of windows that span more than one chunk.  The pages
+// are located by each window's page_off / pitch; d_out must be 4-byte aligned.
+cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const RefineWin* d_wins, int n_wins,
                              const RefineChunk* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
                              void* scratch, int refine_mode, uint8_t* d_out, cudaStream_t s);
 

@@ -10,9 +10,12 @@
 // for the pages of the batch on a few host threads and enqueues phase C on a second stream, so the host stage and
 // the refine kernels of batch i overlap the forward of batch i+1.  ctd_detect_page is the blocking single-page form
 // for pages of any size (letterbox + back-projection on the GPU), the call behind the drop-in TextDetector.
+// ctd_submit_pages runs batches of pages of any size through the same two-in-flight schedule, with one letterbox and
+// one back-projection launch per batch (TextDetector.detect_batch / detect_stream).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math.h>
+#include <stdint.h>
 #include <string.h>
 
 #include <algorithm>
@@ -41,7 +44,7 @@ inline void norm_slice(int& lo, int& hi, int n) {
 }
 }  // namespace
 
-void RefineJob::add(int x1, int y1, int x2, int y2, int page, int iw, int ih) {
+void RefineJob::add(int x1, int y1, int x2, int y2, size_t page_off, int iw, int ih) {
   norm_slice(x1, x2, iw);
   norm_slice(y1, y2, ih);
   const size_t a = (x2 > x1 && y2 > y1) ? size_t(x2 - x1) * (y2 - y1) : 0;
@@ -53,7 +56,7 @@ void RefineJob::add(int x1, int y1, int x2, int y2, int page, int iw, int ih) {
   if (rows_per >= 8) rows_per &= ~3;   // chunk starts on multiples of 4 rows -> 4-byte aligned in the window planes
   for (int y0 = 0; y0 < rh; y0 += rows_per)
     for (int x0 = 0; x0 < rw; x0 += kRefineChunkPx) chunks.push_back(RefineChunk{wi, y0, x0, std::min(rows_per, rh - y0)});
-  wins.push_back(RefineWin{x1, y1, x2, y2, (long long)total_px, page});
+  wins.push_back(RefineWin{x1, y1, x2, y2, (long long)total_px, (long long)page_off, iw});
   total_px = (total_px + a + 3) / 4 * 4;
 }
 size_t RefineJob::table_bytes() const {
@@ -61,25 +64,27 @@ size_t RefineJob::table_bytes() const {
   return al(wins.size() * sizeof(RefineWin)) + al(chunks.size() * sizeof(RefineChunk));
 }
 
-// uploads the window tables of `job` into the (grown on demand) refine scratch and launches the refine kernels:
-// d_img / d_mask / d_out are device planes of `ih*iw` pixels per page.  Stream-ordered on `st`; `pinned` (optional)
-// is a host staging buffer of >= job.table_bytes() bytes that stays valid until the copy has executed.
-int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int ih, int iw,
-                  int refine_mode, uint8_t* d_out, cudaStream_t st, char* pinned) {
+// uploads the window tables of `job` into the refine scratch *scratch / *cap and launches the refine kernels:
+// d_img / d_mask / d_out are device planes holding each window's page at its page_off.  Stream-ordered on `st`, the
+// only stream that may use that scratch (it is grown here after synchronising `st`): the caller's calls use
+// h->d_refine_scratch on h->stream, the pipeline worker h->d_post_refine on h->post.  `pinned` (optional) is a host
+// staging buffer of >= job.table_bytes() bytes that stays valid until the copy has executed.
+int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int refine_mode,
+                  uint8_t* d_out, cudaStream_t st, void** scratch, size_t* cap, char* pinned) {
   if (job.wins.empty()) return CTD_OK;
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t tb = job.table_bytes();   // a multiple of 256
   const size_t sb = refine_mk_state_bytes(int(job.wins.size()));
   const size_t need = tb + sb + refine_scratch_bytes(job.total_px);
-  if (need > h->refine_scratch_cap) {
-    CK(cudaDeviceSynchronize());         // the old scratch may still be in use by an earlier launch
-    cudaFree(h->d_refine_scratch);
-    h->d_refine_scratch = nullptr;
-    h->refine_scratch_cap = 0;
-    CK(cudaMalloc(&h->d_refine_scratch, need + need / 2));
-    h->refine_scratch_cap = need + need / 2;
+  if (need > *cap) {
+    CK(cudaStreamSynchronize(st));       // the old scratch may still be in use by an earlier launch on `st`
+    cudaFree(*scratch);
+    *scratch = nullptr;
+    *cap = 0;
+    CK(cudaMalloc(scratch, need + need / 2));
+    *cap = need + need / 2;
   }
-  char* base = static_cast<char*>(h->d_refine_scratch);
+  char* base = static_cast<char*>(*scratch);
   const size_t wb = al(job.wins.size() * sizeof(RefineWin));
   std::vector<char> local;
   char* stage = pinned;
@@ -105,7 +110,7 @@ int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, con
   }
   CK(cudaMemcpyAsync(base, stage, tb, cudaMemcpyHostToDevice, st));
   if (!pinned) CK(cudaStreamSynchronize(st));   // pageable staging dies with this frame
-  CK(refine_mk_launch(d_img, d_mask, ih, iw, reinterpret_cast<const RefineWin*>(base), int(job.wins.size()),
+  CK(refine_mk_launch(d_img, d_mask, reinterpret_cast<const RefineWin*>(base), int(job.wins.size()),
                       reinterpret_cast<const RefineChunk*>(base + wb), int(job.chunks.size()), n_multi, base + tb,
                       job.total_px, base + tb + sb, refine_mode, d_out, st));
   return CTD_OK;
@@ -126,7 +131,9 @@ extern "C" int ctd_refine_mask(ctd_handle* h, const uint8_t* img, const uint8_t*
   CK(cudaMemcpyAsync(d_img, img, px * 3, cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(d_mask, mask, px, cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemsetAsync(d_out, 0, pxa, h->stream));
-  if (int rc = launch_refine(h, job, d_img, d_mask, ih, iw, refine_mode, d_out, h->stream, nullptr)) return rc;
+  if (int rc = launch_refine(h, job, d_img, d_mask, refine_mode, d_out, h->stream, &h->d_refine_scratch,
+                             &h->refine_scratch_cap, nullptr))
+    return rc;
   CK(cudaMemcpyAsync(out, d_out, px, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return CTD_OK;
@@ -144,7 +151,7 @@ struct PageIn {
 
 // inference.py:101-114 (postprocess_yolo casts), 158-172 (box_thresh, line rescale), textblock.group_output,
 // expand_textwindow(.., 16): fills the page's block section and appends its refine windows
-int host_group_page(const PageIn& in, char* section, const ArenaLayout& L, std::vector<int32_t>& win_out) {
+int host_group_page(const PageIn& in, char* section, const BlockSection& L, std::vector<int32_t>& win_out) {
   std::vector<int32_t> bxy(size_t(in.n_det) * 4), bcls(size_t(in.n_det));
   for (int i = 0; i < in.n_det; ++i) {
     const float* d = in.det + 6 * i;
@@ -202,6 +209,138 @@ int host_group_page(const PageIn& in, char* section, const ArenaLayout& L, std::
   }
   return CTD_OK;
 }
+
+// fn(i) for the n pages of a batch, on up to `threads` host threads
+template <typename F>
+void for_each_page(int n, int threads, F fn) {
+  const int nthreads = std::max(1, std::min(n, threads));
+  if (nthreads == 1) {
+    for (int i = 0; i < n; ++i) fn(i);
+    return;
+  }
+  std::vector<std::thread> th;
+  for (int t = 0; t < nthreads; ++t)
+    th.emplace_back([&, t] { for (int i = t; i < n; i += nthreads) fn(i); });
+  for (auto& x : th) x.join();
+}
+
+__global__ void undetected_prep_kernel(uint8_t* __restrict__ mask, const uint8_t* __restrict__ refined,
+                                       uint8_t* __restrict__ thr, size_t n) {
+  // mask_pred[mask_refined > 30] = 0; cv2.threshold(mask_pred, 30, 255, THRESH_BINARY)  (textmask.py:136-137)
+  const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  uint8_t m = mask[i];
+  if (refined[i] > 30) { m = 0; mask[i] = 0; }
+  thr[i] = m > 30 ? 255 : 0;
+}
+__global__ void or_kernel(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, size_t n) {
+  const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
+  if (i < n) dst[i] |= src[i];
+}
+
+// one page of refine_undetected: its planes start at pixel `off` (x3 in the image); rec[0..nb) its blocks
+struct UndetPage {
+  size_t off;
+  int ih, iw;
+  const ctd_block* rec;
+  int nb;
+};
+
+// refine_undetected_mask (textmask.py:135-156) for a set of pages whose planes lie in [0, total_px) of d_mask, d_ref
+// (mask_refined), d_ref2 and d_thr (and x3 of d_img): one prep launch over all planes, connected components + stats of
+// each page on `st` (the scratch *cc / *cc_cap grows here), the host loop over each page's stats rows, then one refine
+// launch for the extra windows of all pages (refine scratch *refine_scratch / *refine_cap) and one OR launch.  The
+// masks are modified in place, as in the reference.
+// Synchronises `st` once for the label counts and once for the stats rows.
+int refine_undetected(ctd_handle* h, const std::vector<UndetPage>& pages, size_t total_px, const uint8_t* d_img,
+                      uint8_t* d_mask, uint8_t* d_ref, uint8_t* d_ref2, uint8_t* d_thr, int refine_mode, cudaStream_t st,
+                      void** cc, size_t* cc_cap, void** refine_scratch, size_t* refine_cap, char* pinned,
+                      size_t pinned_cap) {
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  const int n = int(pages.size());
+  undetected_prep_kernel<<<unsigned((total_px + 255) / 256), 256, 0, st>>>(d_mask, d_ref, d_thr, total_px);
+  CK(cudaGetLastError());
+  // scratch: labels | 3 ints/px of CCL scratch for the largest page (reused page after page) | one stats table per
+  // page (worst case of 8-connected components + background) | the label counts
+  size_t max_px = 0;
+  std::vector<int> cap(static_cast<size_t>(n));
+  std::vector<size_t> stats_off(static_cast<size_t>(n));
+  for (int i = 0; i < n; ++i) max_px = std::max(max_px, size_t(pages[i].ih) * pages[i].iw);
+  const size_t o_scr = al(max_px * 4);
+  size_t o = o_scr + al(max_px * 12);
+  for (int i = 0; i < n; ++i) {
+    cap[size_t(i)] = ((pages[i].ih + 1) / 2) * ((pages[i].iw + 1) / 2) + 2;
+    stats_off[size_t(i)] = o;
+    o += al(size_t(cap[size_t(i)]) * 5 * 4);
+  }
+  const size_t o_nl = o, need = o_nl + al(size_t(n) * 4);
+  if (need > *cc_cap) {
+    CK(cudaStreamSynchronize(st));
+    cudaFree(*cc);
+    *cc = nullptr;
+    *cc_cap = 0;
+    CK(cudaMalloc(cc, need + need / 4));
+    *cc_cap = need + need / 4;
+  }
+  uint8_t* base = static_cast<uint8_t*>(*cc);
+  int32_t* d_labels = reinterpret_cast<int32_t*>(base);
+  int32_t* d_scr = reinterpret_cast<int32_t*>(base + o_scr);
+  int32_t* d_nl = reinterpret_cast<int32_t*>(base + o_nl);
+  for (int i = 0; i < n; ++i) {
+    const UndetPage& p = pages[size_t(i)];
+    int32_t* d_stats = reinterpret_cast<int32_t*>(base + stats_off[size_t(i)]);
+    CK(ccl_launch(d_thr + p.off, 1, p.ih, p.iw, d_labels, d_scr, d_nl + i, st));
+    CK(ccl_stats_launch(d_labels, p.ih, p.iw, d_stats, cap[size_t(i)], st));
+  }
+  std::vector<int32_t> n_lab(static_cast<size_t>(n));
+  CK(cudaMemcpyAsync(n_lab.data(), d_nl, size_t(n) * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  std::vector<std::vector<int32_t>> stats(static_cast<size_t>(n));
+  for (int i = 0; i < n; ++i) {
+    stats[size_t(i)].resize(size_t(std::max(n_lab[size_t(i)], 0)) * 5);
+    if (n_lab[size_t(i)] > 0)
+      CK(cudaMemcpyAsync(stats[size_t(i)].data(), base + stats_off[size_t(i)], stats[size_t(i)].size() * 4,
+                         cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaStreamSynchronize(st));
+  RefineJob rj2;
+  for (int i = 0; i < n; ++i) {
+    const UndetPage& p = pages[size_t(i)];
+    bool first_valid = true;
+    for (int li = 0; li < n_lab[size_t(i)]; ++li) {
+      const int32_t* s5 = &stats[size_t(i)][size_t(li) * 5];
+      if (!(s5[4] > 50)) continue;
+      if (first_valid) { first_valid = false; continue; }        // valid_labels[1:]
+      const int64_t bb[4] = {s5[0], s5[1], int64_t(s5[0]) + s5[2], int64_t(s5[1]) + s5[3]};
+      int64_t score = -1;
+      for (int b = 0; b < p.nb; ++b) {
+        const int32_t* q = p.rec[b].xyxy;
+        const int64_t x1 = std::max<int64_t>(q[0], bb[0]), y1 = std::max<int64_t>(q[1], bb[1]);
+        const int64_t x2 = std::min<int64_t>(q[2], bb[2]), y2 = std::min<int64_t>(q[3], bb[3]);
+        const int64_t a = (y2 < y1 || x2 < x1) ? -1 : (y2 - y1) * (x2 - x1);
+        if (a > score) score = a;
+      }
+      if (double(score) / double(s5[2]) / double(s5[3]) < 0.5) {
+        int32_t xy[4] = {int32_t(bb[0]), int32_t(bb[1]), int32_t(bb[2]), int32_t(bb[3])}, w4[4];
+        const int64_t w = bb[2] - bb[0], hh = bb[3] - bb[1];
+        const int64_t pad = int64_t(nearbyint((double(std::max(hh, w)) * 0.25 + double(std::min(hh, w)) * 0.75) / 16.0));
+        w4[0] = int32_t(std::max<int64_t>(0, xy[0] - pad)); w4[1] = int32_t(std::max<int64_t>(0, xy[1] - pad));
+        w4[2] = int32_t(std::min<int64_t>(p.iw - 1, xy[2] + pad)); w4[3] = int32_t(std::min<int64_t>(p.ih - 1, xy[3] + pad));
+        rj2.add(w4[0], w4[1], w4[2], w4[3], p.off, p.iw, p.ih);
+      }
+    }
+  }
+  if (!rj2.wins.empty()) {
+    CK(cudaMemsetAsync(d_ref2, 0, total_px, st));
+    // the stream is idle here, so the pinned staging of an earlier launch is free again
+    char* stage = rj2.table_bytes() <= pinned_cap ? pinned : nullptr;
+    if (int rc = launch_refine(h, rj2, d_img, d_mask, refine_mode, d_ref2, st, refine_scratch, refine_cap, stage))
+      return rc;
+    or_kernel<<<unsigned((total_px + 255) / 256), 256, 0, st>>>(d_ref, d_ref2, total_px);
+    CK(cudaGetLastError());
+  }
+  return CTD_OK;
+}
 }  // namespace
 
 extern "C" int ctd_results_layout(ctd_handle* h, ctd_results_layout_t* out) {
@@ -214,6 +353,120 @@ extern "C" int ctd_results_layout(ctd_handle* h, ctd_results_layout_t* out) {
   out->phase_a_bytes = L.a_bytes;
   out->mask_refined = L.refined; out->blocks = L.blocks; out->blocks_stride = L.blocks_stride;
   out->blk_records_off = L.rec_off; out->blk_lines_off = L.lines_off; out->blk_dist_off = L.dist_off;
+  return CTD_OK;
+}
+
+// ---- pages of any size: batch layout ---------------------------------------------------------------------------------
+PagesHead pages_head(int n) {
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  const size_t nb = size_t(n);
+  PagesHead hd;
+  hd.det = 0;
+  hd.cnt = hd.det + al(nb * 300 * 6 * 4);
+  hd.lb = hd.cnt + al(nb * 4);
+  hd.ls = hd.lb + al(nb * 1000 * 8 * 2);
+  hd.lc = hd.ls + al(nb * 1000 * 4);
+  hd.masks = hd.lc + al(nb * 4);
+  return hd;
+}
+
+// Results buffer: pages_head(n) | masks | mask_refined planes | block sections.  Page i's pixel offset P_i (the sum of
+// the earlier pages' pixels, each rounded up to 256) is the same in every plane: image bytes at 3 P_i, mask at
+// masks + P_i, mask_refined at masks + P + P_i (P = the sum over the batch), so refine_mask addresses the image and the
+// mask planes of a page with one offset.
+extern "C" int ctd_pages_plan(ctd_page_entry* pages, int32_t n, int32_t net_h, int32_t net_w, size_t* input_bytes,
+                              size_t* results_bytes) {
+  if (!input_bytes || !results_bytes || n < 0 || (n > 0 && !pages)) return CTD_E_INVALID;
+  if (net_h < 64 || net_w < 64 || net_h % 64 || net_w % 64) return CTD_E_SHAPE;
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  const PagesHead hd = pages_head(n);
+  size_t total = 0;
+  for (int i = 0; i < n; ++i) {
+    Letterbox lb;
+    if (!letterbox_of(pages[i].ih, pages[i].iw, net_h, net_w, lb)) return CTD_E_SHAPE;
+    pages[i].unpad_h = lb.unpad_h;
+    pages[i].unpad_w = lb.unpad_w;
+    pages[i].page_off = int64_t(total * 3);
+    pages[i].mask_off = int64_t(hd.masks + total);
+    total += al(size_t(pages[i].ih) * size_t(pages[i].iw));
+  }
+  const size_t stride = al(block_section_layout().stride);
+  const size_t blocks = hd.masks + 2 * total;
+  for (int i = 0; i < n; ++i) {
+    pages[i].refined_off = pages[i].mask_off + int64_t(total);
+    pages[i].blocks_off = int64_t(blocks + size_t(i) * stride);
+  }
+  *input_bytes = total * 3;
+  *results_bytes = blocks + size_t(n) * stride;
+  return CTD_OK;
+}
+
+// phases B and C of a ctd_submit_pages batch, on the worker thread
+static int run_pages_job(ctd_handle* h, const PipeJob& job) {
+  const int slot = job.slot, n = job.n;
+  CK(cudaEventSynchronize(h->ev_out_done[slot]));          // phase A results are in results_host
+  char* res = static_cast<char*>(job.results_host);
+  const PagesHead hd = pages_head(n);
+  const BlockSection bs = block_section_layout();
+  const std::vector<ctd_page_entry>& pg = job.pages;
+  const int32_t* det_cnt = reinterpret_cast<const int32_t*>(res + hd.cnt);
+  const int32_t* line_cnt = reinterpret_cast<const int32_t*>(res + hd.lc);
+  std::vector<std::vector<int32_t>> wins(static_cast<size_t>(n));
+  std::vector<int> prc(size_t(n), CTD_OK);
+  for_each_page(n, h->host_threads, [&](int i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    Letterbox lb;
+    letterbox_of(e.ih, e.iw, job.ph, job.pw, lb);   // planned: cannot fail
+    PageIn in;
+    in.det = reinterpret_cast<const float*>(res + hd.det) + size_t(i) * 300 * 6;
+    in.n_det = std::min(std::max(det_cnt[i], 0), 300);
+    in.line_boxes = reinterpret_cast<const int16_t*>(res + hd.lb) + size_t(i) * 1000 * 8;
+    in.line_scores = reinterpret_cast<const float*>(res + hd.ls) + size_t(i) * 1000;
+    in.n_lines = std::min(std::max(line_cnt[i], 0), 1000);
+    in.mask = reinterpret_cast<const uint8_t*>(res + e.mask_off);
+    in.im_w = e.iw; in.im_h = e.ih; in.ratio_x = lb.ratio_x; in.ratio_y = lb.ratio_y;
+    prc[size_t(i)] = host_group_page(in, res + e.blocks_off, bs, wins[size_t(i)]);
+  });
+  for (int i = 0; i < n; ++i)
+    if (prc[size_t(i)] != CTD_OK) return ctd_fail(h, prc[size_t(i)], "group_output failed on page %d of the batch", i);
+  RefineJob rj;
+  for (int i = 0; i < n; ++i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    for (size_t k = 0; k + 3 < wins[size_t(i)].size(); k += 4)
+      rj.add(wins[size_t(i)][k], wins[size_t(i)][k + 1], wins[size_t(i)][k + 2], wins[size_t(i)][k + 3],
+             size_t(e.mask_off) - hd.masks, e.iw, e.ih);
+  }
+  // phase C on the post stream over the slot's resident pages and masks
+  cudaStream_t st = h->post;
+  // enqueued here, not at submit: a wait enqueued at submit time would also hold this batch's phase C behind the
+  // forward of every batch submitted before the worker reached it
+  CK(cudaStreamWaitEvent(st, h->ev_out_ready[slot], 0));   // phase C never starts before its phase A copy
+  const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);   // pixels of all planes of the batch
+  uint8_t* d_res = h->d_pg_res[slot];
+  uint8_t* d_mask = d_res + hd.masks;
+  uint8_t* d_ref = d_res + pg[0].refined_off;
+  CK(cudaMemsetAsync(d_ref, 0, total, st));
+  char* stage_tab = rj.table_bytes() <= h->pipe_pinned_cap ? h->pipe_pinned[slot] : nullptr;   // else: pageable + sync
+  if (int rc = launch_refine(h, rj, h->d_pg_in[slot], d_mask, job.refine_mode, d_ref, st, &h->d_post_refine,
+                             &h->post_refine_cap, stage_tab))
+    return rc;
+  if (job.keep_undetected) {
+    std::vector<UndetPage> up(static_cast<size_t>(n));
+    for (int i = 0; i < n; ++i) {
+      const ctd_page_entry& e = pg[size_t(i)];
+      const ctd_page_blocks* hdr = reinterpret_cast<const ctd_page_blocks*>(res + e.blocks_off);
+      up[size_t(i)] = UndetPage{size_t(e.mask_off) - hd.masks, e.ih, e.iw,
+                                reinterpret_cast<const ctd_block*>(res + e.blocks_off + bs.rec_off), hdr->n_blocks};
+    }
+    uint8_t* d_ref2 = h->d_pg_aux[slot];
+    if (int rc = refine_undetected(h, up, total, h->d_pg_in[slot], d_mask, d_ref, d_ref2, d_ref2 + total, job.refine_mode,
+                                   st, &h->d_pg_cc, &h->pg_cc_cap, &h->d_post_refine, &h->post_refine_cap,
+                                   h->pipe_pinned[slot], h->pipe_pinned_cap))
+      return rc;
+    CK(cudaMemcpyAsync(res + hd.masks, d_mask, total, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaMemcpyAsync(res + pg[0].refined_off, d_ref, total, cudaMemcpyDeviceToHost, st));
+  CK(cudaEventRecord(h->ev_post_done[slot], st));
   return CTD_OK;
 }
 
@@ -251,23 +504,17 @@ static void pipe_worker(ctd_handle* h) {
         in.n_lines = std::min(std::max(line_cnt[i], 0), 1000);
         in.mask = reinterpret_cast<const uint8_t*>(res) + size_t(i) * px;
         in.im_w = pw; in.im_h = ph; in.ratio_x = 1.f; in.ratio_y = 1.f;
-        prc[size_t(i)] = host_group_page(in, res + L.blocks + size_t(i) * L.blocks_stride, L, wins[size_t(i)]);
+        prc[size_t(i)] = host_group_page(in, res + L.blocks + size_t(i) * L.blocks_stride, block_section_layout(),
+                                         wins[size_t(i)]);
       };
-      const int nthreads = std::max(1, std::min(n, h->host_threads));
-      if (nthreads == 1) {
-        for (int i = 0; i < n; ++i) one(i);
-      } else {
-        std::vector<std::thread> th;
-        for (int t = 0; t < nthreads; ++t)
-          th.emplace_back([&, t] { for (int i = t; i < n; i += nthreads) one(i); });
-        for (auto& x : th) x.join();
-      }
+      for_each_page(n, h->host_threads, one);
       for (int i = 0; i < n; ++i)
         if (prc[size_t(i)] != CTD_OK) return ctd_fail(h, prc[size_t(i)], "group_output failed on page %d of the batch", i);
       RefineJob rj;
       for (int i = 0; i < n; ++i)
         for (size_t k = 0; k + 3 < wins[size_t(i)].size(); k += 4)
-          rj.add(wins[size_t(i)][k], wins[size_t(i)][k + 1], wins[size_t(i)][k + 2], wins[size_t(i)][k + 3], i, pw, ph);
+          rj.add(wins[size_t(i)][k], wins[size_t(i)][k + 1], wins[size_t(i)][k + 2], wins[size_t(i)][k + 3],
+                 size_t(i) * ph * pw, pw, ph);
       // phase C on the post stream: block sections to the device arena copy (one gather then moves everything),
       // refine on the resident pages + mask, mask_refined back to the host
       cudaStream_t st = h->post;
@@ -276,13 +523,14 @@ static void pipe_worker(ctd_handle* h) {
       CK(cudaMemsetAsync(d_arena + L.refined, 0, size_t(n) * px, st));
       char* stage_tab = rj.table_bytes() <= h->pipe_pinned_cap ? h->pipe_pinned[slot] : nullptr;   // else: pageable + sync
       const uint8_t* d_pages = job.pages_dev ? job.pages_dev : h->d_stage_in[slot];
-      if (int r2 = launch_refine(h, rj, d_pages, d_arena, ph, pw, job.refine_mode, d_arena + L.refined, st, stage_tab))
+      if (int r2 = launch_refine(h, rj, d_pages, d_arena, job.refine_mode, d_arena + L.refined, st, &h->d_post_refine,
+                                 &h->post_refine_cap, stage_tab))
         return r2;
       CK(cudaMemcpyAsync(res + L.refined, d_arena + L.refined, size_t(n) * px, cudaMemcpyDeviceToHost, st));
       CK(cudaEventRecord(h->ev_post_done[slot], st));
       return CTD_OK;
     };
-    rc = run();
+    rc = job.pages.empty() ? run() : run_pages_job(h, job);
     if (rc != CTD_OK) err = h->err;
     {
       std::lock_guard<std::mutex> lk(h->pipe_mu);
@@ -302,7 +550,8 @@ static int ensure_full_pipeline(ctd_handle* h) {
   CK(cudaStreamCreateWithPriority(&h->post, cudaStreamNonBlocking, hi));
   // window tables: <= CTD_MAX_BLOCKS windows per page (32 bytes each) and <= area / chunk + rows chunks per window
   // (16 bytes each)
-  h->pipe_pinned_cap = size_t(h->cfg.max_batch) * (size_t(CTD_MAX_BLOCKS) * 32 + size_t(CTD_MAX_BLOCKS) * 16 * 8) + (size_t(8) << 20);
+  h->pipe_pinned_cap = size_t(h->cfg.max_batch) * (size_t(CTD_MAX_BLOCKS) * sizeof(RefineWin) +
+                                                   size_t(CTD_MAX_BLOCKS) * sizeof(RefineChunk) * 8) + (size_t(8) << 20);
   for (int i = 0; i < 2; ++i) {
     CK(cudaHostAlloc(reinterpret_cast<void**>(&h->pipe_pinned[i]), h->pipe_pinned_cap, cudaHostAllocDefault));
     CK(cudaEventCreateWithFlags(&h->ev_post_done[i], cudaEventDisableTiming));
@@ -332,6 +581,20 @@ void ctd_pipeline_shutdown(ctd_handle* h) {
   }
   if (h->post) cudaStreamDestroy(h->post);
   h->post = nullptr;
+  for (int i = 0; i < 2; ++i) {
+    cudaFree(h->d_pg_in[i]); cudaFree(h->d_pg_res[i]); cudaFree(h->d_pg_aux[i]); cudaFree(h->d_pg_tab[i]);
+    if (h->h_pg_tab[i]) cudaFreeHost(h->h_pg_tab[i]);
+    h->d_pg_in[i] = h->d_pg_res[i] = h->d_pg_aux[i] = nullptr;
+    h->pg_in_cap[i] = h->pg_res_cap[i] = h->pg_aux_cap[i] = 0;
+    h->d_pg_tab[i] = nullptr;
+    h->h_pg_tab[i] = nullptr;
+  }
+  cudaFree(h->d_pg_cc);
+  h->d_pg_cc = nullptr;
+  h->pg_cc_cap = 0;
+  cudaFree(h->d_post_refine);
+  h->d_post_refine = nullptr;
+  h->post_refine_cap = 0;
 }
 
 extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages, int32_t n, int32_t ph, int32_t pw,
@@ -379,7 +642,95 @@ extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages
   return CTD_OK;
 }
 
-// called by ctd_collect for slots submitted with ctd_submit_full
+// device buffer of a slot, grown (never shrunk) to `bytes`; only called while the slot is idle
+static int grow_slot_buffer(ctd_handle* h, uint8_t** buf, size_t* cap, size_t bytes) {
+  if (bytes <= *cap) return CTD_OK;
+  cudaFree(*buf);
+  *buf = nullptr;
+  *cap = 0;
+  CK(cudaMalloc(reinterpret_cast<void**>(buf), bytes + bytes / 4));
+  *cap = bytes + bytes / 4;
+  return CTD_OK;
+}
+
+extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                                int32_t net_w, const uint8_t* input_host, int32_t refine_mode, int32_t keep_undetected,
+                                void* results_host) {
+  if (!h || !pages || !input_host || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit_pages needs the full pipeline");
+  if (h->slot_busy[slot]) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
+  // the offsets decide where the copies write: they must be the plan's
+  std::vector<ctd_page_entry> pg(pages, pages + n);
+  size_t in_bytes = 0, res_bytes = 0;
+  if (int rc = ctd_pages_plan(pg.data(), n, net_h, net_w, &in_bytes, &res_bytes))
+    return ctd_fail(h, rc, "the pages do not letterbox into a %dx%d net input", net_h, net_w);
+  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
+    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_pages_plan returns");
+  size_t rows = 0;
+  for (int i = 0; i < n; ++i) rows += size_t(pg[size_t(i)].ih);
+  if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
+  ShapePlan* sp = nullptr;
+  if (int rc = prepare_forward(h, n, net_h, net_w, &sp)) return rc;
+  if (int rc = ensure_full_pipeline(h)) return rc;
+  const ArenaLayout& L = h->layout;
+  const PagesHead hd = pages_head(n);
+  const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);
+  const size_t d2h = size_t(pg[0].refined_off);                       // phase-A rows + masks
+  if (int rc = grow_slot_buffer(h, &h->d_pg_in[slot], &h->pg_in_cap[slot], in_bytes)) return rc;
+  if (int rc = grow_slot_buffer(h, &h->d_pg_res[slot], &h->pg_res_cap[slot], d2h + total)) return rc;
+  if (keep_undetected)
+    if (int rc = grow_slot_buffer(h, &h->d_pg_aux[slot], &h->pg_aux_cap[slot], 2 * total)) return rc;
+  if (!h->h_pg_tab[slot]) {
+    CK(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pg_tab[slot]), size_t(h->cfg.max_batch) * sizeof(PageGeom),
+                     cudaHostAllocDefault));
+    CK(cudaMalloc(reinterpret_cast<void**>(&h->d_pg_tab[slot]), size_t(h->cfg.max_batch) * sizeof(PageGeom)));
+  }
+  PageGeom* tab = h->h_pg_tab[slot];
+  int row0 = 0;
+  for (int i = 0; i < n; ++i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    tab[i] = PageGeom{e.page_off, e.mask_off - int64_t(hd.masks), e.ih, e.iw, e.unpad_h, e.unpad_w, row0, 0};
+    row0 += e.ih;
+  }
+  // phase A: pages and table in on copy_in; letterbox, forward, back-projection and the phase-A rows on the engine
+  // stream; rows + masks out on copy_out
+  CK(cudaMemcpyAsync(h->d_pg_tab[slot], tab, size_t(n) * sizeof(PageGeom), cudaMemcpyHostToDevice, h->copy_in));
+  CK(cudaMemcpyAsync(h->d_pg_in[slot], input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
+  CK(cudaEventRecord(h->ev_in_done[slot], h->copy_in));
+  CK(cudaEventRecord(h->ev0, h->stream));
+  CK(cudaStreamWaitEvent(h->stream, h->ev_in_done[slot], 0));
+  CK(letterbox_batch_launch(h->d_pg_in[slot], h->d_pg_tab[slot], n, h->d_pages, net_h, net_w, h->stream));
+  if (int rc = enqueue_forward(h, n, net_h, net_w, *sp)) return rc;
+  uint8_t* d_res = h->d_pg_res[slot];
+  CK(backproject_batch_launch(h->d_mask_u8, net_h, net_w, h->d_pg_tab[slot], n, row0, d_res + hd.masks, h->stream));
+  const size_t nb = size_t(n);
+  CK(cudaMemcpyAsync(d_res + hd.det, h->d_mask_u8 + L.det, nb * 300 * 6 * 4, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaMemcpyAsync(d_res + hd.cnt, h->d_mask_u8 + L.cnt, nb * 4, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaMemcpyAsync(d_res + hd.lb, h->d_mask_u8 + L.lb, nb * 1000 * 8 * 2, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaMemcpyAsync(d_res + hd.ls, h->d_mask_u8 + L.ls, nb * 1000 * 4, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaMemcpyAsync(d_res + hd.lc, h->d_mask_u8 + L.lc, nb * 4, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaEventRecord(h->ev_out_ready[slot], h->stream));
+  CK(cudaStreamWaitEvent(h->copy_out, h->ev_out_ready[slot], 0));
+  CK(cudaMemcpyAsync(results_host, d_res, d2h, cudaMemcpyDeviceToHost, h->copy_out));
+  CK(cudaEventRecord(h->ev_out_done[slot], h->copy_out));
+  {
+    std::lock_guard<std::mutex> lk(h->pipe_mu);
+    PipeJob job;
+    job.slot = slot; job.n = n; job.ph = net_h; job.pw = net_w; job.refine_mode = refine_mode;
+    job.results_host = results_host;
+    job.pages = std::move(pg);
+    job.keep_undetected = keep_undetected ? 1 : 0;
+    h->pipe_state[slot] = 1;
+    h->pipe_queue.push_back(std::move(job));
+  }
+  h->pipe_cv.notify_one();
+  h->slot_busy[slot] = true;
+  h->slot_full[slot] = true;
+  return CTD_OK;
+}
+
+// called by ctd_collect for slots submitted with ctd_submit_full or ctd_submit_pages
 int ctd_collect_full(ctd_handle* h, int slot) {
   int rc;
   {
@@ -404,22 +755,6 @@ extern "C" int ctd_device_arena(ctd_handle* h, int32_t slot, void** base, void**
 }
 
 // ---- single page, any size --------------------------------------------------------------------------------------------
-namespace {
-__global__ void undetected_prep_kernel(uint8_t* __restrict__ mask, const uint8_t* __restrict__ refined,
-                                       uint8_t* __restrict__ thr, size_t n) {
-  // mask_pred[mask_refined > 30] = 0; cv2.threshold(mask_pred, 30, 255, THRESH_BINARY)  (textmask.py:136-137)
-  const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  uint8_t m = mask[i];
-  if (refined[i] > 30) { m = 0; mask[i] = 0; }
-  thr[i] = m > 30 ? 255 : 0;
-}
-__global__ void or_kernel(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, size_t n) {
-  const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
-  if (i < n) dst[i] |= src[i];
-}
-}  // namespace
-
 extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t net_h, int32_t net_w,
                                int32_t refine_mode, int32_t keep_undetected, uint8_t* mask_out, uint8_t* mask_refined_out,
                                ctd_block* blocks, int32_t blocks_cap, int32_t* lines_out, int32_t lines_cap, double* dist_out,
@@ -427,11 +762,8 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   if (!h || !page || !mask_out || !mask_refined_out || !n_blocks) return CTD_E_INVALID;
   if (ih < 1 || iw < 1) return ctd_fail(h, CTD_E_SHAPE, "bad page size %dx%d", ih, iw);
   *n_blocks = 0;
-  // letterbox geometry (imgproc_utils.py:86-117 with auto=False; python round = half to even)
-  const double r = std::min(double(net_h) / ih, double(net_w) / iw);
-  const int unpad_w = int(nearbyint(iw * r)), unpad_h = int(nearbyint(ih * r));
-  const int dw = net_w - unpad_w, dh = net_h - unpad_h;
-  if (unpad_w < 1 || unpad_h < 1 || dw < 0 || dh < 0) return ctd_fail(h, CTD_E_SHAPE, "page does not letterbox into the net input");
+  Letterbox geo;
+  if (!letterbox_of(ih, iw, net_h, net_w, geo)) return ctd_fail(h, CTD_E_SHAPE, "page does not letterbox into the net input");
   ShapePlan* sp = nullptr;
   if (int rc = prepare_forward(h, 1, net_h, net_w, &sp)) return rc;
   const size_t px = size_t(ih) * iw, pxa = (px + 255) / 256 * 256;
@@ -447,11 +779,11 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   CK(cudaMemcpyAsync(d_page, page, px * 3, cudaMemcpyHostToDevice, st));
   const bool same = ih == net_h && iw == net_w;
   if (same) CK(cudaMemcpyAsync(h->d_pages, d_page, px * 3, cudaMemcpyDeviceToDevice, st));
-  else CK(resize_linear_u8_launch(d_page, ih, iw, size_t(iw) * 3, 3, h->d_pages, unpad_h, unpad_w, net_h, net_w, st));
+  else CK(resize_linear_u8_launch(d_page, ih, iw, size_t(iw) * 3, 3, h->d_pages, geo.unpad_h, geo.unpad_w, net_h, net_w, st));
   if (int rc = enqueue_forward(h, 1, net_h, net_w, *sp)) return rc;
   // mask back-projection (inference.py:164-168)
   if (same) CK(cudaMemcpyAsync(d_mask, h->d_mask_u8, px, cudaMemcpyDeviceToDevice, st));
-  else CK(resize_linear_u8_launch(h->d_mask_u8, net_h - dh, net_w - dw, size_t(net_w), 1, d_mask, ih, iw, ih, iw, st));
+  else CK(resize_linear_u8_launch(h->d_mask_u8, geo.unpad_h, geo.unpad_w, size_t(net_w), 1, d_mask, ih, iw, ih, iw, st));
   std::vector<float> det(300 * 6);
   std::vector<int16_t> lb(1000 * 8);
   std::vector<float> ls(1000);
@@ -465,14 +797,14 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   CK(cudaMemsetAsync(d_ref, 0, pxa, st));
   CK(cudaStreamSynchronize(st));
   // phase B
-  const ArenaLayout& L = h->layout;
-  std::vector<char> section(L.blocks_stride);
+  const BlockSection L = block_section_layout();
+  std::vector<char> section(L.stride);
   PageIn in;
   in.det = det.data(); in.n_det = std::min(std::max(n_det, 0), 300);
   in.line_boxes = lb.data(); in.line_scores = ls.data(); in.n_lines = std::min(std::max(n_lines, 0), 1000);
   in.mask = mask_out; in.im_w = iw; in.im_h = ih;
-  in.ratio_x = float(double(iw) / double(net_w - dw));     // resize_ratio (inference.py:148)
-  in.ratio_y = float(double(ih) / double(net_h - dh));
+  in.ratio_x = geo.ratio_x;
+  in.ratio_y = geo.ratio_y;
   std::vector<int32_t> wins;
   if (int rc = host_group_page(in, section.data(), L, wins)) return ctd_fail(h, rc, "group_output failed");
   const ctd_page_blocks* hdr = reinterpret_cast<const ctd_page_blocks*>(section.data());
@@ -490,48 +822,15 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   // phase C
   RefineJob rj;
   for (int i = 0; i < nb; ++i) rj.add(wins[4 * i], wins[4 * i + 1], wins[4 * i + 2], wins[4 * i + 3], 0, iw, ih);
-  if (int rc = launch_refine(h, rj, d_page, d_mask, ih, iw, refine_mode, d_ref, st, nullptr)) return rc;
+  if (int rc = launch_refine(h, rj, d_page, d_mask, refine_mode, d_ref, st, &h->d_refine_scratch, &h->refine_scratch_cap,
+                             nullptr))
+    return rc;
   if (keep_undetected) {
     // refine_undetected_mask (textmask.py:135-156); the page mask is modified in place and returned, as in the reference
-    undetected_prep_kernel<<<unsigned((px + 255) / 256), 256, 0, st>>>(d_mask, d_ref, d_thr, px);
-    CK(cudaGetLastError());
-    int32_t* d_stats = nullptr;
-    int32_t n_lab = 0;
-    const int stats_cap = ((ih + 1) / 2) * ((iw + 1) / 2) + 2;   // worst case of 8-connected components + background
-    if (int rc = cc_device(h, d_thr, ih, iw, stats_cap, &d_stats, &n_lab)) return rc;
-    std::vector<int32_t> stats(size_t(std::max(n_lab, 0)) * 5);
-    if (n_lab > 0) CK(cudaMemcpyAsync(stats.data(), d_stats, stats.size() * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    RefineJob rj2;
-    bool first_valid = true;
-    for (int li = 0; li < n_lab; ++li) {
-      const int32_t* s5 = &stats[size_t(li) * 5];
-      if (!(s5[4] > 50)) continue;
-      if (first_valid) { first_valid = false; continue; }        // valid_labels[1:]
-      const int64_t bb[4] = {s5[0], s5[1], int64_t(s5[0]) + s5[2], int64_t(s5[1]) + s5[3]};
-      int64_t score = -1;
-      for (int b = 0; b < nb; ++b) {
-        const int32_t* q = rec[b].xyxy;
-        const int64_t x1 = std::max<int64_t>(q[0], bb[0]), y1 = std::max<int64_t>(q[1], bb[1]);
-        const int64_t x2 = std::min<int64_t>(q[2], bb[2]), y2 = std::min<int64_t>(q[3], bb[3]);
-        const int64_t a = (y2 < y1 || x2 < x1) ? -1 : (y2 - y1) * (x2 - x1);
-        if (a > score) score = a;
-      }
-      if (double(score) / double(s5[2]) / double(s5[3]) < 0.5) {
-        int32_t xy[4] = {int32_t(bb[0]), int32_t(bb[1]), int32_t(bb[2]), int32_t(bb[3])}, w4[4];
-        const int64_t w = bb[2] - bb[0], hh = bb[3] - bb[1];
-        const int64_t pad = int64_t(nearbyint((double(std::max(hh, w)) * 0.25 + double(std::min(hh, w)) * 0.75) / 16.0));
-        w4[0] = int32_t(std::max<int64_t>(0, xy[0] - pad)); w4[1] = int32_t(std::max<int64_t>(0, xy[1] - pad));
-        w4[2] = int32_t(std::min<int64_t>(iw - 1, xy[2] + pad)); w4[3] = int32_t(std::min<int64_t>(ih - 1, xy[3] + pad));
-        rj2.add(w4[0], w4[1], w4[2], w4[3], 0, iw, ih);
-      }
-    }
-    if (!rj2.wins.empty()) {
-      CK(cudaMemsetAsync(d_ref2, 0, pxa, st));
-      if (int rc = launch_refine(h, rj2, d_page, d_mask, ih, iw, refine_mode, d_ref2, st, nullptr)) return rc;
-      or_kernel<<<unsigned((px + 255) / 256), 256, 0, st>>>(d_ref, d_ref2, px);
-      CK(cudaGetLastError());
-    }
+    const std::vector<UndetPage> pg{UndetPage{0, ih, iw, rec, nb}};
+    if (int rc = refine_undetected(h, pg, px, d_page, d_mask, d_ref, d_ref2, d_thr, refine_mode, st, &h->d_cc_scratch,
+                                   &h->cc_scratch_cap, &h->d_refine_scratch, &h->refine_scratch_cap, nullptr, 0))
+      return rc;
     CK(cudaMemcpyAsync(mask_out, d_mask, px, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaMemcpyAsync(mask_refined_out, d_ref, px, cudaMemcpyDeviceToHost, st));

@@ -44,7 +44,7 @@ struct Ctx {
   const RefineWin* wins;
   const RefineChunk* chunks;
   WinState* st;
-  int H, W, mode;
+  int mode;
   // planes (window-pixel indexed)
   int* L;
   int* acc;
@@ -74,8 +74,8 @@ __device__ __forceinline__ View view_of(const Ctx& c, int chunk) {
   v.i0 = ch.y0 * v.rw + ch.x0;
   v.cnt = ch.rows * v.cols;
   v.aligned = (v.i0 & 3) == 0;   // the window planes start on 4-byte boundaries
-  v.img = c.img_all + size_t(v.win.page) * c.H * c.W * 3;
-  v.mask = c.mask_all + size_t(v.win.page) * c.H * c.W;
+  v.img = c.img_all + size_t(v.win.page_off) * 3;
+  v.mask = c.mask_all + size_t(v.win.page_off);
   return v;
 }
 
@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
     if (e < hl.ext) {
       int ye, xe;
       divmod(e, dv, ye, xe);
-      mv = v.mask[size_t(v.win.y1 + hl.ystart + ye) * c.W + v.win.x1 + hl.xs + xe];
+      mv = v.mask[size_t(v.win.y1 + hl.ystart + ye) * v.win.pitch + v.win.x1 + hl.xs + xe];
     }
     const unsigned b60 = __ballot_sync(0xffffffffu, mv <= 60), b127 = __ballot_sync(0xffffffffu, mv <= 127);
     if ((threadIdx.x & 31) == 0 && e < hl.ext) { N60[e >> 5] = b60; N127[e >> 5] = b127; }
@@ -235,7 +235,7 @@ __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
       if (k < v.cnt) {
         int y, x;
         divmod(v.i0 + k, dvw, y, x);
-        const size_t gp = size_t(v.win.y1 + y) * c.W + v.win.x1 + x;
+        const size_t gp = size_t(v.win.y1 + y) * v.win.pitch + v.win.x1 + x;
         b[u] = v.img[gp * 3]; g[u] = v.img[gp * 3 + 1]; r[u] = v.img[gp * 3 + 2];
       }
     }
@@ -395,7 +395,7 @@ __global__ void __launch_bounds__(kThreads) k_xor(Ctx c) {
       if (k < v.cnt) {
         int y, x;
         divmod(v.i0 + k, dv, y, x);
-        const size_t gp = size_t(v.win.y1 + y) * c.W + v.win.x1 + x;
+        const size_t gp = size_t(v.win.y1 + y) * v.win.pitch + v.win.x1 + x;
         mk[u] = v.mask[gp];
         gr[u] = grey[v.i0 + k];
 #pragma unroll
@@ -577,7 +577,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
               if (k + j < v.cnt) {
                 int yl, x;
                 divmod(k + j, dv, yl, x);
-                s4 |= unsigned(v.img[(size_t(v.win.y1 + v.y0 + yl) * c.W + v.win.x1 + v.x0 + x) * 3 + (kind - 3)]) << (8 * j);
+                s4 |= unsigned(v.img[(size_t(v.win.y1 + v.y0 + yl) * v.win.pitch + v.win.x1 + v.x0 + x) * 3 + (kind - 3)]) << (8 * j);
               }
             }
           }
@@ -645,7 +645,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
           else {
             int yl, x;
             divmod(k, dv, yl, x);
-            raw[u] = v.img[(size_t(v.win.y1 + v.y0 + yl) * c.W + v.win.x1 + v.x0 + x) * 3 + (kind - 3)];
+            raw[u] = v.img[(size_t(v.win.y1 + v.y0 + yl) * v.win.pitch + v.win.x1 + v.x0 + x) * 3 + (kind - 3)];
           }
         }
       }
@@ -1003,7 +1003,6 @@ __global__ void __launch_bounds__(kThreads) k_dilate(Ctx c) {
 __global__ void __launch_bounds__(kThreads) k_or(Ctx c) {
   const View v = view_of(c, blockIdx.x);
   const uint8_t* merged = c.merged + v.win.off;
-  uint32_t* out_words = c.out_all + size_t(v.win.page) * c.H * c.W / 4;
   const DivW dv = make_div(v.rw, v.rw * v.rh);
   constexpr int U = 8;
   for (int k0 = 0; k0 < v.cnt; k0 += kThreads * U) {
@@ -1018,8 +1017,8 @@ __global__ void __launch_bounds__(kThreads) k_or(Ctx c) {
       if (!mg[u]) continue;
       int y, x;
       divmod(v.i0 + k0 + u * kThreads + threadIdx.x, dv, y, x);
-      const size_t gp = size_t(v.win.y1 + y) * c.W + v.win.x1 + x;
-      atomicOr(&out_words[gp >> 2], 0xffu << (8 * (gp & 3)));
+      const size_t gp = size_t(v.win.page_off) + size_t(v.win.y1 + y) * v.win.pitch + v.win.x1 + x;
+      atomicOr(&c.out_all[gp >> 2], 0xffu << (8 * (gp & 3)));
     }
   }
 }
@@ -1031,8 +1030,9 @@ size_t refine_mk_state_bytes(int n_wins) { return (size_t(n_wins) * sizeof(WinSt
 size_t refine_scratch_bytes(size_t total_px) { return total_px * (4 + 16 + 4) + 4096; }
 
 // d_wins: n_wins windows; d_chunks: n_chunks chunks (RefineChunk, kernels.h); d_state: refine_mk_state_bytes(n_wins)
-// bytes (zeroed here); scratch: refine_scratch_bytes(total_px) bytes.  img / mask / out hold H*W-pixel planes per page.
-cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, int H, int W, const RefineWin* d_wins, int n_wins,
+// bytes (zeroed here); scratch: refine_scratch_bytes(total_px) bytes.  img / mask / out hold the pages' planes at the
+// windows' page_off (3 bytes per pixel in img).
+cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const RefineWin* d_wins, int n_wins,
                              const RefineChunk* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
                              void* scratch, int refine_mode, uint8_t* d_out, cudaStream_t s) {
   if (n_wins <= 0 || n_chunks <= 0) return cudaSuccess;
@@ -1041,7 +1041,7 @@ cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, int H,
   c.wins = d_wins;
   c.chunks = d_chunks;
   c.st = static_cast<WinState*>(d_state);
-  c.H = H; c.W = W; c.mode = refine_mode;
+  c.mode = refine_mode;
   char* p = static_cast<char*>(scratch);
   c.L = reinterpret_cast<int*>(p); p += total_px * 4;
   c.acc = reinterpret_cast<int*>(p); p += total_px * 16;

@@ -36,14 +36,12 @@ __device__ __forceinline__ AxisTap axis_tap(int d, int ssize, int dsize, bool cl
   return t;
 }
 
-// One thread per canvas pixel (all C channels).  Pixels outside the dw x dh image are zero (letterbox padding).
+// One output pixel (all C channels) of the dh x dw resize of src, written at `o`; pixels outside the dh x dw image are
+// zero (letterbox padding).  Every kernel of this file computes its pixels here, so the single-image and the batched
+// paths cannot drift apart.
 template <int C>
-__global__ void resize_linear_u8_kernel(const uint8_t* __restrict__ src, int sh, int sw, size_t src_pitch,
-                                        uint8_t* __restrict__ dst, int dh, int dw, int canvas_h, int canvas_w) {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const int y = blockIdx.y;
-  if (x >= canvas_w || y >= canvas_h) return;
-  uint8_t* o = dst + (size_t(y) * canvas_w + x) * C;
+__device__ __forceinline__ void resize_pixel(const uint8_t* __restrict__ src, int sh, int sw, size_t src_pitch,
+                                             uint8_t* __restrict__ o, int x, int y, int dh, int dw) {
   if (x >= dw || y >= dh) {
 #pragma unroll
     for (int c = 0; c < C; ++c) o[c] = 0;
@@ -67,6 +65,45 @@ __global__ void resize_linear_u8_kernel(const uint8_t* __restrict__ src, int sh,
   }
 }
 
+// One thread per canvas pixel.
+template <int C>
+__global__ void resize_linear_u8_kernel(const uint8_t* __restrict__ src, int sh, int sw, size_t src_pitch,
+                                        uint8_t* __restrict__ dst, int dh, int dw, int canvas_h, int canvas_w) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y;
+  if (x >= canvas_w || y >= canvas_h) return;
+  resize_pixel<C>(src, sh, sw, src_pitch, dst + (size_t(y) * canvas_w + x) * C, x, y, dh, dw);
+}
+
+// Letterbox of every page of a batch: blockIdx.z = page, one thread per pixel of its net_h x net_w canvas.
+__global__ void letterbox_batch_kernel(const uint8_t* __restrict__ src, const PageGeom* __restrict__ tab,
+                                       uint8_t* __restrict__ dst, int net_h, int net_w) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  const int y = blockIdx.y;
+  if (x >= net_w) return;
+  const PageGeom g = tab[blockIdx.z];
+  uint8_t* o = dst + ((size_t(blockIdx.z) * net_h + y) * net_w + x) * 3;
+  resize_pixel<3>(src + g.src_off, g.ih, g.iw, size_t(g.iw) * 3, o, x, y, g.unpad_h, g.unpad_w);
+}
+
+// Mask back-projection of every page of a batch: one CTA per output row over the pages' stacked rows (page p owns rows
+// [row0, row0 + ih)), so no CTA is launched for a row that does not exist; the threads stride over the row's columns.
+__global__ void backproject_batch_kernel(const uint8_t* __restrict__ mask, int net_h, int net_w,
+                                         const PageGeom* __restrict__ tab, int n, uint8_t* __restrict__ dst) {
+  const int r = blockIdx.x;
+  int lo = 0, hi = n - 1;   // last page with row0 <= r
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (tab[mid].row0 <= r) lo = mid; else hi = mid - 1;
+  }
+  const PageGeom g = tab[lo];
+  const int y = r - g.row0;
+  const uint8_t* src = mask + size_t(lo) * net_h * net_w;
+  uint8_t* orow = dst + g.dst_off + size_t(y) * g.iw;
+  for (int x = threadIdx.x; x < g.iw; x += blockDim.x)
+    resize_pixel<1>(src, g.unpad_h, g.unpad_w, size_t(net_w), orow + x, x, y, g.ih, g.iw);
+}
+
 cudaError_t resize_linear_u8_launch(const uint8_t* src, int sh, int sw, size_t src_pitch, int channels, uint8_t* dst,
                                     int dh, int dw, int canvas_h, int canvas_w, cudaStream_t s) {
   if (sh < 1 || sw < 1 || dh < 1 || dw < 1 || canvas_h < dh || canvas_w < dw) return cudaErrorInvalidValue;
@@ -74,6 +111,21 @@ cudaError_t resize_linear_u8_launch(const uint8_t* src, int sh, int sw, size_t s
   if (channels == 3) resize_linear_u8_kernel<3><<<grid, 128, 0, s>>>(src, sh, sw, src_pitch, dst, dh, dw, canvas_h, canvas_w);
   else if (channels == 1) resize_linear_u8_kernel<1><<<grid, 128, 0, s>>>(src, sh, sw, src_pitch, dst, dh, dw, canvas_h, canvas_w);
   else return cudaErrorInvalidValue;
+  return cudaGetLastError();
+}
+
+cudaError_t letterbox_batch_launch(const uint8_t* src, const PageGeom* d_tab, int n, uint8_t* dst, int net_h, int net_w,
+                                   cudaStream_t s) {
+  if (n < 1 || net_h < 1 || net_w < 1) return cudaErrorInvalidValue;
+  letterbox_batch_kernel<<<dim3(unsigned((net_w + 127) / 128), unsigned(net_h), unsigned(n)), 128, 0, s>>>(src, d_tab, dst,
+                                                                                                        net_h, net_w);
+  return cudaGetLastError();
+}
+
+cudaError_t backproject_batch_launch(const uint8_t* mask, int net_h, int net_w, const PageGeom* d_tab, int n,
+                                     int total_rows, uint8_t* dst, cudaStream_t s) {
+  if (n < 1 || total_rows < 1) return cudaErrorInvalidValue;
+  backproject_batch_kernel<<<unsigned(total_rows), 256, 0, s>>>(mask, net_h, net_w, d_tab, n, dst);
   return cudaGetLastError();
 }
 

@@ -4,11 +4,14 @@ Same constructor and call signature as the reference's `inference.TextDetector`
 (inference.py:116-178): `TextDetector(model_path, input_size=1024, device=..., half=False, nms_thresh=0.35,
 conf_thresh=0.4, mask_thresh=0.3, act='leaky')` and
 `detector(img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False) -> (mask, mask_refined, blk_list)`.
+`detect_batch` / `detect_stream` give the same results for many pages of any sizes, batched on the GPU.
 
 Everything runs in libctd_b200.so: network, NMS, mask u8, DB binarize, connected components, contour boxes + scores,
 refine_mask on the GPU; ratio scaling, `group_output` and the window expansion in host C++ (csrc/group.cpp,
-csrc/pipeline.cu).  This module is the reference-shaped Python surface over `ctd_detect_page`.
+csrc/pipeline.cu).  This module is the reference-shaped Python surface over `ctd_detect_page` and, for batches,
+`ctd_submit_pages`.
 """
+from collections import deque
 from pathlib import Path
 from typing import List
 
@@ -59,7 +62,7 @@ class TextDetector:
     langcls2idx = {'eng': 0, 'ja': 1, 'unknown': 2}
 
     def __init__(self, model_path, input_size=1024, device='cuda', half=False, nms_thresh=0.35, conf_thresh=0.4,
-                 mask_thresh=0.3, act='leaky', precision=None, device_index=0):
+                 mask_thresh=0.3, act='leaky', precision=None, device_index=0, max_batch=1):
         if isinstance(model_path, (str, Path)):
             import torch
             ckpt = torch.load(str(model_path), map_location='cpu')  # reference basemodel.py:212
@@ -77,7 +80,9 @@ class TextDetector:
             precision = PREC_FP16_TC
         self.program = compiler.compile_checkpoint(ckpt, head_act=act)
         # DB threshold is hard-coded 0.3 in the reference (inference.py:139 ignores mask_thresh)
-        self.net = Engine(self.program, device=device_index, precision=precision, max_batch=1, max_h=input_size[0],
+        # max_batch: pages per GPU batch of detect_batch / detect_stream (the workspace is sized for it)
+        self.max_batch = int(max_batch)
+        self.net = Engine(self.program, device=device_index, precision=precision, max_batch=self.max_batch, max_h=input_size[0],
                           max_w=input_size[1], conf_thresh=conf_thresh, nms_thresh=nms_thresh, db_thresh=0.3)
 
     def close(self):
@@ -100,3 +105,62 @@ class TextDetector:
         on this detector's engine.  img: u8 BGR [h][w][3], the page `blk_list` was detected on.  Raises CtdError,
         naming the block and the line, before any GPU work if the reference would raise on a line."""
         return transformed_regions(self.net, img, blk_list, textheight)
+
+    def detect_batch(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
+        """`[self(img, refine_mode, keep_undetected_mask) for img in imgs]`, with the same results byte for byte, computed
+        in GPU batches of up to `max_batch` pages of any sizes (see detect_stream).  Every page is checked before any
+        GPU work: a page that is not u8 [h][w][3] raises ValueError."""
+        imgs = [check_page(img) for img in imgs]
+        return list(self.detect_stream(imgs, refine_mode, keep_undetected_mask))
+
+    def detect_stream(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
+        """Generator over an iterable of pages: yields `(mask, mask_refined, blk_list)` for each page in input order,
+        equal to `self(img, refine_mode, keep_undetected_mask)`.  Pages are grouped into batches of up to `max_batch`
+        and two batches are kept in flight (`ctd_submit_pages`): while one batch runs on the GPU and in the engine's
+        host stage, the next one is read from `imgs` and packed.  A page that is not u8 [h][w][3] raises ValueError
+        before it reaches the GPU."""
+        net_h, net_w = self.input_size
+        inflight = deque()   # slots in submission order
+        free = [0, 1]
+        try:
+            batch = []
+            for img in imgs:
+                batch.append(check_page(img))
+                if len(batch) < self.max_batch:
+                    continue
+                if not free:
+                    yield from self._collect(inflight, free)
+                slot = free.pop(0)
+                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask)
+                inflight.append(slot)
+                batch = []
+            if batch:
+                if not free:
+                    yield from self._collect(inflight, free)
+                slot = free.pop(0)
+                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask)
+                inflight.append(slot)
+            while inflight:
+                yield from self._collect(inflight, free)
+        finally:
+            while inflight:   # an error or an abandoned generator: leave the engine with no batch in flight
+                slot = inflight.popleft()
+                try:
+                    self.net.collect_pages(slot)
+                except Exception:
+                    pass
+
+    def _collect(self, inflight, free):
+        slot = inflight.popleft()
+        pages = self.net.collect_pages(slot)
+        free.append(slot)
+        for mask, mask_refined, rec, lines, dist in pages:
+            yield mask, mask_refined, blocks_from_records(rec, lines, dist)
+
+
+def check_page(img):
+    """A page as TextDetector's batch calls take it: u8 BGR [h][w][3] with h, w >= 1, else ValueError."""
+    a = np.asarray(img)
+    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] < 1 or a.shape[1] < 1:
+        raise ValueError("a page must be a uint8 array of shape [h][w][3], got %s %s" % (a.dtype, a.shape))
+    return np.ascontiguousarray(a)

@@ -54,17 +54,14 @@ def unpack_arena(arena_u8, layout, n, h, w, full=False):
     out = dict(mask=mask, det=[det[i, :cnt[i]] for i in range(n)], n_labels=nl,
                line_boxes=[lb[i, :lc[i]] for i in range(n)], line_scores=[ls[i, :lc[i]] for i in range(n)])
     if full:
-        from .binding import BLOCK_DTYPE, MAX_BLOCKS, MAX_BLOCK_DIST
+        from .binding import decode_block_section
         from .textblock import blocks_from_records
         out["mask_refined"] = a[lay["mask_refined"]:lay["mask_refined"] + n * h * w].reshape(n, h, w)
         blocks, flags = [], []
         for i in range(n):
             sec = a[lay["blocks"] + i * lay["blocks_stride"]:lay["blocks"] + (i + 1) * lay["blocks_stride"]]
-            hdr = sec[:16].view(np.int32)
-            rec = sec[lay["blk_records_off"]:lay["blk_records_off"] + MAX_BLOCKS * BLOCK_DTYPE.itemsize].view(BLOCK_DTYPE)
-            lines = sec[lay["blk_lines_off"]:lay["blk_lines_off"] + MAX_BLOCKS * 32].view(np.int32).reshape(-1, 8)
-            dist = sec[lay["blk_dist_off"]:lay["blk_dist_off"] + MAX_BLOCK_DIST * 8].view(np.float64)
-            blocks.append(blocks_from_records(rec[:int(hdr[0])], lines, dist))
+            hdr, rec, lines, dist = decode_block_section(sec, lay)
+            blocks.append(blocks_from_records(rec, lines, dist))
             flags.append(int(hdr[3]))
         out["blocks"], out["block_flags"] = blocks, flags
     return out

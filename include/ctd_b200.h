@@ -361,6 +361,40 @@ CTD_API int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages, i
 /* Device copy of slot `slot`'s complete results (same layout) and the stream its last writes were enqueued on.   */
 CTD_API int ctd_device_arena(ctd_handle* h, int32_t slot, void** base, void** post_stream);
 
+/* Batches of pages of ANY size through the whole chain, two batches in flight per handle: per page the same results
+ * as ctd_detect_page, byte for byte.
+ *
+ * ctd_pages_plan (host code, no handle, thread-safe, needs no GPU) lays a batch out.  The caller fills ih, iw of each
+ * entry; the plan fills the rest.  Every offset is a multiple of 256.
+ *   input  (*input_bytes):   page i, u8 BGR [ih][iw][3], at page_off
+ *   results (*results_bytes): page i's u8 [ih][iw] mask at mask_off and mask_refined at refined_off, and its block
+ *                            section (ctd_page_blocks header, ctd_block records at +blk_records_off, i32 lines
+ *                            [..][4][2] at +blk_lines_off, f64 distances at +blk_dist_off; ctd_results_layout gives
+ *                            these offsets, which do not depend on the handle) at blocks_off
+ * The page's pixel offsets inside the image and mask planes agree: page_off / 3 == mask_off - mask_off of page 0.
+ * Returns CTD_E_SHAPE where ctd_detect_page does: a page side < 1, a side that letterboxes to 0 px, or a net side
+ * that is not a positive multiple of 64.                                                                          */
+typedef struct ctd_page_entry {
+  int32_t ih, iw;                  /* in : page size (u8 BGR HWC)                                               */
+  int32_t unpad_h, unpad_w;        /* out: letterbox size, round(size * r), half to even (imgproc_utils.py:86-117) */
+  int64_t page_off;                /* out: byte offset of the page in the packed input buffer                   */
+  int64_t mask_off, refined_off;   /* out: page-sized u8 mask / mask_refined in the results buffer              */
+  int64_t blocks_off;              /* out: the page's block section in the results buffer                       */
+} ctd_page_entry;
+CTD_API int ctd_pages_plan(ctd_page_entry* pages, int32_t n, int32_t net_h, int32_t net_w, size_t* input_bytes,
+                           size_t* results_bytes);
+/* Asynchronous: the batch runs like a ctd_submit_full batch and is collected with ctd_collect(h, slot), after which
+ * `results_host` holds every page's mask (modified by refine_undetected_mask when keep_undetected != 0, as in
+ * ctd_detect_page), mask_refined and block section.  pages / n: the planned entries (checked against a fresh plan);
+ * input_host: the packed pages (pinned, input_bytes); results_host: pinned, results_bytes.  Both buffers must stay
+ * untouched until the slot is collected.  On the GPU: one letterbox launch for the batch, the forward at
+ * (n, net_h, net_w), one launch back-projecting every page's mask to its size, one refine_mask launch for every
+ * window of every page.  Same checks as ctd_submit_full (slot 0/1 and collected, n <= max_batch, net shape <= the
+ * engine's max shape, not a debug_skip_postproc engine).                                                          */
+CTD_API int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                             int32_t net_w, const uint8_t* input_host, int32_t refine_mode, int32_t keep_undetected,
+                             void* results_host);
+
 /* ---- text-line crops for OCR (SURVEY 8f row f4) ----------------------------------------------------------------
  * `TextBlock.get_transformed_region(img, idx, textheight)` (utils/textblock.py:162-194): line `idx` of a block, pushed
  * out by font_size / 3 for 'eng' (and horizontal 'unknown') blocks and clipped to [0, im_w] x [0, im_h], cut out of the
