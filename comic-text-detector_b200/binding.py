@@ -74,7 +74,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_results_bytes", "ctd_join", "ctd_forward_resized", "ctd_get_mask_u8_resized",
            "ctd_resize_linear_u8", "ctd_debug_run_ops", "ctd_get_nms_status", "ctd_group_output",
            "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena",
-           "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages"]
+           "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
+           "ctd_submit_pages_regions", "ctd_collect_regions"]
 
 _lib = None
 
@@ -136,6 +137,9 @@ def load_library():
     lib.ctd_transform_regions.argtypes = [vp, vp, i32, i32, i32, vp, i32, vp, C.c_size_t]
     lib.ctd_pages_plan.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.ctd_submit_pages.argtypes = [vp, i32, vp, i32, i32, i32, vp, i32, i32, vp]
+    lib.ctd_submit_pages_regions.argtypes = [vp, i32, vp, i32, i32, i32, vp, i32, i32, i32, vp]
+    lib.ctd_collect_regions.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i32), C.POINTER(vp), C.POINTER(vp),
+                                        C.POINTER(C.c_size_t)]
     for name in EXPORTS[3:]:
         getattr(lib, name).restype = C.c_int
     lib.ctd_expand_textwindow.restype = None
@@ -429,10 +433,11 @@ class Engine:
     def collect(self, slot):
         self._ck(self.lib.ctd_collect(self.h, slot))
 
-    def submit_pages(self, slot, pages, net_h, net_w, refine_mode=0, keep_undetected=False):
-        """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages): the pages (u8 [h][w][3]
-        each) are packed into this slot's pinned input buffer, which like the pinned results buffer belongs to the
-        engine and grows on demand.  Collect with collect_pages(slot)."""
+    def submit_pages(self, slot, pages, net_h, net_w, refine_mode=0, keep_undetected=False, textheight=0):
+        """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages_regions): the pages (u8
+        [h][w][3] each) are packed into this slot's pinned input buffer, which like the pinned results buffer belongs to
+        the engine and grows on demand.  textheight >= 2 also crops every text line of every page on the GPU
+        (0: no crops).  Collect with collect_pages(slot)."""
         import torch
         if not hasattr(self, "_pg_bufs"):
             self._pg_bufs = [[None, None], [None, None]]   # per slot: pinned input, pinned results
@@ -448,18 +453,21 @@ class Engine:
         for e, p in zip(entries, pages):
             o = int(e["page_off"])
             np.copyto(inp[o:o + p.size].reshape(p.shape), p)
-        self._ck(self.lib.ctd_submit_pages(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
-                                           C.c_void_p(bufs[0].data_ptr()), int(refine_mode), int(bool(keep_undetected)),
-                                           C.c_void_p(bufs[1].data_ptr())))
-        self._pg_inflight[slot] = entries
+        self._ck(self.lib.ctd_submit_pages_regions(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
+                                                   C.c_void_p(bufs[0].data_ptr()), int(refine_mode),
+                                                   int(bool(keep_undetected)), int(textheight),
+                                                   C.c_void_p(bufs[1].data_ptr())))
+        self._pg_inflight[slot] = (entries, int(textheight))
         self.shape = (len(entries), net_h, net_w)
 
     def collect_pages(self, slot):
         """blocks until the batch of submit_pages(slot) is done -> per page the 5-tuple detect_page returns
-        (mask, mask_refined, block records, lines, distances), copied out of the slot's pinned buffer."""
-        entries = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
-        if entries is None:
+        (mask, mask_refined, block records, lines, distances), copied out of the slot's pinned buffer.  With a
+        textheight, each tuple has a sixth element, the page's crops (see collect_regions)."""
+        inflight = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
+        if inflight is None:
             raise CtdError("slot %d has no submit_pages batch in flight" % slot)
+        entries, textheight = inflight
         self._pg_inflight[slot] = None
         self.collect(slot)
         res = self._pg_bufs[slot][1].numpy()
@@ -472,6 +480,42 @@ class Engine:
             _hdr, rec, lines, dist = decode_block_section(res[bo:bo + stride], lay)
             out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy(), res[ro:ro + ih * iw].reshape(ih, iw).copy(),
                         rec.copy(), lines.copy(), dist.copy()))
+        if textheight:
+            crops = self.collect_regions(slot, [o[2]["n_lines"] for o in out])
+            out = [o + (c,) for o, c in zip(out, crops)]
+        return out
+
+    def collect_regions(self, slot, n_lines):
+        """the crops of the collected ctd_submit_pages_regions batch of `slot` (ctd_collect_regions): per page, per
+        block a list of u8 [h][w][3] arrays in line order, None for a line the planner gives no crop (status != 0).
+        n_lines: per page the block records' n_lines.  Each page's crops are views into one fresh array of that page
+        (copied out of the engine's pinned buffer by torch's multi-threaded CPU copy: a single-threaded copy into fresh
+        memory was most of the cost of this call)."""
+        import torch
+        plan_p, n_reg, first_p, pix_p, nbytes = C.c_void_p(), C.c_int32(), C.c_void_p(), C.c_void_p(), C.c_size_t()
+        self._ck(self.lib.ctd_collect_regions(self.h, slot, C.byref(plan_p), C.byref(n_reg), C.byref(first_p),
+                                              C.byref(pix_p), C.byref(nbytes)))
+        n, total = int(n_reg.value), int(nbytes.value)
+        first = np.ctypeslib.as_array(C.cast(first_p, C.POINTER(C.c_int32)), (len(n_lines) + 1,)).tolist()
+        plan = np.frombuffer((C.c_char * (n * REGION_DTYPE.itemsize)).from_address(plan_p.value), REGION_DTYPE) \
+            if n else np.zeros((0,), REGION_DTYPE)
+        pix = torch.from_numpy(np.ctypeslib.as_array(C.cast(pix_p, C.POINTER(C.c_uint8)), (total,))) if total else None
+        off, oh, ow = plan["offset"].tolist(), plan["out_h"].tolist(), plan["out_w"].tolist()
+        ok = (plan["status"] == 0).tolist()
+        out = []
+        for p, counts in enumerate(n_lines):
+            a, b = first[p], first[p + 1]
+            counts = np.asarray(counts).tolist()
+            assert sum(counts) == b - a, (p, sum(counts), b - a)
+            lo = off[a] if b > a else 0
+            hi = off[b - 1] + oh[b - 1] * ow[b - 1] * 3 if b > a else 0
+            buf = torch.empty((hi - lo,), dtype=torch.uint8).copy_(pix[lo:hi]).numpy() if hi > lo else None
+            page, k = [], a
+            for c in counts:
+                page.append([buf[off[j] - lo:off[j] - lo + oh[j] * ow[j] * 3].reshape(oh[j], ow[j], 3) if ok[j] else None
+                             for j in range(k, k + c)])
+                k += c
+            out.append(page)
         return out
 
     def join(self, other):

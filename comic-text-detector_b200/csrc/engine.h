@@ -79,6 +79,7 @@ struct PipeJob {
   // ctd_submit_pages: the batch's pages (ph x pw is the net shape), and whether to run refine_undetected_mask
   std::vector<ctd_page_entry> pages;
   int keep_undetected = 0;
+  int textheight = 0;   // > 0: also crop every text line of every page (ctd_submit_pages_regions)
 };
 
 // refine windows of one launch (all pages of a batch) and the chunks they are cut into
@@ -89,6 +90,18 @@ struct RefineJob {
   // window of the iw x ih page whose planes start at pixel page_off; python slice semantics; empty windows dropped
   void add(int x1, int y1, int x2, int y2, size_t page_off, int iw, int ih);
   size_t table_bytes() const;
+};
+
+// crops of one k_warp_regions launch (all pages of a batch, or one page) and the tiles they are cut into
+struct RegionJob {
+  std::vector<ctd::RegionDev> regs;
+  std::vector<ctd::RegionTile> tiles;
+  size_t out_bytes = 0;   // end of the last crop in the packed output
+  // the status-0 entries of plan[0..n), the crops of the ih x iw page at byte page_off, each written at out_base + its
+  // plan offset; returns the index of a malformed entry, or -1
+  int add(const ctd_region* plan, int n, long long page_off, int ih, int iw, long long out_base);
+  size_t table_bytes() const;   // RegionDev[] | RegionTile[], each 256-aligned
+  void write_tables(char* dst) const;
 };
 
 struct ShapePlan {
@@ -185,6 +198,16 @@ struct ctd_handle {
   // refine scratch of the worker's phase C on the post stream (d_refine_scratch belongs to the caller's stream)
   void* d_post_refine = nullptr;
   size_t post_refine_cap = 0;
+  // text-line crops of a ctd_submit_pages_regions batch, per slot, written by the worker: the concatenated plans, the
+  // first plan entry of each page (n + 1 entries), the device buffer (crop tables | crop pixels) and the pinned host
+  // buffer (the same tables staged for upload | the pixels copied back), both grown on demand and never shrunk
+  std::vector<ctd_region> crop_plan[2];
+  std::vector<int32_t> crop_first[2];
+  uint8_t* d_crop[2] = {nullptr, nullptr};
+  uint8_t* h_crop[2] = {nullptr, nullptr};
+  size_t crop_dcap[2] = {0, 0}, crop_hcap[2] = {0, 0};
+  size_t crop_px_off[2] = {0, 0}, crop_bytes[2] = {0, 0};   // pixels at h_crop + crop_px_off, crop_bytes long
+  bool crop_ready[2] = {false, false};                      // the collected batch of the slot asked for crops
   // last forward
   int n = 0, ph = 0, pw = 0;
   int last_launches = 0;

@@ -231,4 +231,20 @@ cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const 
                              const RefineChunk* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
                              void* scratch, int refine_mode, uint8_t* d_out, cudaStream_t s);
 
+// ---- text-line crops (region.cu) ----
+constexpr int kRegionTilePx = 256;   // output pixels per CTA of k_warp_regions = threads per CTA
+// one crop of a k_warp_regions launch: where its page and its output are, its shape and the inverse homography
+struct RegionDev {
+  long long offset;        // byte offset of the crop in the packed output
+  long long page_off;      // byte offset of the crop's page (u8 BGR [ih][iw][3]) in the pages buffer
+  int out_h, out_w;        // returned shape
+  int warp_w, bw0;         // width of the warped (un-rotated) image, OpenCV's block width
+  int rotate, ih, iw, pad;
+  double m[9];             // inverse homography (destination -> page)
+};
+struct RegionTile { int region, first; };   // kRegionTilePx consecutive output pixels of one crop
+// one CTA per tile; d_pages holds every crop's page at its page_off
+cudaError_t warp_regions_launch(const uint8_t* d_pages, const RegionDev* d_regs, const RegionTile* d_tiles, int n_tiles,
+                                uint8_t* d_out, cudaStream_t s);
+
 }  // namespace ctd

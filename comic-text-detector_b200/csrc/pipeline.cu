@@ -11,7 +11,8 @@
 // the refine kernels of batch i overlap the forward of batch i+1.  ctd_detect_page is the blocking single-page form
 // for pages of any size (letterbox + back-projection on the GPU), the call behind the drop-in TextDetector.
 // ctd_submit_pages runs batches of pages of any size through the same two-in-flight schedule, with one letterbox and
-// one back-projection launch per batch (TextDetector.detect_batch / detect_stream).
+// one back-projection launch per batch (TextDetector.detect_batch / detect_stream); ctd_submit_pages_regions also cuts
+// every text line of every page of the batch out of the resident pages in one k_warp_regions launch (region.cu).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -401,6 +402,53 @@ extern "C" int ctd_pages_plan(ctd_page_entry* pages, int32_t n, int32_t net_h, i
   return CTD_OK;
 }
 
+// device buffer of a slot, grown (never shrunk) to `bytes`; only called while no enqueued work uses the buffer (the
+// page and results buffers at submit, while the slot is idle; the crop buffer by the worker, after syncing `post`)
+static int grow_slot_buffer(ctd_handle* h, uint8_t** buf, size_t* cap, size_t bytes) {
+  if (bytes <= *cap) return CTD_OK;
+  cudaFree(*buf);
+  *buf = nullptr;
+  *cap = 0;
+  CK(cudaMalloc(reinterpret_cast<void**>(buf), bytes + bytes / 4));
+  *cap = bytes + bytes / 4;
+  return CTD_OK;
+}
+
+// the same for a pinned host buffer
+static int grow_slot_pinned(ctd_handle* h, uint8_t** buf, size_t* cap, size_t bytes) {
+  if (bytes <= *cap) return CTD_OK;
+  if (*buf) cudaFreeHost(*buf);
+  *buf = nullptr;
+  *cap = 0;
+  CK(cudaHostAlloc(reinterpret_cast<void**>(buf), bytes + bytes / 4, cudaHostAllocDefault));
+  *cap = bytes + bytes / 4;
+  return CTD_OK;
+}
+
+// ctd_region_plan of every line of one page's block section, in block then line order (textblock.region_lines)
+static int plan_page_regions(const char* section, const BlockSection& bs, int iw, int ih, int textheight,
+                             std::vector<ctd_region>& plan, size_t* bytes) {
+  const ctd_page_blocks* hdr = reinterpret_cast<const ctd_page_blocks*>(section);
+  const ctd_block* rec = reinterpret_cast<const ctd_block*>(section + bs.rec_off);
+  const int32_t* quads = reinterpret_cast<const int32_t*>(section + bs.lines_off);
+  std::vector<ctd_region_line> lines;
+  lines.reserve(size_t(std::max(hdr->n_lines, 0)));
+  for (int b = 0; b < hdr->n_blocks; ++b)
+    for (int k = 0; k < rec[b].n_lines; ++k) {
+      ctd_region_line l{};
+      const int32_t* q = quads + size_t(rec[b].line_off + k) * 8;
+      for (int j = 0; j < 8; ++j) l.quad[j] = double(q[j]);
+      l.language = rec[b].language;
+      l.vertical = rec[b].vertical ? 1 : 0;
+      l.font_size = rec[b].font_size;
+      lines.push_back(l);
+    }
+  plan.resize(lines.size());
+  *bytes = 0;
+  if (lines.empty()) return CTD_OK;   // nothing to plan, whatever the page size
+  return ctd_region_plan(lines.data(), int32_t(lines.size()), iw, ih, textheight, plan.data(), bytes);
+}
+
 // phases B and C of a ctd_submit_pages batch, on the worker thread
 static int run_pages_job(ctd_handle* h, const PipeJob& job) {
   const int slot = job.slot, n = job.n;
@@ -413,6 +461,11 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
   const int32_t* line_cnt = reinterpret_cast<const int32_t*>(res + hd.lc);
   std::vector<std::vector<int32_t>> wins(static_cast<size_t>(n));
   std::vector<int> prc(size_t(n), CTD_OK);
+  // text-line crops: each page's plan on the host threads, right after its group_output
+  const bool crops = job.textheight > 0;
+  std::vector<std::vector<ctd_region>> plans(crops ? size_t(n) : 0);
+  std::vector<size_t> plan_bytes(size_t(n), 0);
+  std::vector<int> crc(size_t(n), CTD_OK);
   for_each_page(n, h->host_threads, [&](int i) {
     const ctd_page_entry& e = pg[size_t(i)];
     Letterbox lb;
@@ -426,9 +479,42 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
     in.mask = reinterpret_cast<const uint8_t*>(res + e.mask_off);
     in.im_w = e.iw; in.im_h = e.ih; in.ratio_x = lb.ratio_x; in.ratio_y = lb.ratio_y;
     prc[size_t(i)] = host_group_page(in, res + e.blocks_off, bs, wins[size_t(i)]);
+    if (crops && prc[size_t(i)] == CTD_OK)
+      crc[size_t(i)] = plan_page_regions(res + e.blocks_off, bs, e.iw, e.ih, job.textheight, plans[size_t(i)],
+                                         &plan_bytes[size_t(i)]);
   });
   for (int i = 0; i < n; ++i)
     if (prc[size_t(i)] != CTD_OK) return ctd_fail(h, prc[size_t(i)], "group_output failed on page %d of the batch", i);
+  for (int i = 0; i < n; ++i)
+    if (crc[size_t(i)] != CTD_OK)
+      return ctd_fail(h, crc[size_t(i)], "ctd_region_plan refused page %d of the batch (%dx%d, textheight %d)", i,
+                      pg[size_t(i)].ih, pg[size_t(i)].iw, job.textheight);
+  // the batch's plans, concatenated with each page's crops after the previous page's; one warp job for all pages
+  RegionJob rg;
+  if (crops) {
+    std::vector<ctd_region>& plan = h->crop_plan[slot];
+    std::vector<int32_t>& first = h->crop_first[slot];
+    plan.clear();
+    first.assign(size_t(n) + 1, 0);
+    size_t base = 0;
+    for (int i = 0; i < n; ++i) {
+      const ctd_page_entry& e = pg[size_t(i)];
+      const std::vector<ctd_region>& p = plans[size_t(i)];
+      if (int bad = rg.add(p.data(), int(p.size()), e.page_off, e.ih, e.iw, (long long)base); bad >= 0)
+        return ctd_fail(h, CTD_E_INVALID, "malformed crop plan entry %d on page %d of the batch", bad, i);
+      first[size_t(i)] = int32_t(plan.size());
+      for (ctd_region r : p) {
+        r.offset += int64_t(base);
+        plan.push_back(r);
+      }
+      base += plan_bytes[size_t(i)];
+    }
+    first[size_t(n)] = int32_t(plan.size());
+    if (plan.size() > size_t(INT32_MAX) || rg.tiles.size() > size_t(INT32_MAX))
+      return ctd_fail(h, CTD_E_CAPACITY, "too many crops in one batch");
+    h->crop_bytes[slot] = base;
+    h->crop_px_off[slot] = 0;
+  }
   RefineJob rj;
   for (int i = 0; i < n; ++i) {
     const ctd_page_entry& e = pg[size_t(i)];
@@ -441,6 +527,24 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
   // enqueued here, not at submit: a wait enqueued at submit time would also hold this batch's phase C behind the
   // forward of every batch submitted before the worker reached it
   CK(cudaStreamWaitEvent(st, h->ev_out_ready[slot], 0));   // phase C never starts before its phase A copy
+  if (!rg.tiles.empty()) {
+    // crops: tables staged in the slot's pinned crop buffer, one launch over the pages in place in d_pg_in[slot], the
+    // pixels back into the same pinned buffer after the tables.  Both buffers grow only after `st` is idle, since an
+    // earlier failed job of this slot may have left copies on it.
+    const size_t tb = rg.table_bytes(), px = h->crop_bytes[slot];
+    if (tb + px > h->crop_dcap[slot] || tb + px > h->crop_hcap[slot]) CK(cudaStreamSynchronize(st));
+    if (int rc = grow_slot_buffer(h, &h->d_crop[slot], &h->crop_dcap[slot], tb + px)) return rc;
+    if (int rc = grow_slot_pinned(h, &h->h_crop[slot], &h->crop_hcap[slot], tb + px)) return rc;
+    uint8_t* d_tab = h->d_crop[slot];
+    rg.write_tables(reinterpret_cast<char*>(h->h_crop[slot]));
+    CK(cudaMemcpyAsync(d_tab, h->h_crop[slot], tb, cudaMemcpyHostToDevice, st));
+    const size_t rb = (rg.regs.size() * sizeof(ctd::RegionDev) + 255) / 256 * 256;
+    CK(ctd::warp_regions_launch(h->d_pg_in[slot], reinterpret_cast<const ctd::RegionDev*>(d_tab),
+                                reinterpret_cast<const ctd::RegionTile*>(d_tab + rb), int(rg.tiles.size()), d_tab + tb,
+                                st));
+    CK(cudaMemcpyAsync(h->h_crop[slot] + tb, d_tab + tb, px, cudaMemcpyDeviceToHost, st));
+    h->crop_px_off[slot] = tb;
+  }
   const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);   // pixels of all planes of the batch
   uint8_t* d_res = h->d_pg_res[slot];
   uint8_t* d_mask = d_res + hd.masks;
@@ -589,6 +693,13 @@ void ctd_pipeline_shutdown(ctd_handle* h) {
     h->d_pg_tab[i] = nullptr;
     h->h_pg_tab[i] = nullptr;
   }
+  for (int i = 0; i < 2; ++i) {
+    cudaFree(h->d_crop[i]);
+    if (h->h_crop[i]) cudaFreeHost(h->h_crop[i]);
+    h->d_crop[i] = h->h_crop[i] = nullptr;
+    h->crop_dcap[i] = h->crop_hcap[i] = 0;
+    h->crop_ready[i] = false;
+  }
   cudaFree(h->d_pg_cc);
   h->d_pg_cc = nullptr;
   h->pg_cc_cap = 0;
@@ -605,6 +716,7 @@ extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages
   ShapePlan* sp = nullptr;
   if (int rc = prepare_forward(h, n, ph, pw, &sp)) return rc;
   if (int rc = ensure_full_pipeline(h)) return rc;
+  h->crop_ready[slot] = false;
   const ArenaLayout& L = h->layout;
   const size_t bytes = size_t(n) * ph * pw * 3;
   // the previous use of this slot's staging (refine reads stage_in / stage_out) ended with its collect
@@ -642,21 +754,18 @@ extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages
   return CTD_OK;
 }
 
-// device buffer of a slot, grown (never shrunk) to `bytes`; only called while the slot is idle
-static int grow_slot_buffer(ctd_handle* h, uint8_t** buf, size_t* cap, size_t bytes) {
-  if (bytes <= *cap) return CTD_OK;
-  cudaFree(*buf);
-  *buf = nullptr;
-  *cap = 0;
-  CK(cudaMalloc(reinterpret_cast<void**>(buf), bytes + bytes / 4));
-  *cap = bytes + bytes / 4;
-  return CTD_OK;
-}
-
 extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
                                 int32_t net_w, const uint8_t* input_host, int32_t refine_mode, int32_t keep_undetected,
                                 void* results_host) {
+  return ctd_submit_pages_regions(h, slot, pages, n, net_h, net_w, input_host, refine_mode, keep_undetected, 0,
+                                  results_host);
+}
+
+extern "C" int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
+                                        int32_t net_h, int32_t net_w, const uint8_t* input_host, int32_t refine_mode,
+                                        int32_t keep_undetected, int32_t textheight, void* results_host) {
   if (!h || !pages || !input_host || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (textheight != 0 && textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
   if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit_pages needs the full pipeline");
   if (h->slot_busy[slot]) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
   if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
@@ -677,6 +786,7 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   const PagesHead hd = pages_head(n);
   const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);
   const size_t d2h = size_t(pg[0].refined_off);                       // phase-A rows + masks
+  h->crop_ready[slot] = false;
   if (int rc = grow_slot_buffer(h, &h->d_pg_in[slot], &h->pg_in_cap[slot], in_bytes)) return rc;
   if (int rc = grow_slot_buffer(h, &h->d_pg_res[slot], &h->pg_res_cap[slot], d2h + total)) return rc;
   if (keep_undetected)
@@ -721,12 +831,14 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
     job.results_host = results_host;
     job.pages = std::move(pg);
     job.keep_undetected = keep_undetected ? 1 : 0;
+    job.textheight = textheight;
     h->pipe_state[slot] = 1;
     h->pipe_queue.push_back(std::move(job));
   }
   h->pipe_cv.notify_one();
   h->slot_busy[slot] = true;
   h->slot_full[slot] = true;
+  h->crop_ready[slot] = textheight > 0;   // cleared again if the batch fails
   return CTD_OK;
 }
 
@@ -741,8 +853,24 @@ int ctd_collect_full(ctd_handle* h, int slot) {
     h->pipe_state[slot] = 0;
   }
   h->slot_full[slot] = false;
-  if (rc != CTD_OK) return rc;
+  if (rc != CTD_OK) {
+    h->crop_ready[slot] = false;
+    return rc;
+  }
   CK(cudaEventSynchronize(h->ev_post_done[slot]));
+  return CTD_OK;
+}
+
+extern "C" int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region** plan, int32_t* n_regions,
+                                   const int32_t** page_first, const uint8_t** pixels, size_t* bytes) {
+  if (!h || slot < 0 || slot > 1 || !plan || !n_regions || !page_first || !pixels || !bytes) return CTD_E_INVALID;
+  if (h->slot_busy[slot] || !h->crop_ready[slot])
+    return ctd_fail(h, CTD_E_INVALID, "slot %d holds no collected ctd_submit_pages_regions batch", slot);
+  *plan = h->crop_plan[slot].data();
+  *n_regions = int32_t(h->crop_plan[slot].size());
+  *page_first = h->crop_first[slot].data();
+  *bytes = h->crop_bytes[slot];
+  *pixels = h->crop_bytes[slot] ? h->h_crop[slot] + h->crop_px_off[slot] : nullptr;
   return CTD_OK;
 }
 

@@ -1,12 +1,13 @@
 // Text-line crops (C ABI `ctd_transform_regions`, include/ctd_b200.h): `cv2.warpPerspective(img, M, (w, h))` with
 // INTER_LINEAR / BORDER_CONSTANT 0, followed for vertical lines by `cv2.rotate(.., ROTATE_90_COUNTERCLOCKWISE)`, for
 // every line of a page in ONE launch (reference utils/textblock.py:162-194; the matrices come from ctd_region_plan,
-// csrc/region_plan.cpp).
+// csrc/region_plan.cpp).  The same kernel crops every line of every page of a ctd_submit_pages_regions batch in one
+// launch (pipeline.cu): each crop record carries its page's byte offset and size, so the pages are read in place.
 //
-// Work split: the host cuts every crop into tiles of kTilePx consecutive output pixels (row-major in the RETURNED array,
-// i.e. after the rotation) and uploads a tile table {region, first pixel}; one CTA per tile, one thread per output
-// pixel, all three channels, the rotation folded into the index map.  A crop of 48 x 4000 px is spread over 750 CTAs,
-// a 48 x 60 one takes 12, so the grid is balanced whatever the mix of line lengths.
+// Work split: the host (RegionJob) cuts every crop into tiles of kRegionTilePx consecutive output pixels (row-major in
+// the RETURNED array, i.e. after the rotation) and uploads a tile table {region, first pixel}; one CTA per tile, one
+// thread per output pixel, all three channels, the rotation folded into the index map.  A crop of 48 x 4000 px is
+// spread over 750 CTAs, a 48 x 60 one takes 12, so the grid is balanced whatever the mix of line lengths.
 //
 // Sampling, bit-exact with OpenCV's fixed-point warp (imgwarp.cpp's perspective invoker + remap's bilinear path):
 //   X0 = (M0*xb + M1*y) + M2,  W = (M6*xb + M7*y) + M8 + M6*x1,  W = W ? 32/W : 0,  X = rint((X0 + M0*x1) * W)
@@ -35,22 +36,18 @@
 
 namespace {
 
-constexpr int kTilePx = 256;   // output pixels per CTA = threads per CTA
+using ctd::kRegionTilePx;
+using ctd::RegionDev;
+using ctd::RegionTile;
 
-struct RegionDev {
-  long long offset;        // byte offset of the crop in the packed output
-  int out_h, out_w;        // returned shape
-  int warp_w, bw0;         // width of the warped (un-rotated) image, OpenCV's block width
-  int rotate, pad;
-  double m[9];             // inverse homography (destination -> page)
-};
-struct Tile { int region, first; };
-
-__global__ void __launch_bounds__(kTilePx) k_warp_regions(const uint8_t* __restrict__ page, int ih, int iw,
-                                                         const RegionDev* __restrict__ regs,
-                                                         const Tile* __restrict__ tiles, uint8_t* __restrict__ out) {
-  const Tile t = tiles[blockIdx.x];
+__global__ void __launch_bounds__(kRegionTilePx) k_warp_regions(const uint8_t* __restrict__ pages,
+                                                               const RegionDev* __restrict__ regs,
+                                                               const RegionTile* __restrict__ tiles,
+                                                               uint8_t* __restrict__ out) {
+  const RegionTile t = tiles[blockIdx.x];
   const RegionDev& r = regs[t.region];
+  const uint8_t* page = pages + r.page_off;
+  const int ih = r.ih, iw = r.iw;
   const int p = t.first + int(threadIdx.x);
   const int ow = r.out_w;
   if (p >= r.out_h * ow) return;
@@ -100,27 +97,30 @@ __global__ void __launch_bounds__(kTilePx) k_warp_regions(const uint8_t* __restr
 
 }  // namespace
 
-extern "C" int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t page_on_device,
-                                     const ctd_region* plan, int32_t n, uint8_t* pixels_out, size_t pixels_bytes) {
-  if (!h || !page || n < 0 || (n > 0 && !plan)) return CTD_E_INVALID;
-  if (ih < 1 || iw < 1) return ctd_fail(h, CTD_E_SHAPE, "bad page size %dx%d", ih, iw);
-  std::vector<RegionDev> regs;
-  std::vector<Tile> tiles;
-  size_t total = 0;
+cudaError_t ctd::warp_regions_launch(const uint8_t* d_pages, const RegionDev* d_regs, const RegionTile* d_tiles,
+                                     int n_tiles, uint8_t* d_out, cudaStream_t s) {
+  if (n_tiles <= 0) return cudaSuccess;
+  k_warp_regions<<<unsigned(n_tiles), kRegionTilePx, 0, s>>>(d_pages, d_regs, d_tiles, d_out);
+  return cudaGetLastError();
+}
+
+int RegionJob::add(const ctd_region* plan, int n, long long page_off, int ih, int iw, long long out_base) {
   for (int i = 0; i < n; ++i) {
     const ctd_region& r = plan[i];
     if (r.status != 0) continue;
     if (r.out_h < 1 || r.out_w < 1 || r.offset < 0 || (r.rotate != 0 && r.rotate != 1) ||
         (long long)r.out_h * r.out_w > INT_MAX / 4)
-      return ctd_fail(h, CTD_E_INVALID, "malformed plan entry %d (%dx%d at offset %lld)", i, r.out_h, r.out_w,
-                      (long long)r.offset);
+      return i;
     const size_t px = size_t(r.out_h) * r.out_w;
-    total = std::max(total, size_t(r.offset) + px * 3);
+    out_bytes = std::max(out_bytes, size_t(out_base + r.offset) + px * 3);
     RegionDev d{};
-    d.offset = r.offset;
+    d.offset = out_base + r.offset;
+    d.page_off = page_off;
     d.out_h = r.out_h;
     d.out_w = r.out_w;
     d.rotate = r.rotate;
+    d.ih = ih;
+    d.iw = iw;
     const int ww = r.rotate ? r.out_h : r.out_w, wh = r.rotate ? r.out_w : r.out_h;
     d.warp_w = ww;
     const int bh0 = std::min(16, wh);   // OpenCV's block shape for a ww x wh destination
@@ -128,32 +128,53 @@ extern "C" int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t
     memcpy(d.m, r.inverse, sizeof(d.m));
     const int ri = int(regs.size());
     regs.push_back(d);
-    for (size_t f = 0; f < px; f += kTilePx) tiles.push_back(Tile{ri, int(f)});
+    for (size_t f = 0; f < px; f += kRegionTilePx) tiles.push_back(RegionTile{ri, int(f)});
   }
+  return -1;
+}
+
+static size_t al256(size_t v) { return (v + 255) / 256 * 256; }
+size_t RegionJob::table_bytes() const {
+  return al256(regs.size() * sizeof(RegionDev)) + al256(tiles.size() * sizeof(RegionTile));
+}
+void RegionJob::write_tables(char* dst) const {
+  memcpy(dst, regs.data(), regs.size() * sizeof(RegionDev));
+  memcpy(dst + al256(regs.size() * sizeof(RegionDev)), tiles.data(), tiles.size() * sizeof(RegionTile));
+}
+
+extern "C" int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t page_on_device,
+                                     const ctd_region* plan, int32_t n, uint8_t* pixels_out, size_t pixels_bytes) {
+  if (!h || !page || n < 0 || (n > 0 && !plan)) return CTD_E_INVALID;
+  if (ih < 1 || iw < 1) return ctd_fail(h, CTD_E_SHAPE, "bad page size %dx%d", ih, iw);
+  RegionJob job;
+  if (int bad = job.add(plan, n, 0, ih, iw, 0); bad >= 0) {
+    const ctd_region& r = plan[bad];
+    return ctd_fail(h, CTD_E_INVALID, "malformed plan entry %d (%dx%d at offset %lld)", bad, r.out_h, r.out_w,
+                    (long long)r.offset);
+  }
+  const size_t total = job.out_bytes;
   if (total > 0 && !pixels_out) return CTD_E_INVALID;
   if (pixels_bytes < total)
     return ctd_fail(h, CTD_E_CAPACITY, "the crops need %zu bytes, the output holds %zu", total, pixels_bytes);
-  if (tiles.empty()) return CTD_OK;
-  if (tiles.size() > size_t(INT_MAX)) return ctd_fail(h, CTD_E_INVALID, "too many crop pixels");
+  if (job.tiles.empty()) return CTD_OK;
+  if (job.tiles.size() > size_t(INT_MAX)) return ctd_fail(h, CTD_E_INVALID, "too many crop pixels");
   CK(cudaSetDevice(h->cfg.device));
-  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
-  const size_t rb = al(regs.size() * sizeof(RegionDev)), tb = al(tiles.size() * sizeof(Tile));
-  const size_t pb = page_on_device ? 0 : al(size_t(ih) * iw * 3);
-  if (int rc = ensure_io_scratch(h, rb + tb + pb + total)) return rc;
+  const size_t tb = job.table_bytes();
+  const size_t rb = al256(job.regs.size() * sizeof(RegionDev));
+  const size_t pb = page_on_device ? 0 : al256(size_t(ih) * iw * 3);
+  if (int rc = ensure_io_scratch(h, tb + pb + total)) return rc;
   char* base = reinterpret_cast<char*>(h->d_io_scratch);
-  std::vector<char> stage(rb + tb);
-  memcpy(stage.data(), regs.data(), regs.size() * sizeof(RegionDev));
-  memcpy(stage.data() + rb, tiles.data(), tiles.size() * sizeof(Tile));
-  CK(cudaMemcpyAsync(base, stage.data(), rb + tb, cudaMemcpyHostToDevice, h->stream));
+  std::vector<char> stage(tb);
+  job.write_tables(stage.data());
+  CK(cudaMemcpyAsync(base, stage.data(), tb, cudaMemcpyHostToDevice, h->stream));
   const uint8_t* d_page = page;
   if (!page_on_device) {
-    CK(cudaMemcpyAsync(base + rb + tb, page, size_t(ih) * iw * 3, cudaMemcpyHostToDevice, h->stream));
-    d_page = reinterpret_cast<const uint8_t*>(base + rb + tb);
+    CK(cudaMemcpyAsync(base + tb, page, size_t(ih) * iw * 3, cudaMemcpyHostToDevice, h->stream));
+    d_page = reinterpret_cast<const uint8_t*>(base + tb);
   }
-  uint8_t* d_out = reinterpret_cast<uint8_t*>(base + rb + tb + pb);
-  k_warp_regions<<<unsigned(tiles.size()), kTilePx, 0, h->stream>>>(d_page, ih, iw, reinterpret_cast<const RegionDev*>(base),
-                                                                    reinterpret_cast<const Tile*>(base + rb), d_out);
-  CK(cudaGetLastError());
+  uint8_t* d_out = reinterpret_cast<uint8_t*>(base + tb + pb);
+  CK(ctd::warp_regions_launch(d_page, reinterpret_cast<const RegionDev*>(base),
+                              reinterpret_cast<const RegionTile*>(base + rb), int(job.tiles.size()), d_out, h->stream));
   CK(cudaMemcpyAsync(pixels_out, d_out, total, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return CTD_OK;

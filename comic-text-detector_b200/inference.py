@@ -4,7 +4,8 @@ Same constructor and call signature as the reference's `inference.TextDetector`
 (inference.py:116-178): `TextDetector(model_path, input_size=1024, device=..., half=False, nms_thresh=0.35,
 conf_thresh=0.4, mask_thresh=0.3, act='leaky')` and
 `detector(img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False) -> (mask, mask_refined, blk_list)`.
-`detect_batch` / `detect_stream` give the same results for many pages of any sizes, batched on the GPU.
+`detect_batch` / `detect_stream` give the same results for many pages of any sizes, batched on the GPU, and with a
+`textheight` also the OCR crops of every text line (`get_transformed_regions`), cut in the same batches.
 
 Everything runs in libctd_b200.so: network, NMS, mask u8, DB binarize, connected components, contour boxes + scores,
 refine_mask on the GPU; ratio scaling, `group_output` and the window expansion in host C++ (csrc/group.cpp,
@@ -19,7 +20,8 @@ import numpy as np
 
 from . import compiler
 from .binding import Engine, PREC_FP16_TC, PREC_FP32_SIMT
-from .textblock import TextBlock, blocks_from_records, group_output, overlap_area, transformed_regions  # noqa: F401
+from .textblock import (TextBlock, _check_textheight, blocks_from_records, group_output, overlap_area,  # noqa: F401
+                        transformed_regions)
 
 REFINEMASK_INPAINT = 0
 REFINEMASK_ANNOTATION = 1
@@ -106,19 +108,36 @@ class TextDetector:
         naming the block and the line, before any GPU work if the reference would raise on a line."""
         return transformed_regions(self.net, img, blk_list, textheight)
 
-    def detect_batch(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
+    def detect_batch(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, textheight=None):
         """`[self(img, refine_mode, keep_undetected_mask) for img in imgs]`, with the same results byte for byte, computed
         in GPU batches of up to `max_batch` pages of any sizes (see detect_stream).  Every page is checked before any
-        GPU work: a page that is not u8 [h][w][3] raises ValueError."""
+        GPU work: a page that is not u8 [h][w][3] raises ValueError.  With a textheight, each result is the 4-tuple
+        detect_stream yields, crops included."""
         imgs = [check_page(img) for img in imgs]
-        return list(self.detect_stream(imgs, refine_mode, keep_undetected_mask))
+        return list(self.detect_stream(imgs, refine_mode, keep_undetected_mask, textheight))
 
-    def detect_stream(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
+    def detect_stream(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, textheight=None):
         """Generator over an iterable of pages: yields `(mask, mask_refined, blk_list)` for each page in input order,
         equal to `self(img, refine_mode, keep_undetected_mask)`.  Pages are grouped into batches of up to `max_batch`
         and two batches are kept in flight (`ctd_submit_pages`): while one batch runs on the GPU and in the engine's
         host stage, the next one is read from `imgs` and packed.  A page that is not u8 [h][w][3] raises ValueError
-        before it reaches the GPU."""
+        before it reaches the GPU.
+
+        textheight (an integer >= 2; checked here, before any page is read): yields `(mask, mask_refined, blk_list,
+        crops)` instead, where crops[b][i] is line i of blk_list[b] cut out as `get_transformed_regions(img, blk_list,
+        textheight)` cuts it, byte for byte, except that a line on which the reference's `get_transformed_region`
+        raises (a crop side of 1 px, a degenerate quad; or a side of 32767 px or more) gets None instead of raising,
+        so one such line does not end the stream.  The crops are planned on the engine's worker threads and cut in
+        one GPU launch per batch from the pages already in device memory (`ctd_submit_pages_regions`).  Each page's
+        crops are views into one array of that page's own."""
+        th = 0
+        if textheight is not None:
+            th = _check_textheight(textheight)
+            if th < 2:
+                raise ValueError("textheight must be at least 2 px, got %r" % (textheight,))
+        return self._stream(imgs, refine_mode, keep_undetected_mask, th)
+
+    def _stream(self, imgs, refine_mode, keep_undetected_mask, th):
         net_h, net_w = self.input_size
         inflight = deque()   # slots in submission order
         free = [0, 1]
@@ -131,14 +150,14 @@ class TextDetector:
                 if not free:
                     yield from self._collect(inflight, free)
                 slot = free.pop(0)
-                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask)
+                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask, th)
                 inflight.append(slot)
                 batch = []
             if batch:
                 if not free:
                     yield from self._collect(inflight, free)
                 slot = free.pop(0)
-                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask)
+                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask, th)
                 inflight.append(slot)
             while inflight:
                 yield from self._collect(inflight, free)
@@ -154,8 +173,8 @@ class TextDetector:
         slot = inflight.popleft()
         pages = self.net.collect_pages(slot)
         free.append(slot)
-        for mask, mask_refined, rec, lines, dist in pages:
-            yield mask, mask_refined, blocks_from_records(rec, lines, dist)
+        for mask, mask_refined, rec, lines, dist, *crops in pages:
+            yield (mask, mask_refined, blocks_from_records(rec, lines, dist)) + tuple(crops)
 
 
 def check_page(img):

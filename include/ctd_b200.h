@@ -432,6 +432,25 @@ CTD_API int ctd_region_plan(const ctd_region_line* lines, int32_t n, int32_t im_
  * CTD_E_SHAPE for a bad page size, CTD_E_INVALID for a malformed plan entry.                                       */
 CTD_API int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t page_on_device,
                                   const ctd_region* plan, int32_t n, uint8_t* pixels_out, size_t pixels_bytes);
+/* ctd_submit_pages plus the OCR crops of every text line of every page of the batch (ctd_region_plan above):
+ * the same batch, and with textheight = 0 exactly ctd_submit_pages (ctd_submit_pages is this call with textheight 0).
+ * textheight >= 2 (else CTD_E_INVALID): the handle's worker plans each page's lines with ctd_region_plan right after
+ * its group_output, on the same host threads, then one k_warp_regions launch on the post stream cuts every status-0
+ * crop of every page out of the pages where they already are in device memory, and the pixels are copied back into a
+ * pinned buffer of the handle before the batch counts as done.  A batch without a single crop launches and allocates
+ * nothing.  A page the planner refuses (a side >= 32767) fails the batch, and ctd_collect names the page.      */
+CTD_API int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                                     int32_t net_w, const uint8_t* input_host, int32_t refine_mode,
+                                     int32_t keep_undetected, int32_t textheight, void* results_host);
+/* After ctd_collect(h, slot) of a ctd_submit_pages_regions batch with textheight > 0: the concatenated ctd_region
+ * plans of the batch, *n_regions entries in page, then block, then line order (the order of each page's block
+ * section), page i's entries at [(*page_first)[i], (*page_first)[i + 1]) (n + 1 values), and the packed crops,
+ * *bytes bytes at *pixels (HOST, NULL when *bytes is 0).  Each entry's offset is relative to *pixels; page i's crops
+ * follow page i - 1's.  Entries with status != 0 have no bytes, exactly as ctd_region_plan gives them.  All pointers
+ * belong to the handle and stay valid until the slot's next submission or ctd_destroy.  CTD_E_INVALID for a slot that
+ * is in flight or whose last collected batch did not ask for crops.                                            */
+CTD_API int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region** plan, int32_t* n_regions,
+                                const int32_t** page_first, const uint8_t** pixels, size_t* bytes);
 
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
  * [rows][5+nc]); output as ctd_get_detections for one page.                                */
