@@ -66,6 +66,13 @@ REGION_DTYPE = np.dtype([("out_h", np.int32), ("out_w", np.int32), ("rotate", np
                          ("offset", np.int64), ("homography", np.float64, (9,)), ("inverse", np.float64, (9,))],
                         align=True)
 
+
+class CtdDevicePage(C.Structure):
+    """ctypes mirror of `ctd_device_page` (include/ctd_b200.h)"""
+    _fields_ = [("data", C.c_void_p), ("stride_h", C.c_int64), ("stride_w", C.c_int64), ("stride_c", C.c_int64),
+                ("event", C.c_void_p)]
+
+
 EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_get_net_outputs", "ctd_get_mask_u8",
            "ctd_get_detections", "ctd_get_db_components", "ctd_last_forward_ms", "ctd_last_launch_count",
            "ctd_debug_read_buffer", "ctd_debug_write_buffer", "ctd_connected_components", "ctd_nms",
@@ -75,7 +82,7 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_resize_linear_u8", "ctd_debug_run_ops", "ctd_get_nms_status", "ctd_group_output",
            "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena",
            "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
-           "ctd_submit_pages_regions", "ctd_collect_regions"]
+           "ctd_submit_pages_regions", "ctd_collect_regions", "ctd_submit_pages_device", "ctd_collect_device"]
 
 _lib = None
 
@@ -140,6 +147,8 @@ def load_library():
     lib.ctd_submit_pages_regions.argtypes = [vp, i32, vp, i32, i32, i32, vp, i32, i32, i32, vp]
     lib.ctd_collect_regions.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i32), C.POINTER(vp), C.POINTER(vp),
                                         C.POINTER(C.c_size_t)]
+    lib.ctd_submit_pages_device.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, i32, i32, i32, i32, vp]
+    lib.ctd_collect_device.argtypes = [vp, i32, vp]
     for name in EXPORTS[3:]:
         getattr(lib, name).restype = C.c_int
     lib.ctd_expand_textwindow.restype = None
@@ -189,6 +198,36 @@ def decode_block_section(sec, layout):
     return hdr, rec, lines, dist
 
 
+class _BatchPlan:
+    """The concatenated crop plan of a collected batch (ctd_collect_regions): page p's entries are
+    [first[p], first[p + 1]), its crops the bytes page_range(p) of the batch's packed crops."""
+
+    def __init__(self, plan, first, pixels, total):
+        self.first, self.pixels, self.total = first, pixels, total
+        self.off, self.oh, self.ow = plan["offset"].tolist(), plan["out_h"].tolist(), plan["out_w"].tolist()
+        self.ok = (plan["status"] == 0).tolist()
+
+    def page_range(self, p):
+        a, b = self.first[p], self.first[p + 1]
+        if b == a:
+            return 0, 0
+        return self.off[a], self.off[b - 1] + self.oh[b - 1] * self.ow[b - 1] * 3
+
+    def page_crops(self, p, counts, view):
+        """page p's crops: per block (counts = its lines) a list of [h][w][3] arrays, view(o, h, w) for the crop at
+        byte o from the page's first crop, None where the planner gives no crop"""
+        a, b = self.first[p], self.first[p + 1]
+        counts = np.asarray(counts).tolist()
+        assert sum(counts) == b - a, (p, sum(counts), b - a)
+        off, oh, ow, ok = self.off, self.oh, self.ow, self.ok
+        lo = off[a] if b > a else 0
+        page, k = [], a
+        for c in counts:
+            page.append([view(off[j] - lo, oh[j], ow[j]) if ok[j] else None for j in range(k, k + c)])
+            k += c
+        return page
+
+
 class Engine:
     """One engine handle = one GPU + one stream + one compiled program."""
 
@@ -196,6 +235,7 @@ class Engine:
                  conf_thresh=0.4, nms_thresh=0.35, db_thresh=0.3, skip_postproc=False):
         self.lib = load_library()
         self.h = C.c_void_p()
+        self.device = int(device)
         self.program = program
         self.nc = int(getattr(program, "nc", 2))
         ops = (CtdOp * len(program.ops))()
@@ -433,57 +473,128 @@ class Engine:
     def collect(self, slot):
         self._ck(self.lib.ctd_collect(self.h, slot))
 
-    def submit_pages(self, slot, pages, net_h, net_w, refine_mode=0, keep_undetected=False, textheight=0):
-        """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages_regions): the pages (u8
-        [h][w][3] each) are packed into this slot's pinned input buffer, which like the pinned results buffer belongs to
-        the engine and grows on demand.  textheight >= 2 also crops every text line of every page on the GPU
-        (0: no crops).  Collect with collect_pages(slot)."""
+    def submit_pages(self, slot, pages, net_h, net_w, refine_mode=0, keep_undetected=False, textheight=0, events=None,
+                     device_results=False):
+        """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages_device).  A page is a u8
+        [h][w][3] numpy array, packed into this slot's pinned input buffer (which like the pinned results buffer belongs
+        to the engine and grows on demand), or a torch.uint8 CUDA tensor [h][w][3] on this engine's GPU with any
+        strides, gathered on the GPU without a host copy; events[i] (a recorded torch.cuda.Event, or None) is waited on
+        before CUDA page i is read.  The CUDA pages are referenced until the slot is collected and must not be written
+        before.  textheight >= 2 also crops every text line of every page on the GPU (0: no crops).  device_results:
+        masks and crops stay on the GPU (see collect_pages).  Collect with collect_pages(slot)."""
         import torch
         if not hasattr(self, "_pg_bufs"):
             self._pg_bufs = [[None, None], [None, None]]   # per slot: pinned input, pinned results
             self._pg_inflight = [None, None]
         if self._pg_inflight[slot] is not None:
             raise CtdError("slot %d has an uncollected submission" % slot)
-        entries, in_bytes, res_bytes = pages_plan([p.shape[:2] for p in pages], net_h, net_w)
+        entries, in_bytes, res_bytes = pages_plan([tuple(p.shape[:2]) for p in pages], net_h, net_w)
+        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
         bufs = self._pg_bufs[slot]
-        for k, need in ((0, in_bytes), (1, res_bytes)):
-            if bufs[k] is None or bufs[k].numel() < need:
-                bufs[k] = torch.empty((max(need, 1) * 5 // 4,), dtype=torch.uint8, pin_memory=True)
-        inp = bufs[0].numpy()
-        for e, p in zip(entries, pages):
-            o = int(e["page_off"])
-            np.copyto(inp[o:o + p.size].reshape(p.shape), p)
-        self._ck(self.lib.ctd_submit_pages_regions(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
-                                                   C.c_void_p(bufs[0].data_ptr()), int(refine_mode),
-                                                   int(bool(keep_undetected)), int(textheight),
-                                                   C.c_void_p(bufs[1].data_ptr())))
-        self._pg_inflight[slot] = (entries, int(textheight))
+        for k, need in ((0, 0 if all(on_dev) else in_bytes), (1, res_bytes)):
+            if need and (bufs[k] is None or bufs[k].numel() < need):
+                bufs[k] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        dev = None
+        if any(on_dev):
+            dev = (CtdDevicePage * len(pages))()
+            for i, p in enumerate(pages):
+                if on_dev[i]:
+                    ev = events[i] if events is not None else None
+                    sh, sw, sc = p.stride()   # uint8: element strides are byte strides
+                    dev[i] = CtdDevicePage(p.data_ptr(), sh, sw, sc, ev.cuda_event if ev is not None else None)
+        if not all(on_dev):
+            inp = bufs[0].numpy()
+            for e, p, d in zip(entries, pages, on_dev):
+                if not d:
+                    o = int(e["page_off"])
+                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+        self._ck(self.lib.ctd_submit_pages_device(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
+                                                  None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
+                                                  None if dev is None else C.cast(dev, C.c_void_p), int(refine_mode),
+                                                  int(bool(keep_undetected)), int(textheight), int(bool(device_results)),
+                                                  C.c_void_p(bufs[1].data_ptr())))
+        kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]]
+        self._pg_inflight[slot] = (entries, int(textheight), bool(device_results), kept)
         self.shape = (len(entries), net_h, net_w)
 
-    def collect_pages(self, slot):
+    def collect_pages(self, slot, discard=False):
         """blocks until the batch of submit_pages(slot) is done -> per page the 5-tuple detect_page returns
         (mask, mask_refined, block records, lines, distances), copied out of the slot's pinned buffer.  With a
-        textheight, each tuple has a sixth element, the page's crops (see collect_regions)."""
+        textheight, each tuple has a sixth element, the page's crops (see collect_regions).  With device_results, mask,
+        mask_refined and the crops are torch.uint8 CUDA tensors, views into one allocation of that page's own (filled by
+        ctd_collect_device; complete on return).  discard: only wait for the batch and return None."""
         inflight = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
         if inflight is None:
             raise CtdError("slot %d has no submit_pages batch in flight" % slot)
-        entries, textheight = inflight
+        entries, textheight, device_results, _kept = inflight
         self._pg_inflight[slot] = None
         self.collect(slot)
+        if discard:
+            return None
         res = self._pg_bufs[slot][1].numpy()
         lay = self.results_layout()
         stride = lay["blocks_stride"]
-        out = []
+        blocks = []
         for e in entries:
-            ih, iw = int(e["ih"]), int(e["iw"])
-            mo, ro, bo = int(e["mask_off"]), int(e["refined_off"]), int(e["blocks_off"])
+            bo = int(e["blocks_off"])
             _hdr, rec, lines, dist = decode_block_section(res[bo:bo + stride], lay)
-            out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy(), res[ro:ro + ih * iw].reshape(ih, iw).copy(),
-                        rec.copy(), lines.copy(), dist.copy()))
+            blocks.append((rec.copy(), lines.copy(), dist.copy()))
+        n_lines = [b[0]["n_lines"] for b in blocks]
+        if device_results:
+            return self._collect_device(slot, entries, blocks, n_lines if textheight else None)
+        out = []
+        for e, b in zip(entries, blocks):
+            ih, iw = int(e["ih"]), int(e["iw"])
+            mo, ro = int(e["mask_off"]), int(e["refined_off"])
+            out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy(), res[ro:ro + ih * iw].reshape(ih, iw).copy()) + b)
         if textheight:
-            crops = self.collect_regions(slot, [o[2]["n_lines"] for o in out])
+            crops = self.collect_regions(slot, n_lines)
             out = [o + (c,) for o, c in zip(out, crops)]
         return out
+
+    def _collect_device(self, slot, entries, blocks, n_lines):
+        """collect_pages of a device_results batch: one CUDA allocation per page, [mask | mask_refined | crops]
+        (ctd_collect_device).  The allocations are made on a stream of the engine's own, so the caching allocator
+        cannot hand out memory that work still queued on the caller's stream uses (the copies do not wait for that
+        stream), and are marked as used on the caller's current stream."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if getattr(self, "_alloc_stream", None) is None:
+            self._alloc_stream = torch.cuda.Stream(dev)
+        plan = self._collected_plan(slot, len(entries)) if n_lines is not None else None
+        sizes = []
+        for p, e in enumerate(entries):
+            px = int(e["ih"]) * int(e["iw"])
+            lo, hi = plan.page_range(p) if plan is not None else (0, 0)
+            sizes.append((px, lo, hi))
+        with torch.cuda.stream(self._alloc_stream):
+            bufs = [torch.empty((2 * px + hi - lo,), dtype=torch.uint8, device=dev) for px, lo, hi in sizes]
+        ptrs = (C.c_void_p * len(bufs))(*[b.data_ptr() for b in bufs])
+        self._ck(self.lib.ctd_collect_device(self.h, slot, ptrs))
+        cur = torch.cuda.current_stream(dev)
+        out = []
+        for p, (e, b, buf, (px, _lo, _hi)) in enumerate(zip(entries, blocks, bufs, sizes)):
+            buf.record_stream(cur)
+            ih, iw = int(e["ih"]), int(e["iw"])
+            o = (buf[:px].view(ih, iw), buf[px:2 * px].view(ih, iw)) + b
+            if plan is not None:
+                # as_strided on the fresh allocation (storage offset 0): the cheapest view torch makes, which matters
+                # at thousands of crops per batch
+                o += (plan.page_crops(p, n_lines[p], lambda c, h, w, buf=buf, px=px:
+                                      buf.as_strided((h, w, 3), (w * 3, 3, 1), 2 * px + c)),)
+            out.append(o)
+        return out
+
+    def _collected_plan(self, slot, n_pages):
+        """the plan of the collected ctd_submit_pages_regions batch of `slot` (ctd_collect_regions)"""
+        plan_p, n_reg, first_p, pix_p, nbytes = C.c_void_p(), C.c_int32(), C.c_void_p(), C.c_void_p(), C.c_size_t()
+        self._ck(self.lib.ctd_collect_regions(self.h, slot, C.byref(plan_p), C.byref(n_reg), C.byref(first_p),
+                                              C.byref(pix_p), C.byref(nbytes)))
+        n = int(n_reg.value)
+        first = np.ctypeslib.as_array(C.cast(first_p, C.POINTER(C.c_int32)), (n_pages + 1,)).tolist()
+        plan = np.frombuffer((C.c_char * (n * REGION_DTYPE.itemsize)).from_address(plan_p.value), REGION_DTYPE) \
+            if n else np.zeros((0,), REGION_DTYPE)
+        return _BatchPlan(plan, first, pix_p.value, int(nbytes.value))
 
     def collect_regions(self, slot, n_lines):
         """the crops of the collected ctd_submit_pages_regions batch of `slot` (ctd_collect_regions): per page, per
@@ -492,30 +603,15 @@ class Engine:
         (copied out of the engine's pinned buffer by torch's multi-threaded CPU copy: a single-threaded copy into fresh
         memory was most of the cost of this call)."""
         import torch
-        plan_p, n_reg, first_p, pix_p, nbytes = C.c_void_p(), C.c_int32(), C.c_void_p(), C.c_void_p(), C.c_size_t()
-        self._ck(self.lib.ctd_collect_regions(self.h, slot, C.byref(plan_p), C.byref(n_reg), C.byref(first_p),
-                                              C.byref(pix_p), C.byref(nbytes)))
-        n, total = int(n_reg.value), int(nbytes.value)
-        first = np.ctypeslib.as_array(C.cast(first_p, C.POINTER(C.c_int32)), (len(n_lines) + 1,)).tolist()
-        plan = np.frombuffer((C.c_char * (n * REGION_DTYPE.itemsize)).from_address(plan_p.value), REGION_DTYPE) \
-            if n else np.zeros((0,), REGION_DTYPE)
-        pix = torch.from_numpy(np.ctypeslib.as_array(C.cast(pix_p, C.POINTER(C.c_uint8)), (total,))) if total else None
-        off, oh, ow = plan["offset"].tolist(), plan["out_h"].tolist(), plan["out_w"].tolist()
-        ok = (plan["status"] == 0).tolist()
+        plan = self._collected_plan(slot, len(n_lines))
+        total = plan.total
+        pix = torch.from_numpy(np.ctypeslib.as_array(C.cast(C.c_void_p(plan.pixels), C.POINTER(C.c_uint8)), (total,))) \
+            if total else None
         out = []
         for p, counts in enumerate(n_lines):
-            a, b = first[p], first[p + 1]
-            counts = np.asarray(counts).tolist()
-            assert sum(counts) == b - a, (p, sum(counts), b - a)
-            lo = off[a] if b > a else 0
-            hi = off[b - 1] + oh[b - 1] * ow[b - 1] * 3 if b > a else 0
+            lo, hi = plan.page_range(p)
             buf = torch.empty((hi - lo,), dtype=torch.uint8).copy_(pix[lo:hi]).numpy() if hi > lo else None
-            page, k = [], a
-            for c in counts:
-                page.append([buf[off[j] - lo:off[j] - lo + oh[j] * ow[j] * 3].reshape(oh[j], ow[j], 3) if ok[j] else None
-                             for j in range(k, k + c)])
-                k += c
-            out.append(page)
+            out.append(plan.page_crops(p, counts, lambda o, h, w, buf=buf: buf[o:o + h * w * 3].reshape(h, w, 3)))
         return out
 
     def join(self, other):

@@ -608,6 +608,7 @@ extern "C" int ctd_submit(ctd_handle* h, int32_t slot, const uint8_t* pages_host
   if (int rc = prepare_forward(h, n, ph, pw, &sp)) return rc;
   if (int rc = ensure_pipeline(h)) return rc;
   h->crop_ready[slot] = false;
+  h->dev_ready[slot] = false;
   const size_t bytes = size_t(n) * ph * pw * 3;
   CK(cudaStreamWaitEvent(h->copy_in, h->ev_in_free[slot], 0));   // no-op before the slot's first use
   CK(cudaMemcpyAsync(h->d_stage_in[slot], pages_host, bytes, cudaMemcpyHostToDevice, h->copy_in));

@@ -80,6 +80,7 @@ struct PipeJob {
   std::vector<ctd_page_entry> pages;
   int keep_undetected = 0;
   int textheight = 0;   // > 0: also crop every text line of every page (ctd_submit_pages_regions)
+  int results_on_device = 0;   // mask_refined, the modified mask and the crops stay on the device (ctd_collect_device)
 };
 
 // refine windows of one launch (all pages of a batch) and the chunks they are cut into
@@ -186,13 +187,20 @@ struct ctd_handle {
   int host_threads = 4;
   // any-size batches (ctd_submit_pages): per-slot device planes (packed pages | results head, masks, mask_refined |
   // second refine output and threshold planes of refine_undetected_mask), grown while the slot is idle; per-slot page
-  // tables (pinned + device, max_batch entries); the worker's own connected-components scratch
+  // tables (pinned + device: max_batch PageGeom entries, then at pg_gather_off max_batch GatherPage entries for the
+  // pages gathered from device memory, uploaded together); the worker's own connected-components scratch
   uint8_t* d_pg_in[2] = {nullptr, nullptr};
   uint8_t* d_pg_res[2] = {nullptr, nullptr};
   uint8_t* d_pg_aux[2] = {nullptr, nullptr};
   size_t pg_in_cap[2] = {0, 0}, pg_res_cap[2] = {0, 0}, pg_aux_cap[2] = {0, 0};
   ctd::PageGeom* h_pg_tab[2] = {nullptr, nullptr};
   ctd::PageGeom* d_pg_tab[2] = {nullptr, nullptr};
+  size_t pg_gather_off = 0;
+  // results_on_device batches (ctd_submit_pages_device): the slot's page entries, whether its collected batch left
+  // its results on the device, and the stream ctd_collect_device copies on
+  std::vector<ctd_page_entry> dev_pages[2];
+  bool dev_ready[2] = {false, false};
+  cudaStream_t dev_out = nullptr;
   void* d_pg_cc = nullptr;
   size_t pg_cc_cap = 0;
   // refine scratch of the worker's phase C on the post stream (d_refine_scratch belongs to the caller's stream)
@@ -203,6 +211,7 @@ struct ctd_handle {
   // buffer (the same tables staged for upload | the pixels copied back), both grown on demand and never shrunk
   std::vector<ctd_region> crop_plan[2];
   std::vector<int32_t> crop_first[2];
+  std::vector<size_t> crop_base[2];   // n + 1 entries: page i's crops are bytes [crop_base[i], crop_base[i + 1])
   uint8_t* d_crop[2] = {nullptr, nullptr};
   uint8_t* h_crop[2] = {nullptr, nullptr};
   size_t crop_dcap[2] = {0, 0}, crop_hcap[2] = {0, 0};

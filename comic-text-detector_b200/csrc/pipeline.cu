@@ -13,6 +13,8 @@
 // ctd_submit_pages runs batches of pages of any size through the same two-in-flight schedule, with one letterbox and
 // one back-projection launch per batch (TextDetector.detect_batch / detect_stream); ctd_submit_pages_regions also cuts
 // every text line of every page of the batch out of the resident pages in one k_warp_regions launch (region.cu).
+// ctd_submit_pages_device is the one implementation behind both: pages may already be in device memory (any strides;
+// one gather_pages_kernel launch packs them, gather.cu) and the masks and crops may stay there (ctd_collect_device).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -494,8 +496,10 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
   if (crops) {
     std::vector<ctd_region>& plan = h->crop_plan[slot];
     std::vector<int32_t>& first = h->crop_first[slot];
+    std::vector<size_t>& page_base = h->crop_base[slot];
     plan.clear();
     first.assign(size_t(n) + 1, 0);
+    page_base.assign(size_t(n) + 1, 0);
     size_t base = 0;
     for (int i = 0; i < n; ++i) {
       const ctd_page_entry& e = pg[size_t(i)];
@@ -503,6 +507,7 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
       if (int bad = rg.add(p.data(), int(p.size()), e.page_off, e.ih, e.iw, (long long)base); bad >= 0)
         return ctd_fail(h, CTD_E_INVALID, "malformed crop plan entry %d on page %d of the batch", bad, i);
       first[size_t(i)] = int32_t(plan.size());
+      page_base[size_t(i)] = base;
       for (ctd_region r : p) {
         r.offset += int64_t(base);
         plan.push_back(r);
@@ -510,6 +515,7 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
       base += plan_bytes[size_t(i)];
     }
     first[size_t(n)] = int32_t(plan.size());
+    page_base[size_t(n)] = base;
     if (plan.size() > size_t(INT32_MAX) || rg.tiles.size() > size_t(INT32_MAX))
       return ctd_fail(h, CTD_E_CAPACITY, "too many crops in one batch");
     h->crop_bytes[slot] = base;
@@ -527,14 +533,17 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
   // enqueued here, not at submit: a wait enqueued at submit time would also hold this batch's phase C behind the
   // forward of every batch submitted before the worker reached it
   CK(cudaStreamWaitEvent(st, h->ev_out_ready[slot], 0));   // phase C never starts before its phase A copy
+  const bool to_host = !job.results_on_device;
   if (!rg.tiles.empty()) {
     // crops: tables staged in the slot's pinned crop buffer, one launch over the pages in place in d_pg_in[slot], the
-    // pixels back into the same pinned buffer after the tables.  Both buffers grow only after `st` is idle, since an
-    // earlier failed job of this slot may have left copies on it.
+    // pixels back into the same pinned buffer after the tables (unless they stay on the device, after the tables in
+    // d_crop[slot]).  Both buffers grow only after `st` is idle, since an earlier failed job of this slot may have left
+    // copies on it.
     const size_t tb = rg.table_bytes(), px = h->crop_bytes[slot];
-    if (tb + px > h->crop_dcap[slot] || tb + px > h->crop_hcap[slot]) CK(cudaStreamSynchronize(st));
+    const size_t host_need = to_host ? tb + px : tb;
+    if (tb + px > h->crop_dcap[slot] || host_need > h->crop_hcap[slot]) CK(cudaStreamSynchronize(st));
     if (int rc = grow_slot_buffer(h, &h->d_crop[slot], &h->crop_dcap[slot], tb + px)) return rc;
-    if (int rc = grow_slot_pinned(h, &h->h_crop[slot], &h->crop_hcap[slot], tb + px)) return rc;
+    if (int rc = grow_slot_pinned(h, &h->h_crop[slot], &h->crop_hcap[slot], host_need)) return rc;
     uint8_t* d_tab = h->d_crop[slot];
     rg.write_tables(reinterpret_cast<char*>(h->h_crop[slot]));
     CK(cudaMemcpyAsync(d_tab, h->h_crop[slot], tb, cudaMemcpyHostToDevice, st));
@@ -542,7 +551,7 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
     CK(ctd::warp_regions_launch(h->d_pg_in[slot], reinterpret_cast<const ctd::RegionDev*>(d_tab),
                                 reinterpret_cast<const ctd::RegionTile*>(d_tab + rb), int(rg.tiles.size()), d_tab + tb,
                                 st));
-    CK(cudaMemcpyAsync(h->h_crop[slot] + tb, d_tab + tb, px, cudaMemcpyDeviceToHost, st));
+    if (to_host) CK(cudaMemcpyAsync(h->h_crop[slot] + tb, d_tab + tb, px, cudaMemcpyDeviceToHost, st));
     h->crop_px_off[slot] = tb;
   }
   const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);   // pixels of all planes of the batch
@@ -567,9 +576,9 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
                                    st, &h->d_pg_cc, &h->pg_cc_cap, &h->d_post_refine, &h->post_refine_cap,
                                    h->pipe_pinned[slot], h->pipe_pinned_cap))
       return rc;
-    CK(cudaMemcpyAsync(res + hd.masks, d_mask, total, cudaMemcpyDeviceToHost, st));
+    if (to_host) CK(cudaMemcpyAsync(res + hd.masks, d_mask, total, cudaMemcpyDeviceToHost, st));
   }
-  CK(cudaMemcpyAsync(res + pg[0].refined_off, d_ref, total, cudaMemcpyDeviceToHost, st));
+  if (to_host) CK(cudaMemcpyAsync(res + pg[0].refined_off, d_ref, total, cudaMemcpyDeviceToHost, st));
   CK(cudaEventRecord(h->ev_post_done[slot], st));
   return CTD_OK;
 }
@@ -699,7 +708,10 @@ void ctd_pipeline_shutdown(ctd_handle* h) {
     h->d_crop[i] = h->h_crop[i] = nullptr;
     h->crop_dcap[i] = h->crop_hcap[i] = 0;
     h->crop_ready[i] = false;
+    h->dev_ready[i] = false;
   }
+  if (h->dev_out) cudaStreamDestroy(h->dev_out);
+  h->dev_out = nullptr;
   cudaFree(h->d_pg_cc);
   h->d_pg_cc = nullptr;
   h->pg_cc_cap = 0;
@@ -717,6 +729,7 @@ extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages
   if (int rc = prepare_forward(h, n, ph, pw, &sp)) return rc;
   if (int rc = ensure_full_pipeline(h)) return rc;
   h->crop_ready[slot] = false;
+  h->dev_ready[slot] = false;
   const ArenaLayout& L = h->layout;
   const size_t bytes = size_t(n) * ph * pw * 3;
   // the previous use of this slot's staging (refine reads stage_in / stage_out) ended with its collect
@@ -764,7 +777,26 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
 extern "C" int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
                                         int32_t net_h, int32_t net_w, const uint8_t* input_host, int32_t refine_mode,
                                         int32_t keep_undetected, int32_t textheight, void* results_host) {
-  if (!h || !pages || !input_host || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (!input_host) return CTD_E_INVALID;
+  return ctd_submit_pages_device(h, slot, pages, n, net_h, net_w, input_host, nullptr, refine_mode, keep_undetected,
+                                 textheight, 0, results_host);
+}
+
+// true when [p, p + 1) is device memory of `device` (cudaPointerGetAttributes; clears the error it may leave)
+static bool is_device_memory(const void* p, int device) {
+  cudaPointerAttributes a{};
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    return false;
+  }
+  return a.type == cudaMemoryTypeDevice && a.device == device;
+}
+
+extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
+                                       int32_t net_h, int32_t net_w, const uint8_t* input_host,
+                                       const ctd_device_page* dev, int32_t refine_mode, int32_t keep_undetected,
+                                       int32_t textheight, int32_t results_on_device, void* results_host) {
+  if (!h || !pages || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
   if (textheight != 0 && textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
   if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit_pages needs the full pipeline");
   if (h->slot_busy[slot]) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
@@ -779,6 +811,27 @@ extern "C" int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_p
   size_t rows = 0;
   for (int i = 0; i < n; ++i) rows += size_t(pg[size_t(i)].ih);
   if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
+  // pages in device memory: strides, and the first and last byte each page reads must be memory of this GPU
+  CK(cudaSetDevice(h->cfg.device));
+  int n_dev = 0;
+  for (int i = 0; i < n; ++i) {
+    if (!dev || !dev[i].data) {
+      if (!input_host) return ctd_fail(h, CTD_E_INVALID, "page %d is in neither input_host nor device memory", i);
+      continue;
+    }
+    const ctd_device_page& d = dev[i];
+    const int64_t kMaxStride = int64_t(1) << 31;   // keeps the page's last byte offset inside int64
+    if (d.stride_h < 0 || d.stride_w < 0 || d.stride_c < 0 || d.stride_h > kMaxStride || d.stride_w > kMaxStride ||
+        d.stride_c > kMaxStride)
+      return ctd_fail(h, CTD_E_INVALID, "page %d: strides (%lld, %lld, %lld) out of range [0, 2^31]", i,
+                      (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c);
+    const ctd_page_entry& e = pg[size_t(i)];
+    const uint8_t* last = d.data + (e.ih - 1) * d.stride_h + (e.iw - 1) * d.stride_w + 2 * d.stride_c;
+    if (!is_device_memory(d.data, h->cfg.device) || !is_device_memory(last, h->cfg.device))
+      return ctd_fail(h, CTD_E_INVALID, "page %d (%p) is not device memory of GPU %d", i, (const void*)d.data,
+                      h->cfg.device);
+    ++n_dev;
+  }
   ShapePlan* sp = nullptr;
   if (int rc = prepare_forward(h, n, net_h, net_w, &sp)) return rc;
   if (int rc = ensure_full_pipeline(h)) return rc;
@@ -787,29 +840,60 @@ extern "C" int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_p
   const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);
   const size_t d2h = size_t(pg[0].refined_off);                       // phase-A rows + masks
   h->crop_ready[slot] = false;
+  h->dev_ready[slot] = false;
   if (int rc = grow_slot_buffer(h, &h->d_pg_in[slot], &h->pg_in_cap[slot], in_bytes)) return rc;
   if (int rc = grow_slot_buffer(h, &h->d_pg_res[slot], &h->pg_res_cap[slot], d2h + total)) return rc;
   if (keep_undetected)
     if (int rc = grow_slot_buffer(h, &h->d_pg_aux[slot], &h->pg_aux_cap[slot], 2 * total)) return rc;
   if (!h->h_pg_tab[slot]) {
-    CK(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pg_tab[slot]), size_t(h->cfg.max_batch) * sizeof(PageGeom),
-                     cudaHostAllocDefault));
-    CK(cudaMalloc(reinterpret_cast<void**>(&h->d_pg_tab[slot]), size_t(h->cfg.max_batch) * sizeof(PageGeom)));
+    h->pg_gather_off = (size_t(h->cfg.max_batch) * sizeof(PageGeom) + 255) / 256 * 256;
+    const size_t tab_bytes = h->pg_gather_off + size_t(h->cfg.max_batch) * sizeof(GatherPage);
+    CK(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pg_tab[slot]), tab_bytes, cudaHostAllocDefault));
+    CK(cudaMalloc(reinterpret_cast<void**>(&h->d_pg_tab[slot]), tab_bytes));
   }
   PageGeom* tab = h->h_pg_tab[slot];
-  int row0 = 0;
+  GatherPage* gtab = reinterpret_cast<GatherPage*>(reinterpret_cast<char*>(tab) + h->pg_gather_off);
+  int row0 = 0, n_gather = 0, gather_rows = 0;
   for (int i = 0; i < n; ++i) {
     const ctd_page_entry& e = pg[size_t(i)];
     tab[i] = PageGeom{e.page_off, e.mask_off - int64_t(hd.masks), e.ih, e.iw, e.unpad_h, e.unpad_w, row0, 0};
     row0 += e.ih;
+    if (dev && dev[i].data) {
+      const ctd_device_page& d = dev[i];
+      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c,
+                                    (long long)e.page_off, e.ih, e.iw, gather_rows,
+                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0};
+      gather_rows += e.ih;
+    }
   }
-  // phase A: pages and table in on copy_in; letterbox, forward, back-projection and the phase-A rows on the engine
-  // stream; rows + masks out on copy_out
-  CK(cudaMemcpyAsync(h->d_pg_tab[slot], tab, size_t(n) * sizeof(PageGeom), cudaMemcpyHostToDevice, h->copy_in));
-  CK(cudaMemcpyAsync(h->d_pg_in[slot], input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
+  // phase A: tables and host pages in on copy_in (a batch with device pages copies only its host pages' byte ranges,
+  // one copy per run of consecutive host pages); the device pages' events, the gather of the device pages, letterbox,
+  // forward, back-projection and the phase-A rows on the engine stream; rows + masks out on copy_out
+  const size_t tab_bytes = n_gather ? h->pg_gather_off + size_t(n_gather) * sizeof(GatherPage) : size_t(n) * sizeof(PageGeom);
+  CK(cudaMemcpyAsync(h->d_pg_tab[slot], tab, tab_bytes, cudaMemcpyHostToDevice, h->copy_in));
+  if (n_dev == 0) {
+    CK(cudaMemcpyAsync(h->d_pg_in[slot], input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
+  } else {
+    for (int i = 0; i < n;) {
+      if (dev[i].data) { ++i; continue; }
+      int j = i;
+      while (j + 1 < n && !dev[j + 1].data) ++j;
+      const size_t lo = size_t(pg[size_t(i)].page_off);
+      const size_t hi = size_t(pg[size_t(j)].page_off) + size_t(pg[size_t(j)].ih) * size_t(pg[size_t(j)].iw) * 3;
+      CK(cudaMemcpyAsync(h->d_pg_in[slot] + lo, input_host + lo, hi - lo, cudaMemcpyHostToDevice, h->copy_in));
+      i = j + 1;
+    }
+  }
   CK(cudaEventRecord(h->ev_in_done[slot], h->copy_in));
   CK(cudaEventRecord(h->ev0, h->stream));
   CK(cudaStreamWaitEvent(h->stream, h->ev_in_done[slot], 0));
+  if (n_gather) {
+    for (int i = 0; i < n; ++i)
+      if (dev[i].data && dev[i].event) CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(dev[i].event), 0));
+    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(reinterpret_cast<const char*>(h->d_pg_tab[slot]) +
+                                                               h->pg_gather_off),
+                           n_gather, gather_rows, h->d_pg_in[slot], h->stream));
+  }
   CK(letterbox_batch_launch(h->d_pg_in[slot], h->d_pg_tab[slot], n, h->d_pages, net_h, net_w, h->stream));
   if (int rc = enqueue_forward(h, n, net_h, net_w, *sp)) return rc;
   uint8_t* d_res = h->d_pg_res[slot];
@@ -832,13 +916,16 @@ extern "C" int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_p
     job.pages = std::move(pg);
     job.keep_undetected = keep_undetected ? 1 : 0;
     job.textheight = textheight;
+    job.results_on_device = results_on_device ? 1 : 0;
+    if (results_on_device) h->dev_pages[slot] = job.pages;
     h->pipe_state[slot] = 1;
     h->pipe_queue.push_back(std::move(job));
   }
   h->pipe_cv.notify_one();
   h->slot_busy[slot] = true;
   h->slot_full[slot] = true;
-  h->crop_ready[slot] = textheight > 0;   // cleared again if the batch fails
+  h->crop_ready[slot] = textheight > 0;          // both cleared again if the batch fails
+  h->dev_ready[slot] = results_on_device != 0;
   return CTD_OK;
 }
 
@@ -855,9 +942,41 @@ int ctd_collect_full(ctd_handle* h, int slot) {
   h->slot_full[slot] = false;
   if (rc != CTD_OK) {
     h->crop_ready[slot] = false;
+    h->dev_ready[slot] = false;
     return rc;
   }
   CK(cudaEventSynchronize(h->ev_post_done[slot]));
+  return CTD_OK;
+}
+
+extern "C" int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page_dst) {
+  if (!h || slot < 0 || slot > 1 || !page_dst) return CTD_E_INVALID;
+  if (h->slot_busy[slot] || !h->dev_ready[slot])
+    return ctd_fail(h, CTD_E_INVALID, "slot %d holds no collected batch with results on the device", slot);
+  CK(cudaSetDevice(h->cfg.device));
+  const std::vector<ctd_page_entry>& pg = h->dev_pages[slot];
+  const int n = int(pg.size());
+  for (int i = 0; i < n; ++i)
+    if (!page_dst[i] || !is_device_memory(page_dst[i], h->cfg.device))
+      return ctd_fail(h, CTD_E_INVALID, "page_dst[%d] (%p) is not device memory of GPU %d", i, page_dst[i],
+                      h->cfg.device);
+  if (!h->dev_out) CK(cudaStreamCreateWithFlags(&h->dev_out, cudaStreamNonBlocking));
+  // the slot's planes: the collect has synchronised the batch's last writes (ev_post_done)
+  const uint8_t* d_res = h->d_pg_res[slot];
+  const bool crops = h->crop_ready[slot];
+  const uint8_t* d_px = crops ? h->d_crop[slot] + h->crop_px_off[slot] : nullptr;
+  for (int i = 0; i < n; ++i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    const size_t px = size_t(e.ih) * size_t(e.iw);
+    uint8_t* dst = static_cast<uint8_t*>(page_dst[i]);
+    CK(cudaMemcpyAsync(dst, d_res + e.mask_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
+    CK(cudaMemcpyAsync(dst + px, d_res + e.refined_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
+    if (crops) {
+      const size_t b0 = h->crop_base[slot][size_t(i)], b1 = h->crop_base[slot][size_t(i) + 1];
+      if (b1 > b0) CK(cudaMemcpyAsync(dst + 2 * px, d_px + b0, b1 - b0, cudaMemcpyDeviceToDevice, h->dev_out));
+    }
+  }
+  CK(cudaStreamSynchronize(h->dev_out));
   return CTD_OK;
 }
 
@@ -870,7 +989,7 @@ extern "C" int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region
   *n_regions = int32_t(h->crop_plan[slot].size());
   *page_first = h->crop_first[slot].data();
   *bytes = h->crop_bytes[slot];
-  *pixels = h->crop_bytes[slot] ? h->h_crop[slot] + h->crop_px_off[slot] : nullptr;
+  *pixels = h->crop_bytes[slot] && !h->dev_ready[slot] ? h->h_crop[slot] + h->crop_px_off[slot] : nullptr;
   return CTD_OK;
 }
 

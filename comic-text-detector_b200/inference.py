@@ -5,7 +5,8 @@ Same constructor and call signature as the reference's `inference.TextDetector`
 conf_thresh=0.4, mask_thresh=0.3, act='leaky')` and
 `detector(img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False) -> (mask, mask_refined, blk_list)`.
 `detect_batch` / `detect_stream` give the same results for many pages of any sizes, batched on the GPU, and with a
-`textheight` also the OCR crops of every text line (`get_transformed_regions`), cut in the same batches.
+`textheight` also the OCR crops of every text line (`get_transformed_regions`), cut in the same batches; their pages may
+be torch.uint8 CUDA tensors, and with `device_results=True` the masks and crops come back as CUDA tensors.
 
 Everything runs in libctd_b200.so: network, NMS, mask u8, DB binarize, connected components, contour boxes + scores,
 refine_mask on the GPU; ratio scaling, `group_output` and the window expansion in host C++ (csrc/group.cpp,
@@ -84,6 +85,7 @@ class TextDetector:
         # DB threshold is hard-coded 0.3 in the reference (inference.py:139 ignores mask_thresh)
         # max_batch: pages per GPU batch of detect_batch / detect_stream (the workspace is sized for it)
         self.max_batch = int(max_batch)
+        self.device_index = int(device_index)
         self.net = Engine(self.program, device=device_index, precision=precision, max_batch=self.max_batch, max_h=input_size[0],
                           max_w=input_size[1], conf_thresh=conf_thresh, nms_thresh=nms_thresh, db_thresh=0.3)
 
@@ -108,20 +110,31 @@ class TextDetector:
         naming the block and the line, before any GPU work if the reference would raise on a line."""
         return transformed_regions(self.net, img, blk_list, textheight)
 
-    def detect_batch(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, textheight=None):
+    def detect_batch(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, textheight=None,
+                     device_results=False):
         """`[self(img, refine_mode, keep_undetected_mask) for img in imgs]`, with the same results byte for byte, computed
-        in GPU batches of up to `max_batch` pages of any sizes (see detect_stream).  Every page is checked before any
-        GPU work: a page that is not u8 [h][w][3] raises ValueError.  With a textheight, each result is the 4-tuple
-        detect_stream yields, crops included."""
-        imgs = [check_page(img) for img in imgs]
-        return list(self.detect_stream(imgs, refine_mode, keep_undetected_mask, textheight))
+        in GPU batches of up to `max_batch` pages of any sizes (see detect_stream, which also describes CUDA-tensor
+        pages and device_results).  Every page is checked before any GPU work: a page that is not u8 [h][w][3], or a
+        CUDA tensor on another device, raises ValueError.  With a textheight, each result is the 4-tuple detect_stream
+        yields, crops included."""
+        imgs = [check_page(img, self.device_index) for img in imgs]
+        return list(self.detect_stream(imgs, refine_mode, keep_undetected_mask, textheight, device_results))
 
-    def detect_stream(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, textheight=None):
+    def detect_stream(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, textheight=None,
+                      device_results=False):
         """Generator over an iterable of pages: yields `(mask, mask_refined, blk_list)` for each page in input order,
         equal to `self(img, refine_mode, keep_undetected_mask)`.  Pages are grouped into batches of up to `max_batch`
         and two batches are kept in flight (`ctd_submit_pages`): while one batch runs on the GPU and in the engine's
         host stage, the next one is read from `imgs` and packed.  A page that is not u8 [h][w][3] raises ValueError
         before it reaches the GPU.
+
+        A page may also be a torch.uint8 CUDA tensor [h][w][3], BGR, on cuda:device_index, with any strides (a crop
+        `big[y0:y1, x0:x1]`, `chw.permute(1, 2, 0)`): it is read on the GPU where it is, without a copy through the
+        host, and one batch may mix such pages with numpy pages.  When the page is read from `imgs`, an event is
+        recorded on the current torch stream of its device, and the engine waits for it before reading the page, so
+        a page written by work still queued on that stream is read correctly.  The stream keeps a reference to the
+        tensor until its batch is collected; do not write into it before its result has been yielded.  The results
+        are the same as for `page.cpu().numpy()`.
 
         textheight (an integer >= 2; checked here, before any page is read): yields `(mask, mask_refined, blk_list,
         crops)` instead, where crops[b][i] is line i of blk_list[b] cut out as `get_transformed_regions(img, blk_list,
@@ -129,43 +142,52 @@ class TextDetector:
         raises (a crop side of 1 px, a degenerate quad; or a side of 32767 px or more) gets None instead of raising,
         so one such line does not end the stream.  The crops are planned on the engine's worker threads and cut in
         one GPU launch per batch from the pages already in device memory (`ctd_submit_pages_regions`).  Each page's
-        crops are views into one array of that page's own."""
+        crops are views into one array of that page's own.
+
+        device_results=True: mask, mask_refined and every crop are torch.uint8 CUDA tensors on cuda:device_index
+        ([ih][iw], [ih][iw], [h][w][3]; None where the numpy stream gives None), byte for byte what the numpy stream
+        gives, never copied to the host; blk_list stays the host TextBlock list.  A page's tensors are views into one
+        allocation of that page's own, complete when yielded, and marked as used on the current stream; like any
+        tensor made on another stream, call `record_stream` before using one on a different stream."""
         th = 0
         if textheight is not None:
             th = _check_textheight(textheight)
             if th < 2:
                 raise ValueError("textheight must be at least 2 px, got %r" % (textheight,))
-        return self._stream(imgs, refine_mode, keep_undetected_mask, th)
+        return self._stream(imgs, refine_mode, keep_undetected_mask, th, bool(device_results))
 
-    def _stream(self, imgs, refine_mode, keep_undetected_mask, th):
+    def _stream(self, imgs, refine_mode, keep_undetected_mask, th, device_results):
         net_h, net_w = self.input_size
         inflight = deque()   # slots in submission order
         free = [0, 1]
+
+        def submit(batch, events):
+            if not free:
+                yield from self._collect(inflight, free)
+            slot = free.pop(0)
+            self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask, th, events,
+                                  device_results)
+            inflight.append(slot)
+
         try:
-            batch = []
+            batch, events = [], []
             for img in imgs:
-                batch.append(check_page(img))
+                page = check_page(img, self.device_index)
+                batch.append(page)
+                events.append(_page_ready_event(page))
                 if len(batch) < self.max_batch:
                     continue
-                if not free:
-                    yield from self._collect(inflight, free)
-                slot = free.pop(0)
-                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask, th)
-                inflight.append(slot)
-                batch = []
+                yield from submit(batch, events)
+                batch, events = [], []
             if batch:
-                if not free:
-                    yield from self._collect(inflight, free)
-                slot = free.pop(0)
-                self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask, th)
-                inflight.append(slot)
+                yield from submit(batch, events)
             while inflight:
                 yield from self._collect(inflight, free)
         finally:
             while inflight:   # an error or an abandoned generator: leave the engine with no batch in flight
                 slot = inflight.popleft()
                 try:
-                    self.net.collect_pages(slot)
+                    self.net.collect_pages(slot, discard=True)
                 except Exception:
                     pass
 
@@ -177,9 +199,33 @@ class TextDetector:
             yield (mask, mask_refined, blocks_from_records(rec, lines, dist)) + tuple(crops)
 
 
-def check_page(img):
-    """A page as TextDetector's batch calls take it: u8 BGR [h][w][3] with h, w >= 1, else ValueError."""
+def check_page(img, device_index=None):
+    """A page as TextDetector's batch calls take it: u8 BGR [h][w][3] with h, w >= 1, else ValueError.  A CUDA tensor
+    (torch.uint8 [h][w][3], any strides) is returned as it is; with a device_index it must be on that GPU.  Anything
+    else, CPU tensors included, goes through np.asarray and comes back as a C-contiguous array."""
+    if getattr(img, "is_cuda", False):
+        if img.dtype != _torch().uint8 or img.dim() != 3 or img.shape[2] != 3 or img.shape[0] < 1 or img.shape[1] < 1:
+            raise ValueError("a page must be a uint8 tensor of shape [h][w][3], got %s %s"
+                             % (img.dtype, tuple(img.shape)))
+        if device_index is not None and img.device.index != device_index:
+            raise ValueError("a CUDA page must be on the detector's device cuda:%d, got %s" % (device_index, img.device))
+        return img
     a = np.asarray(img)
     if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] < 1 or a.shape[1] < 1:
         raise ValueError("a page must be a uint8 array of shape [h][w][3], got %s %s" % (a.dtype, a.shape))
     return np.ascontiguousarray(a)
+
+
+def _page_ready_event(page):
+    """for a CUDA page: an event recorded on its device's current torch stream (the engine waits for it); else None"""
+    if not getattr(page, "is_cuda", False):
+        return None
+    torch = _torch()
+    ev = torch.cuda.Event()
+    ev.record(torch.cuda.current_stream(page.device))
+    return ev
+
+
+def _torch():
+    import torch
+    return torch

@@ -432,7 +432,8 @@ CTD_API int ctd_region_plan(const ctd_region_line* lines, int32_t n, int32_t im_
  * CTD_E_SHAPE for a bad page size, CTD_E_INVALID for a malformed plan entry.                                       */
 CTD_API int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t page_on_device,
                                   const ctd_region* plan, int32_t n, uint8_t* pixels_out, size_t pixels_bytes);
-/* ctd_submit_pages plus the OCR crops of every text line of every page of the batch (ctd_region_plan above):
+/* ctd_submit_pages plus the OCR crops of every text line of every page of the batch (ctd_region_plan above;
+ * pages in device memory and results left there: ctd_submit_pages_device below):
  * the same batch, and with textheight = 0 exactly ctd_submit_pages (ctd_submit_pages is this call with textheight 0).
  * textheight >= 2 (else CTD_E_INVALID): the handle's worker plans each page's lines with ctd_region_plan right after
  * its group_output, on the same host threads, then one k_warp_regions launch on the post stream cuts every status-0
@@ -451,6 +452,43 @@ CTD_API int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_page
  * is in flight or whose last collected batch did not ask for crops.                                            */
 CTD_API int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region** plan, int32_t* n_regions,
                                 const int32_t** page_first, const uint8_t** pixels, size_t* bytes);
+
+/* ---- pages and results in device memory ------------------------------------------------------------------------
+ * A page that is already on the GPU (decoded there, or made by an earlier GPU stage) goes into a batch without a trip
+ * through host memory, and the masks and crops of a batch can stay on the GPU for the next model (OCR, inpainting).
+ *
+ * ctd_device_page describes page i of a batch: `data` is the DEVICE address of pixel (0, 0), channel 0 (B) of the u8
+ * BGR page, or NULL when the page is in `input_host` at its page_off.  Byte (y, x, c) is at
+ * data + y * stride_h + x * stride_w + c * stride_c (each stride >= 0: a sub-window of a larger image, a permuted
+ * channels-first image).  `event` (a cudaEvent_t, may be NULL) is waited on by the engine stream before the page is
+ * read, so a page still being written by a kernel on the caller's stream is read after that kernel.               */
+typedef struct ctd_device_page {
+  const uint8_t* data;
+  int64_t stride_h, stride_w, stride_c;
+  void* event;
+} ctd_device_page;
+/* ctd_submit_pages_regions with pages in device memory and, optionally, results left there.
+ *   dev: n entries (NULL: every page is in input_host).  input_host may be NULL when every page is on the device;
+ *        then no page byte is copied from the host, and a mixed batch copies only its host pages' byte ranges.  Each
+ *        device page must be device memory of the handle's GPU (checked with cudaPointerGetAttributes, else
+ *        CTD_E_INVALID naming the page) and must stay unwritten until the slot is collected.  One gather launch on
+ *        the engine stream copies every device page into the slot's packed page buffer after the waits on the pages'
+ *        events and after the host pages' copy; letterbox, refine_mask and the crops read that buffer as before.
+ *   results_on_device != 0: mask_refined, the mask refine_undetected_mask modified (keep_undetected) and the crop
+ *        pixels are NOT copied to the host; results_host still gets the phase-A rows, the masks group_output reads
+ *        and the block sections, and ctd_collect_regions gives the plan with *pixels = NULL and *bytes = the batch's
+ *        crop bytes on the device.  Fetch the device results with ctd_collect_device after ctd_collect.
+ * ctd_submit_pages_regions is this call with dev = NULL and results_on_device = 0.                                   */
+CTD_API int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                                    int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
+                                    int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
+                                    int32_t results_on_device, void* results_host);
+/* After ctd_collect(h, slot) of a results_on_device batch: copies into page_dst[i] (a DEVICE buffer on the handle's
+ * GPU, one per page of the batch) page i's [mask ih*iw | mask_refined ih*iw | the page's crops, packed as the plan
+ * lays them out, offsets relative to the page's first plan entry].  The mask is the one refine_undetected_mask
+ * modified when the batch asked for it.  Blocks until the copies are done, so the buffers may then be used on any
+ * stream.  CTD_E_INVALID for a slot in flight or whose last batch was not submitted with results_on_device.       */
+CTD_API int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page_dst);
 
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
  * [rows][5+nc]); output as ctd_get_detections for one page.                                */
