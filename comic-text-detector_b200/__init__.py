@@ -3,5 +3,5 @@
 (the directory name carries a hyphen; ctd_b200.py at the repository root aliases it)."""
 from . import compiler  # noqa: F401
 from .binding import Engine, CtdError, load_library, LIB_PATH  # noqa: F401
-from . import binding, multigpu, textblock  # noqa: F401
+from . import binding, multigpu, onnx_model, textblock  # noqa: F401
 from .inference import TextDetector, REFINEMASK_INPAINT, REFINEMASK_ANNOTATION  # noqa: F401

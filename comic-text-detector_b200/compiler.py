@@ -159,7 +159,10 @@ class Program:
 
 def fold_bn(w, conv_bias, sd, bn_prefix, eps, transposed=False):
     """(w, b) of conv followed by eval-mode BatchNorm -> single affine conv
-    (same algebra as utils/yolov5_utils.py:23-43, carried out in float64)."""
+    (same algebra as utils/yolov5_utils.py:23-43, carried out in float64).  A conv with a bias and no BatchNorm
+    entries is one whose BatchNorm was already folded (the ONNX exporter does that, onnx_model.py): returned as is."""
+    if conv_bias is not None and bn_prefix + ".weight" not in sd:
+        return w, conv_bias
     g, beta = _np(sd[bn_prefix + ".weight"]), _np(sd[bn_prefix + ".bias"])
     mu, var = _np(sd[bn_prefix + ".running_mean"]), _np(sd[bn_prefix + ".running_var"])
     scale = g / np.sqrt(var + eps)
@@ -179,11 +182,14 @@ def compile_checkpoint(ckpt, head_act="leaky"):
     layers = parse_cfg(cfg)
     hact = {"leaky": ACT_LEAKY, "relu": ACT_RELU}.get(head_act, ACT_SILU if head_act is True else ACT_NONE)
 
+    def bias(sd, key):   # only convs whose BatchNorm is already folded have one
+        return _np(sd[key]) if key in sd else None
+
     def yconv(prefix):
-        return fold_bn(_np(ysd[prefix + ".conv.weight"]), None, ysd, prefix + ".bn", 1e-3)
+        return fold_bn(_np(ysd[prefix + ".conv.weight"]), bias(ysd, prefix + ".conv.bias"), ysd, prefix + ".bn", 1e-3)
 
     def hconv(sd, prefix):
-        return fold_bn(_np(sd[prefix + ".conv.weight"]), None, sd, prefix + ".bn", 1e-5)
+        return fold_bn(_np(sd[prefix + ".conv.weight"]), bias(sd, prefix + ".conv.bias"), sd, prefix + ".bn", 1e-5)
 
     def c3(srcs, get, prefix, n, shortcut, act):
         """C3.forward (common.py:137-138): cv3(cat(m(cv1(x)), cv2(x))); cv1||cv2 share x -> one GEMM."""

@@ -4,6 +4,7 @@ Same constructor and call signature as the reference's `inference.TextDetector`
 (inference.py:116-178): `TextDetector(model_path, input_size=1024, device=..., half=False, nms_thresh=0.35,
 conf_thresh=0.4, mask_thresh=0.3, act='leaky')` and
 `detector(img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False) -> (mask, mask_refined, blk_list)`.
+A `.onnx` model_path is read as the reference's OpenCV-DNN backend reads it (onnx_model.py): same engine, same calls.
 `detect_batch` / `detect_stream` give the same results for many pages of any sizes, batched on the GPU, and with a
 `textheight` also the OCR crops of every text line (`get_transformed_regions`), cut in the same batches; their pages may
 be torch.uint8 CUDA tensors, and with `device_results=True` the masks and crops come back as CUDA tensors.
@@ -19,7 +20,7 @@ from typing import List
 
 import numpy as np
 
-from . import compiler
+from . import compiler, onnx_model
 from .binding import Engine, PREC_FP16_TC, PREC_FP32_SIMT
 from .textblock import (TextBlock, _check_textheight, blocks_from_records, group_output, overlap_area,  # noqa: F401
                         transformed_regions)
@@ -66,13 +67,20 @@ class TextDetector:
 
     def __init__(self, model_path, input_size=1024, device='cuda', half=False, nms_thresh=0.35, conf_thresh=0.4,
                  mask_thresh=0.3, act='leaky', precision=None, device_index=0, max_batch=1):
-        if isinstance(model_path, (str, Path)):
+        if isinstance(input_size, int):
+            input_size = (input_size, input_size)
+        if isinstance(model_path, (str, Path)) and Path(model_path).suffix == '.onnx':
+            # the reference's OpenCV-DNN backend (inference.py:124-130): the activation comes from the graph, `act` is
+            # ignored as there, and the network sees RGB (onnx_model.py reverses the stem's input channels)
+            ckpt, act, net_size = onnx_model.load_checkpoint(str(model_path))
+            if tuple(input_size) != (net_size, net_size):
+                raise ValueError("%s was exported for %d x %d input, input_size is %s"
+                                 % (model_path, net_size, net_size, tuple(input_size)))
+        elif isinstance(model_path, (str, Path)):
             import torch
             ckpt = torch.load(str(model_path), map_location='cpu')  # reference basemodel.py:212
         else:
             ckpt = model_path  # already a checkpoint dict
-        if isinstance(input_size, int):
-            input_size = (input_size, input_size)
         self.input_size = input_size
         self.device = device
         self.half = half
