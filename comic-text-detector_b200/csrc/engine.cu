@@ -57,19 +57,14 @@ extern "C" void ctd_destroy(ctd_handle* h) {
   cudaFree(h->d_wsplit);
   cudaFree(h->d_blob); cudaFree(h->d_pages); cudaFree(h->d_blks); cudaFree(h->d_mask); cudaFree(h->d_mask_u8);
   cudaFree(h->d_lines); cudaFree(h->d_bitmap); cudaFree(h->d_labels);
-  cudaFree(h->d_ccl_scratch); cudaFree(h->d_nms_ws); cudaFree(h->d_segrep_scratch); cudaFree(h->d_refine_scratch); cudaFree(h->d_cc_scratch); cudaFree(h->d_io_scratch);
+  cudaFree(h->d_ccl_scratch); cudaFree(h->d_nms_ws); cudaFree(h->d_segrep_scratch);
+  h->refine_scratch.release(); h->cc_scratch.release(); h->io_scratch.release();
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->tev0) cudaEventDestroy(h->tev0);
   if (h->tev1) cudaEventDestroy(h->tev1);
   for (auto e : h->op_events) cudaEventDestroy(e);
-  for (int i = 0; i < 2; ++i) {
-    cudaFree(h->d_stage_in[i]); cudaFree(h->d_stage_out[i]);
-    if (h->ev_in_done[i]) cudaEventDestroy(h->ev_in_done[i]);
-    if (h->ev_in_free[i]) cudaEventDestroy(h->ev_in_free[i]);
-    if (h->ev_out_ready[i]) cudaEventDestroy(h->ev_out_ready[i]);
-    if (h->ev_out_done[i]) cudaEventDestroy(h->ev_out_done[i]);
-  }
+  for (Slot& s : h->slot) s.release();
   if (h->ev_fork) cudaEventDestroy(h->ev_fork);
   if (h->ev_join) cudaEventDestroy(h->ev_join);
   if (h->ev_fork2) cudaEventDestroy(h->ev_fork2);
@@ -583,19 +578,75 @@ extern "C" int ctd_forward(ctd_handle* h, const uint8_t* pages, int32_t n, int32
 //               compute: [wait H2D] stage_in -> d_pages (D2D), forward, arena -> stage_out[slot] (D2D)
 //               copy_out: [wait arena copy] D2H stage_out[slot] -> results_host
 // so the H2D of batch i+1 and the D2H of batch i-1 run under the forward of batch i.
+template <bool kPinned>
+int GrowBuf<kPinned>::grow(ctd_handle* h, size_t bytes, std::optional<cudaStream_t> sync, size_t headroom) {
+  if (bytes <= cap) return CTD_OK;
+  if (sync) CK(cudaStreamSynchronize(*sync));
+  release();
+  const size_t alloc = bytes + bytes / headroom;
+  if (kPinned) CK(cudaHostAlloc(reinterpret_cast<void**>(&p), alloc, cudaHostAllocDefault));
+  else CK(cudaMalloc(reinterpret_cast<void**>(&p), alloc));
+  cap = alloc;
+  return CTD_OK;
+}
+template <bool kPinned>
+void GrowBuf<kPinned>::release() {
+  if (kPinned && p) cudaFreeHost(p);
+  if (!kPinned) cudaFree(p);
+  p = nullptr;
+  cap = 0;
+}
+template struct GrowBuf<false>;
+template struct GrowBuf<true>;
+
+void Slot::release() {
+  cudaFree(d_stage_in);
+  cudaFree(d_stage_out);
+  for (cudaEvent_t e : {ev_in_done, ev_in_free, ev_out_ready, ev_out_done, ev_post_done})
+    if (e) cudaEventDestroy(e);
+  if (pinned) cudaFreeHost(pinned);
+  pg_in.release(); pg_res.release(); pg_aux.release(); d_crop.release(); h_crop.release();
+  cudaFree(d_pg_tab);
+  if (h_pg_tab) cudaFreeHost(h_pg_tab);
+  *this = Slot();
+}
+
 int ensure_pipeline(ctd_handle* h) {
   if (h->copy_in) return CTD_OK;
   CK(cudaStreamCreateWithFlags(&h->copy_in, cudaStreamNonBlocking));
   CK(cudaStreamCreateWithFlags(&h->copy_out, cudaStreamNonBlocking));
   const size_t in_bytes = size_t(h->cfg.max_batch) * h->cfg.max_h * h->cfg.max_w * 3;
-  for (int i = 0; i < 2; ++i) {
-    CK(cudaMalloc(&h->d_stage_in[i], in_bytes));
-    CK(cudaMalloc(&h->d_stage_out[i], h->results_bytes));
-    CK(cudaEventCreateWithFlags(&h->ev_in_done[i], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&h->ev_in_free[i], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&h->ev_out_ready[i], cudaEventDisableTiming));
-    CK(cudaEventCreateWithFlags(&h->ev_out_done[i], cudaEventDisableTiming));
+  for (Slot& s : h->slot) {
+    CK(cudaMalloc(&s.d_stage_in, in_bytes));
+    CK(cudaMalloc(&s.d_stage_out, h->results_bytes));
+    for (cudaEvent_t* e : {&s.ev_in_done, &s.ev_in_free, &s.ev_out_ready, &s.ev_out_done})
+      CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
   }
+  return CTD_OK;
+}
+
+int stage_phase_a(ctd_handle* h, Slot& s, const uint8_t* pages, bool pages_on_device, int n, int ph, int pw,
+                  ShapePlan& sp, void* results_host) {
+  const size_t bytes = size_t(n) * ph * pw * 3;
+  if (!pages_on_device) {
+    CK(cudaStreamWaitEvent(h->copy_in, s.ev_in_free, 0));   // no-op before the slot's first use
+    CK(cudaMemcpyAsync(s.d_stage_in, pages, bytes, cudaMemcpyHostToDevice, h->copy_in));
+    CK(cudaEventRecord(s.ev_in_done, h->copy_in));
+    CK(cudaEventRecord(h->ev0, h->stream));
+    CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
+    CK(cudaMemcpyAsync(h->d_pages, s.d_stage_in, bytes, cudaMemcpyDeviceToDevice, h->stream));
+    CK(cudaEventRecord(s.ev_in_free, h->stream));
+  } else {
+    CK(cudaEventRecord(h->ev0, h->stream));
+    CK(cudaMemcpyAsync(h->d_pages, pages, bytes, cudaMemcpyDeviceToDevice, h->stream));
+  }
+  if (int rc = enqueue_forward(h, n, ph, pw, sp)) return rc;
+  CK(cudaStreamWaitEvent(h->stream, s.ev_out_done, 0));  // previous D2H of this slot has drained
+  CK(cudaMemcpyAsync(s.d_stage_out, h->d_mask_u8, h->layout.a_bytes, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaEventRecord(s.ev_out_ready, h->stream));
+  CK(cudaStreamWaitEvent(h->copy_out, s.ev_out_ready, 0));
+  CK(cudaMemcpyAsync(results_host, s.d_stage_out, h->layout.a_bytes, cudaMemcpyDeviceToHost, h->copy_out));
+  CK(cudaEventRecord(s.ev_out_done, h->copy_out));
   return CTD_OK;
 }
 
@@ -603,53 +654,30 @@ extern "C" int ctd_submit(ctd_handle* h, int32_t slot, const uint8_t* pages_host
                           void* results_host) {
   if (!h || !pages_host || !results_host || slot < 0 || slot > 1) return CTD_E_INVALID;
   if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit needs the full pipeline");
-  if (h->slot_busy[slot]) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  Slot& s = h->slot[slot];
+  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
   ShapePlan* sp = nullptr;
   if (int rc = prepare_forward(h, n, ph, pw, &sp)) return rc;
   if (int rc = ensure_pipeline(h)) return rc;
-  h->crop_ready[slot] = false;
-  h->dev_ready[slot] = false;
-  const size_t bytes = size_t(n) * ph * pw * 3;
-  CK(cudaStreamWaitEvent(h->copy_in, h->ev_in_free[slot], 0));   // no-op before the slot's first use
-  CK(cudaMemcpyAsync(h->d_stage_in[slot], pages_host, bytes, cudaMemcpyHostToDevice, h->copy_in));
-  CK(cudaEventRecord(h->ev_in_done[slot], h->copy_in));
-  CK(cudaEventRecord(h->ev0, h->stream));
-  CK(cudaStreamWaitEvent(h->stream, h->ev_in_done[slot], 0));
-  CK(cudaMemcpyAsync(h->d_pages, h->d_stage_in[slot], bytes, cudaMemcpyDeviceToDevice, h->stream));
-  CK(cudaEventRecord(h->ev_in_free[slot], h->stream));
-  if (int rc = enqueue_forward(h, n, ph, pw, *sp)) return rc;
-  CK(cudaStreamWaitEvent(h->stream, h->ev_out_done[slot], 0));  // previous D2H of this slot has drained
-  CK(cudaMemcpyAsync(h->d_stage_out[slot], h->d_mask_u8, h->layout.a_bytes, cudaMemcpyDeviceToDevice, h->stream));
-  CK(cudaEventRecord(h->ev_out_ready[slot], h->stream));
-  CK(cudaStreamWaitEvent(h->copy_out, h->ev_out_ready[slot], 0));
-  CK(cudaMemcpyAsync(results_host, h->d_stage_out[slot], h->layout.a_bytes, cudaMemcpyDeviceToHost, h->copy_out));
-  CK(cudaEventRecord(h->ev_out_done[slot], h->copy_out));
-  h->slot_busy[slot] = true;
+  s.start(false, false);
+  if (int rc = stage_phase_a(h, s, pages_host, false, n, ph, pw, *sp, results_host)) return rc;
+  s.busy = true;
   return CTD_OK;
 }
 
 extern "C" int ctd_collect(ctd_handle* h, int32_t slot) {
   if (!h || slot < 0 || slot > 1) return CTD_E_INVALID;
-  if (!h->slot_busy[slot]) return ctd_fail(h, CTD_E_INVALID, "slot %d has nothing in flight", slot);
+  Slot& s = h->slot[slot];
+  if (!s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has nothing in flight", slot);
   CK(cudaSetDevice(h->cfg.device));
-  if (h->slot_full[slot]) {
+  if (s.full) {
     const int rc = ctd_collect_full(h, slot);
-    h->slot_busy[slot] = false;
+    s.busy = false;
     return rc;
   }
-  CK(cudaEventSynchronize(h->ev_out_done[slot]));
-  h->slot_busy[slot] = false;
-  return CTD_OK;
-}
-
-int ensure_io_scratch(ctd_handle* h, size_t bytes) {
-  if (bytes <= h->io_scratch_cap) return CTD_OK;
-  CK(cudaStreamSynchronize(h->stream));
-  cudaFree(h->d_io_scratch);
-  h->d_io_scratch = nullptr;
-  h->io_scratch_cap = 0;
-  CK(cudaMalloc(&h->d_io_scratch, bytes + bytes / 4));
-  h->io_scratch_cap = bytes + bytes / 4;
+  CK(cudaEventSynchronize(s.ev_out_done));
+  s.busy = false;
+  s.collected = true;
   return CTD_OK;
 }
 
@@ -661,10 +689,10 @@ extern "C" int ctd_forward_resized(ctd_handle* h, const uint8_t* page, int32_t i
   ShapePlan* sp = nullptr;
   if (int rc = prepare_forward(h, 1, net_h, net_w, &sp)) return rc;
   const size_t bytes = size_t(ih) * iw * 3;
-  if (int rc = ensure_io_scratch(h, bytes)) return rc;
+  if (int rc = h->io_scratch.grow(h, bytes, h->stream)) return rc;
   CK(cudaEventRecord(h->ev0, h->stream));
-  CK(cudaMemcpyAsync(h->d_io_scratch, page, bytes, cudaMemcpyHostToDevice, h->stream));
-  CK(resize_linear_u8_launch(h->d_io_scratch, ih, iw, size_t(iw) * 3, 3, h->d_pages, unpad_h, unpad_w, net_h, net_w, h->stream));
+  CK(cudaMemcpyAsync(h->io_scratch.p, page, bytes, cudaMemcpyHostToDevice, h->stream));
+  CK(resize_linear_u8_launch(h->io_scratch.p, ih, iw, size_t(iw) * 3, 3, h->d_pages, unpad_h, unpad_w, net_h, net_w, h->stream));
   return enqueue_forward(h, 1, net_h, net_w, *sp);
 }
 
@@ -676,9 +704,9 @@ extern "C" int ctd_get_mask_u8_resized(ctd_handle* h, int32_t crop_h, int32_t cr
     return ctd_fail(h, CTD_E_SHAPE, "bad crop %dx%d of the %dx%d mask", crop_h, crop_w, h->ph, h->pw);
   CK(cudaSetDevice(h->cfg.device));
   const size_t bytes = size_t(out_h) * out_w;
-  if (int rc = ensure_io_scratch(h, bytes)) return rc;
-  CK(resize_linear_u8_launch(h->d_mask_u8, crop_h, crop_w, size_t(h->pw), 1, h->d_io_scratch, out_h, out_w, out_h, out_w, h->stream));
-  CK(cudaMemcpyAsync(mask_out, h->d_io_scratch, bytes, cudaMemcpyDeviceToHost, h->stream));
+  if (int rc = h->io_scratch.grow(h, bytes, h->stream)) return rc;
+  CK(resize_linear_u8_launch(h->d_mask_u8, crop_h, crop_w, size_t(h->pw), 1, h->io_scratch.p, out_h, out_w, out_h, out_w, h->stream));
+  CK(cudaMemcpyAsync(mask_out, h->io_scratch.p, bytes, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return CTD_OK;
 }
@@ -690,10 +718,10 @@ extern "C" int ctd_resize_linear_u8(ctd_handle* h, const uint8_t* src, int32_t s
   CK(cudaSetDevice(h->cfg.device));
   const size_t sb = size_t(sh) * sw * channels, db = size_t(dh) * dw * channels;
   const size_t so = (sb + 255) / 256 * 256;
-  if (int rc = ensure_io_scratch(h, so + db)) return rc;
-  CK(cudaMemcpyAsync(h->d_io_scratch, src, sb, cudaMemcpyHostToDevice, h->stream));
-  CK(resize_linear_u8_launch(h->d_io_scratch, sh, sw, size_t(sw) * channels, channels, h->d_io_scratch + so, dh, dw, dh, dw, h->stream));
-  CK(cudaMemcpyAsync(dst, h->d_io_scratch + so, db, cudaMemcpyDeviceToHost, h->stream));
+  if (int rc = h->io_scratch.grow(h, so + db, h->stream)) return rc;
+  CK(cudaMemcpyAsync(h->io_scratch.p, src, sb, cudaMemcpyHostToDevice, h->stream));
+  CK(resize_linear_u8_launch(h->io_scratch.p, sh, sw, size_t(sw) * channels, channels, h->io_scratch.p + so, dh, dw, dh, dw, h->stream));
+  CK(cudaMemcpyAsync(dst, h->io_scratch.p + so, db, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return CTD_OK;
 }
@@ -952,16 +980,9 @@ int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t o_scr = al(px * 4);
   const size_t scr_bytes = al(std::max(px * 12, size_t(stats_cap > 0 ? stats_cap : 0) * 5 * 4));
-  const size_t o_nl = o_scr + scr_bytes, need = o_nl + 256;
-  if (need > h->cc_scratch_cap) {
-    CK(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_cc_scratch);
-    h->d_cc_scratch = nullptr;
-    h->cc_scratch_cap = 0;
-    CK(cudaMalloc(&h->d_cc_scratch, need + need / 4));
-    h->cc_scratch_cap = need + need / 4;
-  }
-  uint8_t* base = static_cast<uint8_t*>(h->d_cc_scratch);
+  const size_t o_nl = o_scr + scr_bytes;
+  if (int rc = h->cc_scratch.grow(h, o_nl + 256, h->stream)) return rc;
+  uint8_t* base = h->cc_scratch.p;
   int32_t* d_labels = reinterpret_cast<int32_t*>(base);
   int32_t* d_scr = reinterpret_cast<int32_t*>(base + o_scr);
   int32_t* d_nl = reinterpret_cast<int32_t*>(base + o_nl);
@@ -979,11 +1000,11 @@ extern "C" int ctd_connected_components(ctd_handle* h, const uint8_t* img, int32
   if (ih < 1 || iw < 1 || size_t(ih) * iw > (size_t(1) << 28)) return ctd_fail(h, CTD_E_SHAPE, "bad image size %dx%d", ih, iw);
   CK(cudaSetDevice(h->cfg.device));
   const size_t px = size_t(ih) * iw;
-  if (int rc = ensure_io_scratch(h, px + 256)) return rc;
-  CK(cudaMemcpyAsync(h->d_io_scratch, img, px, cudaMemcpyHostToDevice, h->stream));
+  if (int rc = h->io_scratch.grow(h, px + 256, h->stream)) return rc;
+  CK(cudaMemcpyAsync(h->io_scratch.p, img, px, cudaMemcpyHostToDevice, h->stream));
   int32_t* d_stats = nullptr;
-  if (int rc = cc_device(h, h->d_io_scratch, ih, iw, (stats && stats_cap > 0) ? stats_cap : 0, &d_stats, n_labels)) return rc;
-  CK(cudaMemcpyAsync(labels, h->d_cc_scratch, px * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (int rc = cc_device(h, h->io_scratch.p, ih, iw, (stats && stats_cap > 0) ? stats_cap : 0, &d_stats, n_labels)) return rc;
+  CK(cudaMemcpyAsync(labels, h->cc_scratch.p, px * 4, cudaMemcpyDeviceToHost, h->stream));
   if (stats && stats_cap > 0) CK(cudaMemcpyAsync(stats, d_stats, size_t(stats_cap) * 5 * 4, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return CTD_OK;

@@ -13,6 +13,7 @@
 #include <deque>
 #include <map>
 #include <mutex>
+#include <optional>
 #include <string>
 #include <thread>
 #include <tuple>
@@ -66,21 +67,100 @@ inline bool letterbox_of(int ih, int iw, int net_h, int net_w, Letterbox& lb) {
 }
 
 // results of a ctd_submit_pages batch of n pages: the phase-A rows (sized for n pages) at the start of the results
-// buffer, then the packed page masks, the mask_refined planes and the block sections at the ctd_page_entry offsets
+// buffer, then the packed page masks, the mask_refined planes and the block sections at the ctd_page_entry offsets.
+// The result arena of ctd_submit_full has its rows at ArenaLayout's offsets and its masks at 0.
 struct PagesHead {
   size_t det, cnt, lb, ls, lc, masks;
 };
 PagesHead pages_head(int n);
 
+// one page of a batch as phases B and C see it
+struct JobPage {
+  int ih, iw;
+  float ratio_x, ratio_y;   // resize_ratio (inference.py:148)
+  size_t off;               // pixel offset P_i of the page in the image (x3), mask and mask_refined planes
+  char* section;            // its block section in results_host
+};
+
+// phases B and C of a submitted batch: what the worker thread needs of it
 struct PipeJob {
-  int slot = 0, n = 0, ph = 0, pw = 0, refine_mode = 0;
-  void* results_host = nullptr;
-  const uint8_t* pages_dev = nullptr;   // caller's device pages (pages_on_device) or null: the slot's staging copy
-  // ctd_submit_pages: the batch's pages (ph x pw is the net shape), and whether to run refine_undetected_mask
-  std::vector<ctd_page_entry> pages;
+  int slot = 0, refine_mode = 0;
+  char* results_host = nullptr;
+  PagesHead head{};                // phase-A rows and the mask plane in results_host
+  size_t refined = 0;              // mask_refined plane in results_host
+  std::vector<JobPage> pages;
+  size_t total = 0;                // pixels of each plane (every page's, each rounded up to 256)
+  // device planes: the pages, their masks, mask_refined, and (keep_undetected) 2 * total bytes of the second refine
+  // output and threshold planes
+  const uint8_t* d_img = nullptr;
+  uint8_t* d_mask = nullptr;
+  uint8_t* d_ref = nullptr;
+  uint8_t* d_aux = nullptr;
+  // ctd_submit_full: the block sections are uploaded here (blocks_bytes from the first page's section) before the
+  // refine, so ctd_device_arena holds the same bytes as results_host
+  uint8_t* d_blocks = nullptr;
+  size_t blocks_bytes = 0;
   int keep_undetected = 0;
   int textheight = 0;   // > 0: also crop every text line of every page (ctd_submit_pages_regions)
   int results_on_device = 0;   // mask_refined, the modified mask and the crops stay on the device (ctd_collect_device)
+};
+
+struct ctd_handle;
+// a buffer grown on demand and never shrunk (device memory, or pinned host memory): grow() replaces a smaller
+// allocation by one of bytes + bytes / headroom, after synchronising `sync`, the stream whose work may still use it
+// (none: no enqueued work can use it)
+template <bool kPinned>
+struct GrowBuf {
+  uint8_t* p = nullptr;
+  size_t cap = 0;
+  int grow(ctd_handle* h, size_t bytes, std::optional<cudaStream_t> sync, size_t headroom = 4);
+  void release();
+};
+using DevBuf = GrowBuf<false>;
+using PinnedBuf = GrowBuf<true>;
+
+// one of the two slots of the pipelined paths (ctd_submit, ctd_submit_full, ctd_submit_pages*): the staging and events
+// of a batch in flight, its hand-over from the worker, and the buffers its results stay in until the next submission
+struct Slot {
+  // ctd_submit / ctd_submit_full staging (ensure_pipeline): the pages, and the phase-A section of the arena
+  uint8_t* d_stage_in = nullptr;
+  uint8_t* d_stage_out = nullptr;
+  cudaEvent_t ev_in_done = nullptr, ev_in_free = nullptr, ev_out_ready = nullptr, ev_out_done = nullptr;
+  cudaEvent_t ev_post_done = nullptr;   // phase C of the batch has run (post stream)
+  bool busy = false;                    // submitted and not collected
+  bool full = false;                    // collected through the worker (ctd_submit_full, ctd_submit_pages*)
+  // what the batch asked for (start()), and whether it was collected without error: the results ctd_collect_regions
+  // and ctd_collect_device hand out
+  bool crops = false, on_device = false, collected = false;
+  // worker hand-over, under pipe_mu: 0 idle, 1 queued / running, 2 phase C enqueued, 3 failed
+  int state = 0;
+  int rc = 0;
+  std::string err;
+  char* pinned = nullptr;   // pinned staging of the refine window tables, pipe_pinned_cap bytes
+  // ctd_submit_pages: packed pages | results head, masks, mask_refined | second refine output and threshold planes of
+  // refine_undetected_mask, grown while the slot is idle; page tables (pinned + device: max_batch PageGeom entries,
+  // then at pg_gather_off max_batch GatherPage entries for the pages gathered from device memory, uploaded together)
+  DevBuf pg_in, pg_res, pg_aux;
+  ctd::PageGeom* h_pg_tab = nullptr;
+  ctd::PageGeom* d_pg_tab = nullptr;
+  std::vector<ctd_page_entry> dev_pages;   // the page entries of a results_on_device batch (ctd_collect_device)
+  // text-line crops, written by the worker: the concatenated plans, the first plan entry of each page (n + 1
+  // entries), the device buffer (crop tables | crop pixels) and the pinned host buffer (the same tables staged for
+  // upload | the pixels copied back)
+  std::vector<ctd_region> crop_plan;
+  std::vector<int32_t> crop_first;
+  std::vector<size_t> crop_base;   // n + 1 entries: page i's crops are bytes [crop_base[i], crop_base[i + 1])
+  DevBuf d_crop;
+  PinnedBuf h_crop;
+  size_t crop_px_off = 0, crop_bytes = 0;   // pixels at h_crop + crop_px_off, crop_bytes long
+
+  // a submission starts on the slot: the results of its last batch are given up
+  void start(bool want_crops, bool want_on_device) {
+    crops = want_crops;
+    on_device = want_on_device;
+    collected = false;
+  }
+  void release();   // frees the slot's buffers and events
 };
 
 // refine windows of one launch (all pages of a batch) and the chunks they are cut into
@@ -143,25 +223,18 @@ struct ctd_handle {
   int32_t* d_nlabels = nullptr;
   int32_t* d_ccl_scratch = nullptr;
   void* d_segrep_scratch = nullptr;
-  void* d_refine_scratch = nullptr;
-  size_t refine_scratch_cap = 0;
-  void* d_cc_scratch = nullptr;      // ctd_connected_components: grow-on-demand, any image size
-  size_t cc_scratch_cap = 0;
-  uint8_t* d_io_scratch = nullptr;   // page upload / resized mask staging of the resize entry points
-  size_t io_scratch_cap = 0;
+  DevBuf refine_scratch;   // refine_mask on the engine stream
+  DevBuf cc_scratch;       // ctd_connected_components: any image size
+  DevBuf io_scratch;       // page upload / resized mask staging of the resize entry points
   int16_t* d_line_boxes = nullptr;
   float* d_line_scores = nullptr;
   int32_t* d_line_count = nullptr;
   void* d_nms_ws = nullptr;
   NmsWorkspace nms{};
   std::map<std::tuple<int, int, int>, ShapePlan> plans;
-  // pipelined host path (ctd_submit / ctd_collect): two staging slots, copy streams either side of compute
+  // pipelined host path (ctd_submit / ctd_collect): two slots, copy streams either side of compute
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
-  uint8_t* d_stage_in[2] = {nullptr, nullptr};
-  uint8_t* d_stage_out[2] = {nullptr, nullptr};
-  cudaEvent_t ev_in_done[2] = {nullptr, nullptr}, ev_in_free[2] = {nullptr, nullptr};
-  cudaEvent_t ev_out_ready[2] = {nullptr, nullptr}, ev_out_done[2] = {nullptr, nullptr};
-  bool slot_busy[2] = {false, false};
+  Slot slot[2];
   // overlapped schedule (programs with a DB tail): post-processing of the DB maps / the Detect rows runs on side
   // streams under the remaining network ops (see run_ops)
   bool overlap = false;
@@ -172,51 +245,19 @@ struct ctd_handle {
   // result arena layout (ctd_results_layout) and the full pipeline (pipeline.cu): worker thread + post stream
   ArenaLayout layout{};
   cudaStream_t post = nullptr;
-  cudaEvent_t ev_post_done[2] = {nullptr, nullptr};
-  char* pipe_pinned[2] = {nullptr, nullptr};     // pinned staging of the refine window tables, one per slot
   size_t pipe_pinned_cap = 0;
-  bool slot_full[2] = {false, false};            // slot was submitted with ctd_submit_full
   std::thread pipe_thread;
   std::mutex pipe_mu;
   std::condition_variable pipe_cv, pipe_done_cv;
   std::deque<PipeJob> pipe_queue;
   bool pipe_quit = false;
-  int pipe_state[2] = {0, 0};                    // 0 idle, 1 queued / running, 2 phase C enqueued, 3 failed
-  int pipe_rc[2] = {0, 0};
-  std::string pipe_err[2];
   int host_threads = 4;
-  // any-size batches (ctd_submit_pages): per-slot device planes (packed pages | results head, masks, mask_refined |
-  // second refine output and threshold planes of refine_undetected_mask), grown while the slot is idle; per-slot page
-  // tables (pinned + device: max_batch PageGeom entries, then at pg_gather_off max_batch GatherPage entries for the
-  // pages gathered from device memory, uploaded together); the worker's own connected-components scratch
-  uint8_t* d_pg_in[2] = {nullptr, nullptr};
-  uint8_t* d_pg_res[2] = {nullptr, nullptr};
-  uint8_t* d_pg_aux[2] = {nullptr, nullptr};
-  size_t pg_in_cap[2] = {0, 0}, pg_res_cap[2] = {0, 0}, pg_aux_cap[2] = {0, 0};
-  ctd::PageGeom* h_pg_tab[2] = {nullptr, nullptr};
-  ctd::PageGeom* d_pg_tab[2] = {nullptr, nullptr};
   size_t pg_gather_off = 0;
-  // results_on_device batches (ctd_submit_pages_device): the slot's page entries, whether its collected batch left
-  // its results on the device, and the stream ctd_collect_device copies on
-  std::vector<ctd_page_entry> dev_pages[2];
-  bool dev_ready[2] = {false, false};
-  cudaStream_t dev_out = nullptr;
-  void* d_pg_cc = nullptr;
-  size_t pg_cc_cap = 0;
-  // refine scratch of the worker's phase C on the post stream (d_refine_scratch belongs to the caller's stream)
-  void* d_post_refine = nullptr;
-  size_t post_refine_cap = 0;
-  // text-line crops of a ctd_submit_pages_regions batch, per slot, written by the worker: the concatenated plans, the
-  // first plan entry of each page (n + 1 entries), the device buffer (crop tables | crop pixels) and the pinned host
-  // buffer (the same tables staged for upload | the pixels copied back), both grown on demand and never shrunk
-  std::vector<ctd_region> crop_plan[2];
-  std::vector<int32_t> crop_first[2];
-  std::vector<size_t> crop_base[2];   // n + 1 entries: page i's crops are bytes [crop_base[i], crop_base[i + 1])
-  uint8_t* d_crop[2] = {nullptr, nullptr};
-  uint8_t* h_crop[2] = {nullptr, nullptr};
-  size_t crop_dcap[2] = {0, 0}, crop_hcap[2] = {0, 0};
-  size_t crop_px_off[2] = {0, 0}, crop_bytes[2] = {0, 0};   // pixels at h_crop + crop_px_off, crop_bytes long
-  bool crop_ready[2] = {false, false};                      // the collected batch of the slot asked for crops
+  cudaStream_t dev_out = nullptr;   // the stream ctd_collect_device copies on
+  // the worker's phase C on the post stream: its own connected-components and refine scratch (refine_scratch and
+  // cc_scratch belong to the caller's stream)
+  DevBuf pg_cc;
+  DevBuf post_refine;
   // last forward
   int n = 0, ph = 0, pw = 0;
   int last_launches = 0;
@@ -228,11 +269,15 @@ int ctd_fail(ctd_handle* h, int code, const char* fmt, ...);
 int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out);
 int enqueue_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan& sp);
 int ensure_pipeline(ctd_handle* h);
-int ensure_io_scratch(ctd_handle* h, size_t bytes);
+// phase A of a batch of n net-sized pages on slot s, enqueued on the copy streams and the engine stream: the pages
+// (host pages through s.d_stage_in) into d_pages, the forward, the arena's phase-A section to s.d_stage_out and on to
+// results_host
+int stage_phase_a(ctd_handle* h, Slot& s, const uint8_t* pages, bool pages_on_device, int n, int ph, int pw,
+                  ShapePlan& sp, void* results_host);
 // connected components + stats of a DEVICE u8 image on the engine stream (grow-on-demand scratch): *d_stats points at
 // [stats_cap][5] ints on the device, *n_labels is read back (synchronises the stream)
 int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap, int32_t** d_stats, int32_t* n_labels);
 int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int refine_mode,
-                  uint8_t* d_out, cudaStream_t st, void** scratch, size_t* cap, char* pinned);
+                  uint8_t* d_out, cudaStream_t st, DevBuf& scratch, char* pinned);
 int ctd_collect_full(ctd_handle* h, int slot);
 void ctd_pipeline_shutdown(ctd_handle* h);

@@ -67,27 +67,19 @@ size_t RefineJob::table_bytes() const {
   return al(wins.size() * sizeof(RefineWin)) + al(chunks.size() * sizeof(RefineChunk));
 }
 
-// uploads the window tables of `job` into the refine scratch *scratch / *cap and launches the refine kernels:
-// d_img / d_mask / d_out are device planes holding each window's page at its page_off.  Stream-ordered on `st`, the
-// only stream that may use that scratch (it is grown here after synchronising `st`): the caller's calls use
-// h->d_refine_scratch on h->stream, the pipeline worker h->d_post_refine on h->post.  `pinned` (optional) is a host
-// staging buffer of >= job.table_bytes() bytes that stays valid until the copy has executed.
+// uploads the window tables of `job` into the refine scratch and launches the refine kernels: d_img / d_mask / d_out
+// are device planes holding each window's page at its page_off.  Stream-ordered on `st`, the only stream that may use
+// that scratch (it is grown here after synchronising `st`): the caller's calls use h->refine_scratch on h->stream, the
+// pipeline worker h->post_refine on h->post.  `pinned` (optional) is a host staging buffer of >= job.table_bytes()
+// bytes that stays valid until the copy has executed.
 int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int refine_mode,
-                  uint8_t* d_out, cudaStream_t st, void** scratch, size_t* cap, char* pinned) {
+                  uint8_t* d_out, cudaStream_t st, DevBuf& scratch, char* pinned) {
   if (job.wins.empty()) return CTD_OK;
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t tb = job.table_bytes();   // a multiple of 256
   const size_t sb = refine_mk_state_bytes(int(job.wins.size()));
-  const size_t need = tb + sb + refine_scratch_bytes(job.total_px);
-  if (need > *cap) {
-    CK(cudaStreamSynchronize(st));       // the old scratch may still be in use by an earlier launch on `st`
-    cudaFree(*scratch);
-    *scratch = nullptr;
-    *cap = 0;
-    CK(cudaMalloc(scratch, need + need / 2));
-    *cap = need + need / 2;
-  }
-  char* base = static_cast<char*>(*scratch);
+  if (int rc = scratch.grow(h, tb + sb + refine_scratch_bytes(job.total_px), st, 2)) return rc;
+  char* base = reinterpret_cast<char*>(scratch.p);
   const size_t wb = al(job.wins.size() * sizeof(RefineWin));
   std::vector<char> local;
   char* stage = pinned;
@@ -127,15 +119,14 @@ extern "C" int ctd_refine_mask(ctd_handle* h, const uint8_t* img, const uint8_t*
   RefineJob job;
   for (int i = 0; i < n_win; ++i) job.add(windows[4 * i], windows[4 * i + 1], windows[4 * i + 2], windows[4 * i + 3], 0, iw, ih);
   const size_t px = size_t(ih) * iw, pxa = (px + 255) / 256 * 256;
-  if (int rc = ensure_io_scratch(h, pxa * 5 + 1024)) return rc;
-  uint8_t* d_img = h->d_io_scratch;
+  if (int rc = h->io_scratch.grow(h, pxa * 5 + 1024, h->stream)) return rc;
+  uint8_t* d_img = h->io_scratch.p;
   uint8_t* d_mask = d_img + pxa * 3;
   uint8_t* d_out = d_mask + pxa;
   CK(cudaMemcpyAsync(d_img, img, px * 3, cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemcpyAsync(d_mask, mask, px, cudaMemcpyHostToDevice, h->stream));
   CK(cudaMemsetAsync(d_out, 0, pxa, h->stream));
-  if (int rc = launch_refine(h, job, d_img, d_mask, refine_mode, d_out, h->stream, &h->d_refine_scratch,
-                             &h->refine_scratch_cap, nullptr))
+  if (int rc = launch_refine(h, job, d_img, d_mask, refine_mode, d_out, h->stream, h->refine_scratch, nullptr))
     return rc;
   CK(cudaMemcpyAsync(out, d_out, px, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
@@ -151,6 +142,19 @@ struct PageIn {
   const uint8_t* mask; int im_w, im_h;          // page-sized mask
   float ratio_x, ratio_y;                      // resize_ratio (inference.py:148)
 };
+
+// page i of a batch whose phase-A rows are at `head` in `res` ([n][300][6] detections, [n] counts, [n][1000][8] line
+// boxes, [n][1000] scores, [n] counts), with its page-sized host mask
+PageIn page_in(const char* res, const PagesHead& head, int i, const JobPage& p, const uint8_t* mask) {
+  PageIn in;
+  in.det = reinterpret_cast<const float*>(res + head.det) + size_t(i) * 300 * 6;
+  in.n_det = std::min(std::max(reinterpret_cast<const int32_t*>(res + head.cnt)[i], 0), 300);
+  in.line_boxes = reinterpret_cast<const int16_t*>(res + head.lb) + size_t(i) * 1000 * 8;
+  in.line_scores = reinterpret_cast<const float*>(res + head.ls) + size_t(i) * 1000;
+  in.n_lines = std::min(std::max(reinterpret_cast<const int32_t*>(res + head.lc)[i], 0), 1000);
+  in.mask = mask; in.im_w = p.iw; in.im_h = p.ih; in.ratio_x = p.ratio_x; in.ratio_y = p.ratio_y;
+  return in;
+}
 
 // inference.py:101-114 (postprocess_yolo casts), 158-172 (box_thresh, line rescale), textblock.group_output,
 // expand_textwindow(.., 16): fills the page's block section and appends its refine windows
@@ -241,27 +245,25 @@ __global__ void or_kernel(uint8_t* __restrict__ dst, const uint8_t* __restrict__
   if (i < n) dst[i] |= src[i];
 }
 
-// one page of refine_undetected: its planes start at pixel `off` (x3 in the image); rec[0..nb) its blocks
-struct UndetPage {
-  size_t off;
-  int ih, iw;
-  const ctd_block* rec;
-  int nb;
+// device planes of a set of pages, each page's at its pixel offset: the image (x3), the mask, mask_refined, and the
+// second refine output and threshold planes of refine_undetected_mask; `total` pixels each
+struct Planes {
+  const uint8_t* img;
+  uint8_t *mask, *ref, *ref2, *thr;
+  size_t total;
 };
 
-// refine_undetected_mask (textmask.py:135-156) for a set of pages whose planes lie in [0, total_px) of d_mask, d_ref
-// (mask_refined), d_ref2 and d_thr (and x3 of d_img): one prep launch over all planes, connected components + stats of
-// each page on `st` (the scratch *cc / *cc_cap grows here), the host loop over each page's stats rows, then one refine
-// launch for the extra windows of all pages (refine scratch *refine_scratch / *refine_cap) and one OR launch.  The
-// masks are modified in place, as in the reference.
+// refine_undetected_mask (textmask.py:135-156) for a set of pages: one prep launch over all planes, connected
+// components + stats of each page on `st` (the scratch `cc` grows here), the host loop over each page's stats rows
+// against its blocks, then one refine launch for the extra windows of all pages and one OR launch.  The masks are
+// modified in place, as in the reference.
 // Synchronises `st` once for the label counts and once for the stats rows.
-int refine_undetected(ctd_handle* h, const std::vector<UndetPage>& pages, size_t total_px, const uint8_t* d_img,
-                      uint8_t* d_mask, uint8_t* d_ref, uint8_t* d_ref2, uint8_t* d_thr, int refine_mode, cudaStream_t st,
-                      void** cc, size_t* cc_cap, void** refine_scratch, size_t* refine_cap, char* pinned,
-                      size_t pinned_cap) {
+int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Planes& pl, int refine_mode,
+                      cudaStream_t st, DevBuf& cc, DevBuf& refine_scratch, char* pinned, size_t pinned_cap) {
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const int n = int(pages.size());
-  undetected_prep_kernel<<<unsigned((total_px + 255) / 256), 256, 0, st>>>(d_mask, d_ref, d_thr, total_px);
+  const size_t total_px = pl.total;
+  undetected_prep_kernel<<<unsigned((total_px + 255) / 256), 256, 0, st>>>(pl.mask, pl.ref, pl.thr, total_px);
   CK(cudaGetLastError());
   // scratch: labels | 3 ints/px of CCL scratch for the largest page (reused page after page) | one stats table per
   // page (worst case of 8-connected components + background) | the label counts
@@ -276,23 +278,16 @@ int refine_undetected(ctd_handle* h, const std::vector<UndetPage>& pages, size_t
     stats_off[size_t(i)] = o;
     o += al(size_t(cap[size_t(i)]) * 5 * 4);
   }
-  const size_t o_nl = o, need = o_nl + al(size_t(n) * 4);
-  if (need > *cc_cap) {
-    CK(cudaStreamSynchronize(st));
-    cudaFree(*cc);
-    *cc = nullptr;
-    *cc_cap = 0;
-    CK(cudaMalloc(cc, need + need / 4));
-    *cc_cap = need + need / 4;
-  }
-  uint8_t* base = static_cast<uint8_t*>(*cc);
+  const size_t o_nl = o;
+  if (int rc = cc.grow(h, o_nl + al(size_t(n) * 4), st)) return rc;
+  uint8_t* base = cc.p;
   int32_t* d_labels = reinterpret_cast<int32_t*>(base);
   int32_t* d_scr = reinterpret_cast<int32_t*>(base + o_scr);
   int32_t* d_nl = reinterpret_cast<int32_t*>(base + o_nl);
   for (int i = 0; i < n; ++i) {
-    const UndetPage& p = pages[size_t(i)];
+    const JobPage& p = pages[size_t(i)];
     int32_t* d_stats = reinterpret_cast<int32_t*>(base + stats_off[size_t(i)]);
-    CK(ccl_launch(d_thr + p.off, 1, p.ih, p.iw, d_labels, d_scr, d_nl + i, st));
+    CK(ccl_launch(pl.thr + p.off, 1, p.ih, p.iw, d_labels, d_scr, d_nl + i, st));
     CK(ccl_stats_launch(d_labels, p.ih, p.iw, d_stats, cap[size_t(i)], st));
   }
   std::vector<int32_t> n_lab(static_cast<size_t>(n));
@@ -306,9 +301,12 @@ int refine_undetected(ctd_handle* h, const std::vector<UndetPage>& pages, size_t
                          cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
+  const BlockSection bs = block_section_layout();
   RefineJob rj2;
   for (int i = 0; i < n; ++i) {
-    const UndetPage& p = pages[size_t(i)];
+    const JobPage& p = pages[size_t(i)];
+    const int nb = reinterpret_cast<const ctd_page_blocks*>(p.section)->n_blocks;
+    const ctd_block* rec = reinterpret_cast<const ctd_block*>(p.section + bs.rec_off);
     bool first_valid = true;
     for (int li = 0; li < n_lab[size_t(i)]; ++li) {
       const int32_t* s5 = &stats[size_t(i)][size_t(li) * 5];
@@ -316,8 +314,8 @@ int refine_undetected(ctd_handle* h, const std::vector<UndetPage>& pages, size_t
       if (first_valid) { first_valid = false; continue; }        // valid_labels[1:]
       const int64_t bb[4] = {s5[0], s5[1], int64_t(s5[0]) + s5[2], int64_t(s5[1]) + s5[3]};
       int64_t score = -1;
-      for (int b = 0; b < p.nb; ++b) {
-        const int32_t* q = p.rec[b].xyxy;
+      for (int b = 0; b < nb; ++b) {
+        const int32_t* q = rec[b].xyxy;
         const int64_t x1 = std::max<int64_t>(q[0], bb[0]), y1 = std::max<int64_t>(q[1], bb[1]);
         const int64_t x2 = std::min<int64_t>(q[2], bb[2]), y2 = std::min<int64_t>(q[3], bb[3]);
         const int64_t a = (y2 < y1 || x2 < x1) ? -1 : (y2 - y1) * (x2 - x1);
@@ -334,15 +332,30 @@ int refine_undetected(ctd_handle* h, const std::vector<UndetPage>& pages, size_t
     }
   }
   if (!rj2.wins.empty()) {
-    CK(cudaMemsetAsync(d_ref2, 0, total_px, st));
+    CK(cudaMemsetAsync(pl.ref2, 0, total_px, st));
     // the stream is idle here, so the pinned staging of an earlier launch is free again
     char* stage = rj2.table_bytes() <= pinned_cap ? pinned : nullptr;
-    if (int rc = launch_refine(h, rj2, d_img, d_mask, refine_mode, d_ref2, st, refine_scratch, refine_cap, stage))
-      return rc;
-    or_kernel<<<unsigned((total_px + 255) / 256), 256, 0, st>>>(d_ref, d_ref2, total_px);
+    if (int rc = launch_refine(h, rj2, pl.img, pl.mask, refine_mode, pl.ref2, st, refine_scratch, stage)) return rc;
+    or_kernel<<<unsigned((total_px + 255) / 256), 256, 0, st>>>(pl.ref, pl.ref2, total_px);
     CK(cudaGetLastError());
   }
   return CTD_OK;
+}
+
+// phase C of a set of pages, mask_refined already zeroed: one refine launch over the windows of every page
+// (wins[i]: x1 y1 x2 y2 each), then with keep_undetected refine_undetected_mask.  Stream-ordered on `st` with the
+// scratch that belongs to it; `pinned` (optional, pinned_cap bytes) stages the window tables.
+int phase_c(ctd_handle* h, const std::vector<JobPage>& pages, const std::vector<std::vector<int32_t>>& wins,
+            const Planes& pl, int refine_mode, bool keep_undetected, cudaStream_t st, DevBuf& refine_scratch,
+            DevBuf& cc, char* pinned, size_t pinned_cap) {
+  RefineJob rj;
+  for (size_t i = 0; i < pages.size(); ++i)
+    for (size_t k = 0; k + 3 < wins[i].size(); k += 4)
+      rj.add(wins[i][k], wins[i][k + 1], wins[i][k + 2], wins[i][k + 3], pages[i].off, pages[i].iw, pages[i].ih);
+  char* stage = rj.table_bytes() <= pinned_cap ? pinned : nullptr;   // else: pageable + sync
+  if (int rc = launch_refine(h, rj, pl.img, pl.mask, refine_mode, pl.ref, st, refine_scratch, stage)) return rc;
+  if (!keep_undetected) return CTD_OK;
+  return refine_undetected(h, pages, pl, refine_mode, st, cc, refine_scratch, pinned, pinned_cap);
 }
 }  // namespace
 
@@ -404,29 +417,6 @@ extern "C" int ctd_pages_plan(ctd_page_entry* pages, int32_t n, int32_t net_h, i
   return CTD_OK;
 }
 
-// device buffer of a slot, grown (never shrunk) to `bytes`; only called while no enqueued work uses the buffer (the
-// page and results buffers at submit, while the slot is idle; the crop buffer by the worker, after syncing `post`)
-static int grow_slot_buffer(ctd_handle* h, uint8_t** buf, size_t* cap, size_t bytes) {
-  if (bytes <= *cap) return CTD_OK;
-  cudaFree(*buf);
-  *buf = nullptr;
-  *cap = 0;
-  CK(cudaMalloc(reinterpret_cast<void**>(buf), bytes + bytes / 4));
-  *cap = bytes + bytes / 4;
-  return CTD_OK;
-}
-
-// the same for a pinned host buffer
-static int grow_slot_pinned(ctd_handle* h, uint8_t** buf, size_t* cap, size_t bytes) {
-  if (bytes <= *cap) return CTD_OK;
-  if (*buf) cudaFreeHost(*buf);
-  *buf = nullptr;
-  *cap = 0;
-  CK(cudaHostAlloc(reinterpret_cast<void**>(buf), bytes + bytes / 4, cudaHostAllocDefault));
-  *cap = bytes + bytes / 4;
-  return CTD_OK;
-}
-
 // ctd_region_plan of every line of one page's block section, in block then line order (textblock.region_lines)
 static int plan_page_regions(const char* section, const BlockSection& bs, int iw, int ih, int textheight,
                              std::vector<ctd_region>& plan, size_t* bytes) {
@@ -451,16 +441,13 @@ static int plan_page_regions(const char* section, const BlockSection& bs, int iw
   return ctd_region_plan(lines.data(), int32_t(lines.size()), iw, ih, textheight, plan.data(), bytes);
 }
 
-// phases B and C of a ctd_submit_pages batch, on the worker thread
-static int run_pages_job(ctd_handle* h, const PipeJob& job) {
-  const int slot = job.slot, n = job.n;
-  CK(cudaEventSynchronize(h->ev_out_done[slot]));          // phase A results are in results_host
-  char* res = static_cast<char*>(job.results_host);
-  const PagesHead hd = pages_head(n);
+// phases B and C of a submitted batch, on the worker thread
+static int run_batch(ctd_handle* h, const PipeJob& job) {
+  Slot& s = h->slot[job.slot];
+  const int n = int(job.pages.size());
+  CK(cudaEventSynchronize(s.ev_out_done));          // phase A results are in results_host
+  char* res = job.results_host;
   const BlockSection bs = block_section_layout();
-  const std::vector<ctd_page_entry>& pg = job.pages;
-  const int32_t* det_cnt = reinterpret_cast<const int32_t*>(res + hd.cnt);
-  const int32_t* line_cnt = reinterpret_cast<const int32_t*>(res + hd.lc);
   std::vector<std::vector<int32_t>> wins(static_cast<size_t>(n));
   std::vector<int> prc(size_t(n), CTD_OK);
   // text-line crops: each page's plan on the host threads, right after its group_output
@@ -469,20 +456,11 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
   std::vector<size_t> plan_bytes(size_t(n), 0);
   std::vector<int> crc(size_t(n), CTD_OK);
   for_each_page(n, h->host_threads, [&](int i) {
-    const ctd_page_entry& e = pg[size_t(i)];
-    Letterbox lb;
-    letterbox_of(e.ih, e.iw, job.ph, job.pw, lb);   // planned: cannot fail
-    PageIn in;
-    in.det = reinterpret_cast<const float*>(res + hd.det) + size_t(i) * 300 * 6;
-    in.n_det = std::min(std::max(det_cnt[i], 0), 300);
-    in.line_boxes = reinterpret_cast<const int16_t*>(res + hd.lb) + size_t(i) * 1000 * 8;
-    in.line_scores = reinterpret_cast<const float*>(res + hd.ls) + size_t(i) * 1000;
-    in.n_lines = std::min(std::max(line_cnt[i], 0), 1000);
-    in.mask = reinterpret_cast<const uint8_t*>(res + e.mask_off);
-    in.im_w = e.iw; in.im_h = e.ih; in.ratio_x = lb.ratio_x; in.ratio_y = lb.ratio_y;
-    prc[size_t(i)] = host_group_page(in, res + e.blocks_off, bs, wins[size_t(i)]);
+    const JobPage& p = job.pages[size_t(i)];
+    const uint8_t* mask = reinterpret_cast<const uint8_t*>(res + job.head.masks + p.off);
+    prc[size_t(i)] = host_group_page(page_in(res, job.head, i, p, mask), p.section, bs, wins[size_t(i)]);
     if (crops && prc[size_t(i)] == CTD_OK)
-      crc[size_t(i)] = plan_page_regions(res + e.blocks_off, bs, e.iw, e.ih, job.textheight, plans[size_t(i)],
+      crc[size_t(i)] = plan_page_regions(p.section, bs, p.iw, p.ih, job.textheight, plans[size_t(i)],
                                          &plan_bytes[size_t(i)]);
   });
   for (int i = 0; i < n; ++i)
@@ -490,96 +468,72 @@ static int run_pages_job(ctd_handle* h, const PipeJob& job) {
   for (int i = 0; i < n; ++i)
     if (crc[size_t(i)] != CTD_OK)
       return ctd_fail(h, crc[size_t(i)], "ctd_region_plan refused page %d of the batch (%dx%d, textheight %d)", i,
-                      pg[size_t(i)].ih, pg[size_t(i)].iw, job.textheight);
+                      job.pages[size_t(i)].ih, job.pages[size_t(i)].iw, job.textheight);
   // the batch's plans, concatenated with each page's crops after the previous page's; one warp job for all pages
   RegionJob rg;
   if (crops) {
-    std::vector<ctd_region>& plan = h->crop_plan[slot];
-    std::vector<int32_t>& first = h->crop_first[slot];
-    std::vector<size_t>& page_base = h->crop_base[slot];
-    plan.clear();
-    first.assign(size_t(n) + 1, 0);
-    page_base.assign(size_t(n) + 1, 0);
+    s.crop_plan.clear();
+    s.crop_first.assign(size_t(n) + 1, 0);
+    s.crop_base.assign(size_t(n) + 1, 0);
     size_t base = 0;
     for (int i = 0; i < n; ++i) {
-      const ctd_page_entry& e = pg[size_t(i)];
+      const JobPage& pg = job.pages[size_t(i)];
       const std::vector<ctd_region>& p = plans[size_t(i)];
-      if (int bad = rg.add(p.data(), int(p.size()), e.page_off, e.ih, e.iw, (long long)base); bad >= 0)
+      if (int bad = rg.add(p.data(), int(p.size()), (long long)(pg.off * 3), pg.ih, pg.iw, (long long)base); bad >= 0)
         return ctd_fail(h, CTD_E_INVALID, "malformed crop plan entry %d on page %d of the batch", bad, i);
-      first[size_t(i)] = int32_t(plan.size());
-      page_base[size_t(i)] = base;
+      s.crop_first[size_t(i)] = int32_t(s.crop_plan.size());
+      s.crop_base[size_t(i)] = base;
       for (ctd_region r : p) {
         r.offset += int64_t(base);
-        plan.push_back(r);
+        s.crop_plan.push_back(r);
       }
       base += plan_bytes[size_t(i)];
     }
-    first[size_t(n)] = int32_t(plan.size());
-    page_base[size_t(n)] = base;
-    if (plan.size() > size_t(INT32_MAX) || rg.tiles.size() > size_t(INT32_MAX))
+    s.crop_first[size_t(n)] = int32_t(s.crop_plan.size());
+    s.crop_base[size_t(n)] = base;
+    if (s.crop_plan.size() > size_t(INT32_MAX) || rg.tiles.size() > size_t(INT32_MAX))
       return ctd_fail(h, CTD_E_CAPACITY, "too many crops in one batch");
-    h->crop_bytes[slot] = base;
-    h->crop_px_off[slot] = 0;
-  }
-  RefineJob rj;
-  for (int i = 0; i < n; ++i) {
-    const ctd_page_entry& e = pg[size_t(i)];
-    for (size_t k = 0; k + 3 < wins[size_t(i)].size(); k += 4)
-      rj.add(wins[size_t(i)][k], wins[size_t(i)][k + 1], wins[size_t(i)][k + 2], wins[size_t(i)][k + 3],
-             size_t(e.mask_off) - hd.masks, e.iw, e.ih);
+    s.crop_bytes = base;
+    s.crop_px_off = 0;
   }
   // phase C on the post stream over the slot's resident pages and masks
   cudaStream_t st = h->post;
-  // enqueued here, not at submit: a wait enqueued at submit time would also hold this batch's phase C behind the
-  // forward of every batch submitted before the worker reached it
-  CK(cudaStreamWaitEvent(st, h->ev_out_ready[slot], 0));   // phase C never starts before its phase A copy
+  // enqueued here for ctd_submit_pages*, not at submit: a wait enqueued at submit time would also hold this batch's
+  // phase C behind the forward of every batch submitted before the worker reached it (ctd_submit_full enqueues it at
+  // submit as well)
+  CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // phase C never starts before its phase A copy
+  // ctd_submit_full: block sections to the device arena copy (one gather then moves everything)
+  if (job.d_blocks)
+    CK(cudaMemcpyAsync(job.d_blocks, job.pages[0].section, job.blocks_bytes, cudaMemcpyHostToDevice, st));
   const bool to_host = !job.results_on_device;
   if (!rg.tiles.empty()) {
-    // crops: tables staged in the slot's pinned crop buffer, one launch over the pages in place in d_pg_in[slot], the
-    // pixels back into the same pinned buffer after the tables (unless they stay on the device, after the tables in
-    // d_crop[slot]).  Both buffers grow only after `st` is idle, since an earlier failed job of this slot may have left
+    // crops: tables staged in the slot's pinned crop buffer, one launch over the pages in place in the page buffer,
+    // the pixels back into the same pinned buffer after the tables (unless they stay on the device, after the tables
+    // in d_crop).  Both buffers grow only after `st` is idle, since an earlier failed job of this slot may have left
     // copies on it.
-    const size_t tb = rg.table_bytes(), px = h->crop_bytes[slot];
-    const size_t host_need = to_host ? tb + px : tb;
-    if (tb + px > h->crop_dcap[slot] || host_need > h->crop_hcap[slot]) CK(cudaStreamSynchronize(st));
-    if (int rc = grow_slot_buffer(h, &h->d_crop[slot], &h->crop_dcap[slot], tb + px)) return rc;
-    if (int rc = grow_slot_pinned(h, &h->h_crop[slot], &h->crop_hcap[slot], host_need)) return rc;
-    uint8_t* d_tab = h->d_crop[slot];
-    rg.write_tables(reinterpret_cast<char*>(h->h_crop[slot]));
-    CK(cudaMemcpyAsync(d_tab, h->h_crop[slot], tb, cudaMemcpyHostToDevice, st));
+    const size_t tb = rg.table_bytes(), px = s.crop_bytes;
+    if (int rc = s.d_crop.grow(h, tb + px, st)) return rc;
+    if (int rc = s.h_crop.grow(h, to_host ? tb + px : tb, st)) return rc;
+    uint8_t* d_tab = s.d_crop.p;
+    rg.write_tables(reinterpret_cast<char*>(s.h_crop.p));
+    CK(cudaMemcpyAsync(d_tab, s.h_crop.p, tb, cudaMemcpyHostToDevice, st));
     const size_t rb = (rg.regs.size() * sizeof(ctd::RegionDev) + 255) / 256 * 256;
-    CK(ctd::warp_regions_launch(h->d_pg_in[slot], reinterpret_cast<const ctd::RegionDev*>(d_tab),
+    CK(ctd::warp_regions_launch(job.d_img, reinterpret_cast<const ctd::RegionDev*>(d_tab),
                                 reinterpret_cast<const ctd::RegionTile*>(d_tab + rb), int(rg.tiles.size()), d_tab + tb,
                                 st));
-    if (to_host) CK(cudaMemcpyAsync(h->h_crop[slot] + tb, d_tab + tb, px, cudaMemcpyDeviceToHost, st));
-    h->crop_px_off[slot] = tb;
+    if (to_host) CK(cudaMemcpyAsync(s.h_crop.p + tb, d_tab + tb, px, cudaMemcpyDeviceToHost, st));
+    s.crop_px_off = tb;
   }
-  const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);   // pixels of all planes of the batch
-  uint8_t* d_res = h->d_pg_res[slot];
-  uint8_t* d_mask = d_res + hd.masks;
-  uint8_t* d_ref = d_res + pg[0].refined_off;
-  CK(cudaMemsetAsync(d_ref, 0, total, st));
-  char* stage_tab = rj.table_bytes() <= h->pipe_pinned_cap ? h->pipe_pinned[slot] : nullptr;   // else: pageable + sync
-  if (int rc = launch_refine(h, rj, h->d_pg_in[slot], d_mask, job.refine_mode, d_ref, st, &h->d_post_refine,
-                             &h->post_refine_cap, stage_tab))
+  CK(cudaMemsetAsync(job.d_ref, 0, job.total, st));
+  const Planes pl{job.d_img, job.d_mask, job.d_ref, job.d_aux, job.d_aux ? job.d_aux + job.total : nullptr, job.total};
+  if (int rc = phase_c(h, job.pages, wins, pl, job.refine_mode, job.keep_undetected, st, h->post_refine, h->pg_cc,
+                       s.pinned, h->pipe_pinned_cap))
     return rc;
-  if (job.keep_undetected) {
-    std::vector<UndetPage> up(static_cast<size_t>(n));
-    for (int i = 0; i < n; ++i) {
-      const ctd_page_entry& e = pg[size_t(i)];
-      const ctd_page_blocks* hdr = reinterpret_cast<const ctd_page_blocks*>(res + e.blocks_off);
-      up[size_t(i)] = UndetPage{size_t(e.mask_off) - hd.masks, e.ih, e.iw,
-                                reinterpret_cast<const ctd_block*>(res + e.blocks_off + bs.rec_off), hdr->n_blocks};
-    }
-    uint8_t* d_ref2 = h->d_pg_aux[slot];
-    if (int rc = refine_undetected(h, up, total, h->d_pg_in[slot], d_mask, d_ref, d_ref2, d_ref2 + total, job.refine_mode,
-                                   st, &h->d_pg_cc, &h->pg_cc_cap, &h->d_post_refine, &h->post_refine_cap,
-                                   h->pipe_pinned[slot], h->pipe_pinned_cap))
-      return rc;
-    if (to_host) CK(cudaMemcpyAsync(res + hd.masks, d_mask, total, cudaMemcpyDeviceToHost, st));
+  if (to_host) {
+    if (job.keep_undetected) CK(cudaMemcpyAsync(res + job.head.masks, job.d_mask, job.total, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(res + job.refined, job.d_ref, job.total, cudaMemcpyDeviceToHost, st));
   }
-  if (to_host) CK(cudaMemcpyAsync(res + pg[0].refined_off, d_ref, total, cudaMemcpyDeviceToHost, st));
-  CK(cudaEventRecord(h->ev_post_done[slot], st));
+  CK(cudaEventRecord(s.ev_post_done, st));
   return CTD_OK;
 }
 
@@ -592,67 +546,34 @@ static void pipe_worker(ctd_handle* h) {
       std::unique_lock<std::mutex> lk(h->pipe_mu);
       h->pipe_cv.wait(lk, [&] { return h->pipe_quit || !h->pipe_queue.empty(); });
       if (h->pipe_queue.empty()) return;    // quit requested and nothing left
-      job = h->pipe_queue.front();
+      job = std::move(h->pipe_queue.front());
       h->pipe_queue.pop_front();
     }
-    int rc = CTD_OK;
+    const int rc = run_batch(h, job);
     std::string err;
-    auto run = [&]() -> int {
-      const ArenaLayout& L = h->layout;
-      const int slot = job.slot, n = job.n, ph = job.ph, pw = job.pw;
-      CK(cudaEventSynchronize(h->ev_out_done[slot]));          // phase A results are in results_host
-      char* res = static_cast<char*>(job.results_host);
-      const size_t px = size_t(ph) * pw;
-      const int32_t* det_cnt = reinterpret_cast<const int32_t*>(res + L.cnt);
-      const int32_t* line_cnt = reinterpret_cast<const int32_t*>(res + L.lc);
-      std::vector<std::vector<int32_t>> wins;
-      wins.resize(size_t(n));
-      std::vector<int> prc(size_t(n), CTD_OK);
-      auto one = [&](int i) {
-        PageIn in;
-        in.det = reinterpret_cast<const float*>(res + L.det) + size_t(i) * 300 * 6;
-        in.n_det = std::min(std::max(det_cnt[i], 0), 300);
-        in.line_boxes = reinterpret_cast<const int16_t*>(res + L.lb) + size_t(i) * 1000 * 8;
-        in.line_scores = reinterpret_cast<const float*>(res + L.ls) + size_t(i) * 1000;
-        in.n_lines = std::min(std::max(line_cnt[i], 0), 1000);
-        in.mask = reinterpret_cast<const uint8_t*>(res) + size_t(i) * px;
-        in.im_w = pw; in.im_h = ph; in.ratio_x = 1.f; in.ratio_y = 1.f;
-        prc[size_t(i)] = host_group_page(in, res + L.blocks + size_t(i) * L.blocks_stride, block_section_layout(),
-                                         wins[size_t(i)]);
-      };
-      for_each_page(n, h->host_threads, one);
-      for (int i = 0; i < n; ++i)
-        if (prc[size_t(i)] != CTD_OK) return ctd_fail(h, prc[size_t(i)], "group_output failed on page %d of the batch", i);
-      RefineJob rj;
-      for (int i = 0; i < n; ++i)
-        for (size_t k = 0; k + 3 < wins[size_t(i)].size(); k += 4)
-          rj.add(wins[size_t(i)][k], wins[size_t(i)][k + 1], wins[size_t(i)][k + 2], wins[size_t(i)][k + 3],
-                 size_t(i) * ph * pw, pw, ph);
-      // phase C on the post stream: block sections to the device arena copy (one gather then moves everything),
-      // refine on the resident pages + mask, mask_refined back to the host
-      cudaStream_t st = h->post;
-      uint8_t* d_arena = h->d_stage_out[slot];
-      CK(cudaMemcpyAsync(d_arena + L.blocks, res + L.blocks, size_t(n) * L.blocks_stride, cudaMemcpyHostToDevice, st));
-      CK(cudaMemsetAsync(d_arena + L.refined, 0, size_t(n) * px, st));
-      char* stage_tab = rj.table_bytes() <= h->pipe_pinned_cap ? h->pipe_pinned[slot] : nullptr;   // else: pageable + sync
-      const uint8_t* d_pages = job.pages_dev ? job.pages_dev : h->d_stage_in[slot];
-      if (int r2 = launch_refine(h, rj, d_pages, d_arena, job.refine_mode, d_arena + L.refined, st, &h->d_post_refine,
-                                 &h->post_refine_cap, stage_tab))
-        return r2;
-      CK(cudaMemcpyAsync(res + L.refined, d_arena + L.refined, size_t(n) * px, cudaMemcpyDeviceToHost, st));
-      CK(cudaEventRecord(h->ev_post_done[slot], st));
-      return CTD_OK;
-    };
-    rc = job.pages.empty() ? run() : run_pages_job(h, job);
     if (rc != CTD_OK) err = h->err;
     {
       std::lock_guard<std::mutex> lk(h->pipe_mu);
-      h->pipe_state[job.slot] = rc == CTD_OK ? 2 : 3;
-      h->pipe_rc[job.slot] = rc;
-      h->pipe_err[job.slot] = err;
+      Slot& s = h->slot[job.slot];
+      s.state = rc == CTD_OK ? 2 : 3;
+      s.rc = rc;
+      s.err = err;
     }
     h->pipe_done_cv.notify_all();
   }
+}
+
+// hands a submitted batch to the worker
+static void queue_job(ctd_handle* h, PipeJob&& job) {
+  Slot& s = h->slot[job.slot];
+  {
+    std::lock_guard<std::mutex> lk(h->pipe_mu);
+    s.state = 1;
+    h->pipe_queue.push_back(std::move(job));
+  }
+  h->pipe_cv.notify_one();
+  s.busy = true;
+  s.full = true;
 }
 
 static int ensure_full_pipeline(ctd_handle* h) {
@@ -665,9 +586,9 @@ static int ensure_full_pipeline(ctd_handle* h) {
   // (16 bytes each)
   h->pipe_pinned_cap = size_t(h->cfg.max_batch) * (size_t(CTD_MAX_BLOCKS) * sizeof(RefineWin) +
                                                    size_t(CTD_MAX_BLOCKS) * sizeof(RefineChunk) * 8) + (size_t(8) << 20);
-  for (int i = 0; i < 2; ++i) {
-    CK(cudaHostAlloc(reinterpret_cast<void**>(&h->pipe_pinned[i]), h->pipe_pinned_cap, cudaHostAllocDefault));
-    CK(cudaEventCreateWithFlags(&h->ev_post_done[i], cudaEventDisableTiming));
+  for (Slot& s : h->slot) {
+    CK(cudaHostAlloc(reinterpret_cast<void**>(&s.pinned), h->pipe_pinned_cap, cudaHostAllocDefault));
+    CK(cudaEventCreateWithFlags(&s.ev_post_done, cudaEventDisableTiming));
   }
   const char* ht = getenv("CTD_HOST_THREADS");
   const unsigned hc = std::thread::hardware_concurrency();
@@ -677,6 +598,7 @@ static int ensure_full_pipeline(ctd_handle* h) {
   return CTD_OK;
 }
 
+// stops the worker and frees the handle-wide pipeline state (each slot's own: Slot::release)
 void ctd_pipeline_shutdown(ctd_handle* h) {
   if (h->pipe_thread.joinable()) {
     {
@@ -686,84 +608,44 @@ void ctd_pipeline_shutdown(ctd_handle* h) {
     h->pipe_cv.notify_all();
     h->pipe_thread.join();
   }
-  for (int i = 0; i < 2; ++i) {
-    if (h->pipe_pinned[i]) cudaFreeHost(h->pipe_pinned[i]);
-    if (h->ev_post_done[i]) cudaEventDestroy(h->ev_post_done[i]);
-    h->pipe_pinned[i] = nullptr;
-    h->ev_post_done[i] = nullptr;
-  }
   if (h->post) cudaStreamDestroy(h->post);
   h->post = nullptr;
-  for (int i = 0; i < 2; ++i) {
-    cudaFree(h->d_pg_in[i]); cudaFree(h->d_pg_res[i]); cudaFree(h->d_pg_aux[i]); cudaFree(h->d_pg_tab[i]);
-    if (h->h_pg_tab[i]) cudaFreeHost(h->h_pg_tab[i]);
-    h->d_pg_in[i] = h->d_pg_res[i] = h->d_pg_aux[i] = nullptr;
-    h->pg_in_cap[i] = h->pg_res_cap[i] = h->pg_aux_cap[i] = 0;
-    h->d_pg_tab[i] = nullptr;
-    h->h_pg_tab[i] = nullptr;
-  }
-  for (int i = 0; i < 2; ++i) {
-    cudaFree(h->d_crop[i]);
-    if (h->h_crop[i]) cudaFreeHost(h->h_crop[i]);
-    h->d_crop[i] = h->h_crop[i] = nullptr;
-    h->crop_dcap[i] = h->crop_hcap[i] = 0;
-    h->crop_ready[i] = false;
-    h->dev_ready[i] = false;
-  }
   if (h->dev_out) cudaStreamDestroy(h->dev_out);
   h->dev_out = nullptr;
-  cudaFree(h->d_pg_cc);
-  h->d_pg_cc = nullptr;
-  h->pg_cc_cap = 0;
-  cudaFree(h->d_post_refine);
-  h->d_post_refine = nullptr;
-  h->post_refine_cap = 0;
+  h->pg_cc.release();
+  h->post_refine.release();
 }
 
 extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages, int32_t n, int32_t ph, int32_t pw,
                                int32_t pages_on_device, int32_t refine_mode, void* results_host) {
   if (!h || !pages || !results_host || slot < 0 || slot > 1) return CTD_E_INVALID;
   if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit_full needs the full pipeline");
-  if (h->slot_busy[slot]) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  Slot& s = h->slot[slot];
+  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
   ShapePlan* sp = nullptr;
   if (int rc = prepare_forward(h, n, ph, pw, &sp)) return rc;
   if (int rc = ensure_full_pipeline(h)) return rc;
-  h->crop_ready[slot] = false;
-  h->dev_ready[slot] = false;
-  const ArenaLayout& L = h->layout;
-  const size_t bytes = size_t(n) * ph * pw * 3;
+  s.start(false, false);
   // the previous use of this slot's staging (refine reads stage_in / stage_out) ended with its collect
-  if (!pages_on_device) {
-    CK(cudaStreamWaitEvent(h->copy_in, h->ev_in_free[slot], 0));
-    CK(cudaMemcpyAsync(h->d_stage_in[slot], pages, bytes, cudaMemcpyHostToDevice, h->copy_in));
-    CK(cudaEventRecord(h->ev_in_done[slot], h->copy_in));
-    CK(cudaEventRecord(h->ev0, h->stream));
-    CK(cudaStreamWaitEvent(h->stream, h->ev_in_done[slot], 0));
-    CK(cudaMemcpyAsync(h->d_pages, h->d_stage_in[slot], bytes, cudaMemcpyDeviceToDevice, h->stream));
-    CK(cudaEventRecord(h->ev_in_free[slot], h->stream));
-  } else {
-    CK(cudaEventRecord(h->ev0, h->stream));
-    CK(cudaMemcpyAsync(h->d_pages, pages, bytes, cudaMemcpyDeviceToDevice, h->stream));
-  }
-  if (int rc = enqueue_forward(h, n, ph, pw, *sp)) return rc;
-  CK(cudaMemcpyAsync(h->d_stage_out[slot], h->d_mask_u8, L.a_bytes, cudaMemcpyDeviceToDevice, h->stream));
-  CK(cudaEventRecord(h->ev_out_ready[slot], h->stream));
-  CK(cudaStreamWaitEvent(h->copy_out, h->ev_out_ready[slot], 0));
-  CK(cudaMemcpyAsync(results_host, h->d_stage_out[slot], L.a_bytes, cudaMemcpyDeviceToHost, h->copy_out));
-  CK(cudaEventRecord(h->ev_out_done[slot], h->copy_out));
-  CK(cudaStreamWaitEvent(h->post, h->ev_out_ready[slot], 0));   // phase C never starts before its phase A copy
-  {
-    std::lock_guard<std::mutex> lk(h->pipe_mu);
-    PipeJob job;
-    job.slot = slot; job.n = n; job.ph = ph; job.pw = pw; job.refine_mode = refine_mode;
-    job.results_host = results_host;
-    job.pages_dev = pages_on_device ? pages : nullptr;
-    h->pipe_state[slot] = 1;
-    h->pipe_queue.push_back(job);
-  }
-  h->pipe_cv.notify_one();
-  h->slot_busy[slot] = true;
-  h->slot_full[slot] = true;
+  if (int rc = stage_phase_a(h, s, pages, pages_on_device != 0, n, ph, pw, *sp, results_host)) return rc;
+  CK(cudaStreamWaitEvent(h->post, s.ev_out_ready, 0));   // phase C never starts before its phase A copy
+  // net-sized pages letterbox to themselves: resize_ratio 1
+  const ArenaLayout& L = h->layout;
+  const size_t px = size_t(ph) * pw;
+  PipeJob job;
+  job.slot = slot; job.refine_mode = refine_mode;
+  job.results_host = static_cast<char*>(results_host);
+  job.head = PagesHead{L.det, L.cnt, L.lb, L.ls, L.lc, 0};
+  job.refined = L.refined;
+  for (int i = 0; i < n; ++i)
+    job.pages.push_back(JobPage{ph, pw, 1.f, 1.f, size_t(i) * px, job.results_host + L.blocks + size_t(i) * L.blocks_stride});
+  job.total = size_t(n) * px;
+  job.d_img = pages_on_device ? pages : s.d_stage_in;
+  job.d_mask = s.d_stage_out;
+  job.d_ref = s.d_stage_out + L.refined;
+  job.d_blocks = s.d_stage_out + L.blocks;
+  job.blocks_bytes = size_t(n) * L.blocks_stride;
+  queue_job(h, std::move(job));
   return CTD_OK;
 }
 
@@ -799,7 +681,8 @@ extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_pa
   if (!h || !pages || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
   if (textheight != 0 && textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
   if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit_pages needs the full pipeline");
-  if (h->slot_busy[slot]) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  Slot& s = h->slot[slot];
+  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
   if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
   // the offsets decide where the copies write: they must be the plan's
   std::vector<ctd_page_entry> pg(pages, pages + n);
@@ -839,19 +722,19 @@ extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_pa
   const PagesHead hd = pages_head(n);
   const size_t total = size_t(pg[0].refined_off - pg[0].mask_off);
   const size_t d2h = size_t(pg[0].refined_off);                       // phase-A rows + masks
-  h->crop_ready[slot] = false;
-  h->dev_ready[slot] = false;
-  if (int rc = grow_slot_buffer(h, &h->d_pg_in[slot], &h->pg_in_cap[slot], in_bytes)) return rc;
-  if (int rc = grow_slot_buffer(h, &h->d_pg_res[slot], &h->pg_res_cap[slot], d2h + total)) return rc;
+  s.start(textheight > 0, results_on_device != 0);
+  // grown while the slot is idle: its collect has synchronised the work of its last batch
+  if (int rc = s.pg_in.grow(h, in_bytes, std::nullopt)) return rc;
+  if (int rc = s.pg_res.grow(h, d2h + total, std::nullopt)) return rc;
   if (keep_undetected)
-    if (int rc = grow_slot_buffer(h, &h->d_pg_aux[slot], &h->pg_aux_cap[slot], 2 * total)) return rc;
-  if (!h->h_pg_tab[slot]) {
+    if (int rc = s.pg_aux.grow(h, 2 * total, std::nullopt)) return rc;
+  if (!s.h_pg_tab) {
     h->pg_gather_off = (size_t(h->cfg.max_batch) * sizeof(PageGeom) + 255) / 256 * 256;
     const size_t tab_bytes = h->pg_gather_off + size_t(h->cfg.max_batch) * sizeof(GatherPage);
-    CK(cudaHostAlloc(reinterpret_cast<void**>(&h->h_pg_tab[slot]), tab_bytes, cudaHostAllocDefault));
-    CK(cudaMalloc(reinterpret_cast<void**>(&h->d_pg_tab[slot]), tab_bytes));
+    CK(cudaHostAlloc(reinterpret_cast<void**>(&s.h_pg_tab), tab_bytes, cudaHostAllocDefault));
+    CK(cudaMalloc(reinterpret_cast<void**>(&s.d_pg_tab), tab_bytes));
   }
-  PageGeom* tab = h->h_pg_tab[slot];
+  PageGeom* tab = s.h_pg_tab;
   GatherPage* gtab = reinterpret_cast<GatherPage*>(reinterpret_cast<char*>(tab) + h->pg_gather_off);
   int row0 = 0, n_gather = 0, gather_rows = 0;
   for (int i = 0; i < n; ++i) {
@@ -870,9 +753,9 @@ extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_pa
   // one copy per run of consecutive host pages); the device pages' events, the gather of the device pages, letterbox,
   // forward, back-projection and the phase-A rows on the engine stream; rows + masks out on copy_out
   const size_t tab_bytes = n_gather ? h->pg_gather_off + size_t(n_gather) * sizeof(GatherPage) : size_t(n) * sizeof(PageGeom);
-  CK(cudaMemcpyAsync(h->d_pg_tab[slot], tab, tab_bytes, cudaMemcpyHostToDevice, h->copy_in));
+  CK(cudaMemcpyAsync(s.d_pg_tab, tab, tab_bytes, cudaMemcpyHostToDevice, h->copy_in));
   if (n_dev == 0) {
-    CK(cudaMemcpyAsync(h->d_pg_in[slot], input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
+    CK(cudaMemcpyAsync(s.pg_in.p, input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
   } else {
     for (int i = 0; i < n;) {
       if (dev[i].data) { ++i; continue; }
@@ -880,81 +763,83 @@ extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_pa
       while (j + 1 < n && !dev[j + 1].data) ++j;
       const size_t lo = size_t(pg[size_t(i)].page_off);
       const size_t hi = size_t(pg[size_t(j)].page_off) + size_t(pg[size_t(j)].ih) * size_t(pg[size_t(j)].iw) * 3;
-      CK(cudaMemcpyAsync(h->d_pg_in[slot] + lo, input_host + lo, hi - lo, cudaMemcpyHostToDevice, h->copy_in));
+      CK(cudaMemcpyAsync(s.pg_in.p + lo, input_host + lo, hi - lo, cudaMemcpyHostToDevice, h->copy_in));
       i = j + 1;
     }
   }
-  CK(cudaEventRecord(h->ev_in_done[slot], h->copy_in));
+  CK(cudaEventRecord(s.ev_in_done, h->copy_in));
   CK(cudaEventRecord(h->ev0, h->stream));
-  CK(cudaStreamWaitEvent(h->stream, h->ev_in_done[slot], 0));
+  CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
   if (n_gather) {
     for (int i = 0; i < n; ++i)
       if (dev[i].data && dev[i].event) CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(dev[i].event), 0));
-    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(reinterpret_cast<const char*>(h->d_pg_tab[slot]) +
+    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(reinterpret_cast<const char*>(s.d_pg_tab) +
                                                                h->pg_gather_off),
-                           n_gather, gather_rows, h->d_pg_in[slot], h->stream));
+                           n_gather, gather_rows, s.pg_in.p, h->stream));
   }
-  CK(letterbox_batch_launch(h->d_pg_in[slot], h->d_pg_tab[slot], n, h->d_pages, net_h, net_w, h->stream));
+  CK(letterbox_batch_launch(s.pg_in.p, s.d_pg_tab, n, h->d_pages, net_h, net_w, h->stream));
   if (int rc = enqueue_forward(h, n, net_h, net_w, *sp)) return rc;
-  uint8_t* d_res = h->d_pg_res[slot];
-  CK(backproject_batch_launch(h->d_mask_u8, net_h, net_w, h->d_pg_tab[slot], n, row0, d_res + hd.masks, h->stream));
+  uint8_t* d_res = s.pg_res.p;
+  CK(backproject_batch_launch(h->d_mask_u8, net_h, net_w, s.d_pg_tab, n, row0, d_res + hd.masks, h->stream));
   const size_t nb = size_t(n);
   CK(cudaMemcpyAsync(d_res + hd.det, h->d_mask_u8 + L.det, nb * 300 * 6 * 4, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(d_res + hd.cnt, h->d_mask_u8 + L.cnt, nb * 4, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(d_res + hd.lb, h->d_mask_u8 + L.lb, nb * 1000 * 8 * 2, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(d_res + hd.ls, h->d_mask_u8 + L.ls, nb * 1000 * 4, cudaMemcpyDeviceToDevice, h->stream));
   CK(cudaMemcpyAsync(d_res + hd.lc, h->d_mask_u8 + L.lc, nb * 4, cudaMemcpyDeviceToDevice, h->stream));
-  CK(cudaEventRecord(h->ev_out_ready[slot], h->stream));
-  CK(cudaStreamWaitEvent(h->copy_out, h->ev_out_ready[slot], 0));
+  CK(cudaEventRecord(s.ev_out_ready, h->stream));
+  CK(cudaStreamWaitEvent(h->copy_out, s.ev_out_ready, 0));
   CK(cudaMemcpyAsync(results_host, d_res, d2h, cudaMemcpyDeviceToHost, h->copy_out));
-  CK(cudaEventRecord(h->ev_out_done[slot], h->copy_out));
-  {
-    std::lock_guard<std::mutex> lk(h->pipe_mu);
-    PipeJob job;
-    job.slot = slot; job.n = n; job.ph = net_h; job.pw = net_w; job.refine_mode = refine_mode;
-    job.results_host = results_host;
-    job.pages = std::move(pg);
-    job.keep_undetected = keep_undetected ? 1 : 0;
-    job.textheight = textheight;
-    job.results_on_device = results_on_device ? 1 : 0;
-    if (results_on_device) h->dev_pages[slot] = job.pages;
-    h->pipe_state[slot] = 1;
-    h->pipe_queue.push_back(std::move(job));
+  CK(cudaEventRecord(s.ev_out_done, h->copy_out));
+  PipeJob job;
+  job.slot = slot; job.refine_mode = refine_mode;
+  job.results_host = static_cast<char*>(results_host);
+  job.head = hd;
+  job.refined = size_t(pg[0].refined_off);
+  for (const ctd_page_entry& e : pg) {
+    Letterbox lb;
+    letterbox_of(e.ih, e.iw, net_h, net_w, lb);   // planned: cannot fail
+    job.pages.push_back(JobPage{e.ih, e.iw, lb.ratio_x, lb.ratio_y, size_t(e.mask_off) - hd.masks,
+                                job.results_host + e.blocks_off});
   }
-  h->pipe_cv.notify_one();
-  h->slot_busy[slot] = true;
-  h->slot_full[slot] = true;
-  h->crop_ready[slot] = textheight > 0;          // both cleared again if the batch fails
-  h->dev_ready[slot] = results_on_device != 0;
+  job.total = total;
+  job.d_img = s.pg_in.p;
+  job.d_mask = d_res + hd.masks;
+  job.d_ref = d_res + pg[0].refined_off;
+  job.d_aux = keep_undetected ? s.pg_aux.p : nullptr;
+  job.keep_undetected = keep_undetected ? 1 : 0;
+  job.textheight = textheight;
+  job.results_on_device = results_on_device ? 1 : 0;
+  if (results_on_device) s.dev_pages = std::move(pg);
+  queue_job(h, std::move(job));
   return CTD_OK;
 }
 
 // called by ctd_collect for slots submitted with ctd_submit_full or ctd_submit_pages
 int ctd_collect_full(ctd_handle* h, int slot) {
+  Slot& s = h->slot[slot];
   int rc;
   {
     std::unique_lock<std::mutex> lk(h->pipe_mu);
-    h->pipe_done_cv.wait(lk, [&] { return h->pipe_state[slot] >= 2; });
-    rc = h->pipe_rc[slot];
-    if (rc != CTD_OK) h->err = h->pipe_err[slot];
-    h->pipe_state[slot] = 0;
+    h->pipe_done_cv.wait(lk, [&] { return s.state >= 2; });
+    rc = s.rc;
+    if (rc != CTD_OK) h->err = s.err;
+    s.state = 0;
   }
-  h->slot_full[slot] = false;
-  if (rc != CTD_OK) {
-    h->crop_ready[slot] = false;
-    h->dev_ready[slot] = false;
-    return rc;
-  }
-  CK(cudaEventSynchronize(h->ev_post_done[slot]));
+  s.full = false;
+  if (rc != CTD_OK) return rc;
+  CK(cudaEventSynchronize(s.ev_post_done));
+  s.collected = true;
   return CTD_OK;
 }
 
 extern "C" int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page_dst) {
   if (!h || slot < 0 || slot > 1 || !page_dst) return CTD_E_INVALID;
-  if (h->slot_busy[slot] || !h->dev_ready[slot])
+  const Slot& s = h->slot[slot];
+  if (s.busy || !s.collected || !s.on_device)
     return ctd_fail(h, CTD_E_INVALID, "slot %d holds no collected batch with results on the device", slot);
   CK(cudaSetDevice(h->cfg.device));
-  const std::vector<ctd_page_entry>& pg = h->dev_pages[slot];
+  const std::vector<ctd_page_entry>& pg = s.dev_pages;
   const int n = int(pg.size());
   for (int i = 0; i < n; ++i)
     if (!page_dst[i] || !is_device_memory(page_dst[i], h->cfg.device))
@@ -962,17 +847,16 @@ extern "C" int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page
                       h->cfg.device);
   if (!h->dev_out) CK(cudaStreamCreateWithFlags(&h->dev_out, cudaStreamNonBlocking));
   // the slot's planes: the collect has synchronised the batch's last writes (ev_post_done)
-  const uint8_t* d_res = h->d_pg_res[slot];
-  const bool crops = h->crop_ready[slot];
-  const uint8_t* d_px = crops ? h->d_crop[slot] + h->crop_px_off[slot] : nullptr;
+  const uint8_t* d_res = s.pg_res.p;
+  const uint8_t* d_px = s.crops ? s.d_crop.p + s.crop_px_off : nullptr;
   for (int i = 0; i < n; ++i) {
     const ctd_page_entry& e = pg[size_t(i)];
     const size_t px = size_t(e.ih) * size_t(e.iw);
     uint8_t* dst = static_cast<uint8_t*>(page_dst[i]);
     CK(cudaMemcpyAsync(dst, d_res + e.mask_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
     CK(cudaMemcpyAsync(dst + px, d_res + e.refined_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
-    if (crops) {
-      const size_t b0 = h->crop_base[slot][size_t(i)], b1 = h->crop_base[slot][size_t(i) + 1];
+    if (s.crops) {
+      const size_t b0 = s.crop_base[size_t(i)], b1 = s.crop_base[size_t(i) + 1];
       if (b1 > b0) CK(cudaMemcpyAsync(dst + 2 * px, d_px + b0, b1 - b0, cudaMemcpyDeviceToDevice, h->dev_out));
     }
   }
@@ -983,20 +867,22 @@ extern "C" int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page
 extern "C" int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region** plan, int32_t* n_regions,
                                    const int32_t** page_first, const uint8_t** pixels, size_t* bytes) {
   if (!h || slot < 0 || slot > 1 || !plan || !n_regions || !page_first || !pixels || !bytes) return CTD_E_INVALID;
-  if (h->slot_busy[slot] || !h->crop_ready[slot])
+  const Slot& s = h->slot[slot];
+  if (s.busy || !s.collected || !s.crops)
     return ctd_fail(h, CTD_E_INVALID, "slot %d holds no collected ctd_submit_pages_regions batch", slot);
-  *plan = h->crop_plan[slot].data();
-  *n_regions = int32_t(h->crop_plan[slot].size());
-  *page_first = h->crop_first[slot].data();
-  *bytes = h->crop_bytes[slot];
-  *pixels = h->crop_bytes[slot] && !h->dev_ready[slot] ? h->h_crop[slot] + h->crop_px_off[slot] : nullptr;
+  *plan = s.crop_plan.data();
+  *n_regions = int32_t(s.crop_plan.size());
+  *page_first = s.crop_first.data();
+  *bytes = s.crop_bytes;
+  *pixels = s.crop_bytes && !s.on_device ? s.h_crop.p + s.crop_px_off : nullptr;
   return CTD_OK;
 }
 
 extern "C" int ctd_device_arena(ctd_handle* h, int32_t slot, void** base, void** post_stream) {
   if (!h || slot < 0 || slot > 1 || !base) return CTD_E_INVALID;
-  if (!h->d_stage_out[slot]) return ctd_fail(h, CTD_E_INVALID, "no pipelined submission has been made on this handle");
-  *base = h->d_stage_out[slot];
+  if (!h->slot[slot].d_stage_out)
+    return ctd_fail(h, CTD_E_INVALID, "no pipelined submission has been made on this handle");
+  *base = h->slot[slot].d_stage_out;
   if (post_stream) *post_stream = h->post;
   return CTD_OK;
 }
@@ -1015,8 +901,8 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   if (int rc = prepare_forward(h, 1, net_h, net_w, &sp)) return rc;
   const size_t px = size_t(ih) * iw, pxa = (px + 255) / 256 * 256;
   // io scratch: page (3 px) | page-sized mask | mask_refined | second refine output | thresholded mask
-  if (int rc = ensure_io_scratch(h, pxa * 7 + 1024)) return rc;
-  uint8_t* d_page = h->d_io_scratch;
+  if (int rc = h->io_scratch.grow(h, pxa * 7 + 1024, h->stream)) return rc;
+  uint8_t* d_page = h->io_scratch.p;
   uint8_t* d_mask = d_page + pxa * 3;
   uint8_t* d_ref = d_mask + pxa;
   uint8_t* d_ref2 = d_ref + pxa;
@@ -1031,29 +917,24 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   // mask back-projection (inference.py:164-168)
   if (same) CK(cudaMemcpyAsync(d_mask, h->d_mask_u8, px, cudaMemcpyDeviceToDevice, st));
   else CK(resize_linear_u8_launch(h->d_mask_u8, geo.unpad_h, geo.unpad_w, size_t(net_w), 1, d_mask, ih, iw, ih, iw, st));
-  std::vector<float> det(300 * 6);
-  std::vector<int16_t> lb(1000 * 8);
-  std::vector<float> ls(1000);
-  int32_t n_det = 0, n_lines = 0;
+  // the phase-A rows of the page, laid out as those of a one-page batch
+  const PagesHead hd = pages_head(1);
+  std::vector<char> rows(hd.masks);
   CK(cudaMemcpyAsync(mask_out, d_mask, px, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(det.data(), h->d_det, det.size() * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(&n_det, h->d_det_count, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(lb.data(), h->d_line_boxes, lb.size() * 2, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(ls.data(), h->d_line_scores, ls.size() * 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(&n_lines, h->d_line_count, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rows.data() + hd.det, h->d_det, 300 * 6 * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rows.data() + hd.cnt, h->d_det_count, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rows.data() + hd.lb, h->d_line_boxes, 1000 * 8 * 2, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rows.data() + hd.ls, h->d_line_scores, 1000 * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(rows.data() + hd.lc, h->d_line_count, 4, cudaMemcpyDeviceToHost, st));
   CK(cudaMemsetAsync(d_ref, 0, pxa, st));
   CK(cudaStreamSynchronize(st));
   // phase B
   const BlockSection L = block_section_layout();
   std::vector<char> section(L.stride);
-  PageIn in;
-  in.det = det.data(); in.n_det = std::min(std::max(n_det, 0), 300);
-  in.line_boxes = lb.data(); in.line_scores = ls.data(); in.n_lines = std::min(std::max(n_lines, 0), 1000);
-  in.mask = mask_out; in.im_w = iw; in.im_h = ih;
-  in.ratio_x = geo.ratio_x;
-  in.ratio_y = geo.ratio_y;
-  std::vector<int32_t> wins;
-  if (int rc = host_group_page(in, section.data(), L, wins)) return ctd_fail(h, rc, "group_output failed");
+  const std::vector<JobPage> pages{JobPage{ih, iw, geo.ratio_x, geo.ratio_y, 0, section.data()}};
+  std::vector<std::vector<int32_t>> wins(1);
+  if (int rc = host_group_page(page_in(rows.data(), hd, 0, pages[0], mask_out), section.data(), L, wins[0]))
+    return ctd_fail(h, rc, "group_output failed");
   const ctd_page_blocks* hdr = reinterpret_cast<const ctd_page_blocks*>(section.data());
   const ctd_block* rec = reinterpret_cast<const ctd_block*>(section.data() + L.rec_off);
   const int nb = hdr->n_blocks;
@@ -1066,20 +947,11 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
     memcpy(lines_out, section.data() + L.lines_off, size_t(hdr->n_lines) * 32);
     if (hdr->n_dist > 0) memcpy(dist_out, section.data() + L.dist_off, size_t(hdr->n_dist) * 8);
   }
-  // phase C
-  RefineJob rj;
-  for (int i = 0; i < nb; ++i) rj.add(wins[4 * i], wins[4 * i + 1], wins[4 * i + 2], wins[4 * i + 3], 0, iw, ih);
-  if (int rc = launch_refine(h, rj, d_page, d_mask, refine_mode, d_ref, st, &h->d_refine_scratch, &h->refine_scratch_cap,
-                             nullptr))
+  // phase C; refine_undetected_mask modifies the page mask in place and it is returned, as in the reference
+  const Planes pl{d_page, d_mask, d_ref, d_ref2, d_thr, px};
+  if (int rc = phase_c(h, pages, wins, pl, refine_mode, keep_undetected, st, h->refine_scratch, h->cc_scratch, nullptr, 0))
     return rc;
-  if (keep_undetected) {
-    // refine_undetected_mask (textmask.py:135-156); the page mask is modified in place and returned, as in the reference
-    const std::vector<UndetPage> pg{UndetPage{0, ih, iw, rec, nb}};
-    if (int rc = refine_undetected(h, pg, px, d_page, d_mask, d_ref, d_ref2, d_thr, refine_mode, st, &h->d_cc_scratch,
-                                   &h->cc_scratch_cap, &h->d_refine_scratch, &h->refine_scratch_cap, nullptr, 0))
-      return rc;
-    CK(cudaMemcpyAsync(mask_out, d_mask, px, cudaMemcpyDeviceToHost, st));
-  }
+  if (keep_undetected) CK(cudaMemcpyAsync(mask_out, d_mask, px, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(mask_refined_out, d_ref, px, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return CTD_OK;

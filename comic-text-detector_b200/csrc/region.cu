@@ -162,8 +162,8 @@ extern "C" int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t
   const size_t tb = job.table_bytes();
   const size_t rb = al256(job.regs.size() * sizeof(RegionDev));
   const size_t pb = page_on_device ? 0 : al256(size_t(ih) * iw * 3);
-  if (int rc = ensure_io_scratch(h, tb + pb + total)) return rc;
-  char* base = reinterpret_cast<char*>(h->d_io_scratch);
+  if (int rc = h->io_scratch.grow(h, tb + pb + total, h->stream)) return rc;
+  char* base = reinterpret_cast<char*>(h->io_scratch.p);
   std::vector<char> stage(tb);
   job.write_tables(stage.data());
   CK(cudaMemcpyAsync(base, stage.data(), tb, cudaMemcpyHostToDevice, h->stream));
