@@ -7,7 +7,7 @@ NVCC=${NVCC:-/usr/local/cuda/bin/nvcc}
 FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -Xcompiler -fvisibility=hidden"
 mkdir -p _obj
 pids=()
-for f in engine pipeline conv_tc simt postproc segrep refine_mk resize gather group region_plan region; do
+for f in engine pipeline conv_tc conv_ends simt postproc segrep refine_mk resize gather group region_plan region; do
   [ -f $f.cu ] || [ -f $f.cpp ] || continue
   src=$f.cu; [ -f $src ] || src=$f.cpp
   extra=""

@@ -12,7 +12,7 @@
 // Activations are 4-D TMA boxes over the NHWC buffers: out-of-bounds zero-fill IS the convolution padding, there is
 // no im2col buffer; torch.cat inputs are K-concatenated from up to 3 tensor maps; stride 2 reads four parity maps;
 // ConvTranspose 4x4 s2 p1 runs as 4 sub-pixel phases of 2x2 taps; Detect heads decode sigmoid / boxes in the epilogue.
-// The fp16 NHWC epilogue (CONV, DECONV4, stem) writes the warpgroup's tile into a swizzled staging buffer with stmatrix
+// The fp16 NHWC epilogue (CONV, DECONV4) writes the warpgroup's tile into a swizzled staging buffer with stmatrix
 // and one elected thread stores it with TMA through the destination map, so the store drains while the warpgroup
 // runs the next tile's mainloop; an in-place residual is TMA-loaded into the same buffer at the start of the tile.
 //
@@ -264,7 +264,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   int stage = 0;
   uint32_t full_par = 0;
   constexpr int R = BN / 2;
-  // fp16 NHWC destination (CONV, DECONV4, stem): the epilogue stages the warpgroup's 8*TH x BN tile in shared memory
+  // fp16 NHWC destination (CONV, DECONV4): the epilogue stages the warpgroup's 8*TH x BN tile in shared memory
   // and one elected thread stores it with TMA while the warpgroup goes on to the next tile's mainloop
   const bool nhwc16 = p.dst != nullptr && !p.split;
   const bool res16 = nhwc16 && g.residual != 0;
@@ -441,26 +441,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
         const int oy = gy[h] * g.out_mul + ph_y, ox = gx[h] * g.out_mul + ph_x;
         pix[h] = valid[h] ? size_t(img) * g.dst_h * g.dst_w + size_t(oy) * g.dst_w + ox : 0;
       }
-      if constexpr (BN == 16) {
-        if (p.seg_f32 != nullptr) {
-          // seg tail: 4 phase logits per grid pixel -> sigmoid -> one row (py2 = the column pair lane & 3) of the
-          // pixel's 2x2 block in the f32 and u8 masks
-          const int py2 = lane & 3;
-          if (py2 < 2) {
-            const size_t ow2 = size_t(g.gw) * 2;
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              if (!valid[h]) continue;
-              const size_t o = (size_t(img) * g.gh * 2 + size_t(gy[h]) * 2 + py2) * ow2 + size_t(gx[h]) * 2;
-              const float s0 = 1.0f / (1.0f + expf(-acc[m][2 * h]));
-              const float s1 = 1.0f / (1.0f + expf(-acc[m][2 * h + 1]));
-              *reinterpret_cast<float2*>(p.seg_f32 + o) = make_float2(s0, s1);
-              *reinterpret_cast<uchar2*>(p.seg_u8 + o) = make_uchar2((uint8_t)(s0 * 255.0f), (uint8_t)(s1 * 255.0f));
-            }
-          }
-          continue;
-        }
-      }
       if (p.dst == nullptr) {
         // Detect decode (yolo.py:36-44): columns = anchor*(5+nc) + o
         const int no = 5 + p.nc;
@@ -590,8 +570,8 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
   while (bn > 64 && tiles8 * (g.cout_pad / bn) <= g_num_sms / 2) bn /= 2;
   if (split && bn > 64) bn = 64;   // promoted accumulation keeps three BN/2-float fragments per thread in registers
   // 16x16 tiles (M = 256) read each weight box once per 256 pixels instead of 128.  Used for the fp16 NHWC-store ops
-  // (CONV, DECONV4) whose layer still has a tile per SM at that size; split mode, Detect and the seg tail
-  // (dst == nullptr) stay at 16x8.
+  // (CONV, DECONV4) whose layer still has a tile per SM at that size; split mode and Detect (dst == nullptr) stay at
+  // 16x8.
   int th = 8;
   if (!split && dst != nullptr &&
       g.n_img * p.tiles_x * ((g.gh + 15) / 16) * g.n_phase * (g.cout_pad / bn) >= g_num_sms)
@@ -652,47 +632,6 @@ const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& 
   }
   if (g.cout_pad > 512) return "conv_tc: cout_pad > 512 not supported (bias staging)";
   plan.smem_bytes = th == 16 ? smem_for<16>(bn) : smem_for<8>(bn);
-  return nullptr;
-}
-
-const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void* s2d, int n, int ph, int pw,
-                              const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff, int cout,
-                              int act) {
-  ConvTcParams& p = plan.p;
-  memset(&p, 0, sizeof(p));
-  ConvGeom& g = p.g;
-  const int oh = ph / 2, ow = pw / 2, pitch = ow + 4;
-  g.n_img = n; g.gh = oh; g.gw = ow; g.dst_h = oh; g.dst_w = ow; g.out_mul = 1; g.n_phase = 1;
-  g.taps = 3; g.cin_total = 64; g.k_total = 192; g.n_src = 1; g.src_c[0] = 64; g.src_cstride[0] = 16;
-  g.src_h = oh; g.src_w = ow; g.in_stride = 1;
-  for (int t = 0; t < 3; ++t) { g.tap_dy[0][t] = int8_t(t - 1); g.tap_dx[0][t] = 0; }
-  g.cout = cout; g.cout_pad = 32; g.dst_cstride = dst_cstride; g.dst_coff = dst_coff; g.act = act; g.residual = 0;
-  p.kb_elems = 64;
-  p.src_kblocks[0] = 1;
-  p.tiles_x = (ow + kTileW - 1) / kTileW;
-  p.tiles_y = (oh + 7) / 8;   // 16x8 tiles
-  p.dst = dst;
-  p.bias = bias;
-  {
-    // overlapping windows: element stride of dim 1 is ONE s2d pixel (16 channels = 32 B) while the box takes
-    // 64 contiguous channels (4 pixels); window x starts at padded pixel x = original pixel x-1
-    cuuint64_t dims[4] = {64, cuuint64_t(ow), cuuint64_t(oh), cuuint64_t(n)};
-    cuuint64_t str[3] = {32, cuuint64_t(pitch) * 32, cuuint64_t(pitch) * 32 * oh};
-    cuuint32_t box[4] = {64, kTileW, 8, 1};
-    if (const char* e = encode_map(enc, &p.a_map[0][0], s2d, 4, dims, str, box, 64)) return e;
-  }
-  plan.block_n = 32;
-  plan.tile_h = 8;
-  if (const char* e = encode_dst_maps(enc, p, dst, 32, 8)) return e;
-  {
-    cuuint64_t dims[2] = {192, 32};
-    cuuint64_t str[1] = {192 * 2};
-    cuuint32_t box[2] = {64, 32};
-    if (const char* e = encode_map(enc, &p.b_map, w16, 2, dims, str, box, 64)) return e;
-  }
-  const int total_tiles = n * p.tiles_x * p.tiles_y;
-  plan.grid = dim3(unsigned(total_tiles < g_num_sms ? total_tiles : g_num_sms), 1, 1);
-  plan.smem_bytes = TcCfg<32, 8>::kSmem;
   return nullptr;
 }
 

@@ -166,6 +166,7 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
     h->enc = reinterpret_cast<PFN_encodeTiled>(fn);
   }
   CKC(conv_tc_init());
+  CKC(conv_ends_init());
   h->blob_bytes = blob_bytes;
   CKC(cudaMalloc(&h->d_blob, blob_bytes));
   CKC(cudaMemcpy(h->d_blob, blob, blob_bytes, cudaMemcpyHostToDevice));
@@ -300,7 +301,8 @@ static void set_detect(const ctd_handle* h, size_t i, int ph, int pw, P& p) {
   for (int k = 0; k < 6; ++k) p.anchor_wh[k] = h->detect_prm[i][1 + k];
 }
 
-// Ops that run conv_tc_kernel; every other op runs on the CUDA cores.
+// Ops that run on the tensor cores (conv_tc_kernel, or the stem / seg-tail kernels); every other op runs on the CUDA
+// cores.
 static bool runs_on_tensor_cores(int precision, int kind) {
   switch (precision) {
     case CTD_PREC_SPLIT_TC: return is_gemm(kind);
@@ -312,6 +314,7 @@ static bool runs_on_tensor_cores(int precision, int kind) {
 // tensor-core launch plans of one shape: the only place that picks an op's kernel by precision
 static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
   sp.tc.resize(h->ops.size());
+  sp.ends.resize(h->ops.size());
   const bool split = h->cfg.precision == CTD_PREC_SPLIT_TC;
   for (size_t i = 0; i < h->ops.size(); ++i) {
     const ctd_op& op = h->ops[i];
@@ -319,18 +322,21 @@ static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
     const float* bias = reinterpret_cast<const float*>(h->d_blob + op.b_off);
     const char* e = nullptr;
     if (op.kind == CTD_OP_STEM) {
-      e = conv_tc_plan_stem(sp.tc[i], h->enc, h->d_buf[op.src_buf[0]], n, ph, pw, h->d_blob + op.w16_off, bias,
-                            static_cast<__half*>(h->d_buf[op.dst_buf]), h->bufs[op.dst_buf].channels, op.dst_coff,
-                            op.cout, op.act);
+      // reads the u8 pages itself: the space-to-depth form is built per tile in shared memory
+      e = conv_ends_plan_stem(sp.ends[i], h->enc, h->d_pages, n, ph, pw, h->d_blob + op.w16_off, bias,
+                              static_cast<__half*>(h->d_buf[op.dst_buf]), h->bufs[op.dst_buf].channels, op.dst_coff,
+                              op.cout, op.act);
+    } else if (op.kind == CTD_OP_SEG_TAIL) {
+      // the final ConvT 4x4 s2 (C -> 1) as a 3x3 convolution whose 4 output channels are the sub-pixel phases, with
+      // the sigmoid / u8-mask epilogue
+      if (op.cout_pad != 16) return ctd_fail(h, CTD_E_INVALID, "op %zu: seg tail needs cout_pad 16", i);
+      const ctd_bufdesc& sb = h->bufs[op.src_buf[0]];
+      e = conv_ends_plan_seg(sp.ends[i], h->enc, static_cast<const __half*>(h->d_buf[op.src_buf[0]]), sb.channels,
+                             op.src_coff[0], op.src_c[0], n, ph / sb.down, pw / sb.down, h->d_blob + op.w16_off,
+                             h->d_mask, h->d_mask_u8);
     } else {
-      // the seg tail (final ConvT 4x4 s2, C -> 1) is a 3x3 convolution whose 4 output channels are the sub-pixel
-      // phases, with the sigmoid / u8-mask epilogue
-      const bool seg = op.kind == CTD_OP_SEG_TAIL;
-      if (seg && op.cout_pad != 16) return ctd_fail(h, CTD_E_INVALID, "op %zu: seg tail needs cout_pad 16", i);
-      ctd_op gop = op;
-      if (seg) { gop.kind = CTD_OP_CONV; gop.ksize = 3; gop.stride = 1; }
       ConvGeom g;
-      if (int rc = op_geom(h, gop, n, ph, pw, g)) return rc;
+      if (int rc = op_geom(h, op, n, ph, pw, g)) return rc;
       const void* src[CTD_MAX_SRC];
       int coff[CTD_MAX_SRC];
       for (int s = 0; s < op.n_src; ++s) {
@@ -338,13 +344,9 @@ static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
         coff[s] = op.src_coff[s];
       }
       const void* w = split ? h->d_wsplit + h->wsplit_off[i] : h->d_blob + op.w16_off;
-      __half* dst = (seg || op.kind == CTD_OP_DETECT) ? nullptr : static_cast<__half*>(h->d_buf[op.dst_buf]);
-      e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, w, seg ? nullptr : bias, dst, split);
+      __half* dst = op.kind == CTD_OP_DETECT ? nullptr : static_cast<__half*>(h->d_buf[op.dst_buf]);
+      e = conv_tc_plan(sp.tc[i], h->enc, g, src, coff, w, bias, dst, split);
       if (op.kind == CTD_OP_DETECT) set_detect(h, i, ph, pw, sp.tc[i].p);
-      if (seg) {
-        sp.tc[i].p.seg_f32 = h->d_mask;
-        sp.tc[i].p.seg_u8 = h->d_mask_u8;
-      }
     }
     if (e) return ctd_fail(h, CTD_E_INVALID, "op %zu: %s", i, e);
   }
@@ -422,15 +424,9 @@ static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, const Shap
   const ctd_op& op = h->ops[i];
   const ConvTcPlan& tc = sp.tc[i];
   int rc = CTD_OK;
-  if (tc.block_n) {
-    cudaError_t e = cudaSuccess;
-    if (op.kind == CTD_OP_STEM) {
-      // space-to-depth pre-pass into the padded window buffer the tensor-core stem reads
-      e = s2d_launch(h->d_pages, n, ph, pw, static_cast<__half*>(h->d_buf[op.src_buf[0]]), h->stream);
-      ++*cnt;
-    }
-    if (e == cudaSuccess) e = conv_tc_launch(tc, h->stream);
-    if (e != cudaSuccess) rc = ctd_fail(h, CTD_E_CUDA, "conv_tc op %zu: %s", i, cudaGetErrorString(e));
+  if (tc.block_n || sp.ends[i].kind != ctd::CTD_END_NONE) {
+    const cudaError_t e = tc.block_n ? conv_tc_launch(tc, h->stream) : conv_ends_launch(sp.ends[i], h->stream);
+    if (e != cudaSuccess) rc = ctd_fail(h, CTD_E_CUDA, "tensor-core op %zu: %s", i, cudaGetErrorString(e));
   } else if (is_gemm(op.kind)) {
     rc = h->elem == 4 ? run_op_simt<float>(h, i, n, ph, pw) : run_op_simt<__half>(h, i, n, ph, pw);
   } else {

@@ -22,6 +22,7 @@
 #include "kernels.h"
 
 using ctd::ConvTcPlan;
+using ctd::ConvEndsPlan;
 using ctd::NmsWorkspace;
 using ctd::PFN_encodeTiled;
 
@@ -186,7 +187,8 @@ struct RegionJob {
 };
 
 struct ShapePlan {
-  std::vector<ConvTcPlan> tc;  // index = op index; block_n == 0: the op runs on the CUDA cores
+  std::vector<ConvTcPlan> tc;  // index = op index; block_n == 0: the op does not run conv_tc_kernel
+  std::vector<ConvEndsPlan> ends;   // index = op index; kind != CTD_END_NONE: the tensor-core stem or seg tail
   cudaGraphExec_t graph = nullptr;
   int launches = 0;
 };

@@ -74,10 +74,6 @@ struct alignas(64) ConvTcParams {
   float det_stride;
   float anchor_wh[6];     // pixels
   int nc;
-  // seg-tail epilogue (BN = 16, seg_f32 != nullptr): accumulator columns 0..3 are the sub-pixel phases of the final
-  // ConvT 4x4 s2 (C -> 1) computed as a 3x3 convolution; sigmoid -> f32 mask + truncated u8 mask at (2y+py, 2x+px)
-  float* seg_f32;
-  uint8_t* seg_u8;
   // split-fp16 mode (CTD_PREC_SPLIT_TC): every fp32 operand x is carried as two fp16 planes
   // hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale); a K block issues (hi,hi) + (lo,hi) + (hi,lo) into fp32
   // accumulators, the cross terms are merged as cross * kSplitLoUnscale, and the epilogue writes FP32.  Activation
@@ -106,13 +102,43 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 // w16 holds hi rows then lo rows, dst is an FP32 NHWC buffer.
 const char* conv_tc_plan(ConvTcPlan& plan, PFN_encodeTiled enc, const ConvGeom& g, const void* const src_ptr[],
                          const int src_coff[], const void* w16, const float* bias, __half* dst, int split = 0);
-// Stem in tensor-core form: 3 filter rows x (4-pixel window x 16 channels) over the padded space-to-depth page
-// (`s2d`: [n][ph/2][pw/2 + 4][16] fp16), output [n][ph/2][pw/2][cstride] at channel offset `dst_coff`.
-const char* conv_tc_plan_stem(ConvTcPlan& plan, PFN_encodeTiled enc, const void* s2d, int n, int ph, int pw,
-                              const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff, int cout,
-                              int act);
 cudaError_t conv_tc_launch(const ConvTcPlan& plan, cudaStream_t s);
 cudaError_t conv_tc_init();  // sets max dynamic smem attributes once
+
+// ---------------------------------------------------------------------------------------
+// The network's two ends on the tensor cores (conv_ends.cu): the stem, reading the u8 pages itself, and the seg tail.
+// Each 16x16-pixel output tile loads its input region once, halo included, into shared memory.
+enum { CTD_END_NONE = 0, CTD_END_STEM = 1, CTD_END_SEG = 2 };
+struct alignas(64) ConvEndsParams {
+  CUtensorMap a_map;   // stem: u8 pages {3*pw, ph, n}; seg tail: its fp16 NHWC input {64, gw, gh, n}
+  CUtensorMap b_map;   // fp16 K-major weights: stem [32][192], seg tail [16][576]
+  CUtensorMap d_map;   // stem: fp16 NHWC destination slice {cout, gw, gh, n}
+  int n_img, gh, gw;   // output grid (seg tail: input grid; the mask is 2gh x 2gw)
+  int tiles_x, tiles_y;
+  const float* bias;   // stem: 32 floats
+  float* mask_f32;     // seg tail: [n][2gh][2gw]
+  uint8_t* mask_u8;
+};
+struct ConvEndsPlan {
+  ConvEndsParams p;
+  int kind = CTD_END_NONE;
+  dim3 grid;
+  size_t smem_bytes;
+};
+// Stem: Conv 6x6 s2 p2 (3 -> cout <= 32) + SiLU over the u8 BGR pages [n][ph][pw][3], in the space-to-depth window
+// form of the compiler's weights `w16` ([32][3 rows][4 pixels][16 channels] fp16, K = 192); output
+// [n][ph/2][pw/2][dst_cstride] fp16 at channel offset dst_coff.
+const char* conv_ends_plan_stem(ConvEndsPlan& plan, PFN_encodeTiled enc, const uint8_t* pages, int n, int ph, int pw,
+                                const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff,
+                                int cout, int act);
+// Seg tail: ConvT 4x4 s2 p1 (64 -> 1) + sigmoid as a 3x3 convolution whose 4 output channels are the sub-pixel phases
+// (weights `w16` [16][9 taps][64] fp16, rows 4..15 zero) over the fp16 NHWC input (64 channels at src_coff of a
+// src_cstride-channel buffer, gh x gw); writes the f32 and truncated-u8 masks [n][2gh][2gw].
+const char* conv_ends_plan_seg(ConvEndsPlan& plan, PFN_encodeTiled enc, const __half* src, int src_cstride,
+                               int src_coff, int src_c, int n, int gh, int gw, const void* w16, float* mask_f32,
+                               uint8_t* mask_u8);
+cudaError_t conv_ends_launch(const ConvEndsPlan& plan, cudaStream_t s);
+cudaError_t conv_ends_init();  // sets max dynamic smem attributes once
 
 // ---------------------------------------------------------------------------------------
 // CUDA-core kernels (simt.cu): accurate/bisecting path and the thin layers.  T = float | __half.
@@ -133,10 +159,6 @@ cudaError_t conv_simt_launch(const ConvSimtParams& p, cudaStream_t s);
 template <typename T>
 cudaError_t stem_launch(const uint8_t* pages, int n, int h, int w, const float* wgt /*[32][108] (ky,kx,c)*/,
                         const float* bias, T* dst, int dst_cstride, int dst_coff, int cout, int act, cudaStream_t s);
-// Pre-pass of the tensor-core stem: u8 BGR HWC page -> /255 -> space-to-depth(2) into the padded window buffer
-// dst[n][h/2][w/2 + 4][16] fp16 (see conv_tc_plan_stem): pixel x at column x + 1, channel = (dy*2+dx)*3 + c, 12..15 = 0,
-// padding columns zeroed.
-cudaError_t s2d_launch(const uint8_t* pages, int n, int h, int w, __half* dst, cudaStream_t s);
 // fp32 NHWC channel slice -> fp16 hi / lo planes (split-fp16 mode): hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale).
 // src / hi / lo point at the first channel of the slice; `cstride` elements between pixels (same in all three).
 cudaError_t split_planes_launch(const float* src, __half* hi, __half* lo, size_t npix, int c, int cstride,

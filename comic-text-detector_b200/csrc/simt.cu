@@ -295,43 +295,6 @@ __device__ __forceinline__ void stv8(float* p, const Vec8& r) {
   *reinterpret_cast<float4*>(p + 4) = make_float4(r.v[4], r.v[5], r.v[6], r.v[7]);
 }
 
-// space-to-depth stem pre-pass (one thread per output pixel: reads 2x2x3 bytes, writes 16 channels).  The tensor-core
-// stem reads 4-pixel windows from rows of w/2 + 4 pixels padded by one zero pixel on the left and three on the right.
-__global__ void s2d_kernel(const uint8_t* __restrict__ pages, int n, int h, int w, __half* __restrict__ dst) {
-  const int oh = h / 2, ow = w / 2, pitch = ow + 4;
-  const long long total = (long long)n * oh * ow;
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const int ox = int(i % ow), oy = int((i / ow) % oh), img = int(i / ((long long)ow * oh));
-  const uint8_t* p0 = pages + ((size_t(img) * h + 2 * oy) * w + 2 * ox) * 3;
-  const uint8_t* p1 = p0 + size_t(w) * 3;
-  float v[16];
-#pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    v[k] = float(p0[k]) / 255.0f;       // (dy=0,dx=0,c), (dy=0,dx=1,c)
-    v[6 + k] = float(p1[k]) / 255.0f;   // (dy=1,dx=0,c), (dy=1,dx=1,c)
-  }
-  v[12] = v[13] = v[14] = v[15] = 0.f;
-  __half* o = dst + ((size_t(img) * oh + oy) * pitch + ox + 1) * 16;
-  Vec8 a, b;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) { a.v[k] = v[k]; b.v[k] = v[8 + k]; }
-  stv8(o, a);
-  stv8(o + 8, b);
-  // keep the window padding (1 pixel left, 3 right) zero whatever this buffer held before
-  Vec8 z;
-#pragma unroll
-  for (int k = 0; k < 8; ++k) z.v[k] = 0.f;
-  if (ox == 0) { stv8(o - 16, z); stv8(o - 8, z); }
-  if (ox == ow - 1)
-    for (int q = 1; q <= 3; ++q) { stv8(o + q * 16, z); stv8(o + q * 16 + 8, z); }
-}
-cudaError_t s2d_launch(const uint8_t* pages, int n, int h, int w, __half* dst, cudaStream_t s) {
-  const long long total = (long long)n * (h / 2) * (w / 2);
-  s2d_kernel<<<unsigned((total + 255) / 256), 256, 0, s>>>(pages, n, h, w, dst);
-  return cudaGetLastError();
-}
-
 // SPPF pools: buf[..., 0:c] = x (already written); writes y1=mp5(x), y2=mp5(y1)=mp9(x), y3=mp13(x)
 // into channel slots [c,2c), [2c,3c), [3c,4c).  Chained 5x5 s1 p2 max pools equal 9x9 / 13x13 windows
 // clipped at the border (-inf padding).  One thread = one pixel x 8 channels.

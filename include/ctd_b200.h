@@ -49,7 +49,8 @@ extern "C" {
 enum ctd_op_kind {
   CTD_OP_STEM = 0,      /* 6x6 s2 p2 conv on the u8 BGR page (/255 fused), common.py:30-49 cfg L0;
                            w32_off: direct form, w16_off: 3x3 window form over the 2x2 space-to-depth page
-                           (tensor cores; src_buf[0] is its padded space-to-depth buffer)  */
+                           (tensor cores, built per tile in shared memory; src_buf[0], the 16-channel
+                           space-to-depth buffer older engines staged it in, is no longer read)  */
   CTD_OP_CONV = 1,      /* k in {1,3}, stride in {1,2}, pad k/2; K-concatenated sources     */
   CTD_OP_DECONV4 = 2,   /* ConvTranspose2d 4x4 s2 p1 (basemodel.py:26) as 4 sub-pixel phases */
   CTD_OP_AVGPOOL2 = 3,  /* AvgPool2d(2,2)                (basemodel.py:38)                  */

@@ -1,13 +1,15 @@
 #!/usr/bin/env python
-"""Per-op table of the wgmma convolutions (conv_tc_kernel) of the flagship program at one batch shape.
+"""Per-op table of the wgmma convolutions (conv_tc_kernel; the stem and seg tail: csrc/conv_ends.cu) of the flagship
+program at one batch shape.
 
     python scripts/conv_op_table.py [--batch 16 --size 1024] [--gpu] [--runs 5] [--json FILE]
 
 One row per tensor-core op (stem, CONV, DECONV4, DETECT, seg tail) of the synthetic checkpoint's program: the launch
 plan conv_tc_plan picks (N-block width BN, tile shape, tiles, tiles per persistent CTA), the algorithmic FLOPs, the
 least HBM traffic (every input read once, the weights read once, the output written once) and the operand bytes TMA
-moves from L2 into shared memory (A = activation boxes, B = weight boxes; every K block of every tap of every tile
-loads one A box and one B box).  The plan is computed here from the same rules as csrc/conv_tc.cu (132 SMs).
+moves from L2 into shared memory (A = activation boxes, B = weight boxes; in conv_tc_kernel every K block of every tap
+of every tile loads one A box and one B box, in the stem and seg-tail kernels every tile loads one halo box and every
+CTA the weights once).  The plan is computed here from the same rules as csrc/conv_tc.cu (132 SMs).
 
 With --gpu, the program also runs on cuda:0: each op's device time is the minimum over --runs un-graphed forwards
 (Engine.profile_forward, CUDA events around every op), and the row adds the achieved TFLOP/s, operand TB/s and HBM
@@ -80,45 +82,54 @@ def op_rows(prog, n, h, w, tile_h=None):
         cin = sum(src_c)
         cout, cout_pad = o["cout"], o["cout_pad"]
         if kind == cc.OP_STEM:
-            # 3 taps of 64 channels (4-pixel windows of the 2x2 space-to-depth page), BN = 32, 16x8 tiles
+            # stem_tc_kernel (csrc/conv_ends.cu): 16x16 output tiles, each loading one box of 36 page rows x 144
+            # bytes of u8 (its space-to-depth rows and their halo); the 12 KB of window weights once per CTA
             gh, gw, res = h // 2, w // 2, h // 2
-            k, stride, taps, n_phase, kb, kin = 6, 2, 3, 1, 64, 64
-            bn, th = 32, 8
+            k, stride = 6, 2
+            bn, th = 32, 16
             tiles = n * -(-gw // TILE_W) * -(-gh // th)
-            tpc = -(-tiles // min(tiles, SMS))
+            grid = min(tiles, SMS)
+            tpc = -(-tiles // grid)
             flops = 2.0 * n * gh * gw * 108 * cout
-            hbm = n * h * w * 3 + n * gh * (gw + 4) * 16 * 2 + cout_pad * 192 * 2 + n * gh * gw * cout * 2
+            hbm = n * h * w * 3 + cout_pad * 192 * 2 + n * gh * gw * cout * 2
+            a_bytes = float(tiles) * (2 * th + 4) * 144
+            b_bytes = float(grid) * cout_pad * 192 * 2
+        elif kind == cc.OP_SEG_TAIL:
+            # seg_tc_kernel (csrc/conv_ends.cu): 16x16 tiles of the 64-channel input, each loading one (16+2)^2-pixel
+            # halo box; 9 taps x the first 8 of the 16 (4 phases, zero-padded) weight rows once per CTA (m64n8 MMAs);
+            # f32 + u8 mask at twice the resolution
+            down = prog.bufs[o["src_buf"][0]][1]
+            sh, sw = h // down, w // down
+            k, stride, gh, gw, res = 4, 2, sh, sw, sh
+            bn, th = 8, 16
+            tiles = n * -(-gw // TILE_W) * -(-gh // th)
+            grid = min(tiles, SMS)
+            tpc = -(-tiles // grid)
+            flops = 2.0 * n * sh * sw * 16 * cin
+            hbm = n * sh * sw * cin * 2 + cout_pad * 9 * cin * 2 + n * 4 * sh * sw * (4 + 1)
+            a_bytes = float(tiles) * (th + 2) * (TILE_W + 2) * cin * 2
+            b_bytes = float(grid) * bn * 9 * cin * 2
         else:
             down = prog.bufs[o["src_buf"][0]][1]
             sh, sw = h // down, w // down
-            kb, kin = k_block(src_c), cin
+            kb = k_block(src_c)
             if kind == cc.OP_DECONV4:
                 k, stride, taps, n_phase, gh, gw = 4, 2, 4, 4, sh, sw
-            elif kind == cc.OP_SEG_TAIL:
-                k, stride, taps, n_phase, gh, gw = 4, 2, 9, 1, sh, sw
             else:
                 k, stride, n_phase = o["ksize"], o["stride"], 1
                 taps, gh, gw = k * k, sh // stride, sw // stride
             res = sh
-            if kind == cc.OP_SEG_TAIL:
-                bn, th = 16, 8
-                tiles = n * -(-gw // TILE_W) * -(-gh // th)
-                tpc = -(-tiles // min(tiles, SMS))
-            else:
-                bn, th, tiles, tpc = tc_plan(cout_pad, gh, gw, n, n_phase, kind != cc.OP_DETECT, tile_h)
-            if kind == cc.OP_SEG_TAIL:
-                flops = 2.0 * n * sh * sw * 16 * cin
-                out_b = n * 4 * sh * sw * (4 + 1)              # f32 + u8 mask at twice the resolution
-            elif kind == cc.OP_DECONV4:
+            bn, th, tiles, tpc = tc_plan(cout_pad, gh, gw, n, n_phase, kind != cc.OP_DETECT, tile_h)
+            if kind == cc.OP_DECONV4:
                 flops = 2.0 * n * sh * sw * 16 * cin * cout
                 out_b = n * 4 * sh * sw * cout * 2
             else:
                 flops = 2.0 * n * gh * gw * taps * cin * cout
                 out_b = n * gh * gw * cout * (4 if kind == cc.OP_DETECT else 2) * (2 if o["residual"] else 1)
             hbm = n * sh * sw * cin * 2 + n_phase * cout_pad * taps * cin * 2 + out_b
-        its = taps * (kin // kb)                                  # K iterations of a tile
-        a_bytes = float(tiles) * its * th * TILE_W * kb * 2
-        b_bytes = float(tiles) * its * bn * kb * 2
+            its = taps * (cin // kb)                              # K iterations of a tile
+            a_bytes = float(tiles) * its * th * TILE_W * kb * 2
+            b_bytes = float(tiles) * its * bn * kb * 2
         rows.append(dict(op=i, kind=KIND[kind], k=k, stride=stride, res=res, cin=cin, cout=cout, bn=bn,
                          tile="16x%d" % th, tiles=tiles, tiles_per_cta=tpc, gflop=flops / 1e9, hbm_gb=hbm / 1e9,
                          a_gb=a_bytes / 1e9, b_gb=b_bytes / 1e9))
