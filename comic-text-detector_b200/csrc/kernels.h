@@ -257,8 +257,14 @@ struct RefineWin {
 // segments (rows = 1, x0 a multiple of kRefineChunkPx).
 struct RefineChunk { int win, y0, x0, rows; };
 constexpr int kRefineChunkPx = 8192;
-// scratch planes for `total_px` window pixels (the sum of the window areas, each rounded up to 4)
-size_t refine_scratch_bytes(size_t total_px);
+// Rows per chunk of a window of width rw <= kRefineChunkPx: as many whole rows as fit, a multiple of 4 from 8 rows up
+// (chunk starts 4-byte aligned in the window planes).  The host cuts the windows with it (RefineJob::add) and the
+// labelling finds the chunk of a neighbouring pixel with it (refine_mk.cu).
+__host__ __device__ constexpr int refine_rows_per_chunk(int rw) {
+  return kRefineChunkPx / rw >= 8 ? (kRefineChunkPx / rw) & ~3 : (kRefineChunkPx / rw > 0 ? kRefineChunkPx / rw : 1);
+}
+// scratch planes for `total_px` window pixels (the sum of the window areas, each rounded up to 4) cut into n_chunks
+size_t refine_scratch_bytes(size_t total_px, size_t n_chunks);
 // d_state: refine_mk_state_bytes(n_wins) bytes of per-window state
 size_t refine_mk_state_bytes(int n_wins);
 // the first n_multi_chunks records of d_chunks are the chunks of windows that span more than one chunk.  The pages

@@ -55,8 +55,7 @@ void RefineJob::add(int x1, int y1, int x2, int y2, size_t page_off, int iw, int
   const int wi = int(wins.size());
   const int rw = x2 - x1, rh = y2 - y1;
   // whole rows per chunk, or one row segment of <= kRefineChunkPx pixels per chunk when a row is longer
-  int rows_per = std::max(1, kRefineChunkPx / rw);
-  if (rows_per >= 8) rows_per &= ~3;   // chunk starts on multiples of 4 rows -> 4-byte aligned in the window planes
+  const int rows_per = refine_rows_per_chunk(rw);
   for (int y0 = 0; y0 < rh; y0 += rows_per)
     for (int x0 = 0; x0 < rw; x0 += kRefineChunkPx) chunks.push_back(RefineChunk{wi, y0, x0, std::min(rows_per, rh - y0)});
   wins.push_back(RefineWin{x1, y1, x2, y2, (long long)total_px, (long long)page_off, iw});
@@ -78,7 +77,7 @@ int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, con
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t tb = job.table_bytes();   // a multiple of 256
   const size_t sb = refine_mk_state_bytes(int(job.wins.size()));
-  if (int rc = scratch.grow(h, tb + sb + refine_scratch_bytes(job.total_px), st, 2)) return rc;
+  if (int rc = scratch.grow(h, tb + sb + refine_scratch_bytes(job.total_px, job.chunks.size()), st, 2)) return rc;
   char* base = reinterpret_cast<char*>(scratch.p);
   const size_t wb = al(job.wins.size() * sizeof(RefineWin));
   std::vector<char> local;

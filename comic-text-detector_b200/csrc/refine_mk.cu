@@ -46,10 +46,15 @@ struct Ctx {
   WinState* st;
   int mode;
   // planes (window-pixel indexed)
-  int* L;
+  uint16_t* lab;     // chunk-local root of every pixel, as an offset in its chunk; kNoLabel = background
+  uint16_t* roots;   // chunk-local roots of each chunk (offsets), at the chunk's own pixel range; nroots[chunk] of them
+  int* nroots;       // per chunk
+  int* P;            // union-find parents of the chunk-local roots (only root entries are ever touched)
   int* acc;
   uint8_t *grey, *predm, *merged, *tmp;
 };
+constexpr uint16_t kNoLabel = 0xffffu;
+static_assert(kChunkPx <= 0xffff, "a chunk-local offset fits 16 bits below kNoLabel");
 
 // A chunk's pixels are contiguous in the window planes: chunk pixel k is window pixel i0 + k, at window row
 // y0 + k / cols and column x0 + k % cols.  A chunk is one row (rows == 1) or whole rows (x0 == 0, cols == rw).
@@ -79,7 +84,16 @@ __device__ __forceinline__ View view_of(const Ctx& c, int chunk) {
   return v;
 }
 
-// ---- union-find on a window's L plane (other CTAs update it: parent reads bypass L1) -------------------------------
+// Window pixel index of the first pixel of the chunk that holds window pixel (y, x): the host's cut (RefineJob::add,
+// pipeline.cu) into whole rows per chunk, or row segments of kChunkPx pixels when a row is longer.
+__device__ __forceinline__ int chunk_start(int y, int x, int rw) {
+  if (rw > kChunkPx) return y * rw + (x & ~(kChunkPx - 1));
+  const int rows_per = refine_rows_per_chunk(rw);
+  return (y / rows_per) * rows_per * rw;
+}
+static_assert((kChunkPx & (kChunkPx - 1)) == 0, "row segments start on multiples of kChunkPx");
+
+// ---- union-find over a window's chunk-local roots (other CTAs update it: parent reads bypass L1) ---------------------
 __device__ __forceinline__ int uf_find(const int* L, int a) {
   int p = __ldcg(L + a);
   while (p != a) {
@@ -471,11 +485,12 @@ __global__ void k_decide2(Ctx c, int n_wins) {
 
 // ---- labelling of a source plane: candidate `round` (0..3) or, round == 4, the inverse of `merged` (hole filling) -----
 // Level 1, one CTA per chunk (<= kChunkPx pixels), everything in SHARED memory: source pixels (coalesced), run starts by
-// warp ballot, seams between warps and the contacts between the rows of the chunk united in a shared union-find, one
-// root per chunk-local component written to L (tmp = 1 marks those roots: they are the chain nodes of the global
-// forest).  Level 2: only the first row of every chunk issues global unions with the row above it, and the first pixel
-// of a row segment with the last pixel of the segment to its left.  Level 3: compress from the chain nodes, then every
-// pixel takes its (chunk-local) parent's root.
+// warp ballot, seams between warps and the contacts between the rows of the chunk united in a shared union-find; every
+// pixel's chunk-local root goes to the 16-bit `lab` plane as an offset in its chunk, and the chunk's roots (the nodes of
+// the global forest P, which only ever touches root entries) to the chunk's root list.  Level 2: only the first row of
+// every chunk issues global unions with the row above it, and the first pixel of a row segment with the last pixel of
+// the segment to its left.  Level 3: compress from the roots of the list; a pixel's global root is then
+// P[chunk start + lab].
 // In the chunk-local passes a chunk pixel k is treated as at column k % rw of row k / rw: right for whole rows, and for
 // a row segment (k < cnt <= kChunkPx < rw) one row whose first pixel starts a run and which has no row above.
 constexpr int kLabelThreads = 512;
@@ -525,15 +540,16 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
   __shared__ unsigned Sw[kChunkPx / 32];          // run-start bits (the only nodes of the chunk-local forest)
   __shared__ unsigned Gw[kChunkPx / 32];          // foreground & not yet merged & predicted     ("gain" pixels)
   __shared__ unsigned Bw[kChunkPx / 32];          // foreground & not yet merged & not predicted ("loss" pixels)
-  __shared__ int s_fg;
+  __shared__ int s_fg, s_nroot;
   const View v = view_of(c, blockIdx.x);
   WinState& st = c.st[v.w];
   if (round < 4 && round >= st.nproc) return;
   for (int i = threadIdx.x; i < kChunkPx / 32 + 2; i += kLabelThreads) Mw[i] = 0u;
-  if (threadIdx.x == 0) s_fg = 0;
+  if (threadIdx.x == 0) { s_fg = 0; s_nroot = 0; }
   __syncthreads();
-  uint8_t* rootflag = c.tmp + v.win.off;
-  int* L = c.L + v.win.off;
+  uint16_t* lab = c.lab + v.win.off + v.i0;
+  uint16_t* roots = c.roots + v.win.off + v.i0;
+  int* P = c.P + v.win.off;
   int* acc = c.acc + 4 * v.win.off;
   const int n = v.rw * v.rh;
   int* area = acc; int* gain = acc + n; int* loss = acc + 2 * n; int* maxi = acc + 3 * n;
@@ -739,7 +755,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
   // pass 3a: flatten the forest.  Its nodes are the run starts only (every other foreground pixel points at its run
   // start and is never re-parented): after this pass every run start points straight at its root, so the root of ANY
   // foreground pixel is Ls[Ls[k]] -- two loads instead of a walk (the walks were 10 hops on average, ncu).  The roots
-  // zero their per-label sums here (area, gain, loss, max pixel index).
+  // zero their per-label sums here (area, gain, loss, max pixel index), start their tree of P and join the root list.
   int fgc = 0;
   for (int hw = threadIdx.x; hw * 16 < v.cnt; hw += kLabelThreads) {
     const unsigned half = (hw & 1) ? 0xffff0000u : 0x0000ffffu;
@@ -755,6 +771,8 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
       } else {
         const int gi = v.i0 + s0;
         area[gi] = 0; gain[gi] = 0; loss[gi] = 0; maxi[gi] = -1;
+        P[gi] = gi;
+        roots[atomicAdd(&s_nroot, 1)] = uint16_t(s0);
       }
     }
   }
@@ -763,16 +781,14 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     if (lane == 0 && fgc) atomicAdd(&s_fg, fgc);
   }
   __syncthreads();
-  if (round == 4 && threadIdx.x == 0) {
+  if (threadIdx.x == 0) {
+    c.nroots[blockIdx.x] = s_nroot;
     const int a0 = v.cnt - s_fg;
-    if (a0) atomicAdd(&st.area0, a0);
+    if (round == 4 && a0) atomicAdd(&st.area0, a0);
   }
-  // pass 3b: chunk-local root of every pixel to global memory (window-local pixel indices; -1 = background)
-  for (int k = threadIdx.x; k < v.cnt; k += kLabelThreads) {
-    const int r = ((Mw[k >> 5] >> (k & 31)) & 1u) ? Ls[start_of(k)] : -1;
-    L[v.i0 + k] = r < 0 ? -1 : v.i0 + r;
-    rootflag[v.i0 + k] = (r == k) ? 1 : 0;
-  }
+  // pass 3b: chunk-local root of every pixel to global memory (an offset in the chunk; kNoLabel = background)
+  for (int k = threadIdx.x; k < v.cnt; k += kLabelThreads)
+    lab[k] = ((Mw[k >> 5] >> (k & 31)) & 1u) ? uint16_t(Ls[start_of(k)]) : kNoLabel;
   // pass 3c: per-label sums, one update per RUN (popcounts of the run's bits in the foreground / gain / loss masks) into
   // the sums of its chunk-local root.  k_flat1 adds the sums of the chunk roots of a multi-chunk window to their global
   // root; there is no per-pixel accumulation sweep any more.
@@ -805,54 +821,50 @@ __global__ void __launch_bounds__(kBorderThreads) k_union_border(Ctx c, int roun
   const View v = view_of(c, blockIdx.x);
   if (round < 4 && round >= c.st[v.w].nproc) return;
   if (v.i0 == 0) return;      // the window's first chunk
-  int* L = c.L + v.win.off;   // foreground <=> L >= 0 (written for every pixel by k_label_local)
-  if (v.x0 > 0 && threadIdx.x == 0 && __ldcg(L + v.i0) >= 0 && __ldcg(L + v.i0 - 1) >= 0) uf_union(L, v.i0, v.i0 - 1);
-  if (v.y0 == 0) return;
+  const uint16_t* lab = c.lab + v.win.off;   // foreground <=> lab != kNoLabel (written for every pixel by k_label_local)
+  int* P = c.P + v.win.off;
+  // chunk-local root of the foreground pixel at window row y, column x, as a window pixel index
+  auto root_at = [&](int y, int x) { const int i = y * v.rw + x; return chunk_start(y, x, v.rw) + lab[i]; };
+  const int y = v.y0;
+  if (v.x0 > 0 && threadIdx.x == 0 && lab[v.i0] != kNoLabel && lab[v.i0 - 1] != kNoLabel)
+    uf_union(P, v.i0 + lab[v.i0], root_at(y, v.x0 - 1));
+  if (y == 0) return;
   for (int k = threadIdx.x; k < v.cols; k += int(blockDim.x)) {
     const int i = v.i0 + k, x = v.x0 + k;
-    if (__ldcg(L + i) < 0) continue;
+    if (lab[i] == kNoLabel) continue;
     const int up = i - v.rw;
-    if (__ldcg(L + up) >= 0) {
+    const int r = v.i0 + lab[i];
+    if (lab[up] != kNoLabel) {
       // only the first pixel of each (run x run above) overlap: the pixels left of it are united with it (in the chunk
       // or across the segment seam) and so are the ones above
-      const bool first = x == 0 || __ldcg(L + i - 1) < 0 || __ldcg(L + up - 1) < 0;
-      if (first) uf_union(L, i, up);
+      const bool first = x == 0 || lab[i - 1] == kNoLabel || lab[up - 1] == kNoLabel;
+      if (first) uf_union(P, r, root_at(y - 1, x));
     } else {
-      if (x > 0 && __ldcg(L + up - 1) >= 0) uf_union(L, i, up - 1);
-      if (x + 1 < v.rw && __ldcg(L + up + 1) >= 0) uf_union(L, i, up + 1);
+      if (x > 0 && lab[up - 1] != kNoLabel) uf_union(P, r, root_at(y - 1, x - 1));
+      if (x + 1 < v.rw && lab[up + 1] != kNoLabel) uf_union(P, r, root_at(y - 1, x + 1));
     }
   }
 }
-// level 3a: compress from the chain nodes (chunk-local roots); 3b: every pixel takes its parent's root
+// level 3: every chunk-local root of the chunk's list points straight at its global root
 __global__ void __launch_bounds__(kThreads) k_flat1(Ctx c, int round) {
   const View v = view_of(c, blockIdx.x);
   if (round < 4 && round >= c.st[v.w].nproc) return;
-  const uint8_t* rootflag = c.tmp + v.win.off;
-  int* L = c.L + v.win.off;
+  const uint16_t* roots = c.roots + v.win.off + v.i0;
+  const int nr = c.nroots[blockIdx.x];
+  int* P = c.P + v.win.off;
   int* acc = c.acc + 4 * v.win.off;
   const int n = v.rw * v.rh;
   int* area = acc; int* gain = acc + n; int* loss = acc + 2 * n; int* maxi = acc + 3 * n;
-  constexpr int U = 8;
-  for (int k0 = 0; k0 < v.cnt; k0 += kThreads * U) {
-    uint8_t rf[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int k = k0 + u * kThreads + threadIdx.x;
-      rf[u] = k < v.cnt ? rootflag[v.i0 + k] : 0;
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (!rf[u]) continue;
-      // chunk-local root: point it straight at its global root and hand its sums (complete since k_label_local) over
-      const int cr = v.i0 + k0 + u * kThreads + threadIdx.x;
-      const int g = uf_find_compress(L, cr);
-      if (g != cr) {
-        atomicAdd(&area[g], area[cr]);
-        atomicMax(&maxi[g], maxi[cr]);
-        const int g_ = gain[cr], l_ = loss[cr];
-        if (g_) atomicAdd(&gain[g], g_);
-        if (l_) atomicAdd(&loss[g], l_);
-      }
+  for (int j = threadIdx.x; j < nr; j += kThreads) {
+    // chunk-local root: point it straight at its global root and hand its sums (complete since k_label_local) over
+    const int cr = v.i0 + roots[j];
+    const int g = uf_find_compress(P, cr);
+    if (g != cr) {
+      atomicAdd(&area[g], area[cr]);
+      atomicMax(&maxi[g], maxi[cr]);
+      const int g_ = gain[cr], l_ = loss[cr];
+      if (g_) atomicAdd(&gain[g], g_);
+      if (l_) atomicAdd(&loss[g], l_);
     }
   }
 }
@@ -861,23 +873,14 @@ __global__ void __launch_bounds__(kThreads) k_flat1(Ctx c, int round) {
 __global__ void __launch_bounds__(kThreads) k_top_a(Ctx c) {
   const View v = view_of(c, blockIdx.x);
   WinState& st = c.st[v.w];
-  const int* L = c.L + v.win.off;
+  const int* P = c.P + v.win.off;
   const int* area = c.acc + 4 * v.win.off;
-  const uint8_t* rootflag = c.tmp + v.win.off;
+  const uint16_t* roots = c.roots + v.win.off + v.i0;   // chunk-local roots: the only candidates for a global root
+  const int nr = c.nroots[blockIdx.x];
   int m = -1;
-  constexpr int U = 8;
-  for (int k0 = 0; k0 < v.cnt; k0 += kThreads * U) {
-    uint8_t rf[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int k = k0 + u * kThreads + threadIdx.x;
-      rf[u] = k < v.cnt ? rootflag[v.i0 + k] : 0;     // chunk-local roots: the only candidates for a global root
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int i = v.i0 + k0 + u * kThreads + threadIdx.x;
-      if (rf[u] && L[i] == i) m = max(m, area[i]);
-    }
+  for (int j = threadIdx.x; j < nr; j += kThreads) {
+    const int i = v.i0 + roots[j];
+    if (P[i] == i) m = max(m, area[i]);
   }
   if (v.i0 == 0 && threadIdx.x == 0) m = max(m, st.area0);   // once per window: its first chunk
   for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_down_sync(0xffffffffu, m, o));
@@ -886,25 +889,16 @@ __global__ void __launch_bounds__(kThreads) k_top_a(Ctx c) {
 __global__ void __launch_bounds__(kThreads) k_top_b(Ctx c) {
   const View v = view_of(c, blockIdx.x);
   WinState& st = c.st[v.w];
-  const int* L = c.L + v.win.off;
+  const int* P = c.P + v.win.off;
   const int* area = c.acc + 4 * v.win.off;
-  const uint8_t* rootflag = c.tmp + v.win.off;
+  const uint16_t* roots = c.roots + v.win.off + v.i0;
+  const int nr = c.nroots[blockIdx.x];
   const int m1 = st.max1;
   int m2 = -1, c1 = 0;
   auto push = [&](int a) { if (a == m1) ++c1; else m2 = max(m2, a); };
-  constexpr int U = 8;
-  for (int k0 = 0; k0 < v.cnt; k0 += kThreads * U) {
-    uint8_t rf[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int k = k0 + u * kThreads + threadIdx.x;
-      rf[u] = k < v.cnt ? rootflag[v.i0 + k] : 0;
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int i = v.i0 + k0 + u * kThreads + threadIdx.x;
-      if (rf[u] && L[i] == i) push(area[i]);
-    }
+  for (int j = threadIdx.x; j < nr; j += kThreads) {
+    const int i = v.i0 + roots[j];
+    if (P[i] == i) push(area[i]);
   }
   if (v.i0 == 0 && threadIdx.x == 0) push(st.area0);
   for (int o = 16; o > 0; o >>= 1) {
@@ -920,7 +914,8 @@ __global__ void __launch_bounds__(kThreads) k_mapply(Ctx c, int round) {
   const View v = view_of(c, blockIdx.x);
   const WinState& st = c.st[v.w];
   if (round < 4 && round >= st.nproc) return;
-  const int* L = c.L + v.win.off;
+  const uint16_t* lab = c.lab + v.win.off + v.i0;
+  const int* P = c.P + v.win.off;
   uint8_t* merged = c.merged + v.win.off;
   const int* acc = c.acc + 4 * v.win.off;
   const int n = v.rw * v.rh;
@@ -928,35 +923,44 @@ __global__ void __launch_bounds__(kThreads) k_mapply(Ctx c, int round) {
   // sorted_area[-2] if more than one label else sorted_area[-1] (textmask.py:114-118); label 0 always exists
   const int second = st.cnt1 >= 2 ? st.max1 : st.max2;
   const int thresh = second >= 0 ? second : st.max1;
-  for (int k0 = 0; k0 < v.cnt; k0 += kThreads * kU) {
-    int r[kU], a[kU], g[kU], l[kU], mx[kU];
-#pragma unroll
-    for (int u = 0; u < kU; ++u) {
-      const int k = k0 + u * kThreads + threadIdx.x;
-      r[u] = k < v.cnt ? L[v.i0 + k] : -1;      // chunk-local root of the pixel ...
+  // the merge decision of every chunk-local root, from the sums of its global root (P[cr]: k_flat1, or cr itself in a
+  // single-chunk window), into shared memory at the root's chunk offset: the pixels then read one label and one
+  // shared byte instead of a parent and four sums each
+  __shared__ uint8_t dec[kChunkPx];
+  const uint16_t* roots = c.roots + v.win.off + v.i0;
+  const int nr = c.nroots[blockIdx.x];
+  for (int j = threadIdx.x; j < nr; j += kThreads) {
+    const int cl = roots[j];
+    const int g = P[v.i0 + cl];
+    const int a = area[g];
+    bool ok;
+    if (round < 4) {
+      // `if w * h < 3: continue` (textmask.py:97): bounding boxes 1x1, 1x2, 2x1
+      const int mx = maxi[g];
+      ok = !(a == 1 || (a == 2 && (mx == g + 1 || mx == g + v.rw)));
+    } else {
+      ok = a < thresh;  // textmask.py:120
     }
-#pragma unroll
-    for (int u = 0; u < kU; ++u)
-      if (r[u] >= 0) r[u] = L[r[u]];             // ... which points straight at the global root (k_flat1)
-#pragma unroll
-    for (int u = 0; u < kU; ++u) {
-      a[u] = 0; g[u] = 0; l[u] = 0; mx[u] = 0;
-      if (r[u] >= 0) { a[u] = area[r[u]]; g[u] = gain[r[u]]; l[u] = loss[r[u]]; if (round < 4) mx[u] = maxi[r[u]]; }
-    }
-#pragma unroll
-    for (int u = 0; u < kU; ++u) {
-      if (r[u] < 0) continue;
-      bool ok;
-      if (round < 4) {
-        // `if w * h < 3: continue` (textmask.py:97): bounding boxes 1x1, 1x2, 2x1
-        const bool tiny = a[u] == 1 || (a[u] == 2 && (mx[u] == r[u] + 1 || mx[u] == r[u] + v.rw));
-        ok = !tiny;
-      } else {
-        ok = a[u] < thresh;  // textmask.py:120
-      }
-      if (ok && g[u] > l[u]) merged[v.i0 + k0 + u * kThreads + threadIdx.x] = 255;
-    }
+    dec[cl] = ok && gain[g] > loss[g];
   }
+  __syncthreads();
+  auto merges = [&](unsigned l) { return l != kNoLabel && dec[l]; };
+  int k_tail = 0;
+  if (v.aligned) {
+    // four labels per 8-byte load (lab + i0 is 8-byte aligned), and one 4-byte OR into `merged` where any merges
+    const uint2* lab4 = reinterpret_cast<const uint2*>(lab);
+    uint32_t* mg32 = reinterpret_cast<uint32_t*>(merged + v.i0);
+    const int n4 = v.cnt >> 2;
+    for (int q = threadIdx.x; q < n4; q += kThreads) {
+      const uint2 l4 = lab4[q];
+      const unsigned m = (merges(l4.x & 0xffffu) ? 0xffu : 0u) | (merges(l4.x >> 16) ? 0xff00u : 0u) |
+                         (merges(l4.y & 0xffffu) ? 0xff0000u : 0u) | (merges(l4.y >> 16) ? 0xff000000u : 0u);
+      if (m) mg32[q] |= m;
+    }
+    k_tail = n4 << 2;
+  }
+  for (int k = k_tail + threadIdx.x; k < v.cnt; k += kThreads)
+    if (merges(lab[k])) merged[v.i0 + k] = 255;
 }
 
 // ---- dilate 3x3 (inpaint mode): merged -> tmp; the caller swaps the two planes afterwards -----------------------------
@@ -1026,11 +1030,14 @@ __global__ void __launch_bounds__(kThreads) k_or(Ctx c) {
 }  // namespace
 
 size_t refine_mk_state_bytes(int n_wins) { return (size_t(n_wins) * sizeof(WinState) + 255) / 256 * 256; }
-// L (4 B), per-root sums (16 B), grey, predm, merged, tmp (1 B each) per window pixel
-size_t refine_scratch_bytes(size_t total_px) { return total_px * (4 + 16 + 4) + 4096; }
+// per window pixel: P (4 B) and the per-root sums (16 B), of which only root entries are touched; lab and the root
+// lists (2 B each); grey, predm, merged, tmp (1 B each).  Per chunk: its root count.
+size_t refine_scratch_bytes(size_t total_px, size_t n_chunks) {
+  return total_px * (4 + 16 + 2 + 2 + 4) + n_chunks * 4 + 4096;
+}
 
 // d_wins: n_wins windows; d_chunks: n_chunks chunks (RefineChunk, kernels.h); d_state: refine_mk_state_bytes(n_wins)
-// bytes (zeroed here); scratch: refine_scratch_bytes(total_px) bytes.  img / mask / out hold the pages' planes at the
+// bytes (zeroed here); scratch: refine_scratch_bytes(total_px, n_chunks) bytes.  img / mask / out hold the pages' planes at the
 // windows' page_off (3 bytes per pixel in img).
 cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const RefineWin* d_wins, int n_wins,
                              const RefineChunk* d_chunks, int n_chunks, int n_multi_chunks, void* d_state, size_t total_px,
@@ -1043,8 +1050,11 @@ cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const 
   c.st = static_cast<WinState*>(d_state);
   c.mode = refine_mode;
   char* p = static_cast<char*>(scratch);
-  c.L = reinterpret_cast<int*>(p); p += total_px * 4;
+  c.P = reinterpret_cast<int*>(p); p += total_px * 4;
   c.acc = reinterpret_cast<int*>(p); p += total_px * 16;
+  c.lab = reinterpret_cast<uint16_t*>(p); p += total_px * 2;
+  c.roots = reinterpret_cast<uint16_t*>(p); p += total_px * 2;
+  c.nroots = reinterpret_cast<int*>(p); p += size_t(n_chunks) * 4;
   c.grey = reinterpret_cast<uint8_t*>(p); p += total_px;
   c.predm = reinterpret_cast<uint8_t*>(p); p += total_px;
   c.merged = reinterpret_cast<uint8_t*>(p); p += total_px;
