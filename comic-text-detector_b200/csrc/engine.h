@@ -169,6 +169,7 @@ struct RefineJob {
   std::vector<ctd::RefineWin> wins;
   std::vector<ctd::RefineChunk> chunks;
   size_t total_px = 0;
+  size_t total_words = 0;   // bit-plane words handed to the chunks so far (RefineChunk::woff)
   // window of the iw x ih page whose planes start at pixel page_off; python slice semantics; empty windows dropped
   void add(int x1, int y1, int x2, int y2, size_t page_off, int iw, int ih);
   size_t table_bytes() const;

@@ -254,8 +254,10 @@ struct RefineWin {
 };
 // Pixels [i0, i0 + rows * cols) of the window planes, i0 = y0 * rw + x0, cols = min(rw - x0, kRefineChunkPx).  A
 // window of width rw <= kRefineChunkPx is cut into chunks of whole rows (x0 = 0, cols = rw); a wider window into row
-// segments (rows = 1, x0 a multiple of kRefineChunkPx).
-struct RefineChunk { int win, y0, x0, rows; };
+// segments (rows = 1, x0 a multiple of kRefineChunkPx).  In the 1-bit planes (32 pixels per word) every chunk has its
+// own run of ceil(rows * cols / 32) words from word `woff`: bit j of word w is chunk pixel 32 * w + j.  The chunks of
+// a window are consecutive in the table, row by row.
+struct RefineChunk { int win, y0, x0, rows, woff; };
 constexpr int kRefineChunkPx = 8192;
 // Rows per chunk of a window of width rw <= kRefineChunkPx: as many whole rows as fit, a multiple of 4 from 8 rows up
 // (chunk starts 4-byte aligned in the window planes).  The host cuts the windows with it (RefineJob::add) and the
@@ -263,7 +265,8 @@ constexpr int kRefineChunkPx = 8192;
 __host__ __device__ constexpr int refine_rows_per_chunk(int rw) {
   return kRefineChunkPx / rw >= 8 ? (kRefineChunkPx / rw) & ~3 : (kRefineChunkPx / rw > 0 ? kRefineChunkPx / rw : 1);
 }
-// scratch planes for `total_px` window pixels (the sum of the window areas, each rounded up to 4) cut into n_chunks
+// scratch planes for `total_px` window pixels (the sum of the window areas, each rounded up to 4) cut into n_chunks,
+// whose bit-plane runs end at or below word total_px / 32 + n_chunks
 size_t refine_scratch_bytes(size_t total_px, size_t n_chunks);
 // d_state: refine_mk_state_bytes(n_wins) bytes of per-window state
 size_t refine_mk_state_bytes(int n_wins);

@@ -57,7 +57,11 @@ void RefineJob::add(int x1, int y1, int x2, int y2, size_t page_off, int iw, int
   // whole rows per chunk, or one row segment of <= kRefineChunkPx pixels per chunk when a row is longer
   const int rows_per = refine_rows_per_chunk(rw);
   for (int y0 = 0; y0 < rh; y0 += rows_per)
-    for (int x0 = 0; x0 < rw; x0 += kRefineChunkPx) chunks.push_back(RefineChunk{wi, y0, x0, std::min(rows_per, rh - y0)});
+    for (int x0 = 0; x0 < rw; x0 += kRefineChunkPx) {
+      const int rows = std::min(rows_per, rh - y0);
+      chunks.push_back(RefineChunk{wi, y0, x0, rows, int(total_words)});
+      total_words += (size_t(rows) * std::min(rw - x0, kRefineChunkPx) + 31) / 32;
+    }
   wins.push_back(RefineWin{x1, y1, x2, y2, (long long)total_px, (long long)page_off, iw});
   total_px = (total_px + a + 3) / 4 * 4;
 }

@@ -11,10 +11,10 @@
 // in global memory; per-window scalar decisions are one-CTA-per-window kernels.  Results are bit-identical to the
 // oracle (tests/test_gpu_refine.py).
 //
-// The sweeps are instruction-issue bound, not memory bound, so the binary planes
-// are handled as BIT masks wherever a neighbourhood is involved: warp ballots pack 32 pixels per shared-memory word and one
-// thread per (half) word does the work of 16 - 32 pixels with funnel shifts, ANDs and popcounts -- the erosions of phase 0,
-// the dilation, the run contacts of the labelling and the per-label sums (one update per RUN, not per pixel).
+// The binary planes are BIT planes, 32 pixels per word, in global memory as in shared memory: the six positive
+// candidates (k_xor thresholds every pixel once), the predicted mask, `merged` and the dilation's output.  One thread per
+// (half) word does the work of 16 - 32 pixels with funnel shifts, ANDs and popcounts -- the erosions of phase 0, the
+// dilation, the run contacts of the labelling, the per-label sums and the merges (one update per RUN, not per pixel).
 #include <cuda_runtime.h>
 #include <limits.h>
 #include <math.h>
@@ -51,16 +51,21 @@ struct Ctx {
   int* nroots;       // per chunk
   int* P;            // union-find parents of the chunk-local roots (only root entries are ever touched)
   int* acc;
-  uint8_t *grey, *predm, *merged, *tmp;
+  uint8_t* grey;
+  // bit planes, each chunk's words at its RefineChunk::woff; the bits past a chunk's last pixel are zero
+  unsigned* cand;    // 6 planes of plane_words: grey in [lo, hi] of colour 0..2, then channel B, G, R > its Otsu threshold
+  unsigned *pred, *merged, *tmp;
+  size_t plane_words;
 };
 constexpr uint16_t kNoLabel = 0xffffu;
-static_assert(kChunkPx <= 0xffff, "a chunk-local offset fits 16 bits below kNoLabel");
+constexpr unsigned kMergeBit = 0x8000u;   // of a root list entry: the root's component merges (k_decide_roots)
+static_assert(kChunkPx <= int(kMergeBit), "a chunk-local offset fits the 15 bits below kMergeBit");
 
 // A chunk's pixels are contiguous in the window planes: chunk pixel k is window pixel i0 + k, at window row
 // y0 + k / cols and column x0 + k % cols.  A chunk is one row (rows == 1) or whole rows (x0 == 0, cols == rw).
 struct View {
   RefineWin win;
-  int w, rw, rh, y0, x0, rows, cols, i0, cnt, aligned;   // aligned: the chunk starts on a 4-byte boundary of the planes
+  int w, rw, rh, y0, x0, rows, cols, i0, cnt, woff;   // woff: the chunk's first word in the bit planes
   const uint8_t* img;
   const uint8_t* mask;
 };
@@ -78,7 +83,7 @@ __device__ __forceinline__ View view_of(const Ctx& c, int chunk) {
   v.cols = min(v.rw - ch.x0, kChunkPx);
   v.i0 = ch.y0 * v.rw + ch.x0;
   v.cnt = ch.rows * v.cols;
-  v.aligned = (v.i0 & 3) == 0;   // the window planes start on 4-byte boundaries
+  v.woff = ch.woff;
   v.img = c.img_all + size_t(v.win.page_off) * 3;
   v.mask = c.mask_all + size_t(v.win.page_off);
   return v;
@@ -158,7 +163,38 @@ __device__ __forceinline__ void divmod(int i, const DivW& dv, int& q, int& r) {
   }
 }
 
-// ---- phase 0: grey, pred mask (cross erosion > 60), merged = 0, histograms ------------------------------------------
+// ---- bit-plane words of a chunk -----------------------------------------------------------------------------------------
+__device__ __forceinline__ unsigned tail_mask(int w, int cnt) {   // the bits of word w that are pixels of the chunk
+  const int rem = cnt - 32 * w;
+  return rem >= 32 ? 0xffffffffu : (1u << rem) - 1u;
+}
+// of 32 consecutive pixels from column x0 of rows rw wide: the bits whose pixel is the first of its row
+__device__ __forceinline__ unsigned row_start_bits(int x0, int rw) {
+  unsigned rs = 0u;
+  for (int j = x0 == 0 ? 0 : rw - x0; j < 32; j += rw) rs |= 1u << j;
+  return rs;
+}
+// A run: consecutive foreground pixels of one row and one word.  M: foreground bits; S = run starts = M & (~(M << 1) | row
+// starts).  Last bit of the run that starts at bit sbit, and the bits lo..hi:
+__device__ __forceinline__ int run_end(unsigned M, unsigned S, int sbit) {
+  const unsigned stop = (~M | S) & (0xfffffffeu << sbit);          // first position after the run
+  return stop ? __ffs(stop) - 2 : 31;
+}
+__device__ __forceinline__ unsigned span_bits(int lo, int hi) {
+  return (hi == 31 ? 0xffffffffu : ((2u << hi) - 1u)) & ~((1u << lo) - 1u);
+}
+// Word d of a bit array into which the `len` bits of `src` from bit sb on are copied at bit db (0 where the word holds
+// none of them).  May read the word after the last one that holds a copied bit.
+__device__ __forceinline__ unsigned copied_word(const unsigned* src, int sb, int len, int db, int d) {
+  const int r = 32 * d - db;                      // index in the copied range of the word's bit 0
+  if (r <= -32 || r >= len) return 0u;
+  const int pos = sb + max(r, 0);
+  unsigned o = __funnelshift_r(src[pos >> 5], src[(pos >> 5) + 1], pos & 31);
+  if (len - max(r, 0) < 32) o &= (1u << (len - max(r, 0))) - 1u;
+  return r < 0 ? o << -r : o;
+}
+
+// ---- phase 0: grey, pred bits (cross erosion > 60), merged = 0, histograms ------------------------------------------
 constexpr int kU = 4;   // pixels per thread and outer iteration: the loads of all kU pixels are issued before the first use
 // Halo rectangle of a chunk: its rows plus one row above and below, its columns plus one column left and right, clipped
 // to the window.  Whole rows: <= 3 * kChunkPx pixels (the rows of a chunk, two halo rows of <= kChunkPx); a row
@@ -188,8 +224,7 @@ __device__ __forceinline__ unsigned bits_from(const unsigned* M, int pos) {   //
 // 32 pixels of a chunk starting at window column x: the bits whose pixel is the first (rs) / last (re) of its window row
 // (bits past the end of a row segment are not pixels of the chunk)
 __device__ __forceinline__ void row_ends(int x, int rw, unsigned& rs, unsigned& re) {
-  rs = 0u;
-  for (int j = x == 0 ? 0 : rw - x; j < 32; j += rw) rs |= 1u << j;
+  rs = row_start_bits(x, rw);
   int xe = x + 32;                                  // column of the pixel after the 32
   if (xe >= rw) xe %= rw;
   re = (rs >> 1) | (xe == 0 ? 0x80000000u : 0u);
@@ -201,14 +236,12 @@ __device__ __forceinline__ void row_ends(int x, int rw, unsigned& rs, unsigned& 
 __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
   __shared__ int sh[4][256];
   __shared__ unsigned N60[kExtWords], N127[kExtWords];
-  __shared__ unsigned F60[kChunkPx / 32 + 1], F127[kChunkPx / 32 + 1];
+  __shared__ unsigned F127[kChunkPx / 32 + 1];
   const View v = view_of(c, blockIdx.x);
   for (int i = threadIdx.x; i < 1024; i += kThreads) (&sh[0][0])[i] = 0;
   for (int i = threadIdx.x; i < kExtWords; i += kThreads) { N60[i] = 0u; N127[i] = 0u; }
   __syncthreads();
   uint8_t* grey = c.grey + v.win.off;
-  uint8_t* predm = c.predm + v.win.off;
-  uint8_t* merged = c.merged + v.win.off;
   const Halo hl = halo_of(v);
   const DivW dv = make_div(hl.ew, 3 * (kChunkPx + 2) + 1);
   for (int e0 = 0; e0 < hl.ext; e0 += kThreads) {
@@ -230,9 +263,11 @@ __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
     divmod(p, dv, ye, xe);
     unsigned rs, re;
     row_ends(hl.xs + xe, v.rw, rs, re);
-    // cross (textmask.py:86-89, MORPH_CROSS 3x3) on the <= 60 mask
-    F60[w] = bits_from(N60, p) | bits_from(N60, p - ew) | bits_from(N60, p + ew) | (bits_from(N60, p - 1) & ~rs) |
-             (bits_from(N60, p + 1) & ~re);
+    // cross (textmask.py:86-89, MORPH_CROSS 3x3) on the <= 60 mask: the predicted mask is the cross erosion > 60
+    const unsigned f60 = bits_from(N60, p) | bits_from(N60, p - ew) | bits_from(N60, p + ew) | (bits_from(N60, p - 1) & ~rs) |
+                         (bits_from(N60, p + 1) & ~re);
+    c.pred[v.woff + w] = ~f60 & tail_mask(w, v.cnt);
+    c.merged[v.woff + w] = 0u;
     // full 3x3 (textmask.py:60, the eroded mask of get_topk_color) on the <= 127 mask
     F127[w] = bits_from(N127, p) | bits_from(N127, p - ew) | bits_from(N127, p + ew) |
               ((bits_from(N127, p - 1) | bits_from(N127, p - ew - 1) | bits_from(N127, p + ew - 1)) & ~rs) |
@@ -263,8 +298,6 @@ __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
         const int i = v.i0 + k;
         gr = (b[u] * 1868 + g[u] * 9617 + r[u] * 4899 + 8192) >> 14;  // cv2.COLOR_BGR2GRAY, 8u fixed point
         grey[i] = (uint8_t)gr;
-        predm[i] = ((F60[k >> 5] >> (k & 31)) & 1u) ? 0 : 255;          // cross erosion > 60 (textmask.py:86-89)
-        merged[i] = 0;
         core = !((F127[k >> 5] >> (k & 31)) & 1u);                       // 3x3 erosion > 127 (textmask.py:60)
       }
       if (k0 + u * kThreads < v.cnt) {   // CTA-uniform: skip the histogram votes of iterations past the chunk
@@ -382,9 +415,11 @@ __global__ void __launch_bounds__(kDecideThreads) k_decide1(Ctx c) {
   }
 }
 
-// ---- phase 2: xor sums of every candidate and of its negative against the mask crop -----------------------------------
+// ---- phase 2: xor sums of every candidate and of its negative against the mask crop; the positive candidates' bit
+// planes (a warp's 32 pixels are one word of the chunk).  No later kernel reads grey, the image or the mask.
 __global__ void __launch_bounds__(kThreads) k_xor(Ctx c) {
   __shared__ unsigned long long sx[12];
+  __shared__ unsigned Cw[6][kChunkPx / 32];   // the chunk's candidate words, written to the planes coalesced at the end
   const View v = view_of(c, blockIdx.x);
   const WinState& st = c.st[v.w];
   if (threadIdx.x < 12) sx[threadIdx.x] = 0ull;
@@ -405,7 +440,9 @@ __global__ void __launch_bounds__(kThreads) k_xor(Ctx c) {
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
       const int k = k0 + u * kThreads + threadIdx.x;
-      mk[u] = -1;
+      mk[u] = -1; gr[u] = 0;
+#pragma unroll
+      for (int q = 0; q < 3; ++q) ch[u][q] = 0;
       if (k < v.cnt) {
         int y, x;
         divmod(v.i0 + k, dv, y, x);
@@ -418,14 +455,20 @@ __global__ void __launch_bounds__(kThreads) k_xor(Ctx c) {
     }
 #pragma unroll
     for (int u = 0; u < kU; ++u) {
-      if (mk[u] < 0) continue;
-      ++npx;
+      const int kb = k0 + u * kThreads + (int(threadIdx.x) & ~31);   // the first pixel of the warp's word
+      if (kb >= v.cnt) continue;                                      // warp-uniform
+      const bool in = mk[u] >= 0;
+      npx += in;
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
-        const int t = (gr[u] >= lo[k] && gr[u] <= hi[k]) ? 255 : 0;     // only read for k < ncol
-        pos[k] += (unsigned)(t ^ mk[u]);
-        const int t2 = ch[u][k] > ot[k] ? 255 : 0;
-        pos[3 + k] += (unsigned)(t2 ^ mk[u]);
+        const bool t = in && gr[u] >= lo[k] && gr[u] <= hi[k];          // only read for k < ncol
+        const bool t2 = in && ch[u][k] > ot[k];
+        if (in) {
+          pos[k] += (unsigned)((t ? 255 : 0) ^ mk[u]);
+          pos[3 + k] += (unsigned)((t2 ? 255 : 0) ^ mk[u]);
+        }
+        const unsigned b = __ballot_sync(0xffffffffu, t), b2 = __ballot_sync(0xffffffffu, t2);
+        if ((threadIdx.x & 31) == 0) { Cw[k][kb >> 5] = b; Cw[3 + k][kb >> 5] = b2; }
       }
     }
   }
@@ -445,6 +488,12 @@ __global__ void __launch_bounds__(kThreads) k_xor(Ctx c) {
   }
   __syncthreads();
   if (threadIdx.x < 12 && sx[threadIdx.x]) atomicAdd(&c.st[v.w].xs[threadIdx.x], sx[threadIdx.x]);
+  const int nw = (v.cnt + 31) >> 5;
+  for (int k = 0; k < 6; ++k) {
+    if (k < 3 && k >= ncol) continue;   // no round reads the plane of a colour the window does not have
+    unsigned* cw = c.cand + k * c.plane_words + v.woff;
+    for (int w = threadIdx.x; w < nw; w += kThreads) cw[w] = Cw[k][w];
+  }
 }
 
 // candidate order (one thread per window): minxor_thresh + sort
@@ -484,8 +533,8 @@ __global__ void k_decide2(Ctx c, int n_wins) {
 }
 
 // ---- labelling of a source plane: candidate `round` (0..3) or, round == 4, the inverse of `merged` (hole filling) -----
-// Level 1, one CTA per chunk (<= kChunkPx pixels), everything in SHARED memory: source pixels (coalesced), run starts by
-// warp ballot, seams between warps and the contacts between the rows of the chunk united in a shared union-find; every
+// Level 1, one CTA per chunk (<= kChunkPx pixels), everything in SHARED memory: the source words, the run starts inside
+// each word, seams between words and the contacts between the rows of the chunk united in a shared union-find; every
 // pixel's chunk-local root goes to the 16-bit `lab` plane as an offset in its chunk, and the chunk's roots (the nodes of
 // the global forest P, which only ever touches root entries) to the chunk's root list.  Level 2: only the first row of
 // every chunk issues global unions with the row above it, and the first pixel of a row segment with the last pixel of
@@ -494,6 +543,61 @@ __global__ void k_decide2(Ctx c, int n_wins) {
 // In the chunk-local passes a chunk pixel k is treated as at column k % rw of row k / rw: right for whole rows, and for
 // a row segment (k < cnt <= kChunkPx < rw) one row whose first pixel starts a run and which has no row above.
 constexpr int kLabelThreads = 512;
+
+// The source of a labelling round as words of the chunk: foreground word w = (words[w] ^ flip) & tail_mask(w, cnt)
+struct Source { const unsigned* words; unsigned flip; };
+__device__ __forceinline__ Source source_of(const Ctx& c, const WinState& st, const View& v, int round) {
+  if (round == 4) return Source{c.merged + v.woff, 0xffffffffu};
+  return Source{c.cand + size_t(st.proc_kind[round]) * c.plane_words + v.woff, st.proc_neg[round] ? 0xffffffffu : 0u};
+}
+
+// The merge of labelling round `round` (textmask.py:92-108 / 118-131), for one chunk, by all threads of its CTA: every run
+// of the round's source whose root merges (kMergeBit in the chunk's root list, k_decide_roots) is ORed into the chunk's
+// `merged` words.  The runs are the labelling's, recomputed from the same source words (in round 4 the source is `merged`
+// itself, untouched since the labelling), and a run's root is the label at its first pixel.  `dec`: kChunkPx / 32 words
+// of shared memory.
+// Who applies which round: `merged` is current up to round r - 2 when k_label_local(r) starts, r = 1..3, and that
+// kernel applies round r - 1 to its own chunk before it reads `merged` (also for a window whose last candidate round
+// was r - 1, which then returns); k_merge applies round 3 before the dilation, which reads neighbouring chunks, and the
+// hole filling; k_or applies round 4.
+__device__ void apply_merges(const Ctx& c, const View& v, int chunk, int round, unsigned* dec) {
+  for (int i = threadIdx.x; i < kChunkPx / 32; i += blockDim.x) dec[i] = 0u;
+  __syncthreads();
+  const uint16_t* roots = c.roots + v.win.off + v.i0;
+  const int nr = c.nroots[chunk];
+  bool any = false;
+  for (int j = threadIdx.x; j < nr; j += blockDim.x) {
+    const unsigned e = roots[j];
+    if (e & kMergeBit) { atomicOr(&dec[(e ^ kMergeBit) >> 5], 1u << (e & 31)); any = true; }
+  }
+  if (!__syncthreads_or(any)) return;   // no root of the chunk merges
+  const uint16_t* lab = c.lab + v.win.off + v.i0;
+  const Source src = source_of(c, c.st[v.w], v, round);
+  unsigned* merged = c.merged + v.woff;
+  const DivW dv = make_div(v.rw, kChunkPx + 1);
+  // two threads per word, each with the run starts of its half; the even lane writes the word.  The trip count is
+  // the same for a whole warp: both lanes have read the source word (`merged` itself in round 4) before the shuffle.
+  for (int hw0 = 0; hw0 * 16 < v.cnt; hw0 += blockDim.x) {
+    const int hw = hw0 + threadIdx.x, w = hw >> 1;
+    unsigned add = 0u;
+    if (hw * 16 < v.cnt) {
+      const unsigned M = (src.words[w] ^ src.flip) & tail_mask(w, v.cnt);
+      if (M) {
+        int yl, x0;
+        divmod(w * 32, dv, yl, x0);
+        const unsigned S = M & (~(M << 1) | row_start_bits(x0, v.rw));
+        for (unsigned f = S & ((hw & 1) ? 0xffff0000u : 0x0000ffffu); f; f &= f - 1u) {
+          const int sbit = __ffs(f) - 1;
+          const unsigned l = lab[w * 32 + sbit];
+          if ((dec[l >> 5] >> (l & 31)) & 1u) add |= span_bits(sbit, run_end(M, S, sbit));
+        }
+      }
+    }
+    add |= __shfl_xor_sync(0xffffffffu, add, 1);
+    if (add && !(hw & 1)) merged[w] |= add;
+  }
+  __syncthreads();
+}
 
 __device__ __forceinline__ int suf_find(const int* L, int a) {
   int p = L[a];
@@ -534,6 +638,26 @@ __device__ __forceinline__ void suf_union(int* L, int a, int b) {
   } while (!done);
 }
 
+// Pass timing of k_label_local (scripts/refine_table.py --passes builds a second library with -DCTD_REFINE_PASS_CLOCKS):
+// thread 0 of every CTA adds the clock64() ticks between two pass boundaries, each behind a CTA barrier, to
+// g_pass_clocks[round][pass].  Without the macro nothing is compiled in.
+#ifdef CTD_REFINE_PASS_CLOCKS
+__device__ unsigned long long g_pass_clocks[5][8];
+#define PASS_CLOCK_BEGIN() long long pass_t0 = clock64()
+#define PASS_CLOCK(pass)                                                                        \
+  do {                                                                                          \
+    __syncthreads();                                                                            \
+    if (threadIdx.x == 0) {                                                                     \
+      const long long t = clock64();                                                            \
+      atomicAdd(&g_pass_clocks[round][pass], (unsigned long long)(t - pass_t0));                \
+      pass_t0 = t;                                                                              \
+    }                                                                                           \
+  } while (0)
+#else
+#define PASS_CLOCK_BEGIN()
+#define PASS_CLOCK(pass)
+#endif
+
 __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int round) {
   __shared__ int Ls[kChunkPx];
   __shared__ unsigned Mw[kChunkPx / 32 + 2];      // foreground bits, 32 pixels per word (+ zero padding)
@@ -543,7 +667,10 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
   __shared__ int s_fg, s_nroot;
   const View v = view_of(c, blockIdx.x);
   WinState& st = c.st[v.w];
+  PASS_CLOCK_BEGIN();
+  if (round >= 1 && round <= 3 && round - 1 < st.nproc) apply_merges(c, v, blockIdx.x, round - 1, Sw);
   if (round < 4 && round >= st.nproc) return;
+  PASS_CLOCK(0);
   for (int i = threadIdx.x; i < kChunkPx / 32 + 2; i += kLabelThreads) Mw[i] = 0u;
   if (threadIdx.x == 0) { s_fg = 0; s_nroot = 0; }
   __syncthreads();
@@ -553,150 +680,32 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
   int* acc = c.acc + 4 * v.win.off;
   const int n = v.rw * v.rh;
   int* area = acc; int* gain = acc + n; int* loss = acc + 2 * n; int* maxi = acc + 3 * n;
-  const uint8_t* grey = c.grey + v.win.off;
-  const uint8_t* merged = c.merged + v.win.off;
-  const uint8_t* predm = c.predm + v.win.off;
-  int kind = 0, neg = 0, lo = 0, hi = 0, ot = 0;
-  if (round < 4) {
-    kind = st.proc_kind[round]; neg = st.proc_neg[round];
-    if (kind < 3) { lo = st.lo[kind]; hi = st.hi[kind]; } else ot = st.otsu_t[kind - 3];
-  }
-  const int lane = threadIdx.x & 31;
   const DivW dv = make_div(v.rw, kChunkPx + 1);   // chunk-local indices: k = row * rw + x, k < kChunkPx
-  constexpr int kIt = kChunkPx / kLabelThreads;    // 16 pixels per thread
-  // pass 1: source value, `merged` and `pred` of every pixel (coalesced; the loads of a batch are issued before their
-  // first use) -> foreground / gain / loss BIT masks and the run starts inside each warp's 32 consecutive pixels
-  if (v.aligned) {
-    // pass 1, vector form (the chunk starts on a 4-byte boundary of the byte planes): FOUR consecutive pixels per thread from
-    // one 32-bit load per plane; the three 4-bit results of 8 lanes are OR-reduced into the 32-pixel words (redux.sync) --
-    // a quarter of the loads / address arithmetic and no per-pixel ballots or shared-memory stores.
-    const uint32_t* mg32 = reinterpret_cast<const uint32_t*>(merged + v.i0);
-    const uint32_t* pd32 = reinterpret_cast<const uint32_t*>(predm + v.i0);
-    const uint32_t* gr32 = reinterpret_cast<const uint32_t*>(grey + v.i0);
-    const int sh = 4 * (lane & 7);
-    const unsigned grp = 0xffu << (8 * (lane >> 3));
-#pragma unroll 1
-    for (int it = 0; it < kChunkPx / (4 * kLabelThreads); ++it) {
-      if (it * 4 * kLabelThreads >= v.cnt) break;      // CTA-uniform
-      const int k = 4 * (it * kLabelThreads + int(threadIdx.x));
-      unsigned fg4 = 0u, g4 = 0u, b4 = 0u;
-      if (k < v.cnt) {
-        const unsigned m4 = mg32[k >> 2], p4 = pd32[k >> 2];
-        unsigned s4 = m4;
-        if (round < 4) {
-          if (kind < 3) {
-            s4 = gr32[k >> 2];
-          } else {
-            s4 = 0u;
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              if (k + j < v.cnt) {
-                int yl, x;
-                divmod(k + j, dv, yl, x);
-                s4 |= unsigned(v.img[(size_t(v.win.y1 + v.y0 + yl) * v.win.pitch + v.win.x1 + v.x0 + x) * 3 + (kind - 3)]) << (8 * j);
-              }
-            }
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          if (k + j < v.cnt) {
-            const int sbv = int((s4 >> (8 * j)) & 0xffu), mb = int((m4 >> (8 * j)) & 0xffu), pb = int((p4 >> (8 * j)) & 0xffu);
-            bool fg;
-            if (round == 4) {
-              fg = sbv == 0;
-            } else {
-              const bool t = kind < 3 ? (sbv >= lo && sbv <= hi) : (sbv > ot);
-              fg = neg ? !t : t;
-            }
-            const bool un = fg && mb == 0;
-            fg4 |= unsigned(fg) << j;
-            g4 |= unsigned(un && pb != 0) << j;
-            b4 |= unsigned(un && pb == 0) << j;
-          }
-        }
-      }
-      const unsigned M = __reduce_or_sync(grp, fg4 << sh), G = __reduce_or_sync(grp, g4 << sh), B = __reduce_or_sync(grp, b4 << sh);
-      if ((lane & 7) == 0) { const int w = k >> 5; Mw[w] = M; Gw[w] = G; Bw[w] = B; }
-    }
-    __syncthreads();
-    // run starts: a foreground pixel whose left neighbour in the same row AND word is not foreground
-    for (int w = threadIdx.x; w * 32 < v.cnt; w += kLabelThreads) {
-      const unsigned M = Mw[w];
+  // pass 1: the source, `merged` and `pred` words -> foreground / gain / loss masks and the run starts inside each word
+  // (a foreground pixel whose left neighbour in the same row AND word is not foreground), two threads per word
+  {
+    const Source src = source_of(c, st, v, round);
+    const unsigned* mgw = c.merged + v.woff;
+    const unsigned* pdw = c.pred + v.woff;
+    for (int hw = threadIdx.x; hw * 16 < v.cnt; hw += kLabelThreads) {
+      const int w = hw >> 1;
+      const unsigned M = (src.words[w] ^ src.flip) & tail_mask(w, v.cnt);
       int yl, x0;
       divmod(w * 32, dv, yl, x0);
-      unsigned rs = 0u;
-      for (int j = x0 == 0 ? 0 : v.rw - x0; j < 32; j += v.rw) rs |= 1u << j;
-      const unsigned S = M & (~(M << 1) | rs);
-      Sw[w] = S;
-      unsigned f = S;
-      while (f) {
+      const unsigned S = M & (~(M << 1) | row_start_bits(x0, v.rw));
+      if (!(hw & 1)) {
+        const unsigned un = M & ~mgw[w], pd = pdw[w];
+        Mw[w] = M; Sw[w] = S; Gw[w] = un & pd; Bw[w] = un & ~pd;
+      }
+      // forest nodes = run starts; any other foreground pixel maps to its run start via start_of()
+      for (unsigned f = S & ((hw & 1) ? 0xffff0000u : 0x0000ffffu); f; f &= f - 1u) {
         const int k = w * 32 + __ffs(f) - 1;
-        f &= f - 1u;
         Ls[k] = k;
-      }
-    }
-  } else {
-    constexpr int kB = 4;
-    int xrun, xstep;                                 // x = k % rw without a division per pixel: k advances by kLabelThreads
-    {
-      int q;
-      divmod(int(threadIdx.x), dv, q, xrun);
-      divmod(kLabelThreads, dv, q, xstep);
-    }
-  #pragma unroll 1
-    for (int ub = 0; ub < kIt; ub += kB) {
-      if (ub * kLabelThreads >= v.cnt) break;        // CTA-uniform
-      int raw[kB], mg[kB], pd[kB];
-  #pragma unroll
-      for (int u = 0; u < kB; ++u) {
-        const int k = (ub + u) * kLabelThreads + threadIdx.x;
-        raw[u] = 0; mg[u] = 1; pd[u] = 0;
-        if (k < v.cnt) {
-          const int i = v.i0 + k;
-          mg[u] = merged[i];
-          pd[u] = predm[i];
-          if (round == 4) raw[u] = mg[u];
-          else if (kind < 3) raw[u] = grey[i];
-          else {
-            int yl, x;
-            divmod(k, dv, yl, x);
-            raw[u] = v.img[(size_t(v.win.y1 + v.y0 + yl) * v.win.pitch + v.win.x1 + v.x0 + x) * 3 + (kind - 3)];
-          }
-        }
-      }
-  #pragma unroll
-      for (int u = 0; u < kB; ++u) {
-        const int k0 = (ub + u) * kLabelThreads;
-        if (k0 >= v.cnt) break;                       // CTA-uniform
-        const int k = k0 + threadIdx.x;
-        const bool in = k < v.cnt;
-        int sv = 0;
-        const int x = xrun;                           // x of pixel k, carried from iteration to iteration
-        xrun += xstep;
-        if (xrun >= v.rw) xrun -= v.rw;
-        if (in) {
-          if (round == 4) {
-            sv = raw[u] ? 0 : 255;
-          } else {
-            const int tv = kind < 3 ? ((raw[u] >= lo && raw[u] <= hi) ? 255 : 0) : (raw[u] > ot ? 255 : 0);
-            sv = neg ? 255 - tv : tv;
-          }
-        }
-        const bool fg = in && sv != 0;
-        const bool un = fg && mg[u] == 0;
-        const unsigned m = __ballot_sync(0xffffffffu, fg);
-        const unsigned gb = __ballot_sync(0xffffffffu, un && pd[u] != 0);
-        const unsigned lb = __ballot_sync(0xffffffffu, un && pd[u] == 0);
-        // a run starts at a foreground pixel whose left neighbour (same row, same warp) is not foreground
-        const bool starts = fg && (lane == 0 || x == 0 || !((m >> (lane - 1)) & 1u));
-        const unsigned sb = __ballot_sync(0xffffffffu, starts);
-        if (lane == 0) { Mw[k >> 5] = m; Sw[k >> 5] = sb; Gw[k >> 5] = gb; Bw[k >> 5] = lb; }
-        if (starts) Ls[k] = k;    // forest nodes = run starts; any other foreground pixel maps to its run start via start_of()
       }
     }
   }
   __syncthreads();
+  PASS_CLOCK(1);
   // pass 2: seams between warps, contacts with the row above inside the chunk -- on the foreground BIT masks, two
   // threads per 32-pixel word: the neighbour tests of 32 pixels are a handful of shifts and ANDs, and only the pixels
   // that really start a (run x upper run) contact walk the union-find (first version: every foreground pixel tested
@@ -719,8 +728,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     const int k0 = w * 32;
     int yl, x0;
     divmod(k0, dv, yl, x0);
-    unsigned rs = 0u;                               // bits whose pixel is the FIRST of its row (x == 0)
-    for (int j = x0 == 0 ? 0 : v.rw - x0; j < 32; j += v.rw) rs |= 1u << j;
+    const unsigned rs = row_start_bits(x0, v.rw);   // bits whose pixel is the FIRST of its row (x == 0)
     int xe = x0 + 32;                               // x of the pixel after this word
     if (xe >= v.rw) xe %= v.rw;
     const unsigned re = (rs >> 1) | (xe == 0 ? 0x80000000u : 0u);   // bits whose pixel is the LAST of its row
@@ -752,6 +760,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     }
   }
   __syncthreads();
+  PASS_CLOCK(3);
   // pass 3a: flatten the forest.  Its nodes are the run starts only (every other foreground pixel points at its run
   // start and is never re-parented): after this pass every run start points straight at its root, so the root of ANY
   // foreground pixel is Ls[Ls[k]] -- two loads instead of a walk (the walks were 10 hops on average, ncu).  The roots
@@ -778,7 +787,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
   }
   if (round == 4) {   // label 0 of the inverse = the pixels already in `merged`
     for (int o = 16; o > 0; o >>= 1) fgc += __shfl_down_sync(0xffffffffu, fgc, o);
-    if (lane == 0 && fgc) atomicAdd(&s_fg, fgc);
+    if ((threadIdx.x & 31) == 0 && fgc) atomicAdd(&s_fg, fgc);
   }
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -786,9 +795,11 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     const int a0 = v.cnt - s_fg;
     if (round == 4 && a0) atomicAdd(&st.area0, a0);
   }
+  PASS_CLOCK(4);
   // pass 3b: chunk-local root of every pixel to global memory (an offset in the chunk; kNoLabel = background)
   for (int k = threadIdx.x; k < v.cnt; k += kLabelThreads)
     lab[k] = ((Mw[k >> 5] >> (k & 31)) & 1u) ? uint16_t(Ls[start_of(k)]) : kNoLabel;
+  PASS_CLOCK(5);
   // pass 3c: per-label sums, one update per RUN (popcounts of the run's bits in the foreground / gain / loss masks) into
   // the sums of its chunk-local root.  k_flat1 adds the sums of the chunk roots of a multi-chunk window to their global
   // root; there is no per-pixel accumulation sweep any more.
@@ -802,9 +813,8 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     while (f) {
       const int sbit = __ffs(f) - 1;
       f &= f - 1u;
-      const unsigned stop = (~M | S) & (0xfffffffeu << sbit);          // first position after the run
-      const int e = stop ? __ffs(stop) - 2 : 31;                       // last pixel of the run
-      const unsigned rm = (e == 31 ? 0xffffffffu : ((2u << e) - 1u)) & ~((1u << sbit) - 1u);
+      const int e = run_end(M, S, sbit);                               // last pixel of the run
+      const unsigned rm = span_bits(sbit, e);
       const int gi = v.i0 + Ls[k0 + sbit];
       atomicAdd(&area[gi], __popc(rm));
       atomicMax(&maxi[gi], v.i0 + k0 + e);
@@ -813,6 +823,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
       if (l_) atomicAdd(&loss[gi], l_);
     }
   }
+  PASS_CLOCK(6);
 }
 // level 2: the first row of every chunk against the row above it (x-1, x, x+1, possibly in the neighbouring row
 // segments), and the first pixel of a row segment against the last pixel of the segment to its left
@@ -910,24 +921,22 @@ __global__ void __launch_bounds__(kThreads) k_top_b(Ctx c) {
     if (m2 >= 0) atomicMax(&st.max2, m2);
   }
 }
-__global__ void __launch_bounds__(kThreads) k_mapply(Ctx c, int round) {
+// The merge decision of every chunk-local root, from the sums of its global root (P[cr]: k_flat1, or cr itself in a
+// single-chunk window), as kMergeBit of its root list entry.  It has a kernel of its own because a global root's sums
+// are complete only when k_flat1 has ended, and the next labelling of the root's chunk zeroes them.  apply_merges ORs
+// the runs of the merging roots into `merged`.
+__global__ void __launch_bounds__(kThreads) k_decide_roots(Ctx c, int round) {
   const View v = view_of(c, blockIdx.x);
   const WinState& st = c.st[v.w];
   if (round < 4 && round >= st.nproc) return;
-  const uint16_t* lab = c.lab + v.win.off + v.i0;
   const int* P = c.P + v.win.off;
-  uint8_t* merged = c.merged + v.win.off;
   const int* acc = c.acc + 4 * v.win.off;
   const int n = v.rw * v.rh;
   const int* area = acc; const int* gain = acc + n; const int* loss = acc + 2 * n; const int* maxi = acc + 3 * n;
   // sorted_area[-2] if more than one label else sorted_area[-1] (textmask.py:114-118); label 0 always exists
   const int second = st.cnt1 >= 2 ? st.max1 : st.max2;
   const int thresh = second >= 0 ? second : st.max1;
-  // the merge decision of every chunk-local root, from the sums of its global root (P[cr]: k_flat1, or cr itself in a
-  // single-chunk window), into shared memory at the root's chunk offset: the pixels then read one label and one
-  // shared byte instead of a parent and four sums each
-  __shared__ uint8_t dec[kChunkPx];
-  const uint16_t* roots = c.roots + v.win.off + v.i0;
+  uint16_t* roots = c.roots + v.win.off + v.i0;
   const int nr = c.nroots[blockIdx.x];
   for (int j = threadIdx.x; j < nr; j += kThreads) {
     const int cl = roots[j];
@@ -941,54 +950,70 @@ __global__ void __launch_bounds__(kThreads) k_mapply(Ctx c, int round) {
     } else {
       ok = a < thresh;  // textmask.py:120
     }
-    dec[cl] = ok && gain[g] > loss[g];
+    if (ok && gain[g] > loss[g]) roots[j] = uint16_t(cl | kMergeBit);
   }
-  __syncthreads();
-  auto merges = [&](unsigned l) { return l != kNoLabel && dec[l]; };
-  int k_tail = 0;
-  if (v.aligned) {
-    // four labels per 8-byte load (lab + i0 is 8-byte aligned), and one 4-byte OR into `merged` where any merges
-    const uint2* lab4 = reinterpret_cast<const uint2*>(lab);
-    uint32_t* mg32 = reinterpret_cast<uint32_t*>(merged + v.i0);
-    const int n4 = v.cnt >> 2;
-    for (int q = threadIdx.x; q < n4; q += kThreads) {
-      const uint2 l4 = lab4[q];
-      const unsigned m = (merges(l4.x & 0xffffu) ? 0xffu : 0u) | (merges(l4.x >> 16) ? 0xff00u : 0u) |
-                         (merges(l4.y & 0xffffu) ? 0xff0000u : 0u) | (merges(l4.y >> 16) ? 0xff000000u : 0u);
-      if (m) mg32[q] |= m;
-    }
-    k_tail = n4 << 2;
-  }
-  for (int k = k_tail + threadIdx.x; k < v.cnt; k += kThreads)
-    if (merges(lab[k])) merged[v.i0 + k] = 255;
+}
+__global__ void __launch_bounds__(kThreads) k_merge(Ctx c, int round) {
+  __shared__ unsigned dec[kChunkPx / 32];
+  const View v = view_of(c, blockIdx.x);
+  if (round >= c.st[v.w].nproc) return;
+  apply_merges(c, v, blockIdx.x, round, dec);
 }
 
 // ---- dilate 3x3 (inpaint mode): merged -> tmp; the caller swaps the two planes afterwards -----------------------------
-// `merged` is binary (0 / 255): the 3x3 maximum is an OR of nine shifted copies of the foreground BIT mask.  The chunk's
-// halo rectangle (see k_phase0) is packed into shared-memory words by warp ballots, one thread per 32-pixel word ORs
-// the nine views (window row ends masked), and the bytes are written back coalesced: ~25 instructions per pixel instead
-// of ~120 (nine bounds-checked byte loads).
+// The 3x3 maximum of a binary plane is an OR of nine shifted copies of its bits.  The chunk's halo rectangle (see
+// k_phase0) is gathered into shared-memory words at the rectangle's row stride -- its rows above and below, and for a
+// row segment the columns left and right, are bits of the neighbouring chunks' words -- and one thread per 32-pixel
+// word ORs the nine views (window row ends masked) and writes the word of `tmp`.
 __global__ void __launch_bounds__(kThreads) k_dilate(Ctx c) {
   __shared__ unsigned Mw[kExtWords];
-  __shared__ unsigned Ow[kChunkPx / 32 + 1];
   const View v = view_of(c, blockIdx.x);
-  const uint8_t* merged = c.merged + v.win.off;
-  uint8_t* tmp = c.tmp + v.win.off;
   for (int i = threadIdx.x; i < kExtWords; i += kThreads) Mw[i] = 0u;
   __syncthreads();
   const Halo hl = halo_of(v);
   const int ew = hl.ew;
-  // rectangle position e -> window pixel: contiguous for whole rows (gap 0); a row segment's rectangle has <= 3 rows
-  const int gap = v.rw - ew;
-  const uint8_t* src = merged + size_t(hl.ystart) * v.rw + hl.xs;
-  for (int e0 = 0; e0 < hl.ext; e0 += kThreads) {
+  const DivW dv = make_div(ew, 3 * (kChunkPx + 2) + 1);
+  // The chunks of a window are consecutive in the table, row by row: whole-row chunks one after the other (all but the
+  // window's last have refine_rows_per_chunk rows), row segments nseg per window row.
+  const bool seg = v.rw > kChunkPx;
+  const int nseg = (v.rw + kChunkPx - 1) / kChunkPx;
+  const int rows_up = seg ? 1 : refine_rows_per_chunk(v.rw);
+  if (!seg) {
+    // whole rows: the rectangle is the last row of the chunk above, the chunk, and the first row of the chunk below,
+    // one after the other -- three copies of consecutive bits
+    const bool up = v.y0 > 0, down = v.y0 + v.rows < v.rh;
+    const unsigned* mu = up ? c.merged + c.chunks[blockIdx.x - 1].woff : nullptr;
+    const unsigned* md = down ? c.merged + c.chunks[blockIdx.x + 1].woff : nullptr;
+    for (int d = threadIdx.x; d * 32 < hl.ext; d += kThreads) {
+      unsigned m = copied_word(c.merged + v.woff, 0, v.cnt, hl.off, d);
+      if (up) m |= copied_word(mu, (rows_up - 1) * v.rw, v.rw, 0, d);
+      if (down) m |= copied_word(md, 0, v.rw, hl.off + v.cnt, d);
+      Mw[d] = m;
+    }
+  }
+  for (int e0 = 0; seg && e0 < hl.ext; e0 += kThreads) {
     const int e = e0 + threadIdx.x;
-    const int row = gap == 0 ? 0 : (e >= ew) + (e >= 2 * ew);
-    const unsigned m = __ballot_sync(0xffffffffu, e < hl.ext && src[e + row * gap] != 0);
+    bool bit = false;
+    if (e < hl.ext) {
+      int ye, xe;
+      divmod(e, dv, ye, xe);
+      const int y = hl.ystart + ye, x = hl.xs + xe;
+      const int dy = y < v.y0 ? -1 : (y >= v.y0 + v.rows ? 1 : 0);
+      // the chunk that holds window pixel (y, x), and the pixel's offset k in it
+      int ch = int(blockIdx.x) + dy * (seg ? nseg : 1), k;
+      if (seg) {
+        ch += x / kChunkPx - v.x0 / kChunkPx;
+        k = x % kChunkPx;
+      } else {
+        k = (dy < 0 ? rows_up - 1 : (dy > 0 ? 0 : y - v.y0)) * v.rw + x;
+      }
+      const int wo = ch == int(blockIdx.x) ? v.woff : c.chunks[ch].woff;
+      bit = (c.merged[wo + (k >> 5)] >> (k & 31)) & 1u;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, bit);
     if ((threadIdx.x & 31) == 0 && e < hl.ext) Mw[e >> 5] = m;
   }
   __syncthreads();
-  const DivW dv = make_div(ew, 3 * (kChunkPx + 2) + 1);
   for (int w = threadIdx.x; w * 32 < v.cnt; w += kThreads) {
     const int p = w * 32 + hl.off;
     int ye, xe;
@@ -998,42 +1023,45 @@ __global__ void __launch_bounds__(kThreads) k_dilate(Ctx c) {
     unsigned o = bits_from(Mw, p) | bits_from(Mw, p - ew) | bits_from(Mw, p + ew);
     o |= (bits_from(Mw, p - 1) | bits_from(Mw, p - ew - 1) | bits_from(Mw, p + ew - 1)) & ~rs;
     o |= (bits_from(Mw, p + 1) | bits_from(Mw, p - ew + 1) | bits_from(Mw, p + ew + 1)) & ~re;
-    Ow[w] = o;
+    c.tmp[v.woff + w] = o & tail_mask(w, v.cnt);
   }
-  __syncthreads();
-  for (int k = threadIdx.x; k < v.cnt; k += kThreads) tmp[v.i0 + k] = ((Ow[k >> 5] >> (k & 31)) & 1u) ? 255 : 0;
 }
-// mask_refined[window] |= merged (textmask.py:168); windows may overlap -> atomic OR
+// the hole filling's merge, then mask_refined[window] |= merged (textmask.py:168); windows may overlap -> atomic OR,
+// issued for the set bits only
 __global__ void __launch_bounds__(kThreads) k_or(Ctx c) {
+  __shared__ unsigned dec[kChunkPx / 32];
   const View v = view_of(c, blockIdx.x);
-  const uint8_t* merged = c.merged + v.win.off;
+  apply_merges(c, v, blockIdx.x, 4, dec);
+  const unsigned* merged = c.merged + v.woff;
   const DivW dv = make_div(v.rw, v.rw * v.rh);
-  constexpr int U = 8;
-  for (int k0 = 0; k0 < v.cnt; k0 += kThreads * U) {
-    uint8_t mg[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int k = k0 + u * kThreads + threadIdx.x;
-      mg[u] = k < v.cnt ? merged[v.i0 + k] : 0;
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      if (!mg[u]) continue;
-      int y, x;
-      divmod(v.i0 + k0 + u * kThreads + threadIdx.x, dv, y, x);
-      const size_t gp = size_t(v.win.page_off) + size_t(v.win.y1 + y) * v.win.pitch + v.win.x1 + x;
-      atomicOr(&c.out_all[gp >> 2], 0xffu << (8 * (gp & 3)));
-    }
+  for (int k = threadIdx.x; k < v.cnt; k += kThreads) {   // a warp reads one word and spreads its set bits over its lanes
+    if (!((merged[k >> 5] >> (k & 31)) & 1u)) continue;
+    int y, x;
+    divmod(v.i0 + k, dv, y, x);
+    const size_t gp = size_t(v.win.page_off) + size_t(v.win.y1 + y) * v.win.pitch + v.win.x1 + x;
+    atomicOr(&c.out_all[gp >> 2], 0xffu << (8 * (gp & 3)));
   }
 }
 
 }  // namespace
 
+#ifdef CTD_REFINE_PASS_CLOCKS
+// copies g_pass_clocks to out[5 * 8] and zeroes it
+extern "C" __attribute__((visibility("default"))) int ctd_refine_pass_clocks(unsigned long long* out) {
+  static const unsigned long long zero[5 * 8] = {};
+  cudaError_t e = cudaMemcpyFromSymbol(out, g_pass_clocks, sizeof(zero));
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_pass_clocks, zero, sizeof(zero));
+  return int(e);
+}
+#endif
+
 size_t refine_mk_state_bytes(int n_wins) { return (size_t(n_wins) * sizeof(WinState) + 255) / 256 * 256; }
 // per window pixel: P (4 B) and the per-root sums (16 B), of which only root entries are touched; lab and the root
-// lists (2 B each); grey, predm, merged, tmp (1 B each).  Per chunk: its root count.
+// lists (2 B each); grey (1 B).  Per chunk: its root count.  Nine bit planes (six candidates, pred, merged, tmp) of
+// plane_words 4-byte words, 1.1 B per window pixel together.
+static size_t plane_words(size_t total_px, size_t n_chunks) { return total_px / 32 + n_chunks + 1; }
 size_t refine_scratch_bytes(size_t total_px, size_t n_chunks) {
-  return total_px * (4 + 16 + 2 + 2 + 4) + n_chunks * 4 + 4096;
+  return total_px * (4 + 16 + 2 + 2 + 1) + n_chunks * 4 + 9 * 4 * plane_words(total_px, n_chunks) + 4096;
 }
 
 // d_wins: n_wins windows; d_chunks: n_chunks chunks (RefineChunk, kernels.h); d_state: refine_mk_state_bytes(n_wins)
@@ -1055,10 +1083,12 @@ cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const 
   c.lab = reinterpret_cast<uint16_t*>(p); p += total_px * 2;
   c.roots = reinterpret_cast<uint16_t*>(p); p += total_px * 2;
   c.nroots = reinterpret_cast<int*>(p); p += size_t(n_chunks) * 4;
-  c.grey = reinterpret_cast<uint8_t*>(p); p += total_px;
-  c.predm = reinterpret_cast<uint8_t*>(p); p += total_px;
-  c.merged = reinterpret_cast<uint8_t*>(p); p += total_px;
-  c.tmp = reinterpret_cast<uint8_t*>(p);
+  c.grey = reinterpret_cast<uint8_t*>(p); p += total_px;   // total_px is a multiple of 4: the words below are aligned
+  c.plane_words = plane_words(total_px, size_t(n_chunks));
+  c.cand = reinterpret_cast<unsigned*>(p); p += 6 * 4 * c.plane_words;
+  c.pred = reinterpret_cast<unsigned*>(p); p += 4 * c.plane_words;
+  c.merged = reinterpret_cast<unsigned*>(p); p += 4 * c.plane_words;
+  c.tmp = reinterpret_cast<unsigned*>(p);
   cudaError_t e = cudaMemsetAsync(d_state, 0, refine_mk_state_bytes(n_wins), s);
   if (e != cudaSuccess) return e;
   const unsigned g = unsigned(n_chunks);
@@ -1067,9 +1097,10 @@ cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const 
   k_xor<<<g, kThreads, 0, s>>>(c);
   k_decide2<<<unsigned((n_wins + 127) / 128), 128, 0, s>>>(c, n_wins);
   for (int round = 0; round < 5; ++round) {
+    if (round == 4) k_merge<<<g, kThreads, 0, s>>>(c, 3);
     if (round == 4 && refine_mode == 0) {
       k_dilate<<<g, kThreads, 0, s>>>(c);
-      uint8_t* t = c.merged; c.merged = c.tmp; c.tmp = t;   // the dilated plane IS `merged` from here on (no copy back)
+      unsigned* t = c.merged; c.merged = c.tmp; c.tmp = t;   // the dilated plane IS `merged` from here on (no copy back)
     }
     k_label_local<<<g, kLabelThreads, 0, s>>>(c, round);
     if (n_multi_chunks > 0) {   // single-chunk windows: the chunk-local roots ARE the global roots
@@ -1080,7 +1111,7 @@ cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const 
       k_top_a<<<g, kThreads, 0, s>>>(c);
       k_top_b<<<g, kThreads, 0, s>>>(c);
     }
-    k_mapply<<<g, kThreads, 0, s>>>(c, round);
+    k_decide_roots<<<g, kThreads, 0, s>>>(c, round);
   }
   k_or<<<g, kThreads, 0, s>>>(c);
   return cudaGetLastError();

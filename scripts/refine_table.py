@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel table of refine_mask (csrc/refine_mk.cu) on the benchmark's batch.
 
-    python scripts/refine_table.py [--batch 16 --size 1024] [--gpu] [--mode 0] [--json FILE]
+    python scripts/refine_table.py [--batch 16 --size 1024] [--gpu | --passes] [--mode 0] [--json FILE] [--lib FILE]
 
 The batch is the one bench.py measures: the synthetic checkpoint of seed 0 and structured_page(1000 + i) for i < B,
 on the fp16 tensor-core engine.  One row per refine kernel: its launches per batch, the bytes it moves per window
@@ -13,15 +13,23 @@ chunks and window pixels, and the card's name and power limit, read in the same 
 Without --gpu (or without a GPU) the script prints the byte model per window pixel only: the windows come from the
 network's output, so their pixel count needs the engine.
 
+--passes measures how the time of k_label_local divides among its passes, per round.  It runs the same batch on a
+second build of the library, compiled with -DCTD_REFINE_PASS_CLOCKS into --passes-dir (built there by csrc/build.sh if
+it holds no library yet; the shipped library is not touched), in which thread 0 of every k_label_local CTA adds the
+clock64() ticks between pass boundaries to a global table.  The table printed is each pass's share of the summed CTA
+ticks of the round's launch: a share of CTA residency, not of the launch's wall time.  --lib runs --gpu on another
+build of the library (a parent's, to alternate it with this tree's).
+
 Byte model, per window pixel and launch (HBM; the window planes of a batch are ~1 GB, far over the 50 MB L2):
-  k_phase0        mask (+ halo rows) 1 + image 3 in; grey, predm, merged out 3                       7
-  k_xor           mask 1 + grey 1 + image 3                                                          5
-  k_label_local   merged 1 + predm 1 + source 1 (grey, or 1 of the image's 3 B) in; 16-bit label out  5
-  k_mapply        16-bit label in (merged is read and written only where a pixel merges)              2
-  k_dilate        merged (+ halo) 1 in, tmp 1 out (inpaint mode only)                                 2
-  k_or            merged 1 (the set pixels' atomics on mask_refined are not counted)                  1
-The per-window kernels (k_decide1, k_decide2), k_union_border (the first row of each chunk) and the kernels that walk
-the per-chunk root lists (k_flat1, k_top_a, k_top_b) move a negligible number of bytes.  Rounds a window skips
+  k_phase0        mask (+ halo rows) 1 + image 3 in; grey 1 + pred, merged bits 0.25 out             5.25
+  k_xor           mask 1 + grey 1 + image 3 in; six candidate bit planes 0.75 out                    5.75
+  k_label_local   source, merged, pred bits 0.375 in; 16-bit label out 2                             2.375
+  k_merge         source, merged bits 0.25 (labels are read at run starts only)                      0.25
+  k_dilate        merged bits (+ halo) in, tmp bits out (inpaint mode only)                          0.25
+  k_or            merged bits (the set pixels' atomics on mask_refined are not counted)              0.125
+The bit planes hold 32 pixels per 4-byte word: 0.125 B per pixel and plane.  The per-window kernels (k_decide1,
+k_decide2), k_union_border (the first row of each chunk) and the kernels that walk the per-chunk root lists (k_flat1,
+k_top_a, k_top_b, k_decide_roots) move a negligible number of bytes.  Rounds a window skips
 (nproc < 4) still launch but return at once: the model counts every round of every window, so it is an upper bound on
 the bytes of rounds 0..3.
 """
@@ -40,18 +48,19 @@ CHUNK_PX = 8192   # kRefineChunkPx (csrc/kernels.h)
 
 # name: (bytes per window pixel and launch, launches per batch in inpaint mode, pixels it sweeps: "all" / "multi")
 MODEL = {
-    "k_phase0": (7, 1, "all"),
+    "k_phase0": (5.25, 1, "all"),
     "k_decide1": (0, 1, "all"),
-    "k_xor": (5, 1, "all"),
+    "k_xor": (5.75, 1, "all"),
     "k_decide2": (0, 1, "all"),
-    "k_label_local": (5, 5, "all"),
+    "k_label_local": (2.375, 5, "all"),
     "k_union_border": (0, 5, "multi"),
     "k_flat1": (0, 5, "multi"),
     "k_top_a": (0, 1, "all"),
     "k_top_b": (0, 1, "all"),
-    "k_mapply": (2, 5, "all"),
-    "k_dilate": (2, 1, "all"),
-    "k_or": (1, 1, "all"),
+    "k_decide_roots": (0, 5, "all"),
+    "k_merge": (0.25, 1, "all"),
+    "k_dilate": (0.25, 1, "all"),
+    "k_or": (0.125, 1, "all"),
 }
 
 
@@ -81,11 +90,35 @@ def card():
     return q
 
 
-def gpu_run(n, h, w, mode):
+# g_pass_clocks[round][i] (csrc/refine_mk.cu): the merge of the round before, then the labelling's passes
+PASSES = ["merge r-1", "pass 1", "-", "pass 2", "pass 3a", "pass 3b", "pass 3c"]
+
+
+def build_passes_lib(build_dir):
+    lib = os.path.join(build_dir, "libctd_b200.so")
+    if not os.path.isfile(lib):
+        subprocess.run(["bash", os.path.join(ROOT, "comic-text-detector_b200", "csrc", "build.sh"),
+                        "-DCTD_REFINE_PASS_CLOCKS"], env=dict(os.environ, CTD_BUILD_DIR=os.path.abspath(build_dir)),
+                       check=True)
+    return lib
+
+
+def print_passes(clk, cardq):
+    print("k_label_local, share of the summed CTA clock ticks per pass and round; %s" % cardq)
+    print("%-6s %10s " % ("round", "Mticks") + " ".join("%10s" % p for p in PASSES))
+    for r in range(5):
+        tot = float(sum(clk[r]))
+        if tot > 0:
+            print("%-6d %10.1f " % (r, tot / 1e6) + " ".join("%9.1f%%" % (100.0 * c / tot) for c in clk[r][0:7]))
+
+
+def gpu_run(n, h, w, mode, lib=None, passes=False):
     import numpy as np
     import torch
     from torch.profiler import profile, ProfilerActivity
     import ctd_b200
+    if lib:
+        ctd_b200.binding.LIB_PATH = os.path.abspath(lib)   # read when the library is first loaded, below
     from ctd_b200 import multigpu
     from oracle import postproc_ref, synth
     ck = synth.make_checkpoint(0, smooth=True)
@@ -100,6 +133,17 @@ def gpu_run(n, h, w, mode):
             eng.submit_full(0, dev.data_ptr(), n, h, w, out.data_ptr(), refine_mode=mode, pages_on_device=True)
             eng.collect(0)
         torch.cuda.synchronize()
+        if passes:
+            import ctypes
+            clk = ((ctypes.c_ulonglong * 8) * 5)()
+            fn = ctd_b200.binding.load_library().ctd_refine_pass_clocks
+            fn(clk)   # drop the warm-up's ticks
+            eng.submit_full(0, dev.data_ptr(), n, h, w, out.data_ptr(), refine_mode=mode, pages_on_device=True)
+            eng.collect(0)
+            torch.cuda.synchronize()
+            if fn(clk) != 0:
+                raise RuntimeError("ctd_refine_pass_clocks failed")
+            return [[int(clk[r][i]) for i in range(8)] for r in range(5)], card()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             eng.submit_full(0, dev.data_ptr(), n, h, w, out.data_ptr(), refine_mode=mode, pages_on_device=True)
             eng.collect(0)
@@ -133,10 +177,21 @@ def main():
     ap.add_argument("--size", type=int, default=1024, help="square page size")
     ap.add_argument("--mode", type=int, choices=(0, 1), default=0, help="refine mode (0 = inpaint, as the benchmark)")
     ap.add_argument("--gpu", action="store_true", help="run the batch on cuda:0 and add the measured device times")
+    ap.add_argument("--passes", action="store_true", help="pass shares of k_label_local on a -DCTD_REFINE_PASS_CLOCKS build")
+    ap.add_argument("--passes-dir", default=None, help="build directory of that library (default: a temporary one)")
+    ap.add_argument("--lib", default=None, help="with --gpu: another build of libctd_b200.so to run")
     ap.add_argument("--json", default=None, help="also write the rows to this file")
     args = ap.parse_args()
     n, h, w = args.batch, args.size, args.size
     names = [k for k in MODEL if not (k == "k_dilate" and args.mode == 1)]
+    if args.passes:
+        with tempfile.TemporaryDirectory() as td:
+            clk, cardq = gpu_run(n, h, w, args.mode, lib=build_passes_lib(args.passes_dir or td), passes=True)
+        print_passes(clk, cardq)
+        if args.json:
+            with open(args.json, "w") as f:
+                json.dump({"shape": [n, h, w], "mode": args.mode, "card": cardq, "passes": PASSES, "ticks": clk}, f)
+        return
     if not args.gpu:
         print("refine_mask byte model per window pixel (CPU model; --gpu measures the batch)")
         print("%-15s %8s %6s %6s" % ("kernel", "launches", "B/px", "sweeps"))
@@ -144,11 +199,11 @@ def main():
         for k in names:
             b, l, sel = MODEL[k]
             tot += b * l if sel == "all" else 0
-            print("%-15s %8d %6d %6s" % (k, l, b, sel))
-        print("total over every window pixel: %d B (+ %d B per pixel of multi-chunk windows)"
+            print("%-15s %8d %6.3f %6s" % (k, l, b, sel))
+        print("total over every window pixel: %.2f B (+ %d B per pixel of multi-chunk windows)"
               % (tot, sum(MODEL[k][0] * MODEL[k][1] for k in names if MODEL[k][2] == "multi")))
         return
-    wins, times, counts, other_ms, cardq = gpu_run(n, h, w, args.mode)
+    wins, times, counts, other_ms, cardq = gpu_run(n, h, w, args.mode, lib=args.lib)
     n_chunks, n_multi, px, multi_px = plan_chunks(wins)
     print("refine_mask at %d x %d x %d, mode %d; %s" % (n, h, w, args.mode, cardq))
     print("windows %d, chunks %d (%d in multi-chunk windows), window pixels %.2f M (%.2f M in multi-chunk windows)"
@@ -164,7 +219,7 @@ def main():
         tot_ms += ms
         tot_gb += gb
         rows.append(dict(kernel=k, launches=launches, bytes_per_px=b, gb=gb, ms=ms))
-        print("%-15s %8d %6d %8.3f %8.3f %7s" % (k, launches, b, gb, ms, "%.2f" % (gb / ms) if ms > 0 and gb > 0 else "-"))
+        print("%-15s %8d %6.3f %8.3f %8.3f %7s" % (k, launches, b, gb, ms, "%.2f" % (gb / ms) if ms > 0 and gb > 0 else "-"))
     print("refine total: %.3f ms, %.2f GB modelled (%.2f TB/s); other kernels of the step: %.3f ms"
           % (tot_ms, tot_gb, tot_gb / tot_ms if tot_ms > 0 else 0.0, other_ms))
     if args.json:
