@@ -534,7 +534,8 @@ __global__ void k_decide2(Ctx c, int n_wins) {
 
 // ---- labelling of a source plane: candidate `round` (0..3) or, round == 4, the inverse of `merged` (hole filling) -----
 // Level 1, one CTA per chunk (<= kChunkPx pixels), everything in SHARED memory: the source words, the run starts inside
-// each word, seams between words and the contacts between the rows of the chunk united in a shared union-find; every
+// each word, each word seam a run crosses linked to the run's first pixel, and the contacts between the rows of the
+// chunk united in a shared union-find; every
 // pixel's chunk-local root goes to the 16-bit `lab` plane as an offset in its chunk, and the chunk's roots (the nodes of
 // the global forest P, which only ever touches root entries) to the chunk's root list.  Level 2: only the first row of
 // every chunk issues global unions with the row above it, and the first pixel of a row segment with the last pixel of
@@ -542,7 +543,12 @@ __global__ void k_decide2(Ctx c, int n_wins) {
 // P[chunk start + lab].
 // In the chunk-local passes a chunk pixel k is treated as at column k % rw of row k / rw: right for whole rows, and for
 // a row segment (k < cnt <= kChunkPx < rw) one row whose first pixel starts a run and which has no row above.
-constexpr int kLabelThreads = 512;
+// The labelling's passes are short and separated by CTA barriers, each bound by shared-memory and L2 latency: what
+// hides that latency is the number of chunks resident per SM.  256 threads and 39 registers (ptxas, sm_90a) with
+// 36.9 KB of shared memory fit six CTAs per SM; 512-thread CTAs fit three, and the kernel took 25 % longer (measured
+// on an H100 SXM on the bench batch; 384 threads, four CTAs: 17 % longer).
+constexpr int kLabelThreads = 256;
+constexpr int kLabelCtasPerSm = 6;
 
 // The source of a labelling round as words of the chunk: foreground word w = (words[w] ^ flip) & tail_mask(w, cnt)
 struct Source { const unsigned* words; unsigned flip; };
@@ -640,9 +646,18 @@ __device__ __forceinline__ void suf_union(int* L, int a, int b) {
 
 // Pass timing of k_label_local (scripts/refine_table.py --passes builds a second library with -DCTD_REFINE_PASS_CLOCKS):
 // thread 0 of every CTA adds the clock64() ticks between two pass boundaries, each behind a CTA barrier, to
-// g_pass_clocks[round][pass].  Without the macro nothing is compiled in.
+// g_pass_clocks[round][pass], and every warp adds its threads' union counts to g_pass_counts[round]: [0] word seams a
+// run crosses (linked in pass 1b), [1] shared unions of vertical and diagonal contacts (pass 2).  Without the macro
+// nothing is compiled in.  PASS_COUNT is called by all threads of the CTA.
 #ifdef CTD_REFINE_PASS_CLOCKS
 __device__ unsigned long long g_pass_clocks[5][8];
+__device__ unsigned long long g_pass_counts[5][2];
+#define PASS_COUNT(i, n)                                                                        \
+  do {                                                                                          \
+    const unsigned pc_ = __reduce_add_sync(0xffffffffu, unsigned(n));                           \
+    if ((threadIdx.x & 31) == 0 && pc_)                                                         \
+      atomicAdd(&g_pass_counts[round][i], (unsigned long long)pc_);                             \
+  } while (0)
 #define PASS_CLOCK_BEGIN() long long pass_t0 = clock64()
 #define PASS_CLOCK(pass)                                                                        \
   do {                                                                                          \
@@ -654,16 +669,18 @@ __device__ unsigned long long g_pass_clocks[5][8];
     }                                                                                           \
   } while (0)
 #else
+#define PASS_COUNT(i, n) (void)(n)
 #define PASS_CLOCK_BEGIN()
 #define PASS_CLOCK(pass)
 #endif
 
-__global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int round) {
+__global__ void __launch_bounds__(kLabelThreads, kLabelCtasPerSm) k_label_local(Ctx c, int round) {
   __shared__ int Ls[kChunkPx];
   __shared__ unsigned Mw[kChunkPx / 32 + 2];      // foreground bits, 32 pixels per word (+ zero padding)
   __shared__ unsigned Sw[kChunkPx / 32];          // run-start bits (the only nodes of the chunk-local forest)
   __shared__ unsigned Gw[kChunkPx / 32];          // foreground & not yet merged & predicted     ("gain" pixels)
   __shared__ unsigned Bw[kChunkPx / 32];          // foreground & not yet merged & not predicted ("loss" pixels)
+  __shared__ unsigned Tw[kChunkPx / 32 / 32];     // words that a run passes through (pass 1b), one bit per word
   __shared__ int s_fg, s_nroot;
   const View v = view_of(c, blockIdx.x);
   WinState& st = c.st[v.w];
@@ -705,12 +722,43 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     }
   }
   __syncthreads();
+  // pass 1b: a run that crosses word seams is ONE forest node, its first pixel.  Bit 0 of a word that continues the run
+  // of the word before it (the same row, both pixels foreground) is linked straight to that run's first pixel, with a
+  // plain store: a parent has a smaller index than its child, and the pass-2 unions only ever lower a root's entry.
+  // The run's first pixel is the highest run start of the last word before this one that the run does not pass through
+  // (a word passes through when it is foreground throughout and its bit 0 continues the run: Sw == 1 and cont).
+  static_assert(kChunkPx / 32 <= kLabelThreads, "pass 1b: one thread per word");
+  {
+    const int w = threadIdx.x;
+    bool cont = false;
+    if (w > 0 && w * 32 < v.cnt && (Mw[w] & 1u) && (Mw[w - 1] >> 31)) {
+      int yl, x0;
+      divmod(w * 32, dv, yl, x0);
+      cont = x0 != 0;                               // bit 0 does not start a row
+    }
+    const unsigned tb = __ballot_sync(0xffffffffu, cont && Sw[w] == 1u);
+    if ((threadIdx.x & 31) == 0 && threadIdx.x < kChunkPx / 32) Tw[threadIdx.x >> 5] = tb;
+    __syncthreads();
+    if (cont) {                                     // word 0 never passes through: the walk ends
+      int u = w - 1;
+      unsigned t = ~Tw[u >> 5] & (0xffffffffu >> (31 - (u & 31)));
+      while (!t) {
+        u = (u & ~31) - 1;
+        t = ~Tw[u >> 5];
+      }
+      u = (u & ~31) + 31 - __clz(t);
+      Ls[w * 32] = u * 32 + 31 - __clz(Sw[u]);
+    }
+    PASS_COUNT(0, cont);
+  }
+  __syncthreads();
   PASS_CLOCK(1);
-  // pass 2: seams between warps, contacts with the row above inside the chunk -- on the foreground BIT masks, two
+  // pass 2: contacts with the row above inside the chunk -- on the foreground BIT masks, two
   // threads per 32-pixel word: the neighbour tests of 32 pixels are a handful of shifts and ANDs, and only the pixels
   // that really start a (run x upper run) contact walk the union-find (first version: every foreground pixel tested
   // its four neighbours with byte loads; half of the kernel's instructions, ncu).
-  // run start of foreground pixel p: the highest run-start bit at or below p in its word (runs restart at every word)
+  // run start of foreground pixel p: the highest run-start bit at or below p in its word (a node of the forest; one
+  // that continues the run of the word before points at the run's first pixel since pass 1b)
   auto start_of = [&](int pos) -> int {
     return (pos & ~31) + 31 - __clz(Sw[pos >> 5] & (0xffffffffu >> (31 - (pos & 31))));
   };
@@ -720,6 +768,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     const int w = pos >> 5, sft = pos & 31;
     return __funnelshift_r(Mw[w], Mw[w + 1], sft);
   };
+  unsigned n_contacts = 0;   // shared unions of this thread (counted in the CTD_REFINE_PASS_CLOCKS build)
   for (int hw = threadIdx.x; hw * 16 < v.cnt; hw += kLabelThreads) {
     const int w = hw >> 1;
     const unsigned half = (hw & 1) ? 0xffff0000u : 0x0000ffffu;
@@ -733,13 +782,12 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
     if (xe >= v.rw) xe %= v.rw;
     const unsigned re = (rs >> 1) | (xe == 0 ? 0x80000000u : 0u);   // bits whose pixel is the LAST of its row
     const unsigned lft = bits_at(k0 - 1);           // fg(k - 1)
-    // seam: the run labelling of pass 1 restarts at every word
-    if (!(hw & 1) && (cur & 1u) && !(rs & 1u) && (lft & 1u)) suf_union(Ls, k0, start_of(k0 - 1));
     if (k0 + 32 <= v.rw) continue;                  // the whole word lies in the first row of the chunk
     const unsigned vup = (k0 >= v.rw ? 0xffffffffu : (0xffffffffu << (v.rw - k0))) & half;   // pixels that have a row above
     const unsigned up = bits_at(k0 - v.rw), upl = bits_at(k0 - v.rw - 1), upr = bits_at(k0 - v.rw + 1);
     // pixel and the pixel above are foreground: only the first pixel of each (current run x upper run) overlap unions
     unsigned f = cur & up & vup & (rs | ~lft | ~upl);
+    n_contacts += __popc(f) + __popc(cur & ~up & vup & upl & ~rs) + __popc(cur & ~up & vup & upr & ~re);
     while (f) {
       const int j = __ffs(f) - 1;
       f &= f - 1u;
@@ -759,6 +807,7 @@ __global__ void __launch_bounds__(kLabelThreads, 3) k_label_local(Ctx c, int rou
       suf_union(Ls, start_of(k0 + j), start_of(k0 + j - v.rw + 1));
     }
   }
+  PASS_COUNT(1, n_contacts);
   __syncthreads();
   PASS_CLOCK(3);
   // pass 3a: flatten the forest.  Its nodes are the run starts only (every other foreground pixel points at its run
@@ -1046,11 +1095,13 @@ __global__ void __launch_bounds__(kThreads) k_or(Ctx c) {
 }  // namespace
 
 #ifdef CTD_REFINE_PASS_CLOCKS
-// copies g_pass_clocks to out[5 * 8] and zeroes it
+// copies g_pass_clocks to out[0, 5 * 8) and g_pass_counts to out[5 * 8, 5 * 8 + 5 * 2), and zeroes both
 extern "C" __attribute__((visibility("default"))) int ctd_refine_pass_clocks(unsigned long long* out) {
   static const unsigned long long zero[5 * 8] = {};
-  cudaError_t e = cudaMemcpyFromSymbol(out, g_pass_clocks, sizeof(zero));
-  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_pass_clocks, zero, sizeof(zero));
+  cudaError_t e = cudaMemcpyFromSymbol(out, g_pass_clocks, sizeof(g_pass_clocks));
+  if (e == cudaSuccess) e = cudaMemcpyFromSymbol(out + 5 * 8, g_pass_counts, sizeof(g_pass_counts));
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_pass_clocks, zero, sizeof(g_pass_clocks));
+  if (e == cudaSuccess) e = cudaMemcpyToSymbol(g_pass_counts, zero, sizeof(g_pass_counts));
   return int(e);
 }
 #endif

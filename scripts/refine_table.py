@@ -17,7 +17,9 @@ network's output, so their pixel count needs the engine.
 second build of the library, compiled with -DCTD_REFINE_PASS_CLOCKS into --passes-dir (built there by csrc/build.sh if
 it holds no library yet; the shipped library is not touched), in which thread 0 of every k_label_local CTA adds the
 clock64() ticks between pass boundaries to a global table.  The table printed is each pass's share of the summed CTA
-ticks of the round's launch: a share of CTA residency, not of the launch's wall time.  --lib runs --gpu on another
+ticks of the round's launch: a share of CTA residency, not of the launch's wall time.  It also counts, per round, the
+word seams that runs cross (pass 1 links each to its run's first pixel; they were shared unions before) and the shared
+unions of vertical and diagonal contacts in pass 2.  --lib runs --gpu on another
 build of the library (a parent's, to alternate it with this tree's).
 
 Byte model, per window pixel and launch (HBM; the window planes of a batch are ~1 GB, far over the 50 MB L2):
@@ -92,6 +94,8 @@ def card():
 
 # g_pass_clocks[round][i] (csrc/refine_mk.cu): the merge of the round before, then the labelling's passes
 PASSES = ["merge r-1", "pass 1", "-", "pass 2", "pass 3a", "pass 3b", "pass 3c"]
+# g_pass_counts[round][i]: word seams that a run crosses, and the shared unions of vertical and diagonal contacts
+COUNTS = ["seams", "contacts"]
 
 
 def build_passes_lib(build_dir):
@@ -103,13 +107,14 @@ def build_passes_lib(build_dir):
     return lib
 
 
-def print_passes(clk, cardq):
-    print("k_label_local, share of the summed CTA clock ticks per pass and round; %s" % cardq)
-    print("%-6s %10s " % ("round", "Mticks") + " ".join("%10s" % p for p in PASSES))
+def print_passes(clk, counts, cardq):
+    print("k_label_local, share of the summed CTA clock ticks per pass and round, and union counts; %s" % cardq)
+    print("%-6s %10s " % ("round", "Mticks") + " ".join("%10s" % p for p in PASSES + COUNTS))
     for r in range(5):
         tot = float(sum(clk[r]))
         if tot > 0:
-            print("%-6d %10.1f " % (r, tot / 1e6) + " ".join("%9.1f%%" % (100.0 * c / tot) for c in clk[r][0:7]))
+            print("%-6d %10.1f " % (r, tot / 1e6) + " ".join("%9.1f%%" % (100.0 * c / tot) for c in clk[r][0:7])
+                  + " " + " ".join("%10d" % c for c in counts[r]))
 
 
 def gpu_run(n, h, w, mode, lib=None, passes=False):
@@ -135,7 +140,7 @@ def gpu_run(n, h, w, mode, lib=None, passes=False):
         torch.cuda.synchronize()
         if passes:
             import ctypes
-            clk = ((ctypes.c_ulonglong * 8) * 5)()
+            clk = (ctypes.c_ulonglong * (5 * 8 + 5 * 2))()   # ticks [5][8], then counts [5][2]
             fn = ctd_b200.binding.load_library().ctd_refine_pass_clocks
             fn(clk)   # drop the warm-up's ticks
             eng.submit_full(0, dev.data_ptr(), n, h, w, out.data_ptr(), refine_mode=mode, pages_on_device=True)
@@ -143,7 +148,8 @@ def gpu_run(n, h, w, mode, lib=None, passes=False):
             torch.cuda.synchronize()
             if fn(clk) != 0:
                 raise RuntimeError("ctd_refine_pass_clocks failed")
-            return [[int(clk[r][i]) for i in range(8)] for r in range(5)], card()
+            return ([[int(clk[8 * r + i]) for i in range(8)] for r in range(5)],
+                    [[int(clk[40 + 2 * r + i]) for i in range(2)] for r in range(5)], card())
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             eng.submit_full(0, dev.data_ptr(), n, h, w, out.data_ptr(), refine_mode=mode, pages_on_device=True)
             eng.collect(0)
@@ -186,11 +192,12 @@ def main():
     names = [k for k in MODEL if not (k == "k_dilate" and args.mode == 1)]
     if args.passes:
         with tempfile.TemporaryDirectory() as td:
-            clk, cardq = gpu_run(n, h, w, args.mode, lib=build_passes_lib(args.passes_dir or td), passes=True)
-        print_passes(clk, cardq)
+            clk, counts, cardq = gpu_run(n, h, w, args.mode, lib=build_passes_lib(args.passes_dir or td), passes=True)
+        print_passes(clk, counts, cardq)
         if args.json:
             with open(args.json, "w") as f:
-                json.dump({"shape": [n, h, w], "mode": args.mode, "card": cardq, "passes": PASSES, "ticks": clk}, f)
+                json.dump({"shape": [n, h, w], "mode": args.mode, "card": cardq, "passes": PASSES, "ticks": clk,
+                           "counts": COUNTS, "unions": counts}, f)
         return
     if not args.gpu:
         print("refine_mask byte model per window pixel (CPU model; --gpu measures the batch)")
