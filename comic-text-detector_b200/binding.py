@@ -82,7 +82,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_resize_linear_u8", "ctd_debug_run_ops", "ctd_get_nms_status", "ctd_group_output",
            "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena",
            "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
-           "ctd_submit_pages_regions", "ctd_collect_regions", "ctd_submit_pages_device", "ctd_collect_device"]
+           "ctd_submit_pages_regions", "ctd_collect_regions", "ctd_submit_pages_device", "ctd_collect_device",
+           "ctd_forward_tensor"]
 
 _lib = None
 
@@ -109,6 +110,7 @@ def load_library():
     lib.ctd_last_error.restype = C.c_char_p
     lib.ctd_forward.argtypes = [vp, vp, i32, i32, i32, i32]
     lib.ctd_get_net_outputs.argtypes = [vp, vp, vp, vp]
+    lib.ctd_forward_tensor.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp]
     lib.ctd_get_mask_u8.argtypes = [vp, vp]
     lib.ctd_get_detections.argtypes = [vp, vp, vp]
     lib.ctd_get_db_components.argtypes = [vp, vp, vp, vp]
@@ -309,6 +311,16 @@ class Engine:
     def forward_device(self, dev_ptr, n, h, w):
         """pages already resident in HBM (device pointer as int)."""
         self._ck(self.lib.ctd_forward(self.h, C.c_void_p(dev_ptr), n, h, w, 1))
+        self.shape = (n, h, w)
+
+    def forward_tensor(self, x_ptr, n, h, w, stream, blks_ptr, mask_ptr, lines_ptr):
+        """`ctd_forward_tensor`: the forward of a float32 NCHW [n][3][h][w] device tensor (pointer as int, 16-byte
+        aligned) into caller-allocated device outputs (pointers as int, or None), ordered after the work enqueued on
+        `stream` (a cudaStream_t as int; 0 is the legacy default stream), which then waits for the outputs.  No host
+        synchronisation."""
+        vp = C.c_void_p
+        self._ck(self.lib.ctd_forward_tensor(self.h, vp(x_ptr), n, h, w, vp(stream), vp(blks_ptr), vp(mask_ptr),
+                                             vp(lines_ptr)))
         self.shape = (n, h, w)
 
     def rows_per_image(self):

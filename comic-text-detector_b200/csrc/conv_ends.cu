@@ -13,6 +13,8 @@
 //             warpgroup converts its rows to the fp16 space-to-depth tile (s2d pixel (Y, X), channel (dy*2+dx)*3 + c =
 //             page(2Y+dy, 2X+dx, c) / 255, channels 12..15 zero) -> 3 filter rows x (4-pixel window x 16 channels) =
 //             K 192, the compiler's window weight order -> bias + SiLU -> fp16 NHWC slice through a TMA store.
+//             The same kernel also reads an fp16 HWC page (the staging page of a float input, ctd_forward_tensor): the
+//             box keeps its 144 elements per row (288 bytes) and the conversion copies the fp16 values as they are.
 //   seg tail  fp16 input tile (16+2) x (16+2) pixels x 64 channels, 128-byte swizzle -> 9 taps x 64 channels, the
 //             4 output channels being the sub-pixel phases of ConvT 4x4 s2 p1 -> sigmoid -> each warpgroup's 16 x 32
 //             mask pixels staged in shared memory and written as whole rows (f32 and truncated u8).
@@ -36,14 +38,15 @@ constexpr int kTile = 16;   // output tile: 16 x 16 pixels; consumer warpgroup w
 
 constexpr uint32_t align1k(uint32_t x) { return (x + 1023u) & ~1023u; }
 
-// ---- stem
-struct Stem {
+// ---- stem; P = uint8_t (the u8 pages) or __half (the fp16 staging page of a float input)
+template <typename P>
+struct StemT {
   static constexpr int kBoxRows = 2 * kTile + 4;      // page rows of a tile: s2d rows y0-1 .. y0+16
-  // bytes per page row: s2d pixels x0-1 .. x0+18 are the 120 bytes from 6*x0 - 6; the box starts 10 bytes earlier, at
-  // 6*x0 - 16, so that its innermost coordinate is 16-byte aligned
-  static constexpr int kBoxBytes = 144;
+  // elements per page row: s2d pixels x0-1 .. x0+18 are the 120 elements from 6*x0 - 6; the box starts 10 elements
+  // earlier, at 6*x0 - 16, so that its innermost coordinate is 16-byte aligned (144 bytes per row for u8, 288 for fp16)
+  static constexpr int kBoxElems = 144;
   static constexpr int kBoxSkip = 10;
-  static constexpr int kStageBytes = kBoxRows * kBoxBytes;
+  static constexpr int kStageBytes = kBoxRows * kBoxElems * int(sizeof(P));
   static constexpr int kStageStride = (kStageBytes + 127) / 128 * 128;   // TMA destinations are 128-byte aligned
   static constexpr int kStages = 4;
   static constexpr int kS2dRows = kTile / 2 + 2;      // s2d rows of one warpgroup: its 8 rows and one halo row each side
@@ -56,10 +59,10 @@ struct Stem {
   static constexpr uint32_t kIn = kStg + 2 * kStgBytes;
   static constexpr uint32_t kS2d = kIn + kStages * kStageStride;
   static constexpr uint32_t kBar = kS2d + 2 * kS2dBytes;
-  static constexpr uint32_t kLut = kBar + 256;          // fp16(u8 / 255) for the 256 byte values
-  static constexpr size_t kSmem = 1024 + kLut + 512;
+  static constexpr uint32_t kLut = kBar + 256;          // u8 pages: fp16(u8 / 255) for the 256 byte values
+  static constexpr size_t kSmem = 1024 + kLut + (sizeof(P) == 1 ? 512 : 0);
 };
-static_assert(Stem::kSmem <= 227 * 1024, "stem: shared memory");
+static_assert(StemT<uint8_t>::kSmem <= 227 * 1024 && StemT<__half>::kSmem <= 227 * 1024, "stem: shared memory");
 
 // ---- seg tail
 struct Seg {
@@ -103,7 +106,9 @@ __device__ __forceinline__ void ends_decode(const ConvEndsParams& p, int t, int&
 }
 
 // ================================================================================================ stem
+template <typename P>
 __global__ void __launch_bounds__(kThreads, 1) stem_tc_kernel(const __grid_constant__ ConvEndsParams p) {
+  using Stem = StemT<P>;
   extern __shared__ __align__(1024) uint8_t smem_ends[];
   const uint32_t base = ends_smem_base(smem_ends);
   uint8_t* const gen = smem_ends + (base - smem_u32(smem_ends));
@@ -123,9 +128,11 @@ __global__ void __launch_bounds__(kThreads, 1) stem_tc_kernel(const __grid_const
     mbar_init(w_bar, 1);
     fence_barrier_init();
   }
-  // the conversion of a page byte, as fp16(float(u8) / 255): the same expression for every byte, computed once
+  // the conversion of a page byte, as fp16(float(u8) / 255): the same expression for every byte, computed once.  An
+  // fp16 page holds fp16(x) already, which for x = float(u8) / 255 is the same table entry.
   __half* const lut = reinterpret_cast<__half*>(gen + Stem::kLut);
-  for (int i = threadIdx.x; i < 256; i += kThreads) lut[i] = __float2half_rn(float(i) / 255.0f);
+  if constexpr (sizeof(P) == 1)
+    for (int i = threadIdx.x; i < 256; i += kThreads) lut[i] = __float2half_rn(float(i) / 255.0f);
   __syncthreads();
 
   if (warp < 4) {
@@ -169,22 +176,31 @@ __global__ void __launch_bounds__(kThreads, 1) stem_tc_kernel(const __grid_const
     ends_decode(p, t, img, y0, x0);
     const int stage = it % S;
     mbar_wait(full_bar + 8 * stage, (it / S) & 1);
-    // u8 -> fp16 space-to-depth tile of this warpgroup: s2d rows y0 + 8*wg - 1 .. +8, pixels x0-1 .. x0+18.  16-byte
+    // page -> fp16 space-to-depth tile of this warpgroup: s2d rows y0 + 8*wg - 1 .. +8, pixels x0-1 .. x0+18.  16-byte
     // chunk h of pixel X sits at chunk h ^ ((X >> 2) & 1), so that ldmatrix rows (8 consecutive pixels) hit 8 distinct
     // bank groups.
     {
-      const uint8_t* in = gen + Stem::kIn + stage * Stem::kStageStride + Stem::kBoxSkip;
+      const P* in = reinterpret_cast<const P*>(gen + Stem::kIn + stage * Stem::kStageStride) + Stem::kBoxSkip;
       for (int px = tid; px < Stem::kS2dRows * Stem::kS2dCols; px += 128) {
         const int r = px / Stem::kS2dCols, c = px - r * Stem::kS2dCols;
-        const uint8_t* b0 = in + (2 * (8 * wg + r)) * Stem::kBoxBytes + 6 * c;
-        const uint8_t* b1 = b0 + Stem::kBoxBytes;
+        const P* b0 = in + (2 * (8 * wg + r)) * Stem::kBoxElems + 6 * c;
+        const P* b1 = b0 + Stem::kBoxElems;
         // channels 0..5: (dy=0, dx=0, c), (dy=0, dx=1, c); 6..11: (dy=1, dx=0, c), (dy=1, dx=1, c); 12..15: 0
         uint4 lo, hi;
         __half2 h2[8];
+        if constexpr (sizeof(P) == 1) {
 #pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          h2[k] = __halves2half2(lut[b0[2 * k]], lut[b0[2 * k + 1]]);
-          h2[3 + k] = __halves2half2(lut[b1[2 * k]], lut[b1[2 * k + 1]]);
+          for (int k = 0; k < 3; ++k) {
+            h2[k] = __halves2half2(lut[b0[2 * k]], lut[b0[2 * k + 1]]);
+            h2[3 + k] = __halves2half2(lut[b1[2 * k]], lut[b1[2 * k + 1]]);
+          }
+        } else {
+          // element offsets 10 + 144 * row + 6 * c are even: 4-byte aligned pairs
+#pragma unroll
+          for (int k = 0; k < 3; ++k) {
+            h2[k] = reinterpret_cast<const __half2*>(b0)[k];
+            h2[3 + k] = reinterpret_cast<const __half2*>(b1)[k];
+          }
         }
         h2[6] = h2[7] = __floats2half2_rn(0.f, 0.f);
         memcpy(&lo, &h2[0], 16);
@@ -399,9 +415,9 @@ __global__ void __launch_bounds__(kThreads, 1) seg_tc_kernel(const __grid_consta
 // =========================================================================================
 // host side
 
-const char* conv_ends_plan_stem(ConvEndsPlan& plan, PFN_encodeTiled enc, const uint8_t* pages, int n, int ph, int pw,
-                                const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff,
-                                int cout, int act) {
+const char* conv_ends_plan_stem(ConvEndsPlan& plan, PFN_encodeTiled enc, const void* pages, bool f16_page, int n,
+                                int ph, int pw, const void* w16, const float* bias, __half* dst, int dst_cstride,
+                                int dst_coff, int cout, int act) {
   ConvEndsParams& p = plan.p;
   memset(&p, 0, sizeof(p));
   if (act != CTD_ACT_SILU) return "stem: the tensor-core stem fuses SiLU only";
@@ -416,12 +432,14 @@ const char* conv_ends_plan_stem(ConvEndsPlan& plan, PFN_encodeTiled enc, const u
   p.bias = bias;
   const cuuint32_t e1[3] = {1, 1, 1};
   {
+    using Stem = StemT<uint8_t>;   // the box in elements is the same for both page types
+    const cuuint64_t es = f16_page ? 2 : 1;
     const cuuint64_t dims[3] = {cuuint64_t(pw) * 3, cuuint64_t(ph), cuuint64_t(n)};
-    const cuuint64_t str[2] = {cuuint64_t(pw) * 3, cuuint64_t(pw) * 3 * ph};
-    const cuuint32_t box[3] = {Stem::kBoxBytes, Stem::kBoxRows, 1};
-    if (enc(&p.a_map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, const_cast<uint8_t*>(pages), dims, str, box, e1,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    const cuuint64_t str[2] = {cuuint64_t(pw) * 3 * es, cuuint64_t(pw) * 3 * ph * es};
+    const cuuint32_t box[3] = {Stem::kBoxElems, Stem::kBoxRows, 1};
+    if (enc(&p.a_map, f16_page ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, 3,
+            const_cast<void*>(pages), dims, str, box, e1, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+            CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
       return "stem: page tensor map";
   }
   {
@@ -446,9 +464,9 @@ const char* conv_ends_plan_stem(ConvEndsPlan& plan, PFN_encodeTiled enc, const u
       return "stem: destination tensor map";
   }
   const int total = n * p.tiles_x * p.tiles_y;
-  plan.kind = CTD_END_STEM;
+  plan.kind = f16_page ? CTD_END_STEM_F16 : CTD_END_STEM;
   plan.grid = dim3(unsigned(total < g_sms ? total : g_sms), 1, 1);
-  plan.smem_bytes = Stem::kSmem;
+  plan.smem_bytes = f16_page ? StemT<__half>::kSmem : StemT<uint8_t>::kSmem;
   return nullptr;
 }
 
@@ -501,13 +519,18 @@ cudaError_t conv_ends_init() {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) g_sms = n;
   }
-  cudaError_t e = cudaFuncSetAttribute(stem_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(Stem::kSmem));
+  cudaError_t e = cudaFuncSetAttribute(stem_tc_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       int(StemT<uint8_t>::kSmem));
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(stem_tc_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           int(StemT<__half>::kSmem));
   if (e != cudaSuccess) return e;
   return cudaFuncSetAttribute(seg_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, int(Seg::kSmem));
 }
 
 cudaError_t conv_ends_launch(const ConvEndsPlan& plan, cudaStream_t s) {
-  if (plan.kind == CTD_END_STEM) stem_tc_kernel<<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p);
+  if (plan.kind == CTD_END_STEM) stem_tc_kernel<uint8_t><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p);
+  else if (plan.kind == CTD_END_STEM_F16) stem_tc_kernel<__half><<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p);
   else if (plan.kind == CTD_END_SEG) seg_tc_kernel<<<plan.grid, kThreads, plan.smem_bytes, s>>>(plan.p);
   else return cudaErrorInvalidValue;
   return cudaGetLastError();

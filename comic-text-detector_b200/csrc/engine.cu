@@ -58,7 +58,7 @@ extern "C" void ctd_destroy(ctd_handle* h) {
   cudaFree(h->d_blob); cudaFree(h->d_pages); cudaFree(h->d_blks); cudaFree(h->d_mask); cudaFree(h->d_mask_u8);
   cudaFree(h->d_lines); cudaFree(h->d_bitmap); cudaFree(h->d_labels);
   cudaFree(h->d_ccl_scratch); cudaFree(h->d_nms_ws); cudaFree(h->d_segrep_scratch);
-  h->refine_scratch.release(); h->cc_scratch.release(); h->io_scratch.release();
+  h->refine_scratch.release(); h->cc_scratch.release(); h->io_scratch.release(); h->in_stage.release();
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->tev0) cudaEventDestroy(h->tev0);
@@ -70,6 +70,8 @@ extern "C" void ctd_destroy(ctd_handle* h) {
   if (h->ev_fork2) cudaEventDestroy(h->ev_fork2);
   if (h->ev_xjoin) cudaEventDestroy(h->ev_xjoin);
   if (h->ev_join2) cudaEventDestroy(h->ev_join2);
+  if (h->ev_tin) cudaEventDestroy(h->ev_tin);
+  if (h->ev_tout) cudaEventDestroy(h->ev_tout);
   if (h->side) cudaStreamDestroy(h->side);
   if (h->side2) cudaStreamDestroy(h->side2);
   if (h->copy_in) cudaStreamDestroy(h->copy_in);
@@ -151,6 +153,8 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
   CKC(cudaEventCreateWithFlags(&h->ev_fork2, cudaEventDisableTiming));
   CKC(cudaEventCreateWithFlags(&h->ev_xjoin, cudaEventDisableTiming));
   CKC(cudaEventCreateWithFlags(&h->ev_join2, cudaEventDisableTiming));
+  CKC(cudaEventCreateWithFlags(&h->ev_tin, cudaEventDisableTiming));
+  CKC(cudaEventCreateWithFlags(&h->ev_tout, cudaEventDisableTiming));
   CKC(cudaEventCreate(&h->ev0));
   CKC(cudaEventCreate(&h->ev1));
   CKC(cudaEventCreate(&h->tev0));
@@ -322,10 +326,12 @@ static int build_plans(ctd_handle* h, int n, int ph, int pw, ShapePlan& sp) {
     const float* bias = reinterpret_cast<const float*>(h->d_blob + op.b_off);
     const char* e = nullptr;
     if (op.kind == CTD_OP_STEM) {
-      // reads the u8 pages itself: the space-to-depth form is built per tile in shared memory
-      e = conv_ends_plan_stem(sp.ends[i], h->enc, h->d_pages, n, ph, pw, h->d_blob + op.w16_off, bias,
-                              static_cast<__half*>(h->d_buf[op.dst_buf]), h->bufs[op.dst_buf].channels, op.dst_coff,
-                              op.cout, op.act);
+      // reads the u8 pages (or the fp16 staging page of a float input) itself: the space-to-depth form is built per
+      // tile in shared memory
+      const bool f16 = sp.input == INPUT_F32;
+      e = conv_ends_plan_stem(sp.ends[i], h->enc, f16 ? static_cast<const void*>(h->in_stage.p) : h->d_pages, f16, n,
+                              ph, pw, h->d_blob + op.w16_off, bias, static_cast<__half*>(h->d_buf[op.dst_buf]),
+                              h->bufs[op.dst_buf].channels, op.dst_coff, op.cout, op.act);
     } else if (op.kind == CTD_OP_SEG_TAIL) {
       // the final ConvT 4x4 s2 (C -> 1) as a 3x3 convolution whose 4 output channels are the sub-pixel phases, with
       // the sigmoid / u8-mask epilogue
@@ -370,17 +376,25 @@ static int run_op_simt(ctd_handle* h, size_t i, int n, int ph, int pw) {
 }
 
 template <typename T>
-static int run_op_thin(ctd_handle* h, const ctd_op& op, int n, int ph, int pw) {
+static int run_op_thin(ctd_handle* h, const ctd_op& op, int n, int ph, int pw, int input) {
   cudaStream_t s = h->stream;
   const ctd_bufdesc* sb = op.kind == CTD_OP_STEM ? nullptr : &h->bufs[op.src_buf[0]];
   const int sh = sb ? ph / sb->down : ph, sw = sb ? pw / sb->down : pw;
   const T* src = sb ? static_cast<const T*>(h->d_buf[op.src_buf[0]]) + op.src_coff[0] : nullptr;
   switch (op.kind) {
-    case CTD_OP_STEM:
-      CK(stem_launch<T>(h->d_pages, n, ph, pw, reinterpret_cast<const float*>(h->d_blob + op.w32_off),
-                        reinterpret_cast<const float*>(h->d_blob + op.b_off), static_cast<T*>(h->d_buf[op.dst_buf]),
-                        h->bufs[op.dst_buf].channels, op.dst_coff, op.cout, op.act, s));
+    case CTD_OP_STEM: {
+      const float* w = reinterpret_cast<const float*>(h->d_blob + op.w32_off);
+      const float* b = reinterpret_cast<const float*>(h->d_blob + op.b_off);
+      T* dst = static_cast<T*>(h->d_buf[op.dst_buf]);
+      const int dc = h->bufs[op.dst_buf].channels;
+      if (input == INPUT_U8) {
+        CK(stem_launch<T>(h->d_pages, n, ph, pw, w, b, dst, dc, op.dst_coff, op.cout, op.act, s));
+      } else {   // the f32 staging page: the fp16 tensor-core engine runs its stem in stem_tc_kernel
+        CK(stem_launch<T>(reinterpret_cast<const float*>(h->in_stage.p), n, ph, pw, w, b, dst, dc, op.dst_coff,
+                          op.cout, op.act, s));
+      }
       return CTD_OK;
+    }
     case CTD_OP_AVGPOOL2:
       CK(avgpool2_launch<T>(src, n, sh, sw, op.src_c[0], sb->channels,
                             static_cast<T*>(h->d_buf[op.dst_buf]) + op.dst_coff, h->bufs[op.dst_buf].channels, s));
@@ -430,7 +444,7 @@ static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, const Shap
   } else if (is_gemm(op.kind)) {
     rc = h->elem == 4 ? run_op_simt<float>(h, i, n, ph, pw) : run_op_simt<__half>(h, i, n, ph, pw);
   } else {
-    rc = h->elem == 4 ? run_op_thin<float>(h, op, n, ph, pw) : run_op_thin<__half>(h, op, n, ph, pw);
+    rc = h->elem == 4 ? run_op_thin<float>(h, op, n, ph, pw, sp.input) : run_op_thin<__half>(h, op, n, ph, pw, sp.input);
   }
   ++*cnt;
   if (rc || h->d_buf16.empty()) return rc;
@@ -509,16 +523,25 @@ static int run_ops(ctd_handle* h, int n, int ph, int pw, const ShapePlan& sp, in
   return CTD_OK;
 }
 
-// shape checks + the launch plans of (n, ph, pw), built on first use
-static int find_plan(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out) {
+// bytes per element of ctd_forward_tensor's staging page: fp16 for the fp16 tensor-core stem, f32 for the CUDA-core stem
+static size_t stage_elem(const ctd_handle* h) { return h->cfg.precision == CTD_PREC_FP16_TC ? 2 : 4; }
+
+// shape checks + the launch plans of (n, ph, pw, input), built on first use
+static int find_plan(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out, int input = INPUT_U8) {
   if (n < 1 || n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
   if (ph % 64 || pw % 64 || ph > h->cfg.max_h || pw > h->cfg.max_w || ph < 64 || pw < 64)
     return ctd_fail(h, CTD_E_SHAPE, "page %dx%d must be a multiple of 64 and <= %dx%d", ph, pw, h->cfg.max_h, h->cfg.max_w);
   CK(cudaSetDevice(h->cfg.device));
-  auto key = std::make_tuple(int(n), int(ph), int(pw));
+  auto key = std::make_tuple(int(n), int(ph), int(pw), input);
   auto it = h->plans.find(key);
   if (it == h->plans.end()) {
     ShapePlan sp;
+    sp.input = input;
+    if (input == INPUT_F32) {
+      // the whole workspace at once: the page never moves, so every plan's tensor map and captured graph stays valid
+      const size_t bytes = size_t(h->cfg.max_batch) * h->cfg.max_h * h->cfg.max_w * 3 * stage_elem(h);
+      if (int rc = h->in_stage.grow(h, bytes, std::nullopt, size_t(1) << 40)) return rc;
+    }
     if (int rc = build_plans(h, n, ph, pw, sp)) return rc;
     it = h->plans.emplace(key, std::move(sp)).first;
   }
@@ -527,9 +550,9 @@ static int find_plan(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan
 }
 
 // plan lookup + (first time, use_graph) graph capture; the forward itself is enqueue_forward()
-int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out) {
+int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out, int input) {
   ShapePlan* sp = nullptr;
-  if (int rc = find_plan(h, n, ph, pw, &sp)) return rc;
+  if (int rc = find_plan(h, n, ph, pw, &sp, input)) return rc;
   if (h->cfg.use_graph && !sp->graph) {
     cudaGraph_t graph;
     CK(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
@@ -567,6 +590,32 @@ extern "C" int ctd_forward(ctd_handle* h, const uint8_t* pages, int32_t n, int32
   CK(cudaMemcpyAsync(h->d_pages, pages, bytes, pages_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
                      h->stream));
   return enqueue_forward(h, n, ph, pw, *sp);
+}
+
+extern "C" int ctd_forward_tensor(ctd_handle* h, const float* x, int32_t n, int32_t ph, int32_t pw, void* stream,
+                                  float* blks, float* mask, float* lines) {
+  if (!h || !x) return CTD_E_INVALID;
+  if (reinterpret_cast<uintptr_t>(x) % 16) return ctd_fail(h, CTD_E_INVALID, "x must be 16-byte aligned");
+  ShapePlan* sp = nullptr;
+  if (int rc = prepare_forward(h, n, ph, pw, &sp, INPUT_F32)) return rc;
+  cudaStream_t cs = static_cast<cudaStream_t>(stream);
+  CK(cudaEventRecord(h->ev_tin, cs));   // x and the outputs are ready for the engine once the caller's work so far ran
+  CK(cudaStreamWaitEvent(h->stream, h->ev_tin, 0));
+  CK(cudaEventRecord(h->ev0, h->stream));
+  if (stage_elem(h) == 2)
+    CK(nchw_to_hwc_launch(x, n, ph, pw, reinterpret_cast<__half*>(h->in_stage.p), h->stream));
+  else
+    CK(nchw_to_hwc_launch(x, n, ph, pw, reinterpret_cast<float*>(h->in_stage.p), h->stream));
+  if (int rc = enqueue_forward(h, n, ph, pw, *sp)) return rc;
+  const size_t px = size_t(n) * ph * pw;
+  if (blks)
+    CK(cudaMemcpyAsync(blks, h->d_blks, size_t(n) * rows_per_image(ph, pw) * (5 + h->cfg.nc) * 4,
+                       cudaMemcpyDeviceToDevice, h->stream));
+  if (mask) CK(cudaMemcpyAsync(mask, h->d_mask, px * 4, cudaMemcpyDeviceToDevice, h->stream));
+  if (lines) CK(cudaMemcpyAsync(lines, h->d_lines, px * 8, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaEventRecord(h->ev_tout, h->stream));
+  CK(cudaStreamWaitEvent(cs, h->ev_tout, 0));
+  return CTD_OK;
 }
 
 // ---- pipelined host path ---------------------------------------------------------------------------

@@ -187,7 +187,12 @@ struct RegionJob {
   void write_tables(char* dst) const;
 };
 
+// what the stem of a plan reads: the u8 pages (d_pages), or the staging page ctd_forward_tensor's pre-pass writes from
+// a float NCHW tensor (in_stage: fp16 in CTD_PREC_FP16_TC, f32 in the other precisions)
+enum { INPUT_U8 = 0, INPUT_F32 = 1 };
+
 struct ShapePlan {
+  int input = INPUT_U8;
   std::vector<ConvTcPlan> tc;  // index = op index; block_n == 0: the op does not run conv_tc_kernel
   std::vector<ConvEndsPlan> ends;   // index = op index; kind != CTD_END_NONE: the tensor-core stem or seg tail
   cudaGraphExec_t graph = nullptr;
@@ -234,7 +239,11 @@ struct ctd_handle {
   int32_t* d_line_count = nullptr;
   void* d_nms_ws = nullptr;
   NmsWorkspace nms{};
-  std::map<std::tuple<int, int, int>, ShapePlan> plans;
+  std::map<std::tuple<int, int, int, int>, ShapePlan> plans;   // key (n, ph, pw, input)
+  // ctd_forward_tensor: the staging page (allocated at its full size on first use, so the plans' tensor maps stay
+  // valid), and the events that order the engine stream after the caller's stream and back
+  DevBuf in_stage;
+  cudaEvent_t ev_tin = nullptr, ev_tout = nullptr;
   // pipelined host path (ctd_submit / ctd_collect): two slots, copy streams either side of compute
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
   Slot slot[2];
@@ -269,7 +278,7 @@ struct ctd_handle {
 
 
 int ctd_fail(ctd_handle* h, int code, const char* fmt, ...);
-int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out);
+int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out, int input = INPUT_U8);
 int enqueue_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan& sp);
 int ensure_pipeline(ctd_handle* h);
 // phase A of a batch of n net-sized pages on slot s, enqueued on the copy streams and the engine stream: the pages

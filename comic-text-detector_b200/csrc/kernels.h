@@ -108,9 +108,9 @@ cudaError_t conv_tc_init();  // sets max dynamic smem attributes once
 // ---------------------------------------------------------------------------------------
 // The network's two ends on the tensor cores (conv_ends.cu): the stem, reading the u8 pages itself, and the seg tail.
 // Each 16x16-pixel output tile loads its input region once, halo included, into shared memory.
-enum { CTD_END_NONE = 0, CTD_END_STEM = 1, CTD_END_SEG = 2 };
+enum { CTD_END_NONE = 0, CTD_END_STEM = 1, CTD_END_SEG = 2, CTD_END_STEM_F16 = 3 };
 struct alignas(64) ConvEndsParams {
-  CUtensorMap a_map;   // stem: u8 pages {3*pw, ph, n}; seg tail: its fp16 NHWC input {64, gw, gh, n}
+  CUtensorMap a_map;   // stem: u8 or fp16 pages {3*pw, ph, n}; seg tail: its fp16 NHWC input {64, gw, gh, n}
   CUtensorMap b_map;   // fp16 K-major weights: stem [32][192], seg tail [16][576]
   CUtensorMap d_map;   // stem: fp16 NHWC destination slice {cout, gw, gh, n}
   int n_img, gh, gw;   // output grid (seg tail: input grid; the mask is 2gh x 2gw)
@@ -125,12 +125,13 @@ struct ConvEndsPlan {
   dim3 grid;
   size_t smem_bytes;
 };
-// Stem: Conv 6x6 s2 p2 (3 -> cout <= 32) + SiLU over the u8 BGR pages [n][ph][pw][3], in the space-to-depth window
-// form of the compiler's weights `w16` ([32][3 rows][4 pixels][16 channels] fp16, K = 192); output
-// [n][ph/2][pw/2][dst_cstride] fp16 at channel offset dst_coff.
-const char* conv_ends_plan_stem(ConvEndsPlan& plan, PFN_encodeTiled enc, const uint8_t* pages, int n, int ph, int pw,
-                                const void* w16, const float* bias, __half* dst, int dst_cstride, int dst_coff,
-                                int cout, int act);
+// Stem: Conv 6x6 s2 p2 (3 -> cout <= 32) + SiLU over the BGR pages [n][ph][pw][3] (u8, read as u8 / 255; or, with
+// f16_page, fp16 values used as they are), in the space-to-depth window form of the compiler's weights `w16`
+// ([32][3 rows][4 pixels][16 channels] fp16, K = 192); output [n][ph/2][pw/2][dst_cstride] fp16 at channel offset
+// dst_coff.
+const char* conv_ends_plan_stem(ConvEndsPlan& plan, PFN_encodeTiled enc, const void* pages, bool f16_page, int n,
+                                int ph, int pw, const void* w16, const float* bias, __half* dst, int dst_cstride,
+                                int dst_coff, int cout, int act);
 // Seg tail: ConvT 4x4 s2 p1 (64 -> 1) + sigmoid as a 3x3 convolution whose 4 output channels are the sub-pixel phases
 // (weights `w16` [16][9 taps][64] fp16, rows 4..15 zero) over the fp16 NHWC input (64 channels at src_coff of a
 // src_cstride-channel buffer, gh x gw); writes the f32 and truncated-u8 masks [n][2gh][2gw].
@@ -156,9 +157,15 @@ struct ConvSimtParams {
 template <typename T>
 cudaError_t conv_simt_launch(const ConvSimtParams& p, cudaStream_t s);
 
-template <typename T>
-cudaError_t stem_launch(const uint8_t* pages, int n, int h, int w, const float* wgt /*[32][108] (ky,kx,c)*/,
+// P = uint8_t: u8 pages, each value read as float(u) / 255; P = float: the f32 staging page of a float input, read as
+// it is
+template <typename T, typename P>
+cudaError_t stem_launch(const P* pages, int n, int h, int w, const float* wgt /*[32][108] (ky,kx,c)*/,
                         const float* bias, T* dst, int dst_cstride, int dst_coff, int cout, int act, cudaStream_t s);
+// the input pre-pass of ctd_forward_tensor: f32 NCHW [n][3][h][w] -> the HWC staging page [n][h][w][3] of element S
+// (__half: round to nearest; float: a copy)
+template <typename S>
+cudaError_t nchw_to_hwc_launch(const float* x, int n, int h, int w, S* dst, cudaStream_t s);
 // fp32 NHWC channel slice -> fp16 hi / lo planes (split-fp16 mode): hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale).
 // src / hi / lo point at the first channel of the slice; `cstride` elements between pixels (same in all three).
 cudaError_t split_planes_launch(const float* src, __half* hi, __half* lo, size_t npix, int c, int cstride,

@@ -169,9 +169,13 @@ template cudaError_t conv_simt_launch<float>(const ConvSimtParams&, cudaStream_t
 template cudaError_t conv_simt_launch<__half>(const ConvSimtParams&, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------
-// stem: Conv 6x6 s2 p2, 3 -> cout(32), reads the u8 BGR HWC page, fuses /255 (inference.py:78)
-template <typename T>
-__global__ void __launch_bounds__(256) stem_kernel(const uint8_t* __restrict__ pages, int n, int h, int w,
+// stem: Conv 6x6 s2 p2, 3 -> cout(32), reads the BGR HWC page: u8 with the /255 fused (inference.py:78), or the f32
+// staging page of a float input as it is
+__device__ __forceinline__ float page_value(const uint8_t* p) { return float(*p) / 255.0f; }
+__device__ __forceinline__ float page_value(const float* p) { return *p; }
+
+template <typename T, typename P>
+__global__ void __launch_bounds__(256) stem_kernel(const P* __restrict__ pages, int n, int h, int w,
                                                    const float* __restrict__ wgt, const float* __restrict__ bias,
                                                    T* __restrict__ dst, int dst_cstride, int dst_coff, int cout,
                                                    int act) {
@@ -193,13 +197,13 @@ __global__ void __launch_bounds__(256) stem_kernel(const uint8_t* __restrict__ p
     ws[i] = co < cout ? wgt[co * 108 + k] : 0.f;
   }
   if (threadIdx.x < 32) bs[threadIdx.x] = threadIdx.x < cout ? bias[threadIdx.x] : 0.f;
-  const uint8_t* page = pages + size_t(img) * h * w * 3;
+  const P* page = pages + size_t(img) * h * w * 3;
   for (int i = threadIdx.x; i < PH * PW * 3; i += 256) {
     const int py = i / (PW * 3), rem = i - py * (PW * 3);
     const int px = rem / 3, c = rem - px * 3;
     const int iy = iy0 + py, ix = ix0 + px;
     float v = 0.f;
-    if (iy >= 0 && iy < h && ix >= 0 && ix < w) v = float(page[(size_t(iy) * w + ix) * 3 + c]) / 255.0f;
+    if (iy >= 0 && iy < h && ix >= 0 && ix < w) v = page_value(page + (size_t(iy) * w + ix) * 3 + c);
     patch[py][rem] = v;
   }
   __syncthreads();
@@ -222,19 +226,65 @@ __global__ void __launch_bounds__(256) stem_kernel(const uint8_t* __restrict__ p
   }
 }
 
-template <typename T>
-cudaError_t stem_launch(const uint8_t* pages, int n, int h, int w, const float* wgt, const float* bias, T* dst,
+template <typename T, typename P>
+cudaError_t stem_launch(const P* pages, int n, int h, int w, const float* wgt, const float* bias, T* dst,
                         int dst_cstride, int dst_coff, int cout, int act, cudaStream_t s) {
   if (cout > 32) return cudaErrorInvalidValue;
   const int oh = h / 2, ow = w / 2;
   const int tiles = ((ow + 31) / 32) * ((oh + 7) / 8);
-  stem_kernel<T><<<n * tiles, 256, 0, s>>>(pages, n, h, w, wgt, bias, dst, dst_cstride, dst_coff, cout, act);
+  stem_kernel<T, P><<<n * tiles, 256, 0, s>>>(pages, n, h, w, wgt, bias, dst, dst_cstride, dst_coff, cout, act);
   return cudaGetLastError();
 }
-template cudaError_t stem_launch<float>(const uint8_t*, int, int, int, const float*, const float*, float*, int, int,
-                                        int, int, cudaStream_t);
-template cudaError_t stem_launch<__half>(const uint8_t*, int, int, int, const float*, const float*, __half*, int, int,
-                                         int, int, cudaStream_t);
+template cudaError_t stem_launch<float, uint8_t>(const uint8_t*, int, int, int, const float*, const float*, float*, int,
+                                                 int, int, int, cudaStream_t);
+template cudaError_t stem_launch<__half, uint8_t>(const uint8_t*, int, int, int, const float*, const float*, __half*,
+                                                  int, int, int, int, cudaStream_t);
+template cudaError_t stem_launch<float, float>(const float*, int, int, int, const float*, const float*, float*, int,
+                                               int, int, int, cudaStream_t);
+template cudaError_t stem_launch<__half, float>(const float*, int, int, int, const float*, const float*, __half*, int,
+                                                int, int, int, cudaStream_t);
+
+// ---------------------------------------------------------------------------------------
+// input pre-pass: f32 NCHW -> HWC staging page.  One thread per 4 pixels (h * w is a multiple of 4096): three float4
+// plane loads, then the 12 values of the 4 pixels as three 16-byte (f32) or 8-byte (fp16) stores.
+__device__ __forceinline__ void st_hwc4(float* d, const float (&v)[12]) {
+  float4* o = reinterpret_cast<float4*>(d);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) o[k] = make_float4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
+}
+__device__ __forceinline__ void st_hwc4(__half* d, const float (&v)[12]) {
+  uint2* o = reinterpret_cast<uint2*>(d);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const __half2 a = __floats2half2_rn(v[4 * k], v[4 * k + 1]), b = __floats2half2_rn(v[4 * k + 2], v[4 * k + 3]);
+    uint2 u;
+    memcpy(&u.x, &a, 4);
+    memcpy(&u.y, &b, 4);
+    o[k] = u;
+  }
+}
+
+template <typename S>
+__global__ void __launch_bounds__(256) nchw_to_hwc_kernel(const float* __restrict__ x, size_t hw4, size_t total4,
+                                                          S* __restrict__ dst) {
+  const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
+  if (i >= total4) return;
+  const size_t img = i / hw4, q = i - img * hw4;
+  const float4* src = reinterpret_cast<const float4*>(x) + img * 3 * hw4 + q;
+  const float4 b = __ldcs(src), g = __ldcs(src + hw4), r = __ldcs(src + 2 * hw4);
+  const float v[12] = {b.x, g.x, r.x, b.y, g.y, r.y, b.z, g.z, r.z, b.w, g.w, r.w};
+  st_hwc4(dst + i * 12, v);
+}
+
+template <typename S>
+cudaError_t nchw_to_hwc_launch(const float* x, int n, int h, int w, S* dst, cudaStream_t s) {
+  if ((size_t(h) * w) % 4) return cudaErrorInvalidValue;
+  const size_t hw4 = size_t(h) * w / 4, total4 = size_t(n) * hw4;
+  nchw_to_hwc_kernel<S><<<unsigned((total4 + 255) / 256), 256, 0, s>>>(x, hw4, total4, dst);
+  return cudaGetLastError();
+}
+template cudaError_t nchw_to_hwc_launch<float>(const float*, int, int, int, float*, cudaStream_t);
+template cudaError_t nchw_to_hwc_launch<__half>(const float*, int, int, int, __half*, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------
 template <typename T>

@@ -142,6 +142,20 @@ CTD_API int ctd_forward(ctd_handle* h, const uint8_t* pages, int32_t n, int32_t 
  * Any pointer may be NULL to skip it.                                                      */
 CTD_API int ctd_get_net_outputs(ctd_handle* h, float* blks, float* mask, float* lines);
 
+/* `TextDetBase.forward(img_in) -> (blks, mask, lines_map)` (basemodel.py:240-244) on DEVICE memory, in stream order.
+ * x     : DEVICE f32 [n][3][ph][pw], contiguous NCHW, 16-byte aligned: the BGR tensor preprocess_img makes (values
+ *         in [0, 1] for a page; any float is taken).  The engine reads it as it is, rounded to fp16 in
+ *         CTD_PREC_FP16_TC and exact in the other precisions; for x = float(u8) / 255 the outputs are bit-identical
+ *         to ctd_forward on the u8 pages.
+ * stream: the caller's cudaStream_t (NULL: the legacy default stream).  The engine stream first waits for the work
+ *         enqueued on it so far, then runs an input pre-pass into the engine's staging page, the forward (its CUDA
+ *         graph with use_graph), and device-to-device copies into blks / mask / lines (DEVICE, the layouts of
+ *         ctd_get_net_outputs; any may be NULL to skip it); `stream` then waits for those copies.  No host
+ *         synchronisation.  Post-processing runs as ctd_config::debug_skip_postproc says.  Shape and batch limits are
+ *         ctd_forward's.                                                                        */
+CTD_API int ctd_forward_tensor(ctd_handle* h, const float* x, int32_t n, int32_t ph, int32_t pw, void* stream,
+                               float* blks, float* mask, float* lines);
+
 /* `postprocess_mask` (inference.py:85-99): (mask*255) truncated to u8, [n][h][w], HOST.   */
 CTD_API int ctd_get_mask_u8(ctd_handle* h, uint8_t* mask_u8);
 
