@@ -296,7 +296,9 @@ __global__ void __launch_bounds__(kThreads) k_phase0(Ctx c) {
       bool core = false;
       if (in) {
         const int i = v.i0 + k;
-        gr = (b[u] * 1868 + g[u] * 9617 + r[u] * 4899 + 8192) >> 14;  // cv2.COLOR_BGR2GRAY, 8u fixed point
+        // cv2.COLOR_BGR2GRAY on 8u (OpenCV 4.13): 15-bit fixed point, equal to cv2 on all 2^24 colours.  The 14-bit
+        // coefficients (1868, 9617, 4899) differ by one grey level on 43 864 of them.
+        gr = (b[u] * 3735 + g[u] * 19235 + r[u] * 9798 + 16384) >> 15;
         grey[i] = (uint8_t)gr;
         core = !((F127[k >> 5] >> (k & 31)) & 1u);                       // 3x3 erosion > 127 (textmask.py:60)
       }
@@ -993,9 +995,11 @@ __global__ void __launch_bounds__(kThreads) k_decide_roots(Ctx c, int round) {
     const int a = area[g];
     bool ok;
     if (round < 4) {
-      // `if w * h < 3: continue` (textmask.py:97): bounding boxes 1x1, 1x2, 2x1
+      // `if w * h < 3: continue` (textmask.py:97): bounding boxes 1x1, 1x2, 2x1.  g and mx are the first and last
+      // pixel; a horizontal pair is mx == g + 1 in ONE row (in a window 2 px wide an anti-diagonal pair, a 2x2 box,
+      // is mx == g + 1 too, across a row end)
       const int mx = maxi[g];
-      ok = !(a == 1 || (a == 2 && (mx == g + 1 || mx == g + v.rw)));
+      ok = !(a == 1 || (a == 2 && ((mx == g + 1 && mx % v.rw != 0) || mx == g + v.rw)));
     } else {
       ok = a < thresh;  // textmask.py:120
     }

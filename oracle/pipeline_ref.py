@@ -8,8 +8,9 @@ import torch
 from oracle import postproc_ref
 
 
-def refine_undetected_mask(img, mask_pred, mask_refined, blk_xyxy, make_window_list, refine_mode, tie_order="stable"):
-    """utils/textmask.py:135-156 (mutates mask_pred in place like the reference)."""
+def undetected_blocks(mask_pred, mask_refined, blk_xyxy):
+    """utils/textmask.py:136-153: the blocks of refine_undetected_mask's second refine_mask (mutates mask_pred in place
+    like the reference)."""
     import cv2
     mask_pred[np.where(mask_refined > 30)] = 0
     _, pred_t = cv2.threshold(mask_pred, 30, 255, cv2.THRESH_BINARY)
@@ -28,6 +29,13 @@ def refine_undetected_mask(img, mask_pred, mask_refined, blk_xyxy, make_window_l
                     score = s
             if score / w / h < 0.5:
                 extra.append([int(v) for v in bbox])
+    return extra
+
+
+def refine_undetected_mask(img, mask_pred, mask_refined, blk_xyxy, make_window_list, refine_mode, tie_order="stable"):
+    """utils/textmask.py:135-156 (mutates mask_pred in place like the reference)."""
+    import cv2
+    extra = undetected_blocks(mask_pred, mask_refined, blk_xyxy)
     if len(extra) > 0:
         mask_refined = cv2.bitwise_or(mask_refined, postproc_ref.refine_mask(img, mask_pred, extra, refine_mode, tie_order))
     return mask_refined

@@ -89,10 +89,8 @@ def test_letterbox_kernel_equals_host_letterbox(det):
 
 def test_batched_page_matches_oracle_at_page_scale(det):
     # oracle chain for a non-net-sized page that never goes through ctd_detect_page: host letterbox -> engine forward ->
-    # oracle post-processing at the page's scale, against the batched result for that page.  (With
-    # keep_undetected_mask this page's mask_refined differs from the oracle in 1 pixel: the refine of one of the extra
-    # windows, DESIGN section 4, for ctd_detect_page as much as for the batch; the batch is pinned to ctd_detect_page.)
-    keep = False
+    # oracle post-processing at the page's scale, against the batched result for that page, with refine_undetected_mask
+    keep = True
     pages = _pages([(1654 * NET // 1024, 1170 * NET // 1024), (NET, NET)], seed=42)
     page = pages[0]
     got = det.detect_batch([p.copy() for p in pages], refine_mode=1, keep_undetected_mask=keep)[0]
