@@ -6,3 +6,4 @@ from .binding import Engine, CtdError, load_library, LIB_PATH  # noqa: F401
 from . import binding, multigpu, onnx_model, textblock  # noqa: F401
 from .inference import TextDetector, REFINEMASK_INPAINT, REFINEMASK_ANNOTATION  # noqa: F401
 from .basemodel import TextDetBase  # noqa: F401
+from .jpeg import JpegDecoder, jpeg_probe  # noqa: F401

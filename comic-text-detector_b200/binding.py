@@ -67,6 +67,13 @@ REGION_DTYPE = np.dtype([("out_h", np.int32), ("out_w", np.int32), ("rotate", np
                         align=True)
 
 
+class CtdJpegInfo(C.Structure):
+    """ctypes mirror of `ctd_jpeg_info` (include/ctd_b200.h)"""
+    _fields_ = [(k, C.c_int32) for k in ("status", "height", "width", "frame_height", "frame_width", "components",
+                                         "h_samp", "v_samp", "orientation", "restart_interval")] + \
+               [("ecs_bytes", C.c_int64)]
+
+
 class CtdDevicePage(C.Structure):
     """ctypes mirror of `ctd_device_page` (include/ctd_b200.h)"""
     _fields_ = [("data", C.c_void_p), ("stride_h", C.c_int64), ("stride_w", C.c_int64), ("stride_c", C.c_int64),
@@ -83,7 +90,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena",
            "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
            "ctd_submit_pages_regions", "ctd_collect_regions", "ctd_submit_pages_device", "ctd_collect_device",
-           "ctd_forward_tensor"]
+           "ctd_forward_tensor", "ctd_jpeg_probe", "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy",
+           "ctd_jpeg_decode"]
 
 _lib = None
 
@@ -151,8 +159,13 @@ def load_library():
                                         C.POINTER(C.c_size_t)]
     lib.ctd_submit_pages_device.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_collect_device.argtypes = [vp, i32, vp]
+    lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
+    lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
+    lib.ctd_jpeg_decoder_destroy.argtypes = [vp]
+    lib.ctd_jpeg_decode.argtypes = [vp, vp, vp, i32, vp, vp]
     for name in EXPORTS[3:]:
         getattr(lib, name).restype = C.c_int
+    lib.ctd_jpeg_decoder_destroy.restype = None
     lib.ctd_expand_textwindow.restype = None
     _lib = lib
     return lib

@@ -7,7 +7,8 @@ conf_thresh=0.4, mask_thresh=0.3, act='leaky')` and
 A `.onnx` model_path is read as the reference's OpenCV-DNN backend reads it (onnx_model.py): same engine, same calls.
 `detect_batch` / `detect_stream` give the same results for many pages of any sizes, batched on the GPU, and with a
 `textheight` also the OCR crops of every text line (`get_transformed_regions`), cut in the same batches; their pages may
-be torch.uint8 CUDA tensors, and with `device_results=True` the masks and crops come back as CUDA tensors.
+be torch.uint8 CUDA tensors or encoded files (JPEGs decoded on the GPU, jpeg.py), and with `device_results=True` the
+masks and crops come back as CUDA tensors.
 
 Everything runs in libctd_b200.so: network, NMS, mask u8, DB binarize, connected components, contour boxes + scores,
 refine_mask on the GPU; ratio scaling, `group_output` and the window expansion in host C++ (csrc/group.cpp,
@@ -22,6 +23,7 @@ import numpy as np
 
 from . import compiler, onnx_model
 from .binding import Engine, PREC_FP16_TC, PREC_FP32_SIMT
+from .jpeg import JpegDecoder, is_encoded, read_encoded
 from .textblock import (TextBlock, _check_textheight, blocks_from_records, group_output, overlap_area,  # noqa: F401
                         transformed_regions)
 
@@ -96,9 +98,13 @@ class TextDetector:
         self.device_index = int(device_index)
         self.net = Engine(self.program, device=device_index, precision=precision, max_batch=self.max_batch, max_h=input_size[0],
                           max_w=input_size[1], conf_thresh=conf_thresh, nms_thresh=nms_thresh, db_thresh=0.3)
+        self._jpeg = None   # the JpegDecoder of encoded pages, made on first use
 
     def close(self):
         self.net.close()
+        if self._jpeg is not None:
+            self._jpeg.close()
+            self._jpeg = None
 
     def __call__(self, img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
         """reference inference.py:141-178.  One native call (`ctd_detect_page`): letterbox (cv2-exact INTER_LINEAR) +
@@ -123,9 +129,10 @@ class TextDetector:
         """`[self(img, refine_mode, keep_undetected_mask) for img in imgs]`, with the same results byte for byte, computed
         in GPU batches of up to `max_batch` pages of any sizes (see detect_stream, which also describes CUDA-tensor
         pages and device_results).  Every page is checked before any GPU work: a page that is not u8 [h][w][3], or a
-        CUDA tensor on another device, raises ValueError.  With a textheight, each result is the 4-tuple detect_stream
-        yields, crops included."""
-        imgs = [check_page(img, self.device_index) for img in imgs]
+        CUDA tensor on another device, raises ValueError.  An encoded page (see detect_stream) is decoded with its
+        batch; one cv2 cannot decode raises ValueError then.  With a textheight, each result is the 4-tuple
+        detect_stream yields, crops included."""
+        imgs = [img if is_encoded(img) else check_page(img, self.device_index) for img in imgs]
         return list(self.detect_stream(imgs, refine_mode, keep_undetected_mask, textheight, device_results))
 
     def detect_stream(self, imgs, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, textheight=None,
@@ -143,6 +150,14 @@ class TextDetector:
         a page written by work still queued on that stream is read correctly.  The stream keeps a reference to the
         tensor until its batch is collected; do not write into it before its result has been yielded.  The results
         are the same as for `page.cpu().numpy()`.
+
+        A page may also be an encoded file, read as the reference's `io_utils.imread` reads it, i.e. as
+        `cv2.imdecode(buf, cv2.IMREAD_COLOR)`: bytes, bytearray, memoryview or a 1-D np.uint8 array of the file, or a
+        str / os.PathLike path, read with np.fromfile.  The encoded pages of a batch are decoded in one
+        `JpegDecoder.decode` call right before the batch is submitted: baseline JPEGs on the GPU into CUDA pages (which
+        then enter as CUDA-tensor pages do), every other file by cv2 on the host into a numpy page.  The results are
+        byte for byte those for the `cv2.imdecode` pages of the same files.  A file cv2 cannot decode raises ValueError
+        naming its index in `imgs` (and its path), when its batch is decoded.
 
         textheight (an integer >= 2; checked here, before any page is read): yields `(mask, mask_refined, blk_list,
         crops)` instead, where crops[b][i] is line i of blk_list[b] cut out as `get_transformed_regions(img, blk_list,
@@ -170,6 +185,7 @@ class TextDetector:
         free = [0, 1]
 
         def submit(batch, events):
+            batch = self._decode_batch(batch)
             if not free:
                 yield from self._collect(inflight, free)
             slot = free.pop(0)
@@ -179,8 +195,11 @@ class TextDetector:
 
         try:
             batch, events = [], []
-            for img in imgs:
-                page = check_page(img, self.device_index)
+            for idx, img in enumerate(imgs):
+                if is_encoded(img):
+                    page = _Encoded(idx, img)   # decoded with its batch (_decode_batch)
+                else:
+                    page = check_page(img, self.device_index)
                 batch.append(page)
                 events.append(_page_ready_event(page))
                 if len(batch) < self.max_batch:
@@ -198,6 +217,24 @@ class TextDetector:
                     self.net.collect_pages(slot, discard=True)
                 except Exception:
                     pass
+
+    def _decode_batch(self, batch):
+        """the batch with its encoded pages replaced by their decoded pages (one JpegDecoder.decode call): CUDA
+        tensors for the pages decoded on the GPU, complete when decode returns, numpy pages for the others"""
+        enc = [i for i, p in enumerate(batch) if isinstance(p, _Encoded)]
+        if not enc:
+            return batch
+        bufs = [read_encoded(batch[i].src) for i in enc]
+        if self._jpeg is None:
+            self._jpeg = JpegDecoder(self.device_index)
+        pages = self._jpeg.decode([b for b, _path in bufs])
+        batch = list(batch)
+        for i, (_b, path), page in zip(enc, bufs, pages):
+            if page is None:
+                raise ValueError("page %d%s could not be decoded (cv2.imdecode returns None)"
+                                 % (batch[i].index, "" if path is None else " (%s)" % path))
+            batch[i] = page if getattr(page, "is_cuda", False) else check_page(page, self.device_index)
+        return batch
 
     def _collect(self, inflight, free):
         slot = inflight.popleft()
@@ -222,6 +259,14 @@ def check_page(img, device_index=None):
     if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] < 1 or a.shape[1] < 1:
         raise ValueError("a page must be a uint8 array of shape [h][w][3], got %s %s" % (a.dtype, a.shape))
     return np.ascontiguousarray(a)
+
+
+class _Encoded:
+    """an encoded page of a stream, with its index in the stream, until its batch is decoded"""
+    __slots__ = ("index", "src")
+
+    def __init__(self, index, src):
+        self.index, self.src = index, src
 
 
 def _page_ready_event(page):

@@ -510,6 +510,66 @@ CTD_API int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page_ds
 CTD_API int ctd_nms(ctd_handle* h, const float* pred, int32_t rows, float conf_thresh, float iou_thresh, float* det,
             int32_t* det_count);
 
+/* ---- JPEG pages decoded on the GPU ------------------------------------------------------
+ * The reference reads pages with io_utils.imread = cv2.imdecode(np.fromfile(path), IMREAD_COLOR).  These entry points
+ * decode baseline JPEG files on the GPU to exactly the u8 BGR page cv2.imdecode returns (cv2 4.13's libjpeg-turbo:
+ * ISLOW IDCT, fancy upsampling, EXIF orientation applied).  A file outside the supported set, or one whose entropy
+ * data or IDCT range is not certain to decode as libjpeg-turbo's SIMD build decodes it, gets a non-zero status and
+ * is left to cv2: the GPU path declines a page, it never returns a different one.
+ *
+ * Supported: 8-bit sequential Huffman (SOF0/SOF1), one interleaved scan, one component (B = G = R = Y) or three YCbCr
+ * components with luma sampling 1x1, 2x1 or 2x2 and chroma 1x1, any restart interval, EXIF orientations 1-8.       */
+enum ctd_jpeg_status {
+  CTD_JPEG_OK = 0,
+  CTD_JPEG_NOT_JPEG = 1,     /* no SOI, or bytes that are not a marker where one must be                    */
+  CTD_JPEG_TRUNCATED = 2,    /* ends inside a segment or the scan, no scan, or no EOI after it             */
+  CTD_JPEG_PROGRESSIVE = 3,  /* SOF2 / SOF6, or a scan that is not the full spectrum                       */
+  CTD_JPEG_ARITHMETIC = 4,   /* SOF9-SOF15, DAC                                                            */
+  CTD_JPEG_PRECISION = 5,    /* sample precision other than 8 bits                                         */
+  CTD_JPEG_LOSSLESS = 6,     /* SOF3 / SOF5 / SOF7                                                         */
+  CTD_JPEG_SAMPLING = 7,     /* 4:4:0, 4:1:1 or any other sampling                                         */
+  CTD_JPEG_COLOR = 8,        /* not 1 or 3 components (CMYK, YCCK), Adobe transform other than 1, R/G/B ids */
+  CTD_JPEG_SCANS = 9,        /* a second scan or frame, a scan not of every component in frame order, DNL  */
+  CTD_JPEG_EXIF = 10,        /* an APP1 Exif block that does not parse cleanly, two of them, or two
+                                orientation entries in IFD0                                               */
+  CTD_JPEG_TABLES = 11,      /* a missing or invalid Huffman / quantisation table                          */
+  CTD_JPEG_ENTROPY = 12,     /* entropy-coded data not clean: restart markers out of order or missing, a
+                                marker inside the scan, an invalid code, a run past coefficient 63, too few or
+                                too many MCUs in an interval (set by the probe or by the GPU decode)         */
+  CTD_JPEG_RANGE = 13,       /* a block whose IDCT leaves the range on which libjpeg-turbo's C and SIMD IDCTs
+                                agree (GPU decode)                                                         */
+  CTD_JPEG_SIZE = 14         /* a scan of 2^28 bytes or more                                               */
+};
+typedef struct ctd_jpeg_info {
+  int32_t status;              /* ctd_jpeg_status; the fields below are set only for CTD_JPEG_OK          */
+  int32_t height, width;       /* the decoded page as cv2.imdecode returns it, i.e. after the orientation   */
+  int32_t frame_height, frame_width;
+  int32_t components;          /* 1 or 3                                                                   */
+  int32_t h_samp, v_samp;      /* luma sampling factors (chroma is 1x1); 1, 1 for one component            */
+  int32_t orientation;         /* EXIF orientation 1-8 (1 without an Exif block)                           */
+  int32_t restart_interval;    /* MCUs per restart interval, 0 without DRI                                 */
+  int64_t ecs_bytes;           /* entropy-coded bytes of the scan, stuffing and RST markers included       */
+} ctd_jpeg_info;
+/* Marker walk of one file (host only, no handle, thread-safe), including the scan's restart-marker structure and
+ * its EOI.  Returns 0, with the verdict in info->status; CTD_E_INVALID only for NULL arguments.                   */
+CTD_API int ctd_jpeg_probe(const uint8_t* data, size_t len, ctd_jpeg_info* info);
+
+typedef struct ctd_jpeg_decoder ctd_jpeg_decoder;
+/* A decoder bound to one GPU and one stream of its own.  subsequence_bits (>= 1; 0 picks the default): the length of
+ * the pieces each restart interval's bits are cut into for the parallel Huffman decode (any value decodes the same
+ * pages; it only changes how many threads and rounds the decode takes).  Not thread-safe; errors via
+ * ctd_last_error(NULL).                                                                                             */
+CTD_API int ctd_jpeg_decoder_create(int32_t device, int32_t subsequence_bits, ctd_jpeg_decoder** out);
+CTD_API void ctd_jpeg_decoder_destroy(ctd_jpeg_decoder* dec);
+/* Decodes n files at once: data[i] / len[i] (host memory).  Every file whose probe status is CTD_JPEG_OK is decoded
+ * into dst[i], a DEVICE buffer of height * width * 3 bytes (u8 BGR [h][w][3], the probe's oriented shape) on the
+ * decoder's GPU; dst[i] may be NULL for other files.  status[i] gets the probe status or the decode's verdict
+ * (CTD_JPEG_ENTROPY, CTD_JPEG_RANGE); only pages with status 0 have been written, the others are to be decoded by
+ * cv2.  Blocks until every page is written, so the buffers may be used on any stream.  Staging, tables and the
+ * coefficient buffer belong to the decoder and grow on demand.                                                   */
+CTD_API int ctd_jpeg_decode(ctd_jpeg_decoder* dec, const uint8_t* const* data, const size_t* len, int32_t n,
+                            uint8_t* const* dst, int32_t* status);
+
 #ifdef __cplusplus
 }
 #endif
