@@ -21,7 +21,8 @@ import ctd_b200
 from ctd_b200 import compiler as cc
 from oracle import synth
 from util import (SingleOp, PREC_FP16_TC, PREC_SPLIT_TC, get_checkpoint, tc_plan, fp16_tc_ab, split_tc_ab,
-                  bound_ratio, conv_ref_mag, deconv4_ref_mag, act_f64, detect_decode_f64, program_tc_plans)
+                  bound_ratio, conv_ref_mag, deconv4_ref_mag, act_f64, detect_decode_f64, program_tc_plans, blob_tensor,
+                  nchw_f64)
 
 pytestmark = pytest.mark.gpu
 
@@ -194,16 +195,8 @@ BENCH_SHAPES = [(PREC_FP16_TC, 16, 1024, 1024), (PREC_FP16_TC, 8, 640, 640), (PR
                 (PREC_SPLIT_TC, 1, 1024, 1024)]
 
 
-def _blob(prog, off, count, dtype):
-    return torch.from_numpy(np.frombuffer(prog.blob, dtype=dtype, count=count, offset=off).copy()).to(DEV)
-
-
 def _slices_overlap(a, b):
     return a[0] == b[0] and a[1] < b[1] + b[2] and b[1] < a[1] + a[2]
-
-
-def _nchw(arr, img):
-    return torch.from_numpy(np.ascontiguousarray(arr[img])).to(DEV).permute(2, 0, 1)[None].double()
 
 
 def _check_images(n):
@@ -230,7 +223,7 @@ def test_bench_plans_per_op(prec, n, h, w):
             kind = op["kind"]
             gemm = kind in (cc.OP_CONV, cc.OP_DECONV4, cc.OP_DETECT)
             tc_tail = not split and kind in (cc.OP_STEM, cc.OP_SEG_TAIL)
-            if not (gemm or tc_tail):
+            if not (gemm or tc_tail):      # CUDA-core ops: tests/test_gpu_thin_ops.py
                 continue
             srcs = [(op["src_buf"][j], op["src_coff"][j], op["src_c"][j]) for j in range(op["n_src"])]
             dsl = (op["dst_buf"], op["dst_coff"], op["cout"]) if op["dst_buf"] >= 0 else None
@@ -275,7 +268,7 @@ def _op_ratio(prog, op, ins, res_before, got_all, pages, img, split):
     wdt = np.float32 if split else np.float16
     wsz = 4 if split else 2
     woff = op["w32_off"] if split else op["w16_off"]
-    bias = _blob(prog, op["b_off"], cout, np.float32)
+    bias = blob_tensor(prog, op["b_off"], cout, np.float32)
     if kind == cc.OP_STEM:
         # tensor-core stem: fp16 space-to-depth page (channel (dy * 2 + dx) * 3 + c) and the fp16 window weights
         pg = (torch.from_numpy(pages[img]).to(DEV).permute(2, 0, 1).float() / 255).half().double()
@@ -283,13 +276,13 @@ def _op_ratio(prog, op, ins, res_before, got_all, pages, img, split):
         for dy in range(2):
             for dx in range(2):
                 x[0, (dy * 2 + dx) * 3:(dy * 2 + dx) * 3 + 3] = pg[:, dy::2, dx::2]
-        ww = _blob(prog, op["w16_off"], 32 * 192, np.float16).double().view(32, 3, 4, 16)[:cout, :, :3]
+        ww = blob_tensor(prog, op["w16_off"], 32 * 192, np.float16).double().view(32, 3, 4, 16)[:cout, :, :3]
         ref, mag = conv_ref_mag(x, ww.permute(0, 3, 1, 2), bias, 1, 1)
         K = 192
     elif kind == cc.OP_SEG_TAIL:
         c = op["src_c"][0]
-        x = _nchw(ins[0], img)
-        wc = _blob(prog, op["w16_off"], 16 * 9 * c, np.float16).double().view(16, 3, 3, c)[:4].permute(0, 3, 1, 2)
+        x = nchw_f64(ins[0], img)
+        wc = blob_tensor(prog, op["w16_off"], 16 * 9 * c, np.float16).double().view(16, 3, 3, c)[:4].permute(0, 3, 1, 2)
         y, mag = conv_ref_mag(x, wc, torch.zeros(4, device=DEV), 1, 1)
         K = 9 * c
         nb, _, ih, iw = y.shape
@@ -303,19 +296,19 @@ def _op_ratio(prog, op, ins, res_before, got_all, pages, img, split):
         got = torch.from_numpy(got_all[img].reshape(1, 2 * ih, 2 * iw)).to(DEV)
         return float(bound_ratio(got, ref, m2, 2.0 ** -21, b).max()), K
     else:
-        x = torch.cat([_nchw(a, img) for a in ins], 1)
+        x = torch.cat([nchw_f64(a, img) for a in ins], 1)
         if kind == cc.OP_DECONV4:
             K = 4 * cin
-            wk = _blob(prog, woff, 4 * cout_pad * K, wdt).view(4, cout_pad, K)[:, :cout]
+            wk = blob_tensor(prog, woff, 4 * cout_pad * K, wdt).view(4, cout_pad, K)[:, :cout]
             ref, mag = deconv4_ref_mag(x, wk, bias)
         else:
             ks, st = op["ksize"], op["stride"]
             K = ks * ks * cin
-            wt = _blob(prog, woff, cout_pad * K, wdt).view(cout_pad, ks, ks, cin)[:cout].permute(0, 3, 1, 2)
+            wt = blob_tensor(prog, woff, cout_pad * K, wdt).view(cout_pad, ks, ks, cin)[:cout].permute(0, 3, 1, 2)
             ref, mag = conv_ref_mag(x, wt, bias, st, ks // 2)
     a, b = split_tc_ab(K) if split else fp16_tc_ab(K)
     if kind == cc.OP_DETECT:
-        prm = _blob(prog, op["p_off"], 7, np.float32).double().cpu().numpy()
+        prm = blob_tensor(prog, op["p_off"], 7, np.float32).double().cpu().numpy()
         rf, mo, rmag = detect_decode_f64(ref, mag, float(prm[0]), prm[1:].reshape(3, 2))
         gh, gw = ref.shape[2], ref.shape[3]
         r0 = sum(3 * (h // (8 << l)) * (w // (8 << l)) for l in range(op["aux"]))
@@ -324,7 +317,7 @@ def _op_ratio(prog, op, ins, res_before, got_all, pages, img, split):
         return float(bound_ratio(got, rf, mo, 2.0 ** -21, b, ref_mag=rmag).max()), K
     ref = act_f64(ref, op["act"])
     if res_before is not None:
-        ref = ref + _nchw(res_before, img)
-    got = _nchw(got_all, img)
+        ref = ref + nchw_f64(res_before, img)
+    got = nchw_f64(got_all, img)
     return float(bound_ratio(got, ref, mag, a, b).max()), K
 

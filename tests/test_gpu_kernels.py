@@ -1,7 +1,9 @@
-"""-m gpu: every CUDA kernel against a plain torch fp32 reference of the same op (fp16-rounded
-operands for the fp16 engines, so only accumulation order and the output rounding differ).  The tensor-core engines
-(fp16 and split-fp16) are also held to the elementwise bound of tests/util.py, so a wrong value at a small output
-fails as well as one at the largest."""
+"""-m gpu: the convolution kernels (conv_tc_kernel and conv_simt_kernel, in all four precisions) on one-op convolution
+and 4x4-deconvolution programs against a plain torch reference of the same op (fp16-rounded operands for the fp16
+engines, so only accumulation order and the output rounding differ).  The tensor-core engines (fp16 and split-fp16)
+are also held to the elementwise bound of tests/util.py, so a wrong value at a small output fails as well as one at
+the largest.  The other CUDA-core kernels (stem, pools, upsample, seg and DB tails) are pinned per op in
+tests/test_gpu_thin_ops.py."""
 import numpy as np
 import pytest
 import torch

@@ -90,10 +90,15 @@ def test_benchmark_config_matches_oracle():
     _check_against_oracle(PREC_FP16_TC, True, 16, 1024, 1024, use_graph=True)
 
 
-@pytest.mark.parametrize("prec", [PREC_FP16_TC, PREC_SPLIT_TC], ids=["fp16_tc", "split_tc"])
-@pytest.mark.parametrize("size", [640, 1024, 1536])
+@pytest.mark.parametrize("size,prec", [
+    pytest.param(s, p, id="%d-%s" % (s, name))
+    for s, p, name in [(640, PREC_FP16_TC, "fp16_tc"), (640, PREC_SPLIT_TC, "split_tc"),
+                       (1024, PREC_FP16_TC, "fp16_tc"), (1024, PREC_SPLIT_TC, "split_tc"),
+                       (1024, PREC_FP32_SIMT, "fp32_simt"),
+                       (1536, PREC_FP16_TC, "fp16_tc"), (1536, PREC_SPLIT_TC, "split_tc")]])
 def test_stream_bucket_sizes_match_oracle(prec, size):
-    """BASELINE configs[4] buckets (640 / 1024 / 1536 squares) and config 2 (1024, fp32-accurate tensor-core mode)."""
+    """BASELINE configs[4] buckets (640 / 1024 / 1536 squares) and config 2 (1024, the fp32-accurate engines: split-fp16
+    tensor cores and fp32 CUDA cores) against the fp32 oracle."""
     _check_against_oracle(prec, True, 2, size, size, use_graph=True, seed=2000 + size)
 
 

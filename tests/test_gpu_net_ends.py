@@ -15,8 +15,8 @@ import pytest
 import ctd_b200
 from ctd_b200 import compiler as cc
 from oracle import synth
-from util import get_checkpoint
-from test_gpu_conv_tc import _blob, _op_ratio
+from util import get_checkpoint, blob_tensor
+from test_gpu_conv_tc import _op_ratio
 
 pytestmark = pytest.mark.gpu
 
@@ -81,7 +81,7 @@ def _seg_ref(prog, op, x):
     """float64 mask of the seg tail's fp16 3x3 / 4-phase form over its fp16 input x [n][gh][gw][64]."""
     import torch
     c = op["src_c"][0]
-    wc = _blob(prog, op["w16_off"], 16 * 9 * c, np.float16).double().cpu()
+    wc = blob_tensor(prog, op["w16_off"], 16 * 9 * c, np.float16).double().cpu()
     wt = wc.view(16, 3, 3, c)[:4].permute(0, 3, 1, 2)
     xt = torch.from_numpy(x.astype(np.float64)).permute(0, 3, 1, 2)
     y = torch.nn.functional.conv2d(xt, wt, None, 1, 1)

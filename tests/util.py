@@ -130,6 +130,19 @@ def split_tc_ab(K):
     return a, b
 
 
+def simt_ab(K, fp16_out=False):
+    """CUDA-core engines (conv_simt_kernel, stem_kernel): exact operands (fp32, or fp16 widened to fp32), one fp32
+    FMA chain of K terms per output, fp32 epilogue, fp32 or fp16 output."""
+    # a: expf is within 2 ulps (2^-22 relative), the 1 + e and the division of SiLU / sigmoid and the residual add
+    #    round once each (3 x 2^-24): 1.75 x 2^-22 in all, under 2^-21.  An fp16 output adds its own rounding, 2^-11.
+    a = 2.0 ** -21 + (2.0 ** -11 if fp16_out else 0.0)
+    # b: every FMA rounds once, 2^-24 relative to a partial sum <= M; K FMAs, the bias add and 3 ulps of headroom for
+    #    the activation's internal roundings (the +4 of fp16_tc_ab); 1.1 is SiLU's largest slope, which carries the
+    #    pre-activation error through.
+    b = 1.1 * (K + 4) * 2.0 ** -24
+    return a, b
+
+
 def bound_ratio(got, ref, M, a, b, ref_mag=None):
     """Elementwise |got - ref| / (a * |ref| + b * M) as float64 (torch or numpy in, same kind out).  ref_mag replaces
     |ref| in the bound where the output is computed through a cancellation (Detect box centres)."""
@@ -140,6 +153,16 @@ def bound_ratio(got, ref, M, a, b, ref_mag=None):
     got = np.asarray(got, np.float64)
     rm = np.abs(ref) if ref_mag is None else ref_mag
     return np.abs(got - ref) / (a * rm + b * M + 1e-300)
+
+
+def blob_tensor(prog, off, count, dtype, device="cuda"):
+    """`count` values of `dtype` at byte offset `off` of the program's weight blob, as a torch tensor."""
+    return torch.from_numpy(np.frombuffer(prog.blob, dtype=dtype, count=count, offset=off).copy()).to(device)
+
+
+def nchw_f64(arr, img, device="cuda"):
+    """image `img` of an engine buffer read as [n][h][w][c] -> float64 [1][c][h][w]."""
+    return torch.from_numpy(np.ascontiguousarray(arr[img])).to(device).permute(2, 0, 1)[None].double()
 
 
 def conv_ref_mag(x, w, bias, stride, pad):
@@ -220,3 +243,30 @@ def program_tc_plans(prog, n, h, w, split=False, num_sms=H100_SMS):
         else:
             plans[i] = tc_plan(op["cout"], gh // op["stride"], gw // op["stride"], n, 1, split, num_sms)
     return plans
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Kernel choice of sppf_pool_launch (csrc/simt.cu), replicated: the whole h x w plane of one 8-channel group, twice
+# (ping-pong), must fit in 200 KB of shared memory for sppf_pool_tile_kernel; otherwise sppf_pool_kernel reads a
+# 13 x 13 window per pixel from global memory.  h x w is the SPPF grid, the page at 1/32.
+SPPF_SMEM_LIMIT = 200 * 1024
+
+
+def sppf_uses_tile(h, w, elem_bytes):
+    return 2 * h * w * 8 * elem_bytes <= SPPF_SMEM_LIMIT
+
+
+# (precision, n, page h, page w, tile kernel?) of tests/test_gpu_thin_ops.py::test_sppf_both_kernels: each storage
+# width at its exact tile limit and past it (tests/test_cpu_thin_ops_plan.py checks the sides without a GPU)
+SPPF_SHAPES = [
+    (PREC_SPLIT_TC, 1, 1024, 3200, True),       # 32 x 100 fp32: 204 800 B, the limit itself
+    (PREC_FP32_SIMT, 2, 1856, 1856, False),     # 58 x 58 fp32, two images
+    (PREC_SPLIT_TC, 1, 1024, 4096, False),      # 32 x 128 fp32
+    (PREC_FP16_TC, 1, 2048, 3200, True),        # 64 x 100 fp16: 204 800 B
+    (PREC_FP16_TC, 1, 2624, 2624, False),       # 82 x 82 fp16
+]
+
+
+def storage_bytes(prec):
+    """bytes per stored activation: fp16 engines 2, fp32 and split-fp16 (fp32 master copy) 4."""
+    return 2 if prec in (PREC_FP16_TC, PREC_FP16_SIMT) else 4
