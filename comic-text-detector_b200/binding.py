@@ -91,7 +91,7 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
            "ctd_submit_pages_regions", "ctd_collect_regions", "ctd_submit_pages_device", "ctd_collect_device",
            "ctd_forward_tensor", "ctd_jpeg_probe", "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy",
-           "ctd_jpeg_decode"]
+           "ctd_jpeg_decode", "ctd_debug_postprocess"]
 
 _lib = None
 
@@ -143,6 +143,7 @@ def load_library():
     lib.ctd_get_mask_u8_resized.argtypes = [vp, i32, i32, i32, i32, vp]
     lib.ctd_resize_linear_u8.argtypes = [vp, vp, i32, i32, i32, vp, i32, i32]
     lib.ctd_debug_run_ops.argtypes = [vp, vp, i32, i32, i32, i32, i32]
+    lib.ctd_debug_postprocess.argtypes = [vp, vp, vp, i32, i32, i32]
     lib.ctd_get_nms_status.argtypes = [vp, vp, C.POINTER(i32)]
     lib.ctd_group_output.argtypes = [vp, vp, i32, vp, i32, i32, i32, vp, i32, vp, i32, vp, i32, vp, i32, C.POINTER(i32)]
     lib.ctd_expand_textwindow.argtypes = [i32, i32, vp, i32, vp]
@@ -660,6 +661,18 @@ class Engine:
         if pages is not None:
             pages = np.ascontiguousarray(pages, dtype=np.uint8)
         self._ck(self.lib.ctd_debug_run_ops(self.h, _ptr(pages), n, h, w, first, last))
+        self.shape = (n, h, w)
+
+    def debug_postprocess(self, blks, lines):
+        """the forward's NMS and DB post-processing on given network outputs (ctd_debug_postprocess): blks f32
+        [n][rows_per_image][5 + nc], lines f32 [n][2][h][w].  Read the results with detections(), nms_status(n),
+        db_components() and text_lines()."""
+        blks = np.ascontiguousarray(blks, np.float32)
+        lines = np.ascontiguousarray(lines, np.float32)
+        n, c, h, w = lines.shape
+        assert c == 2 and blks.shape == (n, 3 * ((h // 8) * (w // 8) + (h // 16) * (w // 16) + (h // 32) * (w // 32)),
+                                         5 + self.nc), (blks.shape, lines.shape)
+        self._ck(self.lib.ctd_debug_postprocess(self.h, _ptr(blks), _ptr(lines), n, h, w))
         self.shape = (n, h, w)
 
     # ---- text-line crops (ctd_transform_regions) -------------------------------------------

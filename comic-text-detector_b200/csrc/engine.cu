@@ -1018,6 +1018,29 @@ extern "C" int ctd_debug_run_ops(ctd_handle* h, const uint8_t* pages, int32_t n,
   return CTD_OK;
 }
 
+extern "C" int ctd_debug_postprocess(ctd_handle* h, const float* blks, const float* lines, int32_t n, int32_t ph,
+                                     int32_t pw) {
+  if (!h || !blks || !lines) return CTD_E_INVALID;
+  if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_debug_postprocess needs the full pipeline");
+  ShapePlan* sp = nullptr;
+  if (int rc = find_plan(h, n, ph, pw, &sp)) return rc;
+  const size_t hw = size_t(ph) * pw;
+  CK(cudaMemcpyAsync(h->d_blks, blks, size_t(n) * rows_per_image(ph, pw) * (5 + h->cfg.nc) * 4, cudaMemcpyHostToDevice,
+                     h->stream));
+  CK(cudaMemcpyAsync(h->d_lines, lines, size_t(n) * hw * 2 * 4, cudaMemcpyHostToDevice, h->stream));
+  // the DB tail's bitmap: the shrink map (channel 0 of each page's lines) > db_thresh, compared in float32
+  for (int i = 0; i < n; ++i)
+    CK(binarize_launch(h->d_lines + size_t(i) * 2 * hw, hw, h->cfg.db_thresh, h->d_bitmap + size_t(i) * hw, h->stream));
+  int cnt = 0;
+  if (int rc = launch_nms(h, n, ph, pw, h->stream, &cnt)) return rc;
+  if (int rc = launch_db_post(h, n, ph, pw, h->stream, &cnt)) return rc;
+  CK(cudaStreamSynchronize(h->stream));
+  h->n = n; h->ph = ph; h->pw = pw;
+  h->have_forward = true;
+  h->last_launches = cnt;
+  return CTD_OK;
+}
+
 int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap, int32_t** d_stats, int32_t* n_labels) {
   const size_t px = size_t(ih) * iw;
   // own grow-on-demand scratch (any page size, independent of the net-input workspace; the results of the last
@@ -1042,7 +1065,7 @@ int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap
 extern "C" int ctd_connected_components(ctd_handle* h, const uint8_t* img, int32_t ih, int32_t iw, int32_t* labels,
                                         int32_t* stats, int32_t stats_cap, int32_t* n_labels) {
   if (!h || !img || !labels || !n_labels) return CTD_E_INVALID;
-  if (ih < 1 || iw < 1 || size_t(ih) * iw > (size_t(1) << 28)) return ctd_fail(h, CTD_E_SHAPE, "bad image size %dx%d", ih, iw);
+  if (ih < 1 || iw < 1 || size_t(ih) * iw > kCclMaxPixels) return ctd_fail(h, CTD_E_SHAPE, "bad image size %dx%d", ih, iw);
   CK(cudaSetDevice(h->cfg.device));
   const size_t px = size_t(ih) * iw;
   if (int rc = h->io_scratch.grow(h, px + 256, h->stream)) return rc;

@@ -39,7 +39,13 @@
 
 namespace ctdgeom {
 
-constexpr int kMaxHull = 512;      // convex lattice polygons inside a 2048^2 grid have < 512 vertices
+// Hull capacity for maps up to 2048^2 (ctd_seg_represent's limit).  A strictly convex lattice polygon's edges have
+// pairwise distinct directions, so their primitive vectors are distinct; its edges' |dx| sum to twice its width and
+// their |dy| to twice its height, so their L1 lengths sum to at most 4 * 2047 = 8188.  There are 4j nonzero integer
+// vectors of L1 norm j: all 612 of norm <= 17 already sum to 7140, leaving room for at most 58 of norm 18 -- at most
+// 670 vertices.  The monotone chain holds the closing vertex once more (671); 560-vertex polygons inside 1998^2 exist
+// (tests/lattice_polygon.py).
+constexpr int kMaxHull = 704;
 constexpr int kMaxOffsetPts = 512; // vertices emitted by the round-join offset of a quad
 constexpr double kPi = 3.141592653589793238;
 

@@ -208,6 +208,9 @@ void nms_workspace_bind(NmsWorkspace& ws, void* base, int n, int cap);
 cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* labels, int32_t* scratch /*3*n*h*w ints*/,
                        int32_t* n_labels, cudaStream_t s);
 constexpr int kCclLaunches = 8;   // kernels and memsets ccl_launch enqueues
+// Largest image ccl_launch + ccl_stats_launch label: the kernels index pixels with int and the stats table with
+// 5 ints per label (up to a quarter of the pixels), so 2^28 keeps every index far inside int range.
+constexpr size_t kCclMaxPixels = size_t(1) << 28;
 cudaError_t ccl_stats_launch(const int32_t* labels, int h, int w, int32_t* stats, int cap, cudaStream_t s);
 
 // SegDetectorRepresenter.boxes_from_bitmap (segrep.cu).  Lf = foreground union-find roots left in the CCL

@@ -695,7 +695,12 @@ extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_pa
   if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
     return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_pages_plan returns");
   size_t rows = 0;
-  for (int i = 0; i < n; ++i) rows += size_t(pg[size_t(i)].ih);
+  for (int i = 0; i < n; ++i) {
+    rows += size_t(pg[size_t(i)].ih);
+    if (keep_undetected && size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) > kCclMaxPixels)
+      return ctd_fail(h, CTD_E_CAPACITY, "page %d (%dx%d): refine_undetected_mask labels pages of at most 2^28 pixels", i,
+                      pg[size_t(i)].ih, pg[size_t(i)].iw);
+  }
   if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
   // pages in device memory: strides, and the first and last byte each page reads must be memory of this GPU
   CK(cudaSetDevice(h->cfg.device));
@@ -898,6 +903,8 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   if (!h || !page || !mask_out || !mask_refined_out || !n_blocks) return CTD_E_INVALID;
   if (ih < 1 || iw < 1) return ctd_fail(h, CTD_E_SHAPE, "bad page size %dx%d", ih, iw);
   *n_blocks = 0;
+  if (keep_undetected && size_t(ih) * iw > kCclMaxPixels)
+    return ctd_fail(h, CTD_E_CAPACITY, "page %dx%d: refine_undetected_mask labels pages of at most 2^28 pixels", ih, iw);
   Letterbox geo;
   if (!letterbox_of(ih, iw, net_h, net_w, geo)) return ctd_fail(h, CTD_E_SHAPE, "page does not letterbox into the net input");
   ShapePlan* sp = nullptr;

@@ -514,36 +514,41 @@ __global__ void __launch_bounds__(256) ccl_scan_seg_kernel(int h, int w, int* __
   }
   if (threadIdx.x == 255) segsum[page * nseg + seg] = woff + incl;
 }
-// Pass 5b: exclusive scan of the segment totals (<= 1024 segments per page), n_labels.
+// Pass 5b: exclusive scan of the segment totals, n_labels.  Chunks of 4096 segments (4 consecutive entries per thread,
+// block scan of the per-thread sums) with a running carry, so any segment count works: a 2^28-pixel image has 32768.
 __global__ void __launch_bounds__(1024) ccl_scan_top_kernel(int* __restrict__ segsum, int nseg, int* __restrict__ n_labels) {
-  // exclusive scan of up to 4096 segment sums: 4 consecutive entries per thread, block scan of the per-thread sums
   __shared__ int part[1024];
   const int page = blockIdx.x;
-  int* sgs = segsum + page * nseg;
-  int v[4], loc = 0;
+  int* sgs = segsum + size_t(page) * nseg;
+  int carry = 0;
+  for (int c0 = 0; c0 < nseg; c0 += 4096) {
+    int v[4], loc = 0;
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int i = threadIdx.x * 4 + k;
-    v[k] = i < nseg ? sgs[i] : 0;
-    loc += v[k];
-  }
-  part[threadIdx.x] = loc;
-  __syncthreads();
-  for (int off = 1; off < 1024; off <<= 1) {
-    int u = 0;
-    if (threadIdx.x >= off) u = part[threadIdx.x - off];
+    for (int k = 0; k < 4; ++k) {
+      const int i = c0 + threadIdx.x * 4 + k;
+      v[k] = i < nseg ? sgs[i] : 0;
+      loc += v[k];
+    }
+    part[threadIdx.x] = loc;
     __syncthreads();
-    part[threadIdx.x] += u;
-    __syncthreads();
-  }
-  int run = part[threadIdx.x] - loc;
+    for (int off = 1; off < 1024; off <<= 1) {
+      int u = 0;
+      if (threadIdx.x >= off) u = part[threadIdx.x - off];
+      __syncthreads();
+      part[threadIdx.x] += u;
+      __syncthreads();
+    }
+    int run = carry + part[threadIdx.x] - loc;
 #pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    const int i = threadIdx.x * 4 + k;
-    if (i < nseg) sgs[i] = run;
-    run += v[k];
+    for (int k = 0; k < 4; ++k) {
+      const int i = c0 + threadIdx.x * 4 + k;
+      if (i < nseg) sgs[i] = run;
+      run += v[k];
+    }
+    carry += part[1023];
+    __syncthreads();   // every thread has read part[1023] before the next chunk overwrites it
   }
-  if (threadIdx.x == 1023) n_labels[page] = part[1023] + 1;
+  if (threadIdx.x == 0) n_labels[page] = carry + 1;
 }
 
 __global__ void ccl_relabel_kernel(int h, int w, const int* __restrict__ Lall, const int* __restrict__ keymin_all,
@@ -573,7 +578,6 @@ cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* labels,
   int* bflag = scratch + size_t(2) * n * hw;
   const int nb = ((h + 1) / 2) * ((w + 1) / 2);
   const int nseg = (nb + kScanSeg - 1) / kScanSeg;
-  if (nseg > 4096) return cudaErrorInvalidValue;
   // per page the bflag area has hw ints but only nb (<= hw/4 + ..) are used: keep segsum after them
   int* segsum = bflag + size_t(n - 1) * hw + nb;  // n*nseg ints, fits: nseg*n <= hw - nb for sane shapes
   if (size_t(n) * nseg > size_t(hw - nb)) return cudaErrorInvalidValue;

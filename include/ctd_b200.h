@@ -242,6 +242,14 @@ CTD_API int ctd_debug_write_buffer(ctd_handle* h, int32_t buf, const float* in, 
 CTD_API int ctd_debug_run_ops(ctd_handle* h, const uint8_t* pages, int32_t n, int32_t ph, int32_t pw, int32_t first_op,
                               int32_t last_op);
 
+/* Debug/unit tests: the post-processing stage of a forward on caller-supplied network outputs.  blks HOST f32
+ * [n][rows_per_image][5 + nc] (the Detect rows), lines HOST f32 [n][2][ph][pw] (the DB maps); (n, ph, pw) obey
+ * ctd_forward's shape rules.  Uploads both, writes the bitmap as lines[:, 0] > db_thresh (the DB tail's comparison)
+ * and runs the forward's own NMS and DB post-processing (CCL + text-line boxes) on the engine stream, then
+ * synchronises: ctd_get_detections, ctd_get_nms_status, ctd_get_db_components and ctd_get_text_lines read the
+ * results.  Refused (CTD_E_INVALID) on a debug_skip_postproc engine.                                      */
+CTD_API int ctd_debug_postprocess(ctd_handle* h, const float* blks, const float* lines, int32_t n, int32_t ph, int32_t pw);
+
 /* ---- measurement / interop ------------------------------------------------------------------
  * CUDA-event timer on the ENGINE stream (bench.py times K forwards between start and stop).    */
 CTD_API int ctd_timer_start(ctd_handle* h);
@@ -274,13 +282,14 @@ CTD_API int ctd_get_device_outputs(ctd_handle* h, ctd_device_outputs* out);
  * effectively calls it (utils/textmask.py:93,113,138; SURVEY App. D #16).
  * img u8 [h][w] (non-zero = foreground), HOST pointers.  labels i32 [h][w];
  * stats i32 [n_labels][5] = x,y,w,h,area (row 0 = background); returns count in *n_labels.
- * `stats_cap` = rows available in `stats`.                                                 */
+ * `stats_cap` = rows available in `stats`.  Images of at most 2^28 pixels (CTD_E_SHAPE beyond).     */
 CTD_API int ctd_connected_components(ctd_handle* h, const uint8_t* img, int32_t ih, int32_t iw, int32_t* labels,
                              int32_t* stats, int32_t stats_cap, int32_t* n_labels);
 
 /* Stage-isolated form of the above on a caller-supplied probability map (HOST f32 [ih][iw]):
  * binarize(pred > thresh) -> contours -> boxes/scores, as `SegDetectorRepresenter(thresh).__call__`
- * would return for one image.  boxes i16 [1000][4][2], scores f32 [1000], *count = rows used.       */
+ * would return for one image.  boxes i16 [1000][4][2], scores f32 [1000], *count = rows used.  Maps of at most
+ * 2048 x 2048 that fit the engine's max_h * max_w pixels (CTD_E_CAPACITY beyond).                        */
 CTD_API int ctd_seg_represent(ctd_handle* h, const float* pred, int32_t ih, int32_t iw, float thresh, int16_t* boxes,
                               float* scores, int32_t* count);
 
@@ -346,7 +355,9 @@ CTD_API void ctd_expand_textwindow(int32_t im_w, int32_t im_h, const int32_t* xy
  * 64); mask_out / mask_refined_out HOST u8 [ih][iw] (mask_out is the page-sized mask, modified in place by
  * refine_undetected_mask exactly like the reference's); blocks / lines_out / dist_out as ctd_group_output.
  * Blocking.  Returns CTD_E_CAPACITY with *n_blocks set when an output array is too small (CTD_MAX_BLOCKS blocks and
- * lines, CTD_MAX_BLOCK_DIST distances always suffice).                                                     */
+ * lines, CTD_MAX_BLOCK_DIST distances always suffice).  With keep_undetected != 0 the page may have at most 2^28
+ * pixels (16384 x 16384; an A4 page at 600 dpi has 34.8 M): refine_undetected_mask labels the whole page with the
+ * connected-components kernels, whose pixel and label indices are int; a larger page returns CTD_E_CAPACITY.     */
 CTD_API int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t net_h, int32_t net_w,
                             int32_t refine_mode, int32_t keep_undetected, uint8_t* mask_out, uint8_t* mask_refined_out,
                             ctd_block* blocks, int32_t blocks_cap, int32_t* lines_out, int32_t lines_cap, double* dist_out,
@@ -405,7 +416,8 @@ CTD_API int ctd_pages_plan(ctd_page_entry* pages, int32_t n, int32_t net_h, int3
  * untouched until the slot is collected.  On the GPU: one letterbox launch for the batch, the forward at
  * (n, net_h, net_w), one launch back-projecting every page's mask to its size, one refine_mask launch for every
  * window of every page.  Same checks as ctd_submit_full (slot 0/1 and collected, n <= max_batch, net shape <= the
- * engine's max shape, not a debug_skip_postproc engine).                                                          */
+ * engine's max shape, not a debug_skip_postproc engine), and with keep_undetected != 0 ctd_detect_page's page-size
+ * limit (2^28 pixels per page, CTD_E_CAPACITY beyond).                                                            */
 CTD_API int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
                              int32_t net_w, const uint8_t* input_host, int32_t refine_mode, int32_t keep_undetected,
                              void* results_host);

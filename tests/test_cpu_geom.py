@@ -127,3 +127,17 @@ def test_contour_chain_against_cv2(lib):
     print('contour chain vs cv2:', same, 'of', tot)
     assert skip_mis == 0
     assert same >= 0.985 * tot, (same, tot)
+
+
+def test_560_vertex_hull_on_a_2048_map(lib):
+    """The largest hulls a 2048^2 map can hold (up to 670 vertices): a convex lattice polygon of 560 vertices, filled
+    exactly, must give the oracle's box instead of overflowing the hull buffers (which skips the contour)."""
+    from lattice_polygon import fill_exact, many_vertex_polygon
+    m = fill_exact(many_vertex_polygon(), 2048, 2048, 20, 25)
+    cs, _ = cv2.findContours((m > 0.3).astype(np.uint8), cv2.RETR_LIST, cv2.CHAIN_APPROX_SIMPLE)
+    assert len(cs) == 1 and len(cv2.convexHull(cs[0])) == 560
+    pts = np.ascontiguousarray(cs[0].reshape(-1, 2).astype(np.int32))
+    ref = _ref_box(pts, 2048, 2048)
+    box = np.zeros(8, np.int16)
+    ok = lib.geom_contour_box(pts.ctypes.data, len(pts), 2048, 2048, 2048, 2048, 1.5, box.ctypes.data)
+    assert ok == 1 and np.array_equal(box.reshape(4, 2), ref), (ok, box.tolist(), ref.tolist())
