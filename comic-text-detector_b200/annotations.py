@@ -53,12 +53,16 @@ def imread(path, read_type=None):
     return cv2.imdecode(np.fromfile(path, dtype=np.uint8), cv2.IMREAD_COLOR if read_type is None else read_type)
 
 
-def imwrite(img_path, img, ext=".png"):
-    """io_utils.py:48-53: the suffix is REPLACED by `ext` (first occurrence of the suffix string in the path)."""
-    import cv2
+def png_path(img_path, ext=".png"):
+    """io_utils.py:48-53's file name: the suffix is REPLACED by `ext` (first occurrence of the suffix string)."""
     suffix = Path(img_path).suffix
-    img_path = img_path.replace(suffix, ext) if suffix != "" else img_path + ext
-    cv2.imencode(ext, img)[1].tofile(img_path)
+    return img_path.replace(suffix, ext) if suffix != "" else img_path + ext
+
+
+def imwrite(img_path, img, ext=".png"):
+    """io_utils.py:48-53"""
+    import cv2
+    cv2.imencode(ext, img)[1].tofile(png_path(img_path, ext))
 
 
 def xyxy2yolo(xyxy, w, h):
@@ -82,9 +86,8 @@ def get_yololabel_strings(clslist, labellist):
     return "\n".join(rows)
 
 
-def write_annotations(save_dir, imgname, img, mask_refined, blk_list, save_json=False):
-    """The per-page part of `model2annotations` (inference.py:33-70) for an already detected page."""
-    im_h, im_w = img.shape[:2]
+def write_labels(save_dir, imgname, im_h, im_w, blk_list, save_json=False):
+    """the text files of `write_annotations`: <name>.txt, line-<name>.txt (when there are lines), <name>.json"""
     imname = imgname.replace(Path(imgname).suffix, "")
     polys, blk_xyxy, blk_dicts = [], [], []
     for blk in blk_list:
@@ -100,44 +103,84 @@ def write_annotations(save_dir, imgname, img, mask_refined, blk_list, save_json=
     if save_json:
         with open(osp.join(save_dir, imname + ".json"), "w", encoding="utf8") as f:
             f.write(json.dumps(blk_dicts, ensure_ascii=False, cls=NumpyEncoder))
+    return imname
+
+
+def write_annotations(save_dir, imgname, img, mask_refined, blk_list, save_json=False):
+    """The per-page part of `model2annotations` (inference.py:33-70) for an already detected page, PNGs by cv2."""
+    im_h, im_w = img.shape[:2]
+    imname = write_labels(save_dir, imgname, im_h, im_w, blk_list, save_json)
     imwrite(osp.join(save_dir, imgname), img)
     imwrite(osp.join(save_dir, "mask-" + imname + ".png"), mask_refined)
 
 
+def _read_pages(imglist, det, failed):
+    """(path, page) for each file in order, decoded in batches of det.max_batch with the detector's JpegDecoder
+    (baseline JPEGs on the GPU into CUDA pages, every other file by cv2).  A file that cannot be read ends the pages
+    there: its error goes to `failed`."""
+    for b0 in range(0, len(imglist), det.max_batch):
+        paths = imglist[b0:b0 + det.max_batch]
+        pages = det.jpeg_decoder().decode([np.fromfile(p, dtype=np.uint8) for p in paths])
+        for img_path, img in zip(paths, pages):
+            try:
+                img = check_page(img, det.device_index)
+            except ValueError as ex:
+                failed.append(ValueError("%s: %s" % (img_path, ex)))
+                return
+            yield img_path, img
+
+
 def model2annotations(model_path, img_dir_list, save_dir, save_json=False, detector=None):
-    """`model2annotations(model_path, img_dir_list, save_dir, save_json)` of the reference (inference.py:19-70)."""
+    """`model2annotations(model_path, img_dir_list, save_dir, save_json)` of the reference (inference.py:19-70).
+
+    The files are those `write_annotations` writes page by page, byte for byte.  Pages are read in batches of the
+    detector's max_batch and decoded with its JpegDecoder; a page decoded on the GPU stays there for the detection and
+    for its PNG.  The refined masks stay on the GPU (detect_stream's device_results), and both PNGs of every page of
+    a batch of results are encoded in one PngEncoder call."""
+    from .png import PngEncoder
     if isinstance(img_dir_list, str):
         img_dir_list = [img_dir_list]
     # batches of up to 8 pages (scripts/pages_bench.py: the fastest of the measured batch sizes)
     det = detector if detector is not None else TextDetector(model_path=model_path, input_size=1024, act="leaky",
                                                              max_batch=8)
     os.makedirs(save_dir, exist_ok=True)
+    enc = None
     try:
         imglist = []
         for d in img_dir_list:
             imglist += find_all_imgs(d, abs_path=True)
+        enc = PngEncoder(det.device_index)
         # pages are decoded while the previous batches run on the GPU (TextDetector.detect_stream); results come back
         # in input order, so each one is written with the page it belongs to.  A page that cannot be read ends the
         # stream there: every page before it is still written, then the error is raised, as page by page.
-        read, failed = deque(), []
+        read, failed, done = deque(), [], []
 
         def pages():
-            for img_path in imglist:
-                img = imread(img_path)
-                try:
-                    check_page(img)
-                except ValueError as ex:
-                    failed.append(ValueError("%s: %s" % (img_path, ex)))
-                    return
+            for img_path, img in _read_pages(imglist, det, failed):
                 read.append((img_path, img))
                 yield img
 
+        def flush():
+            files = enc.encode([x for _p, img, mask, _b in done for x in (img, mask)])
+            for k, (img_path, img, _mask, blk_list) in enumerate(done):
+                imgname = osp.basename(img_path)
+                imname = write_labels(save_dir, imgname, img.shape[0], img.shape[1], blk_list, save_json)
+                files[2 * k].tofile(png_path(osp.join(save_dir, imgname)))
+                files[2 * k + 1].tofile(png_path(osp.join(save_dir, "mask-" + imname + ".png")))
+            done.clear()
+
         for _mask, mask_refined, blk_list in det.detect_stream(pages(), refine_mode=REFINEMASK_ANNOTATION,
-                                                                keep_undetected_mask=True):
+                                                                keep_undetected_mask=True, device_results=True):
             img_path, img = read.popleft()
-            write_annotations(save_dir, osp.basename(img_path), img, mask_refined, blk_list, save_json)
+            done.append((img_path, img, mask_refined, blk_list))
+            if len(done) == det.max_batch:
+                flush()
+        if done:
+            flush()
         if failed:
             raise failed[0]
     finally:
+        if enc is not None:
+            enc.close()
         if detector is None:
             det.close()

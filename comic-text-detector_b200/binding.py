@@ -74,6 +74,13 @@ class CtdJpegInfo(C.Structure):
                [("ecs_bytes", C.c_int64)]
 
 
+class CtdPngImage(C.Structure):
+    """ctypes mirror of `ctd_png_image` (include/ctd_b200.h)"""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32),
+                ("bit_depth", C.c_int32), ("on_device", C.c_int32), ("stride_h", C.c_int64), ("stride_w", C.c_int64),
+                ("stride_c", C.c_int64), ("event", C.c_void_p)]
+
+
 class CtdDevicePage(C.Structure):
     """ctypes mirror of `ctd_device_page` (include/ctd_b200.h)"""
     _fields_ = [("data", C.c_void_p), ("stride_h", C.c_int64), ("stride_w", C.c_int64), ("stride_c", C.c_int64),
@@ -91,7 +98,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
            "ctd_submit_pages_regions", "ctd_collect_regions", "ctd_submit_pages_device", "ctd_collect_device",
            "ctd_forward_tensor", "ctd_jpeg_probe", "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy",
-           "ctd_jpeg_decode", "ctd_debug_postprocess"]
+           "ctd_jpeg_decode", "ctd_debug_postprocess", "ctd_png_encoder_create", "ctd_png_encoder_destroy",
+           "ctd_png_encode"]
 
 _lib = None
 
@@ -167,6 +175,10 @@ def load_library():
     for name in EXPORTS[3:]:
         getattr(lib, name).restype = C.c_int
     lib.ctd_jpeg_decoder_destroy.restype = None
+    lib.ctd_png_encoder_create.argtypes = [i32, C.POINTER(vp)]
+    lib.ctd_png_encoder_destroy.argtypes = [vp]
+    lib.ctd_png_encode.argtypes = [vp, C.POINTER(CtdPngImage), i32, vp, vp]
+    lib.ctd_png_encoder_destroy.restype = None
     lib.ctd_expand_textwindow.restype = None
     _lib = lib
     return lib

@@ -100,6 +100,12 @@ class TextDetector:
                           max_w=input_size[1], conf_thresh=conf_thresh, nms_thresh=nms_thresh, db_thresh=0.3)
         self._jpeg = None   # the JpegDecoder of encoded pages, made on first use
 
+    def jpeg_decoder(self):
+        """the JpegDecoder this detector decodes encoded pages with (made on first use, closed with the detector)"""
+        if self._jpeg is None:
+            self._jpeg = JpegDecoder(self.device_index)
+        return self._jpeg
+
     def close(self):
         self.net.close()
         if self._jpeg is not None:
@@ -225,9 +231,7 @@ class TextDetector:
         if not enc:
             return batch
         bufs = [read_encoded(batch[i].src) for i in enc]
-        if self._jpeg is None:
-            self._jpeg = JpegDecoder(self.device_index)
-        pages = self._jpeg.decode([b for b, _path in bufs])
+        pages = self.jpeg_decoder().decode([b for b, _path in bufs])
         batch = list(batch)
         for i, (_b, path), page in zip(enc, bufs, pages):
             if page is None:

@@ -582,6 +582,39 @@ CTD_API void ctd_jpeg_decoder_destroy(ctd_jpeg_decoder* dec);
 CTD_API int ctd_jpeg_decode(ctd_jpeg_decoder* dec, const uint8_t* const* data, const size_t* len, int32_t n,
                             uint8_t* const* dst, int32_t* status);
 
+/* ---- PNG files encoded on the GPU -------------------------------------------------------
+ * The reference writes pages and masks with io_utils.imwrite = cv2.imencode('.png', img).tofile(path).  These entry
+ * points encode u8 images on the GPU to exactly the bytes cv2.imencode('.png', img) gives with the libpng and zlib
+ * OpenCV 4.13 is built against (libpng 1.6.53, zlib 1.2.11) at OpenCV's PNG defaults: compression level 1, strategy
+ * Z_RLE, memLevel 8, filter SUB on every row (NONE for an image 1 pixel wide), IHDR / IDAT / IEND only, IDAT chunks of
+ * 8192 bytes of the zlib stream, and libpng's optimize_cmf window field for streams of at most 16 KiB.  The deflate
+ * stream restates zlib 1.2.11's deflate_rle parse and trees.c block by block (csrc/png.cu, oracle/png_ref.py).
+ *
+ * ctd_png_image describes one image: u8, `channels` 1 (grey [h][w]) or 3 (BGR [h][w][3]), bit_depth 8.  With
+ * on_device == 0, `data` is HOST memory, C-contiguous.  With on_device != 0, `data` is the DEVICE address of pixel
+ * (0, 0), channel 0, on the encoder's GPU, byte (y, x, c) at data + y * stride_h + x * stride_w + c * stride_c (each
+ * stride >= 0), and `event` (a cudaEvent_t, may be NULL) is waited on by the encoder's stream before the image is
+ * read.                                                                                                            */
+typedef struct ctd_png_image {
+  const uint8_t* data;
+  int32_t height, width, channels, bit_depth;
+  int32_t on_device;
+  int64_t stride_h, stride_w, stride_c;
+  void* event;
+} ctd_png_image;
+typedef struct ctd_png_encoder ctd_png_encoder;
+/* An encoder bound to one GPU and one stream of its own; staging, scratch and output buffers grow on demand.  Not
+ * thread-safe; errors via ctd_last_error(NULL).                                                                     */
+CTD_API int ctd_png_encoder_create(int32_t device, ctd_png_encoder** out);
+CTD_API void ctd_png_encoder_destroy(ctd_png_encoder* enc);
+/* Encodes n images at once.  files[i] / sizes[i] get image i's complete PNG file in pinned host memory owned by the
+ * encoder, valid until its next call.  Synchronises with the host once, at the end.  CTD_E_INVALID, before any GPU
+ * work, for a side < 1, channels other than 1 or 3, bit_depth other than 8, a negative stride or a device image
+ * that is not memory of the encoder's GPU; CTD_E_CAPACITY for 2^31 or more filtered bytes (h * (1 + w * channels),
+ * summed over the images) in one call.                                                                              */
+CTD_API int ctd_png_encode(ctd_png_encoder* enc, const ctd_png_image* images, int32_t n, const uint8_t** files,
+                           int64_t* sizes);
+
 #ifdef __cplusplus
 }
 #endif
