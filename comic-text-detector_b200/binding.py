@@ -9,7 +9,7 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libctd_b200.so")
 MAX_SRC = 3
-ABI_VERSION = 2
+ABI_VERSION = 3
 PREC_FP16_TC, PREC_FP32_SIMT, PREC_FP16_SIMT, PREC_SPLIT_TC = 0, 1, 2, 3
 
 
@@ -30,12 +30,6 @@ class CtdConfig(C.Structure):
                 ("max_h", C.c_int32), ("max_w", C.c_int32), ("nc", C.c_int32), ("use_graph", C.c_int32),
                 ("conf_thresh", C.c_float), ("nms_thresh", C.c_float), ("db_thresh", C.c_float),
                 ("debug_skip_postproc", C.c_int32)]
-
-
-class CtdDeviceOutputs(C.Structure):
-    _fields_ = [(k, C.c_void_p) for k in ("stream", "mask_u8", "det", "det_count", "bitmap", "labels", "n_labels",
-                                          "line_boxes", "line_scores", "line_count", "results_base")] + \
-               [("results_bytes", C.c_size_t)]
 
 
 # numpy mirror of `ctd_block` (include/ctd_b200.h)
@@ -90,16 +84,13 @@ class CtdDevicePage(C.Structure):
 EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_get_net_outputs", "ctd_get_mask_u8",
            "ctd_get_detections", "ctd_get_db_components", "ctd_last_forward_ms", "ctd_last_launch_count",
            "ctd_debug_read_buffer", "ctd_debug_write_buffer", "ctd_connected_components", "ctd_nms",
-           "ctd_timer_start", "ctd_timer_stop", "ctd_profile_forward", "ctd_get_device_outputs",
-           "ctd_get_text_lines", "ctd_seg_represent", "ctd_refine_mask", "ctd_submit", "ctd_collect",
-           "ctd_results_bytes", "ctd_join", "ctd_forward_resized", "ctd_get_mask_u8_resized",
-           "ctd_resize_linear_u8", "ctd_debug_run_ops", "ctd_get_nms_status", "ctd_group_output",
-           "ctd_expand_textwindow", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full", "ctd_device_arena",
-           "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
-           "ctd_submit_pages_regions", "ctd_collect_regions", "ctd_submit_pages_device", "ctd_collect_device",
-           "ctd_forward_tensor", "ctd_jpeg_probe", "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy",
-           "ctd_jpeg_decode", "ctd_debug_postprocess", "ctd_png_encoder_create", "ctd_png_encoder_destroy",
-           "ctd_png_encode"]
+           "ctd_timer_start", "ctd_timer_stop", "ctd_profile_forward", "ctd_get_text_lines", "ctd_seg_represent",
+           "ctd_refine_mask", "ctd_collect", "ctd_join", "ctd_resize_linear_u8", "ctd_debug_run_ops",
+           "ctd_get_nms_status", "ctd_group_output", "ctd_detect_page", "ctd_results_layout", "ctd_submit_full",
+           "ctd_device_arena", "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
+           "ctd_collect_regions", "ctd_collect_device", "ctd_forward_tensor", "ctd_jpeg_probe",
+           "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy", "ctd_jpeg_decode", "ctd_debug_postprocess",
+           "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode"]
 
 _lib = None
 
@@ -142,19 +133,13 @@ def load_library():
     lib.ctd_timer_start.argtypes = [vp]
     lib.ctd_timer_stop.argtypes = [vp, C.POINTER(C.c_float)]
     lib.ctd_profile_forward.argtypes = [vp, vp, i32, i32, i32, i32, vp, i32]
-    lib.ctd_get_device_outputs.argtypes = [vp, C.POINTER(CtdDeviceOutputs)]
-    lib.ctd_submit.argtypes = [vp, i32, vp, i32, i32, i32, vp]
     lib.ctd_collect.argtypes = [vp, i32]
-    lib.ctd_results_bytes.argtypes = [vp, C.POINTER(C.c_size_t)]
     lib.ctd_join.argtypes = [vp, vp]
-    lib.ctd_forward_resized.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32]
-    lib.ctd_get_mask_u8_resized.argtypes = [vp, i32, i32, i32, i32, vp]
     lib.ctd_resize_linear_u8.argtypes = [vp, vp, i32, i32, i32, vp, i32, i32]
     lib.ctd_debug_run_ops.argtypes = [vp, vp, i32, i32, i32, i32, i32]
     lib.ctd_debug_postprocess.argtypes = [vp, vp, vp, i32, i32, i32]
     lib.ctd_get_nms_status.argtypes = [vp, vp, C.POINTER(i32)]
     lib.ctd_group_output.argtypes = [vp, vp, i32, vp, i32, i32, i32, vp, i32, vp, i32, vp, i32, vp, i32, C.POINTER(i32)]
-    lib.ctd_expand_textwindow.argtypes = [i32, i32, vp, i32, vp]
     lib.ctd_detect_page.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, i32, vp, i32, C.POINTER(i32)]
     lib.ctd_results_layout.argtypes = [vp, C.POINTER(CtdResultsLayout)]
     lib.ctd_submit_full.argtypes = [vp, i32, vp, i32, i32, i32, i32, i32, vp]
@@ -162,11 +147,9 @@ def load_library():
     lib.ctd_region_plan.argtypes = [vp, i32, i32, i32, i32, vp, C.POINTER(C.c_size_t)]
     lib.ctd_transform_regions.argtypes = [vp, vp, i32, i32, i32, vp, i32, vp, C.c_size_t]
     lib.ctd_pages_plan.argtypes = [vp, i32, i32, i32, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
-    lib.ctd_submit_pages.argtypes = [vp, i32, vp, i32, i32, i32, vp, i32, i32, vp]
-    lib.ctd_submit_pages_regions.argtypes = [vp, i32, vp, i32, i32, i32, vp, i32, i32, i32, vp]
+    lib.ctd_submit_pages.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_collect_regions.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i32), C.POINTER(vp), C.POINTER(vp),
                                         C.POINTER(C.c_size_t)]
-    lib.ctd_submit_pages_device.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_collect_device.argtypes = [vp, i32, vp]
     lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
     lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
@@ -179,7 +162,6 @@ def load_library():
     lib.ctd_png_encoder_destroy.argtypes = [vp]
     lib.ctd_png_encode.argtypes = [vp, C.POINTER(CtdPngImage), i32, vp, vp]
     lib.ctd_png_encoder_destroy.restype = None
-    lib.ctd_expand_textwindow.restype = None
     _lib = lib
     return lib
 
@@ -309,21 +291,6 @@ class Engine:
         assert c == 3
         self._ck(self.lib.ctd_forward(self.h, _ptr(pages), n, h, w, 0))
         self.shape = (n, h, w)
-
-    def forward_resized(self, page, unpad_h, unpad_w, net_h, net_w):
-        """letterbox on the GPU: page u8 [ih][iw][3] of any size -> cv2-exact INTER_LINEAR resize to
-        unpad_h x unpad_w, zero padding to net_h x net_w, forward (n = 1)."""
-        page = np.ascontiguousarray(page, dtype=np.uint8)
-        ih, iw, c = page.shape
-        assert c == 3
-        self._ck(self.lib.ctd_forward_resized(self.h, _ptr(page), ih, iw, unpad_h, unpad_w, net_h, net_w))
-        self.shape = (1, net_h, net_w)
-
-    def mask_u8_resized(self, crop_h, crop_w, out_h, out_w):
-        """`cv2.resize(mask[:crop_h, :crop_w], (out_w, out_h), INTER_LINEAR)` of page 0 (inference.py:164-168)."""
-        out = np.empty((out_h, out_w), np.uint8)
-        self._ck(self.lib.ctd_get_mask_u8_resized(self.h, crop_h, crop_w, out_h, out_w, _ptr(out)))
-        return out
 
     def resize_linear_u8(self, src, dsize_wh):
         """`cv2.resize(src, dsize_wh, interpolation=cv2.INTER_LINEAR)` for uint8 [H,W] / [H,W,3] (bit-exact)."""
@@ -459,18 +426,7 @@ class Engine:
         self.shape = (n, h, w)
         return out[:nops], float(out[nops]), float(out[nops + 1])
 
-    # ---- pipelined host path: two batches in flight, copies under compute -----------------------
-    def results_bytes(self):
-        n = C.c_size_t()
-        self._ck(self.lib.ctd_results_bytes(self.h, C.byref(n)))
-        return int(n.value)
-
-    def submit(self, slot, pages_ptr, n, h, w, results_ptr):
-        """asynchronous forward of HOST pages (raw pointers, ideally pinned) into HOST `results`
-        (results_bytes() bytes; unpack with multigpu.unpack_arena)."""
-        self._ck(self.lib.ctd_submit(self.h, slot, C.c_void_p(pages_ptr), n, h, w, C.c_void_p(results_ptr)))
-        self.shape = (n, h, w)
-
+    # ---- batch pipeline: two batches in flight, copies under compute -----------------------------
     def results_layout(self):
         """byte offsets of the result arena (ctd_results_layout): dict of ints."""
         lay = CtdResultsLayout()
@@ -513,7 +469,7 @@ class Engine:
 
     def submit_pages(self, slot, pages, net_h, net_w, refine_mode=0, keep_undetected=False, textheight=0, events=None,
                      device_results=False):
-        """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages_device).  A page is a u8
+        """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages).  A page is a u8
         [h][w][3] numpy array, packed into this slot's pinned input buffer (which like the pinned results buffer belongs
         to the engine and grows on demand), or a torch.uint8 CUDA tensor [h][w][3] on this engine's GPU with any
         strides, gathered on the GPU without a host copy; events[i] (a recorded torch.cuda.Event, or None) is waited on
@@ -546,11 +502,11 @@ class Engine:
                 if not d:
                     o = int(e["page_off"])
                     np.copyto(inp[o:o + p.size].reshape(p.shape), p)
-        self._ck(self.lib.ctd_submit_pages_device(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
-                                                  None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
-                                                  None if dev is None else C.cast(dev, C.c_void_p), int(refine_mode),
-                                                  int(bool(keep_undetected)), int(textheight), int(bool(device_results)),
-                                                  C.c_void_p(bufs[1].data_ptr())))
+        self._ck(self.lib.ctd_submit_pages(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
+                                           None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
+                                           None if dev is None else C.cast(dev, C.c_void_p), int(refine_mode),
+                                           int(bool(keep_undetected)), int(textheight), int(bool(device_results)),
+                                           C.c_void_p(bufs[1].data_ptr())))
         kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]]
         self._pg_inflight[slot] = (entries, int(textheight), bool(device_results), kept)
         self.shape = (len(entries), net_h, net_w)
@@ -624,7 +580,7 @@ class Engine:
         return out
 
     def _collected_plan(self, slot, n_pages):
-        """the plan of the collected ctd_submit_pages_regions batch of `slot` (ctd_collect_regions)"""
+        """the plan of the collected ctd_submit_pages batch of `slot` (ctd_collect_regions)"""
         plan_p, n_reg, first_p, pix_p, nbytes = C.c_void_p(), C.c_int32(), C.c_void_p(), C.c_void_p(), C.c_size_t()
         self._ck(self.lib.ctd_collect_regions(self.h, slot, C.byref(plan_p), C.byref(n_reg), C.byref(first_p),
                                               C.byref(pix_p), C.byref(nbytes)))
@@ -635,7 +591,7 @@ class Engine:
         return _BatchPlan(plan, first, pix_p.value, int(nbytes.value))
 
     def collect_regions(self, slot, n_lines):
-        """the crops of the collected ctd_submit_pages_regions batch of `slot` (ctd_collect_regions): per page, per
+        """the crops of the collected ctd_submit_pages batch of `slot` (ctd_collect_regions): per page, per
         block a list of u8 [h][w][3] arrays in line order, None for a line the planner gives no crop (status != 0).
         n_lines: per page the block records' n_lines.  Each page's crops are views into one fresh array of that page
         (copied out of the engine's pinned buffer by torch's multi-threaded CPU copy: a single-threaded copy into fresh
@@ -655,11 +611,6 @@ class Engine:
     def join(self, other):
         """everything enqueued so far on `other`'s stream becomes a dependency of this engine's stream."""
         self._ck(self.lib.ctd_join(self.h, other.h))
-
-    def device_outputs(self):
-        o = CtdDeviceOutputs()
-        self._ck(self.lib.ctd_get_device_outputs(self.h, C.byref(o)))
-        return o
 
     def debug_write(self, tensor, arr, n, h, w):
         """fill a whole buffer (all its channels) from float32 [n][h/down][w/down][channels]."""

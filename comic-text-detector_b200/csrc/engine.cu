@@ -238,9 +238,8 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
     const BlockSection bs = block_section_layout();
     L.rec_off = bs.rec_off; L.lines_off = bs.lines_off; L.dist_off = bs.dist_off; L.blocks_stride = bs.stride;
     L.total = L.blocks + nb * L.blocks_stride;
-    h->results_bytes = L.total;
-    CKC(cudaMalloc(&h->d_mask_u8, h->results_bytes));
-    CKC(cudaMemset(h->d_mask_u8, 0, h->results_bytes));
+    CKC(cudaMalloc(&h->d_mask_u8, L.total));
+    CKC(cudaMemset(h->d_mask_u8, 0, L.total));
     h->d_det = reinterpret_cast<float*>(h->d_mask_u8 + L.det);
     h->d_det_count = reinterpret_cast<int*>(h->d_mask_u8 + L.cnt);
     h->d_nlabels = reinterpret_cast<int32_t*>(h->d_mask_u8 + L.nl);
@@ -618,11 +617,6 @@ extern "C" int ctd_forward_tensor(ctd_handle* h, const float* x, int32_t n, int3
   return CTD_OK;
 }
 
-// ---- pipelined host path ---------------------------------------------------------------------------
-// submit(slot): copy_in: [wait slot's staging free] H2D pages -> stage_in[slot]
-//               compute: [wait H2D] stage_in -> d_pages (D2D), forward, arena -> stage_out[slot] (D2D)
-//               copy_out: [wait arena copy] D2H stage_out[slot] -> results_host
-// so the H2D of batch i+1 and the D2H of batch i-1 run under the forward of batch i.
 template <bool kPinned>
 int GrowBuf<kPinned>::grow(ctd_handle* h, size_t bytes, std::optional<cudaStream_t> sync, size_t headroom) {
   if (bytes <= cap) return CTD_OK;
@@ -656,106 +650,6 @@ void Slot::release() {
   *this = Slot();
 }
 
-int ensure_pipeline(ctd_handle* h) {
-  if (h->copy_in) return CTD_OK;
-  CK(cudaStreamCreateWithFlags(&h->copy_in, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&h->copy_out, cudaStreamNonBlocking));
-  const size_t in_bytes = size_t(h->cfg.max_batch) * h->cfg.max_h * h->cfg.max_w * 3;
-  for (Slot& s : h->slot) {
-    CK(cudaMalloc(&s.d_stage_in, in_bytes));
-    CK(cudaMalloc(&s.d_stage_out, h->results_bytes));
-    for (cudaEvent_t* e : {&s.ev_in_done, &s.ev_in_free, &s.ev_out_ready, &s.ev_out_done})
-      CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-  }
-  return CTD_OK;
-}
-
-int stage_phase_a(ctd_handle* h, Slot& s, const uint8_t* pages, bool pages_on_device, int n, int ph, int pw,
-                  ShapePlan& sp, void* results_host) {
-  const size_t bytes = size_t(n) * ph * pw * 3;
-  if (!pages_on_device) {
-    CK(cudaStreamWaitEvent(h->copy_in, s.ev_in_free, 0));   // no-op before the slot's first use
-    CK(cudaMemcpyAsync(s.d_stage_in, pages, bytes, cudaMemcpyHostToDevice, h->copy_in));
-    CK(cudaEventRecord(s.ev_in_done, h->copy_in));
-    CK(cudaEventRecord(h->ev0, h->stream));
-    CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
-    CK(cudaMemcpyAsync(h->d_pages, s.d_stage_in, bytes, cudaMemcpyDeviceToDevice, h->stream));
-    CK(cudaEventRecord(s.ev_in_free, h->stream));
-  } else {
-    CK(cudaEventRecord(h->ev0, h->stream));
-    CK(cudaMemcpyAsync(h->d_pages, pages, bytes, cudaMemcpyDeviceToDevice, h->stream));
-  }
-  if (int rc = enqueue_forward(h, n, ph, pw, sp)) return rc;
-  CK(cudaStreamWaitEvent(h->stream, s.ev_out_done, 0));  // previous D2H of this slot has drained
-  CK(cudaMemcpyAsync(s.d_stage_out, h->d_mask_u8, h->layout.a_bytes, cudaMemcpyDeviceToDevice, h->stream));
-  CK(cudaEventRecord(s.ev_out_ready, h->stream));
-  CK(cudaStreamWaitEvent(h->copy_out, s.ev_out_ready, 0));
-  CK(cudaMemcpyAsync(results_host, s.d_stage_out, h->layout.a_bytes, cudaMemcpyDeviceToHost, h->copy_out));
-  CK(cudaEventRecord(s.ev_out_done, h->copy_out));
-  return CTD_OK;
-}
-
-extern "C" int ctd_submit(ctd_handle* h, int32_t slot, const uint8_t* pages_host, int32_t n, int32_t ph, int32_t pw,
-                          void* results_host) {
-  if (!h || !pages_host || !results_host || slot < 0 || slot > 1) return CTD_E_INVALID;
-  if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit needs the full pipeline");
-  Slot& s = h->slot[slot];
-  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
-  ShapePlan* sp = nullptr;
-  if (int rc = prepare_forward(h, n, ph, pw, &sp)) return rc;
-  if (int rc = ensure_pipeline(h)) return rc;
-  s.start(false, false);
-  if (int rc = stage_phase_a(h, s, pages_host, false, n, ph, pw, *sp, results_host)) return rc;
-  s.busy = true;
-  return CTD_OK;
-}
-
-extern "C" int ctd_collect(ctd_handle* h, int32_t slot) {
-  if (!h || slot < 0 || slot > 1) return CTD_E_INVALID;
-  Slot& s = h->slot[slot];
-  if (!s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has nothing in flight", slot);
-  CK(cudaSetDevice(h->cfg.device));
-  if (s.full) {
-    const int rc = ctd_collect_full(h, slot);
-    s.busy = false;
-    return rc;
-  }
-  CK(cudaEventSynchronize(s.ev_out_done));
-  s.busy = false;
-  s.collected = true;
-  return CTD_OK;
-}
-
-extern "C" int ctd_forward_resized(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t unpad_h,
-                                   int32_t unpad_w, int32_t net_h, int32_t net_w) {
-  if (!h || !page) return CTD_E_INVALID;
-  if (ih < 1 || iw < 1 || unpad_h < 1 || unpad_w < 1 || unpad_h > net_h || unpad_w > net_w)
-    return ctd_fail(h, CTD_E_SHAPE, "letterbox %dx%d -> %dx%d does not fit the %dx%d net input", ih, iw, unpad_h, unpad_w, net_h, net_w);
-  ShapePlan* sp = nullptr;
-  if (int rc = prepare_forward(h, 1, net_h, net_w, &sp)) return rc;
-  const size_t bytes = size_t(ih) * iw * 3;
-  if (int rc = h->io_scratch.grow(h, bytes, h->stream)) return rc;
-  CK(cudaEventRecord(h->ev0, h->stream));
-  CK(cudaMemcpyAsync(h->io_scratch.p, page, bytes, cudaMemcpyHostToDevice, h->stream));
-  CK(resize_linear_u8_launch(h->io_scratch.p, ih, iw, size_t(iw) * 3, 3, h->d_pages, unpad_h, unpad_w, net_h, net_w, h->stream));
-  return enqueue_forward(h, 1, net_h, net_w, *sp);
-}
-
-extern "C" int ctd_get_mask_u8_resized(ctd_handle* h, int32_t crop_h, int32_t crop_w, int32_t out_h, int32_t out_w,
-                                       uint8_t* mask_out) {
-  if (!h || !mask_out) return CTD_E_INVALID;
-  if (!h->have_forward) return ctd_fail(h, CTD_E_INVALID, "no forward pass has been run on this handle");
-  if (crop_h < 1 || crop_w < 1 || crop_h > h->ph || crop_w > h->pw || out_h < 1 || out_w < 1)
-    return ctd_fail(h, CTD_E_SHAPE, "bad crop %dx%d of the %dx%d mask", crop_h, crop_w, h->ph, h->pw);
-  CK(cudaSetDevice(h->cfg.device));
-  const size_t bytes = size_t(out_h) * out_w;
-  if (int rc = h->io_scratch.grow(h, bytes, h->stream)) return rc;
-  CK(resize_linear_u8_launch(h->d_mask_u8, crop_h, crop_w, size_t(h->pw), 1, h->io_scratch.p, out_h, out_w, out_h, out_w, h->stream));
-  CK(cudaMemcpyAsync(mask_out, h->io_scratch.p, bytes, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return CTD_OK;
-}
-
 extern "C" int ctd_resize_linear_u8(ctd_handle* h, const uint8_t* src, int32_t sh, int32_t sw, int32_t channels, uint8_t* dst,
                                     int32_t dh, int32_t dw) {
   if (!h || !src || !dst) return CTD_E_INVALID;
@@ -778,12 +672,6 @@ extern "C" int ctd_join(ctd_handle* h, ctd_handle* other) {
   CK(cudaSetDevice(h->cfg.device));
   CK(cudaEventRecord(other->ev_xjoin, other->stream));
   CK(cudaStreamWaitEvent(h->stream, other->ev_xjoin, 0));
-  return CTD_OK;
-}
-
-extern "C" int ctd_results_bytes(ctd_handle* h, size_t* bytes) {
-  if (!h || !bytes) return CTD_E_INVALID;
-  *bytes = h->results_bytes;
   return CTD_OK;
 }
 
@@ -926,24 +814,6 @@ extern "C" int ctd_profile_forward(ctd_handle* h, const uint8_t* pages, int32_t 
   h->n = n; h->ph = ph; h->pw = pw;
   h->have_forward = true;
   h->last_launches = launches;
-  return CTD_OK;
-}
-
-extern "C" int ctd_get_device_outputs(ctd_handle* h, ctd_device_outputs* out) {
-  NEED_FWD();
-  if (!out) return CTD_E_INVALID;
-  out->stream = h->stream;
-  out->mask_u8 = h->d_mask_u8;
-  out->det = h->d_det;
-  out->det_count = h->d_det_count;
-  out->bitmap = h->d_bitmap;
-  out->labels = h->d_labels;
-  out->n_labels = h->d_nlabels;
-  out->line_boxes = h->d_line_boxes;
-  out->line_scores = h->d_line_scores;
-  out->line_count = h->d_line_count;
-  out->results_base = h->d_mask_u8;
-  out->results_bytes = h->results_bytes;
   return CTD_OK;
 }
 

@@ -102,7 +102,7 @@ struct PipeJob {
   uint8_t* d_blocks = nullptr;
   size_t blocks_bytes = 0;
   int keep_undetected = 0;
-  int textheight = 0;   // > 0: also crop every text line of every page (ctd_submit_pages_regions)
+  int textheight = 0;   // > 0: also crop every text line of every page (ctd_submit_pages)
   int results_on_device = 0;   // mask_refined, the modified mask and the crops stay on the device (ctd_collect_device)
 };
 
@@ -120,16 +120,15 @@ struct GrowBuf {
 using DevBuf = GrowBuf<false>;
 using PinnedBuf = GrowBuf<true>;
 
-// one of the two slots of the pipelined paths (ctd_submit, ctd_submit_full, ctd_submit_pages*): the staging and events
-// of a batch in flight, its hand-over from the worker, and the buffers its results stay in until the next submission
+// one of the two slots of the batch pipeline (ctd_submit_full, ctd_submit_pages): the staging and events of a batch
+// in flight, its hand-over from the worker, and the buffers its results stay in until the next submission
 struct Slot {
-  // ctd_submit / ctd_submit_full staging (ensure_pipeline): the pages, and the phase-A section of the arena
+  // ctd_submit_full staging: the pages, and the device copy of the result arena (ctd_device_arena)
   uint8_t* d_stage_in = nullptr;
   uint8_t* d_stage_out = nullptr;
   cudaEvent_t ev_in_done = nullptr, ev_in_free = nullptr, ev_out_ready = nullptr, ev_out_done = nullptr;
   cudaEvent_t ev_post_done = nullptr;   // phase C of the batch has run (post stream)
   bool busy = false;                    // submitted and not collected
-  bool full = false;                    // collected through the worker (ctd_submit_full, ctd_submit_pages*)
   // what the batch asked for (start()), and whether it was collected without error: the results ctd_collect_regions
   // and ctd_collect_device hand out
   bool crops = false, on_device = false, collected = false;
@@ -222,7 +221,6 @@ struct ctd_handle {
   float* d_blks = nullptr;
   float* d_mask = nullptr;
   uint8_t* d_mask_u8 = nullptr;   // start of the contiguous result arena: mask_u8 | det | det_count | n_labels
-  size_t results_bytes = 0;
   float* d_lines = nullptr;
   uint8_t* d_bitmap = nullptr;
   float* d_det = nullptr;
@@ -233,7 +231,7 @@ struct ctd_handle {
   void* d_segrep_scratch = nullptr;
   DevBuf refine_scratch;   // refine_mask on the engine stream
   DevBuf cc_scratch;       // ctd_connected_components: any image size
-  DevBuf io_scratch;       // page upload / resized mask staging of the resize entry points
+  DevBuf io_scratch;       // page and mask staging of the stand-alone entry points and ctd_detect_page
   int16_t* d_line_boxes = nullptr;
   float* d_line_scores = nullptr;
   int32_t* d_line_count = nullptr;
@@ -244,7 +242,7 @@ struct ctd_handle {
   // valid), and the events that order the engine stream after the caller's stream and back
   DevBuf in_stage;
   cudaEvent_t ev_tin = nullptr, ev_tout = nullptr;
-  // pipelined host path (ctd_submit / ctd_collect): two slots, copy streams either side of compute
+  // batch pipeline (ctd_submit_full, ctd_submit_pages / ctd_collect): two slots, copy streams either side of compute
   cudaStream_t copy_in = nullptr, copy_out = nullptr;
   Slot slot[2];
   // overlapped schedule (programs with a DB tail): post-processing of the DB maps / the Detect rows runs on side
@@ -280,16 +278,9 @@ struct ctd_handle {
 int ctd_fail(ctd_handle* h, int code, const char* fmt, ...);
 int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out, int input = INPUT_U8);
 int enqueue_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan& sp);
-int ensure_pipeline(ctd_handle* h);
-// phase A of a batch of n net-sized pages on slot s, enqueued on the copy streams and the engine stream: the pages
-// (host pages through s.d_stage_in) into d_pages, the forward, the arena's phase-A section to s.d_stage_out and on to
-// results_host
-int stage_phase_a(ctd_handle* h, Slot& s, const uint8_t* pages, bool pages_on_device, int n, int ph, int pw,
-                  ShapePlan& sp, void* results_host);
 // connected components + stats of a DEVICE u8 image on the engine stream (grow-on-demand scratch): *d_stats points at
 // [stats_cap][5] ints on the device, *n_labels is read back (synchronises the stream)
 int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap, int32_t** d_stats, int32_t* n_labels);
 int launch_refine(ctd_handle* h, const RefineJob& job, const uint8_t* d_img, const uint8_t* d_mask, int refine_mode,
                   uint8_t* d_out, cudaStream_t st, DevBuf& scratch, char* pinned);
-int ctd_collect_full(ctd_handle* h, int slot);
 void ctd_pipeline_shutdown(ctd_handle* h);

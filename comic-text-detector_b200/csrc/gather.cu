@@ -1,4 +1,4 @@
-// Batched strided page gather (ctd_submit_pages_device): every page of a batch that is already in device memory, laid
+// Batched strided page gather (ctd_submit_pages): every page of a batch that is already in device memory, laid
 // out with any strides (a sub-window of a larger image, a permuted channels-first image), copied in one launch into the
 // packed page buffer of the batch (u8 BGR [ih][iw][3] at the page's page_off), where the letterbox, refine_mask and the
 // crop kernels read it.  One CTA per row over the stacked rows of the gathered pages, as backproject_batch_kernel.

@@ -2,11 +2,11 @@
 //
 // Replaces the reference's `group_output` and its callees (utils/textblock.py:421-508 group_output, 302-342
 // examine_textblk, 344-373 try_merge_textline, 375-388 merge_textlines, 390-419 split_textblk, 267-300
-// sort_textblk_list, 87-106 adjust_bbox / sort_lines; utils/imgproc_utils.py:13-20 union_area, 151-161
-// expand_textwindow).  The stage is a serial walk over <= 300 detector boxes and <= 1000 line quads per page whose
-// float64 results are truncated to integers, so it runs on the host in IEEE double arithmetic with glibc's
-// acos / sin / atan2 (SURVEY section 7): every sum the reference forms over line coordinates is a sum of
-// half-integers and therefore exact in double, independent of numpy's reduction order or BLAS's use of FMA.
+// sort_textblk_list, 87-106 adjust_bbox / sort_lines; utils/imgproc_utils.py:13-20 union_area).  The stage is a
+// serial walk over <= 300 detector boxes and <= 1000 line quads per page whose float64 results are truncated to
+// integers, so it runs on the host in IEEE double arithmetic with glibc's acos / sin / atan2 (SURVEY section 7): every
+// sum the reference forms over line coordinates is a sum of half-integers and therefore exact in double, independent
+// of numpy's reduction order or BLAS's use of FMA.
 // shapely's `Polygon.intersects` (closed-set intersection of two quads) is an exact integer predicate here.
 //
 // Data model: a block is a struct of scalars plus a list of 4-point lines and a list of per-line distances (the
@@ -433,16 +433,4 @@ extern "C" int ctd_group_output(const int32_t* blk_xyxy, const int32_t* blk_cls,
     for (double d : b.distance) dist_out[d0++] = d;
   }
   return CTD_OK;
-}
-
-// expand_textwindow(img.shape, xyxy, expand_r) (utils/imgproc_utils.py:151-161) followed by the python slice
-// normalisation `img[y1:y2, x1:x2]` applies to it: win = {x1, y1, x2, y2} with 0 <= x1 <= x2 <= im_w etc.
-extern "C" void ctd_expand_textwindow(int32_t im_w, int32_t im_h, const int32_t* xyxy, int32_t expand_r, int32_t* win) {
-  const int64_t w = int64_t(xyxy[2]) - xyxy[0], h = int64_t(xyxy[3]) - xyxy[1];
-  const int64_t pad = int64_t(py_round((double(std::max(h, w)) * 0.25 + double(std::min(h, w)) * 0.75) / double(expand_r)));
-  int64_t x1 = std::max<int64_t>(0, xyxy[0] - pad), y1 = std::max<int64_t>(0, xyxy[1] - pad);
-  int64_t x2 = std::min<int64_t>(im_w - 1, xyxy[2] + pad), y2 = std::min<int64_t>(im_h - 1, xyxy[3] + pad);
-  py_slice(x1, x2, im_w);
-  py_slice(y1, y2, im_h);
-  win[0] = int32_t(x1); win[1] = int32_t(y1); win[2] = int32_t(x2); win[3] = int32_t(y2);
 }

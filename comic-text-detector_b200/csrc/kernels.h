@@ -241,7 +241,7 @@ cudaError_t letterbox_batch_launch(const uint8_t* src, const PageGeom* d_tab, in
 cudaError_t backproject_batch_launch(const uint8_t* mask, int net_h, int net_w, const PageGeom* d_tab, int n,
                                      int total_rows, uint8_t* dst, cudaStream_t s);
 
-// Pages of a batch that are already in device memory (ctd_submit_pages_device), gathered into the packed page buffer
+// Pages of a batch that are already in device memory (ctd_submit_pages), gathered into the packed page buffer
 // (gather.cu): byte (y, x, c) of the source is at src + y * sh + x * sw + c * sc; the packed page is u8 BGR [ih][iw][3]
 // at dst + dst_off.  The page owns rows [row0, row0 + ih) of the stacked rows of the launch's pages.  fast: sc == 1 and
 // sw == 3 (rows are contiguous runs of iw * 3 bytes at any pitch), copied with the widest accesses the alignment of

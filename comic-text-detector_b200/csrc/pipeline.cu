@@ -11,10 +11,10 @@
 // the refine kernels of batch i overlap the forward of batch i+1.  ctd_detect_page is the blocking single-page form
 // for pages of any size (letterbox + back-projection on the GPU), the call behind the drop-in TextDetector.
 // ctd_submit_pages runs batches of pages of any size through the same two-in-flight schedule, with one letterbox and
-// one back-projection launch per batch (TextDetector.detect_batch / detect_stream); ctd_submit_pages_regions also cuts
-// every text line of every page of the batch out of the resident pages in one k_warp_regions launch (region.cu).
-// ctd_submit_pages_device is the one implementation behind both: pages may already be in device memory (any strides;
-// one gather_pages_kernel launch packs them, gather.cu) and the masks and crops may stay there (ctd_collect_device).
+// one back-projection launch per batch (TextDetector.detect_batch / detect_stream); with a textheight it also cuts
+// every text line of every page of the batch out of the resident pages in one k_warp_regions launch (region.cu).  Its
+// pages may already be in device memory (any strides; one gather_pages_kernel launch packs them, gather.cu) and the
+// masks and crops may stay there (ctd_collect_device).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -159,6 +159,15 @@ PageIn page_in(const char* res, const PagesHead& head, int i, const JobPage& p, 
   return in;
 }
 
+// expand_textwindow(img.shape, xyxy, 16) (utils/imgproc_utils.py:151-161) on an im_w x im_h page: win = x1 y1 x2 y2,
+// without the python slice normalisation (RefineJob::add applies it)
+std::array<int32_t, 4> expand_textwindow(int64_t x1, int64_t y1, int64_t x2, int64_t y2, int im_w, int im_h) {
+  const int64_t w = x2 - x1, h = y2 - y1;
+  const int64_t pad = int64_t(nearbyint((double(std::max(h, w)) * 0.25 + double(std::min(h, w)) * 0.75) / 16.0));
+  return {int32_t(std::max<int64_t>(0, x1 - pad)), int32_t(std::max<int64_t>(0, y1 - pad)),
+          int32_t(std::min<int64_t>(im_w - 1, x2 + pad)), int32_t(std::min<int64_t>(im_h - 1, y2 + pad))};
+}
+
 // inference.py:101-114 (postprocess_yolo casts), 158-172 (box_thresh, line rescale), textblock.group_output,
 // expand_textwindow(.., 16): fills the page's block section and appends its refine windows
 int host_group_page(const PageIn& in, char* section, const BlockSection& L, std::vector<int32_t>& win_out) {
@@ -208,14 +217,9 @@ int host_group_page(const PageIn& in, char* section, const BlockSection& L, std:
   hdr->n_dist = td;
   win_out.resize(size_t(nb) * 4);
   for (int i = 0; i < nb; ++i) {
-    // expand_textwindow without the slice normalisation (RefineJob::add applies it)
     const int32_t* xy = rec[i].xyxy;
-    const int64_t w = int64_t(xy[2]) - xy[0], hh = int64_t(xy[3]) - xy[1];
-    const int64_t pad = int64_t(nearbyint((double(std::max(hh, w)) * 0.25 + double(std::min(hh, w)) * 0.75) / 16.0));
-    win_out[4 * i + 0] = int32_t(std::max<int64_t>(0, xy[0] - pad));
-    win_out[4 * i + 1] = int32_t(std::max<int64_t>(0, xy[1] - pad));
-    win_out[4 * i + 2] = int32_t(std::min<int64_t>(in.im_w - 1, xy[2] + pad));
-    win_out[4 * i + 3] = int32_t(std::min<int64_t>(in.im_h - 1, xy[3] + pad));
+    const auto win = expand_textwindow(xy[0], xy[1], xy[2], xy[3], in.im_w, in.im_h);
+    std::copy(win.begin(), win.end(), win_out.begin() + 4 * i);
   }
   return CTD_OK;
 }
@@ -325,11 +329,7 @@ int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Pl
         if (a > score) score = a;
       }
       if (double(score) / double(s5[2]) / double(s5[3]) < 0.5) {
-        int32_t xy[4] = {int32_t(bb[0]), int32_t(bb[1]), int32_t(bb[2]), int32_t(bb[3])}, w4[4];
-        const int64_t w = bb[2] - bb[0], hh = bb[3] - bb[1];
-        const int64_t pad = int64_t(nearbyint((double(std::max(hh, w)) * 0.25 + double(std::min(hh, w)) * 0.75) / 16.0));
-        w4[0] = int32_t(std::max<int64_t>(0, xy[0] - pad)); w4[1] = int32_t(std::max<int64_t>(0, xy[1] - pad));
-        w4[2] = int32_t(std::min<int64_t>(p.iw - 1, xy[2] + pad)); w4[3] = int32_t(std::min<int64_t>(p.ih - 1, xy[3] + pad));
+        const auto w4 = expand_textwindow(bb[0], bb[1], bb[2], bb[3], p.iw, p.ih);
         rj2.add(w4[0], w4[1], w4[2], w4[3], p.off, p.iw, p.ih);
       }
     }
@@ -501,7 +501,7 @@ static int run_batch(ctd_handle* h, const PipeJob& job) {
   }
   // phase C on the post stream over the slot's resident pages and masks
   cudaStream_t st = h->post;
-  // enqueued here for ctd_submit_pages*, not at submit: a wait enqueued at submit time would also hold this batch's
+  // enqueued here for ctd_submit_pages, not at submit: a wait enqueued at submit time would also hold this batch's
   // phase C behind the forward of every batch submitted before the worker reached it (ctd_submit_full enqueues it at
   // submit as well)
   CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // phase C never starts before its phase A copy
@@ -576,12 +576,14 @@ static void queue_job(ctd_handle* h, PipeJob&& job) {
   }
   h->pipe_cv.notify_one();
   s.busy = true;
-  s.full = true;
 }
 
+// the handle's pipeline, set up by its first submission: copy streams, post stream, each slot's staging, events and
+// pinned window tables, and the worker thread
 static int ensure_full_pipeline(ctd_handle* h) {
-  if (int rc = ensure_pipeline(h)) return rc;
   if (h->pipe_thread.joinable()) return CTD_OK;
+  CK(cudaStreamCreateWithFlags(&h->copy_in, cudaStreamNonBlocking));
+  CK(cudaStreamCreateWithFlags(&h->copy_out, cudaStreamNonBlocking));
   int lo = 0, hi = 0;
   CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
   CK(cudaStreamCreateWithPriority(&h->post, cudaStreamNonBlocking, hi));
@@ -589,9 +591,13 @@ static int ensure_full_pipeline(ctd_handle* h) {
   // (16 bytes each)
   h->pipe_pinned_cap = size_t(h->cfg.max_batch) * (size_t(CTD_MAX_BLOCKS) * sizeof(RefineWin) +
                                                    size_t(CTD_MAX_BLOCKS) * sizeof(RefineChunk) * 8) + (size_t(8) << 20);
+  const size_t in_bytes = size_t(h->cfg.max_batch) * h->cfg.max_h * h->cfg.max_w * 3;
   for (Slot& s : h->slot) {
+    CK(cudaMalloc(&s.d_stage_in, in_bytes));
+    CK(cudaMalloc(&s.d_stage_out, h->layout.total));
+    for (cudaEvent_t* e : {&s.ev_in_done, &s.ev_in_free, &s.ev_out_ready, &s.ev_out_done, &s.ev_post_done})
+      CK(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     CK(cudaHostAlloc(reinterpret_cast<void**>(&s.pinned), h->pipe_pinned_cap, cudaHostAllocDefault));
-    CK(cudaEventCreateWithFlags(&s.ev_post_done, cudaEventDisableTiming));
   }
   const char* ht = getenv("CTD_HOST_THREADS");
   const unsigned hc = std::thread::hardware_concurrency();
@@ -617,6 +623,36 @@ void ctd_pipeline_shutdown(ctd_handle* h) {
   h->dev_out = nullptr;
   h->pg_cc.release();
   h->post_refine.release();
+}
+
+// phase A of a batch of n net-sized pages on slot s:
+//   copy_in:  [wait slot's staging free] H2D pages -> stage_in[slot]
+//   compute:  [wait H2D] stage_in -> d_pages (D2D), forward, arena -> stage_out[slot] (D2D)
+//   copy_out: [wait arena copy] D2H stage_out[slot] -> results_host
+// so the H2D of batch i+1 and the D2H of batch i-1 run under the forward of batch i.  Device pages skip copy_in.
+static int stage_phase_a(ctd_handle* h, Slot& s, const uint8_t* pages, bool pages_on_device, int n, int ph, int pw,
+                         ShapePlan& sp, void* results_host) {
+  const size_t bytes = size_t(n) * ph * pw * 3;
+  if (!pages_on_device) {
+    CK(cudaStreamWaitEvent(h->copy_in, s.ev_in_free, 0));   // no-op before the slot's first use
+    CK(cudaMemcpyAsync(s.d_stage_in, pages, bytes, cudaMemcpyHostToDevice, h->copy_in));
+    CK(cudaEventRecord(s.ev_in_done, h->copy_in));
+    CK(cudaEventRecord(h->ev0, h->stream));
+    CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
+    CK(cudaMemcpyAsync(h->d_pages, s.d_stage_in, bytes, cudaMemcpyDeviceToDevice, h->stream));
+    CK(cudaEventRecord(s.ev_in_free, h->stream));
+  } else {
+    CK(cudaEventRecord(h->ev0, h->stream));
+    CK(cudaMemcpyAsync(h->d_pages, pages, bytes, cudaMemcpyDeviceToDevice, h->stream));
+  }
+  if (int rc = enqueue_forward(h, n, ph, pw, sp)) return rc;
+  CK(cudaStreamWaitEvent(h->stream, s.ev_out_done, 0));  // previous D2H of this slot has drained
+  CK(cudaMemcpyAsync(s.d_stage_out, h->d_mask_u8, h->layout.a_bytes, cudaMemcpyDeviceToDevice, h->stream));
+  CK(cudaEventRecord(s.ev_out_ready, h->stream));
+  CK(cudaStreamWaitEvent(h->copy_out, s.ev_out_ready, 0));
+  CK(cudaMemcpyAsync(results_host, s.d_stage_out, h->layout.a_bytes, cudaMemcpyDeviceToHost, h->copy_out));
+  CK(cudaEventRecord(s.ev_out_done, h->copy_out));
+  return CTD_OK;
 }
 
 extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages, int32_t n, int32_t ph, int32_t pw,
@@ -652,21 +688,6 @@ extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages
   return CTD_OK;
 }
 
-extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
-                                int32_t net_w, const uint8_t* input_host, int32_t refine_mode, int32_t keep_undetected,
-                                void* results_host) {
-  return ctd_submit_pages_regions(h, slot, pages, n, net_h, net_w, input_host, refine_mode, keep_undetected, 0,
-                                  results_host);
-}
-
-extern "C" int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
-                                        int32_t net_h, int32_t net_w, const uint8_t* input_host, int32_t refine_mode,
-                                        int32_t keep_undetected, int32_t textheight, void* results_host) {
-  if (!input_host) return CTD_E_INVALID;
-  return ctd_submit_pages_device(h, slot, pages, n, net_h, net_w, input_host, nullptr, refine_mode, keep_undetected,
-                                 textheight, 0, results_host);
-}
-
 // true when [p, p + 1) is device memory of `device` (cudaPointerGetAttributes; clears the error it may leave)
 static bool is_device_memory(const void* p, int device) {
   cudaPointerAttributes a{};
@@ -677,10 +698,10 @@ static bool is_device_memory(const void* p, int device) {
   return a.type == cudaMemoryTypeDevice && a.device == device;
 }
 
-extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
-                                       int32_t net_h, int32_t net_w, const uint8_t* input_host,
-                                       const ctd_device_page* dev, int32_t refine_mode, int32_t keep_undetected,
-                                       int32_t textheight, int32_t results_on_device, void* results_host) {
+extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                                int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
+                                int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
+                                int32_t results_on_device, void* results_host) {
   if (!h || !pages || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
   if (textheight != 0 && textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
   if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit_pages needs the full pipeline");
@@ -823,9 +844,11 @@ extern "C" int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_pa
   return CTD_OK;
 }
 
-// called by ctd_collect for slots submitted with ctd_submit_full or ctd_submit_pages
-int ctd_collect_full(ctd_handle* h, int slot) {
+extern "C" int ctd_collect(ctd_handle* h, int32_t slot) {
+  if (!h || slot < 0 || slot > 1) return CTD_E_INVALID;
   Slot& s = h->slot[slot];
+  if (!s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has nothing in flight", slot);
+  CK(cudaSetDevice(h->cfg.device));
   int rc;
   {
     std::unique_lock<std::mutex> lk(h->pipe_mu);
@@ -834,7 +857,7 @@ int ctd_collect_full(ctd_handle* h, int slot) {
     if (rc != CTD_OK) h->err = s.err;
     s.state = 0;
   }
-  s.full = false;
+  s.busy = false;
   if (rc != CTD_OK) return rc;
   CK(cudaEventSynchronize(s.ev_post_done));
   s.collected = true;
@@ -877,7 +900,7 @@ extern "C" int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region
   if (!h || slot < 0 || slot > 1 || !plan || !n_regions || !page_first || !pixels || !bytes) return CTD_E_INVALID;
   const Slot& s = h->slot[slot];
   if (s.busy || !s.collected || !s.crops)
-    return ctd_fail(h, CTD_E_INVALID, "slot %d holds no collected ctd_submit_pages_regions batch", slot);
+    return ctd_fail(h, CTD_E_INVALID, "slot %d holds no collected ctd_submit_pages batch with a textheight", slot);
   *plan = s.crop_plan.data();
   *n_regions = int32_t(s.crop_plan.size());
   *page_first = s.crop_first.data();

@@ -1,8 +1,9 @@
 // Text-line crops (C ABI `ctd_transform_regions`, include/ctd_b200.h): `cv2.warpPerspective(img, M, (w, h))` with
 // INTER_LINEAR / BORDER_CONSTANT 0, followed for vertical lines by `cv2.rotate(.., ROTATE_90_COUNTERCLOCKWISE)`, for
 // every line of a page in ONE launch (reference utils/textblock.py:162-194; the matrices come from ctd_region_plan,
-// csrc/region_plan.cpp).  The same kernel crops every line of every page of a ctd_submit_pages_regions batch in one
-// launch (pipeline.cu): each crop record carries its page's byte offset and size, so the pages are read in place.
+// csrc/region_plan.cpp).  The same kernel crops every line of every page of a ctd_submit_pages batch with a textheight
+// in one launch (pipeline.cu): each crop record carries its page's byte offset and size, so the pages are read in
+// place.
 //
 // Work split: the host (RegionJob) cuts every crop into tiles of kRegionTilePx consecutive output pixels (row-major in
 // the RETURNED array, i.e. after the rotation) and uploads a tile table {region, first pixel}; one CTA per tile, one

@@ -41,8 +41,8 @@ def letterbox_geometry(shape_hw, new_shape=(1024, 1024)):
 
 
 def letterbox(im, new_shape=(1024, 1024)):
-    """Host restatement of the reference's `letterbox` (kept for tests / tools; the detector itself resizes on the
-    GPU through `Engine.forward_resized`, bit-exact with cv2.INTER_LINEAR)."""
+    """Host restatement of the reference's `letterbox` (kept for tests / tools; the detector itself letterboxes on the
+    GPU inside `ctd_detect_page` and `ctd_submit_pages`, bit-exact with cv2.INTER_LINEAR)."""
     r, new_unpad, dw, dh = letterbox_geometry(im.shape[:2], new_shape)
     if im.shape[:2][::-1] != new_unpad:
         import cv2
@@ -52,15 +52,6 @@ def letterbox(im, new_shape=(1024, 1024)):
         padded[:im.shape[0], :im.shape[1]] = im
         im = padded
     return im, (r, r), (dw, dh)
-
-
-def expand_textwindow(img_size, xyxy, expand_r=8):
-    """utils/imgproc_utils.py:151-161"""
-    im_h, im_w = img_size[:2]
-    x1, y1, x2, y2 = xyxy
-    w, h = x2 - x1, y2 - y1
-    pad = int(round((max(h, w) * 0.25 + min(h, w) * 0.75) / expand_r))
-    return [max(0, x1 - pad), max(0, y1 - pad), min(im_w - 1, x2 + pad), min(im_h - 1, y2 + pad)]
 
 
 class TextDetector:
@@ -170,7 +161,7 @@ class TextDetector:
         textheight)` cuts it, byte for byte, except that a line on which the reference's `get_transformed_region`
         raises (a crop side of 1 px, a degenerate quad; or a side of 32767 px or more) gets None instead of raising,
         so one such line does not end the stream.  The crops are planned on the engine's worker threads and cut in
-        one GPU launch per batch from the pages already in device memory (`ctd_submit_pages_regions`).  Each page's
+        one GPU launch per batch from the pages already in device memory (`ctd_submit_pages`).  Each page's
         crops are views into one array of that page's own.
 
         device_results=True: mask, mask_refined and every crop are torch.uint8 CUDA tensors on cuda:device_index

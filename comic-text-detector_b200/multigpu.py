@@ -15,8 +15,9 @@ def shard_range(n_pages, rank, world):
 
 def arena_layout(max_batch, max_h, max_w):
     """Byte offsets of the phase-A section of an engine's result arena for an engine created with
-    (max_batch, max_h, max_w) -- the section ctd_submit delivers.  Mirrors engine.cu (256-byte aligned fields); prefer
-    `Engine.results_layout()`, which asks the library and also covers mask_refined and the block sections."""
+    (max_batch, max_h, max_w) -- the first phase_a_bytes of what ctd_submit_full delivers.  Mirrors engine.cu (256-byte
+    aligned fields) without a GPU; prefer `Engine.results_layout()`, which asks the library and also covers
+    mask_refined and the block sections."""
     al = lambda v: (v + 255) // 256 * 256
     o_det = al(max_batch * max_h * max_w)
     o_cnt = o_det + al(max_batch * 300 * 6 * 4)

@@ -24,7 +24,7 @@
 extern "C" {
 #endif
 
-#define CTD_ABI_VERSION 2
+#define CTD_ABI_VERSION 3
 #if defined(__GNUC__)
 #define CTD_API __attribute__((visibility("default")))
 #else
@@ -187,37 +187,10 @@ CTD_API int ctd_get_db_components(ctd_handle* h, uint8_t* bitmap, int32_t* label
  * left to the caller, as in the reference.                                                        */
 CTD_API int ctd_get_text_lines(ctd_handle* h, int16_t* boxes, float* scores, int32_t* counts);
 
-/* ---- pages that are not net-sized (SURVEY 8f row f1) -----------------------------------------
- * `letterbox(im, new_shape, auto=False)` + `preprocess_img` (imgproc_utils.py:86-117, inference.py:72-83) on the
- * GPU: the HOST page (u8 BGR HWC, any size ih x iw) is resized with OpenCV-exact INTER_LINEAR to
- * unpad_h x unpad_w (the caller computes these with the reference's formula: r = min(net_h/ih, net_w/iw),
- * unpad = round(size * r)), zero-padded bottom/right to net_h x net_w (multiples of 64) and forwarded (n = 1).   */
-CTD_API int ctd_forward_resized(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t unpad_h, int32_t unpad_w,
-                                int32_t net_h, int32_t net_w);
-/* Mask back-projection (inference.py:164-168): `mask[:crop_h, :crop_w]` of page 0 of the last forward,
- * `cv2.resize(.., (out_w, out_h), INTER_LINEAR)` -> HOST u8 [out_h][out_w].                                      */
-CTD_API int ctd_get_mask_u8_resized(ctd_handle* h, int32_t crop_h, int32_t crop_w, int32_t out_h, int32_t out_w,
-                                    uint8_t* mask_out);
 /* Stand-alone `cv2.resize(src, (dw, dh), interpolation=cv2.INTER_LINEAR)` for u8 images with 1 or 3 channels
  * (HOST in, HOST out); bit-exact with OpenCV 4.x, see csrc/resize.cu.                                            */
 CTD_API int ctd_resize_linear_u8(ctd_handle* h, const uint8_t* src, int32_t sh, int32_t sw, int32_t channels, uint8_t* dst,
                                  int32_t dh, int32_t dw);
-
-/* ---- pipelined host-buffer path (throughput mode of ctd_forward + ctd_get_*) -----------------
- * The reference serves pages one call at a time (inference.py:141-178: H2D, net, D2H, numpy post-
- * processing, all serial).  A caller that streams batches keeps two in flight instead:
- *   ctd_submit(h, slot, pages, n, ph, pw, results)   asynchronous: H2D of the HOST pages on a copy
- *       stream, the whole forward + post-processing on the engine stream, D2H of the result arena
- *       (mask_u8 | det | det_count | n_labels | line_boxes | line_scores | line_count, layout of
- *       ctd_device_outputs / ctd_results_bytes) into HOST `results` on a second copy stream;
- *   ctd_collect(h, slot)                              blocks until that slot's `results` are complete.
- * slot is 0 or 1; a slot must be collected before it is submitted again.  `pages` and `results`
- * should be pinned (cudaHostAlloc / torch pin_memory) or the copies serialise.  Submissions execute
- * in order; ctd_get_* after a submit refer to the most recently submitted batch.               */
-CTD_API int ctd_submit(ctd_handle* h, int32_t slot, const uint8_t* pages_host, int32_t n, int32_t ph, int32_t pw,
-                       void* results_host);
-CTD_API int ctd_collect(ctd_handle* h, int32_t slot);
-CTD_API int ctd_results_bytes(ctd_handle* h, size_t* bytes);
 
 /* Several handles on ONE GPU (one workspace each) let independent batches overlap: the kernels of batch i+1 fill the
  * tails and dependency gaps of batch i (+8 % pages/s with two handles, bench.py).  ctd_join makes everything
@@ -258,24 +231,6 @@ CTD_API int ctd_timer_stop(ctd_handle* h, float* ms); /* synchronises the engine
  * entries after the last op are the NMS and the CCL stage.  cap >= n_ops + 2.                   */
 CTD_API int ctd_profile_forward(ctd_handle* h, const uint8_t* pages, int32_t n, int32_t ph, int32_t pw,
                                 int32_t pages_on_device, float* op_ms, int32_t cap);
-/* Device pointers of the last forward's results (valid until the next call on this handle) and
- * the engine's cudaStream_t, so a caller can hand them to NCCL without a host round trip.       */
-typedef struct ctd_device_outputs {
-  void* stream;      /* cudaStream_t                                  */
-  void* mask_u8;     /* u8  [n][h][w]                                 */
-  void* det;         /* f32 [n][300][6]                               */
-  void* det_count;   /* i32 [n]                                       */
-  void* bitmap;      /* u8  [n][h][w]                                 */
-  void* labels;      /* i32 [n][h][w]                                 */
-  void* n_labels;    /* i32 [n]                                       */
-  void* line_boxes;  /* i16 [n][1000][4][2]                           */
-  void* line_scores; /* f32 [n][1000]                                 */
-  void* line_count;  /* i32 [n]                                       */
-  void* results_base;   /* mask_u8 | det | det_count | n_labels | line_* live in ONE allocation sized for
-                           max_batch, so a single NCCL gather moves a rank's results          */
-  size_t results_bytes;
-} ctd_device_outputs;
-CTD_API int ctd_get_device_outputs(ctd_handle* h, ctd_device_outputs* out);
 
 /* ---- stand-alone array kernels (stage-isolated parity; same kernels the pipeline uses) --
  * cv2.connectedComponentsWithStats(img, connectivity=8, ltype=CV_32S) as the reference
@@ -343,9 +298,6 @@ CTD_API int ctd_group_output(const int32_t* blk_xyxy, const int32_t* blk_cls, in
                              int32_t n_lines, int32_t im_w, int32_t im_h, const uint8_t* mask, int32_t sort_blklist,
                              ctd_block* blocks_out, int32_t blocks_cap, int32_t* lines_out, int32_t lines_cap,
                              double* dist_out, int32_t dist_cap, int32_t* n_blocks);
-/* `expand_textwindow(img.shape, xyxy, expand_r)` (utils/imgproc_utils.py:151-161) followed by the index
- * normalisation of the python slice `img[y1:y2, x1:x2]` (negative bounds wrap, then clamp): win = x1,y1,x2,y2.  */
-CTD_API void ctd_expand_textwindow(int32_t im_w, int32_t im_h, const int32_t* xyxy, int32_t expand_r, int32_t* win);
 
 /* ---- the whole of `TextDetector.__call__` (inference.py:141-178) ---------------------------------------------
  * One page of any size: letterbox + forward + post-processing on the GPU, postprocess_yolo casts / box_thresh /
@@ -364,11 +316,13 @@ CTD_API int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, int3
                             int32_t dist_cap, int32_t* n_blocks);
 
 /* Batches of NET-SIZED pages through the same chain, two batches in flight per handle (throughput form of the
- * above; supersedes ctd_submit for callers that want blocks and mask_refined).  ctd_submit_full returns at once:
- * the forward + device post-processing are enqueued, a worker thread of the handle runs the host stage when their
- * results arrive and enqueues refine_mask; ctd_collect(h, slot) blocks until `results_host` is complete.
+ * above).  ctd_submit_full returns at once: the H2D of host pages runs on a copy stream, the forward + device
+ * post-processing on the engine stream, the D2H of the phase-A section on a second copy stream, and a worker thread of
+ * the handle runs the host stage when those results arrive and enqueues refine_mask; ctd_collect(h, slot) blocks until
+ * `results_host` is complete.  slot is 0 or 1; a slot must be collected before it is submitted again.  Submissions
+ * execute in order; ctd_get_* after a submit refer to the most recently submitted batch.
  * results_host: HOST (pinned) buffer of ctd_results_layout().total_bytes:
- *   [0, phase_a_bytes)  mask_u8 | det | det_count | n_labels | line_boxes | line_scores | line_count (as ctd_submit)
+ *   [0, phase_a_bytes)  mask_u8 | det | det_count | n_labels | line_boxes | line_scores | line_count
  *   mask_refined        u8 [n][ph][pw]
  *   blocks + i*blocks_stride   page i: ctd_page_blocks header, ctd_block[CTD_MAX_BLOCKS] at +blk_records_off,
  *                       i32 lines [..][4][2] at +blk_lines_off, f64 distances at +blk_dist_off
@@ -384,6 +338,8 @@ typedef struct ctd_results_layout_t {
 CTD_API int ctd_results_layout(ctd_handle* h, ctd_results_layout_t* out);
 CTD_API int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages, int32_t n, int32_t ph, int32_t pw,
                             int32_t pages_on_device, int32_t refine_mode, void* results_host);
+/* Blocks until the batch submitted on `slot` (ctd_submit_full or ctd_submit_pages) is complete; returns its error.  */
+CTD_API int ctd_collect(ctd_handle* h, int32_t slot);
 /* Device copy of slot `slot`'s complete results (same layout) and the stream its last writes were enqueued on.   */
 CTD_API int ctd_device_arena(ctd_handle* h, int32_t slot, void** base, void** post_stream);
 
@@ -409,18 +365,15 @@ typedef struct ctd_page_entry {
 } ctd_page_entry;
 CTD_API int ctd_pages_plan(ctd_page_entry* pages, int32_t n, int32_t net_h, int32_t net_w, size_t* input_bytes,
                            size_t* results_bytes);
-/* Asynchronous: the batch runs like a ctd_submit_full batch and is collected with ctd_collect(h, slot), after which
- * `results_host` holds every page's mask (modified by refine_undetected_mask when keep_undetected != 0, as in
- * ctd_detect_page), mask_refined and block section.  pages / n: the planned entries (checked against a fresh plan);
- * input_host: the packed pages (pinned, input_bytes); results_host: pinned, results_bytes.  Both buffers must stay
- * untouched until the slot is collected.  On the GPU: one letterbox launch for the batch, the forward at
- * (n, net_h, net_w), one launch back-projecting every page's mask to its size, one refine_mask launch for every
- * window of every page.  Same checks as ctd_submit_full (slot 0/1 and collected, n <= max_batch, net shape <= the
- * engine's max shape, not a debug_skip_postproc engine), and with keep_undetected != 0 ctd_detect_page's page-size
- * limit (2^28 pixels per page, CTD_E_CAPACITY beyond).                                                            */
-CTD_API int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
-                             int32_t net_w, const uint8_t* input_host, int32_t refine_mode, int32_t keep_undetected,
-                             void* results_host);
+/* ctd_submit_pages (declared below with ctd_device_page) is asynchronous: the batch runs like a ctd_submit_full batch
+ * and is collected with ctd_collect(h, slot), after which `results_host` holds every page's mask (modified by
+ * refine_undetected_mask when keep_undetected != 0, as in ctd_detect_page), mask_refined and block section.  pages / n:
+ * the planned entries (checked against a fresh plan); input_host: the packed pages (pinned, input_bytes);
+ * results_host: pinned, results_bytes.  Both buffers must stay untouched until the slot is collected.  On the GPU: one
+ * letterbox launch for the batch, the forward at (n, net_h, net_w), one launch back-projecting every page's mask to
+ * its size, one refine_mask launch for every window of every page.  Same checks as ctd_submit_full (slot 0/1 and
+ * collected, n <= max_batch, net shape <= the engine's max shape, not a debug_skip_postproc engine), and with
+ * keep_undetected != 0 ctd_detect_page's page-size limit (2^28 pixels per page, CTD_E_CAPACITY beyond).           */
 
 /* ---- text-line crops for OCR (SURVEY 8f row f4) ----------------------------------------------------------------
  * `TextBlock.get_transformed_region(img, idx, textheight)` (utils/textblock.py:162-194): line `idx` of a block, pushed
@@ -459,18 +412,14 @@ CTD_API int ctd_region_plan(const ctd_region_line* lines, int32_t n, int32_t im_
  * CTD_E_SHAPE for a bad page size, CTD_E_INVALID for a malformed plan entry.                                       */
 CTD_API int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t ih, int32_t iw, int32_t page_on_device,
                                   const ctd_region* plan, int32_t n, uint8_t* pixels_out, size_t pixels_bytes);
-/* ctd_submit_pages plus the OCR crops of every text line of every page of the batch (ctd_region_plan above;
- * pages in device memory and results left there: ctd_submit_pages_device below):
- * the same batch, and with textheight = 0 exactly ctd_submit_pages (ctd_submit_pages is this call with textheight 0).
- * textheight >= 2 (else CTD_E_INVALID): the handle's worker plans each page's lines with ctd_region_plan right after
- * its group_output, on the same host threads, then one k_warp_regions launch on the post stream cuts every status-0
- * crop of every page out of the pages where they already are in device memory, and the pixels are copied back into a
- * pinned buffer of the handle before the batch counts as done.  A batch without a single crop launches and allocates
- * nothing.  A page the planner refuses (a side >= 32767) fails the batch, and ctd_collect names the page.      */
-CTD_API int ctd_submit_pages_regions(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
-                                     int32_t net_w, const uint8_t* input_host, int32_t refine_mode,
-                                     int32_t keep_undetected, int32_t textheight, void* results_host);
-/* After ctd_collect(h, slot) of a ctd_submit_pages_regions batch with textheight > 0: the concatenated ctd_region
+/* ctd_submit_pages with a textheight also cuts the OCR crops of every text line of every page of the batch; with
+ * textheight = 0 it cuts none.  textheight >= 2 (else CTD_E_INVALID): the handle's worker plans each page's lines with
+ * ctd_region_plan right after its group_output, on the same host threads, then one k_warp_regions launch on the post
+ * stream cuts every status-0 crop of every page out of the pages where they already are in device memory, and the
+ * pixels are copied back into a pinned buffer of the handle before the batch counts as done.  A batch without a single
+ * crop launches and allocates nothing.  A page the planner refuses (a side >= 32767) fails the batch, and ctd_collect
+ * names the page.
+ * After ctd_collect(h, slot) of a ctd_submit_pages batch with textheight > 0: the concatenated ctd_region
  * plans of the batch, *n_regions entries in page, then block, then line order (the order of each page's block
  * section), page i's entries at [(*page_first)[i], (*page_first)[i + 1]) (n + 1 values), and the packed crops,
  * *bytes bytes at *pixels (HOST, NULL when *bytes is 0).  Each entry's offset is relative to *pixels; page i's crops
@@ -494,7 +443,8 @@ typedef struct ctd_device_page {
   int64_t stride_h, stride_w, stride_c;
   void* event;
 } ctd_device_page;
-/* ctd_submit_pages_regions with pages in device memory and, optionally, results left there.
+/* The batch entry point (see ctd_pages_plan and the crops above), with pages in device memory and, optionally,
+ * results left there.
  *   dev: n entries (NULL: every page is in input_host).  input_host may be NULL when every page is on the device;
  *        then no page byte is copied from the host, and a mixed batch copies only its host pages' byte ranges.  Each
  *        device page must be device memory of the handle's GPU (checked with cudaPointerGetAttributes, else
@@ -505,11 +455,11 @@ typedef struct ctd_device_page {
  *        pixels are NOT copied to the host; results_host still gets the phase-A rows, the masks group_output reads
  *        and the block sections, and ctd_collect_regions gives the plan with *pixels = NULL and *bytes = the batch's
  *        crop bytes on the device.  Fetch the device results with ctd_collect_device after ctd_collect.
- * ctd_submit_pages_regions is this call with dev = NULL and results_on_device = 0.                                   */
-CTD_API int ctd_submit_pages_device(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
-                                    int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
-                                    int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
-                                    int32_t results_on_device, void* results_host);
+ * With dev = NULL and results_on_device = 0 the pages come from input_host and every result goes to results_host.   */
+CTD_API int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                             int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev, int32_t refine_mode,
+                             int32_t keep_undetected, int32_t textheight, int32_t results_on_device,
+                             void* results_host);
 /* After ctd_collect(h, slot) of a results_on_device batch: copies into page_dst[i] (a DEVICE buffer on the handle's
  * GPU, one per page of the batch) page i's [mask ih*iw | mask_refined ih*iw | the page's crops, packed as the plan
  * lays them out, offsets relative to the page's first plan entry].  The mask is the one refine_undetected_mask

@@ -1,6 +1,6 @@
 """Throughput of the batched stream with pages and results in GPU memory: `detect_stream(textheight=48)` fed numpy pages
-or torch.uint8 CUDA pages, yielding numpy results or CUDA tensors (`device_results=True`; ctd_submit_pages_device, one
-batched strided gather launch per batch, ctd_collect_device).
+or torch.uint8 CUDA pages, yielding numpy results or CUDA tensors (`device_results=True`; ctd_submit_pages with device
+pages, one batched strided gather launch per batch, ctd_collect_device).
 
 Workload: the 64 seeded synthetic pages of scripts/stream_regions_bench.py (DESIGN §7.4) at input_size 1024,
 refine_mode INPAINT, textheight 48, max_batch 16.  Every arm runs the workload once to warm up, then twice timed; the

@@ -1,7 +1,7 @@
 """Throughput of "detect + OCR crops" over pages of any size: the batched stream alone, the stream followed by the
 blocking per-page `get_transformed_regions`, and the stream cutting the crops itself (`detect_stream(textheight=)`,
-ctd_submit_pages_regions: planned on the engine's worker threads, one k_warp_regions launch per batch on the pages
-already in device memory).
+ctd_submit_pages with a textheight: planned on the engine's worker threads, one k_warp_regions launch per batch on the
+pages already in device memory).
 
 Workload: the 64 seeded synthetic pages of scripts/pages_bench.py (oracle/synth.structured_page) at input_size 1024,
 refine_mode INPAINT, textheight 48, max_batch 16.  Every arm runs the workload once to warm up, then twice timed; the

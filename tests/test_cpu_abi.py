@@ -36,6 +36,21 @@ def test_struct_layouts_match_header():
     assert ctypes.sizeof(CtdConfig) == 12 * 4
 
 
+def test_stale_abi_version_refused():
+    """a caller built against ABI version 2 (where ctd_submit_pages had another signature) is refused by ctd_create
+    before any device is probed"""
+    from ctd_b200.binding import ABI_VERSION, CtdBufDesc, CtdConfig, CtdOp
+    src = open(os.path.join(ROOT, "include", "ctd_b200.h")).read()
+    assert int(re.search(r"#define CTD_ABI_VERSION (\d+)", src).group(1)) == ABI_VERSION == 3
+    lib = ctd_b200.load_library()
+    cfg = CtdConfig(2, 0, 0, 1, 64, 64, 2, 0, 0.4, 0.35, 0.3, 0)
+    ops, bufs, blob = (CtdOp * 1)(), (CtdBufDesc * 1)(), ctypes.create_string_buffer(64)
+    h = ctypes.c_void_p()
+    rc = lib.ctd_create(ctypes.byref(h), ctypes.byref(cfg), ops, 1, bufs, 1, ctypes.cast(blob, ctypes.c_void_p), 64)
+    assert rc == -1 and not h   # CTD_E_INVALID
+    assert lib.ctd_last_error(None) == b"ABI version mismatch"
+
+
 @pytest.mark.skipif(torch.cuda.is_available(), reason="only meaningful on a box without a GPU")
 def test_no_cpu_fallback():
     P = cc.Program()

@@ -80,7 +80,7 @@ def test_letterboxed_page_keeps_reference_shapes():
         det.close()
 
 
-def test_full_size_forward_is_deterministic_and_batch_invariant(prog):
+def test_full_size_forward_deterministic_batch_invariant_and_arena_layout(prog):
     """1024x1024, batch 3 vs batch 1: bit-identical result arenas run to run, and page k of a batch equals the same page
     processed alone (pages are independent, inference.py:141-178)."""
     h = w = 1024
@@ -105,7 +105,6 @@ def test_full_size_forward_is_deterministic_and_batch_invariant(prog):
             assert np.all((a[3][i] >= 0) & (a[3][i] <= 1))
             assert a[2][i].min(initial=0) >= 0 and a[2][i].max(initial=0) <= 1024
         assert multigpu.arena_layout(3, h, w)["phase_a_bytes"] == eng.results_layout()["phase_a_bytes"]
-        assert eng.results_layout()["total_bytes"] == eng.results_bytes()
     finally:
         eng.close()
 

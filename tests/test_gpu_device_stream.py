@@ -1,5 +1,5 @@
 """-m gpu: pages and results in GPU memory for the batched stream (`TextDetector.detect_stream` / `detect_batch` with
-torch.uint8 CUDA pages and `device_results=True`; ctd_submit_pages_device, the batched strided page gather,
+torch.uint8 CUDA pages and `device_results=True`; ctd_submit_pages with device pages, the batched strided page gather,
 ctd_collect_device).  The numpy stream is the reference (it is pinned against the reference's goldens elsewhere): every
 mask, mask_refined, block and crop must be byte-identical to what it gives for the same pages."""
 import numpy as np
@@ -197,7 +197,7 @@ def test_blank_pages_growth_and_abandoned_stream():
         d.close()
 
 
-def test_errors(det):
+def test_device_page_errors(det):
     pages = _pages(SIZES[:3], seed=5500)
     good = _cuda(pages)
     bad = {
@@ -223,12 +223,12 @@ def test_errors(det):
     host = np.ascontiguousarray(pages[0])
     dev = (binding.CtdDevicePage * 2)(binding.CtdDevicePage(host.ctypes.data, host.strides[0], 3, 1, None),
                                       binding.CtdDevicePage(good[1].data_ptr(), good[1].stride(0), 3, 1, None))
-    rc = eng.lib.ctd_submit_pages_device(eng.h, 1, binding._ptr(ent), 2, NET, NET, None, binding.C.cast(dev, binding.C.c_void_p),
-                                         0, 0, 0, 1, binding.C.c_void_p(out.data_ptr()))
+    rc = eng.lib.ctd_submit_pages(eng.h, 1, binding._ptr(ent), 2, NET, NET, None, binding.C.cast(dev, binding.C.c_void_p),
+                                  0, 0, 0, 1, binding.C.c_void_p(out.data_ptr()))
     assert rc == -1 and b"page 0" in eng.lib.ctd_last_error(eng.h)
     dev[0] = binding.CtdDevicePage(None, 0, 0, 0, None)
-    rc = eng.lib.ctd_submit_pages_device(eng.h, 1, binding._ptr(ent), 2, NET, NET, None, binding.C.cast(dev, binding.C.c_void_p),
-                                         0, 0, 0, 1, binding.C.c_void_p(out.data_ptr()))
+    rc = eng.lib.ctd_submit_pages(eng.h, 1, binding._ptr(ent), 2, NET, NET, None, binding.C.cast(dev, binding.C.c_void_p),
+                                  0, 0, 0, 1, binding.C.c_void_p(out.data_ptr()))
     assert rc == -1
     eng.submit_pages(1, pages[:2], NET, NET)
     eng.collect_pages(1)

@@ -119,10 +119,11 @@ def _collected(items):
             for it in items]
 
 
-def test_slots_reused_across_submission_kinds():
-    """one handle's two slots run, in turn, ctd_submit_full (slot 0), ctd_submit_pages with crops and results on the
-    device (slot 1), ctd_submit (slot 0) and ctd_submit_pages with neither (slot 1): every batch computes what it
-    computes on a fresh handle, and a slot hands out crops or device results only when its last batch made them"""
+def test_slots_reused_across_host_device_and_pages_batches():
+    """one handle's two slots run, in turn, ctd_submit_full on host pages (slot 0), ctd_submit_pages with crops and
+    results on the device (slot 1), ctd_submit_full on device pages (slot 0) and ctd_submit_pages with neither
+    (slot 1): every batch computes what it computes on a fresh handle, and a slot hands out crops or device results
+    only when its last batch made them"""
     prog = ctd_b200.compiler.compile_checkpoint(get_checkpoint(0, True))
     B, N = 2, 256
 
@@ -130,36 +131,33 @@ def test_slots_reused_across_submission_kinds():
         return ctd_b200.Engine(prog, max_batch=B, max_h=N, max_w=N, use_graph=True)
 
     net_pages = torch.from_numpy(np.stack([synth.structured_page(9100 + i, N, N) for i in range(B)])).pin_memory()
+    dev_pages = net_pages.cuda()
     pages_a = [synth.structured_page(9200, 361, 251), synth.structured_page(9201, 414, 292)]
     pages_b = [synth.structured_page(9300, 200, 150), synth.structured_page(9301, 2 * N, 2 * N)]
 
     def run(eng, kind):
-        if kind == "full":
-            out = torch.zeros((eng.results_layout()["total_bytes"],), dtype=torch.uint8).pin_memory()
-            eng.submit_full(0, net_pages.data_ptr(), B, N, N, out.data_ptr())
-            return out
-        out = torch.zeros((eng.results_bytes(),), dtype=torch.uint8).pin_memory()
-        eng.submit(0, net_pages.data_ptr(), B, N, N, out.data_ptr())
+        out = torch.zeros((eng.results_layout()["total_bytes"],), dtype=torch.uint8).pin_memory()
+        pages = dev_pages if kind == "device" else net_pages
+        eng.submit_full(0, pages.data_ptr(), B, N, N, out.data_ptr(), pages_on_device=kind == "device")
         return out
 
-    def arena(eng, out, kind):
+    def arena(eng, out):
         lay = eng.results_layout()
-        if kind == "submit":
-            return out[:lay["phase_a_bytes"]].numpy().tobytes()
         got = multigpu.unpack_arena(out.numpy(), lay, B, N, N, full=True)
-        return _bytes([got["mask"], got["mask_refined"]]), [[_blk_key(b) for b in blks] for blks in got["blocks"]]
+        return (out[:lay["phase_a_bytes"]].numpy().tobytes(), _bytes(got["mask_refined"]),
+                [[_blk_key(b) for b in blks] for blks in got["blocks"]])
 
     eng = engine()
     try:
-        out_full = run(eng, "full")
+        out_host = run(eng, "host")
         eng.submit_pages(1, pages_a, N, N, textheight=32, device_results=True)
         eng.collect(0)
         got_a = eng.collect_pages(1)
-        got_full = arena(eng, out_full, "full")
-        out_sub = run(eng, "submit")
+        got_host = arena(eng, out_host)
+        out_dev = run(eng, "device")
         eng.submit_pages(1, pages_b, N, N)
         eng.collect(0)
-        got_sub = arena(eng, out_sub, "submit")
+        got_dev = arena(eng, out_dev)
         got_b = eng.collect_pages(1)
         # neither slot's last batch asked for crops, and neither left its results on the device.  The destinations
         # are valid device memory with room for pages_a's [mask | mask_refined | crops] (slot 1 still holds that
@@ -168,7 +166,7 @@ def test_slots_reused_across_submission_kinds():
                for p in pages_a]
         ptrs = (ctd_b200.binding.C.c_void_p * B)(*[d.data_ptr() for d in dst])
         for slot in (0, 1):
-            with pytest.raises(ctd_b200.CtdError, match="ctd_submit_pages_regions batch"):
+            with pytest.raises(ctd_b200.CtdError, match="ctd_submit_pages batch with a textheight"):
                 eng.collect_regions(slot, [[], []])
             assert eng.lib.ctd_collect_device(eng.h, slot, ptrs) == -1
             assert b"results on the device" in eng.lib.ctd_last_error(eng.h)
@@ -177,12 +175,12 @@ def test_slots_reused_across_submission_kinds():
     assert sum(len(p[2]) for p in got_a) > 0 and any(c is not None for p in got_a for blk in p[5] for c in blk)
     assert all(isinstance(p[0], torch.Tensor) and p[0].is_cuda for p in got_a)
     ref = {}
-    for kind in ("full", "submit"):
+    for kind in ("host", "device"):
         one = engine()
         try:
             out = run(one, kind)
             one.collect(0)
-            ref[kind] = arena(one, out, kind)
+            ref[kind] = arena(one, out)
         finally:
             one.close()
     for key, pages, kw in (("a", pages_a, dict(textheight=32, device_results=True)), ("b", pages_b, {})):
@@ -192,8 +190,8 @@ def test_slots_reused_across_submission_kinds():
             ref[key] = one.collect_pages(0)
         finally:
             one.close()
-    assert got_full == ref["full"]
-    assert got_sub == ref["submit"]
+    assert got_host == ref["host"]
+    assert got_dev == ref["device"]
     assert _collected(got_a) == _collected(ref["a"])
     assert _collected(got_b) == _collected(ref["b"])
 

@@ -154,7 +154,7 @@ def test_model2annotations_through_stream(det, tmp_path):
     assert not mismatch and not errors
 
 
-def test_errors(det):
+def test_pages_batch_errors(det):
     eng = det.net
     pages = _pages([(300, 200), (200, 300)])
     eng.submit_pages(0, pages, NET, NET)
@@ -179,7 +179,8 @@ def test_errors(det):
     ent[1]["mask_off"] += 256
     buf = np.zeros((ib,), np.uint8)
     out = np.zeros((rb,), np.uint8)
-    rc = eng.lib.ctd_submit_pages(eng.h, 1, binding._ptr(ent), 2, NET, NET, binding._ptr(buf), 0, 0, binding._ptr(out))
+    rc = eng.lib.ctd_submit_pages(eng.h, 1, binding._ptr(ent), 2, NET, NET, binding._ptr(buf), None, 0, 0, 0, 0,
+                                  binding._ptr(out))
     assert rc == -1   # CTD_E_INVALID
     # the engine still works after every refusal
     _same_result(det.detect_batch([pages[0]])[0], det(pages[0]))

@@ -1,5 +1,5 @@
 """-m gpu: text-line crops in the batched stream (`TextDetector.detect_stream` / `detect_batch` with a textheight,
-ctd_submit_pages_regions + ctd_collect_regions).  Every crop is compared byte for byte with the cv2 restatement of the
+ctd_submit_pages + ctd_collect_regions).  Every crop is compared byte for byte with the cv2 restatement of the
 reference method (tests/region_ref.py), None exactly where that method raises, and with the blocking per-page
 `get_transformed_regions` on pages where no line raises; the first three fields of every item must equal the stream
 without a textheight."""
@@ -207,7 +207,7 @@ def test_call_and_crops_between_stream_yields():
         d.close()
 
 
-def test_errors(det):
+def test_stream_region_errors(det):
     pages = _pages(SIZES[:5], seed=900)
     # an abandoned crop stream leaves the engine usable
     g = det.detect_stream([p.copy() for p in pages], textheight=48)
@@ -237,8 +237,8 @@ def test_errors(det):
     buf = np.zeros((ib,), np.uint8)
     out = np.zeros((rb,), np.uint8)
     for th in (1, -1):
-        rc = eng.lib.ctd_submit_pages_regions(eng.h, 1, binding._ptr(ent), 2, NET, NET, binding._ptr(buf), 0, 0, th,
-                                              binding._ptr(out))
+        rc = eng.lib.ctd_submit_pages(eng.h, 1, binding._ptr(ent), 2, NET, NET, binding._ptr(buf), None, 0, 0, th, 0,
+                                      binding._ptr(out))
         assert rc == -1   # CTD_E_INVALID
     eng.submit_pages(1, pages[:2], NET, NET)
     eng.collect_pages(1)
