@@ -7,4 +7,4 @@ from . import binding, multigpu, onnx_model, textblock  # noqa: F401
 from .inference import TextDetector, REFINEMASK_INPAINT, REFINEMASK_ANNOTATION  # noqa: F401
 from .basemodel import TextDetBase  # noqa: F401
 from .jpeg import JpegDecoder, jpeg_probe  # noqa: F401
-from .png import PngEncoder  # noqa: F401
+from .png import PngDecoder, PngEncoder, png_probe  # noqa: F401

@@ -115,12 +115,12 @@ def write_annotations(save_dir, imgname, img, mask_refined, blk_list, save_json=
 
 
 def _read_pages(imglist, det, failed):
-    """(path, page) for each file in order, decoded in batches of det.max_batch with the detector's JpegDecoder
-    (baseline JPEGs on the GPU into CUDA pages, every other file by cv2).  A file that cannot be read ends the pages
+    """(path, page) for each file in order, decoded in batches of det.max_batch as the detector decodes encoded pages
+    (baseline JPEGs and PNGs on the GPU into CUDA pages, every other file by cv2).  A file that cannot be read ends the pages
     there: its error goes to `failed`."""
     for b0 in range(0, len(imglist), det.max_batch):
         paths = imglist[b0:b0 + det.max_batch]
-        pages = det.jpeg_decoder().decode([np.fromfile(p, dtype=np.uint8) for p in paths])
+        pages = det._decode_files([np.fromfile(p, dtype=np.uint8) for p in paths])
         for img_path, img in zip(paths, pages):
             try:
                 img = check_page(img, det.device_index)
@@ -134,8 +134,8 @@ def model2annotations(model_path, img_dir_list, save_dir, save_json=False, detec
     """`model2annotations(model_path, img_dir_list, save_dir, save_json)` of the reference (inference.py:19-70).
 
     The files are those `write_annotations` writes page by page, byte for byte.  Pages are read in batches of the
-    detector's max_batch and decoded with its JpegDecoder; a page decoded on the GPU stays there for the detection and
-    for its PNG.  The refined masks stay on the GPU (detect_stream's device_results), and both PNGs of every page of
+    detector's max_batch and decoded with its JpegDecoder and PngDecoder; a page decoded on the GPU stays there for the
+    detection and for its PNG, so a directory of PNG pages (such as this tool's own output) is read on the GPU too.  The refined masks stay on the GPU (detect_stream's device_results), and both PNGs of every page of
     a batch of results are encoded in one PngEncoder call."""
     from .png import PngEncoder
     if isinstance(img_dir_list, str):

@@ -68,6 +68,12 @@ class CtdJpegInfo(C.Structure):
                [("ecs_bytes", C.c_int64)]
 
 
+class CtdPngInfo(C.Structure):
+    """ctypes mirror of `ctd_png_info` (include/ctd_b200.h)"""
+    _fields_ = [(k, C.c_int32) for k in ("status", "height", "width", "image_height", "image_width", "bit_depth",
+                                         "color_type", "orientation", "palette_entries")] + [("zlib_bytes", C.c_int64)]
+
+
 class CtdPngImage(C.Structure):
     """ctypes mirror of `ctd_png_image` (include/ctd_b200.h)"""
     _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32), ("channels", C.c_int32),
@@ -90,7 +96,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_device_arena", "ctd_region_plan", "ctd_transform_regions", "ctd_pages_plan", "ctd_submit_pages",
            "ctd_collect_regions", "ctd_collect_device", "ctd_forward_tensor", "ctd_jpeg_probe",
            "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy", "ctd_jpeg_decode", "ctd_debug_postprocess",
-           "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode"]
+           "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
+           "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats"]
 
 _lib = None
 
@@ -162,6 +169,12 @@ def load_library():
     lib.ctd_png_encoder_destroy.argtypes = [vp]
     lib.ctd_png_encode.argtypes = [vp, C.POINTER(CtdPngImage), i32, vp, vp]
     lib.ctd_png_encoder_destroy.restype = None
+    lib.ctd_png_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdPngInfo)]
+    lib.ctd_png_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
+    lib.ctd_png_decoder_destroy.argtypes = [vp]
+    lib.ctd_png_decode.argtypes = [vp, vp, vp, i32, vp, vp]
+    lib.ctd_png_decoder_stats.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+    lib.ctd_png_decoder_destroy.restype = None
     _lib = lib
     return lib
 

@@ -34,6 +34,10 @@ struct Frame {
 // The marker walk and the scan's structure check: CTD_JPEG_OK and the frame, or the reason code.
 int parse(const uint8_t* data, size_t len, Frame* f);
 
+// IFD0 orientation of an Exif payload (a TIFF header and its IFDs: after "Exif\0\0" in a JPEG, the whole eXIf chunk
+// of a PNG) as OpenCV's ExifReader reads it: 1..8, or 0 when the block does not parse cleanly
+int exif_orientation(const uint8_t* p, size_t n);
+
 // Unstuffs the scan of a parsed file into out (at most scan_end - scan_begin bytes): FF00 -> FF, RSTn dropped.
 // Writes each restart interval's first byte offset (relative to out) and bit length.  Returns the bytes written.
 size_t stage(const uint8_t* data, const Frame& f, uint8_t* out, int64_t* interval_byte, int32_t* interval_bits);

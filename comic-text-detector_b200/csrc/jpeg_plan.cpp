@@ -27,47 +27,6 @@ inline int u16be(const uint8_t* p) { return (p[0] << 8) | p[1]; }
 
 constexpr size_t kMaxScanBytes = size_t(1) << 28;   // 2^31 bits
 
-struct Tiff {
-  const uint8_t* p;
-  size_t n;
-  bool le;
-  uint32_t u16(size_t o) const { return le ? p[o] | (p[o + 1] << 8) : (p[o] << 8) | p[o + 1]; }
-  uint32_t u32(size_t o) const {
-    return le ? p[o] | (p[o + 1] << 8) | (p[o + 2] << 16) | ((uint32_t)p[o + 3] << 24)
-              : ((uint32_t)p[o] << 24) | (p[o + 1] << 16) | (p[o + 2] << 8) | p[o + 3];
-  }
-};
-
-// IFD0 orientation of an Exif payload (after "Exif\0\0"): 1..8, or 0 when the block does not parse cleanly
-int exif_orientation(const uint8_t* p, size_t n) {
-  if (n < 8 || !((p[0] == 'I' && p[1] == 'I') || (p[0] == 'M' && p[1] == 'M'))) return 0;
-  Tiff t{p, n, p[0] == 'I'};
-  if (t.u16(2) != 42) return 0;
-  uint64_t ifd = t.u32(4);
-  if (ifd < 8 || ifd + 2 > n) return 0;
-  uint64_t cnt = t.u16(ifd);
-  if (ifd + 2 + 12 * cnt > n) return 0;
-  static const int kSize[13] = {0, 1, 1, 2, 4, 8, 1, 1, 2, 4, 8, 4, 8};
-  int orient = 1;
-  bool seen = false;
-  for (uint64_t i = 0; i < cnt; ++i) {
-    size_t o = ifd + 2 + 12 * i;
-    uint32_t tag = t.u16(o), typ = t.u16(o + 2), c = t.u32(o + 4);
-    if (typ < 1 || typ > 12) return 0;
-    uint64_t nb = (uint64_t)kSize[typ] * c;
-    if (nb > 4 && (uint64_t)t.u32(o + 8) + nb > n) return 0;
-    if (tag == 0x0112) {
-      // a second orientation entry: OpenCV takes the first, other readers the last; left to cv2
-      if (seen) return 0;
-      seen = true;
-      if (typ != 3 || c != 1) return 0;
-      orient = (int)t.u16(o + 8);
-      if (orient < 1 || orient > 8) return 0;
-    }
-  }
-  return orient;
-}
-
 // jdhuff.c jpeg_make_d_derived_tbl plus a kLutBits lookahead table; false for a table libjpeg refuses
 bool derive(const uint8_t* counts, const uint8_t* vals, int nvals, bool dc, HuffTable* t) {
   memset(t, 0, sizeof(*t));
@@ -127,6 +86,46 @@ int walk_scan(const uint8_t* d, size_t n, Frame* f) {
 }
 
 }  // namespace
+
+struct Tiff {
+  const uint8_t* p;
+  size_t n;
+  bool le;
+  uint32_t u16(size_t o) const { return le ? p[o] | (p[o + 1] << 8) : (p[o] << 8) | p[o + 1]; }
+  uint32_t u32(size_t o) const {
+    return le ? p[o] | (p[o + 1] << 8) | (p[o + 2] << 16) | ((uint32_t)p[o + 3] << 24)
+              : ((uint32_t)p[o] << 24) | (p[o + 1] << 16) | (p[o + 2] << 8) | p[o + 3];
+  }
+};
+
+int exif_orientation(const uint8_t* p, size_t n) {
+  if (n < 8 || !((p[0] == 'I' && p[1] == 'I') || (p[0] == 'M' && p[1] == 'M'))) return 0;
+  Tiff t{p, n, p[0] == 'I'};
+  if (t.u16(2) != 42) return 0;
+  uint64_t ifd = t.u32(4);
+  if (ifd < 8 || ifd + 2 > n) return 0;
+  uint64_t cnt = t.u16(ifd);
+  if (ifd + 2 + 12 * cnt > n) return 0;
+  static const int kSize[13] = {0, 1, 1, 2, 4, 8, 1, 1, 2, 4, 8, 4, 8};
+  int orient = 1;
+  bool seen = false;
+  for (uint64_t i = 0; i < cnt; ++i) {
+    size_t o = ifd + 2 + 12 * i;
+    uint32_t tag = t.u16(o), typ = t.u16(o + 2), c = t.u32(o + 4);
+    if (typ < 1 || typ > 12) return 0;
+    uint64_t nb = (uint64_t)kSize[typ] * c;
+    if (nb > 4 && (uint64_t)t.u32(o + 8) + nb > n) return 0;
+    if (tag == 0x0112) {
+      // a second orientation entry: OpenCV takes the first, other readers the last; left to cv2
+      if (seen) return 0;
+      seen = true;
+      if (typ != 3 || c != 1) return 0;
+      orient = (int)t.u16(o + 8);
+      if (orient < 1 || orient > 8) return 0;
+    }
+  }
+  return orient;
+}
 
 int parse(const uint8_t* d, size_t n, Frame* f) {
   if (n < 4 || d[0] != 0xFF || d[1] != 0xD8) return CTD_JPEG_NOT_JPEG;

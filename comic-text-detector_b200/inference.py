@@ -7,7 +7,7 @@ conf_thresh=0.4, mask_thresh=0.3, act='leaky')` and
 A `.onnx` model_path is read as the reference's OpenCV-DNN backend reads it (onnx_model.py): same engine, same calls.
 `detect_batch` / `detect_stream` give the same results for many pages of any sizes, batched on the GPU, and with a
 `textheight` also the OCR crops of every text line (`get_transformed_regions`), cut in the same batches; their pages may
-be torch.uint8 CUDA tensors or encoded files (JPEGs decoded on the GPU, jpeg.py), and with `device_results=True` the
+be torch.uint8 CUDA tensors or encoded files (JPEGs and PNGs decoded on the GPU, jpeg.py, png.py), and with `device_results=True` the
 masks and crops come back as CUDA tensors.
 
 Everything runs in libctd_b200.so: network, NMS, mask u8, DB binarize, connected components, contour boxes + scores,
@@ -24,6 +24,7 @@ import numpy as np
 from . import compiler, onnx_model
 from .binding import Engine, PREC_FP16_TC, PREC_FP32_SIMT
 from .jpeg import JpegDecoder, is_encoded, read_encoded
+from .png import PngDecoder, is_png
 from .textblock import (TextBlock, _check_textheight, blocks_from_records, group_output, overlap_area,  # noqa: F401
                         transformed_regions)
 
@@ -90,6 +91,7 @@ class TextDetector:
         self.net = Engine(self.program, device=device_index, precision=precision, max_batch=self.max_batch, max_h=input_size[0],
                           max_w=input_size[1], conf_thresh=conf_thresh, nms_thresh=nms_thresh, db_thresh=0.3)
         self._jpeg = None   # the JpegDecoder of encoded pages, made on first use
+        self._png = None    # the PngDecoder of PNG pages, made on first use
 
     def jpeg_decoder(self):
         """the JpegDecoder this detector decodes encoded pages with (made on first use, closed with the detector)"""
@@ -97,11 +99,33 @@ class TextDetector:
             self._jpeg = JpegDecoder(self.device_index)
         return self._jpeg
 
+    def png_decoder(self):
+        """the PngDecoder this detector decodes PNG pages with (made on first use, closed with the detector)"""
+        if self._png is None:
+            self._png = PngDecoder(self.device_index)
+        return self._png
+
     def close(self):
         self.net.close()
         if self._jpeg is not None:
             self._jpeg.close()
             self._jpeg = None
+        if self._png is not None:
+            self._png.close()
+            self._png = None
+
+    def _decode_files(self, bufs):
+        """encoded files (1-D np.uint8 arrays) -> their pages in input order: files with the PNG signature through
+        png_decoder(), every other file through jpeg_decoder() (baseline JPEGs on the GPU, the rest by cv2); each page
+        is a CUDA tensor or what cv2.imdecode returns"""
+        pngs = [i for i, b in enumerate(bufs) if is_png(b)]
+        others = [i for i, b in enumerate(bufs) if not is_png(b)]
+        out = [None] * len(bufs)
+        for idx, dec in ((pngs, self.png_decoder), (others, self.jpeg_decoder)):
+            if idx:
+                for i, page in zip(idx, dec().decode([bufs[i] for i in idx])):
+                    out[i] = page
+        return out
 
     def __call__(self, img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
         """reference inference.py:141-178.  One native call (`ctd_detect_page`): letterbox (cv2-exact INTER_LINEAR) +
@@ -150,9 +174,10 @@ class TextDetector:
 
         A page may also be an encoded file, read as the reference's `io_utils.imread` reads it, i.e. as
         `cv2.imdecode(buf, cv2.IMREAD_COLOR)`: bytes, bytearray, memoryview or a 1-D np.uint8 array of the file, or a
-        str / os.PathLike path, read with np.fromfile.  The encoded pages of a batch are decoded in one
-        `JpegDecoder.decode` call right before the batch is submitted: baseline JPEGs on the GPU into CUDA pages (which
-        then enter as CUDA-tensor pages do), every other file by cv2 on the host into a numpy page.  The results are
+        str / os.PathLike path, read with np.fromfile.  The encoded pages of a batch are decoded right before the batch
+        is submitted, in one `PngDecoder.decode` call for the files with the PNG signature and one `JpegDecoder.decode`
+        call for the others: baseline JPEGs and the PNGs the GPU takes on the GPU into CUDA pages (which then enter as
+        CUDA-tensor pages do), every other file by cv2 on the host into a numpy page.  The results are
         byte for byte those for the `cv2.imdecode` pages of the same files.  A file cv2 cannot decode raises ValueError
         naming its index in `imgs` (and its path), when its batch is decoded.
 
@@ -216,13 +241,13 @@ class TextDetector:
                     pass
 
     def _decode_batch(self, batch):
-        """the batch with its encoded pages replaced by their decoded pages (one JpegDecoder.decode call): CUDA
-        tensors for the pages decoded on the GPU, complete when decode returns, numpy pages for the others"""
+        """the batch with its encoded pages replaced by their decoded pages (_decode_files): CUDA tensors for the pages
+        decoded on the GPU, complete when decode returns, numpy pages for the others"""
         enc = [i for i, p in enumerate(batch) if isinstance(p, _Encoded)]
         if not enc:
             return batch
         bufs = [read_encoded(batch[i].src) for i in enc]
-        pages = self.jpeg_decoder().decode([b for b, _path in bufs])
+        pages = self._decode_files([b for b, _path in bufs])
         batch = list(batch)
         for i, (_b, path), page in zip(enc, bufs, pages):
             if page is None:

@@ -3,7 +3,8 @@ reads: `cv2.imdecode(buf, cv2.IMREAD_COLOR)`.
 
 `JpegDecoder.decode(bufs)` decodes every baseline JPEG of a list on the GPU in one call and returns a torch.uint8 CUDA
 page for each; every other file (PNG, progressive JPEG, CMYK, a corrupt scan, ...) is decoded by cv2.imdecode on the
-host, so each result is exactly what cv2 returns, a numpy page or None.  `jpeg_probe(buf)` is the host marker walk that
+host, so each result is exactly what cv2 returns, a numpy page or None.  (PNG files have a GPU decoder of their own,
+png.PngDecoder; TextDetector sends each encoded page to the decoder of its format.)  `jpeg_probe(buf)` is the host marker walk that
 decides which files the GPU takes.
 """
 import ctypes as C

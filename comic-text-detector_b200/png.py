@@ -1,14 +1,26 @@
-"""PNG files encoded on the GPU (csrc/png.cu), byte for byte what the reference's `io_utils.imwrite` writes:
-`cv2.imencode('.png', img)[1]`.
+"""PNG files on the GPU.
 
+Encode (csrc/png.cu), byte for byte what the reference's `io_utils.imwrite` writes: `cv2.imencode('.png', img)[1]`.
 `PngEncoder.encode(imgs)` encodes a list of u8 images, grey [h][w] or BGR [h][w][3], numpy arrays or torch.uint8 CUDA
 tensors of any strides on the encoder's GPU, in one call, and returns each file as a 1-D np.uint8 array.
+
+Decode (csrc/png_plan.cpp, csrc/png_dec.cu), equal to what the reference's `io_utils.imread` reads:
+`cv2.imdecode(buf, cv2.IMREAD_COLOR)`.  `PngDecoder.decode(bufs)` decodes every PNG of a list the GPU takes in one call
+and returns a torch.uint8 CUDA page for each; every other file (Adam7, APNG, a bad CRC or corrupt data, a JPEG, ...)
+is decoded by cv2.imdecode on the host, so each result is exactly what cv2 returns, a numpy page or None.
+`png_probe(buf)` is the host chunk walk that decides which files the GPU takes.
 """
 import ctypes as C
 
 import numpy as np
 
-from .binding import CtdError, CtdPngImage, load_library
+from .binding import CtdError, CtdPngImage, CtdPngInfo, load_library
+from .jpeg import _cv2_decode, as_buffer
+
+# ctd_png_status (include/ctd_b200.h)
+PNG_STATUS = ["ok", "not_png", "truncated", "header", "interlaced", "apng", "chunks", "exif", "zlib", "size", "crc",
+              "data"]
+PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
 
 
 def _check(i, shape, dtype_ok):
@@ -90,3 +102,93 @@ class PngEncoder:
         if rc != 0:
             raise CtdError("ctd_png_encode failed (%d): %s" % (rc, self.lib.ctd_last_error(None).decode()))
         return [np.ctypeslib.as_array(C.cast(files[i], C.POINTER(C.c_uint8)), (sizes[i],)).copy() for i in range(n)]
+
+
+def png_probe(buf):
+    """`ctd_png_probe` (host only): dict of the ctd_png_info fields, plus `reason`, the status's name.  status 0: the
+    GPU decodes the file, to a page of shape (height, width, 3) (eXIf orientation applied), unless its CRCs or its
+    image data turn out not to be clean (`PngDecoder.last_status` "crc" / "data")."""
+    a = as_buffer(buf)
+    info = CtdPngInfo()
+    rc = load_library().ctd_png_probe(a.ctypes.data_as(C.c_void_p), a.size, C.byref(info))
+    if rc != 0:
+        raise CtdError("ctd_png_probe failed (%d)" % rc)
+    out = {k: int(getattr(info, k)) for k, _t in CtdPngInfo._fields_}
+    out["reason"] = PNG_STATUS[out["status"]]
+    return out
+
+
+def is_png(buf):
+    """True when an encoded file (1-D np.uint8 array) starts with the PNG signature"""
+    return buf.size >= 8 and buf[:8].tobytes() == PNG_SIGNATURE
+
+
+class PngDecoder:
+    """A GPU PNG decoder on cuda:device_index with a stream of its own.  subsequence_bits (0: the default): the length
+    of the pieces the parallel inflate cuts each Huffman block into; it changes how the work is split, never the
+    result."""
+
+    def __init__(self, device_index=0, subsequence_bits=0):
+        self.lib = load_library()
+        self.device_index = int(device_index)
+        self.h = C.c_void_p()
+        rc = self.lib.ctd_png_decoder_create(self.device_index, int(subsequence_bits), C.byref(self.h))
+        if rc != 0:
+            raise CtdError("ctd_png_decoder_create failed (%d): %s" % (rc, self.lib.ctd_last_error(None).decode()))
+        self._alloc_stream = None
+        self.last_status = []
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.ctd_png_decoder_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def decode(self, bufs):
+        """bufs: a list of encoded files (bytes-like or 1-D np.uint8 arrays).  Returns a list with, per file, a
+        torch.uint8 CUDA tensor [h][w][3] (BGR) when the GPU decoded it, else `cv2.imdecode(buf, IMREAD_COLOR)`: a
+        numpy page or None.  Every result equals cv2.imdecode's.  The tensors are complete on return and marked as
+        used on the current stream.  `last_status` keeps each file's ctd_png_status."""
+        import torch
+        arrs = [as_buffer(b) for b in bufs]
+        n = len(arrs)
+        if n == 0:
+            return []
+        dev = torch.device("cuda", self.device_index)
+        infos = [png_probe(a) for a in arrs]
+        # the pages are allocated on a stream of this decoder's own, so the caching allocator cannot hand out memory
+        # that work still queued on the caller's stream uses (the decode does not wait for that stream)
+        if self._alloc_stream is None:
+            self._alloc_stream = torch.cuda.Stream(dev)
+        with torch.cuda.stream(self._alloc_stream):
+            pages = [torch.empty((i["height"], i["width"], 3), dtype=torch.uint8, device=dev) if i["status"] == 0
+                     else None for i in infos]
+        data = (C.c_void_p * n)(*[a.ctypes.data for a in arrs])
+        lens = (C.c_size_t * n)(*[a.size for a in arrs])
+        dst = (C.c_void_p * n)(*[p.data_ptr() if p is not None else None for p in pages])
+        status = (C.c_int32 * n)()
+        rc = self.lib.ctd_png_decode(self.h, data, lens, n, dst, status)
+        if rc != 0:
+            raise CtdError("ctd_png_decode failed (%d): %s" % (rc, self.lib.ctd_last_error(None).decode()))
+        self.last_status = list(status)
+        cur = torch.cuda.current_stream(dev)
+        out = []
+        for a, p, s in zip(arrs, pages, status):
+            if s == 0:
+                p.record_stream(cur)
+                out.append(p)
+            else:
+                out.append(_cv2_decode(a))
+        return out
+
+    def last_stats(self):
+        """(deflate blocks, self-synchronisation rounds) of the last decode's files decoded on the GPU"""
+        blocks, rounds = C.c_int64(), C.c_int64()
+        if self.lib.ctd_png_decoder_stats(self.h, C.byref(blocks), C.byref(rounds)) != 0:
+            raise CtdError("ctd_png_decoder_stats failed: %s" % self.lib.ctd_last_error(None).decode())
+        return blocks.value, rounds.value

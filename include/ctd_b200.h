@@ -532,6 +532,67 @@ CTD_API void ctd_jpeg_decoder_destroy(ctd_jpeg_decoder* dec);
 CTD_API int ctd_jpeg_decode(ctd_jpeg_decoder* dec, const uint8_t* const* data, const size_t* len, int32_t n,
                             uint8_t* const* dst, int32_t* status);
 
+/* ---- PNG pages decoded on the GPU -------------------------------------------------------
+ * These entry points decode PNG files on the GPU to exactly the u8 BGR page cv2.imdecode(buf, IMREAD_COLOR) returns
+ * (cv2 4.13's libpng 1.6.53 and zlib 1.2.11): 16-bit samples keep their high byte, 1/2/4-bit grey is scaled to 8 bits,
+ * grey is replicated to B = G = R, palette indices are looked up ((0, 0, 0) past the PLTE entries), alpha is dropped
+ * without compositing, tRNS and gAMA have no effect, and an eXIf orientation is applied.  A file outside the supported
+ * set, or one whose data is not clean, gets a non-zero status and is left to cv2: the GPU path declines a file, it
+ * never returns a different one.
+ *
+ * Supported: non-interlaced grey 1/2/4/8/16, RGB 8/16, palette 1/2/4/8, grey+alpha 8/16 and RGBA 8/16 bits, IDAT
+ * chunks in one run, at most one eXIf chunk, no APNG chunks.                                                      */
+enum ctd_png_status {
+  CTD_PNG_OK = 0,
+  CTD_PNG_NOT_PNG = 1,     /* no PNG signature, or the first chunk is not IHDR                                  */
+  CTD_PNG_TRUNCATED = 2,   /* a chunk past the end of the file, no IDAT or no IEND                              */
+  CTD_PNG_HEADER = 3,      /* IHDR invalid: size, colour type / bit depth, compression, filter or interlace method */
+  CTD_PNG_INTERLACED = 4,  /* Adam7                                                                             */
+  CTD_PNG_APNG = 5,        /* acTL, fcTL or fdAT                                                                */
+  CTD_PNG_CHUNKS = 6,      /* IDAT chunks not in one run, PLTE missing, misplaced or invalid, an unknown
+                              critical chunk, a bad chunk name, a second IHDR, IEND with data                    */
+  CTD_PNG_EXIF = 7,        /* an eXIf chunk that does not parse cleanly, or two of them                         */
+  CTD_PNG_ZLIB = 8,        /* zlib header: CM not 8, CINFO above 7, FCHECK wrong or FDICT set                   */
+  CTD_PNG_SIZE = 9,        /* a side above 1000000, more than 2^30 pixels, 2^31 or more filtered bytes, or a
+                              zlib stream of 2^30 bytes or more                                                  */
+  CTD_PNG_CRC = 10,        /* a chunk whose CRC does not match (decode only)                                    */
+  CTD_PNG_DATA = 11        /* image data not clean (GPU decode): an invalid block type, stored length, code-length
+                              set or code, a distance past the output or the window, data after the final block,
+                              too few or too many bytes, a bad Adler-32, a filter type above 4                     */
+};
+typedef struct ctd_png_info {
+  int32_t status;              /* ctd_png_status; the fields below are set only for CTD_PNG_OK               */
+  int32_t height, width;       /* the decoded page as cv2.imdecode returns it, i.e. after the orientation      */
+  int32_t image_height, image_width;
+  int32_t bit_depth, color_type;
+  int32_t orientation;         /* eXIf orientation 1-8 (1 without an eXIf chunk)                              */
+  int32_t palette_entries;     /* PLTE entries, 0 without PLTE                                                */
+  int64_t zlib_bytes;          /* bytes of the zlib stream, the payloads of every IDAT chunk                   */
+} ctd_png_info;
+/* Chunk walk of one file (host only, no handle, thread-safe); chunk CRCs are checked by ctd_png_decode only.
+ * Returns 0, with the verdict in info->status; CTD_E_INVALID only for NULL arguments.                           */
+CTD_API int ctd_png_probe(const uint8_t* data, size_t len, ctd_png_info* info);
+
+typedef struct ctd_png_decoder ctd_png_decoder;
+/* A decoder bound to one GPU and one stream of its own.  subsequence_bits (>= 1; 0 picks the default, 512): the
+ * length of the pieces each Huffman block's bits are cut into for the self-synchronising parallel inflate (any value
+ * decodes the same pages; it only changes how many threads and rounds the inflate takes).  Not thread-safe; errors
+ * via ctd_last_error(NULL).                                                                                        */
+CTD_API int ctd_png_decoder_create(int32_t device, int32_t subsequence_bits, ctd_png_decoder** out);
+CTD_API void ctd_png_decoder_destroy(ctd_png_decoder* dec);
+/* Decodes n files at once: data[i] / len[i] (host memory).  Every file whose probe status is CTD_PNG_OK is decoded
+ * into dst[i], a DEVICE buffer of height * width * 3 bytes (u8 BGR [h][w][3], the probe's oriented shape) on the
+ * decoder's GPU; dst[i] may be NULL for other files.  status[i] gets the probe status or the decode's verdict
+ * (CTD_PNG_CRC, CTD_PNG_DATA); only pages with status 0 have been written, the others are to be decoded by cv2.
+ * Blocks until every page is written, so the buffers may be used on any stream.  Staging and the inflate buffer
+ * belong to the decoder and grow on demand.  CTD_E_CAPACITY, before any GPU work, for more than 65535 files the
+ * GPU takes in one call.                                                                                          */
+CTD_API int ctd_png_decode(ctd_png_decoder* dec, const uint8_t* const* data, const size_t* len, int32_t n,
+                           uint8_t* const* dst, int32_t* status);
+/* Of the last ctd_png_decode call's files decoded on the GPU: deflate blocks, and self-synchronisation rounds summed
+ * over their Huffman chunks (one round per chunk when every guessed start was right).                            */
+CTD_API int ctd_png_decoder_stats(const ctd_png_decoder* dec, int64_t* blocks, int64_t* rounds);
+
 /* ---- PNG files encoded on the GPU -------------------------------------------------------
  * The reference writes pages and masks with io_utils.imwrite = cv2.imencode('.png', img).tofile(path).  These entry
  * points encode u8 images on the GPU to exactly the bytes cv2.imencode('.png', img) gives with the libpng and zlib
