@@ -8,3 +8,4 @@ from .inference import TextDetector, REFINEMASK_INPAINT, REFINEMASK_ANNOTATION  
 from .basemodel import TextDetBase  # noqa: F401
 from .jpeg import JpegDecoder, jpeg_probe  # noqa: F401
 from .png import PngDecoder, PngEncoder, png_probe  # noqa: F401
+from .textmask import MaskRefiner, refine_mask, refine_undetected_mask  # noqa: F401

@@ -8,6 +8,8 @@
   <name>.png        the page re-encoded as PNG;  mask-<name>.png  the refined mask (io_utils.py:48-53 `imwrite`)
 
 -- produced with refine_mode=REFINEMASK_ANNOTATION, keep_undetected_mask=True like the reference.  SURVEY 8f row f2.
+`traverse_by_dict` reads such a directory back and refines each page's mask with the blocks of its json, as the
+reference's second tool does.
 """
 import glob
 import json
@@ -18,7 +20,9 @@ from pathlib import Path
 
 import numpy as np
 
-from .inference import REFINEMASK_ANNOTATION, TextDetector, check_page
+from .inference import REFINEMASK_ANNOTATION, REFINEMASK_INPAINT, TextDetector, check_page, decode_files
+from .png import is_png, png_probe
+from .textblock import TextBlock
 
 IMG_EXT = (".bmp", ".jpg", ".png", ".jpeg")
 
@@ -120,7 +124,7 @@ def _read_pages(imglist, det, failed):
     there: its error goes to `failed`."""
     for b0 in range(0, len(imglist), det.max_batch):
         paths = imglist[b0:b0 + det.max_batch]
-        pages = det._decode_files([np.fromfile(p, dtype=np.uint8) for p in paths])
+        pages = decode_files([np.fromfile(p, dtype=np.uint8) for p in paths], det.png_decoder, det.jpeg_decoder)
         for img_path, img in zip(paths, pages):
             try:
                 img = check_page(img, det.device_index)
@@ -184,3 +188,67 @@ def model2annotations(model_path, img_dir_list, save_dir, save_json=False, detec
             enc.close()
         if detector is None:
             det.close()
+
+
+def read_grey(bufs, png_decoder):
+    """encoded masks (1-D np.uint8 arrays) -> what `cv2.imdecode(buf, cv2.IMREAD_GRAYSCALE)` returns for each: for a
+    greyscale PNG (colour type 0) the GPU decodes, channel 0 of png_decoder()'s page (a strided CUDA view; cv2 reads
+    such a file to equal grey and colour pages), for every other file cv2's grey decode on the host"""
+    import cv2
+    grey = [i for i, b in enumerate(bufs) if is_png(b) and png_probe(b)["color_type"] == 0]
+    out = [None] * len(bufs)
+    if grey:
+        for i, page in zip(grey, png_decoder().decode([bufs[i] for i in grey])):
+            out[i] = None if page is None else page[..., 0]
+    for i, b in enumerate(bufs):
+        if out[i] is None:
+            out[i] = cv2.imdecode(b, cv2.IMREAD_GRAYSCALE)
+    return out
+
+
+def traverse_by_dict(img_dir_list, dict_dir, refiner=None):
+    """The reference's `traverse_by_dict(img_dir_list, dict_dir)` (inference.py:180-200) without its display: for
+    every image of `img_dir_list` in `find_all_imgs` order, the blocks of `dict_dir/<name>.json` (`TextBlock(**d)` for
+    each dict; FileNotFoundError when it is missing) and the mask `dict_dir/mask-<name>.png` (read as
+    `cv2.imread(path, IMREAD_GRAYSCALE)` reads it) refine the page's mask with REFINEMASK_INPAINT.  A generator of
+    `(img_path, img, mask_refined, blk_list)`: img is the page as decoded (a CUDA tensor where the GPU decodes it, else
+    cv2's numpy page), mask_refined a numpy array equal to the reference's `refine_mask(img, mask, blk_list)`.
+
+    Pages and masks are read in batches of the refiner's max_batch (a MaskRefiner; one is made and closed here when
+    none is given) and decoded on the GPU where it takes them (JPEG and PNG pages, greyscale PNG masks)."""
+    from .textmask import MaskRefiner
+    if isinstance(img_dir_list, str):
+        img_dir_list = [img_dir_list]
+    ref = refiner if refiner is not None else MaskRefiner()
+    try:
+        imglist = []
+        for d in img_dir_list:
+            imglist += find_all_imgs(d, abs_path=True)
+        read = deque()
+
+        def items():
+            for b0 in range(0, len(imglist), ref.max_batch):
+                paths = imglist[b0:b0 + ref.max_batch]
+                blks, mask_paths = [], []
+                for img_path in paths:
+                    imgname = osp.basename(img_path)
+                    imname = imgname.replace(Path(imgname).suffix, "")
+                    mask_paths.append(osp.join(dict_dir, "mask-" + imname + ".png"))
+                    with open(osp.join(dict_dir, imname + ".json"), "r", encoding="utf8") as f:
+                        blks.append([TextBlock(**d) for d in json.loads(f.read())])
+                pages = decode_files([np.fromfile(p, dtype=np.uint8) for p in paths], ref.png_decoder, ref.jpeg_decoder)
+                masks = read_grey([np.fromfile(p, dtype=np.uint8) for p in mask_paths], ref.png_decoder)
+                for img_path, img, mask_path, mask, blk_list in zip(paths, pages, mask_paths, masks, blks):
+                    if img is None:
+                        raise ValueError("%s could not be decoded (cv2.imdecode returns None)" % img_path)
+                    if mask is None:
+                        raise ValueError("%s could not be decoded (cv2.imdecode returns None)" % mask_path)
+                    read.append((img_path, img, blk_list))
+                    yield img, mask, blk_list
+
+        for _mask, mask_refined in ref.refine_stream(items(), refine_mode=REFINEMASK_INPAINT):
+            img_path, img, blk_list = read.popleft()
+            yield img_path, img, mask_refined, blk_list
+    finally:
+        if refiner is None:
+            ref.close()

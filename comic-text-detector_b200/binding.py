@@ -97,7 +97,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_collect_regions", "ctd_collect_device", "ctd_forward_tensor", "ctd_jpeg_probe",
            "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy", "ctd_jpeg_decode", "ctd_debug_postprocess",
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
-           "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats"]
+           "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
+           "ctd_refine_plan", "ctd_submit_refine"]
 
 _lib = None
 
@@ -158,6 +159,8 @@ def load_library():
     lib.ctd_collect_regions.argtypes = [vp, i32, C.POINTER(vp), C.POINTER(i32), C.POINTER(vp), C.POINTER(vp),
                                         C.POINTER(C.c_size_t)]
     lib.ctd_collect_device.argtypes = [vp, i32, vp]
+    lib.ctd_refine_plan.argtypes = [vp, i32, vp, vp, vp, vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
+    lib.ctd_submit_refine.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
     lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.ctd_jpeg_decoder_destroy.argtypes = [vp]
@@ -208,6 +211,41 @@ def pages_plan(shapes, net_h, net_w):
         raise CtdError("ctd_pages_plan failed (%d): pages %s do not letterbox into a %dx%d net input"
                        % (rc, list(shapes), net_h, net_w))
     return pages, int(ib.value), int(rb.value)
+
+
+def refine_plan(shapes, xyxy, n_blocks):
+    """`ctd_refine_plan` (host C++, no GPU): page sizes [(ih, iw), ...], every page's block boxes (int32 [k][4], page
+    0's first) and the number of boxes of each page -> (PAGE_ENTRY_DTYPE records, windows int32 [k][4], status int32
+    [k], input bytes, results bytes) of one batch for `Engine.submit_refine`."""
+    lib = load_library()
+    pages = np.zeros((len(shapes),), PAGE_ENTRY_DTYPE)
+    for i, (ih, iw) in enumerate(shapes):
+        pages[i]["ih"], pages[i]["iw"] = ih, iw
+    xyxy = np.ascontiguousarray(np.asarray(xyxy, np.int32).reshape(-1, 4))
+    counts = np.ascontiguousarray(n_blocks, np.int32).reshape(-1)
+    assert len(counts) == len(pages) and int(counts.sum()) == len(xyxy), (len(counts), len(pages), len(xyxy))
+    win = np.zeros((len(xyxy), 4), np.int32)
+    status = np.zeros((len(xyxy),), np.int32)
+    ib, rb = C.c_size_t(), C.c_size_t()
+    rc = lib.ctd_refine_plan(_ptr(pages), len(pages), _ptr(xyxy), _ptr(counts), _ptr(win), _ptr(status), C.byref(ib),
+                             C.byref(rb))
+    if rc != 0:
+        raise CtdError("ctd_refine_plan failed (%d): pages %s" % (rc, list(shapes)))
+    return pages, win, status, int(ib.value), int(rb.value)
+
+
+def _device_images(items, on_dev, events, channels):
+    """ctd_device_page entries of the CUDA images of a batch (NULL entries for the host ones), or None if none is"""
+    if not any(on_dev):
+        return None
+    dev = (CtdDevicePage * len(items))()
+    for i, p in enumerate(items):
+        if on_dev[i]:
+            ev = events[i] if events is not None else None
+            st = p.stride()   # uint8: element strides are byte strides
+            dev[i] = CtdDevicePage(p.data_ptr(), st[0], st[1], st[2] if channels == 3 else 0,
+                                   ev.cuda_event if ev is not None else None)
+    return dev
 
 
 def decode_block_section(sec, layout):
@@ -501,14 +539,7 @@ class Engine:
         for k, need in ((0, 0 if all(on_dev) else in_bytes), (1, res_bytes)):
             if need and (bufs[k] is None or bufs[k].numel() < need):
                 bufs[k] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
-        dev = None
-        if any(on_dev):
-            dev = (CtdDevicePage * len(pages))()
-            for i, p in enumerate(pages):
-                if on_dev[i]:
-                    ev = events[i] if events is not None else None
-                    sh, sw, sc = p.stride()   # uint8: element strides are byte strides
-                    dev[i] = CtdDevicePage(p.data_ptr(), sh, sw, sc, ev.cuda_event if ev is not None else None)
+        dev = _device_images(pages, on_dev, events, 3)
         if not all(on_dev):
             inp = bufs[0].numpy()
             for e, p, d in zip(entries, pages, on_dev):
@@ -557,6 +588,91 @@ class Engine:
         if textheight:
             crops = self.collect_regions(slot, n_lines)
             out = [o + (c,) for o, c in zip(out, crops)]
+        return out
+
+    def submit_refine(self, slot, pages, masks, boxes, refine_mode=0, keep_undetected=False, refined=None,
+                      events=None, device_results=False):
+        """asynchronous refine_mask of a batch (ctd_submit_refine): per page a u8 [h][w][3] page and a u8 [h][w] mask,
+        each a numpy array (packed into this slot's pinned input buffer) or a torch.uint8 CUDA tensor on this engine's
+        GPU with any strides (gathered on the GPU), and its block boxes (int32 [k][4]).  events[i] (a recorded
+        torch.cuda.Event, or None) is waited on before CUDA page i and CUDA mask i are read; the CUDA images are
+        referenced until the slot is collected and must not be written before.  refined: None, or per page a numpy
+        u8 [h][w] mask_refined to run refine_undetected_mask alone on (needs keep_undetected).  Collect with
+        collect_refine(slot)."""
+        import torch
+        if not hasattr(self, "_pg_bufs"):
+            self._pg_bufs = [[None, None], [None, None]]
+            self._pg_inflight = [None, None]
+        if self._pg_inflight[slot] is not None:
+            raise CtdError("slot %d has an uncollected submission" % slot)
+        counts = [len(b) for b in boxes]
+        xyxy = np.concatenate([np.asarray(b, np.int32).reshape(-1, 4) for b in boxes]) if boxes else np.zeros((0, 4))
+        entries, _win, _st, in_bytes, res_bytes = refine_plan([tuple(p.shape[:2]) for p in pages], xyxy, counts)
+        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
+        m_dev = [isinstance(m, torch.Tensor) and m.is_cuda for m in masks]
+        host = refined is not None or not all(on_dev) or not all(m_dev)
+        bufs = self._pg_bufs[slot]
+        for k, need in ((0, in_bytes if host else 0), (1, res_bytes)):
+            if need and (bufs[k] is None or bufs[k].numel() < need):
+                bufs[k] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        if host:
+            inp = bufs[0].numpy()
+            frame = in_bytes // 5 * 3
+            for e, p, d, m, md in zip(entries, pages, on_dev, masks, m_dev):
+                ih, iw = int(e["ih"]), int(e["iw"])
+                if not d:
+                    o = int(e["page_off"])
+                    np.copyto(inp[o:o + ih * iw * 3].reshape(ih, iw, 3), p)
+                if not md:
+                    o = frame + int(e["mask_off"])
+                    np.copyto(inp[o:o + ih * iw].reshape(ih, iw), m)
+            for e, r in zip(entries, refined or []):
+                o = frame + int(e["refined_off"])
+                np.copyto(inp[o:o + r.size].reshape(r.shape), r)
+        dev_p = _device_images(pages, on_dev, events, 3)
+        dev_m = _device_images(masks, m_dev, events, 1)
+        self._ck(self.lib.ctd_submit_refine(self.h, slot, _ptr(entries), len(entries), _ptr(xyxy), _ptr(np.asarray(
+            counts, np.int32)), C.c_void_p(bufs[0].data_ptr()) if host else None,
+            None if dev_p is None else C.cast(dev_p, C.c_void_p), None if dev_m is None else C.cast(dev_m, C.c_void_p),
+            int(refine_mode), int(bool(keep_undetected)), int(refined is not None), int(bool(device_results)),
+            C.c_void_p(bufs[1].data_ptr())))
+        kept = [x for i in range(len(pages)) for x, d in ((pages[i], on_dev[i]), (masks[i], m_dev[i])) if d]
+        self._pg_inflight[slot] = ("refine", entries, bool(keep_undetected), bool(device_results), kept, events)
+
+    def collect_refine(self, slot, discard=False):
+        """blocks until the batch of submit_refine(slot) is done -> per page (mask, mask_refined): mask is the mask
+        refine_undetected_mask modified (keep_undetected), else None.  numpy arrays copied out of the slot's pinned
+        buffer, or with device_results torch.uint8 CUDA tensors, views into one allocation of the page's own
+        (ctd_collect_device, complete on return, marked as used on the current stream).  discard: only wait."""
+        inflight = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
+        if inflight is None or inflight[0] != "refine":
+            raise CtdError("slot %d has no submit_refine batch in flight" % slot)
+        _kind, entries, keep, device_results, _kept, _events = inflight
+        self._pg_inflight[slot] = None
+        self.collect(slot)
+        if discard:
+            return None
+        shapes = [(int(e["ih"]), int(e["iw"])) for e in entries]
+        if device_results:
+            import torch
+            dev = torch.device("cuda", self.device)
+            if getattr(self, "_alloc_stream", None) is None:
+                self._alloc_stream = torch.cuda.Stream(dev)
+            with torch.cuda.stream(self._alloc_stream):
+                bufs = [torch.empty((2 * ih * iw,), dtype=torch.uint8, device=dev) for ih, iw in shapes]
+            self._ck(self.lib.ctd_collect_device(self.h, slot, (C.c_void_p * len(bufs))(*[b.data_ptr() for b in bufs])))
+            cur = torch.cuda.current_stream(dev)
+            out = []
+            for b, (ih, iw) in zip(bufs, shapes):
+                b.record_stream(cur)
+                out.append((b[:ih * iw].view(ih, iw) if keep else None, b[ih * iw:].view(ih, iw)))
+            return out
+        res = self._pg_bufs[slot][1].numpy()
+        out = []
+        for e, (ih, iw) in zip(entries, shapes):
+            mo, ro = int(e["mask_off"]), int(e["refined_off"])
+            out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy() if keep else None,
+                        res[ro:ro + ih * iw].reshape(ih, iw).copy()))
         return out
 
     def _collect_device(self, slot, entries, blocks, n_lines):

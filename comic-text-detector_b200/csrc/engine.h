@@ -104,6 +104,11 @@ struct PipeJob {
   int keep_undetected = 0;
   int textheight = 0;   // > 0: also crop every text line of every page (ctd_submit_pages)
   int results_on_device = 0;   // mask_refined, the modified mask and the crops stay on the device (ctd_collect_device)
+  // ctd_submit_refine: phase C alone, on each page's refine windows (x1 y1 x2 y2 each) and block boxes; with
+  // refined_input, d_ref holds the caller's mask_refined and only refine_undetected_mask runs
+  bool refine = false;
+  int refined_input = 0;
+  std::vector<std::vector<int32_t>> wins, boxes;
 };
 
 struct ctd_handle;
@@ -120,7 +125,7 @@ struct GrowBuf {
 using DevBuf = GrowBuf<false>;
 using PinnedBuf = GrowBuf<true>;
 
-// one of the two slots of the batch pipeline (ctd_submit_full, ctd_submit_pages): the staging and events of a batch
+// one of the two slots of the batch pipeline (ctd_submit_full, ctd_submit_pages, ctd_submit_refine): the staging and events of a batch
 // in flight, its hand-over from the worker, and the buffers its results stay in until the next submission
 struct Slot {
   // ctd_submit_full staging: the pages, and the device copy of the result arena (ctd_device_arena)
@@ -138,8 +143,9 @@ struct Slot {
   std::string err;
   char* pinned = nullptr;   // pinned staging of the refine window tables, pipe_pinned_cap bytes
   // ctd_submit_pages: packed pages | results head, masks, mask_refined | second refine output and threshold planes of
-  // refine_undetected_mask, grown while the slot is idle; page tables (pinned + device: max_batch PageGeom entries,
-  // then at pg_gather_off max_batch GatherPage entries for the pages gathered from device memory, uploaded together)
+  // refine_undetected_mask (ctd_submit_refine: the same without the results head), grown while the slot is idle; page
+  // tables (pinned + device: max_batch PageGeom entries, then at pg_gather_off 2 * max_batch GatherPage entries for
+  // the pages and masks gathered from device memory, uploaded together)
   DevBuf pg_in, pg_res, pg_aux;
   ctd::PageGeom* h_pg_tab = nullptr;
   ctd::PageGeom* d_pg_tab = nullptr;

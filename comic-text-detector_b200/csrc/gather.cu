@@ -1,7 +1,9 @@
-// Batched strided page gather (ctd_submit_pages): every page of a batch that is already in device memory, laid
-// out with any strides (a sub-window of a larger image, a permuted channels-first image), copied in one launch into the
-// packed page buffer of the batch (u8 BGR [ih][iw][3] at the page's page_off), where the letterbox, refine_mask and the
-// crop kernels read it.  One CTA per row over the stacked rows of the gathered pages, as backproject_batch_kernel.
+// Batched strided page gather (ctd_submit_pages, ctd_submit_refine): every page of a batch that is already in device
+// memory, laid out with any strides (a sub-window of a larger image, a permuted channels-first image), copied in one
+// launch into the packed page buffer of the batch (u8 BGR [ih][iw][3] at the page's page_off), where the letterbox,
+// refine_mask and the crop kernels read it; in the same launch, the batch's masks in device memory (u8 [ih][iw], any
+// strides: a channel of a page) into its packed mask plane.  One CTA per row over the stacked rows of the gathered
+// images, as backproject_batch_kernel.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -39,8 +41,7 @@ __device__ __forceinline__ void copy_shifted(const uint8_t* __restrict__ s, uint
   for (int i = head + nw * 4 + threadIdx.x; i < nb; i += blockDim.x) d[i] = s[i];
 }
 
-__global__ void __launch_bounds__(256) gather_pages_kernel(const GatherPage* __restrict__ tab, int n,
-                                                           uint8_t* __restrict__ dst) {
+__global__ void __launch_bounds__(256) gather_pages_kernel(const GatherPage* __restrict__ tab, int n) {
   const int r = blockIdx.x;
   int lo = 0, hi = n - 1;   // last page with row0 <= r
   while (lo < hi) {
@@ -49,14 +50,18 @@ __global__ void __launch_bounds__(256) gather_pages_kernel(const GatherPage* __r
   }
   const GatherPage g = tab[lo];
   const int y = r - g.row0;
-  const int nb = g.iw * 3;
+  const int nb = g.iw * g.ch;
   const uint8_t* s = g.src + y * g.sh;
-  uint8_t* d = dst + g.dst_off + size_t(y) * nb;
+  uint8_t* d = g.dst + size_t(y) * nb;
   if (g.fast) {
     const uintptr_t phase = uintptr_t(s) ^ uintptr_t(d);
     if ((phase & 15) == 0) copy_same_phase<uint4>(s, d, nb);
     else if ((phase & 3) == 0) copy_same_phase<uint32_t>(s, d, nb);
     else copy_shifted(s, d, nb);
+    return;
+  }
+  if (g.ch == 1) {
+    for (int i = threadIdx.x; i < nb; i += blockDim.x) d[i] = s[i * g.sw];
     return;
   }
   for (int i = threadIdx.x; i < nb; i += blockDim.x) {
@@ -67,9 +72,9 @@ __global__ void __launch_bounds__(256) gather_pages_kernel(const GatherPage* __r
 
 }  // namespace
 
-cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, uint8_t* dst, cudaStream_t s) {
+cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, cudaStream_t s) {
   if (n < 1 || total_rows < 1) return cudaErrorInvalidValue;
-  gather_pages_kernel<<<unsigned(total_rows), 256, 0, s>>>(d_tab, n, dst);
+  gather_pages_kernel<<<unsigned(total_rows), 256, 0, s>>>(d_tab, n);
   return cudaGetLastError();
 }
 

@@ -241,19 +241,20 @@ cudaError_t letterbox_batch_launch(const uint8_t* src, const PageGeom* d_tab, in
 cudaError_t backproject_batch_launch(const uint8_t* mask, int net_h, int net_w, const PageGeom* d_tab, int n,
                                      int total_rows, uint8_t* dst, cudaStream_t s);
 
-// Pages of a batch that are already in device memory (ctd_submit_pages), gathered into the packed page buffer
-// (gather.cu): byte (y, x, c) of the source is at src + y * sh + x * sw + c * sc; the packed page is u8 BGR [ih][iw][3]
-// at dst + dst_off.  The page owns rows [row0, row0 + ih) of the stacked rows of the launch's pages.  fast: sc == 1 and
-// sw == 3 (rows are contiguous runs of iw * 3 bytes at any pitch), copied with the widest accesses the alignment of
-// source and destination allows; else one byte per thread.
+// Pages (and masks) of a batch that are already in device memory (ctd_submit_pages, ctd_submit_refine), gathered
+// into the packed planes of the batch (gather.cu): byte (y, x, c) of the source is at src + y * sh + x * sw + c * sc;
+// the packed image is u8 [ih][iw][ch] at dst (ch = 3: a BGR page, ch = 1: a mask; sc is not read then).  The image
+// owns rows [row0, row0 + ih) of the stacked rows of the launch's images.  fast: sc == 1 and sw == ch (rows are
+// contiguous runs of iw * ch bytes at any pitch), copied with the widest accesses the alignment of source and
+// destination allows; else one byte per thread.
 struct GatherPage {
   const uint8_t* src;
   long long sh, sw, sc;
-  long long dst_off;
-  int ih, iw, row0, fast;
+  uint8_t* dst;
+  int ih, iw, row0, fast, ch, pad;
 };
-// one CTA per row of the n pages of d_tab (total_rows = the sum of their ih)
-cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, uint8_t* dst, cudaStream_t s);
+// one CTA per row of the n images of d_tab (total_rows = the sum of their ih)
+cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, cudaStream_t s);
 
 // refine_mask (refine_mk.cu): one kernel per phase over the window pixels of all pages of a batch, one CTA per chunk.
 struct RefineWin {

@@ -14,7 +14,8 @@
 // one back-projection launch per batch (TextDetector.detect_batch / detect_stream); with a textheight it also cuts
 // every text line of every page of the batch out of the resident pages in one k_warp_regions launch (region.cu).  Its
 // pages may already be in device memory (any strides; one gather_pages_kernel launch packs them, gather.cu) and the
-// masks and crops may stay there (ctd_collect_device).
+// masks and crops may stay there (ctd_collect_device).  ctd_submit_refine runs phase C alone on caller pages, masks
+// and block boxes (textmask.refine_mask / refine_undetected_mask, MaskRefiner) through the same two-slot schedule.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -160,12 +161,13 @@ PageIn page_in(const char* res, const PagesHead& head, int i, const JobPage& p, 
 }
 
 // expand_textwindow(img.shape, xyxy, 16) (utils/imgproc_utils.py:151-161) on an im_w x im_h page: win = x1 y1 x2 y2,
-// without the python slice normalisation (RefineJob::add applies it)
-std::array<int32_t, 4> expand_textwindow(int64_t x1, int64_t y1, int64_t x2, int64_t y2, int im_w, int im_h) {
+// without the python slice normalisation (RefineJob::add applies it).  In int64: a caller's box of int32 corners can
+// expand past int32 (ctd_refine_plan gives it status 2).
+std::array<int64_t, 4> expand_textwindow(int64_t x1, int64_t y1, int64_t x2, int64_t y2, int im_w, int im_h) {
   const int64_t w = x2 - x1, h = y2 - y1;
   const int64_t pad = int64_t(nearbyint((double(std::max(h, w)) * 0.25 + double(std::min(h, w)) * 0.75) / 16.0));
-  return {int32_t(std::max<int64_t>(0, x1 - pad)), int32_t(std::max<int64_t>(0, y1 - pad)),
-          int32_t(std::min<int64_t>(im_w - 1, x2 + pad)), int32_t(std::min<int64_t>(im_h - 1, y2 + pad))};
+  return {std::max<int64_t>(0, x1 - pad), std::max<int64_t>(0, y1 - pad), std::min<int64_t>(im_w - 1, x2 + pad),
+          std::min<int64_t>(im_h - 1, y2 + pad)};
 }
 
 // inference.py:101-114 (postprocess_yolo casts), 158-172 (box_thresh, line rescale), textblock.group_output,
@@ -218,8 +220,8 @@ int host_group_page(const PageIn& in, char* section, const BlockSection& L, std:
   win_out.resize(size_t(nb) * 4);
   for (int i = 0; i < nb; ++i) {
     const int32_t* xy = rec[i].xyxy;
-    const auto win = expand_textwindow(xy[0], xy[1], xy[2], xy[3], in.im_w, in.im_h);
-    std::copy(win.begin(), win.end(), win_out.begin() + 4 * i);
+    const auto win = expand_textwindow(xy[0], xy[1], xy[2], xy[3], in.im_w, in.im_h);   // inside the page
+    for (int k = 0; k < 4; ++k) win_out[size_t(4 * i + k)] = int32_t(win[k]);
   }
   return CTD_OK;
 }
@@ -262,11 +264,12 @@ struct Planes {
 
 // refine_undetected_mask (textmask.py:135-156) for a set of pages: one prep launch over all planes, connected
 // components + stats of each page on `st` (the scratch `cc` grows here), the host loop over each page's stats rows
-// against its blocks, then one refine launch for the extra windows of all pages and one OR launch.  The masks are
-// modified in place, as in the reference.
+// against its blocks (boxes[i]: x1 y1 x2 y2 of each block of page i), then one refine launch for the extra windows of
+// all pages and one OR launch.  The masks are modified in place, as in the reference.
 // Synchronises `st` once for the label counts and once for the stats rows.
-int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Planes& pl, int refine_mode,
-                      cudaStream_t st, DevBuf& cc, DevBuf& refine_scratch, char* pinned, size_t pinned_cap) {
+int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const std::vector<std::vector<int32_t>>& boxes,
+                      const Planes& pl, int refine_mode, cudaStream_t st, DevBuf& cc, DevBuf& refine_scratch,
+                      char* pinned, size_t pinned_cap) {
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const int n = int(pages.size());
   const size_t total_px = pl.total;
@@ -308,12 +311,11 @@ int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Pl
                          cudaMemcpyDeviceToHost, st));
   }
   CK(cudaStreamSynchronize(st));
-  const BlockSection bs = block_section_layout();
   RefineJob rj2;
   for (int i = 0; i < n; ++i) {
     const JobPage& p = pages[size_t(i)];
-    const int nb = reinterpret_cast<const ctd_page_blocks*>(p.section)->n_blocks;
-    const ctd_block* rec = reinterpret_cast<const ctd_block*>(p.section + bs.rec_off);
+    const std::vector<int32_t>& xyxy = boxes[size_t(i)];
+    const size_t nb = xyxy.size() / 4;
     bool first_valid = true;
     for (int li = 0; li < n_lab[size_t(i)]; ++li) {
       const int32_t* s5 = &stats[size_t(i)][size_t(li) * 5];
@@ -321,16 +323,16 @@ int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Pl
       if (first_valid) { first_valid = false; continue; }        // valid_labels[1:]
       const int64_t bb[4] = {s5[0], s5[1], int64_t(s5[0]) + s5[2], int64_t(s5[1]) + s5[3]};
       int64_t score = -1;
-      for (int b = 0; b < nb; ++b) {
-        const int32_t* q = rec[b].xyxy;
+      for (size_t b = 0; b < nb; ++b) {
+        const int32_t* q = &xyxy[4 * b];
         const int64_t x1 = std::max<int64_t>(q[0], bb[0]), y1 = std::max<int64_t>(q[1], bb[1]);
         const int64_t x2 = std::min<int64_t>(q[2], bb[2]), y2 = std::min<int64_t>(q[3], bb[3]);
         const int64_t a = (y2 < y1 || x2 < x1) ? -1 : (y2 - y1) * (x2 - x1);
         if (a > score) score = a;
       }
       if (double(score) / double(s5[2]) / double(s5[3]) < 0.5) {
-        const auto w4 = expand_textwindow(bb[0], bb[1], bb[2], bb[3], p.iw, p.ih);
-        rj2.add(w4[0], w4[1], w4[2], w4[3], p.off, p.iw, p.ih);
+        const auto w4 = expand_textwindow(bb[0], bb[1], bb[2], bb[3], p.iw, p.ih);   // inside the page
+        rj2.add(int(w4[0]), int(w4[1]), int(w4[2]), int(w4[3]), p.off, p.iw, p.ih);
       }
     }
   }
@@ -346,11 +348,12 @@ int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Pl
 }
 
 // phase C of a set of pages, mask_refined already zeroed: one refine launch over the windows of every page
-// (wins[i]: x1 y1 x2 y2 each), then with keep_undetected refine_undetected_mask.  Stream-ordered on `st` with the
-// scratch that belongs to it; `pinned` (optional, pinned_cap bytes) stages the window tables.
+// (wins[i]: x1 y1 x2 y2 each), then with keep_undetected refine_undetected_mask against the pages' block boxes
+// (boxes[i], read only then).  Stream-ordered on `st` with the scratch that belongs to it; `pinned` (optional,
+// pinned_cap bytes) stages the window tables.
 int phase_c(ctd_handle* h, const std::vector<JobPage>& pages, const std::vector<std::vector<int32_t>>& wins,
-            const Planes& pl, int refine_mode, bool keep_undetected, cudaStream_t st, DevBuf& refine_scratch,
-            DevBuf& cc, char* pinned, size_t pinned_cap) {
+            const std::vector<std::vector<int32_t>>& boxes, const Planes& pl, int refine_mode, bool keep_undetected,
+            cudaStream_t st, DevBuf& refine_scratch, DevBuf& cc, char* pinned, size_t pinned_cap) {
   RefineJob rj;
   for (size_t i = 0; i < pages.size(); ++i)
     for (size_t k = 0; k + 3 < wins[i].size(); k += 4)
@@ -358,7 +361,19 @@ int phase_c(ctd_handle* h, const std::vector<JobPage>& pages, const std::vector<
   char* stage = rj.table_bytes() <= pinned_cap ? pinned : nullptr;   // else: pageable + sync
   if (int rc = launch_refine(h, rj, pl.img, pl.mask, refine_mode, pl.ref, st, refine_scratch, stage)) return rc;
   if (!keep_undetected) return CTD_OK;
-  return refine_undetected(h, pages, pl, refine_mode, st, cc, refine_scratch, pinned, pinned_cap);
+  return refine_undetected(h, pages, boxes, pl, refine_mode, st, cc, refine_scratch, pinned, pinned_cap);
+}
+
+// the block boxes of each page's block section (the detector's own blocks), for refine_undetected
+std::vector<std::vector<int32_t>> section_boxes(const std::vector<JobPage>& pages) {
+  const BlockSection bs = block_section_layout();
+  std::vector<std::vector<int32_t>> boxes(pages.size());
+  for (size_t i = 0; i < pages.size(); ++i) {
+    const int nb = reinterpret_cast<const ctd_page_blocks*>(pages[i].section)->n_blocks;
+    const ctd_block* rec = reinterpret_cast<const ctd_block*>(pages[i].section + bs.rec_off);
+    for (int b = 0; b < nb; ++b) boxes[i].insert(boxes[i].end(), rec[b].xyxy, rec[b].xyxy + 4);
+  }
+  return boxes;
 }
 }  // namespace
 
@@ -389,34 +404,82 @@ PagesHead pages_head(int n) {
   return hd;
 }
 
-// Results buffer: pages_head(n) | masks | mask_refined planes | block sections.  Page i's pixel offset P_i (the sum of
-// the earlier pages' pixels, each rounded up to 256) is the same in every plane: image bytes at 3 P_i, mask at
-// masks + P_i, mask_refined at masks + P + P_i (P = the sum over the batch), so refine_mask addresses the image and the
-// mask planes of a page with one offset.
+// The pixel planes of a batch: page i's pixel offset P_i is the sum of the earlier pages' pixels, each rounded up to
+// 256, and is the same in every plane: image bytes at 3 P_i, mask at P_i of the mask plane, mask_refined at P_i of the
+// mask_refined plane, so refine_mask addresses the image and the mask planes of a page with one offset.  Fills page_off
+// (3 P_i), mask_off (mask_plane + P_i) and refined_off (mask_off + T) of each entry and returns T, the pixels of a plane
+// (the sum over the batch); the mask_refined plane follows the mask plane.
+static size_t plan_planes(ctd_page_entry* pages, int n, size_t mask_plane) {
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  size_t total = 0;
+  for (int i = 0; i < n; ++i) {
+    pages[i].page_off = int64_t(total * 3);
+    pages[i].mask_off = int64_t(mask_plane + total);
+    total += al(size_t(pages[i].ih) * size_t(pages[i].iw));
+  }
+  for (int i = 0; i < n; ++i) pages[i].refined_off = pages[i].mask_off + int64_t(total);
+  return total;
+}
+
+// Results buffer: pages_head(n) | masks | mask_refined planes | block sections (plan_planes).
 extern "C" int ctd_pages_plan(ctd_page_entry* pages, int32_t n, int32_t net_h, int32_t net_w, size_t* input_bytes,
                               size_t* results_bytes) {
   if (!input_bytes || !results_bytes || n < 0 || (n > 0 && !pages)) return CTD_E_INVALID;
   if (net_h < 64 || net_w < 64 || net_h % 64 || net_w % 64) return CTD_E_SHAPE;
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const PagesHead hd = pages_head(n);
-  size_t total = 0;
   for (int i = 0; i < n; ++i) {
     Letterbox lb;
     if (!letterbox_of(pages[i].ih, pages[i].iw, net_h, net_w, lb)) return CTD_E_SHAPE;
     pages[i].unpad_h = lb.unpad_h;
     pages[i].unpad_w = lb.unpad_w;
-    pages[i].page_off = int64_t(total * 3);
-    pages[i].mask_off = int64_t(hd.masks + total);
-    total += al(size_t(pages[i].ih) * size_t(pages[i].iw));
   }
+  const size_t total = plan_planes(pages, n, hd.masks);
   const size_t stride = al(block_section_layout().stride);
   const size_t blocks = hd.masks + 2 * total;
-  for (int i = 0; i < n; ++i) {
-    pages[i].refined_off = pages[i].mask_off + int64_t(total);
-    pages[i].blocks_off = int64_t(blocks + size_t(i) * stride);
-  }
+  for (int i = 0; i < n; ++i) pages[i].blocks_off = int64_t(blocks + size_t(i) * stride);
   *input_bytes = total * 3;
   *results_bytes = blocks + size_t(n) * stride;
+  return CTD_OK;
+}
+
+// Input: the pages (3 T bytes), then a frame laid out as the results; results: masks | mask_refined (plan_planes).
+extern "C" int ctd_refine_plan(ctd_page_entry* pages, int32_t n, const int32_t* xyxy, const int32_t* n_blocks,
+                               int32_t* windows, int32_t* status, size_t* input_bytes, size_t* results_bytes) {
+  if (!input_bytes || !results_bytes || n < 0 || (n > 0 && (!pages || !n_blocks))) return CTD_E_INVALID;
+  int64_t nb = 0;
+  for (int i = 0; i < n; ++i) {
+    if (pages[i].ih < 1 || pages[i].iw < 1) return CTD_E_SHAPE;
+    if (n_blocks[i] < 0) return CTD_E_INVALID;
+    nb += n_blocks[i];
+  }
+  if (nb > INT32_MAX) return CTD_E_CAPACITY;
+  if (nb > 0 && (!xyxy || !windows || !status)) return CTD_E_INVALID;
+  for (int i = 0; i < n; ++i) {
+    pages[i].unpad_h = pages[i].unpad_w = 0;
+    pages[i].blocks_off = 0;
+  }
+  const size_t total = plan_planes(pages, n, 0);
+  size_t b = 0;
+  for (int i = 0; i < n; ++i) {
+    const int ih = pages[i].ih, iw = pages[i].iw;
+    for (int k = 0; k < n_blocks[i]; ++k, ++b) {
+      const int32_t* q = xyxy + 4 * b;
+      const auto w = expand_textwindow(q[0], q[1], q[2], q[3], iw, ih);
+      bool fits = true;
+      for (int j = 0; j < 4; ++j) {
+        fits = fits && w[j] >= INT32_MIN && w[j] <= INT32_MAX;
+        windows[4 * b + j] = int32_t(std::min<int64_t>(std::max<int64_t>(w[j], INT32_MIN), INT32_MAX));
+      }
+      // img[by1:by2, bx1:bx2] empty: cv2.cvtColor raises in get_topk_masklist
+      int x1 = windows[4 * b], y1 = windows[4 * b + 1], x2 = windows[4 * b + 2], y2 = windows[4 * b + 3];
+      norm_slice(x1, x2, iw);
+      norm_slice(y1, y2, ih);
+      status[b] = !fits ? 2 : (x2 > x1 && y2 > y1) ? 0 : 1;
+    }
+  }
+  *input_bytes = total * 5;
+  *results_bytes = total * 2;
   return CTD_OK;
 }
 
@@ -442,6 +505,23 @@ static int plan_page_regions(const char* section, const BlockSection& bs, int iw
   *bytes = 0;
   if (lines.empty()) return CTD_OK;   // nothing to plan, whatever the page size
   return ctd_region_plan(lines.data(), int32_t(lines.size()), iw, ih, textheight, plan.data(), bytes);
+}
+
+// the device planes of a submitted batch
+static Planes job_planes(const PipeJob& job) {
+  return Planes{job.d_img, job.d_mask, job.d_ref, job.d_aux, job.d_aux ? job.d_aux + job.total : nullptr, job.total};
+}
+
+// the end of a batch on the worker's stream `st`: the masks refine_undetected_mask modified and mask_refined back to
+// results_host (unless they stay on the device), then the batch's done event
+static int finish_batch(ctd_handle* h, const PipeJob& job, cudaStream_t st) {
+  if (!job.results_on_device) {
+    char* res = job.results_host;
+    if (job.keep_undetected) CK(cudaMemcpyAsync(res + job.head.masks, job.d_mask, job.total, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(res + job.refined, job.d_ref, job.total, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaEventRecord(h->slot[job.slot].ev_post_done, st));
+  return CTD_OK;
 }
 
 // phases B and C of a submitted batch, on the worker thread
@@ -528,16 +608,31 @@ static int run_batch(ctd_handle* h, const PipeJob& job) {
     s.crop_px_off = tb;
   }
   CK(cudaMemsetAsync(job.d_ref, 0, job.total, st));
-  const Planes pl{job.d_img, job.d_mask, job.d_ref, job.d_aux, job.d_aux ? job.d_aux + job.total : nullptr, job.total};
-  if (int rc = phase_c(h, job.pages, wins, pl, job.refine_mode, job.keep_undetected, st, h->post_refine, h->pg_cc,
-                       s.pinned, h->pipe_pinned_cap))
+  const auto boxes = job.keep_undetected ? section_boxes(job.pages) : std::vector<std::vector<int32_t>>();
+  if (int rc = phase_c(h, job.pages, wins, boxes, job_planes(job), job.refine_mode, job.keep_undetected, st,
+                       h->post_refine, h->pg_cc, s.pinned, h->pipe_pinned_cap))
     return rc;
-  if (to_host) {
-    if (job.keep_undetected) CK(cudaMemcpyAsync(res + job.head.masks, job.d_mask, job.total, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(res + job.refined, job.d_ref, job.total, cudaMemcpyDeviceToHost, st));
+  return finish_batch(h, job, st);
+}
+
+// ctd_submit_refine's batch on the worker: phase C on the caller's pages, masks and windows, or with a refined input
+// refine_undetected_mask alone
+static int run_refine_batch(ctd_handle* h, const PipeJob& job) {
+  Slot& s = h->slot[job.slot];
+  cudaStream_t st = h->post;
+  CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // the packed pages and masks are in place
+  const Planes pl = job_planes(job);
+  if (job.refined_input) {
+    if (int rc = refine_undetected(h, job.pages, job.boxes, pl, job.refine_mode, st, h->pg_cc, h->post_refine,
+                                   s.pinned, h->pipe_pinned_cap))
+      return rc;
+  } else {
+    CK(cudaMemsetAsync(job.d_ref, 0, job.total, st));
+    if (int rc = phase_c(h, job.pages, job.wins, job.boxes, pl, job.refine_mode, job.keep_undetected, st,
+                         h->post_refine, h->pg_cc, s.pinned, h->pipe_pinned_cap))
+      return rc;
   }
-  CK(cudaEventRecord(s.ev_post_done, st));
-  return CTD_OK;
+  return finish_batch(h, job, st);
 }
 
 // ---- batch pipeline -------------------------------------------------------------------------------------------------
@@ -552,7 +647,7 @@ static void pipe_worker(ctd_handle* h) {
       job = std::move(h->pipe_queue.front());
       h->pipe_queue.pop_front();
     }
-    const int rc = run_batch(h, job);
+    const int rc = job.refine ? run_refine_batch(h, job) : run_batch(h, job);
     std::string err;
     if (rc != CTD_OK) err = h->err;
     {
@@ -698,6 +793,48 @@ static bool is_device_memory(const void* p, int device) {
   return a.type == cudaMemoryTypeDevice && a.device == device;
 }
 
+// a page (ch = 3) or mask (ch = 1) of a batch in device memory: strides in range, and its first and last byte memory
+// of the handle's GPU
+static int check_device_image(ctd_handle* h, const char* what, int i, const ctd_device_page& d, int ih, int iw, int ch) {
+  const int64_t kMaxStride = int64_t(1) << 31;   // keeps the image's last byte offset inside int64
+  const int64_t sc = ch == 3 ? d.stride_c : 0;
+  if (d.stride_h < 0 || d.stride_w < 0 || sc < 0 || d.stride_h > kMaxStride || d.stride_w > kMaxStride || sc > kMaxStride)
+    return ctd_fail(h, CTD_E_INVALID, "%s %d: strides (%lld, %lld, %lld) out of range [0, 2^31]", what, i,
+                    (long long)d.stride_h, (long long)d.stride_w, (long long)sc);
+  const uint8_t* last = d.data + (ih - 1) * d.stride_h + (iw - 1) * d.stride_w + (ch - 1) * sc;
+  if (!is_device_memory(d.data, h->cfg.device) || !is_device_memory(last, h->cfg.device))
+    return ctd_fail(h, CTD_E_INVALID, "%s %d (%p) is not device memory of GPU %d", what, i, (const void*)d.data,
+                    h->cfg.device);
+  return CTD_OK;
+}
+
+// the slot's page tables, allocated at its first batch: max_batch PageGeom entries, then at pg_gather_off room for a
+// GatherPage entry per page and per mask of a batch
+static int ensure_page_tables(ctd_handle* h, Slot& s) {
+  if (s.h_pg_tab) return CTD_OK;
+  h->pg_gather_off = (size_t(h->cfg.max_batch) * sizeof(PageGeom) + 255) / 256 * 256;
+  const size_t tab_bytes = h->pg_gather_off + 2 * size_t(h->cfg.max_batch) * sizeof(GatherPage);
+  CK(cudaHostAlloc(reinterpret_cast<void**>(&s.h_pg_tab), tab_bytes, cudaHostAllocDefault));
+  CK(cudaMalloc(reinterpret_cast<void**>(&s.d_pg_tab), tab_bytes));
+  return CTD_OK;
+}
+
+// H2D on `st` of the byte ranges [off(i), off(i) + bytes(i)) from src to dst of the pages that are not on the device
+// (dev[i].data == NULL, or dev NULL), one copy per run of consecutive such pages
+template <typename Off, typename Len>
+static int copy_host_runs(ctd_handle* h, const ctd_device_page* dev, int n, uint8_t* dst, const uint8_t* src, Off off,
+                          Len bytes, cudaStream_t st) {
+  for (int i = 0; i < n;) {
+    if (dev && dev[i].data) { ++i; continue; }
+    int j = i;
+    while (j + 1 < n && !(dev && dev[j + 1].data)) ++j;
+    const size_t lo = off(i), hi = off(j) + bytes(j);
+    CK(cudaMemcpyAsync(dst + lo, src + lo, hi - lo, cudaMemcpyHostToDevice, st));
+    i = j + 1;
+  }
+  return CTD_OK;
+}
+
 extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
                                 int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
                                 int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
@@ -731,17 +868,7 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
       if (!input_host) return ctd_fail(h, CTD_E_INVALID, "page %d is in neither input_host nor device memory", i);
       continue;
     }
-    const ctd_device_page& d = dev[i];
-    const int64_t kMaxStride = int64_t(1) << 31;   // keeps the page's last byte offset inside int64
-    if (d.stride_h < 0 || d.stride_w < 0 || d.stride_c < 0 || d.stride_h > kMaxStride || d.stride_w > kMaxStride ||
-        d.stride_c > kMaxStride)
-      return ctd_fail(h, CTD_E_INVALID, "page %d: strides (%lld, %lld, %lld) out of range [0, 2^31]", i,
-                      (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c);
-    const ctd_page_entry& e = pg[size_t(i)];
-    const uint8_t* last = d.data + (e.ih - 1) * d.stride_h + (e.iw - 1) * d.stride_w + 2 * d.stride_c;
-    if (!is_device_memory(d.data, h->cfg.device) || !is_device_memory(last, h->cfg.device))
-      return ctd_fail(h, CTD_E_INVALID, "page %d (%p) is not device memory of GPU %d", i, (const void*)d.data,
-                      h->cfg.device);
+    if (int rc = check_device_image(h, "page", i, dev[i], pg[size_t(i)].ih, pg[size_t(i)].iw, 3)) return rc;
     ++n_dev;
   }
   ShapePlan* sp = nullptr;
@@ -757,12 +884,7 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   if (int rc = s.pg_res.grow(h, d2h + total, std::nullopt)) return rc;
   if (keep_undetected)
     if (int rc = s.pg_aux.grow(h, 2 * total, std::nullopt)) return rc;
-  if (!s.h_pg_tab) {
-    h->pg_gather_off = (size_t(h->cfg.max_batch) * sizeof(PageGeom) + 255) / 256 * 256;
-    const size_t tab_bytes = h->pg_gather_off + size_t(h->cfg.max_batch) * sizeof(GatherPage);
-    CK(cudaHostAlloc(reinterpret_cast<void**>(&s.h_pg_tab), tab_bytes, cudaHostAllocDefault));
-    CK(cudaMalloc(reinterpret_cast<void**>(&s.d_pg_tab), tab_bytes));
-  }
+  if (int rc = ensure_page_tables(h, s)) return rc;
   PageGeom* tab = s.h_pg_tab;
   GatherPage* gtab = reinterpret_cast<GatherPage*>(reinterpret_cast<char*>(tab) + h->pg_gather_off);
   int row0 = 0, n_gather = 0, gather_rows = 0;
@@ -773,8 +895,8 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
     if (dev && dev[i].data) {
       const ctd_device_page& d = dev[i];
       gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c,
-                                    (long long)e.page_off, e.ih, e.iw, gather_rows,
-                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0};
+                                    s.pg_in.p + e.page_off, e.ih, e.iw, gather_rows,
+                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0, 3, 0};
       gather_rows += e.ih;
     }
   }
@@ -786,15 +908,10 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   if (n_dev == 0) {
     CK(cudaMemcpyAsync(s.pg_in.p, input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
   } else {
-    for (int i = 0; i < n;) {
-      if (dev[i].data) { ++i; continue; }
-      int j = i;
-      while (j + 1 < n && !dev[j + 1].data) ++j;
-      const size_t lo = size_t(pg[size_t(i)].page_off);
-      const size_t hi = size_t(pg[size_t(j)].page_off) + size_t(pg[size_t(j)].ih) * size_t(pg[size_t(j)].iw) * 3;
-      CK(cudaMemcpyAsync(s.pg_in.p + lo, input_host + lo, hi - lo, cudaMemcpyHostToDevice, h->copy_in));
-      i = j + 1;
-    }
+    if (int rc = copy_host_runs(h, dev, n, s.pg_in.p, input_host, [&](int i) { return size_t(pg[size_t(i)].page_off); },
+                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; },
+                                h->copy_in))
+      return rc;
   }
   CK(cudaEventRecord(s.ev_in_done, h->copy_in));
   CK(cudaEventRecord(h->ev0, h->stream));
@@ -804,7 +921,7 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
       if (dev[i].data && dev[i].event) CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(dev[i].event), 0));
     CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(reinterpret_cast<const char*>(s.d_pg_tab) +
                                                                h->pg_gather_off),
-                           n_gather, gather_rows, s.pg_in.p, h->stream));
+                           n_gather, gather_rows, h->stream));
   }
   CK(letterbox_batch_launch(s.pg_in.p, s.d_pg_tab, n, h->d_pages, net_h, net_w, h->stream));
   if (int rc = enqueue_forward(h, n, net_h, net_w, *sp)) return rc;
@@ -838,6 +955,139 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   job.d_aux = keep_undetected ? s.pg_aux.p : nullptr;
   job.keep_undetected = keep_undetected ? 1 : 0;
   job.textheight = textheight;
+  job.results_on_device = results_on_device ? 1 : 0;
+  if (results_on_device) s.dev_pages = std::move(pg);
+  queue_job(h, std::move(job));
+  return CTD_OK;
+}
+
+extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
+                                 const int32_t* xyxy, const int32_t* n_blocks, const uint8_t* input_host,
+                                 const ctd_device_page* dev_pages, const ctd_device_page* dev_masks,
+                                 int32_t refine_mode, int32_t keep_undetected, int32_t refined_input,
+                                 int32_t results_on_device, void* results_host) {
+  if (!h || !pages || !n_blocks || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  Slot& s = h->slot[slot];
+  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
+  if (refined_input && (!keep_undetected || !input_host))
+    return ctd_fail(h, CTD_E_INVALID, "a refined input needs keep_undetected and input_host");
+  // the offsets and windows decide what the copies and the refine touch: they must be the plan's
+  std::vector<ctd_page_entry> pg(pages, pages + n);
+  int64_t nb = 0;
+  for (int i = 0; i < n; ++i) nb += std::max(n_blocks[i], 0);
+  std::vector<int32_t> win(static_cast<size_t>(nb) * 4), status(static_cast<size_t>(nb));
+  size_t in_bytes = 0, res_bytes = 0;
+  if (int rc = ctd_refine_plan(pg.data(), n, xyxy, n_blocks, win.data(), status.data(), &in_bytes, &res_bytes))
+    return ctd_fail(h, rc, "ctd_refine_plan refuses the batch");
+  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
+    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_refine_plan returns");
+  const size_t total = in_bytes / 5;
+  PipeJob job;
+  job.wins.resize(size_t(n));
+  job.boxes.resize(size_t(n));
+  size_t rows = 0;
+  for (int i = 0, b = 0; i < n; ++i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    rows += size_t(e.ih);
+    if (keep_undetected && size_t(e.ih) * size_t(e.iw) > kCclMaxPixels)
+      return ctd_fail(h, CTD_E_CAPACITY, "page %d (%dx%d): refine_undetected_mask labels pages of at most 2^28 pixels", i,
+                      e.ih, e.iw);
+    for (int k = 0; k < n_blocks[i]; ++k, ++b) {
+      // refine_mask raises on such a block; refine_undetected_mask alone only compares the boxes
+      if (!refined_input && status[size_t(b)] != 0)
+        return ctd_fail(h, CTD_E_INVALID, "page %d, block %d (%d, %d, %d, %d): %s", i, k, xyxy[4 * b], xyxy[4 * b + 1],
+                        xyxy[4 * b + 2], xyxy[4 * b + 3],
+                        status[size_t(b)] == 1 ? "its window is empty, refine_mask raises on it"
+                                               : "its window does not fit int32");
+      job.wins[size_t(i)].insert(job.wins[size_t(i)].end(), &win[4 * size_t(b)], &win[4 * size_t(b)] + 4);
+      job.boxes[size_t(i)].insert(job.boxes[size_t(i)].end(), xyxy + 4 * size_t(b), xyxy + 4 * size_t(b) + 4);
+    }
+  }
+  if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
+  CK(cudaSetDevice(h->cfg.device));
+  int n_dev_pages = 0, n_dev_masks = 0;
+  for (int i = 0; i < n; ++i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    for (int m = 0; m < 2; ++m) {
+      const ctd_device_page* d = m ? dev_masks : dev_pages;
+      if (d && d[i].data) {
+        if (int rc = check_device_image(h, m ? "mask" : "page", i, d[i], e.ih, e.iw, m ? 1 : 3)) return rc;
+        ++(m ? n_dev_masks : n_dev_pages);
+      } else if (!input_host) {
+        return ctd_fail(h, CTD_E_INVALID, "%s %d is in neither input_host nor device memory", m ? "mask" : "page", i);
+      }
+    }
+  }
+  if (int rc = ensure_full_pipeline(h)) return rc;
+  s.start(false, results_on_device != 0);
+  // grown while the slot is idle: its collect has synchronised the work of its last batch.  pg_in: the packed pages;
+  // pg_res: the frame of masks and mask_refined planes the refine reads and writes in place
+  if (int rc = s.pg_in.grow(h, 3 * total, std::nullopt)) return rc;
+  if (int rc = s.pg_res.grow(h, res_bytes, std::nullopt)) return rc;
+  if (keep_undetected)
+    if (int rc = s.pg_aux.grow(h, 2 * total, std::nullopt)) return rc;
+  if (int rc = ensure_page_tables(h, s)) return rc;
+  GatherPage* gtab = reinterpret_cast<GatherPage*>(reinterpret_cast<char*>(s.h_pg_tab) + h->pg_gather_off);
+  int n_gather = 0, gather_rows = 0;
+  for (int i = 0; i < n; ++i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    if (dev_pages && dev_pages[i].data) {
+      const ctd_device_page& d = dev_pages[i];
+      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c,
+                                    s.pg_in.p + e.page_off, e.ih, e.iw, gather_rows,
+                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0, 3, 0};
+      gather_rows += e.ih;
+    }
+    if (dev_masks && dev_masks[i].data) {
+      const ctd_device_page& d = dev_masks[i];
+      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, 0, s.pg_res.p + e.mask_off,
+                                    e.ih, e.iw, gather_rows, d.stride_w == 1 ? 1 : 0, 1, 0};
+      gather_rows += e.ih;
+    }
+  }
+  // the tables and the host pages and masks in on copy_in (only the byte ranges of the images in input_host); the
+  // waits on the device images' events and one gather of every device page and mask on the engine stream
+  cudaStream_t cin = h->copy_in;
+  const uint8_t* host_frame = input_host ? input_host + 3 * total : nullptr;
+  if (n_gather)
+    CK(cudaMemcpyAsync(reinterpret_cast<char*>(s.d_pg_tab) + h->pg_gather_off, gtab, size_t(n_gather) * sizeof(GatherPage),
+                       cudaMemcpyHostToDevice, cin));
+  if (n_dev_pages < n)
+    if (int rc = copy_host_runs(h, dev_pages, n, s.pg_in.p, input_host,
+                                [&](int i) { return size_t(pg[size_t(i)].page_off); },
+                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; }, cin))
+      return rc;
+  if (n_dev_masks < n)
+    if (int rc = copy_host_runs(h, dev_masks, n, s.pg_res.p, host_frame,
+                                [&](int i) { return size_t(pg[size_t(i)].mask_off); },
+                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw); }, cin))
+      return rc;
+  if (refined_input) CK(cudaMemcpyAsync(s.pg_res.p + total, host_frame + total, total, cudaMemcpyHostToDevice, cin));
+  CK(cudaEventRecord(s.ev_in_done, cin));
+  CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
+  if (n_gather) {
+    for (int i = 0; i < n; ++i)
+      for (const ctd_device_page* d : {dev_pages, dev_masks})
+        if (d && d[i].data && d[i].event) CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(d[i].event), 0));
+    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(reinterpret_cast<const char*>(s.d_pg_tab) +
+                                                               h->pg_gather_off),
+                           n_gather, gather_rows, h->stream));
+  }
+  CK(cudaEventRecord(s.ev_out_ready, h->stream));
+  job.refine = true;
+  job.slot = slot; job.refine_mode = refine_mode;
+  job.results_host = static_cast<char*>(results_host);
+  job.head.masks = 0;
+  job.refined = total;
+  for (const ctd_page_entry& e : pg) job.pages.push_back(JobPage{e.ih, e.iw, 1.f, 1.f, size_t(e.mask_off), nullptr});
+  job.total = total;
+  job.d_img = s.pg_in.p;
+  job.d_mask = s.pg_res.p;
+  job.d_ref = s.pg_res.p + total;
+  job.d_aux = keep_undetected ? s.pg_aux.p : nullptr;
+  job.keep_undetected = keep_undetected ? 1 : 0;
+  job.refined_input = refined_input ? 1 : 0;
   job.results_on_device = results_on_device ? 1 : 0;
   if (results_on_device) s.dev_pages = std::move(pg);
   queue_job(h, std::move(job));
@@ -982,7 +1232,9 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   }
   // phase C; refine_undetected_mask modifies the page mask in place and it is returned, as in the reference
   const Planes pl{d_page, d_mask, d_ref, d_ref2, d_thr, px};
-  if (int rc = phase_c(h, pages, wins, pl, refine_mode, keep_undetected, st, h->refine_scratch, h->cc_scratch, nullptr, 0))
+  const auto boxes = keep_undetected ? section_boxes(pages) : std::vector<std::vector<int32_t>>();
+  if (int rc = phase_c(h, pages, wins, boxes, pl, refine_mode, keep_undetected, st, h->refine_scratch, h->cc_scratch,
+                       nullptr, 0))
     return rc;
   if (keep_undetected) CK(cudaMemcpyAsync(mask_out, d_mask, px, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(mask_refined_out, d_ref, px, cudaMemcpyDeviceToHost, st));

@@ -115,17 +115,8 @@ class TextDetector:
             self._png = None
 
     def _decode_files(self, bufs):
-        """encoded files (1-D np.uint8 arrays) -> their pages in input order: files with the PNG signature through
-        png_decoder(), every other file through jpeg_decoder() (baseline JPEGs on the GPU, the rest by cv2); each page
-        is a CUDA tensor or what cv2.imdecode returns"""
-        pngs = [i for i, b in enumerate(bufs) if is_png(b)]
-        others = [i for i, b in enumerate(bufs) if not is_png(b)]
-        out = [None] * len(bufs)
-        for idx, dec in ((pngs, self.png_decoder), (others, self.jpeg_decoder)):
-            if idx:
-                for i, page in zip(idx, dec().decode([bufs[i] for i in idx])):
-                    out[i] = page
-        return out
+        """decode_files with this detector's decoders"""
+        return decode_files(bufs, self.png_decoder, self.jpeg_decoder)
 
     def __call__(self, img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
         """reference inference.py:141-178.  One native call (`ctd_detect_page`): letterbox (cv2-exact INTER_LINEAR) +
@@ -262,6 +253,21 @@ class TextDetector:
         free.append(slot)
         for mask, mask_refined, rec, lines, dist, *crops in pages:
             yield (mask, mask_refined, blocks_from_records(rec, lines, dist)) + tuple(crops)
+
+
+def decode_files(bufs, png_decoder, jpeg_decoder):
+    """encoded files (1-D np.uint8 arrays) -> their pages in input order: files with the PNG signature through
+    png_decoder() (a function returning a PngDecoder), every other file through jpeg_decoder() (baseline JPEGs on the
+    GPU, the rest by cv2); each page is a CUDA tensor or what cv2.imdecode(buf, IMREAD_COLOR) returns.  A decoder is
+    asked for only when a file goes to it."""
+    pngs = [i for i, b in enumerate(bufs) if is_png(b)]
+    others = [i for i, b in enumerate(bufs) if not is_png(b)]
+    out = [None] * len(bufs)
+    for idx, dec in ((pngs, png_decoder), (others, jpeg_decoder)):
+        if idx:
+            for i, page in zip(idx, dec().decode([bufs[i] for i in idx])):
+                out[i] = page
+    return out
 
 
 def check_page(img, device_index=None):

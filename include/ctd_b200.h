@@ -467,6 +467,47 @@ CTD_API int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* 
  * stream.  CTD_E_INVALID for a slot in flight or whose last batch was not submitted with results_on_device.       */
 CTD_API int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page_dst);
 
+/* ---- refine_mask on any block list (utils/textmask.py:135-169) ------------------------------------------------------
+ * `refine_mask(img, pred_mask, blk_list, refine_mode)` and `refine_undetected_mask(img, mask_pred, mask_refined,
+ * blk_list, refine_mode)` for pages, masks and blocks the caller gives: a block list edited after detection (SFX blocks
+ * dropped, a missed block added, blocks merged or moved), or one read back from `model2annotations`'s json.
+ *
+ * ctd_refine_plan (host code, no handle, thread-safe, needs no GPU) lays a batch out and checks its blocks.  The
+ * caller fills ih, iw of each entry (any page of at least 1 x 1: there is no letterbox); the plan fills the rest, with
+ * the pixel offsets of ctd_pages_plan (unpad_h, unpad_w and blocks_off are 0).  Every offset is a multiple of 256.
+ * With T = *results_bytes / 2:
+ *   input  (*input_bytes = 5 T): page i, u8 BGR [ih][iw][3], at page_off; then at byte 3 T a frame laid out as the
+ *                                results: its u8 [ih][iw] mask at 3 T + mask_off and, for a refined input, its
+ *                                mask_refined at 3 T + refined_off
+ *   results (*results_bytes):    page i's mask at mask_off, mask_refined at refined_off
+ * xyxy: the block boxes, i32 [sum n_blocks][4], page 0's n_blocks[0] blocks first.  For each block it writes the
+ * window refine_mask refines, expand_textwindow(img.shape, xyxy, 16) (windows, i32 [.][4], before Python's slice
+ * normalisation, clamped to int32), and a status: 0 the window is fine; 1 the reference raises on the block (the window
+ * is empty after Python's slice normalisation, e.g. y2 <= y1 or an x2 + pad that wraps negative: cv2.cvtColor raises
+ * on the empty crop); 2 a window coordinate does not fit int32.  CTD_E_SHAPE for a page side < 1.                  */
+CTD_API int ctd_refine_plan(ctd_page_entry* pages, int32_t n, const int32_t* xyxy, const int32_t* n_blocks,
+                            int32_t* windows, int32_t* status, size_t* input_bytes, size_t* results_bytes);
+/* ctd_submit_refine runs refine_mask on a planned batch through the schedule of ctd_submit_pages (slots 0 and 1, two
+ * batches in flight, collected with ctd_collect and, with results_on_device, ctd_collect_device, which then gives each
+ * page's [mask | mask_refined]).  pages / n / xyxy / n_blocks: the planned entries and the boxes they were planned
+ * with (checked against a fresh plan).  Pages come from input_host or from device memory (dev_pages, as
+ * ctd_submit_pages takes them); masks from input_host's frame or from device memory (dev_masks, NULL or n entries:
+ * u8 [ih][iw] at data + y * stride_h + x * stride_w, any strides, stride_c not read, e.g. channel 0 of a page).  One
+ * gather launch on the engine stream packs every device page and mask, after the waits on their events.
+ * On the GPU: one refine_mask launch over the windows of every block of every page; with keep_undetected != 0 then
+ * refine_undetected_mask against the caller's boxes, which modifies the mask in place as the reference does.  With
+ * refined_input != 0 (needs keep_undetected and input_host) the frame's mask_refined is an input, refine_mask does not
+ * run, and refine_undetected_mask alone modifies both masks.  results_host (pinned, results_bytes): mask_refined, and
+ * with keep_undetected the modified mask.  No network runs: a handle of any program (a kernels-only one too) takes it.
+ * Refused before any GPU work: a block of status != 0 unless refined_input (CTD_E_INVALID, ctd_last_error names the
+ * page and the block), n > max_batch (CTD_E_CAPACITY), and with keep_undetected a page of more than 2^28 pixels
+ * (CTD_E_CAPACITY, as ctd_detect_page).  Both buffers and the device images stay untouched until the slot is
+ * collected.                                                                                                       */
+CTD_API int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, const int32_t* xyxy,
+                              const int32_t* n_blocks, const uint8_t* input_host, const ctd_device_page* dev_pages,
+                              const ctd_device_page* dev_masks, int32_t refine_mode, int32_t keep_undetected,
+                              int32_t refined_input, int32_t results_on_device, void* results_host);
+
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
  * [rows][5+nc]); output as ctd_get_detections for one page.                                */
 CTD_API int ctd_nms(ctd_handle* h, const float* pred, int32_t rows, float conf_thresh, float iou_thresh, float* det,
