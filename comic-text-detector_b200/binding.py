@@ -98,7 +98,7 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy", "ctd_jpeg_decode", "ctd_debug_postprocess",
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
            "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
-           "ctd_refine_plan", "ctd_submit_refine"]
+           "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions"]
 
 _lib = None
 
@@ -161,6 +161,7 @@ def load_library():
     lib.ctd_collect_device.argtypes = [vp, i32, vp]
     lib.ctd_refine_plan.argtypes = [vp, i32, vp, vp, vp, vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.ctd_submit_refine.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.ctd_submit_regions.argtypes = [vp, i32, vp, i32, vp, vp, i32, vp, vp, i32]
     lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
     lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.ctd_jpeg_decoder_destroy.argtypes = [vp]
@@ -673,6 +674,75 @@ class Engine:
             mo, ro = int(e["mask_off"]), int(e["refined_off"])
             out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy() if keep else None,
                         res[ro:ro + ih * iw].reshape(ih, iw).copy()))
+        return out
+
+    def submit_regions(self, slot, pages, lines, n_lines, textheight, events=None, device_results=False):
+        """asynchronous crops of caller lines (ctd_submit_regions): per page a u8 [h][w][3] numpy page (packed into this
+        slot's pinned input buffer) or a torch.uint8 CUDA tensor on this engine's GPU with any strides (read where it
+        is), lines = REGION_LINE_DTYPE records of every page's lines, page 0's first, n_lines[i] of page i.
+        events[i] (a recorded torch.cuda.Event, or None) is waited on before CUDA page i is read; the CUDA pages are
+        referenced until the slot is collected and must not be written before.  Collect with collect_crops(slot)."""
+        import torch
+        if not hasattr(self, "_pg_bufs"):
+            self._pg_bufs = [[None, None], [None, None]]
+            self._pg_inflight = [None, None]
+        if self._pg_inflight[slot] is not None:
+            raise CtdError("slot %d has an uncollected submission" % slot)
+        shapes = [tuple(p.shape[:2]) for p in pages]
+        entries, _win, _st, in_bytes, _rb = refine_plan(shapes, np.zeros((0, 4), np.int32), [0] * len(pages))
+        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
+        host = not all(on_dev)
+        need = in_bytes // 5 * 3 if host else 0   # the page plane of the layout
+        bufs = self._pg_bufs[slot]
+        if need and (bufs[0] is None or bufs[0].numel() < need):
+            bufs[0] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        if host:
+            inp = bufs[0].numpy()
+            for e, p, d in zip(entries, pages, on_dev):
+                if not d:
+                    o = int(e["page_off"])
+                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+        lines = np.ascontiguousarray(lines, REGION_LINE_DTYPE)
+        counts = np.ascontiguousarray(n_lines, np.int32)
+        dev = _device_images(pages, on_dev, events, 3)
+        self._ck(self.lib.ctd_submit_regions(self.h, slot, _ptr(entries), len(entries), _ptr(lines), _ptr(counts),
+                                             int(textheight), C.c_void_p(bufs[0].data_ptr()) if host else None,
+                                             None if dev is None else C.cast(dev, C.c_void_p), int(bool(device_results))))
+        kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]]
+        self._pg_inflight[slot] = ("regions", len(entries), bool(device_results), kept)
+
+    def collect_crops(self, slot, counts, discard=False):
+        """blocks until the batch of submit_regions(slot) is done -> per page, per block (counts[p]: the number of lines
+        of each block of page p) a list of u8 [h][w][3] crops in line order, None where the planner gives no crop.  Each
+        page's crops are views into one array of that page's own (collect_regions), or with device_results into one
+        CUDA allocation of its own (ctd_collect_device; complete on return, marked as used on the current stream); a
+        page without a crop allocates nothing.  discard: only wait for the batch and return None."""
+        inflight = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
+        if inflight is None or inflight[0] != "regions":
+            raise CtdError("slot %d has no submit_regions batch in flight" % slot)
+        _kind, n_pages, device_results, _kept = inflight
+        self._pg_inflight[slot] = None
+        self.collect(slot)
+        if discard:
+            return None
+        if not device_results:
+            return self.collect_regions(slot, counts)
+        import torch
+        dev = torch.device("cuda", self.device)
+        if getattr(self, "_alloc_stream", None) is None:
+            self._alloc_stream = torch.cuda.Stream(dev)
+        plan = self._collected_plan(slot, n_pages)
+        ranges = [plan.page_range(p) for p in range(n_pages)]
+        with torch.cuda.stream(self._alloc_stream):
+            bufs = [torch.empty((hi - lo,), dtype=torch.uint8, device=dev) if hi > lo else None for lo, hi in ranges]
+        ptrs = (C.c_void_p * n_pages)(*[None if b is None else b.data_ptr() for b in bufs])
+        self._ck(self.lib.ctd_collect_device(self.h, slot, ptrs))
+        cur = torch.cuda.current_stream(dev)
+        out = []
+        for p, buf in enumerate(bufs):
+            if buf is not None:
+                buf.record_stream(cur)
+            out.append(plan.page_crops(p, counts[p], lambda c, h, w, buf=buf: buf.as_strided((h, w, 3), (w * 3, 3, 1), c)))
         return out
 
     def _collect_device(self, slot, entries, blocks, n_lines):

@@ -109,6 +109,12 @@ struct PipeJob {
   bool refine = false;
   int refined_input = 0;
   std::vector<std::vector<int32_t>> wins, boxes;
+  // ctd_submit_regions: the crops alone, of the caller's lines (n_lines[i] of page i, in page order) at textheight;
+  // dev[i].data != NULL: page i is read where it is in device memory (else from d_img at its offset)
+  bool regions = false;
+  std::vector<ctd_region_line> lines;
+  std::vector<int32_t> n_lines;
+  std::vector<ctd_device_page> dev;
 };
 
 struct ctd_handle;
@@ -125,7 +131,8 @@ struct GrowBuf {
 using DevBuf = GrowBuf<false>;
 using PinnedBuf = GrowBuf<true>;
 
-// one of the two slots of the batch pipeline (ctd_submit_full, ctd_submit_pages, ctd_submit_refine): the staging and events of a batch
+// one of the two slots of the batch pipeline (ctd_submit_full, ctd_submit_pages, ctd_submit_refine, ctd_submit_regions):
+// the staging and events of a batch
 // in flight, its hand-over from the worker, and the buffers its results stay in until the next submission
 struct Slot {
   // ctd_submit_full staging: the pages, and the device copy of the result arena (ctd_device_arena)
@@ -135,8 +142,8 @@ struct Slot {
   cudaEvent_t ev_post_done = nullptr;   // phase C of the batch has run (post stream)
   bool busy = false;                    // submitted and not collected
   // what the batch asked for (start()), and whether it was collected without error: the results ctd_collect_regions
-  // and ctd_collect_device hand out
-  bool crops = false, on_device = false, collected = false;
+  // and ctd_collect_device hand out (masks: the batch has masks, false for ctd_submit_regions)
+  bool crops = false, on_device = false, masks = true, collected = false;
   // worker hand-over, under pipe_mu: 0 idle, 1 queued / running, 2 phase C enqueued, 3 failed
   int state = 0;
   int rc = 0;
@@ -161,9 +168,10 @@ struct Slot {
   size_t crop_px_off = 0, crop_bytes = 0;   // pixels at h_crop + crop_px_off, crop_bytes long
 
   // a submission starts on the slot: the results of its last batch are given up
-  void start(bool want_crops, bool want_on_device) {
+  void start(bool want_crops, bool want_on_device, bool want_masks = true) {
     crops = want_crops;
     on_device = want_on_device;
+    masks = want_masks;
     collected = false;
   }
   void release();   // frees the slot's buffers and events
@@ -185,9 +193,9 @@ struct RegionJob {
   std::vector<ctd::RegionDev> regs;
   std::vector<ctd::RegionTile> tiles;
   size_t out_bytes = 0;   // end of the last crop in the packed output
-  // the status-0 entries of plan[0..n), the crops of the ih x iw page at byte page_off, each written at out_base + its
-  // plan offset; returns the index of a malformed entry, or -1
-  int add(const ctd_region* plan, int n, long long page_off, int ih, int iw, long long out_base);
+  // the status-0 entries of plan[0..n), the crops of page `pg`, each written at out_base + its plan offset; returns the
+  // index of a malformed entry, or -1
+  int add(const ctd_region* plan, int n, const ctd::RegionPage& pg, long long out_base);
   size_t table_bytes() const;   // RegionDev[] | RegionTile[], each 256-aligned
   void write_tables(char* dst) const;
 };

@@ -289,18 +289,26 @@ cudaError_t refine_mk_launch(const uint8_t* d_img, const uint8_t* d_mask, const 
 
 // ---- text-line crops (region.cu) ----
 constexpr int kRegionTilePx = 256;   // output pixels per CTA of k_warp_regions = threads per CTA
+// the u8 BGR page a crop reads, in device memory: byte (y, x, c) at data + y * sh + x * sw + c * sc, so a page is read
+// where it is (a packed page: sh = iw * 3, sw = 3, sc = 1; a caller's tensor: any strides >= 0)
+struct RegionPage {
+  const uint8_t* data;
+  long long sh, sw, sc;
+  int ih, iw;
+};
 // one crop of a k_warp_regions launch: where its page and its output are, its shape and the inverse homography
 struct RegionDev {
   long long offset;        // byte offset of the crop in the packed output
-  long long page_off;      // byte offset of the crop's page (u8 BGR [ih][iw][3]) in the pages buffer
+  const uint8_t* page;     // the crop's page (RegionPage::data) and its byte strides
+  long long sh, sw, sc;
   int out_h, out_w;        // returned shape
   int warp_w, bw0;         // width of the warped (un-rotated) image, OpenCV's block width
   int rotate, ih, iw, pad;
   double m[9];             // inverse homography (destination -> page)
 };
 struct RegionTile { int region, first; };   // kRegionTilePx consecutive output pixels of one crop
-// one CTA per tile; d_pages holds every crop's page at its page_off
-cudaError_t warp_regions_launch(const uint8_t* d_pages, const RegionDev* d_regs, const RegionTile* d_tiles, int n_tiles,
-                                uint8_t* d_out, cudaStream_t s);
+// one CTA per tile; each crop reads its own page through RegionDev::page and its strides
+cudaError_t warp_regions_launch(const RegionDev* d_regs, const RegionTile* d_tiles, int n_tiles, uint8_t* d_out,
+                                cudaStream_t s);
 
 }  // namespace ctd

@@ -15,7 +15,8 @@
 // every text line of every page of the batch out of the resident pages in one k_warp_regions launch (region.cu).  Its
 // pages may already be in device memory (any strides; one gather_pages_kernel launch packs them, gather.cu) and the
 // masks and crops may stay there (ctd_collect_device).  ctd_submit_refine runs phase C alone on caller pages, masks
-// and block boxes (textmask.refine_mask / refine_undetected_mask, MaskRefiner) through the same two-slot schedule.
+// and block boxes (textmask.refine_mask / refine_undetected_mask, MaskRefiner) through the same two-slot schedule, and
+// ctd_submit_regions the crop stage alone on caller pages and text lines (regions.RegionCropper).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -524,6 +525,70 @@ static int finish_batch(ctd_handle* h, const PipeJob& job, cudaStream_t st) {
   return CTD_OK;
 }
 
+// the pages of a batch as its crops read them: a page in device memory where it is (job.dev, ctd_submit_regions),
+// every other page in the batch's packed page buffer
+static std::vector<RegionPage> region_pages(const PipeJob& job) {
+  std::vector<RegionPage> src;
+  for (size_t i = 0; i < job.pages.size(); ++i) {
+    const JobPage& p = job.pages[i];
+    if (i < job.dev.size() && job.dev[i].data) {
+      const ctd_device_page& d = job.dev[i];
+      src.push_back(RegionPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c, p.ih, p.iw});
+    } else {
+      src.push_back(RegionPage{job.d_img + p.off * 3, (long long)p.iw * 3, 3, 1, p.ih, p.iw});
+    }
+  }
+  return src;
+}
+
+// the crop stage of a batch, on the worker's stream `st`: the pages' plans (plans[i], plan_bytes[i] packed bytes each)
+// concatenated with each page's crops after the previous page's into the slot's crop plan, the tables staged in the
+// slot's pinned crop buffer, one k_warp_regions launch over every page where it is (src[i]), and the pixels back into
+// the same pinned buffer after the tables (to_host), else left after the tables in d_crop.  A batch without a crop
+// launches and allocates nothing.
+static int crop_stage(ctd_handle* h, Slot& s, const std::vector<RegionPage>& src,
+                      const std::vector<std::vector<ctd_region>>& plans, const std::vector<size_t>& plan_bytes,
+                      bool to_host, cudaStream_t st) {
+  const int n = int(src.size());
+  RegionJob rg;
+  s.crop_plan.clear();
+  s.crop_first.assign(size_t(n) + 1, 0);
+  s.crop_base.assign(size_t(n) + 1, 0);
+  size_t base = 0;
+  for (int i = 0; i < n; ++i) {
+    const std::vector<ctd_region>& p = plans[size_t(i)];
+    if (int bad = rg.add(p.data(), int(p.size()), src[size_t(i)], (long long)base); bad >= 0)
+      return ctd_fail(h, CTD_E_INVALID, "malformed crop plan entry %d on page %d of the batch", bad, i);
+    s.crop_first[size_t(i)] = int32_t(s.crop_plan.size());
+    s.crop_base[size_t(i)] = base;
+    for (ctd_region r : p) {
+      r.offset += int64_t(base);
+      s.crop_plan.push_back(r);
+    }
+    base += plan_bytes[size_t(i)];
+  }
+  s.crop_first[size_t(n)] = int32_t(s.crop_plan.size());
+  s.crop_base[size_t(n)] = base;
+  if (s.crop_plan.size() > size_t(INT32_MAX) || rg.tiles.size() > size_t(INT32_MAX))
+    return ctd_fail(h, CTD_E_CAPACITY, "too many crops in one batch");
+  s.crop_bytes = base;
+  s.crop_px_off = 0;
+  if (rg.tiles.empty()) return CTD_OK;
+  // both buffers grow only after `st` is idle, since an earlier failed job of this slot may have left copies on it
+  const size_t tb = rg.table_bytes(), px = s.crop_bytes;
+  if (int rc = s.d_crop.grow(h, tb + px, st)) return rc;
+  if (int rc = s.h_crop.grow(h, to_host ? tb + px : tb, st)) return rc;
+  uint8_t* d_tab = s.d_crop.p;
+  rg.write_tables(reinterpret_cast<char*>(s.h_crop.p));
+  CK(cudaMemcpyAsync(d_tab, s.h_crop.p, tb, cudaMemcpyHostToDevice, st));
+  const size_t rb = (rg.regs.size() * sizeof(RegionDev) + 255) / 256 * 256;
+  CK(warp_regions_launch(reinterpret_cast<const RegionDev*>(d_tab), reinterpret_cast<const RegionTile*>(d_tab + rb),
+                         int(rg.tiles.size()), d_tab + tb, st));
+  if (to_host) CK(cudaMemcpyAsync(s.h_crop.p + tb, d_tab + tb, px, cudaMemcpyDeviceToHost, st));
+  s.crop_px_off = tb;
+  return CTD_OK;
+}
+
 // phases B and C of a submitted batch, on the worker thread
 static int run_batch(ctd_handle* h, const PipeJob& job) {
   Slot& s = h->slot[job.slot];
@@ -552,33 +617,6 @@ static int run_batch(ctd_handle* h, const PipeJob& job) {
     if (crc[size_t(i)] != CTD_OK)
       return ctd_fail(h, crc[size_t(i)], "ctd_region_plan refused page %d of the batch (%dx%d, textheight %d)", i,
                       job.pages[size_t(i)].ih, job.pages[size_t(i)].iw, job.textheight);
-  // the batch's plans, concatenated with each page's crops after the previous page's; one warp job for all pages
-  RegionJob rg;
-  if (crops) {
-    s.crop_plan.clear();
-    s.crop_first.assign(size_t(n) + 1, 0);
-    s.crop_base.assign(size_t(n) + 1, 0);
-    size_t base = 0;
-    for (int i = 0; i < n; ++i) {
-      const JobPage& pg = job.pages[size_t(i)];
-      const std::vector<ctd_region>& p = plans[size_t(i)];
-      if (int bad = rg.add(p.data(), int(p.size()), (long long)(pg.off * 3), pg.ih, pg.iw, (long long)base); bad >= 0)
-        return ctd_fail(h, CTD_E_INVALID, "malformed crop plan entry %d on page %d of the batch", bad, i);
-      s.crop_first[size_t(i)] = int32_t(s.crop_plan.size());
-      s.crop_base[size_t(i)] = base;
-      for (ctd_region r : p) {
-        r.offset += int64_t(base);
-        s.crop_plan.push_back(r);
-      }
-      base += plan_bytes[size_t(i)];
-    }
-    s.crop_first[size_t(n)] = int32_t(s.crop_plan.size());
-    s.crop_base[size_t(n)] = base;
-    if (s.crop_plan.size() > size_t(INT32_MAX) || rg.tiles.size() > size_t(INT32_MAX))
-      return ctd_fail(h, CTD_E_CAPACITY, "too many crops in one batch");
-    s.crop_bytes = base;
-    s.crop_px_off = 0;
-  }
   // phase C on the post stream over the slot's resident pages and masks
   cudaStream_t st = h->post;
   // enqueued here for ctd_submit_pages, not at submit: a wait enqueued at submit time would also hold this batch's
@@ -588,25 +626,8 @@ static int run_batch(ctd_handle* h, const PipeJob& job) {
   // ctd_submit_full: block sections to the device arena copy (one gather then moves everything)
   if (job.d_blocks)
     CK(cudaMemcpyAsync(job.d_blocks, job.pages[0].section, job.blocks_bytes, cudaMemcpyHostToDevice, st));
-  const bool to_host = !job.results_on_device;
-  if (!rg.tiles.empty()) {
-    // crops: tables staged in the slot's pinned crop buffer, one launch over the pages in place in the page buffer,
-    // the pixels back into the same pinned buffer after the tables (unless they stay on the device, after the tables
-    // in d_crop).  Both buffers grow only after `st` is idle, since an earlier failed job of this slot may have left
-    // copies on it.
-    const size_t tb = rg.table_bytes(), px = s.crop_bytes;
-    if (int rc = s.d_crop.grow(h, tb + px, st)) return rc;
-    if (int rc = s.h_crop.grow(h, to_host ? tb + px : tb, st)) return rc;
-    uint8_t* d_tab = s.d_crop.p;
-    rg.write_tables(reinterpret_cast<char*>(s.h_crop.p));
-    CK(cudaMemcpyAsync(d_tab, s.h_crop.p, tb, cudaMemcpyHostToDevice, st));
-    const size_t rb = (rg.regs.size() * sizeof(ctd::RegionDev) + 255) / 256 * 256;
-    CK(ctd::warp_regions_launch(job.d_img, reinterpret_cast<const ctd::RegionDev*>(d_tab),
-                                reinterpret_cast<const ctd::RegionTile*>(d_tab + rb), int(rg.tiles.size()), d_tab + tb,
-                                st));
-    if (to_host) CK(cudaMemcpyAsync(s.h_crop.p + tb, d_tab + tb, px, cudaMemcpyDeviceToHost, st));
-    s.crop_px_off = tb;
-  }
+  if (crops)
+    if (int rc = crop_stage(h, s, region_pages(job), plans, plan_bytes, !job.results_on_device, st)) return rc;
   CK(cudaMemsetAsync(job.d_ref, 0, job.total, st));
   const auto boxes = job.keep_undetected ? section_boxes(job.pages) : std::vector<std::vector<int32_t>>();
   if (int rc = phase_c(h, job.pages, wins, boxes, job_planes(job), job.refine_mode, job.keep_undetected, st,
@@ -635,6 +656,34 @@ static int run_refine_batch(ctd_handle* h, const PipeJob& job) {
   return finish_batch(h, job, st);
 }
 
+// ctd_submit_regions's batch on the worker: each page's lines planned on the host threads, then the crop stage
+static int run_regions_batch(ctd_handle* h, const PipeJob& job) {
+  Slot& s = h->slot[job.slot];
+  const int n = int(job.pages.size());
+  std::vector<size_t> first(size_t(n) + 1, 0);
+  for (int i = 0; i < n; ++i) first[size_t(i) + 1] = first[size_t(i)] + size_t(job.n_lines[size_t(i)]);
+  std::vector<std::vector<ctd_region>> plans(static_cast<size_t>(n));
+  std::vector<size_t> plan_bytes(size_t(n), 0);
+  std::vector<int> prc(size_t(n), CTD_OK);
+  for_each_page(n, h->host_threads, [&](int i) {
+    const JobPage& p = job.pages[size_t(i)];
+    const int nl = job.n_lines[size_t(i)];
+    plans[size_t(i)].resize(size_t(nl));
+    if (nl > 0)
+      prc[size_t(i)] = ctd_region_plan(job.lines.data() + first[size_t(i)], nl, p.iw, p.ih, job.textheight,
+                                       plans[size_t(i)].data(), &plan_bytes[size_t(i)]);
+  });
+  for (int i = 0; i < n; ++i)
+    if (prc[size_t(i)] != CTD_OK)
+      return ctd_fail(h, prc[size_t(i)], "ctd_region_plan refused page %d of the batch (%dx%d, textheight %d)", i,
+                      job.pages[size_t(i)].ih, job.pages[size_t(i)].iw, job.textheight);
+  cudaStream_t st = h->post;
+  CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // the host pages are in place, the device pages written
+  if (int rc = crop_stage(h, s, region_pages(job), plans, plan_bytes, !job.results_on_device, st)) return rc;
+  CK(cudaEventRecord(s.ev_post_done, st));
+  return CTD_OK;
+}
+
 // ---- batch pipeline -------------------------------------------------------------------------------------------------
 static void pipe_worker(ctd_handle* h) {
   cudaSetDevice(h->cfg.device);
@@ -647,7 +696,7 @@ static void pipe_worker(ctd_handle* h) {
       job = std::move(h->pipe_queue.front());
       h->pipe_queue.pop_front();
     }
-    const int rc = job.refine ? run_refine_batch(h, job) : run_batch(h, job);
+    const int rc = job.refine ? run_refine_batch(h, job) : job.regions ? run_regions_batch(h, job) : run_batch(h, job);
     std::string err;
     if (rc != CTD_OK) err = h->err;
     {
@@ -1094,6 +1143,81 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
   return CTD_OK;
 }
 
+extern "C" int ctd_submit_regions(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
+                                  const ctd_region_line* lines, const int32_t* n_lines, int32_t textheight,
+                                  const uint8_t* input_host, const ctd_device_page* dev_pages,
+                                  int32_t results_on_device) {
+  if (!h || !pages || !n_lines || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
+  Slot& s = h->slot[slot];
+  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
+  int64_t total_lines = 0;
+  for (int i = 0; i < n; ++i) {
+    if (n_lines[i] < 0) return ctd_fail(h, CTD_E_INVALID, "page %d: n_lines %d < 0", i, n_lines[i]);
+    total_lines += n_lines[i];
+  }
+  if (total_lines > INT32_MAX) return ctd_fail(h, CTD_E_CAPACITY, "more than 2^31 lines in one batch");
+  if (total_lines > 0 && !lines) return CTD_E_INVALID;
+  for (int i = 0; i < n; ++i) {
+    const int ih = pages[i].ih, iw = pages[i].iw;
+    if (ih < 1 || iw < 1 || ih >= 32767 || iw >= 32767)
+      return ctd_fail(h, CTD_E_SHAPE, "page %d (%dx%d): the crop planner takes pages with sides in [1, 32767)", i, ih, iw);
+  }
+  // the offsets decide where the copies write: they must be the ones ctd_refine_plan lays out (no blocks)
+  std::vector<ctd_page_entry> pg(pages, pages + n);
+  const std::vector<int32_t> no_blocks(static_cast<size_t>(n), 0);
+  size_t in_bytes = 0, res_bytes = 0;
+  if (int rc = ctd_refine_plan(pg.data(), n, nullptr, no_blocks.data(), nullptr, nullptr, &in_bytes, &res_bytes))
+    return ctd_fail(h, rc, "ctd_refine_plan refuses the pages");
+  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
+    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_refine_plan returns");
+  const size_t total = in_bytes / 5;
+  CK(cudaSetDevice(h->cfg.device));
+  int n_dev = 0;
+  for (int i = 0; i < n; ++i) {
+    if (dev_pages && dev_pages[i].data) {
+      if (int rc = check_device_image(h, "page", i, dev_pages[i], pg[size_t(i)].ih, pg[size_t(i)].iw, 3)) return rc;
+      ++n_dev;
+    } else if (!input_host) {
+      return ctd_fail(h, CTD_E_INVALID, "page %d is in neither input_host nor device memory", i);
+    }
+  }
+  if (int rc = ensure_full_pipeline(h)) return rc;
+  s.start(true, results_on_device != 0, false);
+  // grown while the slot is idle: its collect has synchronised the work of its last batch.  The host pages are
+  // copied into pg_in at their offsets; the device pages are read where they are
+  if (n_dev < n) {
+    if (int rc = s.pg_in.grow(h, 3 * total, std::nullopt)) return rc;
+    if (int rc = copy_host_runs(h, dev_pages, n, s.pg_in.p, input_host,
+                                [&](int i) { return size_t(pg[size_t(i)].page_off); },
+                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; },
+                                h->copy_in))
+      return rc;
+  }
+  CK(cudaEventRecord(s.ev_in_done, h->copy_in));
+  CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
+  if (dev_pages)
+    for (int i = 0; i < n; ++i)
+      if (dev_pages[i].data && dev_pages[i].event)
+        CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(dev_pages[i].event), 0));
+  CK(cudaEventRecord(s.ev_out_ready, h->stream));
+  PipeJob job;
+  job.regions = true;
+  job.slot = slot;
+  job.textheight = textheight;
+  job.results_on_device = results_on_device ? 1 : 0;
+  for (const ctd_page_entry& e : pg) job.pages.push_back(JobPage{e.ih, e.iw, 1.f, 1.f, size_t(e.page_off) / 3, nullptr});
+  job.total = total;
+  job.d_img = s.pg_in.p;
+  job.lines.assign(lines, lines + total_lines);
+  job.n_lines.assign(n_lines, n_lines + n);
+  if (dev_pages) job.dev.assign(dev_pages, dev_pages + n);
+  if (results_on_device) s.dev_pages = std::move(pg);
+  queue_job(h, std::move(job));
+  return CTD_OK;
+}
+
 extern "C" int ctd_collect(ctd_handle* h, int32_t slot) {
   if (!h || slot < 0 || slot > 1) return CTD_E_INVALID;
   Slot& s = h->slot[slot];
@@ -1122,8 +1246,13 @@ extern "C" int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page
   CK(cudaSetDevice(h->cfg.device));
   const std::vector<ctd_page_entry>& pg = s.dev_pages;
   const int n = int(pg.size());
+  // bytes page i receives: its two masks (none in a ctd_submit_regions batch), then its crops
+  auto page_bytes = [&](int i) {
+    const size_t m = s.masks ? 2 * size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) : 0;
+    return m + (s.crops ? s.crop_base[size_t(i) + 1] - s.crop_base[size_t(i)] : 0);
+  };
   for (int i = 0; i < n; ++i)
-    if (!page_dst[i] || !is_device_memory(page_dst[i], h->cfg.device))
+    if (page_bytes(i) > 0 && (!page_dst[i] || !is_device_memory(page_dst[i], h->cfg.device)))
       return ctd_fail(h, CTD_E_INVALID, "page_dst[%d] (%p) is not device memory of GPU %d", i, page_dst[i],
                       h->cfg.device);
   if (!h->dev_out) CK(cudaStreamCreateWithFlags(&h->dev_out, cudaStreamNonBlocking));
@@ -1132,10 +1261,12 @@ extern "C" int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page
   const uint8_t* d_px = s.crops ? s.d_crop.p + s.crop_px_off : nullptr;
   for (int i = 0; i < n; ++i) {
     const ctd_page_entry& e = pg[size_t(i)];
-    const size_t px = size_t(e.ih) * size_t(e.iw);
+    const size_t px = s.masks ? size_t(e.ih) * size_t(e.iw) : 0;
     uint8_t* dst = static_cast<uint8_t*>(page_dst[i]);
-    CK(cudaMemcpyAsync(dst, d_res + e.mask_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
-    CK(cudaMemcpyAsync(dst + px, d_res + e.refined_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
+    if (s.masks) {
+      CK(cudaMemcpyAsync(dst, d_res + e.mask_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
+      CK(cudaMemcpyAsync(dst + px, d_res + e.refined_off, px, cudaMemcpyDeviceToDevice, h->dev_out));
+    }
     if (s.crops) {
       const size_t b0 = s.crop_base[size_t(i)], b1 = s.crop_base[size_t(i) + 1];
       if (b1 > b0) CK(cudaMemcpyAsync(dst + 2 * px, d_px + b0, b1 - b0, cudaMemcpyDeviceToDevice, h->dev_out));
@@ -1150,7 +1281,8 @@ extern "C" int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region
   if (!h || slot < 0 || slot > 1 || !plan || !n_regions || !page_first || !pixels || !bytes) return CTD_E_INVALID;
   const Slot& s = h->slot[slot];
   if (s.busy || !s.collected || !s.crops)
-    return ctd_fail(h, CTD_E_INVALID, "slot %d holds no collected ctd_submit_pages batch with a textheight", slot);
+    return ctd_fail(h, CTD_E_INVALID,
+                    "slot %d holds no collected ctd_submit_pages batch with a textheight or ctd_submit_regions batch", slot);
   *plan = s.crop_plan.data();
   *n_regions = int32_t(s.crop_plan.size());
   *page_first = s.crop_first.data();

@@ -1,9 +1,10 @@
 // Text-line crops (C ABI `ctd_transform_regions`, include/ctd_b200.h): `cv2.warpPerspective(img, M, (w, h))` with
 // INTER_LINEAR / BORDER_CONSTANT 0, followed for vertical lines by `cv2.rotate(.., ROTATE_90_COUNTERCLOCKWISE)`, for
 // every line of a page in ONE launch (reference utils/textblock.py:162-194; the matrices come from ctd_region_plan,
-// csrc/region_plan.cpp).  The same kernel crops every line of every page of a ctd_submit_pages batch with a textheight
-// in one launch (pipeline.cu): each crop record carries its page's byte offset and size, so the pages are read in
-// place.
+// csrc/region_plan.cpp).  The same kernel crops every line of every page of a ctd_submit_pages batch with a textheight,
+// and of a ctd_submit_regions batch, in one launch (pipeline.cu): each crop record carries its page's device address,
+// byte strides and size, so the pages are read in place -- the batch's packed pages, or a caller's CUDA pages with any
+// strides, without a gather.
 //
 // Work split: the host (RegionJob) cuts every crop into tiles of kRegionTilePx consecutive output pixels (row-major in
 // the RETURNED array, i.e. after the rotation) and uploads a tile table {region, first pixel}; one CTA per tile, one
@@ -41,13 +42,12 @@ using ctd::kRegionTilePx;
 using ctd::RegionDev;
 using ctd::RegionTile;
 
-__global__ void __launch_bounds__(kRegionTilePx) k_warp_regions(const uint8_t* __restrict__ pages,
-                                                               const RegionDev* __restrict__ regs,
+__global__ void __launch_bounds__(kRegionTilePx) k_warp_regions(const RegionDev* __restrict__ regs,
                                                                const RegionTile* __restrict__ tiles,
                                                                uint8_t* __restrict__ out) {
   const RegionTile t = tiles[blockIdx.x];
   const RegionDev& r = regs[t.region];
-  const uint8_t* page = pages + r.page_off;
+  const uint8_t* page = r.page;
   const int ih = r.ih, iw = r.iw;
   const int p = t.first + int(threadIdx.x);
   const int ow = r.out_w;
@@ -81,16 +81,16 @@ __global__ void __launch_bounds__(kRegionTilePx) k_warp_regions(const uint8_t* _
   const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
   const bool in_x0 = unsigned(sx) < unsigned(iw), in_x1 = unsigned(sx + 1) < unsigned(iw);
   const bool in_y0 = unsigned(sy) < unsigned(ih), in_y1 = unsigned(sy + 1) < unsigned(ih);
-  const long long t00 = ((long long)sy * iw + sx) * 3;   // only dereferenced for taps inside the page
-  const uint8_t* row0 = page + t00;
-  const uint8_t* row1 = page + t00 + (long long)iw * 3;
+  const long long sw = r.sw, sc = r.sc;
+  const uint8_t* row0 = page + (long long)sy * r.sh + (long long)sx * sw;   // only dereferenced for taps inside the page
+  const uint8_t* row1 = row0 + r.sh;
   uint8_t* dst = out + r.offset + size_t(p) * 3;
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
-    const int v00 = in_y0 && in_x0 ? __ldg(row0 + k) : 0;
-    const int v01 = in_y0 && in_x1 ? __ldg(row0 + 3 + k) : 0;
-    const int v10 = in_y1 && in_x0 ? __ldg(row1 + k) : 0;
-    const int v11 = in_y1 && in_x1 ? __ldg(row1 + 3 + k) : 0;
+    const int v00 = in_y0 && in_x0 ? __ldg(row0 + k * sc) : 0;
+    const int v01 = in_y0 && in_x1 ? __ldg(row0 + sw + k * sc) : 0;
+    const int v10 = in_y1 && in_x0 ? __ldg(row1 + k * sc) : 0;
+    const int v11 = in_y1 && in_x1 ? __ldg(row1 + sw + k * sc) : 0;
     const int s = v00 * w00 + v01 * w01 + v10 * w10 + v11 * w11;
     dst[k] = uint8_t(min(255, max(0, (s + (1 << 14)) >> 15)));
   }
@@ -98,14 +98,14 @@ __global__ void __launch_bounds__(kRegionTilePx) k_warp_regions(const uint8_t* _
 
 }  // namespace
 
-cudaError_t ctd::warp_regions_launch(const uint8_t* d_pages, const RegionDev* d_regs, const RegionTile* d_tiles,
-                                     int n_tiles, uint8_t* d_out, cudaStream_t s) {
+cudaError_t ctd::warp_regions_launch(const RegionDev* d_regs, const RegionTile* d_tiles, int n_tiles, uint8_t* d_out,
+                                     cudaStream_t s) {
   if (n_tiles <= 0) return cudaSuccess;
-  k_warp_regions<<<unsigned(n_tiles), kRegionTilePx, 0, s>>>(d_pages, d_regs, d_tiles, d_out);
+  k_warp_regions<<<unsigned(n_tiles), kRegionTilePx, 0, s>>>(d_regs, d_tiles, d_out);
   return cudaGetLastError();
 }
 
-int RegionJob::add(const ctd_region* plan, int n, long long page_off, int ih, int iw, long long out_base) {
+int RegionJob::add(const ctd_region* plan, int n, const ctd::RegionPage& pg, long long out_base) {
   for (int i = 0; i < n; ++i) {
     const ctd_region& r = plan[i];
     if (r.status != 0) continue;
@@ -116,12 +116,15 @@ int RegionJob::add(const ctd_region* plan, int n, long long page_off, int ih, in
     out_bytes = std::max(out_bytes, size_t(out_base + r.offset) + px * 3);
     RegionDev d{};
     d.offset = out_base + r.offset;
-    d.page_off = page_off;
+    d.page = pg.data;
+    d.sh = pg.sh;
+    d.sw = pg.sw;
+    d.sc = pg.sc;
     d.out_h = r.out_h;
     d.out_w = r.out_w;
     d.rotate = r.rotate;
-    d.ih = ih;
-    d.iw = iw;
+    d.ih = pg.ih;
+    d.iw = pg.iw;
     const int ww = r.rotate ? r.out_h : r.out_w, wh = r.rotate ? r.out_w : r.out_h;
     d.warp_w = ww;
     const int bh0 = std::min(16, wh);   // OpenCV's block shape for a ww x wh destination
@@ -147,8 +150,9 @@ extern "C" int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t
                                      const ctd_region* plan, int32_t n, uint8_t* pixels_out, size_t pixels_bytes) {
   if (!h || !page || n < 0 || (n > 0 && !plan)) return CTD_E_INVALID;
   if (ih < 1 || iw < 1) return ctd_fail(h, CTD_E_SHAPE, "bad page size %dx%d", ih, iw);
+  // the page's address is known once the scratch has grown: set below
   RegionJob job;
-  if (int bad = job.add(plan, n, 0, ih, iw, 0); bad >= 0) {
+  if (int bad = job.add(plan, n, ctd::RegionPage{nullptr, (long long)iw * 3, 3, 1, ih, iw}, 0); bad >= 0) {
     const ctd_region& r = plan[bad];
     return ctd_fail(h, CTD_E_INVALID, "malformed plan entry %d (%dx%d at offset %lld)", bad, r.out_h, r.out_w,
                     (long long)r.offset);
@@ -165,17 +169,15 @@ extern "C" int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t
   const size_t pb = page_on_device ? 0 : al256(size_t(ih) * iw * 3);
   if (int rc = h->io_scratch.grow(h, tb + pb + total, h->stream)) return rc;
   char* base = reinterpret_cast<char*>(h->io_scratch.p);
+  const uint8_t* d_page = page_on_device ? page : reinterpret_cast<const uint8_t*>(base + tb);
+  for (RegionDev& d : job.regs) d.page = d_page;
   std::vector<char> stage(tb);
   job.write_tables(stage.data());
   CK(cudaMemcpyAsync(base, stage.data(), tb, cudaMemcpyHostToDevice, h->stream));
-  const uint8_t* d_page = page;
-  if (!page_on_device) {
-    CK(cudaMemcpyAsync(base + tb, page, size_t(ih) * iw * 3, cudaMemcpyHostToDevice, h->stream));
-    d_page = reinterpret_cast<const uint8_t*>(base + tb);
-  }
+  if (!page_on_device) CK(cudaMemcpyAsync(base + tb, page, size_t(ih) * iw * 3, cudaMemcpyHostToDevice, h->stream));
   uint8_t* d_out = reinterpret_cast<uint8_t*>(base + tb + pb);
-  CK(ctd::warp_regions_launch(d_page, reinterpret_cast<const RegionDev*>(base),
-                              reinterpret_cast<const RegionTile*>(base + rb), int(job.tiles.size()), d_out, h->stream));
+  CK(ctd::warp_regions_launch(reinterpret_cast<const RegionDev*>(base), reinterpret_cast<const RegionTile*>(base + rb),
+                              int(job.tiles.size()), d_out, h->stream));
   CK(cudaMemcpyAsync(pixels_out, d_out, total, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return CTD_OK;

@@ -160,21 +160,32 @@ def group_output(blks, lines, im_w, im_h, mask=None, sort_blklist=True):
     return blocks_from_records(rec[:n.value], lout, dout)
 
 
+_KERNELS_ONLY = None
 _REGION_ENGINE = None
 _REGION_LOCK = threading.Lock()
 
 
+def kernels_only_engine(device_index, max_batch):
+    """an engine on cuda:device_index that runs no network (the program has no ops, and a 64x64 workspace): the
+    stand-alone kernels and the batched jobs of caller blocks take it.  The program is built once per process."""
+    global _KERNELS_ONLY
+    if _KERNELS_ONLY is None:
+        from . import compiler
+        P = compiler.Program()
+        P.nc = 2
+        P.newbuf(8, 1)
+        _KERNELS_ONLY = P
+    return binding.Engine(_KERNELS_ONLY, device=device_index, max_batch=max_batch, max_h=64, max_w=64,
+                          skip_postproc=True)
+
+
 def _region_engine():
-    """the process-wide kernels-only engine behind TextBlock.get_transformed_region (no network ops, a 64x64
-    workspace), created on device 0 at first use; its handle is not thread-safe, so calls hold the returned lock"""
+    """the process-wide kernels-only engine behind TextBlock.get_transformed_region, created on device 0 at first use;
+    its handle is not thread-safe, so calls hold the returned lock"""
     global _REGION_ENGINE
     with _REGION_LOCK:
         if _REGION_ENGINE is None:
-            from . import compiler
-            P = compiler.Program()
-            P.nc = 2
-            P.newbuf(8, 1)
-            _REGION_ENGINE = binding.Engine(P, device=0, max_batch=1, max_h=64, max_w=64, skip_postproc=True)
+            _REGION_ENGINE = kernels_only_engine(0, 1)
     return _REGION_ENGINE, _REGION_LOCK
 
 

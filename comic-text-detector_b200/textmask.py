@@ -12,14 +12,13 @@ Only `blk.xyxy` of a block is read: the reference's `merge_mask_list` reads the 
 with the text lines, which `refine_mask` never asks for.
 """
 import operator
-from collections import deque
 
 import numpy as np
 
 from . import binding
-from .inference import REFINEMASK_INPAINT, _Encoded, _page_ready_event, _torch, check_page, decode_files
-from .jpeg import JpegDecoder, is_encoded, read_encoded
-from .png import PngDecoder
+from .inference import REFINEMASK_INPAINT, _Encoded, _page_ready_event, _torch
+from .jpeg import is_encoded
+from .kernel_jobs import KernelsOnlyJob, checked_page
 from .textblock import _region_engine
 
 
@@ -66,13 +65,6 @@ def check_mask(mask, shape, what="", device_index=None):
     return a
 
 
-def _check_page(img, what, device_index):
-    try:
-        return check_page(img, device_index)
-    except ValueError as ex:
-        raise ValueError("%s%s" % (what, ex)) from None
-
-
 def _one(img, pred_mask, blk_list, refine_mode, keep_undetected, refined):
     """one page through ctd_submit_refine on the process-wide kernels-only engine: (mask, mask_refined)"""
     img = np.asarray(img)
@@ -114,47 +106,16 @@ def refine_undetected_mask(img, mask_pred, mask_refined, blk_list, refine_mode=R
     return refined
 
 
-class MaskRefiner:
+class MaskRefiner(KernelsOnlyJob):
     """refine_mask (and refine_undetected_mask) for many pages on cuda:device_index, in batches of up to max_batch
     pages with two batches in flight, on a kernels-only engine of its own (no network)."""
-
-    def __init__(self, device_index=0, max_batch=16):
-        from . import compiler
-        P = compiler.Program()
-        P.nc = 2
-        P.newbuf(8, 1)
-        self.device_index = int(device_index)
-        self.max_batch = int(max_batch)
-        self.net = binding.Engine(P, device=self.device_index, max_batch=self.max_batch, max_h=64, max_w=64,
-                                  skip_postproc=True)
-        self._jpeg = None
-        self._png = None
-
-    def jpeg_decoder(self):
-        """the JpegDecoder encoded pages are decoded with (made on first use, closed with the refiner)"""
-        if self._jpeg is None:
-            self._jpeg = JpegDecoder(self.device_index)
-        return self._jpeg
-
-    def png_decoder(self):
-        """the PngDecoder PNG pages are decoded with (made on first use, closed with the refiner)"""
-        if self._png is None:
-            self._png = PngDecoder(self.device_index)
-        return self._png
-
-    def close(self):
-        self.net.close()
-        for d in (self._jpeg, self._png):
-            if d is not None:
-                d.close()
-        self._jpeg = self._png = None
 
     def refine_batch(self, items, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False, device_results=False):
         """list(refine_stream(...)), with every item checked before any GPU work"""
         items = list(items)
         for i, (img, mask, blk_list) in enumerate(items):
             if not is_encoded(img):
-                page = _check_page(img, "item %d: " % i, self.device_index)
+                page = checked_page(img, "item %d: " % i, self.device_index)
                 check_mask(mask, tuple(page.shape[:2]), "item %d: " % i, self.device_index)
                 check_blocks(tuple(page.shape[:2]), block_boxes(blk_list), "item %d: " % i)
         return list(self.refine_stream(items, refine_mode, keep_undetected_mask, device_results))
@@ -179,68 +140,32 @@ class MaskRefiner:
         return self._stream(items, refine_mode, bool(keep_undetected_mask), bool(device_results))
 
     def _stream(self, items, refine_mode, keep, device_results):
-        inflight = deque()   # (slot, the caller's masks) in submission order
-        free = [0, 1]
-
-        def submit(batch):
-            batch = self._decode_batch(batch)
-            if not free:
-                yield from collect()
-            slot = free.pop(0)
-            self.net.submit_refine(slot, [b[1] for b in batch], [b[2] for b in batch], [b[3] for b in batch],
-                                   refine_mode, keep, None, [b[4] for b in batch], device_results)
-            inflight.append((slot, [b[2] for b in batch]))
-
-        def collect():
-            slot, masks = inflight.popleft()
-            res = self.net.collect_refine(slot)
-            free.append(slot)
-            for m, (mask, refined) in zip(masks, res):
-                yield (mask if keep else m), refined
-
-        try:
-            batch = []
+        def records():
             for idx, (img, mask, blk_list) in enumerate(items):
                 what = "item %d: " % idx
                 boxes = block_boxes(blk_list)
                 if is_encoded(img):
                     page = _Encoded(idx, img)   # decoded, and its mask and blocks checked, with its batch
                 else:
-                    page = _check_page(img, what, self.device_index)
+                    page = checked_page(img, what, self.device_index)
                     mask = check_mask(mask, tuple(page.shape[:2]), what, self.device_index)
                     check_blocks(tuple(page.shape[:2]), boxes, what)
                 cuda = page if getattr(page, "is_cuda", False) else mask if getattr(mask, "is_cuda", False) else None
-                batch.append((idx, page, mask, boxes, _page_ready_event(cuda)))
-                if len(batch) == self.max_batch:
-                    yield from submit(batch)
-                    batch = []
-            if batch:
-                yield from submit(batch)
-            while inflight:
-                yield from collect()
-        finally:
-            while inflight:   # an error or an abandoned generator: leave the engine with no batch in flight
-                try:
-                    self.net.collect_refine(inflight.popleft()[0], discard=True)
-                except Exception:
-                    pass
+                yield (idx, page, mask, boxes, _page_ready_event(cuda))
 
-    def _decode_batch(self, batch):
-        """the batch with its encoded pages decoded (decode_files) and their masks and blocks checked"""
-        enc = [i for i, b in enumerate(batch) if isinstance(b[1], _Encoded)]
-        if not enc:
-            return batch
-        bufs = [read_encoded(batch[i][1].src) for i in enc]
-        pages = decode_files([b for b, _path in bufs], self.png_decoder, self.jpeg_decoder)
-        batch = list(batch)
-        for i, (_b, path), page in zip(enc, bufs, pages):
-            idx, _e, mask, boxes, ev = batch[i]
-            if page is None:
-                raise ValueError("item %d%s could not be decoded (cv2.imdecode returns None)"
-                                 % (idx, "" if path is None else " (%s)" % path))
-            what = "item %d: " % idx
-            page = page if getattr(page, "is_cuda", False) else _check_page(page, what, self.device_index)
+        def decoded(rec, page, what):
+            idx, _e, mask, boxes, ev = rec
             mask = check_mask(mask, tuple(page.shape[:2]), what, self.device_index)
             check_blocks(tuple(page.shape[:2]), boxes, what)
-            batch[i] = (idx, page, mask, boxes, ev)   # a page decoded on the GPU is complete when decode returns
-        return batch
+            return (idx, page, mask, boxes, ev)
+
+        def submit(slot, batch):
+            self.net.submit_refine(slot, [b[1] for b in batch], [b[2] for b in batch], [b[3] for b in batch],
+                                   refine_mode, keep, None, [b[4] for b in batch], device_results)
+            return [b[2] for b in batch]   # the caller's masks
+
+        def collect(slot, masks, discard):
+            res = self.net.collect_refine(slot, discard=discard)
+            return None if discard else [((mask if keep else m), refined) for m, (mask, refined) in zip(masks, res)]
+
+        return self._pipeline(records(), lambda batch: self._decode(batch, decoded), submit, collect)

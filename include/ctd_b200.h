@@ -424,8 +424,9 @@ CTD_API int ctd_transform_regions(ctd_handle* h, const uint8_t* page, int32_t ih
  * section), page i's entries at [(*page_first)[i], (*page_first)[i + 1]) (n + 1 values), and the packed crops,
  * *bytes bytes at *pixels (HOST, NULL when *bytes is 0).  Each entry's offset is relative to *pixels; page i's crops
  * follow page i - 1's.  Entries with status != 0 have no bytes, exactly as ctd_region_plan gives them.  All pointers
- * belong to the handle and stay valid until the slot's next submission or ctd_destroy.  CTD_E_INVALID for a slot that
- * is in flight or whose last collected batch did not ask for crops.                                            */
+ * belong to the handle and stay valid until the slot's next submission or ctd_destroy.  The same after a
+ * ctd_submit_regions batch.  CTD_E_INVALID for a slot that is in flight or whose last collected batch did not ask for
+ * crops.                                                                                                         */
 CTD_API int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region** plan, int32_t* n_regions,
                                 const int32_t** page_first, const uint8_t** pixels, size_t* bytes);
 
@@ -463,7 +464,8 @@ CTD_API int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* 
 /* After ctd_collect(h, slot) of a results_on_device batch: copies into page_dst[i] (a DEVICE buffer on the handle's
  * GPU, one per page of the batch) page i's [mask ih*iw | mask_refined ih*iw | the page's crops, packed as the plan
  * lays them out, offsets relative to the page's first plan entry].  The mask is the one refine_undetected_mask
- * modified when the batch asked for it.  Blocks until the copies are done, so the buffers may then be used on any
+ * modified when the batch asked for it.  After a ctd_submit_regions batch page_dst[i] gets only page i's crops, and
+ * may be NULL when the page has none.  Blocks until the copies are done, so the buffers may then be used on any
  * stream.  CTD_E_INVALID for a slot in flight or whose last batch was not submitted with results_on_device.       */
 CTD_API int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page_dst);
 
@@ -507,6 +509,28 @@ CTD_API int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_entry*
                               const int32_t* n_blocks, const uint8_t* input_host, const ctd_device_page* dev_pages,
                               const ctd_device_page* dev_masks, int32_t refine_mode, int32_t keep_undetected,
                               int32_t refined_input, int32_t results_on_device, void* results_host);
+
+/* ---- text-line crops of any block list ---------------------------------------------------------------------------
+ * ctd_submit_regions cuts the OCR crops of lines the caller gives (a block list edited after detection, or read back
+ * from `model2annotations`'s json) through the schedule of ctd_submit_pages (slots 0 and 1, two batches in flight).
+ *   pages / n:  the planned entries of ctd_refine_plan for these pages with no blocks (checked against a fresh plan);
+ *               any page of at least 1 x 1 with both sides < 32767 (else CTD_E_SHAPE naming the page).
+ *   lines:      ctd_region_line records of every line of every block of every page, page 0's first, n_lines[i] of
+ *               page i (block then line order within a page, as each page's plan entries are given back).
+ *   pages in:   page i from input_host at its page_off (pinned, the first 3 / 5 of ctd_refine_plan's input_bytes), or
+ *               from device memory (dev_pages, NULL or n entries as ctd_submit_pages takes them, checked the same way;
+ *               the engine waits on each page's event).  A device page is read where it is, with its strides.
+ * The handle's worker plans each page's lines with ctd_region_plan on its host threads, then one k_warp_regions launch
+ * cuts every status-0 crop of the batch.  Collect with ctd_collect, then ctd_collect_regions (the plan, page_first and,
+ * unless results_on_device, the host pixels) or, with results_on_device, ctd_collect_device, which gives page_dst[i]
+ * only page i's packed crops (a page without crop bytes may have a NULL page_dst[i]).  Status 1 and 2 lines get no
+ * bytes, exactly as ctd_region_plan gives them.  No network runs: a handle of any program takes it.
+ * Refused before any GPU work: textheight < 2 (CTD_E_INVALID), n > max_batch (CTD_E_CAPACITY), a page side < 1 or
+ * >= 32767 (CTD_E_SHAPE), and a device page that is not memory of the handle's GPU (CTD_E_INVALID).  input_host and
+ * the device pages must stay untouched until the slot is collected.                                               */
+CTD_API int ctd_submit_regions(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
+                               const ctd_region_line* lines, const int32_t* n_lines, int32_t textheight,
+                               const uint8_t* input_host, const ctd_device_page* dev_pages, int32_t results_on_device);
 
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
  * [rows][5+nc]); output as ctd_get_detections for one page.                                */
