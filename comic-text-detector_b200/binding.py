@@ -98,7 +98,7 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy", "ctd_jpeg_decode", "ctd_debug_postprocess",
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
            "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
-           "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions"]
+           "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot"]
 
 _lib = None
 
@@ -162,6 +162,7 @@ def load_library():
     lib.ctd_refine_plan.argtypes = [vp, i32, vp, vp, vp, vp, C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]
     lib.ctd_submit_refine.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_submit_regions.argtypes = [vp, i32, vp, i32, vp, vp, i32, vp, vp, i32]
+    lib.ctd_debug_read_slot.argtypes = [vp, i32, i32, C.c_size_t, vp, C.c_size_t]
     lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
     lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.ctd_jpeg_decoder_destroy.argtypes = [vp]
@@ -824,6 +825,13 @@ class Engine:
             pages = np.ascontiguousarray(pages, dtype=np.uint8)
         self._ck(self.lib.ctd_debug_run_ops(self.h, _ptr(pages), n, h, w, first, last))
         self.shape = (n, h, w)
+
+    def debug_read_slot(self, slot, plane, offset, nbytes):
+        """u8 [nbytes] at byte `offset` of a collected slot's device plane (ctd_debug_read_slot): 0 the packed pages,
+        1 the results frame, 2 the net input of the last forward"""
+        out = np.empty((nbytes,), np.uint8)
+        self._ck(self.lib.ctd_debug_read_slot(self.h, slot, plane, offset, _ptr(out), nbytes))
+        return out
 
     def debug_postprocess(self, blks, lines):
         """the forward's NMS and DB post-processing on given network outputs (ctd_debug_postprocess): blks f32

@@ -1276,6 +1276,26 @@ extern "C" int ctd_collect_device(ctd_handle* h, int32_t slot, void* const* page
   return CTD_OK;
 }
 
+extern "C" int ctd_debug_read_slot(ctd_handle* h, int32_t slot, int32_t plane, size_t offset, uint8_t* out,
+                                   size_t bytes) {
+  if (!h || slot < 0 || slot > 1 || plane < 0 || plane > 2 || !out) return CTD_E_INVALID;
+  const Slot& s = h->slot[slot];
+  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  const uint8_t* base = plane == 0 ? s.pg_in.p : plane == 1 ? s.pg_res.p : h->d_pages;
+  const size_t size = plane == 0   ? s.pg_in.cap
+                      : plane == 1 ? s.pg_res.cap
+                      : h->have_forward ? size_t(h->n) * h->ph * h->pw * 3 : 0;
+  if (offset > size || bytes > size - offset)
+    return ctd_fail(h, CTD_E_INVALID, "plane %d holds %zu bytes: [%zu, +%zu) is past its end", plane, size, offset,
+                    bytes);
+  if (bytes == 0) return CTD_OK;
+  CK(cudaSetDevice(h->cfg.device));
+  // after the engine stream's work: the gather, the letterbox and the forward that reads d_pages run there
+  CK(cudaMemcpyAsync(out, base + offset, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return CTD_OK;
+}
+
 extern "C" int ctd_collect_regions(ctd_handle* h, int32_t slot, const ctd_region** plan, int32_t* n_regions,
                                    const int32_t** page_first, const uint8_t** pixels, size_t* bytes) {
   if (!h || slot < 0 || slot > 1 || !plan || !n_regions || !page_first || !pixels || !bytes) return CTD_E_INVALID;

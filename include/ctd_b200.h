@@ -223,6 +223,12 @@ CTD_API int ctd_debug_run_ops(ctd_handle* h, const uint8_t* pages, int32_t n, in
  * results.  Refused (CTD_E_INVALID) on a debug_skip_postproc engine.                                      */
 CTD_API int ctd_debug_postprocess(ctd_handle* h, const float* blks, const float* lines, int32_t n, int32_t ph, int32_t pw);
 
+/* Test hook: copies `bytes` bytes at `offset` of one of a collected slot's device buffers to host memory `out`,
+ * synchronously.  plane 0: the packed pages (pg_in); 1: the results frame (pg_res: masks | mask_refined);
+ * 2: the engine's net input of its last forward (d_pages, n x net_h x net_w x 3).  CTD_E_INVALID while the slot
+ * has an uncollected submission, or for a range past the buffer's current size. */
+CTD_API int ctd_debug_read_slot(ctd_handle* h, int32_t slot, int32_t plane, size_t offset, uint8_t* out, size_t bytes);
+
 /* ---- measurement / interop ------------------------------------------------------------------
  * CUDA-event timer on the ENGINE stream (bench.py times K forwards between start and stop).    */
 CTD_API int ctd_timer_start(ctd_handle* h);
