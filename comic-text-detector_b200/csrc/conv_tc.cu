@@ -204,13 +204,15 @@ __global__ void __launch_bounds__(kThreads, 1) conv_tc_kernel(const __grid_const
   for (int i = threadIdx.x; i < g.cout_pad && i < Cfg::kBiasFloats; i += kThreads) bias_s[i] = p.bias ? p.bias[i] : 0.f;
   __syncthreads();
 
-  // tile index -> (phase, spatial tile, n block); n block varies fastest so that CTAs running
-  // concurrently share the A tile in L2
+  // tile index -> (spatial tile, phase, n block); n block varies fastest, then the DECONV4 phase, so that the CTAs
+  // running concurrently share the A tile in L2.  The 4 phases of a deconvolution read the same input pixels, and
+  // the four largest DECONV4 inputs of the benchmark (67-268 MB at 16 pages of 1024^2) exceed the 50 MB L2: with the
+  // phase outermost, each phase's pass would read the whole input from HBM again.
   auto decode = [&](int t, int& phase, int& nblk, int& img, int& y0, int& x0) {
     nblk = t % n_nblk;
     const int r = t / n_nblk;
-    const int sp = r % spatial_tiles;
-    phase = r / spatial_tiles;
+    phase = r % g.n_phase;
+    const int sp = r / g.n_phase;
     img = sp / tiles_per_img;
     const int trem = sp - img * tiles_per_img;
     const int ty = trem / p.tiles_x;
