@@ -10,3 +10,4 @@ from .jpeg import JpegDecoder, jpeg_probe  # noqa: F401
 from .png import PngDecoder, PngEncoder, png_probe  # noqa: F401
 from .textmask import MaskRefiner, refine_mask, refine_undetected_mask  # noqa: F401
 from .regions import RegionCropper  # noqa: F401
+from .postprocess import PostProcessor  # noqa: F401

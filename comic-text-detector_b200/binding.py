@@ -87,6 +87,15 @@ class CtdDevicePage(C.Structure):
                 ("event", C.c_void_p)]
 
 
+class CtdNetOutput(C.Structure):
+    """ctypes mirror of `ctd_net_output` (include/ctd_b200.h)"""
+    _fields_ = [("blks", C.c_void_p), ("blks_stride_r", C.c_int64), ("blks_stride_c", C.c_int64),
+                ("mask", C.c_void_p), ("mask_stride_h", C.c_int64), ("mask_stride_w", C.c_int64),
+                ("lines", C.c_void_p), ("lines_stride_h", C.c_int64), ("lines_stride_w", C.c_int64),
+                ("rows", C.c_int32), ("blks_on_device", C.c_int32), ("mask_on_device", C.c_int32),
+                ("lines_on_device", C.c_int32), ("event", C.c_void_p)]
+
+
 EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_get_net_outputs", "ctd_get_mask_u8",
            "ctd_get_detections", "ctd_get_db_components", "ctd_last_forward_ms", "ctd_last_launch_count",
            "ctd_debug_read_buffer", "ctd_debug_write_buffer", "ctd_connected_components", "ctd_nms",
@@ -98,7 +107,7 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy", "ctd_jpeg_decode", "ctd_debug_postprocess",
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
            "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
-           "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot"]
+           "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot", "ctd_submit_outputs"]
 
 _lib = None
 
@@ -163,6 +172,7 @@ def load_library():
     lib.ctd_submit_refine.argtypes = [vp, i32, vp, i32, vp, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_submit_regions.argtypes = [vp, i32, vp, i32, vp, vp, i32, vp, vp, i32]
     lib.ctd_debug_read_slot.argtypes = [vp, i32, i32, C.c_size_t, vp, C.c_size_t]
+    lib.ctd_submit_outputs.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
     lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.ctd_jpeg_decoder_destroy.argtypes = [vp]
@@ -591,6 +601,74 @@ class Engine:
             crops = self.collect_regions(slot, n_lines)
             out = [o + (c,) for o, c in zip(out, crops)]
         return out
+
+    def submit_outputs(self, slot, pages, outs, net_h, net_w, refine_mode=0, keep_undetected=False, textheight=0,
+                       events=None, device_results=False):
+        """asynchronous post-processing of a batch of pages from the caller's network outputs (ctd_submit_outputs):
+        pages as submit_pages takes them; outs[i] = (blks [A][5 + nc], mask [net_h][net_w], lines [net_h][net_w])
+        of page i, each a float32 numpy array (copied into this slot's pinned output buffer) or a float32 CUDA tensor on
+        this engine's GPU with any strides (read where it is).  events[i] (a recorded torch.cuda.Event, or None) is
+        waited on before CUDA page i and CUDA outputs i are read; the CUDA pages and outputs are referenced until the
+        slot is collected and must not be written before.  Collect with collect_pages(slot)."""
+        import torch
+        if not hasattr(self, "_pg_bufs"):
+            self._pg_bufs = [[None, None], [None, None]]
+            self._pg_inflight = [None, None]
+        if self._pg_inflight[slot] is not None:
+            raise CtdError("slot %d has an uncollected submission" % slot)
+        entries, in_bytes, res_bytes = pages_plan([tuple(p.shape[:2]) for p in pages], net_h, net_w)
+        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
+        o_dev = [[isinstance(m, torch.Tensor) and m.is_cuda for m in o] for o in outs]
+        # the host maps, packed contiguous into the slot's pinned output buffer, 256-byte aligned each
+        offs, need = [], 0
+        for o, d in zip(outs, o_dev):
+            page = []
+            for m, md in zip(o, d):
+                page.append(None if md else need)
+                need += 0 if md else (m.size * 4 + 255) // 256 * 256
+            offs.append(page)
+        if not hasattr(self, "_out_bufs"):
+            self._out_bufs = [None, None]
+        bufs = self._pg_bufs[slot]
+        for k, n_bytes in ((0, 0 if all(on_dev) else in_bytes), (1, res_bytes)):
+            if n_bytes and (bufs[k] is None or bufs[k].numel() < n_bytes):
+                bufs[k] = torch.empty((n_bytes * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        if need and (self._out_bufs[slot] is None or self._out_bufs[slot].numel() < need):
+            self._out_bufs[slot] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        if not all(on_dev):
+            inp = bufs[0].numpy()
+            for e, p, d in zip(entries, pages, on_dev):
+                if not d:
+                    o = int(e["page_off"])
+                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+        rec = (CtdNetOutput * len(outs))()
+        obuf = self._out_bufs[slot].numpy() if need else None
+        base = self._out_bufs[slot].data_ptr() if need else 0
+        for i, (o, d, off) in enumerate(zip(outs, o_dev, offs)):
+            fields = []
+            for m, md, mo in zip(o, d, off):
+                if md:
+                    st = m.stride()
+                    fields.append((m.data_ptr(), st[0], st[1] if len(st) > 1 else 1, 1))
+                else:
+                    np.copyto(obuf[mo:mo + m.size * 4].view(np.float32).reshape(m.shape), m)
+                    fields.append((base + mo, m.shape[1] if m.ndim > 1 else 1, 1, 0))
+            (bp, bsr, bsc, bd), (mp, msh, msw, md_), (lp, lsh, lsw, ld) = fields
+            ev = events[i] if events is not None else None
+            rec[i] = CtdNetOutput(bp, bsr, bsc, mp, msh, msw, lp, lsh, lsw, int(o[0].shape[0]), bd, md_, ld,
+                                  ev.cuda_event if ev is not None else None)
+        dev = _device_images(pages, on_dev, events, 3)
+        self._ck(self.lib.ctd_submit_outputs(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
+                                             None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
+                                             None if dev is None else C.cast(dev, C.c_void_p),
+                                             C.cast(rec, C.c_void_p), int(refine_mode), int(bool(keep_undetected)),
+                                             int(textheight), int(bool(device_results)),
+                                             C.c_void_p(bufs[1].data_ptr())))
+        kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]] + \
+               [(m, None if events is None else events[i]) for i, o in enumerate(outs) for m, md in zip(o, o_dev[i])
+                if md]
+        self._pg_inflight[slot] = (entries, int(textheight), bool(device_results), kept)
+        self.shape = (len(entries), net_h, net_w)
 
     def submit_refine(self, slot, pages, masks, boxes, refine_mode=0, keep_undetected=False, refined=None,
                       events=None, device_results=False):

@@ -40,7 +40,7 @@ int ctd_fail(ctd_handle* h, int code, const char* fmt, ...) {
     if (_e != cudaSuccess) return ctd_fail(h, CTD_E_CUDA, "%s: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
-static int rows_per_image(int ph, int pw) { return 3 * ((ph / 8) * (pw / 8) + (ph / 16) * (pw / 16) + (ph / 32) * (pw / 32)); }
+int rows_per_image(int ph, int pw) { return 3 * ((ph / 8) * (pw / 8) + (ph / 16) * (pw / 16) + (ph / 32) * (pw / 32)); }
 // op kinds that are one implicit GEMM over packed weights (conv_tc_kernel or conv_simt_kernel)
 static bool is_gemm(int kind) { return kind == CTD_OP_CONV || kind == CTD_OP_DECONV4 || kind == CTD_OP_DETECT; }
 
@@ -451,7 +451,7 @@ static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, const Shap
 }
 
 // NMS of the Detect rows
-static int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
+int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
   CK(nms_launch(h->d_blks, n, rows_per_image(ph, pw), h->cfg.nc, h->cfg.conf_thresh, h->cfg.nms_thresh, h->nms, h->d_det,
                 h->d_det_count, s));
   *cnt += kNmsLaunches;
@@ -459,7 +459,7 @@ static int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int*
 }
 
 // DB post-processing: connected components of the bitmap, then the text-line boxes
-static int launch_db_post(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
+int launch_db_post(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
   CK(ccl_launch(h->d_bitmap, n, ph, pw, h->d_labels, h->d_ccl_scratch, h->d_nlabels, s));
   CK(segrep_launch(h->d_bitmap, h->d_lines, size_t(2) * ph * pw, h->d_ccl_scratch, n, ph, pw, 1000, 1.5f,
                    h->d_segrep_scratch, h->d_line_boxes, h->d_line_scores, h->d_line_count, s));
@@ -644,7 +644,7 @@ void Slot::release() {
   for (cudaEvent_t e : {ev_in_done, ev_in_free, ev_out_ready, ev_out_done, ev_post_done})
     if (e) cudaEventDestroy(e);
   if (pinned) cudaFreeHost(pinned);
-  pg_in.release(); pg_res.release(); pg_aux.release(); d_crop.release(); h_crop.release();
+  pg_in.release(); pg_res.release(); pg_aux.release(); out_in.release(); d_crop.release(); h_crop.release();
   cudaFree(d_pg_tab);
   if (h_pg_tab) cudaFreeHost(h_pg_tab);
   *this = Slot();

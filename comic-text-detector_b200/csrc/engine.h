@@ -115,6 +115,9 @@ struct PipeJob {
   std::vector<ctd_region_line> lines;
   std::vector<int32_t> n_lines;
   std::vector<ctd_device_page> dev;
+  // ctd_submit_outputs: per page the ingest's non-finite bits (bit 0 blks, 1 mask, 2 lines; host copy, pinned),
+  // complete with phase A's results; a set bit fails the batch before phase B
+  const int32_t* nonfinite = nullptr;
 };
 
 struct ctd_handle;
@@ -154,6 +157,7 @@ struct Slot {
   // tables (pinned + device: max_batch PageGeom entries, then at pg_gather_off 2 * max_batch GatherPage entries for
   // the pages and masks gathered from device memory, uploaded together)
   DevBuf pg_in, pg_res, pg_aux;
+  DevBuf out_in;   // ctd_submit_outputs: the batch's network outputs that came from host memory
   ctd::PageGeom* h_pg_tab = nullptr;
   ctd::PageGeom* d_pg_tab = nullptr;
   std::vector<ctd_page_entry> dev_pages;   // the page entries of a results_on_device batch (ctd_collect_device)
@@ -277,6 +281,7 @@ struct ctd_handle {
   bool pipe_quit = false;
   int host_threads = 4;
   size_t pg_gather_off = 0;
+  size_t pg_out_off = 0, pg_flag_off = 0;   // the OutputGather table and the non-finite flags in the page tables
   cudaStream_t dev_out = nullptr;   // the stream ctd_collect_device copies on
   // the worker's phase C on the post stream: its own connected-components and refine scratch (refine_scratch and
   // cc_scratch belong to the caller's stream)
@@ -292,6 +297,12 @@ struct ctd_handle {
 int ctd_fail(ctd_handle* h, int code, const char* fmt, ...);
 int prepare_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan** out, int input = INPUT_U8);
 int enqueue_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan& sp);
+// Detect rows per page of a ph x pw net input (yolo.py:44), the rows of d_blks per page
+int rows_per_image(int ph, int pw);
+// the forward's post-processing on the engine workspaces, n pages of ph x pw, on stream s (cnt += the launches):
+// NMS of d_blks into the arena's detections, and connected components + text-line boxes of d_bitmap / d_lines
+int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt);
+int launch_db_post(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt);
 // connected components + stats of a DEVICE u8 image on the engine stream (grow-on-demand scratch): *d_stats points at
 // [stats_cap][5] ints on the device, *n_labels is read back (synchronises the stream)
 int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap, int32_t** d_stats, int32_t* n_labels);

@@ -4,6 +4,8 @@
 // refine_mask and the crop kernels read it; in the same launch, the batch's masks in device memory (u8 [ih][iw], any
 // strides: a channel of a page) into its packed mask plane.  One CTA per row over the stacked rows of the gathered
 // images, as backproject_batch_kernel.
+// gather_outputs_kernel is the ingest of ctd_submit_outputs: a caller's network outputs (float32, any strides) staged
+// into the engine's post-processing workspace in one launch, with postprocess_mask's u8 cast and the DB threshold fused.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -70,7 +72,103 @@ __global__ void __launch_bounds__(256) gather_pages_kernel(const GatherPage* __r
   }
 }
 
+constexpr int kOutThreads = 256;
+constexpr int kBlkPerThread = 8;   // blks elements per thread of a blks CTA
+
+__device__ __forceinline__ bool finite_f(float v) { return (__float_as_uint(v) & 0x7f800000u) != 0x7f800000u; }
+
+// postprocess_mask's `(p * 255).astype(np.uint8)` on float32 p: the product rounded to float32, truncated to int32
+// (0x80000000 where it does not fit, as cvttss2si gives it), and the low byte of that
+__device__ __forceinline__ uint32_t mask_byte(float p) {
+  const float v = __fmul_rn(p, 255.f);
+  return (v >= -2147483648.f && v < 2147483648.f) ? uint32_t(__float2int_rz(v)) & 0xffu : 0u;
+}
+
+// grid (h + blks CTAs per page, n).  CTA x < h: row x of the page's mask and lines channel 0 (16-byte loads when the
+// row is contiguous and 16-byte aligned, else one strided element per thread); the others: kBlkPerThread * 256 blks
+// elements each, in row-major order of the workspace rows
+__global__ void __launch_bounds__(kOutThreads) gather_outputs_kernel(const OutputGather* __restrict__ tab, int h, int w,
+                                                                     int no, int ws_rows, float thresh,
+                                                                     uint8_t* __restrict__ mask_u8,
+                                                                     float* __restrict__ lines,
+                                                                     uint8_t* __restrict__ bitmap,
+                                                                     float* __restrict__ blks,
+                                                                     int32_t* __restrict__ flags) {
+  const int page = blockIdx.y;
+  const OutputGather g = tab[page];
+  uint32_t bad = 0;
+  if (int(blockIdx.x) < h) {
+    const int y = blockIdx.x;
+    const size_t o = (size_t(page) * h + y) * w;
+    const float* ms = g.mask + y * g.msh;
+    const float* ls = g.lines + y * g.lsh;
+    uint8_t* mo = mask_u8 + o;
+    uint8_t* bo = bitmap + o;
+    float* lo = lines + size_t(page) * 2 * h * w + size_t(y) * w;
+    const bool vec = g.msw == 1 && g.lsw == 1 && (w & 3) == 0 && ((uintptr_t(ms) | uintptr_t(ls)) & 15) == 0;
+    if (vec) {
+      for (int x4 = threadIdx.x; x4 < (w >> 2); x4 += kOutThreads) {
+        const float4 m = __ldg(reinterpret_cast<const float4*>(ms) + x4);
+        float4 l = __ldg(reinterpret_cast<const float4*>(ls) + x4);
+        const float mv[4] = {m.x, m.y, m.z, m.w};
+        float* lv[4] = {&l.x, &l.y, &l.z, &l.w};
+        uint32_t mb = 0, bb = 0;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          if (finite_f(mv[k])) mb |= mask_byte(mv[k]) << (8 * k);
+          else bad |= 2;
+          if (!finite_f(*lv[k])) { bad |= 4; *lv[k] = 0.f; }
+          bb |= uint32_t(*lv[k] > thresh) << (8 * k);
+        }
+        reinterpret_cast<uint32_t*>(mo)[x4] = mb;
+        reinterpret_cast<uint32_t*>(bo)[x4] = bb;
+        reinterpret_cast<float4*>(lo)[x4] = l;
+      }
+    } else {
+      for (int x = threadIdx.x; x < w; x += kOutThreads) {
+        const float m = ms[x * g.msw];
+        float l = ls[x * g.lsw];
+        if (!finite_f(m)) bad |= 2;
+        if (!finite_f(l)) { bad |= 4; l = 0.f; }
+        mo[x] = finite_f(m) ? uint8_t(mask_byte(m)) : 0;
+        bo[x] = l > thresh ? 1 : 0;
+        lo[x] = l;
+      }
+    }
+  } else {
+    const size_t total = size_t(ws_rows) * no;
+    const size_t e0 = size_t(blockIdx.x - h) * kOutThreads * kBlkPerThread;
+    float* out = blks + size_t(page) * total;
+#pragma unroll
+    for (int k = 0; k < kBlkPerThread; ++k) {
+      const size_t e = e0 + size_t(k) * kOutThreads + threadIdx.x;
+      if (e >= total) break;
+      const int r = int(e / no), c = int(e - size_t(r) * no);
+      float v;
+      if (r < g.rows) {
+        v = g.blks[r * g.bsr + c * g.bsc];
+        if (!finite_f(v)) { bad |= 1; v = 0.f; }
+      } else {
+        v = c == 4 ? __int_as_float(0x7fc00000) : 0.f;   // NaN objectness: `obj > conf_thres` is false
+      }
+      out[e] = v;
+    }
+  }
+  if (bad) atomicOr(flags + page, int(bad));
+}
+
 }  // namespace
+
+cudaError_t gather_outputs_launch(const OutputGather* d_tab, int n, int h, int w, int no, int ws_rows, float thresh,
+                                  uint8_t* mask_u8, float* lines, uint8_t* bitmap, float* blks, int32_t* flags,
+                                  cudaStream_t s) {
+  if (n < 1 || h < 1 || w < 1 || no < 1 || ws_rows < 0) return cudaErrorInvalidValue;
+  const size_t per_cta = size_t(kOutThreads) * kBlkPerThread;
+  const unsigned blk_ctas = unsigned((size_t(ws_rows) * no + per_cta - 1) / per_cta);
+  gather_outputs_kernel<<<dim3(unsigned(h) + blk_ctas, unsigned(n)), kOutThreads, 0, s>>>(
+      d_tab, h, w, no, ws_rows, thresh, mask_u8, lines, bitmap, blks, flags);
+  return cudaGetLastError();
+}
 
 cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, cudaStream_t s) {
   if (n < 1 || total_rows < 1) return cudaErrorInvalidValue;

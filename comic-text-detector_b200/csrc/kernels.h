@@ -256,6 +256,28 @@ struct GatherPage {
 // one CTA per row of the n images of d_tab (total_rows = the sum of their ih)
 cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, cudaStream_t s);
 
+// A caller's network outputs for one page (ctd_submit_outputs), all in device memory, float32, element strides:
+// blks (r, c) at blks + r * bsr + c * bsc for r < rows, c < no; mask (y, x) at mask + y * msh + x * msw; channel 0 of
+// lines_map (y, x) at lines + y * lsh + x * lsw.
+struct OutputGather {
+  const float* blks;
+  long long bsr, bsc;
+  const float* mask;
+  long long msh, msw;
+  const float* lines;
+  long long lsh, lsw;
+  int rows, pad;
+};
+// One launch over the n pages of d_tab (gather.cu), each h x w: per page the u8 mask `(uint8_t)(int32_t)truncf(p *
+// 255.f)` (0 where the product is outside int32: numpy's float32 -> uint8 cast on x86-64) into mask_u8, channel 0 of
+// lines_map into lines (page stride 2 * h * w floats, where segrep reads it), the DB bitmap `p > thresh` into bitmap,
+// and the blks rows into blks at ws_rows rows per page, rows past `rows` padded with NaN objectness (never a
+// candidate).  flags[i] (zeroed by the caller) gets bit 0 / 1 / 2 for a non-finite value in page i's blks / mask /
+// lines; such a value is staged as 0.
+cudaError_t gather_outputs_launch(const OutputGather* d_tab, int n, int h, int w, int no, int ws_rows, float thresh,
+                                  uint8_t* mask_u8, float* lines, uint8_t* bitmap, float* blks, int32_t* flags,
+                                  cudaStream_t s);
+
 // refine_mask (refine_mk.cu): one kernel per phase over the window pixels of all pages of a batch, one CTA per chunk.
 struct RefineWin {
   int x1, y1, x2, y2;     // window (python slice semantics: rows y1..y2-1, cols x1..x2-1)

@@ -594,6 +594,10 @@ static int run_batch(ctd_handle* h, const PipeJob& job) {
   Slot& s = h->slot[job.slot];
   const int n = int(job.pages.size());
   CK(cudaEventSynchronize(s.ev_out_done));          // phase A results are in results_host
+  for (int i = 0; job.nonfinite && i < n; ++i)
+    if (const int32_t f = job.nonfinite[i])
+      return ctd_fail(h, CTD_E_INVALID, "page %d of the batch: a non-finite value (NaN or inf) in its %s", i,
+                      (f & 1) ? "blks" : (f & 2) ? "mask" : "lines_map");
   char* res = job.results_host;
   const BlockSection bs = block_section_layout();
   std::vector<std::vector<int32_t>> wins(static_cast<size_t>(n));
@@ -858,11 +862,16 @@ static int check_device_image(ctd_handle* h, const char* what, int i, const ctd_
 }
 
 // the slot's page tables, allocated at its first batch: max_batch PageGeom entries, then at pg_gather_off room for a
-// GatherPage entry per page and per mask of a batch
+// GatherPage entry per page and per mask of a batch, at pg_out_off an OutputGather entry per page (ctd_submit_outputs)
+// and at pg_flag_off its non-finite flags (device: written by the ingest; host: their copy back)
 static int ensure_page_tables(ctd_handle* h, Slot& s) {
   if (s.h_pg_tab) return CTD_OK;
-  h->pg_gather_off = (size_t(h->cfg.max_batch) * sizeof(PageGeom) + 255) / 256 * 256;
-  const size_t tab_bytes = h->pg_gather_off + 2 * size_t(h->cfg.max_batch) * sizeof(GatherPage);
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  const size_t nb = size_t(h->cfg.max_batch);
+  h->pg_gather_off = al(nb * sizeof(PageGeom));
+  h->pg_out_off = al(h->pg_gather_off + 2 * nb * sizeof(GatherPage));
+  h->pg_flag_off = al(h->pg_out_off + nb * sizeof(OutputGather));
+  const size_t tab_bytes = h->pg_flag_off + nb * sizeof(int32_t);
   CK(cudaHostAlloc(reinterpret_cast<void**>(&s.h_pg_tab), tab_bytes, cudaHostAllocDefault));
   CK(cudaMalloc(reinterpret_cast<void**>(&s.d_pg_tab), tab_bytes));
   return CTD_OK;
@@ -884,13 +893,38 @@ static int copy_host_runs(ctd_handle* h, const ctd_device_page* dev, int n, uint
   return CTD_OK;
 }
 
-extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
-                                int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
-                                int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
-                                int32_t results_on_device, void* results_host) {
+// a network output map of page i (ctd_submit_outputs): device memory of the handle's GPU from its first to its last
+// element (strides in [0, 2^31]), or a host pointer, whose byte span [*lo, *lo + *bytes) is returned
+static int check_output_map(ctd_handle* h, const char* what, int i, const float* p, int on_device, int64_t s0,
+                            int64_t s1, int n0, int n1, size_t* bytes) {
+  const int64_t kMaxStride = int64_t(1) << 31;
+  *bytes = 0;
+  if (n0 < 1 || n1 < 1) return CTD_OK;   // no element (blks with 0 rows)
+  if (!p) return ctd_fail(h, CTD_E_INVALID, "page %d: %s is NULL", i, what);
+  if (s0 < 0 || s1 < 0 || s0 > kMaxStride || s1 > kMaxStride)
+    return ctd_fail(h, CTD_E_INVALID, "page %d: %s strides (%lld, %lld) out of range [0, 2^31]", i, what, (long long)s0,
+                    (long long)s1);
+  const float* last = p + (n0 - 1) * s0 + (n1 - 1) * s1;
+  if (on_device) {
+    if (!is_device_memory(p, h->cfg.device) || !is_device_memory(last, h->cfg.device))
+      return ctd_fail(h, CTD_E_INVALID, "page %d: %s (%p) is not device memory of GPU %d", i, what, (const void*)p,
+                      h->cfg.device);
+  } else {
+    *bytes = size_t(last - p + 1) * sizeof(float);
+  }
+  return CTD_OK;
+}
+
+// ctd_submit_pages, and with `outs` ctd_submit_outputs: the caller's network outputs staged in place of the letterbox
+// and the forward
+static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                            int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
+                            const ctd_net_output* outs, int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
+                            int32_t results_on_device, void* results_host) {
+  const char* entry = outs ? "ctd_submit_outputs" : "ctd_submit_pages";
   if (!h || !pages || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
   if (textheight != 0 && textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
-  if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "ctd_submit_pages needs the full pipeline");
+  if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "%s needs the full pipeline", entry);
   Slot& s = h->slot[slot];
   if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
   if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
@@ -920,8 +954,38 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
     if (int rc = check_device_image(h, "page", i, dev[i], pg[size_t(i)].ih, pg[size_t(i)].iw, 3)) return rc;
     ++n_dev;
   }
+  // the outputs: shapes, and each map device memory of this GPU or a host span copied into the slot's out_in
+  const int no = 5 + h->cfg.nc, ws_rows = rows_per_image(net_h, net_w);
+  std::vector<std::array<size_t, 3>> host_bytes(outs ? size_t(n) : 0), host_off(outs ? size_t(n) : 0);
+  size_t out_in_bytes = 0;
+  if (outs) {
+    if (net_h > h->cfg.max_h || net_w > h->cfg.max_w)
+      return ctd_fail(h, CTD_E_SHAPE, "net input %dx%d exceeds the engine's %dx%d", net_h, net_w, h->cfg.max_h,
+                      h->cfg.max_w);
+    for (int i = 0; i < n; ++i) {
+      const ctd_net_output& o = outs[i];
+      if (o.rows < 0 || o.rows > ws_rows)
+        return ctd_fail(h, CTD_E_CAPACITY, "page %d: %d blks rows, the %dx%d workspace holds 0 to %d", i, o.rows, net_h,
+                        net_w, ws_rows);
+      auto& hb = host_bytes[size_t(i)];
+      if (int rc = check_output_map(h, "blks", i, o.blks, o.blks_on_device, o.blks_stride_r, o.blks_stride_c, o.rows,
+                                    no, &hb[0]))
+        return rc;
+      if (int rc = check_output_map(h, "mask", i, o.mask, o.mask_on_device, o.mask_stride_h, o.mask_stride_w, net_h,
+                                    net_w, &hb[1]))
+        return rc;
+      if (int rc = check_output_map(h, "lines", i, o.lines, o.lines_on_device, o.lines_stride_h, o.lines_stride_w,
+                                    net_h, net_w, &hb[2]))
+        return rc;
+      for (int k = 0; k < 3; ++k) {
+        host_off[size_t(i)][size_t(k)] = out_in_bytes;
+        out_in_bytes += (hb[size_t(k)] + 255) / 256 * 256;
+      }
+    }
+  }
   ShapePlan* sp = nullptr;
-  if (int rc = prepare_forward(h, n, net_h, net_w, &sp)) return rc;
+  if (!outs)
+    if (int rc = prepare_forward(h, n, net_h, net_w, &sp)) return rc;
   if (int rc = ensure_full_pipeline(h)) return rc;
   const ArenaLayout& L = h->layout;
   const PagesHead hd = pages_head(n);
@@ -933,6 +997,8 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   if (int rc = s.pg_res.grow(h, d2h + total, std::nullopt)) return rc;
   if (keep_undetected)
     if (int rc = s.pg_aux.grow(h, 2 * total, std::nullopt)) return rc;
+  if (out_in_bytes)
+    if (int rc = s.out_in.grow(h, out_in_bytes, std::nullopt)) return rc;
   if (int rc = ensure_page_tables(h, s)) return rc;
   PageGeom* tab = s.h_pg_tab;
   GatherPage* gtab = reinterpret_cast<GatherPage*>(reinterpret_cast<char*>(tab) + h->pg_gather_off);
@@ -952,8 +1018,30 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   // phase A: tables and host pages in on copy_in (a batch with device pages copies only its host pages' byte ranges,
   // one copy per run of consecutive host pages); the device pages' events, the gather of the device pages, letterbox,
   // forward, back-projection and the phase-A rows on the engine stream; rows + masks out on copy_out
-  const size_t tab_bytes = n_gather ? h->pg_gather_off + size_t(n_gather) * sizeof(GatherPage) : size_t(n) * sizeof(PageGeom);
+  OutputGather* otab = reinterpret_cast<OutputGather*>(reinterpret_cast<char*>(tab) + h->pg_out_off);
+  for (int i = 0; outs && i < n; ++i) {
+    const ctd_net_output& o = outs[i];
+    // a host map is read from its copy in out_in, at the same strides
+    auto at = [&](const float* p, int k) {
+      return host_bytes[size_t(i)][size_t(k)] ? reinterpret_cast<const float*>(s.out_in.p + host_off[size_t(i)][size_t(k)])
+                                              : p;
+    };
+    otab[i] = OutputGather{o.blks_on_device ? o.blks : at(o.blks, 0), (long long)o.blks_stride_r,
+                           (long long)o.blks_stride_c, o.mask_on_device ? o.mask : at(o.mask, 1),
+                           (long long)o.mask_stride_h, (long long)o.mask_stride_w,
+                           o.lines_on_device ? o.lines : at(o.lines, 2), (long long)o.lines_stride_h,
+                           (long long)o.lines_stride_w, o.rows, 0};
+  }
+  const size_t tab_bytes = outs       ? h->pg_out_off + size_t(n) * sizeof(OutputGather)
+                           : n_gather ? h->pg_gather_off + size_t(n_gather) * sizeof(GatherPage)
+                                      : size_t(n) * sizeof(PageGeom);
   CK(cudaMemcpyAsync(s.d_pg_tab, tab, tab_bytes, cudaMemcpyHostToDevice, h->copy_in));
+  for (int i = 0; outs && i < n; ++i) {
+    const float* src[3] = {outs[i].blks, outs[i].mask, outs[i].lines};
+    for (int k = 0; k < 3; ++k)
+      if (const size_t b = host_bytes[size_t(i)][size_t(k)])
+        CK(cudaMemcpyAsync(s.out_in.p + host_off[size_t(i)][size_t(k)], src[k], b, cudaMemcpyHostToDevice, h->copy_in));
+  }
   if (n_dev == 0) {
     CK(cudaMemcpyAsync(s.pg_in.p, input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
   } else {
@@ -972,8 +1060,23 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
                                                                h->pg_gather_off),
                            n_gather, gather_rows, h->stream));
   }
-  CK(letterbox_batch_launch(s.pg_in.p, s.d_pg_tab, n, h->d_pages, net_h, net_w, h->stream));
-  if (int rc = enqueue_forward(h, n, net_h, net_w, *sp)) return rc;
+  if (outs) {
+    // the caller's outputs into the workspace the forward would have written, then the forward's NMS and DB tail
+    for (int i = 0; i < n; ++i)
+      if (outs[i].event) CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(outs[i].event), 0));
+    int32_t* d_flags = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(s.d_pg_tab) + h->pg_flag_off);
+    CK(cudaMemsetAsync(d_flags, 0, size_t(n) * sizeof(int32_t), h->stream));
+    CK(gather_outputs_launch(reinterpret_cast<const OutputGather*>(reinterpret_cast<const char*>(s.d_pg_tab) +
+                                                                   h->pg_out_off),
+                             n, net_h, net_w, no, ws_rows, h->cfg.db_thresh, h->d_mask_u8, h->d_lines, h->d_bitmap,
+                             h->d_blks, d_flags, h->stream));
+    int cnt = 0;
+    if (int rc = launch_nms(h, n, net_h, net_w, h->stream, &cnt)) return rc;
+    if (int rc = launch_db_post(h, n, net_h, net_w, h->stream, &cnt)) return rc;
+  } else {
+    CK(letterbox_batch_launch(s.pg_in.p, s.d_pg_tab, n, h->d_pages, net_h, net_w, h->stream));
+    if (int rc = enqueue_forward(h, n, net_h, net_w, *sp)) return rc;
+  }
   uint8_t* d_res = s.pg_res.p;
   CK(backproject_batch_launch(h->d_mask_u8, net_h, net_w, s.d_pg_tab, n, row0, d_res + hd.masks, h->stream));
   const size_t nb = size_t(n);
@@ -985,8 +1088,14 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   CK(cudaEventRecord(s.ev_out_ready, h->stream));
   CK(cudaStreamWaitEvent(h->copy_out, s.ev_out_ready, 0));
   CK(cudaMemcpyAsync(results_host, d_res, d2h, cudaMemcpyDeviceToHost, h->copy_out));
-  CK(cudaEventRecord(s.ev_out_done, h->copy_out));
   PipeJob job;
+  if (outs) {
+    char* h_flags = reinterpret_cast<char*>(s.h_pg_tab) + h->pg_flag_off;
+    CK(cudaMemcpyAsync(h_flags, reinterpret_cast<char*>(s.d_pg_tab) + h->pg_flag_off, size_t(n) * sizeof(int32_t),
+                       cudaMemcpyDeviceToHost, h->copy_out));
+    job.nonfinite = reinterpret_cast<const int32_t*>(h_flags);
+  }
+  CK(cudaEventRecord(s.ev_out_done, h->copy_out));
   job.slot = slot; job.refine_mode = refine_mode;
   job.results_host = static_cast<char*>(results_host);
   job.head = hd;
@@ -1008,6 +1117,23 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
   if (results_on_device) s.dev_pages = std::move(pg);
   queue_job(h, std::move(job));
   return CTD_OK;
+}
+
+extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                                int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
+                                int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
+                                int32_t results_on_device, void* results_host) {
+  return submit_pages_job(h, slot, pages, n, net_h, net_w, input_host, dev, nullptr, refine_mode, keep_undetected,
+                          textheight, results_on_device, results_host);
+}
+
+extern "C" int ctd_submit_outputs(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                                  int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev_pages,
+                                  const ctd_net_output* outs, int32_t refine_mode, int32_t keep_undetected,
+                                  int32_t textheight, int32_t results_on_device, void* results_host) {
+  if (!outs) return CTD_E_INVALID;
+  return submit_pages_job(h, slot, pages, n, net_h, net_w, input_host, dev_pages, outs, refine_mode, keep_undetected,
+                          textheight, results_on_device, results_host);
 }
 
 extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,

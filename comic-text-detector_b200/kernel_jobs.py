@@ -1,6 +1,7 @@
-"""What the batched jobs that run no network share: `MaskRefiner` (textmask.py) and `RegionCropper` (regions.py) each
-own a kernels-only engine, decode encoded pages with decoders made on first use, and run their batches through the
-engine's two slots, two batches in flight, leaving no batch in flight when the caller stops early."""
+"""What the batched jobs that run no network share: `MaskRefiner` (textmask.py), `RegionCropper` (regions.py) and
+`PostProcessor` (postprocess.py) each own a kernels-only engine, decode encoded pages with decoders made on first use,
+and run their batches through the engine's two slots, two batches in flight, leaving no batch in flight when the caller
+stops early."""
 from collections import deque
 
 from .inference import _Encoded, check_page, decode_files
@@ -21,10 +22,11 @@ class KernelsOnlyJob:
     """A kernels-only engine on cuda:device_index for batches of up to max_batch pages, and the decoders of its
     encoded pages."""
 
-    def __init__(self, device_index=0, max_batch=16):
+    def __init__(self, device_index=0, max_batch=16, **engine_args):
+        """engine_args: the workspace and post-processing arguments of kernels_only_engine"""
         self.device_index = int(device_index)
         self.max_batch = int(max_batch)
-        self.net = kernels_only_engine(self.device_index, self.max_batch)
+        self.net = kernels_only_engine(self.device_index, self.max_batch, **engine_args)
         self._jpeg = None
         self._png = None
 

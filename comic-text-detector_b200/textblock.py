@@ -160,23 +160,26 @@ def group_output(blks, lines, im_w, im_h, mask=None, sort_blklist=True):
     return blocks_from_records(rec[:n.value], lout, dout)
 
 
-_KERNELS_ONLY = None
+_KERNELS_ONLY = {}   # nc -> the program with no ops
 _REGION_ENGINE = None
 _REGION_LOCK = threading.Lock()
 
 
-def kernels_only_engine(device_index, max_batch):
-    """an engine on cuda:device_index that runs no network (the program has no ops, and a 64x64 workspace): the
-    stand-alone kernels and the batched jobs of caller blocks take it.  The program is built once per process."""
-    global _KERNELS_ONLY
-    if _KERNELS_ONLY is None:
+def kernels_only_engine(device_index, max_batch, max_size=(64, 64), nc=2, conf_thresh=0.4, nms_thresh=0.35,
+                        skip_postproc=True):
+    """an engine on cuda:device_index that runs no network (the program has no ops): the stand-alone kernels and the
+    batched jobs of caller blocks take it with the defaults (a 64x64 workspace, no post-processing workspaces in use).
+    `PostProcessor` sizes it for max_batch pages of max_size (h, w) with skip_postproc=False, so NMS (nc classes,
+    conf_thresh, nms_thresh), the DB tail and the result arena run on it.  The program is built once per process."""
+    if nc not in _KERNELS_ONLY:
         from . import compiler
         P = compiler.Program()
-        P.nc = 2
+        P.nc = int(nc)
         P.newbuf(8, 1)
-        _KERNELS_ONLY = P
-    return binding.Engine(_KERNELS_ONLY, device=device_index, max_batch=max_batch, max_h=64, max_w=64,
-                          skip_postproc=True)
+        _KERNELS_ONLY[nc] = P
+    return binding.Engine(_KERNELS_ONLY[nc], device=device_index, max_batch=max_batch, max_h=int(max_size[0]),
+                          max_w=int(max_size[1]), conf_thresh=conf_thresh, nms_thresh=nms_thresh,
+                          skip_postproc=skip_postproc)
 
 
 def _region_engine():

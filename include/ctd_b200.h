@@ -538,6 +538,43 @@ CTD_API int ctd_submit_regions(ctd_handle* h, int32_t slot, const ctd_page_entry
                                const ctd_region_line* lines, const int32_t* n_lines, int32_t textheight,
                                const uint8_t* input_host, const ctd_device_page* dev_pages, int32_t results_on_device);
 
+/* ---- the detector's post-processing on a caller's network outputs ------------------------------------------------
+ * ctd_submit_outputs runs everything TextDetector.__call__ does after `self.net(img_in)` (inference.py:148-178) on
+ * outputs the caller computed (this engine's TextDetBase, or any other runtime): NMS, postprocess_mask, the DB
+ * threshold, connected components and text-line boxes, the box_thresh filter, the mask crop and resize back to the
+ * page, the line rescale, group_output, refine_mask and refine_undetected_mask, and with a textheight the crops.  It
+ * takes the arguments of ctd_submit_pages (the same ctd_pages_plan entries for (net_h, net_w), page buffers, slots and
+ * collect calls: ctd_collect, ctd_collect_regions, ctd_collect_device) plus one ctd_net_output per page, and its results
+ * are laid out as theirs.  Instead of the letterbox and the forward, one launch stages every page's outputs into the
+ * handle's post-processing workspace; the rest of the batch is that of ctd_submit_pages.
+ *
+ * ctd_net_output describes the outputs of page i, float32 with element strides (each >= 0):
+ *   blks:  element (r, c), r < rows, c < 5 + nc, at blks + r * blks_stride_r + c * blks_stride_c; 0 <= rows <=
+ *          3 * (net_h/8 * net_w/8 + net_h/16 * net_w/16 + net_h/32 * net_w/32)
+ *   mask:  the [net_h][net_w] segmentation map, (y, x) at mask + y * mask_stride_h + x * mask_stride_w
+ *   lines: channel 0 of lines_map, [net_h][net_w], (y, x) at lines + y * lines_stride_h + x * lines_stride_w
+ * *_on_device: 1 when the map is device memory of the handle's GPU (its first and last element are checked with
+ * cudaPointerGetAttributes), 0 when it is host memory; host maps are copied on the copy stream at submission (pinned
+ * memory keeps that copy asynchronous) and, like device maps, must stay unwritten until the slot is collected.
+ * `event` (a cudaEvent_t, may be NULL) is waited on before the device maps are read.  A non-finite value in any map
+ * fails the batch at ctd_collect (CTD_E_INVALID, naming the page of the batch and the map).  Needs a handle created
+ * without debug_skip_postproc and with max_h >= net_h, max_w >= net_w; the handle's program may have no ops.         */
+typedef struct ctd_net_output {
+  const float* blks;
+  int64_t blks_stride_r, blks_stride_c;
+  const float* mask;
+  int64_t mask_stride_h, mask_stride_w;
+  const float* lines;
+  int64_t lines_stride_h, lines_stride_w;
+  int32_t rows;
+  int32_t blks_on_device, mask_on_device, lines_on_device;
+  void* event;
+} ctd_net_output;
+CTD_API int ctd_submit_outputs(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
+                               int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev_pages,
+                               const ctd_net_output* outs, int32_t refine_mode, int32_t keep_undetected,
+                               int32_t textheight, int32_t results_on_device, void* results_host);
+
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
  * [rows][5+nc]); output as ctd_get_detections for one page.                                */
 CTD_API int ctd_nms(ctd_handle* h, const float* pred, int32_t rows, float conf_thresh, float iou_thresh, float* det,
