@@ -11,3 +11,4 @@ from .png import PngDecoder, PngEncoder, png_probe  # noqa: F401
 from .textmask import MaskRefiner, refine_mask, refine_undetected_mask  # noqa: F401
 from .regions import RegionCropper  # noqa: F401
 from .postprocess import PostProcessor  # noqa: F401
+from .preprocess import NetworkDetector, Preprocessor, preprocess_img  # noqa: F401

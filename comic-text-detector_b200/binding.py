@@ -107,7 +107,9 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_jpeg_decoder_create", "ctd_jpeg_decoder_destroy", "ctd_jpeg_decode", "ctd_debug_postprocess",
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
            "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
-           "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot", "ctd_submit_outputs"]
+           "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot", "ctd_submit_outputs",
+           "ctd_preprocess_pages"]
+PRE_F32_NCHW, PRE_F16_NCHW, PRE_U8_NHWC = 0, 1, 2   # ctd_pre_format
 
 _lib = None
 
@@ -173,6 +175,7 @@ def load_library():
     lib.ctd_submit_regions.argtypes = [vp, i32, vp, i32, vp, vp, i32, vp, vp, i32]
     lib.ctd_debug_read_slot.argtypes = [vp, i32, i32, C.c_size_t, vp, C.c_size_t]
     lib.ctd_submit_outputs.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.ctd_preprocess_pages.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, i32, vp, vp]
     lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
     lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.ctd_jpeg_decoder_destroy.argtypes = [vp]
@@ -669,6 +672,33 @@ class Engine:
                 if md]
         self._pg_inflight[slot] = (entries, int(textheight), bool(device_results), kept)
         self.shape = (len(entries), net_h, net_w)
+
+    def preprocess_pages(self, pages, net_h, net_w, fmt, reverse, dst_ptr, stream, events=None, input_host=None):
+        """`ctd_preprocess_pages`: the letterboxed network input of a batch (fmt: PRE_*; reverse: output channel k is
+        page channel 2 - k) into dst_ptr (a device pointer as int, 16-byte aligned), enqueued on `stream` (a
+        cudaStream_t as int) with no host wait.  A page is a torch.uint8 CUDA tensor [h][w][3] on this engine's GPU
+        with any strides (events[i]: a recorded torch.cuda.Event or None, waited on before page i is read), or a u8
+        [h][w][3] numpy array, packed at its page_off into input_host: a pinned torch.uint8 tensor of at least the
+        plan's input bytes, which the caller keeps unwritten until the stream has run the call.  Returns the
+        ctd_pages_plan entries of the batch."""
+        import torch
+        entries, in_bytes, _res = pages_plan([tuple(p.shape[:2]) for p in pages], net_h, net_w)
+        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
+        host = None
+        if not all(on_dev):
+            if input_host is None or input_host.numel() < in_bytes:
+                raise CtdError("numpy pages need a pinned input_host of %d bytes" % in_bytes)
+            inp = input_host.numpy()
+            for e, p, d in zip(entries, pages, on_dev):
+                if not d:
+                    o = int(e["page_off"])
+                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+            host = C.c_void_p(input_host.data_ptr())
+        dev = _device_images(pages, on_dev, events, 3)
+        self._ck(self.lib.ctd_preprocess_pages(self.h, _ptr(entries), len(entries), int(net_h), int(net_w), host,
+                                               None if dev is None else C.cast(dev, C.c_void_p), int(fmt),
+                                               int(bool(reverse)), C.c_void_p(dst_ptr), C.c_void_p(stream)))
+        return entries
 
     def submit_refine(self, slot, pages, masks, boxes, refine_mode=0, keep_undetected=False, refined=None,
                       events=None, device_results=False):

@@ -50,6 +50,12 @@ extern "C" void ctd_destroy(ctd_handle* h) {
   if (!h) return;
   cudaSetDevice(h->cfg.device);
   ctd_pipeline_shutdown(h);
+  if (h->ev_pre) {   // ctd_preprocess_pages' buffers: free once its last call's kernels ran
+    cudaEventSynchronize(h->ev_pre);
+    cudaEventDestroy(h->ev_pre);
+  }
+  cudaFree(h->pre_in);
+  cudaFree(h->d_pre_tab);
   for (auto& kv : h->plans)
     if (kv.second.graph) cudaGraphExecDestroy(kv.second.graph);
   for (void* p : h->d_buf) cudaFree(p);

@@ -287,6 +287,13 @@ struct ctd_handle {
   // cc_scratch belong to the caller's stream)
   DevBuf pg_cc;
   DevBuf post_refine;
+  // ctd_preprocess_pages: the packed pages (stream-ordered allocations) and the page tables of the last call, and an
+  // event recorded on its stream after its last read of them, which the next call's stream waits on before it writes
+  // them
+  uint8_t* pre_in = nullptr;
+  size_t pre_in_cap = 0;
+  char* d_pre_tab = nullptr;
+  cudaEvent_t ev_pre = nullptr;
   // last forward
   int n = 0, ph = 0, pw = 0;
   int last_launches = 0;

@@ -8,6 +8,7 @@
 // into the engine's post-processing workspace in one launch, with postprocess_mask's u8 cast and the DB threshold fused.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <string.h>
 
 #include "kernels.h"
 
@@ -173,6 +174,27 @@ cudaError_t gather_outputs_launch(const OutputGather* d_tab, int n, int h, int w
 cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, cudaStream_t s) {
   if (n < 1 || total_rows < 1) return cudaErrorInvalidValue;
   gather_pages_kernel<<<unsigned(total_rows), 256, 0, s>>>(d_tab, n);
+  return cudaGetLastError();
+}
+
+namespace {
+struct ParamWords {
+  uint4 w[240];   // 3840 bytes: with the other arguments, inside the 4 KB kernel parameter space
+};
+__global__ void param_words_kernel(const __grid_constant__ ParamWords p, int n, uint4* __restrict__ dst) {
+  for (int i = threadIdx.x; i < n; i += blockDim.x) dst[i] = p.w[i];
+}
+}  // namespace
+
+cudaError_t upload_table_launch(const void* host, size_t bytes, void* dst, cudaStream_t s) {
+  if (bytes % 16 || (uintptr_t(dst) & 15)) return cudaErrorInvalidValue;
+  const size_t chunk = sizeof(ParamWords);
+  for (size_t off = 0; off < bytes; off += chunk) {
+    ParamWords p;
+    const size_t b = bytes - off < chunk ? bytes - off : chunk;
+    memcpy(p.w, static_cast<const char*>(host) + off, b);
+    param_words_kernel<<<1, 256, 0, s>>>(p, int(b / 16), reinterpret_cast<uint4*>(static_cast<char*>(dst) + off));
+  }
   return cudaGetLastError();
 }
 

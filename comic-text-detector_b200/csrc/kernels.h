@@ -240,6 +240,13 @@ cudaError_t letterbox_batch_launch(const uint8_t* src, const PageGeom* d_tab, in
                                    cudaStream_t s);
 cudaError_t backproject_batch_launch(const uint8_t* mask, int net_h, int net_w, const PageGeom* d_tab, int n,
                                      int total_rows, uint8_t* dst, cudaStream_t s);
+// The letterbox of every page of a batch as preprocess_img's tensor (ctd_preprocess_pages), written into dst (16-byte
+// aligned, net_w a multiple of 16) in one launch: format PRE_F32_NCHW / PRE_F16_NCHW gives [n][3][net_h][net_w] with
+// each u8 value v as v / 255 (correctly rounded f32; f16: that f32 rounded to nearest even), PRE_U8_NHWC the u8 pixels
+// [n][net_h][net_w][3]; padding is 0.  reverse: output channel k is channel 2 - k of the page.
+enum PreFormat { PRE_F32_NCHW = 0, PRE_F16_NCHW = 1, PRE_U8_NHWC = 2 };
+cudaError_t letterbox_tensor_launch(const uint8_t* src, const PageGeom* d_tab, int n, void* dst, int net_h, int net_w,
+                                    int format, bool reverse, cudaStream_t s);
 
 // Pages (and masks) of a batch that are already in device memory (ctd_submit_pages, ctd_submit_refine), gathered
 // into the packed planes of the batch (gather.cu): byte (y, x, c) of the source is at src + y * sh + x * sw + c * sc;
@@ -255,6 +262,10 @@ struct GatherPage {
 };
 // one CTA per row of the n images of d_tab (total_rows = the sum of their ih)
 cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, cudaStream_t s);
+// `bytes` (a multiple of 16) of a host table into device memory dst (16-byte aligned), ordered on stream s: the bytes
+// travel as kernel arguments, 3840 per launch, so the host table may be reused as soon as this returns and no pinned
+// staging buffer or host wait orders the copy (ctd_preprocess_pages)
+cudaError_t upload_table_launch(const void* host, size_t bytes, void* dst, cudaStream_t s);
 
 // A caller's network outputs for one page (ctd_submit_outputs), all in device memory, float32, element strides:
 // blks (r, c) at blks + r * bsr + c * bsc for r < rows, c < no; mask (y, x) at mask + y * msh + x * msw; channel 0 of

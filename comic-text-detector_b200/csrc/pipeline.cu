@@ -17,6 +17,8 @@
 // masks and crops may stay there (ctd_collect_device).  ctd_submit_refine runs phase C alone on caller pages, masks
 // and block boxes (textmask.refine_mask / refine_undetected_mask, MaskRefiner) through the same two-slot schedule, and
 // ctd_submit_regions the crop stage alone on caller pages and text lines (regions.RegionCropper).
+// ctd_preprocess_pages letterboxes a batch of pages into a caller's network input tensor on the caller's stream, with
+// no slot (preprocess.Preprocessor).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -1134,6 +1136,93 @@ extern "C" int ctd_submit_outputs(ctd_handle* h, int32_t slot, const ctd_page_en
   if (!outs) return CTD_E_INVALID;
   return submit_pages_job(h, slot, pages, n, net_h, net_w, input_host, dev_pages, outs, refine_mode, keep_undetected,
                           textheight, results_on_device, results_host);
+}
+
+static_assert(int(CTD_PRE_F32_NCHW) == int(PRE_F32_NCHW) && int(CTD_PRE_F16_NCHW) == int(PRE_F16_NCHW) &&
+                  int(CTD_PRE_U8_NHWC) == int(PRE_U8_NHWC),
+              "ctd_preprocess_pages formats");
+
+extern "C" int ctd_preprocess_pages(ctd_handle* h, const ctd_page_entry* pages, int32_t n, int32_t net_h, int32_t net_w,
+                                    const uint8_t* input_host, const ctd_device_page* dev, int32_t format,
+                                    int32_t reverse_channels, void* dst, void* stream) {
+  if (!h || !pages || !dst || n < 1) return CTD_E_INVALID;
+  if (format != CTD_PRE_F32_NCHW && format != CTD_PRE_F16_NCHW && format != CTD_PRE_U8_NHWC)
+    return ctd_fail(h, CTD_E_INVALID, "format %d is not a CTD_PRE_* format", format);
+  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
+  std::vector<ctd_page_entry> pg(pages, pages + n);
+  size_t in_bytes = 0, res_bytes = 0;
+  if (int rc = ctd_pages_plan(pg.data(), n, net_h, net_w, &in_bytes, &res_bytes))
+    return ctd_fail(h, rc, "the pages do not letterbox into a %dx%d net input", net_h, net_w);
+  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
+    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_pages_plan returns");
+  size_t rows = 0;
+  for (int i = 0; i < n; ++i) rows += size_t(pg[size_t(i)].ih);
+  if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
+  CK(cudaSetDevice(h->cfg.device));
+  const size_t elem = format == CTD_PRE_F32_NCHW ? 4 : format == CTD_PRE_F16_NCHW ? 2 : 1;
+  const size_t out_bytes = size_t(n) * 3 * size_t(net_h) * size_t(net_w) * elem;
+  if (reinterpret_cast<uintptr_t>(dst) % 16) return ctd_fail(h, CTD_E_INVALID, "dst must be 16-byte aligned");
+  if (!is_device_memory(dst, h->cfg.device) || !is_device_memory(static_cast<char*>(dst) + out_bytes - 1, h->cfg.device))
+    return ctd_fail(h, CTD_E_INVALID, "dst (%p, %zu bytes) is not device memory of GPU %d", dst, out_bytes,
+                    h->cfg.device);
+  int n_dev = 0;
+  for (int i = 0; i < n; ++i) {
+    if (!dev || !dev[i].data) {
+      if (!input_host) return ctd_fail(h, CTD_E_INVALID, "page %d is in neither input_host nor device memory", i);
+      continue;
+    }
+    if (int rc = check_device_image(h, "page", i, dev[i], pg[size_t(i)].ih, pg[size_t(i)].iw, 3)) return rc;
+    ++n_dev;
+  }
+  // everything from here on is ordered on the caller's stream, after the last call's reads of the page buffer and the
+  // tables (ev_pre): a larger page buffer is a stream-ordered allocation, the old one a stream-ordered free
+  cudaStream_t cs = static_cast<cudaStream_t>(stream);
+  auto al = [](size_t v) { return (v + 255) / 256 * 256; };
+  const size_t gather_off = al(size_t(h->cfg.max_batch) * sizeof(PageGeom));
+  if (!h->d_pre_tab)
+    CK(cudaMalloc(reinterpret_cast<void**>(&h->d_pre_tab), gather_off + size_t(h->cfg.max_batch) * sizeof(GatherPage)));
+  if (!h->ev_pre) CK(cudaEventCreateWithFlags(&h->ev_pre, cudaEventDisableTiming));
+  CK(cudaStreamWaitEvent(cs, h->ev_pre, 0));   // a no-op before the first record
+  if (in_bytes > h->pre_in_cap) {
+    if (h->pre_in) CK(cudaFreeAsync(h->pre_in, cs));
+    h->pre_in = nullptr;
+    h->pre_in_cap = 0;
+    CK(cudaMallocAsync(reinterpret_cast<void**>(&h->pre_in), in_bytes + in_bytes / 4, cs));
+    h->pre_in_cap = in_bytes + in_bytes / 4;
+  }
+  // the tables: PageGeom per page, then at gather_off a GatherPage per device page
+  std::vector<char> tab(gather_off + size_t(n_dev) * sizeof(GatherPage));
+  PageGeom* geo = reinterpret_cast<PageGeom*>(tab.data());
+  GatherPage* gtab = reinterpret_cast<GatherPage*>(tab.data() + gather_off);
+  int n_gather = 0, gather_rows = 0;
+  for (int i = 0; i < n; ++i) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    geo[i] = PageGeom{e.page_off, 0, e.ih, e.iw, e.unpad_h, e.unpad_w, 0, 0};
+    if (dev && dev[i].data) {
+      const ctd_device_page& d = dev[i];
+      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c,
+                                    h->pre_in + e.page_off, e.ih, e.iw, gather_rows,
+                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0, 3, 0};
+      gather_rows += e.ih;
+    }
+  }
+  const size_t tab_bytes = n_gather ? tab.size() : size_t(n) * sizeof(PageGeom);
+  tab.resize((tab_bytes + 15) / 16 * 16);
+  CK(upload_table_launch(tab.data(), tab.size(), h->d_pre_tab, cs));
+  if (n_dev < n) {
+    if (int rc = copy_host_runs(h, dev, n, h->pre_in, input_host, [&](int i) { return size_t(pg[size_t(i)].page_off); },
+                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; }, cs))
+      return rc;
+  }
+  if (n_gather) {
+    for (int i = 0; i < n; ++i)
+      if (dev[i].data && dev[i].event) CK(cudaStreamWaitEvent(cs, static_cast<cudaEvent_t>(dev[i].event), 0));
+    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(h->d_pre_tab + gather_off), n_gather, gather_rows, cs));
+  }
+  CK(letterbox_tensor_launch(h->pre_in, reinterpret_cast<const PageGeom*>(h->d_pre_tab), n, dst, net_h, net_w, format,
+                             reverse_channels != 0, cs));
+  CK(cudaEventRecord(h->ev_pre, cs));
+  return CTD_OK;
 }
 
 extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,

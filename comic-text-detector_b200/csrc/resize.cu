@@ -9,6 +9,9 @@
 //   * dst*2 == src in both axes: computed as INTER_AREA, (p00+p01+p10+p11+2)>>2
 // Oracle: oracle/resize_ref.py (pinned against the installed cv2, tests/test_cpu_resize.py).
 // The output may be a window of a larger zero-padded canvas (letterbox: bottom/right padding).
+// letterbox_tensor_kernel writes the same letterbox as the network tensor of preprocess_img (inference.py:72-83):
+// f32 or f16 NCHW planes of v / 255, or u8 NHWC, in either channel order.
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -86,6 +89,67 @@ __global__ void letterbox_batch_kernel(const uint8_t* __restrict__ src, const Pa
   resize_pixel<3>(src + g.src_off, g.ih, g.iw, size_t(g.iw) * 3, o, x, y, g.unpad_h, g.unpad_w);
 }
 
+// v / 255 as numpy's `astype(float32) / 255` computes it: a correctly rounded float32 division (__fdiv_rn(v, 255.f)),
+// which is not v * RN(1/255) (the two differ on 126 of the 256 u8 values).  The product by RN(1/255) corrected once by
+// its fma residual equals the division on all 256 values (checked in exact arithmetic, tests/test_cpu_preprocess.py),
+// and needs no call to __fdiv_rn's slow path, whose register saves would spill.
+__device__ __forceinline__ float unit_f32(uint8_t v) {
+  const float r = 0x1.010102p-8f;   // RN(1 / 255)
+  const float x = float(v);
+  const float q0 = __fmul_rn(x, r);
+  return __fmaf_rn(__fmaf_rn(-q0, 255.0f, x), r, q0);
+}
+
+// The letterbox of every page of a batch written as the tensor `preprocess_img` makes (ctd_preprocess_pages):
+// blockIdx.z = page, blockIdx.y = row, each thread kPx consecutive pixels of the row, each computed by resize_pixel<3>
+// and packed into the thread's output words as soon as it is computed (so few values are live across the double
+// divisions of axis_tap).  NCHW: one 16-byte store per plane (4 f32 or 8 f16 values); NHWC u8: 16 pixels = three
+// 16-byte stores.  Reverse: output channel k is channel 2 - k of the page.
+template <int Fmt, bool Reverse>
+__global__ void __launch_bounds__(128) letterbox_tensor_kernel(const uint8_t* __restrict__ src,
+                                                               const PageGeom* __restrict__ tab, void* __restrict__ dst,
+                                                               int net_h, int net_w) {
+  constexpr int kPx = Fmt == PRE_F32_NCHW ? 4 : Fmt == PRE_F16_NCHW ? 8 : 16;
+  const int x0 = (blockIdx.x * blockDim.x + threadIdx.x) * kPx;
+  const int y = blockIdx.y;
+  if (x0 >= net_w) return;
+  const PageGeom g = tab[blockIdx.z];
+  // f32: w[k][i] = the bits of pixel i of plane k; f16: w[k][i / 2] holds pixels i, i + 1 of plane k (low half first);
+  // u8: w[0..11] are the 48 bytes of the 16 pixels, little-endian
+  uint32_t w[3][4] = {};
+#pragma unroll
+  for (int i = 0; i < kPx; ++i) {
+    uint8_t p[3];
+    resize_pixel<3>(src + g.src_off, g.ih, g.iw, size_t(g.iw) * 3, p, x0 + i, y, g.unpad_h, g.unpad_w);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const uint8_t v = p[Reverse ? 2 - k : k];
+      if constexpr (Fmt == PRE_F32_NCHW) {
+        w[k][i] = __float_as_uint(unit_f32(v));
+      } else if constexpr (Fmt == PRE_F16_NCHW) {
+        w[k][i / 2] |= uint32_t(__half_as_ushort(__float2half_rn(unit_f32(v)))) << (16 * (i % 2));
+      } else {
+        const int j = 3 * i + k;
+        w[j / 16][(j / 4) % 4] |= uint32_t(v) << (8 * (j % 4));
+      }
+    }
+  }
+  if constexpr (Fmt == PRE_U8_NHWC) {
+    uint4* o = reinterpret_cast<uint4*>(static_cast<uint8_t*>(dst) +
+                                        ((size_t(blockIdx.z) * net_h + y) * net_w + x0) * 3);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) o[k] = make_uint4(w[k][0], w[k][1], w[k][2], w[k][3]);
+  } else {
+    constexpr int kElem = Fmt == PRE_F32_NCHW ? 4 : 2;
+    const size_t plane = size_t(net_h) * net_w;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      const size_t at = (size_t(blockIdx.z) * 3 + k) * plane + size_t(y) * net_w + x0;
+      *reinterpret_cast<uint4*>(static_cast<uint8_t*>(dst) + at * kElem) = make_uint4(w[k][0], w[k][1], w[k][2], w[k][3]);
+    }
+  }
+}
+
 // Mask back-projection of every page of a batch: one CTA per output row over the pages' stacked rows (page p owns rows
 // [row0, row0 + ih)), so no CTA is launched for a row that does not exist; the threads stride over the row's columns.
 __global__ void backproject_batch_kernel(const uint8_t* __restrict__ mask, int net_h, int net_w,
@@ -119,6 +183,29 @@ cudaError_t letterbox_batch_launch(const uint8_t* src, const PageGeom* d_tab, in
   if (n < 1 || net_h < 1 || net_w < 1) return cudaErrorInvalidValue;
   letterbox_batch_kernel<<<dim3(unsigned((net_w + 127) / 128), unsigned(net_h), unsigned(n)), 128, 0, s>>>(src, d_tab, dst,
                                                                                                         net_h, net_w);
+  return cudaGetLastError();
+}
+
+template <int Fmt, bool Reverse>
+static void letterbox_tensor_launch_t(const uint8_t* src, const PageGeom* d_tab, int n, void* dst, int net_h, int net_w,
+                                      cudaStream_t s) {
+  constexpr int kPx = Fmt == PRE_F32_NCHW ? 4 : Fmt == PRE_F16_NCHW ? 8 : 16;
+  const dim3 grid(unsigned((net_w / kPx + 127) / 128), unsigned(net_h), unsigned(n));
+  letterbox_tensor_kernel<Fmt, Reverse><<<grid, 128, 0, s>>>(src, d_tab, dst, net_h, net_w);
+}
+
+cudaError_t letterbox_tensor_launch(const uint8_t* src, const PageGeom* d_tab, int n, void* dst, int net_h, int net_w,
+                                    int format, bool reverse, cudaStream_t s) {
+  if (n < 1 || net_h < 1 || net_w < 16 || net_w % 16 || (uintptr_t(dst) & 15)) return cudaErrorInvalidValue;
+  switch (format * 2 + (reverse ? 1 : 0)) {
+    case PRE_F32_NCHW * 2: letterbox_tensor_launch_t<PRE_F32_NCHW, false>(src, d_tab, n, dst, net_h, net_w, s); break;
+    case PRE_F32_NCHW * 2 + 1: letterbox_tensor_launch_t<PRE_F32_NCHW, true>(src, d_tab, n, dst, net_h, net_w, s); break;
+    case PRE_F16_NCHW * 2: letterbox_tensor_launch_t<PRE_F16_NCHW, false>(src, d_tab, n, dst, net_h, net_w, s); break;
+    case PRE_F16_NCHW * 2 + 1: letterbox_tensor_launch_t<PRE_F16_NCHW, true>(src, d_tab, n, dst, net_h, net_w, s); break;
+    case PRE_U8_NHWC * 2: letterbox_tensor_launch_t<PRE_U8_NHWC, false>(src, d_tab, n, dst, net_h, net_w, s); break;
+    case PRE_U8_NHWC * 2 + 1: letterbox_tensor_launch_t<PRE_U8_NHWC, true>(src, d_tab, n, dst, net_h, net_w, s); break;
+    default: return cudaErrorInvalidValue;
+  }
   return cudaGetLastError();
 }
 

@@ -575,6 +575,32 @@ CTD_API int ctd_submit_outputs(ctd_handle* h, int32_t slot, const ctd_page_entry
                                const ctd_net_output* outs, int32_t refine_mode, int32_t keep_undetected,
                                int32_t textheight, int32_t results_on_device, void* results_host);
 
+/* ---- the detector's pre-processing: the network input preprocess_img makes ---------------------------------------
+ * ctd_preprocess_pages writes, for every page of a batch, what the reference's `preprocess_img(img, (net_h, net_w))`
+ * (inference.py:72-83) makes of it, into the caller's device buffer `dst`, in one launch: the letterbox (cv2.resize
+ * INTER_LINEAR when the size changes, bit-exact, zero padding at the bottom and the right) in one of three layouts
+ *   CTD_PRE_F32_NCHW: float32 [n][3][net_h][net_w], each u8 value v as v / 255 (the correctly rounded float32 division)
+ *   CTD_PRE_F16_NCHW: float16 [n][3][net_h][net_w], that float32 value rounded to nearest even (`.half()`)
+ *   CTD_PRE_U8_NHWC:  u8 [n][net_h][net_w][3], the letterboxed pixels (`to_tensor=False`)
+ * reverse_channels != 0: output channel k is channel 2 - k of the page.  preprocess_img's planes come out in the page's
+ * order with bgr2rgb (cvtColor, then `[::-1]`) and reversed without it; its to_tensor=False pixels the other way round.
+ *   pages / n:  the ctd_pages_plan entries for (net_h, net_w) (checked against a fresh plan); page i from input_host at
+ *               its page_off (pinned: input_bytes of the plan) or from device memory (dev, NULL or n entries, as
+ *               ctd_submit_pages takes them; the stream waits on each page's event), packed by one gather launch.
+ *   dst:        device memory of the handle's GPU, 16-byte aligned, n * 3 * net_h * net_w elements, contiguous.
+ *   stream:     a cudaStream_t of the handle's GPU (NULL: the legacy default stream).
+ * Everything is enqueued on `stream`: the host pages' copy, the waits, the gather and the letterbox; nothing waits on
+ * the host, and the call returns before the GPU work runs.  input_host and the device pages must stay unwritten until
+ * the stream has run it.  The handle's page buffer and tables are reused by the next call after an event wait on the
+ * stream of this one.  No network runs: a handle of any program (a kernels-only one too) takes it.  Refused before any
+ * GPU work: n > max_batch (CTD_E_CAPACITY), a net side that is not a positive multiple of 64 and a page that
+ * letterboxes to 0 px (CTD_E_SHAPE), entries that are not the plan's, a device page or a dst that is not memory of
+ * the handle's GPU, a dst that is not 16-byte aligned and a format that is not CTD_PRE_* (CTD_E_INVALID).          */
+enum ctd_pre_format { CTD_PRE_F32_NCHW = 0, CTD_PRE_F16_NCHW = 1, CTD_PRE_U8_NHWC = 2 };
+CTD_API int ctd_preprocess_pages(ctd_handle* h, const ctd_page_entry* pages, int32_t n, int32_t net_h, int32_t net_w,
+                                 const uint8_t* input_host, const ctd_device_page* dev, int32_t format,
+                                 int32_t reverse_channels, void* dst, void* stream);
+
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
  * [rows][5+nc]); output as ctd_get_detections for one page.                                */
 CTD_API int ctd_nms(ctd_handle* h, const float* pred, int32_t rows, float conf_thresh, float iou_thresh, float* det,
