@@ -23,13 +23,18 @@ class TextDetBase:
 
     model_path: a checkpoint path (the 3-key dict of utils/export.py) or that dict itself.  BatchNorm layers are
     always folded into their convolutions and the network runs in the engine's `precision` (default fp16 tensor
-    cores), so `half` and `fuse` are accepted for the reference's signature only.  max_batch and max_size (an int or
-    (h, w), multiples of 64) size the engine's workspace: the largest batch and page a call may pass.
+    cores), so `fuse` is accepted for the reference's signature only.  max_batch and max_size (an int or (h, w),
+    multiples of 64) size the engine's workspace: the largest batch and page a call may pass.
 
     The outputs are float32 CUDA tensors on `device`, fresh per call and without autograd history:
     blks [N][A][5 + nc] (A = 3 * (H/8 * W/8 + H/16 * W/16 + H/32 * W/32), yolo.py:44), mask [N][1][H][W] and
     lines_map [N][2][H][W].  For an input x = u8 / 255 they are bit for bit what `Engine.forward` on the u8 pages
-    gives; any other float input is rounded to fp16 in the fp16 engine and used exactly in the fp32 and split ones."""
+    gives; any other float input is rounded to fp16 in the fp16 engine and used exactly in the fp32 and split ones.
+
+    half=True is the reference's `.half()` module: forward also takes a float16 img_in (`preprocess_img(half=True)`)
+    and then returns float16 outputs, `tuple(t.half() for t in forward(img_in.float()))` bit for bit (the input is
+    widened exactly, the float32 outputs rounded to nearest even on the GPU, `ctd_forward_tensor_f16`).  A float32
+    img_in gives float32 outputs either way."""
 
     def __init__(self, model_path, device='cuda', half=False, fuse=False, act='leaky', precision=None, max_batch=1,
                  max_size=1024):
@@ -70,8 +75,8 @@ class TextDetBase:
             raise ValueError("img_in must be a torch tensor, got %s" % type(img_in).__name__)
         if not img_in.is_cuda or img_in.device.index != self.device.index:
             raise ValueError("img_in must be on %s, got %s" % (self.device, img_in.device))
-        if img_in.dtype != torch.float32:
-            raise ValueError("img_in must be float32, got %s" % img_in.dtype)
+        if img_in.dtype != torch.float32 and not (self.half and img_in.dtype == torch.float16):
+            raise ValueError("img_in must be float32%s, got %s" % (" or float16" if self.half else "", img_in.dtype))
         if img_in.dim() != 4 or img_in.shape[1] != 3:
             raise ValueError("img_in must be [N][3][H][W], got %s" % (tuple(img_in.shape),))
         n, _, h, w = img_in.shape
@@ -82,8 +87,9 @@ class TextDetBase:
                              % (h, w, self.max_size[0], self.max_size[1]))
 
     def forward(self, img_in):
-        """img_in: float32 [N][3][H][W] BGR on this module's device -> (blks, mask, lines_map), enqueued on the
-        device's current stream.  Raises ValueError, before any GPU work, for any other tensor."""
+        """img_in: float32 (with half also float16) [N][3][H][W] BGR on this module's device -> (blks, mask,
+        lines_map) of img_in's dtype, enqueued on the device's current stream.  Raises ValueError, before any GPU
+        work, for any other tensor."""
         import torch
         self._check(img_in)
         n, _, h, w = img_in.shape
@@ -92,11 +98,12 @@ class TextDetBase:
             x = x.clone()
         rows = 3 * ((h // 8) * (w // 8) + (h // 16) * (w // 16) + (h // 32) * (w // 32))
         stream = torch.cuda.current_stream(self.device)
-        blks = torch.empty((n, rows, 5 + self.nc), dtype=torch.float32, device=self.device)
-        mask = torch.empty((n, 1, h, w), dtype=torch.float32, device=self.device)
-        lines = torch.empty((n, 2, h, w), dtype=torch.float32, device=self.device)
+        dt = x.dtype
+        blks = torch.empty((n, rows, 5 + self.nc), dtype=dt, device=self.device)
+        mask = torch.empty((n, 1, h, w), dtype=dt, device=self.device)
+        lines = torch.empty((n, 2, h, w), dtype=dt, device=self.device)
         self.engine.forward_tensor(x.data_ptr(), n, h, w, stream.cuda_stream, blks.data_ptr(), mask.data_ptr(),
-                                   lines.data_ptr())
+                                   lines.data_ptr(), half=dt == torch.float16)
         return blks, mask, lines
 
     __call__ = forward

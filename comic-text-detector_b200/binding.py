@@ -108,14 +108,20 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
            "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
            "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot", "ctd_submit_outputs",
-           "ctd_preprocess_pages"]
+           "ctd_preprocess_pages", "ctd_submit_outputs_dtype", "ctd_forward_tensor_f16"]
 PRE_F32_NCHW, PRE_F16_NCHW, PRE_U8_NHWC = 0, 1, 2   # ctd_pre_format
+DTYPE_F32, DTYPE_F16 = 0, 1   # ctd_dtype
 
 _lib = None
 
 
 class CtdError(RuntimeError):
     pass
+
+
+def _is_f16(m):
+    """a float16 numpy array or torch tensor"""
+    return str(m.dtype) in ("float16", "torch.float16")
 
 
 def load_library():
@@ -137,6 +143,7 @@ def load_library():
     lib.ctd_forward.argtypes = [vp, vp, i32, i32, i32, i32]
     lib.ctd_get_net_outputs.argtypes = [vp, vp, vp, vp]
     lib.ctd_forward_tensor.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp]
+    lib.ctd_forward_tensor_f16.argtypes = [vp, vp, i32, i32, i32, vp, vp, vp, vp]
     lib.ctd_get_mask_u8.argtypes = [vp, vp]
     lib.ctd_get_detections.argtypes = [vp, vp, vp]
     lib.ctd_get_db_components.argtypes = [vp, vp, vp, vp]
@@ -175,6 +182,7 @@ def load_library():
     lib.ctd_submit_regions.argtypes = [vp, i32, vp, i32, vp, vp, i32, vp, vp, i32]
     lib.ctd_debug_read_slot.argtypes = [vp, i32, i32, C.c_size_t, vp, C.c_size_t]
     lib.ctd_submit_outputs.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, vp, i32, i32, i32, i32, vp]
+    lib.ctd_submit_outputs_dtype.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp]
     lib.ctd_preprocess_pages.argtypes = [vp, vp, i32, i32, i32, vp, vp, i32, i32, vp, vp]
     lib.ctd_jpeg_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdJpegInfo)]
     lib.ctd_jpeg_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
@@ -372,14 +380,14 @@ class Engine:
         self._ck(self.lib.ctd_forward(self.h, C.c_void_p(dev_ptr), n, h, w, 1))
         self.shape = (n, h, w)
 
-    def forward_tensor(self, x_ptr, n, h, w, stream, blks_ptr, mask_ptr, lines_ptr):
+    def forward_tensor(self, x_ptr, n, h, w, stream, blks_ptr, mask_ptr, lines_ptr, half=False):
         """`ctd_forward_tensor`: the forward of a float32 NCHW [n][3][h][w] device tensor (pointer as int, 16-byte
         aligned) into caller-allocated device outputs (pointers as int, or None), ordered after the work enqueued on
         `stream` (a cudaStream_t as int; 0 is the legacy default stream), which then waits for the outputs.  No host
-        synchronisation."""
+        synchronisation.  half: the input and the outputs are float16 (`ctd_forward_tensor_f16`)."""
         vp = C.c_void_p
-        self._ck(self.lib.ctd_forward_tensor(self.h, vp(x_ptr), n, h, w, vp(stream), vp(blks_ptr), vp(mask_ptr),
-                                             vp(lines_ptr)))
+        fn = self.lib.ctd_forward_tensor_f16 if half else self.lib.ctd_forward_tensor
+        self._ck(fn(self.h, vp(x_ptr), n, h, w, vp(stream), vp(blks_ptr), vp(mask_ptr), vp(lines_ptr)))
         self.shape = (n, h, w)
 
     def rows_per_image(self):
@@ -607,10 +615,11 @@ class Engine:
 
     def submit_outputs(self, slot, pages, outs, net_h, net_w, refine_mode=0, keep_undetected=False, textheight=0,
                        events=None, device_results=False):
-        """asynchronous post-processing of a batch of pages from the caller's network outputs (ctd_submit_outputs):
-        pages as submit_pages takes them; outs[i] = (blks [A][5 + nc], mask [net_h][net_w], lines [net_h][net_w])
-        of page i, each a float32 numpy array (copied into this slot's pinned output buffer) or a float32 CUDA tensor on
-        this engine's GPU with any strides (read where it is).  events[i] (a recorded torch.cuda.Event, or None) is
+        """asynchronous post-processing of a batch of pages from the caller's network outputs
+        (ctd_submit_outputs_dtype): pages as submit_pages takes them; outs[i] = (blks [A][5 + nc], mask [net_h][net_w],
+        lines [net_h][net_w]) of page i, each a numpy array (copied into this slot's pinned output buffer) or a CUDA
+        tensor on this engine's GPU with any strides (read where it is), all three float32 or all three float16 (the
+        page is then post-processed with the reference's half arithmetic).  events[i] (a recorded torch.cuda.Event, or None) is
         waited on before CUDA page i and CUDA outputs i are read; the CUDA pages and outputs are referenced until the
         slot is collected and must not be written before.  Collect with collect_pages(slot)."""
         import torch
@@ -628,7 +637,7 @@ class Engine:
             page = []
             for m, md in zip(o, d):
                 page.append(None if md else need)
-                need += 0 if md else (m.size * 4 + 255) // 256 * 256
+                need += 0 if md else (m.size * m.itemsize + 255) // 256 * 256
             offs.append(page)
         if not hasattr(self, "_out_bufs"):
             self._out_bufs = [None, None]
@@ -645,6 +654,7 @@ class Engine:
                     o = int(e["page_off"])
                     np.copyto(inp[o:o + p.size].reshape(p.shape), p)
         rec = (CtdNetOutput * len(outs))()
+        dtypes = (C.c_int32 * len(outs))(*[DTYPE_F16 if _is_f16(o[0]) else DTYPE_F32 for o in outs])
         obuf = self._out_bufs[slot].numpy() if need else None
         base = self._out_bufs[slot].data_ptr() if need else 0
         for i, (o, d, off) in enumerate(zip(outs, o_dev, offs)):
@@ -654,19 +664,19 @@ class Engine:
                     st = m.stride()
                     fields.append((m.data_ptr(), st[0], st[1] if len(st) > 1 else 1, 1))
                 else:
-                    np.copyto(obuf[mo:mo + m.size * 4].view(np.float32).reshape(m.shape), m)
+                    np.copyto(obuf[mo:mo + m.size * m.itemsize].view(m.dtype).reshape(m.shape), m)
                     fields.append((base + mo, m.shape[1] if m.ndim > 1 else 1, 1, 0))
             (bp, bsr, bsc, bd), (mp, msh, msw, md_), (lp, lsh, lsw, ld) = fields
             ev = events[i] if events is not None else None
             rec[i] = CtdNetOutput(bp, bsr, bsc, mp, msh, msw, lp, lsh, lsw, int(o[0].shape[0]), bd, md_, ld,
                                   ev.cuda_event if ev is not None else None)
         dev = _device_images(pages, on_dev, events, 3)
-        self._ck(self.lib.ctd_submit_outputs(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
-                                             None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
-                                             None if dev is None else C.cast(dev, C.c_void_p),
-                                             C.cast(rec, C.c_void_p), int(refine_mode), int(bool(keep_undetected)),
-                                             int(textheight), int(bool(device_results)),
-                                             C.c_void_p(bufs[1].data_ptr())))
+        self._ck(self.lib.ctd_submit_outputs_dtype(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
+                                                   None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
+                                                   None if dev is None else C.cast(dev, C.c_void_p),
+                                                   C.cast(rec, C.c_void_p), C.cast(dtypes, C.c_void_p),
+                                                   int(refine_mode), int(bool(keep_undetected)), int(textheight),
+                                                   int(bool(device_results)), C.c_void_p(bufs[1].data_ptr())))
         kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]] + \
                [(m, None if events is None else events[i]) for i, o in enumerate(outs) for m, md in zip(o, o_dev[i])
                 if md]

@@ -457,9 +457,9 @@ static int run_one_op(ctd_handle* h, size_t i, int n, int ph, int pw, const Shap
 }
 
 // NMS of the Detect rows
-int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
+int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt, const int32_t* half) {
   CK(nms_launch(h->d_blks, n, rows_per_image(ph, pw), h->cfg.nc, h->cfg.conf_thresh, h->cfg.nms_thresh, h->nms, h->d_det,
-                h->d_det_count, s));
+                h->d_det_count, s, half));
   *cnt += kNmsLaunches;
   return CTD_OK;
 }
@@ -597,8 +597,30 @@ extern "C" int ctd_forward(ctd_handle* h, const uint8_t* pages, int32_t n, int32
   return enqueue_forward(h, n, ph, pw, *sp);
 }
 
-extern "C" int ctd_forward_tensor(ctd_handle* h, const float* x, int32_t n, int32_t ph, int32_t pw, void* stream,
-                                  float* blks, float* mask, float* lines) {
+// float32 -> T, round to nearest even for __half
+template <typename T>
+__global__ void from_f32_kernel(const float* src, T* dst, size_t n) {
+  size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
+  if (i < n) dst[i] = T(src[i]);
+}
+
+// a workspace output of the forward into the caller's tensor: a copy (X = float), or rounded to nearest even (__half)
+template <typename X>
+static int copy_output(ctd_handle* h, X* dst, const float* src, size_t elems) {
+  if constexpr (sizeof(X) == 4) {
+    CK(cudaMemcpyAsync(dst, src, elems * 4, cudaMemcpyDeviceToDevice, h->stream));
+  } else {
+    from_f32_kernel<__half><<<unsigned((elems + 255) / 256), 256, 0, h->stream>>>(src, dst, elems);
+    CK(cudaGetLastError());
+  }
+  return CTD_OK;
+}
+
+// ctd_forward_tensor (X = float) and ctd_forward_tensor_f16 (X = __half): the input pre-pass from an X tensor, the
+// forward, and the outputs as X
+template <typename X>
+static int forward_tensor(ctd_handle* h, const X* x, int32_t n, int32_t ph, int32_t pw, void* stream, X* blks, X* mask,
+                          X* lines) {
   if (!h || !x) return CTD_E_INVALID;
   if (reinterpret_cast<uintptr_t>(x) % 16) return ctd_fail(h, CTD_E_INVALID, "x must be 16-byte aligned");
   ShapePlan* sp = nullptr;
@@ -614,13 +636,25 @@ extern "C" int ctd_forward_tensor(ctd_handle* h, const float* x, int32_t n, int3
   if (int rc = enqueue_forward(h, n, ph, pw, *sp)) return rc;
   const size_t px = size_t(n) * ph * pw;
   if (blks)
-    CK(cudaMemcpyAsync(blks, h->d_blks, size_t(n) * rows_per_image(ph, pw) * (5 + h->cfg.nc) * 4,
-                       cudaMemcpyDeviceToDevice, h->stream));
-  if (mask) CK(cudaMemcpyAsync(mask, h->d_mask, px * 4, cudaMemcpyDeviceToDevice, h->stream));
-  if (lines) CK(cudaMemcpyAsync(lines, h->d_lines, px * 8, cudaMemcpyDeviceToDevice, h->stream));
+    if (int rc = copy_output(h, blks, h->d_blks, size_t(n) * rows_per_image(ph, pw) * (5 + h->cfg.nc))) return rc;
+  if (mask)
+    if (int rc = copy_output(h, mask, h->d_mask, px)) return rc;
+  if (lines)
+    if (int rc = copy_output(h, lines, h->d_lines, px * 2)) return rc;
   CK(cudaEventRecord(h->ev_tout, h->stream));
   CK(cudaStreamWaitEvent(cs, h->ev_tout, 0));
   return CTD_OK;
+}
+
+extern "C" int ctd_forward_tensor(ctd_handle* h, const float* x, int32_t n, int32_t ph, int32_t pw, void* stream,
+                                  float* blks, float* mask, float* lines) {
+  return forward_tensor(h, x, n, ph, pw, stream, blks, mask, lines);
+}
+
+extern "C" int ctd_forward_tensor_f16(ctd_handle* h, const void* x, int32_t n, int32_t ph, int32_t pw, void* stream,
+                                      void* blks, void* mask, void* lines) {
+  return forward_tensor(h, static_cast<const __half*>(x), n, ph, pw, stream, static_cast<__half*>(blks),
+                        static_cast<__half*>(mask), static_cast<__half*>(lines));
 }
 
 template <bool kPinned>
@@ -844,12 +878,6 @@ extern "C" int ctd_debug_read_buffer(ctd_handle* h, int32_t buf, float* out, siz
   cudaFree(tmp);
   CK(e);
   return CTD_OK;
-}
-
-template <typename T>
-__global__ void from_f32_kernel(const float* src, T* dst, size_t n) {
-  size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
-  if (i < n) dst[i] = T(src[i]);
 }
 
 extern "C" int ctd_debug_write_buffer(ctd_handle* h, int32_t buf, const float* in, int32_t n, int32_t ph, int32_t pw) {

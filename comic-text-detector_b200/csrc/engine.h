@@ -281,7 +281,8 @@ struct ctd_handle {
   bool pipe_quit = false;
   int host_threads = 4;
   size_t pg_gather_off = 0;
-  size_t pg_out_off = 0, pg_flag_off = 0;   // the OutputGather table and the non-finite flags in the page tables
+  // the OutputGather table, its float16 flags and the non-finite flags in the page tables
+  size_t pg_out_off = 0, pg_half_off = 0, pg_flag_off = 0;
   cudaStream_t dev_out = nullptr;   // the stream ctd_collect_device copies on
   // the worker's phase C on the post stream: its own connected-components and refine scratch (refine_scratch and
   // cc_scratch belong to the caller's stream)
@@ -307,8 +308,9 @@ int enqueue_forward(ctd_handle* h, int32_t n, int32_t ph, int32_t pw, ShapePlan&
 // Detect rows per page of a ph x pw net input (yolo.py:44), the rows of d_blks per page
 int rows_per_image(int ph, int pw);
 // the forward's post-processing on the engine workspaces, n pages of ph x pw, on stream s (cnt += the launches):
-// NMS of d_blks into the arena's detections, and connected components + text-line boxes of d_bitmap / d_lines
-int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt);
+// NMS of d_blks into the arena's detections (half: NULL, or per page the float16 flag of nms_launch), and connected
+// components + text-line boxes of d_bitmap / d_lines
+int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt, const int32_t* half = nullptr);
 int launch_db_post(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt);
 // connected components + stats of a DEVICE u8 image on the engine stream (grow-on-demand scratch): *d_stats points at
 // [stats_cap][5] ints on the device, *n_labels is read back (synchronises the stream)

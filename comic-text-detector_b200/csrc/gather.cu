@@ -4,11 +4,15 @@
 // refine_mask and the crop kernels read it; in the same launch, the batch's masks in device memory (u8 [ih][iw], any
 // strides: a channel of a page) into its packed mask plane.  One CTA per row over the stacked rows of the gathered
 // images, as backproject_batch_kernel.
-// gather_outputs_kernel is the ingest of ctd_submit_outputs: a caller's network outputs (float32, any strides) staged
-// into the engine's post-processing workspace in one launch, with postprocess_mask's u8 cast and the DB threshold fused.
+// gather_outputs_kernel is the ingest of ctd_submit_outputs: a caller's network outputs (float32 or float16, any
+// strides) staged into the engine's post-processing workspace in one launch, with postprocess_mask's u8 cast and the DB
+// threshold fused.
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include "kernels.h"
 
@@ -78,16 +82,75 @@ constexpr int kBlkPerThread = 8;   // blks elements per thread of a blks CTA
 
 __device__ __forceinline__ bool finite_f(float v) { return (__float_as_uint(v) & 0x7f800000u) != 0x7f800000u; }
 
-// postprocess_mask's `(p * 255).astype(np.uint8)` on float32 p: the product rounded to float32, truncated to int32
-// (0x80000000 where it does not fit, as cvttss2si gives it), and the low byte of that
+__device__ __forceinline__ float widen(float v) { return v; }
+__device__ __forceinline__ float widen(__half v) { return __half2float(v); }
+__device__ __forceinline__ float round_half(float v) { return __half2float(__float2half_rn(v)); }
+
+// postprocess_mask's `(p * 255).astype(np.uint8)`: the product rounded to float32 (T = float) or, on a float16 map, to
+// float16 (numpy's half arithmetic: the float product of two halves is exact, so rounding it once is RN_half of the
+// exact product), truncated to int32 (0x80000000 where it does not fit, as cvttss2si gives it; numpy casts a half
+// through float), and the low byte of that
+template <typename T>
 __device__ __forceinline__ uint32_t mask_byte(float p) {
-  const float v = __fmul_rn(p, 255.f);
+  float v = __fmul_rn(p, 255.f);
+  if constexpr (sizeof(T) == 2) v = round_half(v);
   return (v >= -2147483648.f && v < 2147483648.f) ? uint32_t(__float2int_rz(v)) & 0xffu : 0u;
 }
 
-// grid (h + blks CTAs per page, n).  CTA x < h: row x of the page's mask and lines channel 0 (16-byte loads when the
-// row is contiguous and 16-byte aligned, else one strided element per thread); the others: kBlkPerThread * 256 blks
-// elements each, in row-major order of the workspace rows
+// 4 consecutive elements of a row, one aligned load: 16 bytes of float, 8 of __half
+template <typename T>
+using Vec4 = typename std::conditional<sizeof(T) == 4, uint4, uint2>::type;
+
+// row y of one page's mask and lines channel 0 of element T into the staging planes: 4 elements per thread and load
+// (16 bytes of f32, 8 of f16, so every thread of a 1024-wide row has work at either size) when both rows are
+// contiguous and aligned to a load, else one strided element per thread.  thresh is the DB threshold in the page's
+// precision.  Returns the non-finite bits (2: mask, 4: lines).
+template <typename T>
+__device__ __forceinline__ uint32_t gather_row(const OutputGather& g, int y, int w, float thresh, uint8_t* __restrict__ mo,
+                                               uint8_t* __restrict__ bo, float* __restrict__ lo) {
+  using V = Vec4<T>;
+  const T* ms = static_cast<const T*>(g.mask) + y * g.msh;
+  const T* ls = static_cast<const T*>(g.lines) + y * g.lsh;
+  uint32_t bad = 0;
+  const bool vec = g.msw == 1 && g.lsw == 1 && (w & 3) == 0 && ((uintptr_t(ms) | uintptr_t(ls)) & (sizeof(V) - 1)) == 0;
+  if (vec) {
+    for (int x4 = threadIdx.x; x4 < (w >> 2); x4 += kOutThreads) {
+      const V mr = __ldg(reinterpret_cast<const V*>(ms) + x4);
+      const V lr = __ldg(reinterpret_cast<const V*>(ls) + x4);
+      T mv[4], lv[4];
+      memcpy(mv, &mr, sizeof(V));
+      memcpy(lv, &lr, sizeof(V));
+      uint32_t mb = 0, bb = 0;
+      float lf[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float m = widen(mv[k]);
+        lf[k] = widen(lv[k]);
+        if (finite_f(m)) mb |= mask_byte<T>(m) << (8 * k);
+        else bad |= 2;
+        if (!finite_f(lf[k])) { bad |= 4; lf[k] = 0.f; }
+        bb |= uint32_t(lf[k] > thresh) << (8 * k);
+      }
+      reinterpret_cast<uint32_t*>(mo)[x4] = mb;
+      reinterpret_cast<uint32_t*>(bo)[x4] = bb;
+      reinterpret_cast<float4*>(lo)[x4] = make_float4(lf[0], lf[1], lf[2], lf[3]);
+    }
+  } else {
+    for (int x = threadIdx.x; x < w; x += kOutThreads) {
+      const float m = widen(ms[x * g.msw]);
+      float l = widen(ls[x * g.lsw]);
+      if (!finite_f(m)) bad |= 2;
+      if (!finite_f(l)) { bad |= 4; l = 0.f; }
+      mo[x] = finite_f(m) ? uint8_t(mask_byte<T>(m)) : 0;
+      bo[x] = l > thresh ? 1 : 0;
+      lo[x] = l;
+    }
+  }
+  return bad;
+}
+
+// grid (h + blks CTAs per page, n).  CTA x < h: row x of the page's mask and lines channel 0 (gather_row, in the
+// page's dtype); the others: kBlkPerThread * 256 blks elements each, in row-major order of the workspace rows
 __global__ void __launch_bounds__(kOutThreads) gather_outputs_kernel(const OutputGather* __restrict__ tab, int h, int w,
                                                                      int no, int ws_rows, float thresh,
                                                                      uint8_t* __restrict__ mask_u8,
@@ -101,41 +164,9 @@ __global__ void __launch_bounds__(kOutThreads) gather_outputs_kernel(const Outpu
   if (int(blockIdx.x) < h) {
     const int y = blockIdx.x;
     const size_t o = (size_t(page) * h + y) * w;
-    const float* ms = g.mask + y * g.msh;
-    const float* ls = g.lines + y * g.lsh;
-    uint8_t* mo = mask_u8 + o;
-    uint8_t* bo = bitmap + o;
     float* lo = lines + size_t(page) * 2 * h * w + size_t(y) * w;
-    const bool vec = g.msw == 1 && g.lsw == 1 && (w & 3) == 0 && ((uintptr_t(ms) | uintptr_t(ls)) & 15) == 0;
-    if (vec) {
-      for (int x4 = threadIdx.x; x4 < (w >> 2); x4 += kOutThreads) {
-        const float4 m = __ldg(reinterpret_cast<const float4*>(ms) + x4);
-        float4 l = __ldg(reinterpret_cast<const float4*>(ls) + x4);
-        const float mv[4] = {m.x, m.y, m.z, m.w};
-        float* lv[4] = {&l.x, &l.y, &l.z, &l.w};
-        uint32_t mb = 0, bb = 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          if (finite_f(mv[k])) mb |= mask_byte(mv[k]) << (8 * k);
-          else bad |= 2;
-          if (!finite_f(*lv[k])) { bad |= 4; *lv[k] = 0.f; }
-          bb |= uint32_t(*lv[k] > thresh) << (8 * k);
-        }
-        reinterpret_cast<uint32_t*>(mo)[x4] = mb;
-        reinterpret_cast<uint32_t*>(bo)[x4] = bb;
-        reinterpret_cast<float4*>(lo)[x4] = l;
-      }
-    } else {
-      for (int x = threadIdx.x; x < w; x += kOutThreads) {
-        const float m = ms[x * g.msw];
-        float l = ls[x * g.lsw];
-        if (!finite_f(m)) bad |= 2;
-        if (!finite_f(l)) { bad |= 4; l = 0.f; }
-        mo[x] = finite_f(m) ? uint8_t(mask_byte(m)) : 0;
-        bo[x] = l > thresh ? 1 : 0;
-        lo[x] = l;
-      }
-    }
+    bad = g.half ? gather_row<__half>(g, y, w, round_half(thresh), mask_u8 + o, bitmap + o, lo)
+                 : gather_row<float>(g, y, w, thresh, mask_u8 + o, bitmap + o, lo);
   } else {
     const size_t total = size_t(ws_rows) * no;
     const size_t e0 = size_t(blockIdx.x - h) * kOutThreads * kBlkPerThread;
@@ -147,7 +178,8 @@ __global__ void __launch_bounds__(kOutThreads) gather_outputs_kernel(const Outpu
       const int r = int(e / no), c = int(e - size_t(r) * no);
       float v;
       if (r < g.rows) {
-        v = g.blks[r * g.bsr + c * g.bsc];
+        const long long i = r * g.bsr + c * g.bsc;
+        v = g.half ? __half2float(static_cast<const __half*>(g.blks)[i]) : static_cast<const float*>(g.blks)[i];
         if (!finite_f(v)) { bad |= 1; v = 0.f; }
       } else {
         v = c == 4 ? __int_as_float(0x7fc00000) : 0.f;   // NaN objectness: `obj > conf_thres` is false

@@ -162,10 +162,11 @@ cudaError_t conv_simt_launch(const ConvSimtParams& p, cudaStream_t s);
 template <typename T, typename P>
 cudaError_t stem_launch(const P* pages, int n, int h, int w, const float* wgt /*[32][108] (ky,kx,c)*/,
                         const float* bias, T* dst, int dst_cstride, int dst_coff, int cout, int act, cudaStream_t s);
-// the input pre-pass of ctd_forward_tensor: f32 NCHW [n][3][h][w] -> the HWC staging page [n][h][w][3] of element S
-// (__half: round to nearest; float: a copy)
-template <typename S>
-cudaError_t nchw_to_hwc_launch(const float* x, int n, int h, int w, S* dst, cudaStream_t s);
+// the input pre-pass of ctd_forward_tensor (X = float) and ctd_forward_tensor_f16 (X = __half): NCHW [n][3][h][w] of
+// element X -> the HWC staging page [n][h][w][3] of element S.  Each value is widened exactly to float, then stored as
+// S (__half: round to nearest; float: a copy), so an f16 input stages exactly what its float32 copy does.
+template <typename X, typename S>
+cudaError_t nchw_to_hwc_launch(const X* x, int n, int h, int w, S* dst, cudaStream_t s);
 // fp32 NHWC channel slice -> fp16 hi / lo planes (split-fp16 mode): hi = fp16(x), lo = fp16((x - hi) * kSplitLoScale).
 // src / hi / lo point at the first channel of the slice; `cstride` elements between pixels (same in all three).
 cudaError_t split_planes_launch(const float* src, __half* hi, __half* lo, size_t npix, int c, int cstride,
@@ -198,8 +199,11 @@ struct NmsWorkspace {
   unsigned long long* mask;  // [n][cap][cap/64]
   int cap;
 };
+// half (NULL, or one flag per page): where half[i] != 0 the rows of page i are float16 values widened to float, and its
+// candidates follow non_max_suppression on half tensors: `obj > half(conf)`, class scores RN_half(cls * obj), the best
+// kept where `> half(conf)`, corners RN_half(cx -/+ RN_half(w / 2)) (yolov5_utils.py:136,169-180 in float16 arithmetic)
 cudaError_t nms_launch(const float* blks, int n, int rows, int nc, float conf, float iou, NmsWorkspace& ws,
-                       float* det /*[n][300][6]*/, int* det_count, cudaStream_t s);
+                       float* det /*[n][300][6]*/, int* det_count, cudaStream_t s, const int32_t* half = nullptr);
 constexpr int kNmsLaunches = 5;   // kernels nms_launch enqueues
 size_t nms_workspace_bytes(int n, int cap);
 void nms_workspace_bind(NmsWorkspace& ws, void* base, int n, int cap);
@@ -267,24 +271,26 @@ cudaError_t gather_pages_launch(const GatherPage* d_tab, int n, int total_rows, 
 // staging buffer or host wait orders the copy (ctd_preprocess_pages)
 cudaError_t upload_table_launch(const void* host, size_t bytes, void* dst, cudaStream_t s);
 
-// A caller's network outputs for one page (ctd_submit_outputs), all in device memory, float32, element strides:
-// blks (r, c) at blks + r * bsr + c * bsc for r < rows, c < no; mask (y, x) at mask + y * msh + x * msw; channel 0 of
-// lines_map (y, x) at lines + y * lsh + x * lsw.
+// A caller's network outputs for one page (ctd_submit_outputs), all in device memory, float32 (half == 0) or float16
+// (half == 1), element strides: blks (r, c) at blks + r * bsr + c * bsc for r < rows, c < no; mask (y, x) at mask +
+// y * msh + x * msw; channel 0 of lines_map (y, x) at lines + y * lsh + x * lsw.
 struct OutputGather {
-  const float* blks;
+  const void* blks;
   long long bsr, bsc;
-  const float* mask;
+  const void* mask;
   long long msh, msw;
-  const float* lines;
+  const void* lines;
   long long lsh, lsw;
-  int rows, pad;
+  int rows, half;
 };
 // One launch over the n pages of d_tab (gather.cu), each h x w: per page the u8 mask `(uint8_t)(int32_t)truncf(p *
 // 255.f)` (0 where the product is outside int32: numpy's float32 -> uint8 cast on x86-64) into mask_u8, channel 0 of
 // lines_map into lines (page stride 2 * h * w floats, where segrep reads it), the DB bitmap `p > thresh` into bitmap,
 // and the blks rows into blks at ws_rows rows per page, rows past `rows` padded with NaN objectness (never a
-// candidate).  flags[i] (zeroed by the caller) gets bit 0 / 1 / 2 for a non-finite value in page i's blks / mask /
-// lines; such a value is staged as 0.
+// candidate).  A float16 page does postprocess_mask and the binarize in half, as the reference does on half tensors:
+// the mask byte from the product rounded to half, `p > half(thresh)`; its lines plane and blks rows are the half
+// values widened exactly to float.  flags[i] (zeroed by the caller) gets bit 0 / 1 / 2 for a non-finite value in page
+// i's blks / mask / lines; such a value is staged as 0.
 cudaError_t gather_outputs_launch(const OutputGather* d_tab, int n, int h, int w, int no, int ws_rows, float thresh,
                                   uint8_t* mask_u8, float* lines, uint8_t* bitmap, float* blks, int32_t* flags,
                                   cudaStream_t s);

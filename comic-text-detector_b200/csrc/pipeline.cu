@@ -864,15 +864,17 @@ static int check_device_image(ctd_handle* h, const char* what, int i, const ctd_
 }
 
 // the slot's page tables, allocated at its first batch: max_batch PageGeom entries, then at pg_gather_off room for a
-// GatherPage entry per page and per mask of a batch, at pg_out_off an OutputGather entry per page (ctd_submit_outputs)
-// and at pg_flag_off its non-finite flags (device: written by the ingest; host: their copy back)
+// GatherPage entry per page and per mask of a batch, at pg_out_off an OutputGather entry per page (ctd_submit_outputs),
+// at pg_half_off its float16 flags (what NMS reads) and at pg_flag_off its non-finite flags (device: written by the
+// ingest; host: their copy back)
 static int ensure_page_tables(ctd_handle* h, Slot& s) {
   if (s.h_pg_tab) return CTD_OK;
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const size_t nb = size_t(h->cfg.max_batch);
   h->pg_gather_off = al(nb * sizeof(PageGeom));
   h->pg_out_off = al(h->pg_gather_off + 2 * nb * sizeof(GatherPage));
-  h->pg_flag_off = al(h->pg_out_off + nb * sizeof(OutputGather));
+  h->pg_half_off = al(h->pg_out_off + nb * sizeof(OutputGather));
+  h->pg_flag_off = al(h->pg_half_off + nb * sizeof(int32_t));
   const size_t tab_bytes = h->pg_flag_off + nb * sizeof(int32_t);
   CK(cudaHostAlloc(reinterpret_cast<void**>(&s.h_pg_tab), tab_bytes, cudaHostAllocDefault));
   CK(cudaMalloc(reinterpret_cast<void**>(&s.d_pg_tab), tab_bytes));
@@ -895,10 +897,11 @@ static int copy_host_runs(ctd_handle* h, const ctd_device_page* dev, int n, uint
   return CTD_OK;
 }
 
-// a network output map of page i (ctd_submit_outputs): device memory of the handle's GPU from its first to its last
-// element (strides in [0, 2^31]), or a host pointer, whose byte span [*lo, *lo + *bytes) is returned
-static int check_output_map(ctd_handle* h, const char* what, int i, const float* p, int on_device, int64_t s0,
-                            int64_t s1, int n0, int n1, size_t* bytes) {
+// a network output map of page i (ctd_submit_outputs), elements of esz bytes: device memory of the handle's GPU from
+// its first to its last element (strides in [0, 2^31]), or a host pointer, whose byte span [p, p + *bytes) is returned
+static int check_output_map(ctd_handle* h, const char* what, int i, const float* fp, size_t esz, int on_device,
+                            int64_t s0, int64_t s1, int n0, int n1, size_t* bytes) {
+  const char* p = reinterpret_cast<const char*>(fp);
   const int64_t kMaxStride = int64_t(1) << 31;
   *bytes = 0;
   if (n0 < 1 || n1 < 1) return CTD_OK;   // no element (blks with 0 rows)
@@ -906,23 +909,23 @@ static int check_output_map(ctd_handle* h, const char* what, int i, const float*
   if (s0 < 0 || s1 < 0 || s0 > kMaxStride || s1 > kMaxStride)
     return ctd_fail(h, CTD_E_INVALID, "page %d: %s strides (%lld, %lld) out of range [0, 2^31]", i, what, (long long)s0,
                     (long long)s1);
-  const float* last = p + (n0 - 1) * s0 + (n1 - 1) * s1;
+  const char* last = p + ((n0 - 1) * s0 + (n1 - 1) * s1) * int64_t(esz);
   if (on_device) {
     if (!is_device_memory(p, h->cfg.device) || !is_device_memory(last, h->cfg.device))
       return ctd_fail(h, CTD_E_INVALID, "page %d: %s (%p) is not device memory of GPU %d", i, what, (const void*)p,
                       h->cfg.device);
   } else {
-    *bytes = size_t(last - p + 1) * sizeof(float);
+    *bytes = size_t(last - p) + esz;
   }
   return CTD_OK;
 }
 
-// ctd_submit_pages, and with `outs` ctd_submit_outputs: the caller's network outputs staged in place of the letterbox
-// and the forward
+// ctd_submit_pages, and with `outs` ctd_submit_outputs_dtype: the caller's network outputs (page i in dtypes[i])
+// staged in place of the letterbox and the forward
 static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
                             int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
-                            const ctd_net_output* outs, int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
-                            int32_t results_on_device, void* results_host) {
+                            const ctd_net_output* outs, const int32_t* dtypes, int32_t refine_mode,
+                            int32_t keep_undetected, int32_t textheight, int32_t results_on_device, void* results_host) {
   const char* entry = outs ? "ctd_submit_outputs" : "ctd_submit_pages";
   if (!h || !pages || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
   if (textheight != 0 && textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
@@ -966,18 +969,21 @@ static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* p
                       h->cfg.max_w);
     for (int i = 0; i < n; ++i) {
       const ctd_net_output& o = outs[i];
+      if (dtypes[i] != CTD_DTYPE_F32 && dtypes[i] != CTD_DTYPE_F16)
+        return ctd_fail(h, CTD_E_INVALID, "page %d: dtype %d is not a CTD_DTYPE_* value", i, dtypes[i]);
+      const size_t esz = dtypes[i] == CTD_DTYPE_F16 ? 2 : 4;
       if (o.rows < 0 || o.rows > ws_rows)
         return ctd_fail(h, CTD_E_CAPACITY, "page %d: %d blks rows, the %dx%d workspace holds 0 to %d", i, o.rows, net_h,
                         net_w, ws_rows);
       auto& hb = host_bytes[size_t(i)];
-      if (int rc = check_output_map(h, "blks", i, o.blks, o.blks_on_device, o.blks_stride_r, o.blks_stride_c, o.rows,
-                                    no, &hb[0]))
+      if (int rc = check_output_map(h, "blks", i, o.blks, esz, o.blks_on_device, o.blks_stride_r, o.blks_stride_c,
+                                    o.rows, no, &hb[0]))
         return rc;
-      if (int rc = check_output_map(h, "mask", i, o.mask, o.mask_on_device, o.mask_stride_h, o.mask_stride_w, net_h,
-                                    net_w, &hb[1]))
+      if (int rc = check_output_map(h, "mask", i, o.mask, esz, o.mask_on_device, o.mask_stride_h, o.mask_stride_w,
+                                    net_h, net_w, &hb[1]))
         return rc;
-      if (int rc = check_output_map(h, "lines", i, o.lines, o.lines_on_device, o.lines_stride_h, o.lines_stride_w,
-                                    net_h, net_w, &hb[2]))
+      if (int rc = check_output_map(h, "lines", i, o.lines, esz, o.lines_on_device, o.lines_stride_h,
+                                    o.lines_stride_w, net_h, net_w, &hb[2]))
         return rc;
       for (int k = 0; k < 3; ++k) {
         host_off[size_t(i)][size_t(k)] = out_in_bytes;
@@ -1021,20 +1027,22 @@ static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* p
   // one copy per run of consecutive host pages); the device pages' events, the gather of the device pages, letterbox,
   // forward, back-projection and the phase-A rows on the engine stream; rows + masks out on copy_out
   OutputGather* otab = reinterpret_cast<OutputGather*>(reinterpret_cast<char*>(tab) + h->pg_out_off);
+  int32_t* half_tab = reinterpret_cast<int32_t*>(reinterpret_cast<char*>(tab) + h->pg_half_off);
   for (int i = 0; outs && i < n; ++i) {
     const ctd_net_output& o = outs[i];
     // a host map is read from its copy in out_in, at the same strides
-    auto at = [&](const float* p, int k) {
-      return host_bytes[size_t(i)][size_t(k)] ? reinterpret_cast<const float*>(s.out_in.p + host_off[size_t(i)][size_t(k)])
-                                              : p;
+    auto at = [&](const float* p, int k) -> const void* {
+      if (host_bytes[size_t(i)][size_t(k)]) return s.out_in.p + host_off[size_t(i)][size_t(k)];
+      return p;
     };
+    half_tab[i] = dtypes[i] == CTD_DTYPE_F16 ? 1 : 0;
     otab[i] = OutputGather{o.blks_on_device ? o.blks : at(o.blks, 0), (long long)o.blks_stride_r,
                            (long long)o.blks_stride_c, o.mask_on_device ? o.mask : at(o.mask, 1),
                            (long long)o.mask_stride_h, (long long)o.mask_stride_w,
                            o.lines_on_device ? o.lines : at(o.lines, 2), (long long)o.lines_stride_h,
-                           (long long)o.lines_stride_w, o.rows, 0};
+                           (long long)o.lines_stride_w, o.rows, half_tab[i]};
   }
-  const size_t tab_bytes = outs       ? h->pg_out_off + size_t(n) * sizeof(OutputGather)
+  const size_t tab_bytes = outs       ? h->pg_half_off + size_t(n) * sizeof(int32_t)
                            : n_gather ? h->pg_gather_off + size_t(n_gather) * sizeof(GatherPage)
                                       : size_t(n) * sizeof(PageGeom);
   CK(cudaMemcpyAsync(s.d_pg_tab, tab, tab_bytes, cudaMemcpyHostToDevice, h->copy_in));
@@ -1073,7 +1081,9 @@ static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* p
                              n, net_h, net_w, no, ws_rows, h->cfg.db_thresh, h->d_mask_u8, h->d_lines, h->d_bitmap,
                              h->d_blks, d_flags, h->stream));
     int cnt = 0;
-    if (int rc = launch_nms(h, n, net_h, net_w, h->stream, &cnt)) return rc;
+    if (int rc = launch_nms(h, n, net_h, net_w, h->stream, &cnt,
+                            reinterpret_cast<const int32_t*>(reinterpret_cast<const char*>(s.d_pg_tab) + h->pg_half_off)))
+      return rc;
     if (int rc = launch_db_post(h, n, net_h, net_w, h->stream, &cnt)) return rc;
   } else {
     CK(letterbox_batch_launch(s.pg_in.p, s.d_pg_tab, n, h->d_pages, net_h, net_w, h->stream));
@@ -1125,17 +1135,28 @@ extern "C" int ctd_submit_pages(ctd_handle* h, int32_t slot, const ctd_page_entr
                                 int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev,
                                 int32_t refine_mode, int32_t keep_undetected, int32_t textheight,
                                 int32_t results_on_device, void* results_host) {
-  return submit_pages_job(h, slot, pages, n, net_h, net_w, input_host, dev, nullptr, refine_mode, keep_undetected,
-                          textheight, results_on_device, results_host);
+  return submit_pages_job(h, slot, pages, n, net_h, net_w, input_host, dev, nullptr, nullptr, refine_mode,
+                          keep_undetected, textheight, results_on_device, results_host);
 }
 
 extern "C" int ctd_submit_outputs(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n, int32_t net_h,
                                   int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev_pages,
                                   const ctd_net_output* outs, int32_t refine_mode, int32_t keep_undetected,
                                   int32_t textheight, int32_t results_on_device, void* results_host) {
-  if (!outs) return CTD_E_INVALID;
-  return submit_pages_job(h, slot, pages, n, net_h, net_w, input_host, dev_pages, outs, refine_mode, keep_undetected,
-                          textheight, results_on_device, results_host);
+  // every page float32 (the job reads dtypes only once it has checked n against max_batch)
+  const std::vector<int32_t> f32(h && n > 0 && n <= h->cfg.max_batch ? size_t(n) : 1, CTD_DTYPE_F32);
+  return ctd_submit_outputs_dtype(h, slot, pages, n, net_h, net_w, input_host, dev_pages, outs, f32.data(), refine_mode,
+                                  keep_undetected, textheight, results_on_device, results_host);
+}
+
+extern "C" int ctd_submit_outputs_dtype(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
+                                        int32_t net_h, int32_t net_w, const uint8_t* input_host,
+                                        const ctd_device_page* dev_pages, const ctd_net_output* outs,
+                                        const int32_t* dtypes, int32_t refine_mode, int32_t keep_undetected,
+                                        int32_t textheight, int32_t results_on_device, void* results_host) {
+  if (!outs || !dtypes) return CTD_E_INVALID;
+  return submit_pages_job(h, slot, pages, n, net_h, net_w, input_host, dev_pages, outs, dtypes, refine_mode,
+                          keep_undetected, textheight, results_on_device, results_host);
 }
 
 static_assert(int(CTD_PRE_F32_NCHW) == int(PRE_F32_NCHW) && int(CTD_PRE_F16_NCHW) == int(PRE_F16_NCHW) &&

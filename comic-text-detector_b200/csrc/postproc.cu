@@ -1,6 +1,7 @@
 // Post-processing kernels: YOLO candidate filter + NMS (utils/yolov5_utils.py:124-218 with
 // torchvision.ops.nms semantics) and 8-connectivity connected-components labelling with OpenCV's
 // label numbering (cv2.connectedComponentsWithStats as called from utils/textmask.py:93,113,138).
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <limits.h>
 
@@ -31,37 +32,68 @@ void nms_workspace_bind(NmsWorkspace& ws, void* base, int n, int cap) {
   ws.cand_total = reinterpret_cast<int*>(p);
 }
 
-// yolov5_utils.py:136,152,169-182: obj > conf -> cls *= obj -> xywh2xyxy -> best class -> conf > thres
-__global__ void nms_filter_kernel(const float* __restrict__ blks, int rows, int no, float conf_thres,
-                                  float* __restrict__ cand, int* __restrict__ cand_count, int cap) {
-  const int img = blockIdx.y;
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= rows) return;
-  const float* x = blks + (size_t(img) * rows + r) * no;
+__device__ __forceinline__ float round_half(float v) { return __half2float(__float2half_rn(v)); }
+
+// the best class score of row x and its class, or 0 (no candidate): obj > conf -> cls *= obj -> best class -> conf >
+// thres (yolov5_utils.py:136,169,179-180).  hf: the row holds float16 values and the reference's arithmetic is half's:
+// conf_thres is half(conf_thres) there, and each product is rounded to half (the float product of two halves is
+// exact, so this is RN_half of the exact product).  Positive floats: the bit pattern is monotone in the value.
+__device__ __forceinline__ unsigned nms_score_key(const float* __restrict__ x, int no, float conf_thres, bool hf,
+                                                  int* cls) {
   const float obj = x[4];
-  if (!(obj > conf_thres)) return;
+  if (!(obj > conf_thres)) return 0u;
   float best = -INFINITY;
   int bj = 0;
   for (int j = 5; j < no; ++j) {
-    const float c = __fmul_rn(x[j], obj);
+    float c = __fmul_rn(x[j], obj);
+    if (hf) c = round_half(c);
     if (c > best) {
       best = c;
       bj = j - 5;
     }
   }
-  if (!(best > conf_thres)) return;
+  if (!(best > conf_thres)) return 0u;
+  *cls = bj;
+  return __float_as_uint(best);
+}
+
+// the candidate row torch.cat((box, conf, j.float()), 1) (yolov5_utils.py:172,180): xywh2xyxy, in half for a float16
+// row, widened exactly to float32 by the cat
+__device__ __forceinline__ void write_cand(float* __restrict__ o, const float* __restrict__ x, bool hf, unsigned key,
+                                           int cls, int r) {
+  float hw = x[2] / 2.f, hh = x[3] / 2.f;
+  if (hf) {
+    hw = round_half(hw);
+    hh = round_half(hh);
+    o[0] = round_half(x[0] - hw); o[1] = round_half(x[1] - hh); o[2] = round_half(x[0] + hw); o[3] = round_half(x[1] + hh);
+  } else {
+    o[0] = x[0] - hw; o[1] = x[1] - hh; o[2] = x[0] + hw; o[3] = x[1] + hh;
+  }
+  o[4] = __uint_as_float(key); o[5] = float(cls); o[6] = __int_as_float(r); o[7] = 0.f;
+}
+
+// conf_thres as page img compares it: half(conf_thres) for a float16 page
+__device__ __forceinline__ float page_conf(const int32_t* __restrict__ half, int img, float conf_thres, bool* hf) {
+  *hf = half && half[img];
+  return *hf ? round_half(conf_thres) : conf_thres;
+}
+
+// yolov5_utils.py:136,152,169-182: one thread per row, candidates appended at atomic slots
+__global__ void nms_filter_kernel(const float* __restrict__ blks, int rows, int no, float conf_thres,
+                                  const int32_t* __restrict__ half, float* __restrict__ cand,
+                                  int* __restrict__ cand_count, int cap) {
+  const int img = blockIdx.y;
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= rows) return;
+  bool hf;
+  const float conf = page_conf(half, img, conf_thres, &hf);
+  const float* x = blks + (size_t(img) * rows + r) * no;
+  int cls = 0;
+  const unsigned key = nms_score_key(x, no, conf, hf, &cls);
+  if (key == 0u) return;
   const int slot = atomicAdd(&cand_count[img], 1);
   if (slot >= cap) return;
-  float* o = cand + (size_t(img) * cap + slot) * kCandStride;
-  const float hw = x[2] / 2.f, hh = x[3] / 2.f;
-  o[0] = x[0] - hw;
-  o[1] = x[1] - hh;
-  o[2] = x[0] + hw;
-  o[3] = x[1] + hh;
-  o[4] = best;
-  o[5] = float(bj);
-  o[6] = __int_as_float(r);
-  o[7] = 0.f;
+  write_cand(cand + (size_t(img) * cap + slot) * kCandStride, x, hf, key, cls, r);
 }
 
 // Overflow path (more candidates than the workspace holds, `cap`): the atomicAdd slots above are claimed in
@@ -71,25 +103,9 @@ __global__ void nms_filter_kernel(const float* __restrict__ blks, int rows, int 
 // ascending) -- a 3-level radix select over the score bits, then an ordered compaction -- and records the true
 // candidate count so the host can see that the cap was hit (ctd_get_nms_status).  One CTA per page; returns at once
 // when the page did not overflow.
-__device__ __forceinline__ unsigned nms_score_key(const float* __restrict__ x, int no, float conf_thres, int* cls) {
-  const float obj = x[4];
-  if (!(obj > conf_thres)) return 0u;
-  float best = -INFINITY;
-  int bj = 0;
-  for (int j = 5; j < no; ++j) {
-    const float c = __fmul_rn(x[j], obj);
-    if (c > best) {
-      best = c;
-      bj = j - 5;
-    }
-  }
-  if (!(best > conf_thres)) return 0u;
-  *cls = bj;
-  return __float_as_uint(best);   // positive floats: the bit pattern is monotone in the value
-}
-
 __global__ void __launch_bounds__(1024) nms_overflow_kernel(const float* __restrict__ blks, int rows, int no,
-                                                            float conf_thres, float* __restrict__ cand,
+                                                            float conf_thres, const int32_t* __restrict__ half,
+                                                            float* __restrict__ cand,
                                                             int* __restrict__ cand_count, int* __restrict__ cand_total,
                                                             int cap) {
   __shared__ int hist[2048];
@@ -100,16 +116,19 @@ __global__ void __launch_bounds__(1024) nms_overflow_kernel(const float* __restr
   const int total = cand_count[img];
   if (t == 0) cand_total[img] = total;
   if (total <= cap) return;
+  bool hf;
+  const float conf = page_conf(half, img, conf_thres, &hf);
   const float* pb = blks + size_t(img) * rows * no;
   if (t == 0) { s_prefix = 0u; s_maskbits = 0u; s_need = cap; }
   const int shifts[3] = {21, 10, 0}, nbins[3] = {2048, 2048, 1024};
+#pragma unroll
   for (int lvl = 0; lvl < 3; ++lvl) {
     for (int i = t; i < 2048; i += 1024) hist[i] = 0;
     __syncthreads();
     const unsigned prefix = s_prefix, maskbits = s_maskbits;
     for (int r = t; r < rows; r += 1024) {
       int cls;
-      const unsigned key = nms_score_key(pb + size_t(r) * no, no, conf_thres, &cls);
+      const unsigned key = nms_score_key(pb + size_t(r) * no, no, conf, hf, &cls);
       if (key != 0u && (key & maskbits) == prefix) atomicAdd(&hist[(key >> shifts[lvl]) & unsigned(nbins[lvl] - 1)], 1);
     }
     __syncthreads();
@@ -134,7 +153,7 @@ __global__ void __launch_bounds__(1024) nms_overflow_kernel(const float* __restr
     const int r = r0 + t;
     int cls = 0;
     unsigned key = 0u;
-    if (r < rows) key = nms_score_key(pb + size_t(r) * no, no, conf_thres, &cls);
+    if (r < rows) key = nms_score_key(pb + size_t(r) * no, no, conf, hf, &cls);
     const bool tie = key == T && key != 0u;
     const unsigned tb = __ballot_sync(0xffffffffu, tie);
     if (lane == 0) wsum_tie[wid] = __popc(tb);
@@ -148,13 +167,7 @@ __global__ void __launch_bounds__(1024) nms_overflow_kernel(const float* __restr
     if (take) {
       int slot = s_base_take + __popc(kb & ((1u << lane) - 1u));
       for (int w2 = 0; w2 < wid; ++w2) slot += wsum_take[w2];
-      if (slot < cap) {
-        const float* x = pb + size_t(r) * no;
-        float* o = out + size_t(slot) * kCandStride;
-        const float hw = x[2] / 2.f, hh = x[3] / 2.f;
-        o[0] = x[0] - hw; o[1] = x[1] - hh; o[2] = x[0] + hw; o[3] = x[1] + hh;
-        o[4] = __uint_as_float(key); o[5] = float(cls); o[6] = __int_as_float(r); o[7] = 0.f;
-      }
+      if (slot < cap) write_cand(out + size_t(slot) * kCandStride, pb + size_t(r) * no, hf, key, cls, r);
     }
     __syncthreads();
     if (t == 0) {
@@ -326,12 +339,13 @@ __global__ void __launch_bounds__(64) nms_scan_kernel(const float* __restrict__ 
 }
 
 cudaError_t nms_launch(const float* blks, int n, int rows, int nc, float conf, float iou, NmsWorkspace& ws, float* det,
-                       int* det_count, cudaStream_t s) {
+                       int* det_count, cudaStream_t s, const int32_t* half) {
   cudaError_t e = cudaMemsetAsync(ws.cand_count, 0, sizeof(int) * n, s);
   if (e != cudaSuccess) return e;
   // rows of `mask` below the diagonal block are never read; words at/after are always written
-  nms_filter_kernel<<<dim3((rows + 255) / 256, n), 256, 0, s>>>(blks, rows, 5 + nc, conf, ws.cand, ws.cand_count, ws.cap);
-  nms_overflow_kernel<<<n, 1024, 0, s>>>(blks, rows, 5 + nc, conf, ws.cand, ws.cand_count, ws.cand_total, ws.cap);
+  nms_filter_kernel<<<dim3((rows + 255) / 256, n), 256, 0, s>>>(blks, rows, 5 + nc, conf, half, ws.cand, ws.cand_count,
+                                                                 ws.cap);
+  nms_overflow_kernel<<<n, 1024, 0, s>>>(blks, rows, 5 + nc, conf, half, ws.cand, ws.cand_count, ws.cand_total, ws.cap);
   if (ws.cap == 4096) nms_sort_kernel<4096><<<n, 1024, 0, s>>>(ws.cand, ws.cand_count, ws.sorted, ws.cap);
   else if (ws.cap == 1024) nms_sort_kernel<1024><<<n, 1024, 0, s>>>(ws.cand, ws.cand_count, ws.sorted, ws.cap);
   else return cudaErrorInvalidValue;

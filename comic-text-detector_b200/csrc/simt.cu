@@ -245,8 +245,9 @@ template cudaError_t stem_launch<__half, float>(const float*, int, int, int, con
                                                 int, int, int, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------
-// input pre-pass: f32 NCHW -> HWC staging page.  One thread per 4 pixels (h * w is a multiple of 4096): three float4
-// plane loads, then the 12 values of the 4 pixels as three 16-byte (f32) or 8-byte (fp16) stores.
+// input pre-pass: f32 or f16 NCHW -> HWC staging page.  One thread per 4 pixels (h * w is a multiple of 4096): three
+// 4-pixel plane loads (16 bytes of f32, 8 of f16), then the 12 values of the 4 pixels as three 16-byte (f32) or 8-byte
+// (fp16) stores.
 __device__ __forceinline__ void st_hwc4(float* d, const float (&v)[12]) {
   float4* o = reinterpret_cast<float4*>(d);
 #pragma unroll
@@ -264,27 +265,40 @@ __device__ __forceinline__ void st_hwc4(__half* d, const float (&v)[12]) {
   }
 }
 
-template <typename S>
-__global__ void __launch_bounds__(256) nchw_to_hwc_kernel(const float* __restrict__ x, size_t hw4, size_t total4,
+// pixels 4q .. 4q + 3 of a plane, widened exactly to float
+__device__ __forceinline__ float4 ld_px4(const float* p, size_t q) { return __ldcs(reinterpret_cast<const float4*>(p) + q); }
+__device__ __forceinline__ float4 ld_px4(const __half* p, size_t q) {
+  const uint2 u = __ldcs(reinterpret_cast<const uint2*>(p) + q);
+  __half2 a, b;
+  memcpy(&a, &u.x, 4);
+  memcpy(&b, &u.y, 4);
+  const float2 fa = __half22float2(a), fb = __half22float2(b);
+  return make_float4(fa.x, fa.y, fb.x, fb.y);
+}
+
+template <typename X, typename S>
+__global__ void __launch_bounds__(256) nchw_to_hwc_kernel(const X* __restrict__ x, size_t hw4, size_t total4,
                                                           S* __restrict__ dst) {
   const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
   if (i >= total4) return;
   const size_t img = i / hw4, q = i - img * hw4;
-  const float4* src = reinterpret_cast<const float4*>(x) + img * 3 * hw4 + q;
-  const float4 b = __ldcs(src), g = __ldcs(src + hw4), r = __ldcs(src + 2 * hw4);
+  const X* src = x + img * 3 * hw4 * 4;
+  const float4 b = ld_px4(src, q), g = ld_px4(src + hw4 * 4, q), r = ld_px4(src + 2 * hw4 * 4, q);
   const float v[12] = {b.x, g.x, r.x, b.y, g.y, r.y, b.z, g.z, r.z, b.w, g.w, r.w};
   st_hwc4(dst + i * 12, v);
 }
 
-template <typename S>
-cudaError_t nchw_to_hwc_launch(const float* x, int n, int h, int w, S* dst, cudaStream_t s) {
+template <typename X, typename S>
+cudaError_t nchw_to_hwc_launch(const X* x, int n, int h, int w, S* dst, cudaStream_t s) {
   if ((size_t(h) * w) % 4) return cudaErrorInvalidValue;
   const size_t hw4 = size_t(h) * w / 4, total4 = size_t(n) * hw4;
-  nchw_to_hwc_kernel<S><<<unsigned((total4 + 255) / 256), 256, 0, s>>>(x, hw4, total4, dst);
+  nchw_to_hwc_kernel<X, S><<<unsigned((total4 + 255) / 256), 256, 0, s>>>(x, hw4, total4, dst);
   return cudaGetLastError();
 }
-template cudaError_t nchw_to_hwc_launch<float>(const float*, int, int, int, float*, cudaStream_t);
-template cudaError_t nchw_to_hwc_launch<__half>(const float*, int, int, int, __half*, cudaStream_t);
+template cudaError_t nchw_to_hwc_launch<float, float>(const float*, int, int, int, float*, cudaStream_t);
+template cudaError_t nchw_to_hwc_launch<float, __half>(const float*, int, int, int, __half*, cudaStream_t);
+template cudaError_t nchw_to_hwc_launch<__half, float>(const __half*, int, int, int, float*, cudaStream_t);
+template cudaError_t nchw_to_hwc_launch<__half, __half>(const __half*, int, int, int, __half*, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------
 template <typename T>

@@ -27,35 +27,41 @@ def workspace_rows(net_h, net_w):
     return 3 * ((net_h // 8) * (net_w // 8) + (net_h // 16) * (net_w // 16) + (net_h // 32) * (net_w // 32))
 
 
-def _float_map(x, name, what, device_index):
-    """x as a float32 numpy array or a float32 CUDA tensor on cuda:device_index, else ValueError"""
-    if getattr(x, "is_cuda", False):
-        if x.dtype != _torch().float32:
-            raise ValueError("%s%s must be float32, got %s (convert with .float())" % (what, name, x.dtype))
+def _float_map(x, name, what, device_index, half=False):
+    """x as a float32 numpy array or a float32 CUDA tensor on cuda:device_index (with half also float16), else
+    ValueError"""
+    if getattr(x, "is_cuda", None) is not None:   # a torch tensor
+        ok = (_torch().float32, _torch().float16) if half else (_torch().float32,)
+        if x.dtype not in ok:
+            raise ValueError("%s%s must be %s, got %s%s" % (what, name, " or ".join(str(d)[6:] for d in ok), x.dtype,
+                                                           "" if half else " (convert with .float())"))
+        if not x.is_cuda:
+            return x.detach().numpy()
         if device_index is not None and x.device.index != device_index:
             raise ValueError("%sa CUDA %s must be on cuda:%d, got %s" % (what, name, device_index, x.device))
         return x
-    if getattr(x, "is_cuda", None) is not None:   # a CPU tensor
-        if x.dtype != _torch().float32:
-            raise ValueError("%s%s must be float32, got %s (convert with .float())" % (what, name, x.dtype))
-        x = x.detach().numpy()
     a = np.asarray(x)
-    if a.dtype != np.float32:
-        raise ValueError("%s%s must be float32, got %s" % (what, name, a.dtype))
+    if a.dtype != np.float32 and not (half and a.dtype == np.float16):
+        raise ValueError("%s%s must be %s, got %s" % (what, name, "float32 or float16" if half else "float32", a.dtype))
     return a
 
 
-def check_outputs(blks, mask, lines_map, input_size, nc=2, device_index=None, what=""):
+def check_outputs(blks, mask, lines_map, input_size, nc=2, device_index=None, what="", half=False):
     """The network outputs of one page as PostProcessor takes them -> (blks [A][5 + nc], mask [H][W], lines channel 0
     [H][W]), views of the caller's arrays or tensors (never copies), else ValueError naming `what` and the argument.
     blks: [1][A][5 + nc] or [A][5 + nc] with A <= workspace_rows(H, W); mask: [1][1][H][W], [1][H][W] or [H][W];
     lines_map: [1][C][H][W] or [C][H][W] with C >= 1, of which only channel 0 is read (db_utils.py:54); (H, W) =
-    input_size; float32 numpy arrays or float32 CUDA tensors on cuda:device_index.  Needs no GPU."""
+    input_size; float32 numpy arrays or float32 CUDA tensors on cuda:device_index.  With half, all three may instead
+    be float16 (numpy, CPU or CUDA tensors), never a mix within the page.  Needs no GPU."""
     net_h, net_w = input_size
     no = 5 + int(nc)
-    b = _float_map(blks, "blks", what, device_index)
-    m = _float_map(mask, "mask", what, device_index)
-    ln = _float_map(lines_map, "lines_map", what, device_index)
+    b = _float_map(blks, "blks", what, device_index, half)
+    m = _float_map(mask, "mask", what, device_index, half)
+    ln = _float_map(lines_map, "lines_map", what, device_index, half)
+    for name, x in (("mask", m), ("lines_map", ln)):
+        if binding._is_f16(x) != binding._is_f16(b):
+            raise ValueError("%s%s is %s but blks is %s: the three outputs of a page must share one dtype" % (
+                what, name, x.dtype, b.dtype))
     bs, ms, ls = tuple(b.shape), tuple(m.shape), tuple(ln.shape)
     if len(bs) == 3 and bs[0] == 1:
         b = b[0]
@@ -95,9 +101,12 @@ class PostProcessor(KernelsOnlyJob):
     `blks, mask, lines_map` in, `(mask, mask_refined, blk_list)` out.  input_size (an int or (h, w), multiples of 64)
     means what it means for `TextDetector`: the net input the outputs were computed on, the page letterboxed into it
     (`ctd_pages_plan`).  max_batch sizes the engine's workspace; nc, conf_thresh and nms_thresh are those of the
-    reference's TextDetector and Detect head."""
+    reference's TextDetector and Detect head.  half: a page's outputs may also be float16 (all three of one page in
+    one dtype); such a page is post-processed with the reference's arithmetic on half tensors, as its
+    `TextDetector(half=True)` does on a float16 network's outputs (include/ctd_b200.h, ctd_submit_outputs_dtype)."""
 
-    def __init__(self, input_size=1024, device_index=0, max_batch=16, nc=2, conf_thresh=0.4, nms_thresh=0.35):
+    def __init__(self, input_size=1024, device_index=0, max_batch=16, nc=2, conf_thresh=0.4, nms_thresh=0.35,
+                 half=False):
         if isinstance(input_size, int):
             input_size = (input_size, input_size)
         self.input_size = tuple(int(v) for v in input_size)
@@ -105,6 +114,7 @@ class PostProcessor(KernelsOnlyJob):
             raise ValueError("input_size must be positive multiples of 64, got %r" % (input_size,))
         self.nc = int(nc)
         self.conf_thresh, self.nms_thresh = conf_thresh, nms_thresh
+        self.half = bool(half)
         super().__init__(device_index, max_batch, max_size=self.input_size, nc=self.nc, conf_thresh=conf_thresh,
                          nms_thresh=nms_thresh, skip_postproc=False)
 
@@ -119,7 +129,7 @@ class PostProcessor(KernelsOnlyJob):
         items = list(items)
         for i, (img, blks, mask, lines_map) in enumerate(items):
             what = "item %d: " % i
-            check_outputs(blks, mask, lines_map, self.input_size, self.nc, self.device_index, what)
+            check_outputs(blks, mask, lines_map, self.input_size, self.nc, self.device_index, what, self.half)
             if not is_encoded(img):
                 page = checked_page(img, what, self.device_index)
                 check_plan(page.shape[:2], self.input_size, what)
@@ -133,8 +143,8 @@ class PostProcessor(KernelsOnlyJob):
         device_results the masks and crops as CUDA tensors.
 
         img: a page as detect_stream takes it (u8 BGR numpy, a torch.uint8 CUDA tensor with any strides, or an encoded
-        file).  blks, mask, lines_map: see check_outputs; float32 numpy arrays or float32 CUDA tensors on
-        cuda:device_index with any strides (a slice `blks[i]` of a batched output is read where it is).  For CUDA
+        file).  blks, mask, lines_map: see check_outputs; float32 (with half also float16) numpy arrays or CUDA
+        tensors on cuda:device_index with any strides (a slice `blks[i]` of a batched output is read where it is).  For CUDA
         pages and outputs an event is recorded on the device's current stream when the item is read, and the GPU
         waits for it before reading them; they are referenced until the item's batch is collected and must not be
         written before.
@@ -156,7 +166,7 @@ class PostProcessor(KernelsOnlyJob):
         def records():
             for idx, (img, blks, mask, lines_map) in enumerate(items):
                 what = "item %d: " % idx
-                outs = check_outputs(blks, mask, lines_map, self.input_size, self.nc, self.device_index, what)
+                outs = check_outputs(blks, mask, lines_map, self.input_size, self.nc, self.device_index, what, self.half)
                 if is_encoded(img):
                     page = _Encoded(idx, img)   # decoded, and its plan checked, with its batch
                 else:

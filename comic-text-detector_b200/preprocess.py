@@ -156,12 +156,19 @@ class NetworkDetector:
     conf_thresh and nms_thresh as for PostProcessor): per batch one pre-processing launch and one `net` call on the
     current stream, then the batch goes to the post-processing, which keeps two batches in flight, so batch k + 1's
     pre-processing and network are enqueued while batch k is post-processed.  Each page is uploaded or decoded once,
-    and both stages read that CUDA page."""
+    and both stages read that CUDA page.
 
-    def __init__(self, net, input_size=1024, device_index=0, max_batch=16, nc=2, conf_thresh=0.4, nms_thresh=0.35):
+    half: the reference's `TextDetector(half=True)` for a float16 network (a `.half()` module, a TensorRT fp16
+    engine, `TextDetBase(half=True)`): `net` gets the float16 tensor `preprocess_img(half=True)` makes, and float16
+    outputs are post-processed with the reference's half arithmetic (PostProcessor(half=True))."""
+
+    def __init__(self, net, input_size=1024, device_index=0, max_batch=16, nc=2, conf_thresh=0.4, nms_thresh=0.35,
+                 half=False):
         self.net = net
+        self.half = bool(half)
         self.pre = Preprocessor(input_size, device_index, max_batch)
-        self.post = PostProcessor(self.pre.input_size, device_index, max_batch, nc, conf_thresh, nms_thresh)
+        self.post = PostProcessor(self.pre.input_size, device_index, max_batch, nc, conf_thresh, nms_thresh,
+                                  half=self.half)
         self.input_size = self.pre.input_size
         self.device_index = self.pre.device_index
         self.max_batch = self.pre.max_batch
@@ -199,7 +206,7 @@ class NetworkDetector:
         in one launch and run through net"""
         def run(batch):
             pages = self.pre.pages_on_device(batch)
-            img_in = self.pre.run(pages)[0]
+            img_in = self.pre.run(pages, half=self.half)[0]
             blks, mask, lines_map = self.net(img_in)
             for i, page in enumerate(pages):
                 yield page, blks[i], mask[i], lines_map[i]

@@ -156,6 +156,14 @@ CTD_API int ctd_get_net_outputs(ctd_handle* h, float* blks, float* mask, float* 
 CTD_API int ctd_forward_tensor(ctd_handle* h, const float* x, int32_t n, int32_t ph, int32_t pw, void* stream,
                                float* blks, float* mask, float* lines);
 
+/* ctd_forward_tensor for a float16 network: x is DEVICE f16 [n][3][ph][pw] (contiguous NCHW, 16-byte aligned; the
+ * tensor `preprocess_img(half=True)` makes) and blks / mask / lines are DEVICE f16 in the layouts of
+ * ctd_get_net_outputs.  The engine widens every input value exactly to float and runs what ctd_forward_tensor runs on
+ * that float32 tensor; each output is that forward's float32 output rounded to nearest even, written by a conversion
+ * kernel in place of the device-to-device copy.  Stream order, limits and NULL outputs as ctd_forward_tensor.          */
+CTD_API int ctd_forward_tensor_f16(ctd_handle* h, const void* x, int32_t n, int32_t ph, int32_t pw, void* stream,
+                                   void* blks, void* mask, void* lines);
+
 /* `postprocess_mask` (inference.py:85-99): (mask*255) truncated to u8, [n][h][w], HOST.   */
 CTD_API int ctd_get_mask_u8(ctd_handle* h, uint8_t* mask_u8);
 
@@ -574,6 +582,25 @@ CTD_API int ctd_submit_outputs(ctd_handle* h, int32_t slot, const ctd_page_entry
                                int32_t net_w, const uint8_t* input_host, const ctd_device_page* dev_pages,
                                const ctd_net_output* outs, int32_t refine_mode, int32_t keep_undetected,
                                int32_t textheight, int32_t results_on_device, void* results_host);
+
+/* ctd_submit_outputs_dtype is ctd_submit_outputs with the element type of each page's maps in dtypes[i]
+ * (ctd_submit_outputs is this call with every page CTD_DTYPE_F32):
+ *   CTD_DTYPE_F32: the three maps of page i are float32, post-processed as above;
+ *   CTD_DTYPE_F16: they are float16 (the ctd_net_output pointers point at float16 elements, strides count them; host
+ *                  maps are copied at 2 bytes per element), post-processed with the reference's arithmetic on half
+ *                  tensors (inference.py:101-114, 85-99, 158; yolov5_utils.py:136-182; db_utils.py:54-72):
+ *                  candidates `obj > half(conf_thresh)`; class scores RN_half(cls * obj), the first maximal class kept
+ *                  where `> half(conf_thresh)`; box corners RN_half(cx -/+ RN_half(w / 2)) and the same in y, widened
+ *                  exactly to float32 before the class offset and NMS; the mask byte numpy's float16 -> uint8 cast
+ *                  of RN_half(p * 255); the DB bitmap `p > half(0.3)`; contour scores on the map widened exactly to
+ *                  float32 (db_utils.py:209-210).  half(x) is the handle's float32 threshold rounded to nearest even.
+ * Pages of both dtypes may share a batch.  Any other dtype fails the call (CTD_E_INVALID) before any GPU work.       */
+enum ctd_dtype { CTD_DTYPE_F32 = 0, CTD_DTYPE_F16 = 1 };
+CTD_API int ctd_submit_outputs_dtype(ctd_handle* h, int32_t slot, const ctd_page_entry* pages, int32_t n,
+                                     int32_t net_h, int32_t net_w, const uint8_t* input_host,
+                                     const ctd_device_page* dev_pages, const ctd_net_output* outs,
+                                     const int32_t* dtypes, int32_t refine_mode, int32_t keep_undetected,
+                                     int32_t textheight, int32_t results_on_device, void* results_host);
 
 /* ---- the detector's pre-processing: the network input preprocess_img makes ---------------------------------------
  * ctd_preprocess_pages writes, for every page of a batch, what the reference's `preprocess_img(img, (net_h, net_w))`
