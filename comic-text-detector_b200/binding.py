@@ -108,7 +108,7 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
            "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
            "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot", "ctd_submit_outputs",
-           "ctd_preprocess_pages", "ctd_submit_outputs_dtype", "ctd_forward_tensor_f16"]
+           "ctd_preprocess_pages", "ctd_submit_outputs_dtype", "ctd_forward_tensor_f16", "ctd_nms_dtype"]
 PRE_F32_NCHW, PRE_F16_NCHW, PRE_U8_NHWC = 0, 1, 2   # ctd_pre_format
 DTYPE_F32, DTYPE_F16 = 0, 1   # ctd_dtype
 
@@ -122,6 +122,18 @@ class CtdError(RuntimeError):
 def _is_f16(m):
     """a float16 numpy array or torch tensor"""
     return str(m.dtype) in ("float16", "torch.float16")
+
+
+def iou_thresh_f32(t):
+    """the float32 threshold the device compares IoUs with (`IoU > nms_thresh` in float32) for an IoU threshold t:
+    RD_f32(t), t rounded toward -inf to float32.  torchvision's CPU nms, on the reference's default device, compares
+    the float32 IoU with t as a double, and for a float32 x, x > t holds exactly when x > RD_f32(t).  float32(t), the
+    round to nearest, differs from it where it rounds up (0.4, 0.6, ...): an IoU of exactly float32(t) is > t but not
+    > float32(t).  For 0.35, RD_f32 and round to nearest agree."""
+    f = np.float32(t)
+    if float(f) > float(t):
+        f = np.nextafter(f, np.float32(-np.inf))
+    return float(f)
 
 
 def load_library():
@@ -153,6 +165,7 @@ def load_library():
     lib.ctd_debug_write_buffer.argtypes = [vp, i32, vp, i32, i32, i32]
     lib.ctd_connected_components.argtypes = [vp, vp, i32, i32, vp, vp, i32, vp]
     lib.ctd_nms.argtypes = [vp, vp, i32, C.c_float, C.c_float, vp, vp]
+    lib.ctd_nms_dtype.argtypes = [vp, vp, i32, i32, C.c_float, C.c_float, vp, vp]
     lib.ctd_get_text_lines.argtypes = [vp, vp, vp, vp]
     lib.ctd_seg_represent.argtypes = [vp, vp, i32, i32, C.c_float, vp, vp, vp]
     lib.ctd_refine_mask.argtypes = [vp, vp, vp, i32, i32, vp, i32, i32, vp]
@@ -332,7 +345,7 @@ class Engine:
                     setattr(o, k, int(v))
         bufs = (CtdBufDesc * len(program.bufs))(*[CtdBufDesc(c, d) for c, d in program.bufs])
         cfg = CtdConfig(ABI_VERSION, device, precision, max_batch, max_h, max_w, self.nc, int(use_graph), conf_thresh,
-                        nms_thresh, db_thresh, int(skip_postproc))
+                        iou_thresh_f32(nms_thresh), db_thresh, int(skip_postproc))
         blob = (C.c_char * len(program.blob)).from_buffer(program.blob)
         rc = self.lib.ctd_create(C.byref(self.h), C.byref(cfg), ops, len(program.ops), bufs, len(program.bufs),
                                  C.cast(blob, C.c_void_p), len(program.blob))
@@ -995,8 +1008,13 @@ class Engine:
         return n, labels, (stats[:n] if stats is not None else None)
 
     def nms(self, pred, conf_thresh=0.4, iou_thresh=0.35):
-        pred = np.ascontiguousarray(pred, np.float32)
+        """non_max_suppression(pred[None], conf_thresh, iou_thresh)[0] (ctd_nms_dtype) -> float32 [k][6].  pred:
+        [rows][5 + nc]; a float16 array is taken with the reference's arithmetic on half tensors, anything else as
+        float32."""
+        dt = DTYPE_F16 if _is_f16(pred) else DTYPE_F32
+        pred = np.ascontiguousarray(pred, np.float16 if dt == DTYPE_F16 else np.float32)
         det = np.empty((300, 6), np.float32)
         cnt = np.zeros((1,), np.int32)
-        self._ck(self.lib.ctd_nms(self.h, _ptr(pred), pred.shape[0], conf_thresh, iou_thresh, _ptr(det), _ptr(cnt)))
+        self._ck(self.lib.ctd_nms_dtype(self.h, _ptr(pred), pred.shape[0], dt, conf_thresh, iou_thresh_f32(iou_thresh),
+                                        _ptr(det), _ptr(cnt)))
         return det[:int(cnt[0])].copy()

@@ -984,13 +984,36 @@ extern "C" int ctd_connected_components(ctd_handle* h, const uint8_t* img, int32
 
 extern "C" int ctd_nms(ctd_handle* h, const float* pred, int32_t rows, float conf_thresh, float iou_thresh, float* det,
                        int32_t* det_count) {
+  return ctd_nms_dtype(h, pred, rows, CTD_DTYPE_F32, conf_thresh, iou_thresh, det, det_count);
+}
+
+extern "C" int ctd_nms_dtype(ctd_handle* h, const void* pred, int32_t rows, int32_t dtype, float conf_thresh,
+                             float iou_thresh, float* det, int32_t* det_count) {
   if (!h || !pred || !det || !det_count) return CTD_E_INVALID;
+  if (dtype != CTD_DTYPE_F32 && dtype != CTD_DTYPE_F16) return ctd_fail(h, CTD_E_INVALID, "bad dtype %d", dtype);
   const int no = 5 + h->cfg.nc;
   if (rows > rows_per_image(h->cfg.max_h, h->cfg.max_w) * h->cfg.max_batch)
     return ctd_fail(h, CTD_E_CAPACITY, "too many prediction rows");
   CK(cudaSetDevice(h->cfg.device));
-  CK(cudaMemcpyAsync(h->d_blks, pred, size_t(rows) * no * 4, cudaMemcpyHostToDevice, h->stream));
-  CK(nms_launch(h->d_blks, 1, rows, h->cfg.nc, conf_thresh, iou_thresh, h->nms, h->d_det, h->d_det_count, h->stream));
+  const size_t elems = size_t(rows) * no;
+  const int32_t* d_half = nullptr;
+  if (dtype == CTD_DTYPE_F16) {
+    // the rows widened exactly to float32, as the ingest of ctd_submit_outputs_dtype widens a float16 page, and the
+    // page's float16 flag for nms_launch
+    std::vector<float> wide(elems);
+    const __half* p = static_cast<const __half*>(pred);
+    for (size_t i = 0; i < elems; ++i) wide[i] = __half2float(p[i]);
+    if (int rc = h->io_scratch.grow(h, 256, h->stream)) return rc;
+    const int32_t one = 1;
+    CK(cudaMemcpyAsync(h->io_scratch.p, &one, sizeof(one), cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_blks, wide.data(), elems * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaStreamSynchronize(h->stream));   // `one` and `wide` go out of scope here
+    d_half = reinterpret_cast<const int32_t*>(h->io_scratch.p);
+  } else {
+    CK(cudaMemcpyAsync(h->d_blks, pred, elems * 4, cudaMemcpyHostToDevice, h->stream));
+  }
+  CK(nms_launch(h->d_blks, 1, rows, h->cfg.nc, conf_thresh, iou_thresh, h->nms, h->d_det, h->d_det_count, h->stream,
+                d_half));
   CK(cudaMemcpyAsync(det, h->d_det, 300 * 6 * 4, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(det_count, h->d_det_count, 4, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));

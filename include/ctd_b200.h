@@ -112,7 +112,10 @@ typedef struct ctd_config {
   int32_t nc;          /* classes of the Detect head (reference: 2, inference.py:117-118)  */
   int32_t use_graph;   /* 1: capture the op list into a CUDA graph per (n,h,w)             */
   float conf_thresh;   /* 0.4  (inference.py:120)                                          */
-  float nms_thresh;    /* 0.35 (inference.py:120)                                          */
+  float nms_thresh;    /* 0.35 (inference.py:120).  A box is suppressed where its float32
+                          IoU > nms_thresh in float32; torchvision's CPU nms (the reference's
+                          default device) compares with a double t, which is this rule with
+                          nms_thresh = RD_f32(t), t rounded toward -inf to float32            */
   float db_thresh;     /* 0.3  (inference.py:139 -> db_utils.py:71-72)                     */
   int32_t debug_skip_postproc; /* 1: ctd_forward stops after the op list (kernel unit tests)  */
 } ctd_config;
@@ -629,9 +632,18 @@ CTD_API int ctd_preprocess_pages(ctd_handle* h, const ctd_page_entry* pages, int
                                  int32_t reverse_channels, void* dst, void* stream);
 
 /* utils/yolov5_utils.py:124-218 on a caller-supplied prediction tensor (HOST f32
- * [rows][5+nc]); output as ctd_get_detections for one page.                                */
+ * [rows][5+nc]); output as ctd_get_detections for one page.  The device suppresses a box when its float32 IoU with
+ * a kept box is > iou_thresh, compared in float32 (as ctd_config::nms_thresh).  torchvision's CPU nms compares the
+ * float32 IoU with a double threshold t; a caller who wants that rule passes RD_f32(t), t rounded toward -inf to
+ * float32 (the Python binding does).                                                        */
 CTD_API int ctd_nms(ctd_handle* h, const float* pred, int32_t rows, float conf_thresh, float iou_thresh, float* det,
             int32_t* det_count);
+/* ctd_nms with the element type of the rows in dtype (enum ctd_dtype; ctd_nms is this call with CTD_DTYPE_F32):
+ * CTD_DTYPE_F16 rows are HOST f16 [rows][5+nc], widened exactly to float32 and taken with the float16 rules of
+ * ctd_submit_outputs_dtype (half(conf_thresh), RN_half class scores and corners).  The output rows are float32 as
+ * for ctd_nms.  Any other dtype fails the call (CTD_E_INVALID).                             */
+CTD_API int ctd_nms_dtype(ctd_handle* h, const void* pred, int32_t rows, int32_t dtype, float conf_thresh,
+                          float iou_thresh, float* det, int32_t* det_count);
 
 /* ---- JPEG pages decoded on the GPU ------------------------------------------------------
  * The reference reads pages with io_utils.imread = cv2.imdecode(np.fromfile(path), IMREAD_COLOR).  These entry points

@@ -60,3 +60,17 @@ def test_no_cpu_fallback():
     with pytest.raises(ctd_b200.CtdError) as e:
         ctd_b200.Engine(P, max_batch=1, max_h=64, max_w=64)
     assert "no CPU fallback" in str(e.value) or "not sm_90" in str(e.value)
+
+
+def test_nms_dtype_entry():
+    """ctd_nms_dtype: the NMS entry with the rows' ctd_dtype, ctd_nms its float32 case; the binding declares it with the
+    header's argument list"""
+    src = open(os.path.join(ROOT, "include", "ctd_b200.h")).read()
+    decl = re.search(r"CTD_API int ctd_nms_dtype\(([^)]*)\)", src).group(1)
+    assert [a.split()[-1].lstrip("*") for a in decl.replace("\n", " ").split(",")] == [
+        "h", "pred", "rows", "dtype", "conf_thresh", "iou_thresh", "det", "det_count"]
+    lib = ctd_b200.load_library()
+    assert "ctd_nms_dtype" in ctd_b200.binding.EXPORTS
+    assert lib.ctd_nms_dtype.argtypes == [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
+                                          ctypes.c_float, ctypes.c_float, ctypes.c_void_p, ctypes.c_void_p]
+    assert lib.ctd_nms_dtype.restype is ctypes.c_int
