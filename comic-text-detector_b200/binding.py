@@ -1,6 +1,7 @@
 """ctypes binding of libctd_b200.so (include/ctd_b200.h).  Thin: numpy arrays in/out, every
 non-zero return code becomes a Python exception carrying ctd_last_error().  There is no CPU
 fallback: if the library is missing or no sm_90 GPU is visible, construction raises."""
+import collections
 import ctypes as C
 import os
 
@@ -270,8 +271,34 @@ def refine_plan(shapes, xyxy, n_blocks):
     return pages, win, status, int(ib.value), int(rb.value)
 
 
+def _on_device(items):
+    """per item of a batch: is it a CUDA tensor (else a host array)"""
+    import torch
+    return [isinstance(x, torch.Tensor) and x.is_cuda for x in items]
+
+
+def _cuda(items, on_dev):
+    """the CUDA tensors of a batch, which it references until it is collected"""
+    return [x for x, d in zip(items, on_dev) if d]
+
+
+def _tensor_ptr(t):
+    return C.c_void_p(t.data_ptr())
+
+
+def _pack(buf, entries, field, images, on_dev=None, ch=3, base=0):
+    """copies the host images of a batch into the pinned torch.uint8 tensor buf: image i, u8 [ih][iw][3] (ch 3) or
+    [ih][iw] (ch 1) in the plan's shape, at byte base + entries[i][field]; the CUDA ones (on_dev[i]) are skipped"""
+    arr = buf.numpy()
+    for i, (e, img) in enumerate(zip(entries, images)):
+        if on_dev is None or not on_dev[i]:
+            ih, iw, o = int(e["ih"]), int(e["iw"]), base + int(e[field])
+            np.copyto(arr[o:o + ih * iw * ch].reshape((ih, iw, 3) if ch == 3 else (ih, iw)), img)
+
+
 def _device_images(items, on_dev, events, channels):
-    """ctd_device_page entries of the CUDA images of a batch (NULL entries for the host ones), or None if none is"""
+    """a pointer to the ctd_device_page entries of the CUDA images of a batch (NULL entries for the host ones), or None
+    if none is"""
     if not any(on_dev):
         return None
     dev = (CtdDevicePage * len(items))()
@@ -281,7 +308,14 @@ def _device_images(items, on_dev, events, channels):
             st = p.stride()   # uint8: element strides are byte strides
             dev[i] = CtdDevicePage(p.data_ptr(), st[0], st[1], st[2] if channels == 3 else 0,
                                    ev.cuda_event if ev is not None else None)
-    return dev
+    return C.cast(dev, C.c_void_p)   # the pointer keeps the array alive
+
+
+# A batch in flight on an engine slot: kind "pages" (submit_pages, submit_outputs), "refine" or "regions"; its plan
+# entries; device_results; the CUDA tensors and events it references until it is collected; the textheight of a
+# "pages" batch and keep_undetected of a "refine" batch
+_Inflight = collections.namedtuple("_Inflight", "kind entries device_results kept textheight keep", defaults=(0, False))
+_COLLECT = {"pages": "collect_pages", "refine": "collect_refine", "regions": "collect_crops"}
 
 
 def decode_block_section(sec, layout):
@@ -352,6 +386,12 @@ class Engine:
         if rc != 0:
             raise CtdError("ctd_create failed (%d): %s" % (rc, self.lib.ctd_last_error(None).decode()))
         self.shape = None
+        import torch
+        # per slot of the batch calls: the pinned buffers (_pinned) and the batch in flight (_Inflight); the stream the
+        # device results are allocated on (_device_results)
+        self._pg_bufs = [[None, None, None], [None, None, None]]
+        self._pg_inflight = [None, None]
+        self._alloc_stream = torch.cuda.Stream(torch.device("cuda", self.device))
 
     def _ck(self, rc):
         if rc != 0:
@@ -554,6 +594,47 @@ class Engine:
     def collect(self, slot):
         self._ck(self.lib.ctd_collect(self.h, slot))
 
+    # ---- caller batches on the two slots: one refusal, one buffer grow, one in-flight record per slot ---------
+    def _begin(self, slot):
+        if self._pg_inflight[slot] is not None:
+            raise CtdError("slot %d has an uncollected submission" % slot)
+
+    def _pinned(self, slot, k, nbytes):
+        """slot's pinned buffer k (0 the packed host pages, 1 the results, 2 the host network outputs), grown with a
+        quarter of headroom when it holds fewer than nbytes; None while no batch has needed it"""
+        buf = self._pg_bufs[slot][k]
+        if nbytes and (buf is None or buf.numel() < nbytes):
+            import torch
+            buf = self._pg_bufs[slot][k] = torch.empty((nbytes * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        return buf
+
+    def _take(self, slot, kind):
+        """the record of slot's batch, which must be of `kind`; the slot is then free and the batch is collected next.
+        A batch of another kind stays in flight, so its own collect still returns its results."""
+        rec = self._pg_inflight[slot]
+        if rec is None or rec.kind != kind:
+            held = "nothing" if rec is None else "a submit_%s batch, collected with %s" % (rec.kind, _COLLECT[rec.kind])
+            raise CtdError("slot %d has no submit_%s batch in flight: it holds %s" % (slot, kind, held))
+        self._pg_inflight[slot] = None
+        return rec
+
+    def _device_results(self, slot, sizes):
+        """ctd_collect_device of slot's collected batch into one new CUDA allocation per page, of sizes[p] bytes (None
+        for 0).  The allocations are made on the engine's own stream, so the caching allocator cannot hand out memory
+        that work still queued on the caller's stream uses (the copies do not wait for that stream), and are marked as
+        used on the caller's current stream."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        with torch.cuda.stream(self._alloc_stream):
+            bufs = [torch.empty((n,), dtype=torch.uint8, device=dev) if n else None for n in sizes]
+        ptrs = (C.c_void_p * len(bufs))(*[None if b is None else b.data_ptr() for b in bufs])
+        self._ck(self.lib.ctd_collect_device(self.h, slot, ptrs))
+        cur = torch.cuda.current_stream(dev)
+        for b in bufs:
+            if b is not None:
+                b.record_stream(cur)
+        return bufs
+
     def submit_pages(self, slot, pages, net_h, net_w, refine_mode=0, keep_undetected=False, textheight=0, events=None,
                      device_results=False):
         """asynchronous `detect_page` of a batch of pages of any size (ctd_submit_pages).  A page is a u8
@@ -563,32 +644,20 @@ class Engine:
         before CUDA page i is read.  The CUDA pages are referenced until the slot is collected and must not be written
         before.  textheight >= 2 also crops every text line of every page on the GPU (0: no crops).  device_results:
         masks and crops stay on the GPU (see collect_pages).  Collect with collect_pages(slot)."""
-        import torch
-        if not hasattr(self, "_pg_bufs"):
-            self._pg_bufs = [[None, None], [None, None]]   # per slot: pinned input, pinned results
-            self._pg_inflight = [None, None]
-        if self._pg_inflight[slot] is not None:
-            raise CtdError("slot %d has an uncollected submission" % slot)
+        self._begin(slot)
         entries, in_bytes, res_bytes = pages_plan([tuple(p.shape[:2]) for p in pages], net_h, net_w)
-        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
-        bufs = self._pg_bufs[slot]
-        for k, need in ((0, 0 if all(on_dev) else in_bytes), (1, res_bytes)):
-            if need and (bufs[k] is None or bufs[k].numel() < need):
-                bufs[k] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
-        dev = _device_images(pages, on_dev, events, 3)
+        on_dev = _on_device(pages)
+        inp = self._pinned(slot, 0, 0 if all(on_dev) else in_bytes)
+        res = self._pinned(slot, 1, res_bytes)
         if not all(on_dev):
-            inp = bufs[0].numpy()
-            for e, p, d in zip(entries, pages, on_dev):
-                if not d:
-                    o = int(e["page_off"])
-                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+            _pack(inp, entries, "page_off", pages, on_dev)
         self._ck(self.lib.ctd_submit_pages(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
-                                           None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
-                                           None if dev is None else C.cast(dev, C.c_void_p), int(refine_mode),
+                                           None if all(on_dev) else _tensor_ptr(inp),
+                                           _device_images(pages, on_dev, events, 3), int(refine_mode),
                                            int(bool(keep_undetected)), int(textheight), int(bool(device_results)),
-                                           C.c_void_p(bufs[1].data_ptr())))
-        kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]]
-        self._pg_inflight[slot] = (entries, int(textheight), bool(device_results), kept)
+                                           _tensor_ptr(res)))
+        self._pg_inflight[slot] = _Inflight("pages", entries, bool(device_results), (_cuda(pages, on_dev), events),
+                                            textheight=int(textheight))
         self.shape = (len(entries), net_h, net_w)
 
     def collect_pages(self, slot, discard=False):
@@ -597,31 +666,28 @@ class Engine:
         textheight, each tuple has a sixth element, the page's crops (see collect_regions).  With device_results, mask,
         mask_refined and the crops are torch.uint8 CUDA tensors, views into one allocation of that page's own (filled by
         ctd_collect_device; complete on return).  discard: only wait for the batch and return None."""
-        inflight = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
-        if inflight is None:
-            raise CtdError("slot %d has no submit_pages batch in flight" % slot)
-        entries, textheight, device_results, _kept = inflight
-        self._pg_inflight[slot] = None
+        rec = self._take(slot, "pages")
         self.collect(slot)
         if discard:
             return None
+        entries = rec.entries
         res = self._pg_bufs[slot][1].numpy()
         lay = self.results_layout()
         stride = lay["blocks_stride"]
         blocks = []
         for e in entries:
             bo = int(e["blocks_off"])
-            _hdr, rec, lines, dist = decode_block_section(res[bo:bo + stride], lay)
-            blocks.append((rec.copy(), lines.copy(), dist.copy()))
+            _hdr, recs, lines, dist = decode_block_section(res[bo:bo + stride], lay)
+            blocks.append((recs.copy(), lines.copy(), dist.copy()))
         n_lines = [b[0]["n_lines"] for b in blocks]
-        if device_results:
-            return self._collect_device(slot, entries, blocks, n_lines if textheight else None)
+        if rec.device_results:
+            return self._collect_device(slot, entries, blocks, n_lines if rec.textheight else None)
         out = []
         for e, b in zip(entries, blocks):
             ih, iw = int(e["ih"]), int(e["iw"])
             mo, ro = int(e["mask_off"]), int(e["refined_off"])
             out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy(), res[ro:ro + ih * iw].reshape(ih, iw).copy()) + b)
-        if textheight:
+        if rec.textheight:
             crops = self.collect_regions(slot, n_lines)
             out = [o + (c,) for o, c in zip(out, crops)]
         return out
@@ -635,15 +701,10 @@ class Engine:
         page is then post-processed with the reference's half arithmetic).  events[i] (a recorded torch.cuda.Event, or None) is
         waited on before CUDA page i and CUDA outputs i are read; the CUDA pages and outputs are referenced until the
         slot is collected and must not be written before.  Collect with collect_pages(slot)."""
-        import torch
-        if not hasattr(self, "_pg_bufs"):
-            self._pg_bufs = [[None, None], [None, None]]
-            self._pg_inflight = [None, None]
-        if self._pg_inflight[slot] is not None:
-            raise CtdError("slot %d has an uncollected submission" % slot)
+        self._begin(slot)
         entries, in_bytes, res_bytes = pages_plan([tuple(p.shape[:2]) for p in pages], net_h, net_w)
-        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
-        o_dev = [[isinstance(m, torch.Tensor) and m.is_cuda for m in o] for o in outs]
+        on_dev = _on_device(pages)
+        o_dev = [_on_device(o) for o in outs]
         # the host maps, packed contiguous into the slot's pinned output buffer, 256-byte aligned each
         offs, need = [], 0
         for o, d in zip(outs, o_dev):
@@ -652,24 +713,15 @@ class Engine:
                 page.append(None if md else need)
                 need += 0 if md else (m.size * m.itemsize + 255) // 256 * 256
             offs.append(page)
-        if not hasattr(self, "_out_bufs"):
-            self._out_bufs = [None, None]
-        bufs = self._pg_bufs[slot]
-        for k, n_bytes in ((0, 0 if all(on_dev) else in_bytes), (1, res_bytes)):
-            if n_bytes and (bufs[k] is None or bufs[k].numel() < n_bytes):
-                bufs[k] = torch.empty((n_bytes * 5 // 4,), dtype=torch.uint8, pin_memory=True)
-        if need and (self._out_bufs[slot] is None or self._out_bufs[slot].numel() < need):
-            self._out_bufs[slot] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        inp = self._pinned(slot, 0, 0 if all(on_dev) else in_bytes)
+        res = self._pinned(slot, 1, res_bytes)
+        obufs = self._pinned(slot, 2, need)
         if not all(on_dev):
-            inp = bufs[0].numpy()
-            for e, p, d in zip(entries, pages, on_dev):
-                if not d:
-                    o = int(e["page_off"])
-                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+            _pack(inp, entries, "page_off", pages, on_dev)
         rec = (CtdNetOutput * len(outs))()
         dtypes = (C.c_int32 * len(outs))(*[DTYPE_F16 if _is_f16(o[0]) else DTYPE_F32 for o in outs])
-        obuf = self._out_bufs[slot].numpy() if need else None
-        base = self._out_bufs[slot].data_ptr() if need else 0
+        obuf = obufs.numpy() if need else None
+        base = obufs.data_ptr() if need else 0
         for i, (o, d, off) in enumerate(zip(outs, o_dev, offs)):
             fields = []
             for m, md, mo in zip(o, d, off):
@@ -683,17 +735,15 @@ class Engine:
             ev = events[i] if events is not None else None
             rec[i] = CtdNetOutput(bp, bsr, bsc, mp, msh, msw, lp, lsh, lsw, int(o[0].shape[0]), bd, md_, ld,
                                   ev.cuda_event if ev is not None else None)
-        dev = _device_images(pages, on_dev, events, 3)
         self._ck(self.lib.ctd_submit_outputs_dtype(self.h, slot, _ptr(entries), len(entries), net_h, net_w,
-                                                   None if all(on_dev) else C.c_void_p(bufs[0].data_ptr()),
-                                                   None if dev is None else C.cast(dev, C.c_void_p),
+                                                   None if all(on_dev) else _tensor_ptr(inp),
+                                                   _device_images(pages, on_dev, events, 3),
                                                    C.cast(rec, C.c_void_p), C.cast(dtypes, C.c_void_p),
                                                    int(refine_mode), int(bool(keep_undetected)), int(textheight),
-                                                   int(bool(device_results)), C.c_void_p(bufs[1].data_ptr())))
-        kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]] + \
-               [(m, None if events is None else events[i]) for i, o in enumerate(outs) for m, md in zip(o, o_dev[i])
-                if md]
-        self._pg_inflight[slot] = (entries, int(textheight), bool(device_results), kept)
+                                                   int(bool(device_results)), _tensor_ptr(res)))
+        kept = _cuda(pages, on_dev) + [m for o, d in zip(outs, o_dev) for m in _cuda(o, d)]
+        self._pg_inflight[slot] = _Inflight("pages", entries, bool(device_results), (kept, events),
+                                            textheight=int(textheight))
         self.shape = (len(entries), net_h, net_w)
 
     def preprocess_pages(self, pages, net_h, net_w, fmt, reverse, dst_ptr, stream, events=None, input_host=None):
@@ -704,22 +754,16 @@ class Engine:
         [h][w][3] numpy array, packed at its page_off into input_host: a pinned torch.uint8 tensor of at least the
         plan's input bytes, which the caller keeps unwritten until the stream has run the call.  Returns the
         ctd_pages_plan entries of the batch."""
-        import torch
         entries, in_bytes, _res = pages_plan([tuple(p.shape[:2]) for p in pages], net_h, net_w)
-        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
+        on_dev = _on_device(pages)
         host = None
         if not all(on_dev):
             if input_host is None or input_host.numel() < in_bytes:
                 raise CtdError("numpy pages need a pinned input_host of %d bytes" % in_bytes)
-            inp = input_host.numpy()
-            for e, p, d in zip(entries, pages, on_dev):
-                if not d:
-                    o = int(e["page_off"])
-                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
-            host = C.c_void_p(input_host.data_ptr())
-        dev = _device_images(pages, on_dev, events, 3)
+            _pack(input_host, entries, "page_off", pages, on_dev)
+            host = _tensor_ptr(input_host)
         self._ck(self.lib.ctd_preprocess_pages(self.h, _ptr(entries), len(entries), int(net_h), int(net_w), host,
-                                               None if dev is None else C.cast(dev, C.c_void_p), int(fmt),
+                                               _device_images(pages, on_dev, events, 3), int(fmt),
                                                int(bool(reverse)), C.c_void_p(dst_ptr), C.c_void_p(stream)))
         return entries
 
@@ -732,79 +776,48 @@ class Engine:
         referenced until the slot is collected and must not be written before.  refined: None, or per page a numpy
         u8 [h][w] mask_refined to run refine_undetected_mask alone on (needs keep_undetected).  Collect with
         collect_refine(slot)."""
-        import torch
-        if not hasattr(self, "_pg_bufs"):
-            self._pg_bufs = [[None, None], [None, None]]
-            self._pg_inflight = [None, None]
-        if self._pg_inflight[slot] is not None:
-            raise CtdError("slot %d has an uncollected submission" % slot)
+        self._begin(slot)
         counts = [len(b) for b in boxes]
         xyxy = np.concatenate([np.asarray(b, np.int32).reshape(-1, 4) for b in boxes]) if boxes else np.zeros((0, 4))
         entries, _win, _st, in_bytes, res_bytes = refine_plan([tuple(p.shape[:2]) for p in pages], xyxy, counts)
-        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
-        m_dev = [isinstance(m, torch.Tensor) and m.is_cuda for m in masks]
+        on_dev = _on_device(pages)
+        m_dev = _on_device(masks)
         host = refined is not None or not all(on_dev) or not all(m_dev)
-        bufs = self._pg_bufs[slot]
-        for k, need in ((0, in_bytes if host else 0), (1, res_bytes)):
-            if need and (bufs[k] is None or bufs[k].numel() < need):
-                bufs[k] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        inp = self._pinned(slot, 0, in_bytes if host else 0)
+        res = self._pinned(slot, 1, res_bytes)
         if host:
-            inp = bufs[0].numpy()
             frame = in_bytes // 5 * 3
-            for e, p, d, m, md in zip(entries, pages, on_dev, masks, m_dev):
-                ih, iw = int(e["ih"]), int(e["iw"])
-                if not d:
-                    o = int(e["page_off"])
-                    np.copyto(inp[o:o + ih * iw * 3].reshape(ih, iw, 3), p)
-                if not md:
-                    o = frame + int(e["mask_off"])
-                    np.copyto(inp[o:o + ih * iw].reshape(ih, iw), m)
-            for e, r in zip(entries, refined or []):
-                o = frame + int(e["refined_off"])
-                np.copyto(inp[o:o + r.size].reshape(r.shape), r)
-        dev_p = _device_images(pages, on_dev, events, 3)
-        dev_m = _device_images(masks, m_dev, events, 1)
+            _pack(inp, entries, "page_off", pages, on_dev)
+            _pack(inp, entries, "mask_off", masks, m_dev, 1, frame)
+            if refined is not None:
+                _pack(inp, entries, "refined_off", refined, None, 1, frame)
         self._ck(self.lib.ctd_submit_refine(self.h, slot, _ptr(entries), len(entries), _ptr(xyxy), _ptr(np.asarray(
-            counts, np.int32)), C.c_void_p(bufs[0].data_ptr()) if host else None,
-            None if dev_p is None else C.cast(dev_p, C.c_void_p), None if dev_m is None else C.cast(dev_m, C.c_void_p),
-            int(refine_mode), int(bool(keep_undetected)), int(refined is not None), int(bool(device_results)),
-            C.c_void_p(bufs[1].data_ptr())))
-        kept = [x for i in range(len(pages)) for x, d in ((pages[i], on_dev[i]), (masks[i], m_dev[i])) if d]
-        self._pg_inflight[slot] = ("refine", entries, bool(keep_undetected), bool(device_results), kept, events)
+            counts, np.int32)), _tensor_ptr(inp) if host else None, _device_images(pages, on_dev, events, 3),
+            _device_images(masks, m_dev, events, 1), int(refine_mode), int(bool(keep_undetected)),
+            int(refined is not None), int(bool(device_results)), _tensor_ptr(res)))
+        self._pg_inflight[slot] = _Inflight("refine", entries, bool(device_results),
+                                            (_cuda(pages, on_dev) + _cuda(masks, m_dev), events),
+                                            keep=bool(keep_undetected))
 
     def collect_refine(self, slot, discard=False):
         """blocks until the batch of submit_refine(slot) is done -> per page (mask, mask_refined): mask is the mask
         refine_undetected_mask modified (keep_undetected), else None.  numpy arrays copied out of the slot's pinned
         buffer, or with device_results torch.uint8 CUDA tensors, views into one allocation of the page's own
         (ctd_collect_device, complete on return, marked as used on the current stream).  discard: only wait."""
-        inflight = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
-        if inflight is None or inflight[0] != "refine":
-            raise CtdError("slot %d has no submit_refine batch in flight" % slot)
-        _kind, entries, keep, device_results, _kept, _events = inflight
-        self._pg_inflight[slot] = None
+        rec = self._take(slot, "refine")
         self.collect(slot)
         if discard:
             return None
-        shapes = [(int(e["ih"]), int(e["iw"])) for e in entries]
-        if device_results:
-            import torch
-            dev = torch.device("cuda", self.device)
-            if getattr(self, "_alloc_stream", None) is None:
-                self._alloc_stream = torch.cuda.Stream(dev)
-            with torch.cuda.stream(self._alloc_stream):
-                bufs = [torch.empty((2 * ih * iw,), dtype=torch.uint8, device=dev) for ih, iw in shapes]
-            self._ck(self.lib.ctd_collect_device(self.h, slot, (C.c_void_p * len(bufs))(*[b.data_ptr() for b in bufs])))
-            cur = torch.cuda.current_stream(dev)
-            out = []
-            for b, (ih, iw) in zip(bufs, shapes):
-                b.record_stream(cur)
-                out.append((b[:ih * iw].view(ih, iw) if keep else None, b[ih * iw:].view(ih, iw)))
-            return out
+        shapes = [(int(e["ih"]), int(e["iw"])) for e in rec.entries]
+        if rec.device_results:
+            bufs = self._device_results(slot, [2 * ih * iw for ih, iw in shapes])
+            return [(b[:ih * iw].view(ih, iw) if rec.keep else None, b[ih * iw:].view(ih, iw))
+                    for b, (ih, iw) in zip(bufs, shapes)]
         res = self._pg_bufs[slot][1].numpy()
         out = []
-        for e, (ih, iw) in zip(entries, shapes):
+        for e, (ih, iw) in zip(rec.entries, shapes):
             mo, ro = int(e["mask_off"]), int(e["refined_off"])
-            out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy() if keep else None,
+            out.append((res[mo:mo + ih * iw].reshape(ih, iw).copy() if rec.keep else None,
                         res[ro:ro + ih * iw].reshape(ih, iw).copy()))
         return out
 
@@ -814,34 +827,20 @@ class Engine:
         is), lines = REGION_LINE_DTYPE records of every page's lines, page 0's first, n_lines[i] of page i.
         events[i] (a recorded torch.cuda.Event, or None) is waited on before CUDA page i is read; the CUDA pages are
         referenced until the slot is collected and must not be written before.  Collect with collect_crops(slot)."""
-        import torch
-        if not hasattr(self, "_pg_bufs"):
-            self._pg_bufs = [[None, None], [None, None]]
-            self._pg_inflight = [None, None]
-        if self._pg_inflight[slot] is not None:
-            raise CtdError("slot %d has an uncollected submission" % slot)
+        self._begin(slot)
         shapes = [tuple(p.shape[:2]) for p in pages]
         entries, _win, _st, in_bytes, _rb = refine_plan(shapes, np.zeros((0, 4), np.int32), [0] * len(pages))
-        on_dev = [isinstance(p, torch.Tensor) and p.is_cuda for p in pages]
+        on_dev = _on_device(pages)
         host = not all(on_dev)
-        need = in_bytes // 5 * 3 if host else 0   # the page plane of the layout
-        bufs = self._pg_bufs[slot]
-        if need and (bufs[0] is None or bufs[0].numel() < need):
-            bufs[0] = torch.empty((need * 5 // 4,), dtype=torch.uint8, pin_memory=True)
+        inp = self._pinned(slot, 0, in_bytes // 5 * 3 if host else 0)   # the page plane of the layout
         if host:
-            inp = bufs[0].numpy()
-            for e, p, d in zip(entries, pages, on_dev):
-                if not d:
-                    o = int(e["page_off"])
-                    np.copyto(inp[o:o + p.size].reshape(p.shape), p)
+            _pack(inp, entries, "page_off", pages, on_dev)
         lines = np.ascontiguousarray(lines, REGION_LINE_DTYPE)
         counts = np.ascontiguousarray(n_lines, np.int32)
-        dev = _device_images(pages, on_dev, events, 3)
         self._ck(self.lib.ctd_submit_regions(self.h, slot, _ptr(entries), len(entries), _ptr(lines), _ptr(counts),
-                                             int(textheight), C.c_void_p(bufs[0].data_ptr()) if host else None,
-                                             None if dev is None else C.cast(dev, C.c_void_p), int(bool(device_results))))
-        kept = [(p, None if events is None else events[i]) for i, p in enumerate(pages) if on_dev[i]]
-        self._pg_inflight[slot] = ("regions", len(entries), bool(device_results), kept)
+                                             int(textheight), _tensor_ptr(inp) if host else None,
+                                             _device_images(pages, on_dev, events, 3), int(bool(device_results))))
+        self._pg_inflight[slot] = _Inflight("regions", entries, bool(device_results), (_cuda(pages, on_dev), events))
 
     def collect_crops(self, slot, counts, discard=False):
         """blocks until the batch of submit_regions(slot) is done -> per page, per block (counts[p]: the number of lines
@@ -849,64 +848,34 @@ class Engine:
         page's crops are views into one array of that page's own (collect_regions), or with device_results into one
         CUDA allocation of its own (ctd_collect_device; complete on return, marked as used on the current stream); a
         page without a crop allocates nothing.  discard: only wait for the batch and return None."""
-        inflight = self._pg_inflight[slot] if hasattr(self, "_pg_inflight") else None
-        if inflight is None or inflight[0] != "regions":
-            raise CtdError("slot %d has no submit_regions batch in flight" % slot)
-        _kind, n_pages, device_results, _kept = inflight
-        self._pg_inflight[slot] = None
+        rec = self._take(slot, "regions")
         self.collect(slot)
         if discard:
             return None
-        if not device_results:
+        if not rec.device_results:
             return self.collect_regions(slot, counts)
-        import torch
-        dev = torch.device("cuda", self.device)
-        if getattr(self, "_alloc_stream", None) is None:
-            self._alloc_stream = torch.cuda.Stream(dev)
+        n_pages = len(rec.entries)
         plan = self._collected_plan(slot, n_pages)
-        ranges = [plan.page_range(p) for p in range(n_pages)]
-        with torch.cuda.stream(self._alloc_stream):
-            bufs = [torch.empty((hi - lo,), dtype=torch.uint8, device=dev) if hi > lo else None for lo, hi in ranges]
-        ptrs = (C.c_void_p * n_pages)(*[None if b is None else b.data_ptr() for b in bufs])
-        self._ck(self.lib.ctd_collect_device(self.h, slot, ptrs))
-        cur = torch.cuda.current_stream(dev)
-        out = []
-        for p, buf in enumerate(bufs):
-            if buf is not None:
-                buf.record_stream(cur)
-            out.append(plan.page_crops(p, counts[p], lambda c, h, w, buf=buf: buf.as_strided((h, w, 3), (w * 3, 3, 1), c)))
-        return out
+        bufs = self._device_results(slot, [hi - lo for lo, hi in (plan.page_range(p) for p in range(n_pages))])
+        return [plan.page_crops(p, counts[p], lambda c, h, w, buf=buf: buf.as_strided((h, w, 3), (w * 3, 3, 1), c))
+                for p, buf in enumerate(bufs)]
 
     def _collect_device(self, slot, entries, blocks, n_lines):
         """collect_pages of a device_results batch: one CUDA allocation per page, [mask | mask_refined | crops]
-        (ctd_collect_device).  The allocations are made on a stream of the engine's own, so the caching allocator
-        cannot hand out memory that work still queued on the caller's stream uses (the copies do not wait for that
-        stream), and are marked as used on the caller's current stream."""
-        import torch
-        dev = torch.device("cuda", self.device)
-        if getattr(self, "_alloc_stream", None) is None:
-            self._alloc_stream = torch.cuda.Stream(dev)
+        (_device_results)"""
         plan = self._collected_plan(slot, len(entries)) if n_lines is not None else None
-        sizes = []
-        for p, e in enumerate(entries):
-            px = int(e["ih"]) * int(e["iw"])
-            lo, hi = plan.page_range(p) if plan is not None else (0, 0)
-            sizes.append((px, lo, hi))
-        with torch.cuda.stream(self._alloc_stream):
-            bufs = [torch.empty((2 * px + hi - lo,), dtype=torch.uint8, device=dev) for px, lo, hi in sizes]
-        ptrs = (C.c_void_p * len(bufs))(*[b.data_ptr() for b in bufs])
-        self._ck(self.lib.ctd_collect_device(self.h, slot, ptrs))
-        cur = torch.cuda.current_stream(dev)
+        px = [int(e["ih"]) * int(e["iw"]) for e in entries]
+        ranges = [plan.page_range(p) if plan is not None else (0, 0) for p in range(len(entries))]
+        bufs = self._device_results(slot, [2 * n + hi - lo for n, (lo, hi) in zip(px, ranges)])
         out = []
-        for p, (e, b, buf, (px, _lo, _hi)) in enumerate(zip(entries, blocks, bufs, sizes)):
-            buf.record_stream(cur)
+        for p, (e, b, buf, n) in enumerate(zip(entries, blocks, bufs, px)):
             ih, iw = int(e["ih"]), int(e["iw"])
-            o = (buf[:px].view(ih, iw), buf[px:2 * px].view(ih, iw)) + b
+            o = (buf[:n].view(ih, iw), buf[n:2 * n].view(ih, iw)) + b
             if plan is not None:
                 # as_strided on the fresh allocation (storage offset 0): the cheapest view torch makes, which matters
                 # at thousands of crops per batch
-                o += (plan.page_crops(p, n_lines[p], lambda c, h, w, buf=buf, px=px:
-                                      buf.as_strided((h, w, 3), (w * 3, 3, 1), 2 * px + c)),)
+                o += (plan.page_crops(p, n_lines[p], lambda c, h, w, buf=buf, n=n:
+                                      buf.as_strided((h, w, 3), (w * 3, 3, 1), 2 * n + c)),)
             out.append(o)
         return out
 

@@ -881,19 +881,99 @@ static int ensure_page_tables(ctd_handle* h, Slot& s) {
   return CTD_OK;
 }
 
-// H2D on `st` of the byte ranges [off(i), off(i) + bytes(i)) from src to dst of the pages that are not on the device
-// (dev[i].data == NULL, or dev NULL), one copy per run of consecutive such pages
-template <typename Off, typename Len>
-static int copy_host_runs(ctd_handle* h, const ctd_device_page* dev, int n, uint8_t* dst, const uint8_t* src, Off off,
-                          Len bytes, cudaStream_t st) {
+// ---- batch ingest: the checks and copies every entry that takes caller pages shares ---------------------------------
+// Each entry replans the caller's entries with its own planner, then: the row and undetected-mask limits, the source of
+// each image (device memory of the handle's GPU, else input_host), a GatherPage per device image, the host images' byte
+// ranges in, and on the engine (or caller's) stream the device images' event waits and one gather launch.
+
+// at most max_batch entries in one batch
+static int check_batch_size(ctd_handle* h, int n) {
+  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
+  return CTD_OK;
+}
+
+// a batch of n >= 1 entries on `slot`: slot 0 or 1 with nothing in flight, and check_batch_size (nothing is read
+// through h before the arguments pass)
+static int admit_batch(ctd_handle* h, int slot, int n) {
+  if (!h || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (h->slot[slot].busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
+  return check_batch_size(h, n);
+}
+
+// the offsets decide where the copies write: the caller's entries must be the ones `planner` returned (pg)
+static int same_as_plan(ctd_handle* h, const std::vector<ctd_page_entry>& pg, const ctd_page_entry* pages,
+                        const char* planner) {
+  if (memcmp(pg.data(), pages, pg.size() * sizeof(ctd_page_entry)) != 0)
+    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones %s returns", planner);
+  return CTD_OK;
+}
+
+// the gather and back-projection launches index rows in int32
+static int check_batch_rows(ctd_handle* h, const std::vector<ctd_page_entry>& pg) {
+  size_t rows = 0;
+  for (const ctd_page_entry& e : pg) rows += size_t(e.ih);
+  if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
+  return CTD_OK;
+}
+
+// keep_undetected: refine_undetected_mask labels each page with the CCL, which takes at most kCclMaxPixels
+static int check_undetected_size(ctd_handle* h, const std::vector<ctd_page_entry>& pg) {
+  for (size_t i = 0; i < pg.size(); ++i)
+    if (size_t(pg[i].ih) * size_t(pg[i].iw) > kCclMaxPixels)
+      return ctd_fail(h, CTD_E_CAPACITY, "page %d (%dx%d): refine_undetected_mask labels pages of at most 2^28 pixels",
+                      int(i), pg[i].ih, pg[i].iw);
+  return CTD_OK;
+}
+
+// where each page (ch = 3) or mask (ch = 1) of a batch comes from: dev[i] in device memory (check_device_image), or
+// else input_host, which must then be given.  *n_dev: the number of device images
+static int check_sources(ctd_handle* h, const char* what, const ctd_device_page* dev,
+                         const std::vector<ctd_page_entry>& pg, int ch, const uint8_t* input_host, int* n_dev) {
+  *n_dev = 0;
+  for (int i = 0; i < int(pg.size()); ++i) {
+    if (!dev || !dev[i].data) {
+      if (!input_host) return ctd_fail(h, CTD_E_INVALID, "%s %d is in neither input_host nor device memory", what, i);
+      continue;
+    }
+    if (int rc = check_device_image(h, what, i, dev[i], pg[size_t(i)].ih, pg[size_t(i)].iw, ch)) return rc;
+    ++*n_dev;
+  }
+  return CTD_OK;
+}
+
+// the gather of the device page (ch = 3) or mask (ch = 1) d of entry e into its packed place dst, rows from row0 of the
+// launch; `fast` when its pixels are contiguous
+static GatherPage gather_entry(const ctd_device_page& d, uint8_t* dst, const ctd_page_entry& e, int ch, int row0) {
+  const bool contiguous = ch == 3 ? d.stride_c == 1 && d.stride_w == 3 : d.stride_w == 1;
+  return GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, ch == 3 ? (long long)d.stride_c : 0, dst,
+                    e.ih, e.iw, row0, contiguous ? 1 : 0, ch, 0};
+}
+
+// H2D on `st` from src to dst of the images (ch bytes per pixel, at byte offset pg[i].*off) that are not on the device
+// (dev[i].data == NULL, or dev NULL), one copy per run of consecutive such images
+static int copy_host_images(ctd_handle* h, const ctd_device_page* dev, const std::vector<ctd_page_entry>& pg,
+                            uint8_t* dst, const uint8_t* src, int64_t ctd_page_entry::*off, int ch, cudaStream_t st) {
+  const int n = int(pg.size());
   for (int i = 0; i < n;) {
     if (dev && dev[i].data) { ++i; continue; }
     int j = i;
     while (j + 1 < n && !(dev && dev[j + 1].data)) ++j;
-    const size_t lo = off(i), hi = off(j) + bytes(j);
+    const size_t lo = size_t(pg[size_t(i)].*off);
+    const size_t hi = size_t(pg[size_t(j)].*off) + size_t(pg[size_t(j)].ih) * size_t(pg[size_t(j)].iw) * ch;
     CK(cudaMemcpyAsync(dst + lo, src + lo, hi - lo, cudaMemcpyHostToDevice, st));
     i = j + 1;
   }
+  return CTD_OK;
+}
+
+// on `st`: a wait on the event of every device image of the n entries (entry by entry, in the order of `devs`), then
+// one gather launch over the n_gather entries of the device table d_tab (`rows` rows in all)
+static int wait_and_gather(ctd_handle* h, int n, std::initializer_list<const ctd_device_page*> devs, const void* d_tab,
+                           int n_gather, int rows, cudaStream_t st) {
+  for (int i = 0; i < n; ++i)
+    for (const ctd_device_page* d : devs)
+      if (d && d[i].data && d[i].event) CK(cudaStreamWaitEvent(st, static_cast<cudaEvent_t>(d[i].event), 0));
+  CK(gather_pages_launch(static_cast<const GatherPage*>(d_tab), n_gather, rows, st));
   return CTD_OK;
 }
 
@@ -927,38 +1007,22 @@ static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* p
                             const ctd_net_output* outs, const int32_t* dtypes, int32_t refine_mode,
                             int32_t keep_undetected, int32_t textheight, int32_t results_on_device, void* results_host) {
   const char* entry = outs ? "ctd_submit_outputs" : "ctd_submit_pages";
-  if (!h || !pages || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (!pages || !results_host) return CTD_E_INVALID;
+  if (int rc = admit_batch(h, slot, n)) return rc;
   if (textheight != 0 && textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
   if (h->cfg.debug_skip_postproc) return ctd_fail(h, CTD_E_INVALID, "%s needs the full pipeline", entry);
   Slot& s = h->slot[slot];
-  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
-  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
-  // the offsets decide where the copies write: they must be the plan's
   std::vector<ctd_page_entry> pg(pages, pages + n);
   size_t in_bytes = 0, res_bytes = 0;
   if (int rc = ctd_pages_plan(pg.data(), n, net_h, net_w, &in_bytes, &res_bytes))
     return ctd_fail(h, rc, "the pages do not letterbox into a %dx%d net input", net_h, net_w);
-  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
-    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_pages_plan returns");
-  size_t rows = 0;
-  for (int i = 0; i < n; ++i) {
-    rows += size_t(pg[size_t(i)].ih);
-    if (keep_undetected && size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) > kCclMaxPixels)
-      return ctd_fail(h, CTD_E_CAPACITY, "page %d (%dx%d): refine_undetected_mask labels pages of at most 2^28 pixels", i,
-                      pg[size_t(i)].ih, pg[size_t(i)].iw);
-  }
-  if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
-  // pages in device memory: strides, and the first and last byte each page reads must be memory of this GPU
+  if (int rc = same_as_plan(h, pg, pages, "ctd_pages_plan")) return rc;
+  if (keep_undetected)
+    if (int rc = check_undetected_size(h, pg)) return rc;
+  if (int rc = check_batch_rows(h, pg)) return rc;
   CK(cudaSetDevice(h->cfg.device));
   int n_dev = 0;
-  for (int i = 0; i < n; ++i) {
-    if (!dev || !dev[i].data) {
-      if (!input_host) return ctd_fail(h, CTD_E_INVALID, "page %d is in neither input_host nor device memory", i);
-      continue;
-    }
-    if (int rc = check_device_image(h, "page", i, dev[i], pg[size_t(i)].ih, pg[size_t(i)].iw, 3)) return rc;
-    ++n_dev;
-  }
+  if (int rc = check_sources(h, "page", dev, pg, 3, input_host, &n_dev)) return rc;
   // the outputs: shapes, and each map device memory of this GPU or a host span copied into the slot's out_in
   const int no = 5 + h->cfg.nc, ws_rows = rows_per_image(net_h, net_w);
   std::vector<std::array<size_t, 3>> host_bytes(outs ? size_t(n) : 0), host_off(outs ? size_t(n) : 0);
@@ -1016,10 +1080,7 @@ static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* p
     tab[i] = PageGeom{e.page_off, e.mask_off - int64_t(hd.masks), e.ih, e.iw, e.unpad_h, e.unpad_w, row0, 0};
     row0 += e.ih;
     if (dev && dev[i].data) {
-      const ctd_device_page& d = dev[i];
-      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c,
-                                    s.pg_in.p + e.page_off, e.ih, e.iw, gather_rows,
-                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0, 3, 0};
+      gtab[n_gather++] = gather_entry(dev[i], s.pg_in.p + e.page_off, e, 3, gather_rows);
       gather_rows += e.ih;
     }
   }
@@ -1054,22 +1115,16 @@ static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* p
   }
   if (n_dev == 0) {
     CK(cudaMemcpyAsync(s.pg_in.p, input_host, in_bytes, cudaMemcpyHostToDevice, h->copy_in));
-  } else {
-    if (int rc = copy_host_runs(h, dev, n, s.pg_in.p, input_host, [&](int i) { return size_t(pg[size_t(i)].page_off); },
-                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; },
-                                h->copy_in))
-      return rc;
+  } else if (int rc = copy_host_images(h, dev, pg, s.pg_in.p, input_host, &ctd_page_entry::page_off, 3, h->copy_in)) {
+    return rc;
   }
   CK(cudaEventRecord(s.ev_in_done, h->copy_in));
   CK(cudaEventRecord(h->ev0, h->stream));
   CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
-  if (n_gather) {
-    for (int i = 0; i < n; ++i)
-      if (dev[i].data && dev[i].event) CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(dev[i].event), 0));
-    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(reinterpret_cast<const char*>(s.d_pg_tab) +
-                                                               h->pg_gather_off),
-                           n_gather, gather_rows, h->stream));
-  }
+  if (n_gather)
+    if (int rc = wait_and_gather(h, n, {dev}, reinterpret_cast<const char*>(s.d_pg_tab) + h->pg_gather_off, n_gather,
+                                 gather_rows, h->stream))
+      return rc;
   if (outs) {
     // the caller's outputs into the workspace the forward would have written, then the forward's NMS and DB tail
     for (int i = 0; i < n; ++i)
@@ -1169,16 +1224,13 @@ extern "C" int ctd_preprocess_pages(ctd_handle* h, const ctd_page_entry* pages, 
   if (!h || !pages || !dst || n < 1) return CTD_E_INVALID;
   if (format != CTD_PRE_F32_NCHW && format != CTD_PRE_F16_NCHW && format != CTD_PRE_U8_NHWC)
     return ctd_fail(h, CTD_E_INVALID, "format %d is not a CTD_PRE_* format", format);
-  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
+  if (int rc = check_batch_size(h, n)) return rc;
   std::vector<ctd_page_entry> pg(pages, pages + n);
   size_t in_bytes = 0, res_bytes = 0;
   if (int rc = ctd_pages_plan(pg.data(), n, net_h, net_w, &in_bytes, &res_bytes))
     return ctd_fail(h, rc, "the pages do not letterbox into a %dx%d net input", net_h, net_w);
-  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
-    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_pages_plan returns");
-  size_t rows = 0;
-  for (int i = 0; i < n; ++i) rows += size_t(pg[size_t(i)].ih);
-  if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
+  if (int rc = same_as_plan(h, pg, pages, "ctd_pages_plan")) return rc;
+  if (int rc = check_batch_rows(h, pg)) return rc;
   CK(cudaSetDevice(h->cfg.device));
   const size_t elem = format == CTD_PRE_F32_NCHW ? 4 : format == CTD_PRE_F16_NCHW ? 2 : 1;
   const size_t out_bytes = size_t(n) * 3 * size_t(net_h) * size_t(net_w) * elem;
@@ -1187,14 +1239,7 @@ extern "C" int ctd_preprocess_pages(ctd_handle* h, const ctd_page_entry* pages, 
     return ctd_fail(h, CTD_E_INVALID, "dst (%p, %zu bytes) is not device memory of GPU %d", dst, out_bytes,
                     h->cfg.device);
   int n_dev = 0;
-  for (int i = 0; i < n; ++i) {
-    if (!dev || !dev[i].data) {
-      if (!input_host) return ctd_fail(h, CTD_E_INVALID, "page %d is in neither input_host nor device memory", i);
-      continue;
-    }
-    if (int rc = check_device_image(h, "page", i, dev[i], pg[size_t(i)].ih, pg[size_t(i)].iw, 3)) return rc;
-    ++n_dev;
-  }
+  if (int rc = check_sources(h, "page", dev, pg, 3, input_host, &n_dev)) return rc;
   // everything from here on is ordered on the caller's stream, after the last call's reads of the page buffer and the
   // tables (ev_pre): a larger page buffer is a stream-ordered allocation, the old one a stream-ordered free
   cudaStream_t cs = static_cast<cudaStream_t>(stream);
@@ -1220,26 +1265,17 @@ extern "C" int ctd_preprocess_pages(ctd_handle* h, const ctd_page_entry* pages, 
     const ctd_page_entry& e = pg[size_t(i)];
     geo[i] = PageGeom{e.page_off, 0, e.ih, e.iw, e.unpad_h, e.unpad_w, 0, 0};
     if (dev && dev[i].data) {
-      const ctd_device_page& d = dev[i];
-      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c,
-                                    h->pre_in + e.page_off, e.ih, e.iw, gather_rows,
-                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0, 3, 0};
+      gtab[n_gather++] = gather_entry(dev[i], h->pre_in + e.page_off, e, 3, gather_rows);
       gather_rows += e.ih;
     }
   }
   const size_t tab_bytes = n_gather ? tab.size() : size_t(n) * sizeof(PageGeom);
   tab.resize((tab_bytes + 15) / 16 * 16);
   CK(upload_table_launch(tab.data(), tab.size(), h->d_pre_tab, cs));
-  if (n_dev < n) {
-    if (int rc = copy_host_runs(h, dev, n, h->pre_in, input_host, [&](int i) { return size_t(pg[size_t(i)].page_off); },
-                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; }, cs))
-      return rc;
-  }
-  if (n_gather) {
-    for (int i = 0; i < n; ++i)
-      if (dev[i].data && dev[i].event) CK(cudaStreamWaitEvent(cs, static_cast<cudaEvent_t>(dev[i].event), 0));
-    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(h->d_pre_tab + gather_off), n_gather, gather_rows, cs));
-  }
+  if (n_dev < n)
+    if (int rc = copy_host_images(h, dev, pg, h->pre_in, input_host, &ctd_page_entry::page_off, 3, cs)) return rc;
+  if (n_gather)
+    if (int rc = wait_and_gather(h, n, {dev}, h->d_pre_tab + gather_off, n_gather, gather_rows, cs)) return rc;
   CK(letterbox_tensor_launch(h->pre_in, reinterpret_cast<const PageGeom*>(h->d_pre_tab), n, dst, net_h, net_w, format,
                              reverse_channels != 0, cs));
   CK(cudaEventRecord(h->ev_pre, cs));
@@ -1251,13 +1287,12 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
                                  const ctd_device_page* dev_pages, const ctd_device_page* dev_masks,
                                  int32_t refine_mode, int32_t keep_undetected, int32_t refined_input,
                                  int32_t results_on_device, void* results_host) {
-  if (!h || !pages || !n_blocks || !results_host || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (!pages || !n_blocks || !results_host) return CTD_E_INVALID;
+  if (int rc = admit_batch(h, slot, n)) return rc;
   Slot& s = h->slot[slot];
-  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
-  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
   if (refined_input && (!keep_undetected || !input_host))
     return ctd_fail(h, CTD_E_INVALID, "a refined input needs keep_undetected and input_host");
-  // the offsets and windows decide what the copies and the refine touch: they must be the plan's
+  // the windows decide what the refine touches: they are the plan's
   std::vector<ctd_page_entry> pg(pages, pages + n);
   int64_t nb = 0;
   for (int i = 0; i < n; ++i) nb += std::max(n_blocks[i], 0);
@@ -1265,19 +1300,14 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
   size_t in_bytes = 0, res_bytes = 0;
   if (int rc = ctd_refine_plan(pg.data(), n, xyxy, n_blocks, win.data(), status.data(), &in_bytes, &res_bytes))
     return ctd_fail(h, rc, "ctd_refine_plan refuses the batch");
-  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
-    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_refine_plan returns");
+  if (int rc = same_as_plan(h, pg, pages, "ctd_refine_plan")) return rc;
+  if (keep_undetected)
+    if (int rc = check_undetected_size(h, pg)) return rc;
   const size_t total = in_bytes / 5;
   PipeJob job;
   job.wins.resize(size_t(n));
   job.boxes.resize(size_t(n));
-  size_t rows = 0;
   for (int i = 0, b = 0; i < n; ++i) {
-    const ctd_page_entry& e = pg[size_t(i)];
-    rows += size_t(e.ih);
-    if (keep_undetected && size_t(e.ih) * size_t(e.iw) > kCclMaxPixels)
-      return ctd_fail(h, CTD_E_CAPACITY, "page %d (%dx%d): refine_undetected_mask labels pages of at most 2^28 pixels", i,
-                      e.ih, e.iw);
     for (int k = 0; k < n_blocks[i]; ++k, ++b) {
       // refine_mask raises on such a block; refine_undetected_mask alone only compares the boxes
       if (!refined_input && status[size_t(b)] != 0)
@@ -1289,21 +1319,11 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
       job.boxes[size_t(i)].insert(job.boxes[size_t(i)].end(), xyxy + 4 * size_t(b), xyxy + 4 * size_t(b) + 4);
     }
   }
-  if (rows > size_t(INT32_MAX)) return ctd_fail(h, CTD_E_CAPACITY, "the pages of a batch have more than 2^31 rows");
+  if (int rc = check_batch_rows(h, pg)) return rc;
   CK(cudaSetDevice(h->cfg.device));
   int n_dev_pages = 0, n_dev_masks = 0;
-  for (int i = 0; i < n; ++i) {
-    const ctd_page_entry& e = pg[size_t(i)];
-    for (int m = 0; m < 2; ++m) {
-      const ctd_device_page* d = m ? dev_masks : dev_pages;
-      if (d && d[i].data) {
-        if (int rc = check_device_image(h, m ? "mask" : "page", i, d[i], e.ih, e.iw, m ? 1 : 3)) return rc;
-        ++(m ? n_dev_masks : n_dev_pages);
-      } else if (!input_host) {
-        return ctd_fail(h, CTD_E_INVALID, "%s %d is in neither input_host nor device memory", m ? "mask" : "page", i);
-      }
-    }
-  }
+  if (int rc = check_sources(h, "page", dev_pages, pg, 3, input_host, &n_dev_pages)) return rc;
+  if (int rc = check_sources(h, "mask", dev_masks, pg, 1, input_host, &n_dev_masks)) return rc;
   if (int rc = ensure_full_pipeline(h)) return rc;
   s.start(false, results_on_device != 0);
   // grown while the slot is idle: its collect has synchronised the work of its last batch.  pg_in: the packed pages;
@@ -1318,16 +1338,11 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
   for (int i = 0; i < n; ++i) {
     const ctd_page_entry& e = pg[size_t(i)];
     if (dev_pages && dev_pages[i].data) {
-      const ctd_device_page& d = dev_pages[i];
-      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c,
-                                    s.pg_in.p + e.page_off, e.ih, e.iw, gather_rows,
-                                    d.stride_c == 1 && d.stride_w == 3 ? 1 : 0, 3, 0};
+      gtab[n_gather++] = gather_entry(dev_pages[i], s.pg_in.p + e.page_off, e, 3, gather_rows);
       gather_rows += e.ih;
     }
     if (dev_masks && dev_masks[i].data) {
-      const ctd_device_page& d = dev_masks[i];
-      gtab[n_gather++] = GatherPage{d.data, (long long)d.stride_h, (long long)d.stride_w, 0, s.pg_res.p + e.mask_off,
-                                    e.ih, e.iw, gather_rows, d.stride_w == 1 ? 1 : 0, 1, 0};
+      gtab[n_gather++] = gather_entry(dev_masks[i], s.pg_res.p + e.mask_off, e, 1, gather_rows);
       gather_rows += e.ih;
     }
   }
@@ -1339,26 +1354,17 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
     CK(cudaMemcpyAsync(reinterpret_cast<char*>(s.d_pg_tab) + h->pg_gather_off, gtab, size_t(n_gather) * sizeof(GatherPage),
                        cudaMemcpyHostToDevice, cin));
   if (n_dev_pages < n)
-    if (int rc = copy_host_runs(h, dev_pages, n, s.pg_in.p, input_host,
-                                [&](int i) { return size_t(pg[size_t(i)].page_off); },
-                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; }, cin))
-      return rc;
+    if (int rc = copy_host_images(h, dev_pages, pg, s.pg_in.p, input_host, &ctd_page_entry::page_off, 3, cin)) return rc;
   if (n_dev_masks < n)
-    if (int rc = copy_host_runs(h, dev_masks, n, s.pg_res.p, host_frame,
-                                [&](int i) { return size_t(pg[size_t(i)].mask_off); },
-                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw); }, cin))
-      return rc;
+    if (int rc = copy_host_images(h, dev_masks, pg, s.pg_res.p, host_frame, &ctd_page_entry::mask_off, 1, cin)) return rc;
   if (refined_input) CK(cudaMemcpyAsync(s.pg_res.p + total, host_frame + total, total, cudaMemcpyHostToDevice, cin));
   CK(cudaEventRecord(s.ev_in_done, cin));
   CK(cudaStreamWaitEvent(h->stream, s.ev_in_done, 0));
-  if (n_gather) {
-    for (int i = 0; i < n; ++i)
-      for (const ctd_device_page* d : {dev_pages, dev_masks})
-        if (d && d[i].data && d[i].event) CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(d[i].event), 0));
-    CK(gather_pages_launch(reinterpret_cast<const GatherPage*>(reinterpret_cast<const char*>(s.d_pg_tab) +
-                                                               h->pg_gather_off),
-                           n_gather, gather_rows, h->stream));
-  }
+  if (n_gather)
+    if (int rc = wait_and_gather(h, n, {dev_pages, dev_masks},
+                                 reinterpret_cast<const char*>(s.d_pg_tab) + h->pg_gather_off, n_gather, gather_rows,
+                                 h->stream))
+      return rc;
   CK(cudaEventRecord(s.ev_out_ready, h->stream));
   job.refine = true;
   job.slot = slot; job.refine_mode = refine_mode;
@@ -1383,11 +1389,10 @@ extern "C" int ctd_submit_regions(ctd_handle* h, int32_t slot, const ctd_page_en
                                   const ctd_region_line* lines, const int32_t* n_lines, int32_t textheight,
                                   const uint8_t* input_host, const ctd_device_page* dev_pages,
                                   int32_t results_on_device) {
-  if (!h || !pages || !n_lines || slot < 0 || slot > 1 || n < 1) return CTD_E_INVALID;
+  if (!pages || !n_lines) return CTD_E_INVALID;
+  if (int rc = admit_batch(h, slot, n)) return rc;
   if (textheight < 2) return ctd_fail(h, CTD_E_INVALID, "textheight %d < 2", textheight);
   Slot& s = h->slot[slot];
-  if (s.busy) return ctd_fail(h, CTD_E_INVALID, "slot %d has an uncollected submission", slot);
-  if (n > h->cfg.max_batch) return ctd_fail(h, CTD_E_CAPACITY, "batch %d exceeds max_batch %d", n, h->cfg.max_batch);
   int64_t total_lines = 0;
   for (int i = 0; i < n; ++i) {
     if (n_lines[i] < 0) return ctd_fail(h, CTD_E_INVALID, "page %d: n_lines %d < 0", i, n_lines[i]);
@@ -1400,35 +1405,24 @@ extern "C" int ctd_submit_regions(ctd_handle* h, int32_t slot, const ctd_page_en
     if (ih < 1 || iw < 1 || ih >= 32767 || iw >= 32767)
       return ctd_fail(h, CTD_E_SHAPE, "page %d (%dx%d): the crop planner takes pages with sides in [1, 32767)", i, ih, iw);
   }
-  // the offsets decide where the copies write: they must be the ones ctd_refine_plan lays out (no blocks)
+  // the pages are laid out as ctd_refine_plan lays them out with no blocks
   std::vector<ctd_page_entry> pg(pages, pages + n);
   const std::vector<int32_t> no_blocks(static_cast<size_t>(n), 0);
   size_t in_bytes = 0, res_bytes = 0;
   if (int rc = ctd_refine_plan(pg.data(), n, nullptr, no_blocks.data(), nullptr, nullptr, &in_bytes, &res_bytes))
     return ctd_fail(h, rc, "ctd_refine_plan refuses the pages");
-  if (memcmp(pg.data(), pages, size_t(n) * sizeof(ctd_page_entry)) != 0)
-    return ctd_fail(h, CTD_E_INVALID, "the page entries are not the ones ctd_refine_plan returns");
+  if (int rc = same_as_plan(h, pg, pages, "ctd_refine_plan")) return rc;
   const size_t total = in_bytes / 5;
   CK(cudaSetDevice(h->cfg.device));
   int n_dev = 0;
-  for (int i = 0; i < n; ++i) {
-    if (dev_pages && dev_pages[i].data) {
-      if (int rc = check_device_image(h, "page", i, dev_pages[i], pg[size_t(i)].ih, pg[size_t(i)].iw, 3)) return rc;
-      ++n_dev;
-    } else if (!input_host) {
-      return ctd_fail(h, CTD_E_INVALID, "page %d is in neither input_host nor device memory", i);
-    }
-  }
+  if (int rc = check_sources(h, "page", dev_pages, pg, 3, input_host, &n_dev)) return rc;
   if (int rc = ensure_full_pipeline(h)) return rc;
   s.start(true, results_on_device != 0, false);
   // grown while the slot is idle: its collect has synchronised the work of its last batch.  The host pages are
   // copied into pg_in at their offsets; the device pages are read where they are
   if (n_dev < n) {
     if (int rc = s.pg_in.grow(h, 3 * total, std::nullopt)) return rc;
-    if (int rc = copy_host_runs(h, dev_pages, n, s.pg_in.p, input_host,
-                                [&](int i) { return size_t(pg[size_t(i)].page_off); },
-                                [&](int i) { return size_t(pg[size_t(i)].ih) * size_t(pg[size_t(i)].iw) * 3; },
-                                h->copy_in))
+    if (int rc = copy_host_images(h, dev_pages, pg, s.pg_in.p, input_host, &ctd_page_entry::page_off, 3, h->copy_in))
       return rc;
   }
   CK(cudaEventRecord(s.ev_in_done, h->copy_in));

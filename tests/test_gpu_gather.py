@@ -1,6 +1,6 @@
 """-m gpu: the layout stage between the caller's memory and the kernels of a batch, byte for byte.
 
-* gather_pages_kernel (csrc/gather.cu) and copy_host_runs: every batch of tests/gather_cases.py runs once with host
+* gather_pages_kernel (csrc/gather.cu) and copy_host_images: every batch of tests/gather_cases.py runs once with host
   pages (and masks) of the same sizes filled with a sentinel, then once with its own images, through ctd_submit_pages
   or through ctd_submit_refine with no blocks (which leaves the mask plane as gathered).  The packed pages (and the mask
   plane) are read back with ctd_debug_read_slot: every image's bytes at its page_off (mask_off) must equal the numpy
