@@ -20,7 +20,8 @@ from pathlib import Path
 
 import numpy as np
 
-from .inference import REFINEMASK_ANNOTATION, REFINEMASK_INPAINT, TextDetector, check_page, decode_files
+from .inference import REFINEMASK_ANNOTATION, REFINEMASK_INPAINT, TextDetector
+from .kernel_jobs import check_page, decode_files
 from .png import is_png, png_probe
 from .textblock import TextBlock
 

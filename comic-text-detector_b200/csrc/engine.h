@@ -75,46 +75,45 @@ struct PagesHead {
 };
 PagesHead pages_head(int n);
 
-// one page of a batch as phases B and C see it
+// one page of a job as its host and device stages see it
 struct JobPage {
   int ih, iw;
   float ratio_x, ratio_y;   // resize_ratio (inference.py:148)
   size_t off;               // pixel offset P_i of the page in the image (x3), mask and mask_refined planes
-  char* section;            // its block section in results_host
+  char* section;            // with phase-A rows: the block section phase B fills from them and the host mask
+  const uint8_t* mask;
+  // from the caller or phase B: refine windows (x1 y1 x2 y2), block boxes, lines; the lines' crop plan (textheight)
+  std::vector<int32_t> wins, boxes;
+  std::vector<ctd_region_line> lines;
+  std::vector<ctd_region> plan;
+  size_t plan_bytes = 0;
 };
 
-// phases B and C of a submitted batch: what the worker thread needs of it
+// device planes of pages at their pixel offsets, `total` pixels each: image (x3), mask, mask_refined, and the second
+// refine output and threshold planes of refine_undetected_mask
+struct Planes {
+  const uint8_t* img;
+  uint8_t *mask, *ref, *ref2, *thr;
+  size_t total;
+};
+
+// a submitted job: what its host stage and device stage need of it
 struct PipeJob {
   int slot = 0, refine_mode = 0;
   char* results_host = nullptr;
+  bool rows = false;               // phase-A rows at `head` in results_host: phase B makes the pages' inputs from them
   PagesHead head{};                // phase-A rows and the mask plane in results_host
   size_t refined = 0;              // mask_refined plane in results_host
   std::vector<JobPage> pages;
-  size_t total = 0;                // pixels of each plane (every page's, each rounded up to 256)
-  // device planes: the pages, their masks, mask_refined, and (keep_undetected) 2 * total bytes of the second refine
-  // output and threshold planes
-  const uint8_t* d_img = nullptr;
-  uint8_t* d_mask = nullptr;
-  uint8_t* d_ref = nullptr;
-  uint8_t* d_aux = nullptr;
-  // ctd_submit_full: the block sections are uploaded here (blocks_bytes from the first page's section) before the
-  // refine, so ctd_device_arena holds the same bytes as results_host
+  Planes pl{};                     // mask and ref NULL without masks; ref2 and thr only with keep_undetected
+  // ctd_submit_full: the block sections uploaded here before the refine, so ctd_device_arena holds results_host's
   uint8_t* d_blocks = nullptr;
   size_t blocks_bytes = 0;
   int keep_undetected = 0;
-  int textheight = 0;   // > 0: also crop every text line of every page (ctd_submit_pages)
+  int textheight = 0;          // > 0: also crop every text line of every page
   int results_on_device = 0;   // mask_refined, the modified mask and the crops stay on the device (ctd_collect_device)
-  // ctd_submit_refine: phase C alone, on each page's refine windows (x1 y1 x2 y2 each) and block boxes; with
-  // refined_input, d_ref holds the caller's mask_refined and only refine_undetected_mask runs
-  bool refine = false;
-  int refined_input = 0;
-  std::vector<std::vector<int32_t>> wins, boxes;
-  // ctd_submit_regions: the crops alone, of the caller's lines (n_lines[i] of page i, in page order) at textheight;
-  // dev[i].data != NULL: page i is read where it is in device memory (else from d_img at its offset)
-  bool regions = false;
-  std::vector<ctd_region_line> lines;
-  std::vector<int32_t> n_lines;
-  std::vector<ctd_device_page> dev;
+  int refined_input = 0;       // pl.ref holds the caller's mask_refined: only refine_undetected_mask runs
+  std::vector<ctd_device_page> dev;   // dev[i].data != NULL: the crops read page i there, else from pl.img
   // ctd_submit_outputs: per page the ingest's non-finite bits (bit 0 blks, 1 mask, 2 lines; host copy, pinned),
   // complete with phase A's results; a set bit fails the batch before phase B
   const int32_t* nonfinite = nullptr;

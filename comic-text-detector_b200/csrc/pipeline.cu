@@ -16,7 +16,9 @@
 // pages may already be in device memory (any strides; one gather_pages_kernel launch packs them, gather.cu) and the
 // masks and crops may stay there (ctd_collect_device).  ctd_submit_refine runs phase C alone on caller pages, masks
 // and block boxes (textmask.refine_mask / refine_undetected_mask, MaskRefiner) through the same two-slot schedule, and
-// ctd_submit_regions the crop stage alone on caller pages and text lines (regions.RegionCropper).
+// ctd_submit_regions the crop stage alone on caller pages and text lines (regions.RegionCropper).  Every job, on the
+// worker or inline in ctd_detect_page, runs one host stage (phase B, crop plans) and one device stage (crops, phase C);
+// which parts run follows from what the job carries, not from the entry that made it.
 // ctd_preprocess_pages letterboxes a batch of pages into a caller's network input tensor on the caller's stream, with
 // no slot (preprocess.Preprocessor).
 #include <cuda.h>
@@ -152,14 +154,14 @@ struct PageIn {
 
 // page i of a batch whose phase-A rows are at `head` in `res` ([n][300][6] detections, [n] counts, [n][1000][8] line
 // boxes, [n][1000] scores, [n] counts), with its page-sized host mask
-PageIn page_in(const char* res, const PagesHead& head, int i, const JobPage& p, const uint8_t* mask) {
+PageIn page_in(const char* res, const PagesHead& head, int i, const JobPage& p) {
   PageIn in;
   in.det = reinterpret_cast<const float*>(res + head.det) + size_t(i) * 300 * 6;
   in.n_det = std::min(std::max(reinterpret_cast<const int32_t*>(res + head.cnt)[i], 0), 300);
   in.line_boxes = reinterpret_cast<const int16_t*>(res + head.lb) + size_t(i) * 1000 * 8;
   in.line_scores = reinterpret_cast<const float*>(res + head.ls) + size_t(i) * 1000;
   in.n_lines = std::min(std::max(reinterpret_cast<const int32_t*>(res + head.lc)[i], 0), 1000);
-  in.mask = mask; in.im_w = p.iw; in.im_h = p.ih; in.ratio_x = p.ratio_x; in.ratio_y = p.ratio_y;
+  in.mask = p.mask; in.im_w = p.iw; in.im_h = p.ih; in.ratio_x = p.ratio_x; in.ratio_y = p.ratio_y;
   return in;
 }
 
@@ -174,8 +176,10 @@ std::array<int64_t, 4> expand_textwindow(int64_t x1, int64_t y1, int64_t x2, int
 }
 
 // inference.py:101-114 (postprocess_yolo casts), 158-172 (box_thresh, line rescale), textblock.group_output,
-// expand_textwindow(.., 16): fills the page's block section and appends its refine windows
-int host_group_page(const PageIn& in, char* section, const BlockSection& L, std::vector<int32_t>& win_out) {
+// expand_textwindow(.., 16): fills p's block section, its refine windows and block boxes, and with lines_out the
+// ctd_region_line records of its lines in block then line order (textblock.region_lines)
+int host_group_page(const PageIn& in, const BlockSection& L, bool lines_out, JobPage& p) {
+  char* section = p.section;
   std::vector<int32_t> bxy(size_t(in.n_det) * 4), bcls(size_t(in.n_det));
   for (int i = 0; i < in.n_det; ++i) {
     const float* d = in.det + 6 * i;
@@ -220,12 +224,24 @@ int host_group_page(const PageIn& in, char* section, const BlockSection& L, std:
   for (int i = 0; i < nb; ++i) { tl += rec[i].n_lines; td += rec[i].n_dist; }
   hdr->n_lines = tl;
   hdr->n_dist = td;
-  win_out.resize(size_t(nb) * 4);
   for (int i = 0; i < nb; ++i) {
     const int32_t* xy = rec[i].xyxy;
     const auto win = expand_textwindow(xy[0], xy[1], xy[2], xy[3], in.im_w, in.im_h);   // inside the page
-    for (int k = 0; k < 4; ++k) win_out[size_t(4 * i + k)] = int32_t(win[k]);
+    for (int64_t v : win) p.wins.push_back(int32_t(v));
+    p.boxes.insert(p.boxes.end(), xy, xy + 4);
   }
+  if (!lines_out) return CTD_OK;
+  p.lines.reserve(size_t(tl));
+  for (int b = 0; b < nb; ++b)
+    for (int k = 0; k < rec[b].n_lines; ++k) {
+      ctd_region_line l{};
+      const int32_t* q = lout + size_t(rec[b].line_off + k) * 8;
+      for (int j = 0; j < 8; ++j) l.quad[j] = double(q[j]);
+      l.language = rec[b].language;
+      l.vertical = rec[b].vertical ? 1 : 0;
+      l.font_size = rec[b].font_size;
+      p.lines.push_back(l);
+    }
   return CTD_OK;
 }
 
@@ -257,22 +273,13 @@ __global__ void or_kernel(uint8_t* __restrict__ dst, const uint8_t* __restrict__
   if (i < n) dst[i] |= src[i];
 }
 
-// device planes of a set of pages, each page's at its pixel offset: the image (x3), the mask, mask_refined, and the
-// second refine output and threshold planes of refine_undetected_mask; `total` pixels each
-struct Planes {
-  const uint8_t* img;
-  uint8_t *mask, *ref, *ref2, *thr;
-  size_t total;
-};
-
 // refine_undetected_mask (textmask.py:135-156) for a set of pages: one prep launch over all planes, connected
 // components + stats of each page on `st` (the scratch `cc` grows here), the host loop over each page's stats rows
-// against its blocks (boxes[i]: x1 y1 x2 y2 of each block of page i), then one refine launch for the extra windows of
-// all pages and one OR launch.  The masks are modified in place, as in the reference.
+// against its block boxes, then one refine launch for the extra windows of all pages and one OR launch.  The masks
+// are modified in place, as in the reference.
 // Synchronises `st` once for the label counts and once for the stats rows.
-int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const std::vector<std::vector<int32_t>>& boxes,
-                      const Planes& pl, int refine_mode, cudaStream_t st, DevBuf& cc, DevBuf& refine_scratch,
-                      char* pinned, size_t pinned_cap) {
+int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Planes& pl, int refine_mode,
+                      cudaStream_t st, DevBuf& cc, DevBuf& refine_scratch, char* pinned, size_t pinned_cap) {
   auto al = [](size_t v) { return (v + 255) / 256 * 256; };
   const int n = int(pages.size());
   const size_t total_px = pl.total;
@@ -317,7 +324,7 @@ int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const st
   RefineJob rj2;
   for (int i = 0; i < n; ++i) {
     const JobPage& p = pages[size_t(i)];
-    const std::vector<int32_t>& xyxy = boxes[size_t(i)];
+    const std::vector<int32_t>& xyxy = p.boxes;
     const size_t nb = xyxy.size() / 4;
     bool first_valid = true;
     for (int li = 0; li < n_lab[size_t(i)]; ++li) {
@@ -348,35 +355,6 @@ int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const st
     CK(cudaGetLastError());
   }
   return CTD_OK;
-}
-
-// phase C of a set of pages, mask_refined already zeroed: one refine launch over the windows of every page
-// (wins[i]: x1 y1 x2 y2 each), then with keep_undetected refine_undetected_mask against the pages' block boxes
-// (boxes[i], read only then).  Stream-ordered on `st` with the scratch that belongs to it; `pinned` (optional,
-// pinned_cap bytes) stages the window tables.
-int phase_c(ctd_handle* h, const std::vector<JobPage>& pages, const std::vector<std::vector<int32_t>>& wins,
-            const std::vector<std::vector<int32_t>>& boxes, const Planes& pl, int refine_mode, bool keep_undetected,
-            cudaStream_t st, DevBuf& refine_scratch, DevBuf& cc, char* pinned, size_t pinned_cap) {
-  RefineJob rj;
-  for (size_t i = 0; i < pages.size(); ++i)
-    for (size_t k = 0; k + 3 < wins[i].size(); k += 4)
-      rj.add(wins[i][k], wins[i][k + 1], wins[i][k + 2], wins[i][k + 3], pages[i].off, pages[i].iw, pages[i].ih);
-  char* stage = rj.table_bytes() <= pinned_cap ? pinned : nullptr;   // else: pageable + sync
-  if (int rc = launch_refine(h, rj, pl.img, pl.mask, refine_mode, pl.ref, st, refine_scratch, stage)) return rc;
-  if (!keep_undetected) return CTD_OK;
-  return refine_undetected(h, pages, boxes, pl, refine_mode, st, cc, refine_scratch, pinned, pinned_cap);
-}
-
-// the block boxes of each page's block section (the detector's own blocks), for refine_undetected
-std::vector<std::vector<int32_t>> section_boxes(const std::vector<JobPage>& pages) {
-  const BlockSection bs = block_section_layout();
-  std::vector<std::vector<int32_t>> boxes(pages.size());
-  for (size_t i = 0; i < pages.size(); ++i) {
-    const int nb = reinterpret_cast<const ctd_page_blocks*>(pages[i].section)->n_blocks;
-    const ctd_block* rec = reinterpret_cast<const ctd_block*>(pages[i].section + bs.rec_off);
-    for (int b = 0; b < nb; ++b) boxes[i].insert(boxes[i].end(), rec[b].xyxy, rec[b].xyxy + 4);
-  }
-  return boxes;
 }
 }  // namespace
 
@@ -486,42 +464,13 @@ extern "C" int ctd_refine_plan(ctd_page_entry* pages, int32_t n, const int32_t* 
   return CTD_OK;
 }
 
-// ctd_region_plan of every line of one page's block section, in block then line order (textblock.region_lines)
-static int plan_page_regions(const char* section, const BlockSection& bs, int iw, int ih, int textheight,
-                             std::vector<ctd_region>& plan, size_t* bytes) {
-  const ctd_page_blocks* hdr = reinterpret_cast<const ctd_page_blocks*>(section);
-  const ctd_block* rec = reinterpret_cast<const ctd_block*>(section + bs.rec_off);
-  const int32_t* quads = reinterpret_cast<const int32_t*>(section + bs.lines_off);
-  std::vector<ctd_region_line> lines;
-  lines.reserve(size_t(std::max(hdr->n_lines, 0)));
-  for (int b = 0; b < hdr->n_blocks; ++b)
-    for (int k = 0; k < rec[b].n_lines; ++k) {
-      ctd_region_line l{};
-      const int32_t* q = quads + size_t(rec[b].line_off + k) * 8;
-      for (int j = 0; j < 8; ++j) l.quad[j] = double(q[j]);
-      l.language = rec[b].language;
-      l.vertical = rec[b].vertical ? 1 : 0;
-      l.font_size = rec[b].font_size;
-      lines.push_back(l);
-    }
-  plan.resize(lines.size());
-  *bytes = 0;
-  if (lines.empty()) return CTD_OK;   // nothing to plan, whatever the page size
-  return ctd_region_plan(lines.data(), int32_t(lines.size()), iw, ih, textheight, plan.data(), bytes);
-}
-
-// the device planes of a submitted batch
-static Planes job_planes(const PipeJob& job) {
-  return Planes{job.d_img, job.d_mask, job.d_ref, job.d_aux, job.d_aux ? job.d_aux + job.total : nullptr, job.total};
-}
-
-// the end of a batch on the worker's stream `st`: the masks refine_undetected_mask modified and mask_refined back to
-// results_host (unless they stay on the device), then the batch's done event
+// the end of a job on the worker's stream `st`: the masks refine_undetected_mask modified and mask_refined back to
+// results_host (unless they stay on the device; a job without masks has none), then the job's done event
 static int finish_batch(ctd_handle* h, const PipeJob& job, cudaStream_t st) {
-  if (!job.results_on_device) {
+  if (!job.results_on_device && job.pl.ref) {
     char* res = job.results_host;
-    if (job.keep_undetected) CK(cudaMemcpyAsync(res + job.head.masks, job.d_mask, job.total, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(res + job.refined, job.d_ref, job.total, cudaMemcpyDeviceToHost, st));
+    if (job.keep_undetected) CK(cudaMemcpyAsync(res + job.head.masks, job.pl.mask, job.pl.total, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(res + job.refined, job.pl.ref, job.pl.total, cudaMemcpyDeviceToHost, st));
   }
   CK(cudaEventRecord(h->slot[job.slot].ev_post_done, st));
   return CTD_OK;
@@ -537,19 +486,18 @@ static std::vector<RegionPage> region_pages(const PipeJob& job) {
       const ctd_device_page& d = job.dev[i];
       src.push_back(RegionPage{d.data, (long long)d.stride_h, (long long)d.stride_w, (long long)d.stride_c, p.ih, p.iw});
     } else {
-      src.push_back(RegionPage{job.d_img + p.off * 3, (long long)p.iw * 3, 3, 1, p.ih, p.iw});
+      src.push_back(RegionPage{job.pl.img + p.off * 3, (long long)p.iw * 3, 3, 1, p.ih, p.iw});
     }
   }
   return src;
 }
 
-// the crop stage of a batch, on the worker's stream `st`: the pages' plans (plans[i], plan_bytes[i] packed bytes each)
-// concatenated with each page's crops after the previous page's into the slot's crop plan, the tables staged in the
-// slot's pinned crop buffer, one k_warp_regions launch over every page where it is (src[i]), and the pixels back into
-// the same pinned buffer after the tables (to_host), else left after the tables in d_crop.  A batch without a crop
-// launches and allocates nothing.
-static int crop_stage(ctd_handle* h, Slot& s, const std::vector<RegionPage>& src,
-                      const std::vector<std::vector<ctd_region>>& plans, const std::vector<size_t>& plan_bytes,
+// the crop stage of a batch, on the worker's stream `st`: the pages' plans (pages[i].plan, plan_bytes packed bytes
+// each) concatenated with each page's crops after the previous page's into the slot's crop plan, the tables staged in
+// the slot's pinned crop buffer, one k_warp_regions launch over every page where it is (src[i]), and the pixels back
+// into the same pinned buffer after the tables (to_host), else left after the tables in d_crop.  A batch without a
+// crop launches and allocates nothing.
+static int crop_stage(ctd_handle* h, Slot& s, const std::vector<RegionPage>& src, const std::vector<JobPage>& pages,
                       bool to_host, cudaStream_t st) {
   const int n = int(src.size());
   RegionJob rg;
@@ -558,7 +506,7 @@ static int crop_stage(ctd_handle* h, Slot& s, const std::vector<RegionPage>& src
   s.crop_base.assign(size_t(n) + 1, 0);
   size_t base = 0;
   for (int i = 0; i < n; ++i) {
-    const std::vector<ctd_region>& p = plans[size_t(i)];
+    const std::vector<ctd_region>& p = pages[size_t(i)].plan;
     if (int bad = rg.add(p.data(), int(p.size()), src[size_t(i)], (long long)base); bad >= 0)
       return ctd_fail(h, CTD_E_INVALID, "malformed crop plan entry %d on page %d of the batch", bad, i);
     s.crop_first[size_t(i)] = int32_t(s.crop_plan.size());
@@ -567,7 +515,7 @@ static int crop_stage(ctd_handle* h, Slot& s, const std::vector<RegionPage>& src
       r.offset += int64_t(base);
       s.crop_plan.push_back(r);
     }
-    base += plan_bytes[size_t(i)];
+    base += pages[size_t(i)].plan_bytes;
   }
   s.crop_first[size_t(n)] = int32_t(s.crop_plan.size());
   s.crop_base[size_t(n)] = base;
@@ -591,31 +539,23 @@ static int crop_stage(ctd_handle* h, Slot& s, const std::vector<RegionPage>& src
   return CTD_OK;
 }
 
-// phases B and C of a submitted batch, on the worker thread
-static int run_batch(ctd_handle* h, const PipeJob& job) {
-  Slot& s = h->slot[job.slot];
+// The host stage of a job, on the host threads: with phase-A rows, phase B of each page (group_output fills its block
+// section, windows, boxes and with a textheight its lines); with a textheight, the crop plan of each page's lines.
+// Reports the first page group_output failed on, else the first page the planner refused.
+static int host_stage(ctd_handle* h, PipeJob& job) {
   const int n = int(job.pages.size());
-  CK(cudaEventSynchronize(s.ev_out_done));          // phase A results are in results_host
-  for (int i = 0; job.nonfinite && i < n; ++i)
-    if (const int32_t f = job.nonfinite[i])
-      return ctd_fail(h, CTD_E_INVALID, "page %d of the batch: a non-finite value (NaN or inf) in its %s", i,
-                      (f & 1) ? "blks" : (f & 2) ? "mask" : "lines_map");
-  char* res = job.results_host;
+  if (!job.rows && job.textheight <= 0) return CTD_OK;
   const BlockSection bs = block_section_layout();
-  std::vector<std::vector<int32_t>> wins(static_cast<size_t>(n));
-  std::vector<int> prc(size_t(n), CTD_OK);
-  // text-line crops: each page's plan on the host threads, right after its group_output
-  const bool crops = job.textheight > 0;
-  std::vector<std::vector<ctd_region>> plans(crops ? size_t(n) : 0);
-  std::vector<size_t> plan_bytes(size_t(n), 0);
-  std::vector<int> crc(size_t(n), CTD_OK);
+  std::vector<int> prc(size_t(n), CTD_OK), crc(size_t(n), CTD_OK);
   for_each_page(n, h->host_threads, [&](int i) {
-    const JobPage& p = job.pages[size_t(i)];
-    const uint8_t* mask = reinterpret_cast<const uint8_t*>(res + job.head.masks + p.off);
-    prc[size_t(i)] = host_group_page(page_in(res, job.head, i, p, mask), p.section, bs, wins[size_t(i)]);
-    if (crops && prc[size_t(i)] == CTD_OK)
-      crc[size_t(i)] = plan_page_regions(p.section, bs, p.iw, p.ih, job.textheight, plans[size_t(i)],
-                                         &plan_bytes[size_t(i)]);
+    JobPage& p = job.pages[size_t(i)];
+    if (job.rows) prc[size_t(i)] = host_group_page(page_in(job.results_host, job.head, i, p), bs, job.textheight > 0, p);
+    if (job.textheight > 0 && prc[size_t(i)] == CTD_OK) {
+      p.plan.resize(p.lines.size());
+      if (!p.lines.empty())   // nothing to plan, whatever the page size
+        crc[size_t(i)] = ctd_region_plan(p.lines.data(), int32_t(p.lines.size()), p.iw, p.ih, job.textheight,
+                                         p.plan.data(), &p.plan_bytes);
+    }
   });
   for (int i = 0; i < n; ++i)
     if (prc[size_t(i)] != CTD_OK) return ctd_fail(h, prc[size_t(i)], "group_output failed on page %d of the batch", i);
@@ -623,71 +563,52 @@ static int run_batch(ctd_handle* h, const PipeJob& job) {
     if (crc[size_t(i)] != CTD_OK)
       return ctd_fail(h, crc[size_t(i)], "ctd_region_plan refused page %d of the batch (%dx%d, textheight %d)", i,
                       job.pages[size_t(i)].ih, job.pages[size_t(i)].iw, job.textheight);
-  // phase C on the post stream over the slot's resident pages and masks
-  cudaStream_t st = h->post;
-  // enqueued here for ctd_submit_pages, not at submit: a wait enqueued at submit time would also hold this batch's
-  // phase C behind the forward of every batch submitted before the worker reached it (ctd_submit_full enqueues it at
-  // submit as well)
-  CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // phase C never starts before its phase A copy
-  // ctd_submit_full: block sections to the device arena copy (one gather then moves everything)
+  return CTD_OK;
+}
+
+// The device stage of a job on `st`, with the refine and connected-components scratch that belong to `st` and an
+// optional pinned staging of the window tables (pinned_cap bytes): the block sections up to d_blocks, the crops of a
+// job with a textheight (in its slot), mask_refined cleared and one refine launch over the windows of every page
+// (unless the job has no mask_refined plane, or only a refined input), then with keep_undetected
+// refine_undetected_mask against the pages' block boxes.
+static int device_stage(ctd_handle* h, const PipeJob& job, cudaStream_t st, DevBuf& refine_scratch, DevBuf& cc,
+                        char* pinned, size_t pinned_cap) {
   if (job.d_blocks)
     CK(cudaMemcpyAsync(job.d_blocks, job.pages[0].section, job.blocks_bytes, cudaMemcpyHostToDevice, st));
-  if (crops)
-    if (int rc = crop_stage(h, s, region_pages(job), plans, plan_bytes, !job.results_on_device, st)) return rc;
-  CK(cudaMemsetAsync(job.d_ref, 0, job.total, st));
-  const auto boxes = job.keep_undetected ? section_boxes(job.pages) : std::vector<std::vector<int32_t>>();
-  if (int rc = phase_c(h, job.pages, wins, boxes, job_planes(job), job.refine_mode, job.keep_undetected, st,
-                       h->post_refine, h->pg_cc, s.pinned, h->pipe_pinned_cap))
-    return rc;
-  return finish_batch(h, job, st);
-}
-
-// ctd_submit_refine's batch on the worker: phase C on the caller's pages, masks and windows, or with a refined input
-// refine_undetected_mask alone
-static int run_refine_batch(ctd_handle* h, const PipeJob& job) {
-  Slot& s = h->slot[job.slot];
-  cudaStream_t st = h->post;
-  CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // the packed pages and masks are in place
-  const Planes pl = job_planes(job);
-  if (job.refined_input) {
-    if (int rc = refine_undetected(h, job.pages, job.boxes, pl, job.refine_mode, st, h->pg_cc, h->post_refine,
-                                   s.pinned, h->pipe_pinned_cap))
-      return rc;
-  } else {
-    CK(cudaMemsetAsync(job.d_ref, 0, job.total, st));
-    if (int rc = phase_c(h, job.pages, job.wins, job.boxes, pl, job.refine_mode, job.keep_undetected, st,
-                         h->post_refine, h->pg_cc, s.pinned, h->pipe_pinned_cap))
+  if (job.textheight > 0)
+    if (int rc = crop_stage(h, h->slot[job.slot], region_pages(job), job.pages, !job.results_on_device, st)) return rc;
+  if (job.pl.ref && !job.refined_input) {
+    CK(cudaMemsetAsync(job.pl.ref, 0, job.pl.total, st));
+    RefineJob rj;
+    for (const JobPage& p : job.pages)
+      for (size_t k = 0; k + 3 < p.wins.size(); k += 4)
+        rj.add(p.wins[k], p.wins[k + 1], p.wins[k + 2], p.wins[k + 3], p.off, p.iw, p.ih);
+    char* stage = rj.table_bytes() <= pinned_cap ? pinned : nullptr;   // else: pageable + sync
+    if (int rc = launch_refine(h, rj, job.pl.img, job.pl.mask, job.refine_mode, job.pl.ref, st, refine_scratch, stage))
       return rc;
   }
-  return finish_batch(h, job, st);
+  if (!job.keep_undetected) return CTD_OK;
+  return refine_undetected(h, job.pages, job.pl, job.refine_mode, st, cc, refine_scratch, pinned, pinned_cap);
 }
 
-// ctd_submit_regions's batch on the worker: each page's lines planned on the host threads, then the crop stage
-static int run_regions_batch(ctd_handle* h, const PipeJob& job) {
+// a submitted job on the worker thread: its phase-A rows awaited and checked, the host stage, then on the post stream
+// the device stage and the copy-back
+static int run_job(ctd_handle* h, PipeJob& job) {
   Slot& s = h->slot[job.slot];
-  const int n = int(job.pages.size());
-  std::vector<size_t> first(size_t(n) + 1, 0);
-  for (int i = 0; i < n; ++i) first[size_t(i) + 1] = first[size_t(i)] + size_t(job.n_lines[size_t(i)]);
-  std::vector<std::vector<ctd_region>> plans(static_cast<size_t>(n));
-  std::vector<size_t> plan_bytes(size_t(n), 0);
-  std::vector<int> prc(size_t(n), CTD_OK);
-  for_each_page(n, h->host_threads, [&](int i) {
-    const JobPage& p = job.pages[size_t(i)];
-    const int nl = job.n_lines[size_t(i)];
-    plans[size_t(i)].resize(size_t(nl));
-    if (nl > 0)
-      prc[size_t(i)] = ctd_region_plan(job.lines.data() + first[size_t(i)], nl, p.iw, p.ih, job.textheight,
-                                       plans[size_t(i)].data(), &plan_bytes[size_t(i)]);
-  });
-  for (int i = 0; i < n; ++i)
-    if (prc[size_t(i)] != CTD_OK)
-      return ctd_fail(h, prc[size_t(i)], "ctd_region_plan refused page %d of the batch (%dx%d, textheight %d)", i,
-                      job.pages[size_t(i)].ih, job.pages[size_t(i)].iw, job.textheight);
+  if (job.rows) {
+    CK(cudaEventSynchronize(s.ev_out_done));          // phase A results are in results_host
+    for (int i = 0; job.nonfinite && i < int(job.pages.size()); ++i)
+      if (const int32_t f = job.nonfinite[i])
+        return ctd_fail(h, CTD_E_INVALID, "page %d of the batch: a non-finite value (NaN or inf) in its %s", i,
+                        (f & 1) ? "blks" : (f & 2) ? "mask" : "lines_map");
+  }
+  if (int rc = host_stage(h, job)) return rc;
   cudaStream_t st = h->post;
-  CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // the host pages are in place, the device pages written
-  if (int rc = crop_stage(h, s, region_pages(job), plans, plan_bytes, !job.results_on_device, st)) return rc;
-  CK(cudaEventRecord(s.ev_post_done, st));
-  return CTD_OK;
+  // enqueued here, not at submit: a wait enqueued at submit time would also hold this job's device stage behind the
+  // forward of every batch submitted before the worker reached it (ctd_submit_full enqueues it at submit as well)
+  CK(cudaStreamWaitEvent(st, s.ev_out_ready, 0));   // the job's inputs are in place
+  if (int rc = device_stage(h, job, st, h->post_refine, h->pg_cc, s.pinned, h->pipe_pinned_cap)) return rc;
+  return finish_batch(h, job, st);
 }
 
 // ---- batch pipeline -------------------------------------------------------------------------------------------------
@@ -702,7 +623,7 @@ static void pipe_worker(ctd_handle* h) {
       job = std::move(h->pipe_queue.front());
       h->pipe_queue.pop_front();
     }
-    const int rc = job.refine ? run_refine_batch(h, job) : job.regions ? run_regions_batch(h, job) : run_batch(h, job);
+    const int rc = run_job(h, job);
     std::string err;
     if (rc != CTD_OK) err = h->err;
     {
@@ -824,14 +745,14 @@ extern "C" int ctd_submit_full(ctd_handle* h, int32_t slot, const uint8_t* pages
   PipeJob job;
   job.slot = slot; job.refine_mode = refine_mode;
   job.results_host = static_cast<char*>(results_host);
+  job.rows = true;
   job.head = PagesHead{L.det, L.cnt, L.lb, L.ls, L.lc, 0};
   job.refined = L.refined;
   for (int i = 0; i < n; ++i)
-    job.pages.push_back(JobPage{ph, pw, 1.f, 1.f, size_t(i) * px, job.results_host + L.blocks + size_t(i) * L.blocks_stride});
-  job.total = size_t(n) * px;
-  job.d_img = pages_on_device ? pages : s.d_stage_in;
-  job.d_mask = s.d_stage_out;
-  job.d_ref = s.d_stage_out + L.refined;
+    job.pages.push_back(JobPage{ph, pw, 1.f, 1.f, size_t(i) * px, job.results_host + L.blocks + size_t(i) * L.blocks_stride,
+                                reinterpret_cast<uint8_t*>(job.results_host) + size_t(i) * px});
+  job.pl = Planes{pages_on_device ? pages : s.d_stage_in, s.d_stage_out, s.d_stage_out + L.refined, nullptr, nullptr,
+                  size_t(n) * px};
   job.d_blocks = s.d_stage_out + L.blocks;
   job.blocks_bytes = size_t(n) * L.blocks_stride;
   queue_job(h, std::move(job));
@@ -1165,19 +1086,17 @@ static int submit_pages_job(ctd_handle* h, int32_t slot, const ctd_page_entry* p
   CK(cudaEventRecord(s.ev_out_done, h->copy_out));
   job.slot = slot; job.refine_mode = refine_mode;
   job.results_host = static_cast<char*>(results_host);
+  job.rows = true;
   job.head = hd;
   job.refined = size_t(pg[0].refined_off);
   for (const ctd_page_entry& e : pg) {
     Letterbox lb;
     letterbox_of(e.ih, e.iw, net_h, net_w, lb);   // planned: cannot fail
     job.pages.push_back(JobPage{e.ih, e.iw, lb.ratio_x, lb.ratio_y, size_t(e.mask_off) - hd.masks,
-                                job.results_host + e.blocks_off});
+                                job.results_host + e.blocks_off, reinterpret_cast<uint8_t*>(job.results_host) + e.mask_off});
   }
-  job.total = total;
-  job.d_img = s.pg_in.p;
-  job.d_mask = d_res + hd.masks;
-  job.d_ref = d_res + pg[0].refined_off;
-  job.d_aux = keep_undetected ? s.pg_aux.p : nullptr;
+  uint8_t* aux = keep_undetected ? s.pg_aux.p : nullptr;
+  job.pl = Planes{s.pg_in.p, d_res + hd.masks, d_res + pg[0].refined_off, aux, aux ? aux + total : nullptr, total};
   job.keep_undetected = keep_undetected ? 1 : 0;
   job.textheight = textheight;
   job.results_on_device = results_on_device ? 1 : 0;
@@ -1305,9 +1224,9 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
     if (int rc = check_undetected_size(h, pg)) return rc;
   const size_t total = in_bytes / 5;
   PipeJob job;
-  job.wins.resize(size_t(n));
-  job.boxes.resize(size_t(n));
+  for (const ctd_page_entry& e : pg) job.pages.push_back(JobPage{e.ih, e.iw, 1.f, 1.f, size_t(e.mask_off), nullptr, nullptr});
   for (int i = 0, b = 0; i < n; ++i) {
+    JobPage& p = job.pages[size_t(i)];
     for (int k = 0; k < n_blocks[i]; ++k, ++b) {
       // refine_mask raises on such a block; refine_undetected_mask alone only compares the boxes
       if (!refined_input && status[size_t(b)] != 0)
@@ -1315,8 +1234,8 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
                         xyxy[4 * b + 2], xyxy[4 * b + 3],
                         status[size_t(b)] == 1 ? "its window is empty, refine_mask raises on it"
                                                : "its window does not fit int32");
-      job.wins[size_t(i)].insert(job.wins[size_t(i)].end(), &win[4 * size_t(b)], &win[4 * size_t(b)] + 4);
-      job.boxes[size_t(i)].insert(job.boxes[size_t(i)].end(), xyxy + 4 * size_t(b), xyxy + 4 * size_t(b) + 4);
+      p.wins.insert(p.wins.end(), &win[4 * size_t(b)], &win[4 * size_t(b)] + 4);
+      p.boxes.insert(p.boxes.end(), xyxy + 4 * size_t(b), xyxy + 4 * size_t(b) + 4);
     }
   }
   if (int rc = check_batch_rows(h, pg)) return rc;
@@ -1366,17 +1285,12 @@ extern "C" int ctd_submit_refine(ctd_handle* h, int32_t slot, const ctd_page_ent
                                  h->stream))
       return rc;
   CK(cudaEventRecord(s.ev_out_ready, h->stream));
-  job.refine = true;
   job.slot = slot; job.refine_mode = refine_mode;
   job.results_host = static_cast<char*>(results_host);
   job.head.masks = 0;
   job.refined = total;
-  for (const ctd_page_entry& e : pg) job.pages.push_back(JobPage{e.ih, e.iw, 1.f, 1.f, size_t(e.mask_off), nullptr});
-  job.total = total;
-  job.d_img = s.pg_in.p;
-  job.d_mask = s.pg_res.p;
-  job.d_ref = s.pg_res.p + total;
-  job.d_aux = keep_undetected ? s.pg_aux.p : nullptr;
+  uint8_t* aux = keep_undetected ? s.pg_aux.p : nullptr;
+  job.pl = Planes{s.pg_in.p, s.pg_res.p, s.pg_res.p + total, aux, aux ? aux + total : nullptr, total};
   job.keep_undetected = keep_undetected ? 1 : 0;
   job.refined_input = refined_input ? 1 : 0;
   job.results_on_device = results_on_device ? 1 : 0;
@@ -1433,15 +1347,15 @@ extern "C" int ctd_submit_regions(ctd_handle* h, int32_t slot, const ctd_page_en
         CK(cudaStreamWaitEvent(h->stream, static_cast<cudaEvent_t>(dev_pages[i].event), 0));
   CK(cudaEventRecord(s.ev_out_ready, h->stream));
   PipeJob job;
-  job.regions = true;
   job.slot = slot;
   job.textheight = textheight;
   job.results_on_device = results_on_device ? 1 : 0;
-  for (const ctd_page_entry& e : pg) job.pages.push_back(JobPage{e.ih, e.iw, 1.f, 1.f, size_t(e.page_off) / 3, nullptr});
-  job.total = total;
-  job.d_img = s.pg_in.p;
-  job.lines.assign(lines, lines + total_lines);
-  job.n_lines.assign(n_lines, n_lines + n);
+  for (int i = 0, first = 0; i < n; first += n_lines[i++]) {
+    const ctd_page_entry& e = pg[size_t(i)];
+    job.pages.push_back(JobPage{e.ih, e.iw, 1.f, 1.f, size_t(e.page_off) / 3, nullptr, nullptr});
+    job.pages.back().lines.assign(lines + first, lines + first + n_lines[i]);
+  }
+  job.pl = Planes{s.pg_in.p, nullptr, nullptr, nullptr, nullptr, total};
   if (dev_pages) job.dev.assign(dev_pages, dev_pages + n);
   if (results_on_device) s.dev_pages = std::move(pg);
   queue_job(h, std::move(job));
@@ -1591,15 +1505,19 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
   CK(cudaMemcpyAsync(rows.data() + hd.lb, h->d_line_boxes, 1000 * 8 * 2, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(rows.data() + hd.ls, h->d_line_scores, 1000 * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(rows.data() + hd.lc, h->d_line_count, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemsetAsync(d_ref, 0, pxa, st));
   CK(cudaStreamSynchronize(st));
-  // phase B
+  // phase B and phase C as a one-page job's host and device stages, inline on the engine stream
   const BlockSection L = block_section_layout();
   std::vector<char> section(L.stride);
-  const std::vector<JobPage> pages{JobPage{ih, iw, geo.ratio_x, geo.ratio_y, 0, section.data()}};
-  std::vector<std::vector<int32_t>> wins(1);
-  if (int rc = host_group_page(page_in(rows.data(), hd, 0, pages[0], mask_out), section.data(), L, wins[0]))
-    return ctd_fail(h, rc, "group_output failed");
+  PipeJob job;
+  job.refine_mode = refine_mode;
+  job.keep_undetected = keep_undetected ? 1 : 0;
+  job.results_host = rows.data();
+  job.rows = true;
+  job.head = hd;
+  job.pages.push_back(JobPage{ih, iw, geo.ratio_x, geo.ratio_y, 0, section.data(), mask_out});
+  job.pl = Planes{d_page, d_mask, d_ref, d_ref2, d_thr, px};
+  if (int rc = host_stage(h, job)) return ctd_fail(h, rc, "group_output failed");
   const ctd_page_blocks* hdr = reinterpret_cast<const ctd_page_blocks*>(section.data());
   const ctd_block* rec = reinterpret_cast<const ctd_block*>(section.data() + L.rec_off);
   const int nb = hdr->n_blocks;
@@ -1612,12 +1530,8 @@ extern "C" int ctd_detect_page(ctd_handle* h, const uint8_t* page, int32_t ih, i
     memcpy(lines_out, section.data() + L.lines_off, size_t(hdr->n_lines) * 32);
     if (hdr->n_dist > 0) memcpy(dist_out, section.data() + L.dist_off, size_t(hdr->n_dist) * 8);
   }
-  // phase C; refine_undetected_mask modifies the page mask in place and it is returned, as in the reference
-  const Planes pl{d_page, d_mask, d_ref, d_ref2, d_thr, px};
-  const auto boxes = keep_undetected ? section_boxes(pages) : std::vector<std::vector<int32_t>>();
-  if (int rc = phase_c(h, pages, wins, boxes, pl, refine_mode, keep_undetected, st, h->refine_scratch, h->cc_scratch,
-                       nullptr, 0))
-    return rc;
+  // refine_undetected_mask modifies the page mask in place and it is returned, as in the reference
+  if (int rc = device_stage(h, job, st, h->refine_scratch, h->cc_scratch, nullptr, 0)) return rc;
   if (keep_undetected) CK(cudaMemcpyAsync(mask_out, d_mask, px, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(mask_refined_out, d_ref, px, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));

@@ -15,7 +15,6 @@ refine_mask on the GPU; ratio scaling, `group_output` and the window expansion i
 csrc/pipeline.cu).  This module is the reference-shaped Python surface over `ctd_detect_page` and, for batches,
 `ctd_submit_pages`.
 """
-from collections import deque
 from pathlib import Path
 from typing import List
 
@@ -23,9 +22,9 @@ import numpy as np
 
 from . import compiler, onnx_model
 from .binding import Engine, PREC_FP16_TC, PREC_FP32_SIMT
-from .jpeg import JpegDecoder, is_encoded, read_encoded
-from .png import PngDecoder, is_png
-from .textblock import (TextBlock, _check_textheight, blocks_from_records, group_output, overlap_area,  # noqa: F401
+from .jpeg import is_encoded
+from .kernel_jobs import BatchJob, _Encoded, _page_ready_event, check_page
+from .textblock import (TextBlock, blocks_from_records, check_textheight, group_output, overlap_area,  # noqa: F401
                         transformed_regions)
 
 REFINEMASK_INPAINT = 0
@@ -55,9 +54,10 @@ def letterbox(im, new_shape=(1024, 1024)):
     return im, (r, r), (dw, dh)
 
 
-class TextDetector:
+class TextDetector(BatchJob):
     lang_list = ['eng', 'ja', 'unknown']
     langcls2idx = {'eng': 0, 'ja': 1, 'unknown': 2}
+    item = "page"   # an undecodable page of detect_stream is "page <index>"
 
     def __init__(self, model_path, input_size=1024, device='cuda', half=False, nms_thresh=0.35, conf_thresh=0.4,
                  mask_thresh=0.3, act='leaky', precision=None, device_index=0, max_batch=1):
@@ -86,37 +86,9 @@ class TextDetector:
         self.program = compiler.compile_checkpoint(ckpt, head_act=act)
         # DB threshold is hard-coded 0.3 in the reference (inference.py:139 ignores mask_thresh)
         # max_batch: pages per GPU batch of detect_batch / detect_stream (the workspace is sized for it)
-        self.max_batch = int(max_batch)
-        self.device_index = int(device_index)
-        self.net = Engine(self.program, device=device_index, precision=precision, max_batch=self.max_batch, max_h=input_size[0],
-                          max_w=input_size[1], conf_thresh=conf_thresh, nms_thresh=nms_thresh, db_thresh=0.3)
-        self._jpeg = None   # the JpegDecoder of encoded pages, made on first use
-        self._png = None    # the PngDecoder of PNG pages, made on first use
-
-    def jpeg_decoder(self):
-        """the JpegDecoder this detector decodes encoded pages with (made on first use, closed with the detector)"""
-        if self._jpeg is None:
-            self._jpeg = JpegDecoder(self.device_index)
-        return self._jpeg
-
-    def png_decoder(self):
-        """the PngDecoder this detector decodes PNG pages with (made on first use, closed with the detector)"""
-        if self._png is None:
-            self._png = PngDecoder(self.device_index)
-        return self._png
-
-    def close(self):
-        self.net.close()
-        if self._jpeg is not None:
-            self._jpeg.close()
-            self._jpeg = None
-        if self._png is not None:
-            self._png.close()
-            self._png = None
-
-    def _decode_files(self, bufs):
-        """decode_files with this detector's decoders"""
-        return decode_files(bufs, self.png_decoder, self.jpeg_decoder)
+        super().__init__(Engine(self.program, device=device_index, precision=precision, max_batch=int(max_batch),
+                                max_h=input_size[0], max_w=input_size[1], conf_thresh=conf_thresh,
+                                nms_thresh=nms_thresh, db_thresh=0.3), device_index, max_batch)
 
     def __call__(self, img, refine_mode=REFINEMASK_INPAINT, keep_undetected_mask=False):
         """reference inference.py:141-178.  One native call (`ctd_detect_page`): letterbox (cv2-exact INTER_LINEAR) +
@@ -185,126 +157,25 @@ class TextDetector:
         gives, never copied to the host; blk_list stays the host TextBlock list.  A page's tensors are views into one
         allocation of that page's own, complete when yielded, and marked as used on the current stream; like any
         tensor made on another stream, call `record_stream` before using one on a different stream."""
-        th = 0
-        if textheight is not None:
-            th = _check_textheight(textheight)
-            if th < 2:
-                raise ValueError("textheight must be at least 2 px, got %r" % (textheight,))
-        return self._stream(imgs, refine_mode, keep_undetected_mask, th, bool(device_results))
-
-    def _stream(self, imgs, refine_mode, keep_undetected_mask, th, device_results):
+        th = 0 if textheight is None else check_textheight(textheight)
         net_h, net_w = self.input_size
-        inflight = deque()   # slots in submission order
-        free = [0, 1]
 
-        def submit(batch, events):
-            batch = self._decode_batch(batch)
-            if not free:
-                yield from self._collect(inflight, free)
-            slot = free.pop(0)
-            self.net.submit_pages(slot, batch, net_h, net_w, refine_mode, keep_undetected_mask, th, events,
-                                  device_results)
-            inflight.append(slot)
-
-        try:
-            batch, events = [], []
+        def records():
             for idx, img in enumerate(imgs):
-                if is_encoded(img):
-                    page = _Encoded(idx, img)   # decoded with its batch (_decode_batch)
-                else:
-                    page = check_page(img, self.device_index)
-                batch.append(page)
-                events.append(_page_ready_event(page))
-                if len(batch) < self.max_batch:
-                    continue
-                yield from submit(batch, events)
-                batch, events = [], []
-            if batch:
-                yield from submit(batch, events)
-            while inflight:
-                yield from self._collect(inflight, free)
-        finally:
-            while inflight:   # an error or an abandoned generator: leave the engine with no batch in flight
-                slot = inflight.popleft()
-                try:
-                    self.net.collect_pages(slot, discard=True)
-                except Exception:
-                    pass
+                # an encoded page is decoded with its batch
+                page = _Encoded(idx, img) if is_encoded(img) else check_page(img, self.device_index)
+                yield (idx, page, _page_ready_event(page))
 
-    def _decode_batch(self, batch):
-        """the batch with its encoded pages replaced by their decoded pages (_decode_files): CUDA tensors for the pages
-        decoded on the GPU, complete when decode returns, numpy pages for the others"""
-        enc = [i for i, p in enumerate(batch) if isinstance(p, _Encoded)]
-        if not enc:
-            return batch
-        bufs = [read_encoded(batch[i].src) for i in enc]
-        pages = self._decode_files([b for b, _path in bufs])
-        batch = list(batch)
-        for i, (_b, path), page in zip(enc, bufs, pages):
-            if page is None:
-                raise ValueError("page %d%s could not be decoded (cv2.imdecode returns None)"
-                                 % (batch[i].index, "" if path is None else " (%s)" % path))
-            batch[i] = page if getattr(page, "is_cuda", False) else check_page(page, self.device_index)
-        return batch
+        def submit(slot, batch):
+            self.net.submit_pages(slot, [b[1] for b in batch], net_h, net_w, refine_mode, keep_undetected_mask, th,
+                                  [b[2] for b in batch], bool(device_results))
 
-    def _collect(self, inflight, free):
-        slot = inflight.popleft()
-        pages = self.net.collect_pages(slot)
-        free.append(slot)
-        for mask, mask_refined, rec, lines, dist, *crops in pages:
-            yield (mask, mask_refined, blocks_from_records(rec, lines, dist)) + tuple(crops)
+        def collect(slot, _token, discard):
+            pages = self.net.collect_pages(slot, discard=discard)
+            if discard:
+                return None
+            return [(mask, mask_refined, blocks_from_records(rec, lines, dist)) + tuple(crops)
+                    for mask, mask_refined, rec, lines, dist, *crops in pages]
 
-
-def decode_files(bufs, png_decoder, jpeg_decoder):
-    """encoded files (1-D np.uint8 arrays) -> their pages in input order: files with the PNG signature through
-    png_decoder() (a function returning a PngDecoder), every other file through jpeg_decoder() (baseline JPEGs on the
-    GPU, the rest by cv2); each page is a CUDA tensor or what cv2.imdecode(buf, IMREAD_COLOR) returns.  A decoder is
-    asked for only when a file goes to it."""
-    pngs = [i for i, b in enumerate(bufs) if is_png(b)]
-    others = [i for i, b in enumerate(bufs) if not is_png(b)]
-    out = [None] * len(bufs)
-    for idx, dec in ((pngs, png_decoder), (others, jpeg_decoder)):
-        if idx:
-            for i, page in zip(idx, dec().decode([bufs[i] for i in idx])):
-                out[i] = page
-    return out
-
-
-def check_page(img, device_index=None):
-    """A page as TextDetector's batch calls take it: u8 BGR [h][w][3] with h, w >= 1, else ValueError.  A CUDA tensor
-    (torch.uint8 [h][w][3], any strides) is returned as it is; with a device_index it must be on that GPU.  Anything
-    else, CPU tensors included, goes through np.asarray and comes back as a C-contiguous array."""
-    if getattr(img, "is_cuda", False):
-        if img.dtype != _torch().uint8 or img.dim() != 3 or img.shape[2] != 3 or img.shape[0] < 1 or img.shape[1] < 1:
-            raise ValueError("a page must be a uint8 tensor of shape [h][w][3], got %s %s"
-                             % (img.dtype, tuple(img.shape)))
-        if device_index is not None and img.device.index != device_index:
-            raise ValueError("a CUDA page must be on the detector's device cuda:%d, got %s" % (device_index, img.device))
-        return img
-    a = np.asarray(img)
-    if a.dtype != np.uint8 or a.ndim != 3 or a.shape[2] != 3 or a.shape[0] < 1 or a.shape[1] < 1:
-        raise ValueError("a page must be a uint8 array of shape [h][w][3], got %s %s" % (a.dtype, a.shape))
-    return np.ascontiguousarray(a)
-
-
-class _Encoded:
-    """an encoded page of a stream, with its index in the stream, until its batch is decoded"""
-    __slots__ = ("index", "src")
-
-    def __init__(self, index, src):
-        self.index, self.src = index, src
-
-
-def _page_ready_event(page):
-    """for a CUDA page: an event recorded on its device's current torch stream (the engine waits for it); else None"""
-    if not getattr(page, "is_cuda", False):
-        return None
-    torch = _torch()
-    ev = torch.cuda.Event()
-    ev.record(torch.cuda.current_stream(page.device))
-    return ev
-
-
-def _torch():
-    import torch
-    return torch
+        decoded = lambda rec, page, what: (rec[0], page, rec[2])
+        return self._pipeline(records(), lambda batch: self._decode(batch, decoded), submit, collect)

@@ -15,10 +15,10 @@ import numpy as np
 
 from . import binding
 from .binding import CtdError
-from .inference import REFINEMASK_INPAINT, _Encoded, _page_ready_event, _torch
+from .inference import REFINEMASK_INPAINT
 from .jpeg import is_encoded
-from .kernel_jobs import KernelsOnlyJob, checked_page
-from .textblock import _check_textheight, blocks_from_records
+from .kernel_jobs import KernelsOnlyJob, _Encoded, _page_ready_event, _torch, checked_page
+from .textblock import blocks_from_records, check_textheight
 
 
 def workspace_rows(net_h, net_w):
@@ -153,11 +153,7 @@ class PostProcessor(KernelsOnlyJob):
         input_size, raises ValueError naming the item before its batch reaches the GPU (an encoded page: once its batch
         is decoded).  A NaN or inf in an output fails its batch with a ValueError naming the item when the batch is
         collected."""
-        th = 0
-        if textheight is not None:
-            th = _check_textheight(textheight)
-            if th < 2:
-                raise ValueError("textheight must be at least 2 px, got %r" % (textheight,))
+        th = 0 if textheight is None else check_textheight(textheight)
         return self._stream(items, refine_mode, bool(keep_undetected_mask), th, bool(device_results))
 
     def _stream(self, items, refine_mode, keep, th, device_results):

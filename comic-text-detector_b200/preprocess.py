@@ -14,9 +14,9 @@ import threading
 import numpy as np
 
 from .binding import PRE_F16_NCHW, PRE_F32_NCHW, PRE_U8_NHWC
-from .inference import REFINEMASK_INPAINT, _Encoded, _torch, letterbox_geometry
+from .inference import REFINEMASK_INPAINT, letterbox_geometry
 from .jpeg import is_encoded
-from .kernel_jobs import KernelsOnlyJob, checked_page
+from .kernel_jobs import KernelsOnlyJob, _Encoded, _torch, checked_page
 from .postprocess import PostProcessor, check_plan
 
 

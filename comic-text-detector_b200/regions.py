@@ -10,20 +10,11 @@ crop of a batch is cut in one GPU launch, from host pages uploaded once or from 
 import numpy as np
 
 from . import binding
-from .inference import _Encoded, _page_ready_event
 from .jpeg import is_encoded
-from .kernel_jobs import KernelsOnlyJob, checked_page
-from .textblock import LANGCLS2IDX, _check_textheight
+from .kernel_jobs import KernelsOnlyJob, _Encoded, _page_ready_event, checked_page
+from .textblock import LANGCLS2IDX, check_textheight
 
 MAX_SIDE = 32767   # ctd_region_plan takes pages with both sides below this
-
-
-def check_textheight(textheight):
-    """textheight as an int >= 2, else ValueError"""
-    th = _check_textheight(textheight)
-    if th < 2:
-        raise ValueError("textheight must be at least 2 px, got %r" % (textheight,))
-    return th
 
 
 def line_records(blk_list, what=""):

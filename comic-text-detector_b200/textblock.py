@@ -200,6 +200,14 @@ def _check_textheight(textheight):
     raise ValueError("textheight must be an integer number of pixels, got %r" % (textheight,))
 
 
+def check_textheight(textheight):
+    """textheight as an int >= 2, else ValueError: the textheight of the batched streams"""
+    th = _check_textheight(textheight)
+    if th < 2:
+        raise ValueError("textheight must be at least 2 px, got %r" % (textheight,))
+    return th
+
+
 def region_lines(blk_list, line_index=None):
     """REGION_LINE_DTYPE records for every line of every block (or line `line_index` of each), and (block, line) of
     each record"""

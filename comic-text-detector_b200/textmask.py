@@ -16,9 +16,9 @@ import operator
 import numpy as np
 
 from . import binding
-from .inference import REFINEMASK_INPAINT, _Encoded, _page_ready_event, _torch
+from .inference import REFINEMASK_INPAINT
 from .jpeg import is_encoded
-from .kernel_jobs import KernelsOnlyJob, checked_page
+from .kernel_jobs import KernelsOnlyJob, _Encoded, _page_ready_event, _torch, checked_page
 from .textblock import _region_engine
 
 

@@ -151,9 +151,9 @@ def main():
             outs = {}
             for name in ("annotations_cv2_decode", "annotations_gpu_decode"):
                 if name == "annotations_cv2_decode":
-                    det._decode_files = lambda bufs: det.jpeg_decoder().decode(bufs)
+                    det.png_decoder = det.jpeg_decoder   # PNG files to the JPEG decoder, which hands them to cv2
                 else:
-                    del det._decode_files
+                    del det.png_decoder
                 dst = os.path.join(tmp, name)
 
                 def run():
