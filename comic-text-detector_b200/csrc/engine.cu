@@ -63,7 +63,7 @@ extern "C" void ctd_destroy(ctd_handle* h) {
   cudaFree(h->d_wsplit);
   cudaFree(h->d_blob); cudaFree(h->d_pages); cudaFree(h->d_blks); cudaFree(h->d_mask); cudaFree(h->d_mask_u8);
   cudaFree(h->d_lines); cudaFree(h->d_bitmap); cudaFree(h->d_labels);
-  cudaFree(h->d_ccl_scratch); cudaFree(h->d_nms_ws); cudaFree(h->d_segrep_scratch);
+  cudaFree(h->d_ccl_scratch); cudaFree(h->d_nms_ws); cudaFree(h->d_segrep_scratch); cudaFree(h->d_segrep_rows);
   h->refine_scratch.release(); h->cc_scratch.release(); h->io_scratch.release(); h->in_stage.release();
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
@@ -255,6 +255,12 @@ extern "C" int ctd_create(ctd_handle** out, const ctd_config* cfg, const ctd_op*
   }
   CKC(cudaMalloc(&h->d_ccl_scratch, px * 4 * 3));
   CKC(cudaMalloc(&h->d_segrep_scratch, segrep_scratch_bytes(int(nb), int(mh), int(mw), 1000)));
+  {
+    // n x h of the largest launch: a batch, or one ctd_seg_represent map of up to 2048 rows
+    const size_t rows_bytes = std::max(nb * mh, size_t(2048)) * 1000 * sizeof(int2);
+    CKC(cudaMalloc(&h->d_segrep_rows, rows_bytes));
+    CKC(cudaMemset(h->d_segrep_rows, 0xff, rows_bytes));
+  }
   const int cap = 4096;
   CKC(cudaMalloc(&h->d_nms_ws, nms_workspace_bytes(int(nb), cap)));
   nms_workspace_bind(h->nms, h->d_nms_ws, int(nb), cap);
@@ -464,11 +470,12 @@ int launch_nms(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt, c
   return CTD_OK;
 }
 
-// DB post-processing: connected components of the bitmap, then the text-line boxes
+// DB post-processing: connected components of the bitmap, then the text-line boxes.  The label plane numbered like
+// OpenCV is built only when ctd_get_db_components asks for it.
 int launch_db_post(ctd_handle* h, int n, int ph, int pw, cudaStream_t s, int* cnt) {
-  CK(ccl_launch(h->d_bitmap, n, ph, pw, h->d_labels, h->d_ccl_scratch, h->d_nlabels, s));
+  CK(ccl_launch(h->d_bitmap, n, ph, pw, h->d_ccl_scratch, h->d_nlabels, s));
   CK(segrep_launch(h->d_bitmap, h->d_lines, size_t(2) * ph * pw, h->d_ccl_scratch, n, ph, pw, 1000, 1.5f,
-                   h->d_segrep_scratch, h->d_line_boxes, h->d_line_scores, h->d_line_count, s));
+                   h->d_segrep_scratch, h->d_segrep_rows, h->d_line_boxes, h->d_line_scores, h->d_line_count, s));
   *cnt += kCclLaunches + kSegrepLaunches;
   return CTD_OK;
 }
@@ -765,7 +772,10 @@ extern "C" int ctd_get_db_components(ctd_handle* h, uint8_t* bitmap, int32_t* la
   NEED_FWD();
   const size_t px = size_t(h->n) * h->ph * h->pw;
   if (bitmap) CK(cudaMemcpyAsync(bitmap, h->d_bitmap, px, cudaMemcpyDeviceToHost, h->stream));
-  if (labels) CK(cudaMemcpyAsync(labels, h->d_labels, px * 4, cudaMemcpyDeviceToHost, h->stream));
+  if (labels) {
+    CK(ccl_number_launch(h->n, h->ph, h->pw, h->d_ccl_scratch, h->d_labels, h->stream));
+    CK(cudaMemcpyAsync(labels, h->d_labels, px * 4, cudaMemcpyDeviceToHost, h->stream));
+  }
   if (n_labels) CK(cudaMemcpyAsync(n_labels, h->d_nlabels, size_t(h->n) * 4, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return CTD_OK;
@@ -790,9 +800,9 @@ extern "C" int ctd_seg_represent(ctd_handle* h, const float* pred, int32_t ih, i
   const size_t px = size_t(ih) * iw;
   CK(cudaMemcpyAsync(h->d_lines, pred, px * 4, cudaMemcpyHostToDevice, h->stream));
   CK(binarize_launch(h->d_lines, px, thresh, h->d_bitmap, h->stream));
-  CK(ccl_launch(h->d_bitmap, 1, ih, iw, h->d_labels, h->d_ccl_scratch, h->d_nlabels, h->stream));
+  CK(ccl_launch(h->d_bitmap, 1, ih, iw, h->d_ccl_scratch, h->d_nlabels, h->stream));
   CK(segrep_launch(h->d_bitmap, h->d_lines, px, h->d_ccl_scratch, 1, ih, iw, 1000, 1.5f, h->d_segrep_scratch,
-                   h->d_line_boxes, h->d_line_scores, h->d_line_count, h->stream));
+                   h->d_segrep_rows, h->d_line_boxes, h->d_line_scores, h->d_line_count, h->stream));
   CK(cudaMemcpyAsync(boxes, h->d_line_boxes, 1000 * 8 * 2, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(scores, h->d_line_scores, 1000 * 4, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaMemcpyAsync(count, h->d_line_count, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -958,8 +968,9 @@ int cc_device(ctd_handle* h, const uint8_t* d_img, int ih, int iw, int stats_cap
   int32_t* d_labels = reinterpret_cast<int32_t*>(base);
   int32_t* d_scr = reinterpret_cast<int32_t*>(base + o_scr);
   int32_t* d_nl = reinterpret_cast<int32_t*>(base + o_nl);
-  CK(ccl_launch(d_img, 1, ih, iw, d_labels, d_scr, d_nl, h->stream));
-  if (stats_cap > 0) CK(ccl_stats_launch(d_labels, ih, iw, d_scr, stats_cap, h->stream));   // scratch is free after ccl_launch
+  CK(ccl_launch(d_img, 1, ih, iw, d_scr, d_nl, h->stream));
+  CK(ccl_number_launch(1, ih, iw, d_scr, d_labels, h->stream));
+  if (stats_cap > 0) CK(ccl_stats_launch(d_labels, ih, iw, d_scr, stats_cap, h->stream));   // scratch is free after the numbering
   CK(cudaMemcpyAsync(n_labels, d_nl, 4, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   if (d_stats) *d_stats = d_scr;

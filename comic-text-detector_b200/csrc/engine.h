@@ -246,6 +246,7 @@ struct ctd_handle {
   int32_t* d_nlabels = nullptr;
   int32_t* d_ccl_scratch = nullptr;
   void* d_segrep_scratch = nullptr;
+  int2* d_segrep_rows = nullptr;   // segrep_launch's row extents, all 0xff between launches
   DevBuf refine_scratch;   // refine_mask on the engine stream
   DevBuf cc_scratch;       // ctd_connected_components: any image size
   DevBuf io_scratch;       // page and mask staging of the stand-alone entry points and ctd_detect_page

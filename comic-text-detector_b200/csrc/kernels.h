@@ -208,10 +208,13 @@ constexpr int kNmsLaunches = 5;   // kernels nms_launch enqueues
 size_t nms_workspace_bytes(int n, int cap);
 void nms_workspace_bind(NmsWorkspace& ws, void* base, int n, int cap);
 
-// 8-connectivity labelling with OpenCV's label numbering; labels i32, n_labels incl. background.
-cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* labels, int32_t* scratch /*3*n*h*w ints*/,
-                       int32_t* n_labels, cudaStream_t s);
-constexpr int kCclLaunches = 8;   // kernels and memsets ccl_launch enqueues
+// 8-connectivity labelling: the first n*h*w ints of scratch get each foreground pixel's root (the raster index of its
+// component's first pixel, -1 on background); n_labels = components + 1 (incl. background).
+cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* scratch /*3*n*h*w ints*/, int32_t* n_labels,
+                       cudaStream_t s);
+constexpr int kCclLaunches = 3;   // kernels ccl_launch enqueues
+// labels i32 numbered like cv2.connectedComponents, from the roots ccl_launch left in the same scratch (which it reuses)
+cudaError_t ccl_number_launch(int n, int h, int w, int32_t* scratch, int32_t* labels, cudaStream_t s);
 // Largest image ccl_launch + ccl_stats_launch label: the kernels index pixels with int and the stats table with
 // 5 ints per label (up to a quarter of the pixels), so 2^28 keeps every index far inside int range.
 constexpr size_t kCclMaxPixels = size_t(1) << 28;
@@ -219,11 +222,13 @@ cudaError_t ccl_stats_launch(const int32_t* labels, int h, int w, int32_t* stats
 
 // SegDetectorRepresenter.boxes_from_bitmap (segrep.cu).  Lf = foreground union-find roots left in the CCL
 // scratch by ccl_launch (first n*h*w ints).  boxes i16 [n][max_cand][4][2], scores f32 [n][max_cand].
+// rows: the per-contour row extents, int2 {min x, max x} [n][max_cand][h]; filled with 0xff bytes once when they are
+// allocated, and left so by every segrep_launch, which resets only the rows its contours reached.
 size_t segrep_scratch_bytes(int n, int h, int w, int max_cand);
 cudaError_t segrep_launch(const uint8_t* bitmap, const float* pred, size_t pred_page_stride, const int* Lf, int n, int h,
-                          int w, int max_cand, float unclip_ratio, void* scratch, int16_t* boxes, float* scores,
-                          int* n_contours, cudaStream_t s);
-constexpr int kSegrepLaunches = 15;   // kernels and memsets segrep_launch enqueues
+                          int w, int max_cand, float unclip_ratio, void* scratch, int2* rows, int16_t* boxes,
+                          float* scores, int* n_contours, cudaStream_t s);
+constexpr int kSegrepLaunches = 14;   // kernels and memsets segrep_launch enqueues
 cudaError_t binarize_launch(const float* pred, size_t count, float thresh, uint8_t* bitmap, cudaStream_t s);
 
 // cv2.resize INTER_LINEAR, uint8, 1 or 3 channels, bit-exact (resize.cu).  src rows are `src_pitch` bytes apart; the

@@ -307,7 +307,8 @@ int refine_undetected(ctd_handle* h, const std::vector<JobPage>& pages, const Pl
   for (int i = 0; i < n; ++i) {
     const JobPage& p = pages[size_t(i)];
     int32_t* d_stats = reinterpret_cast<int32_t*>(base + stats_off[size_t(i)]);
-    CK(ccl_launch(pl.thr + p.off, 1, p.ih, p.iw, d_labels, d_scr, d_nl + i, st));
+    CK(ccl_launch(pl.thr + p.off, 1, p.ih, p.iw, d_scr, d_nl + i, st));
+    CK(ccl_number_launch(1, p.ih, p.iw, d_scr, d_labels, st));
     CK(ccl_stats_launch(d_labels, p.ih, p.iw, d_stats, cap[size_t(i)], st));
   }
   std::vector<int32_t> n_lab(static_cast<size_t>(n));

@@ -401,7 +401,7 @@ constexpr int kScanSeg = 2048;
 // diagonal contacts with the row above are then united.  Afterwards every pixel points at the
 // GLOBAL raster index of its tile-local root (the smallest index of its local component).
 __global__ void __launch_bounds__(1024) ccl_local_kernel(const uint8_t* __restrict__ img, int h, int w,
-                                                         int* __restrict__ Lall, int* __restrict__ keymin_all) {
+                                                         int* __restrict__ Lall, int32_t* __restrict__ n_labels) {
   __shared__ int s[kCclTile * kCclTile];
   const int page = blockIdx.z;
   const int lx = threadIdx.x & 31, ly = threadIdx.x >> 5;
@@ -409,6 +409,7 @@ __global__ void __launch_bounds__(1024) ccl_local_kernel(const uint8_t* __restri
   const bool inb = x < w && y < h;
   const size_t o = size_t(page) * h * w;
   const int l = threadIdx.x;
+  if (blockIdx.x == 0 && blockIdx.y == 0 && l == 0) n_labels[page] = 1;   // the background; pass 3 adds the components
   const bool fg = inb && img[o + size_t(y) * w + x] != 0;
   const unsigned m = __ballot_sync(0xffffffffu, fg);
   const unsigned zeros_below = ~m & ((1u << lx) - 1u);
@@ -434,7 +435,6 @@ __global__ void __launch_bounds__(1024) ccl_local_kernel(const uint8_t* __restri
       g = (blockIdx.y * kCclTile + (r >> 5)) * w + blockIdx.x * kCclTile + (r & 31);
     }
     Lall[o + size_t(y) * w + x] = g;
-    keymin_all[o + size_t(y) * w + x] = INT_MAX;
   }
 }
 
@@ -463,18 +463,32 @@ __global__ void ccl_border_kernel(int h, int w, int* __restrict__ Lall) {
   }
 }
 
-// Pass 3: flatten + key.  The component's first 2x2 block (block-raster order) lies in the block row
-// of its first pixel (= its root); its block column is the minimum over the component's pixels in
-// that block row.  Only those pixels issue an atomic.
-__global__ void ccl_flatten_key_kernel(int h, int w, int* __restrict__ Lall, int* __restrict__ keymin_all) {
+// Pass 3: flatten, and count the components: every root is its component's first raster pixel.
+__global__ void ccl_flatten_kernel(int h, int w, int* __restrict__ Lall, int32_t* __restrict__ n_labels) {
+  const int page = blockIdx.y;
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw = h * w;
+  int* L = Lall + size_t(page) * hw;
+  bool root = false;
+  if (p < hw && L[p] >= 0) {
+    const int r = uf_find(L, p);
+    L[p] = r;  // racing writers all store a valid ancestor; roots are fixed points
+    root = r == p;
+  }
+  const unsigned roots = __ballot_sync(0xffffffffu, root);
+  if (roots && (threadIdx.x & 31) == 0) atomicAdd(&n_labels[page], __popc(roots));
+}
+
+// OpenCV's numbering, on demand (ccl_number_launch), from the flattened roots.
+// Key: the component's first 2x2 block (block-raster order) lies in the block row of its first pixel (= its root);
+// its block column is the minimum over the component's pixels in that block row.  Only those pixels issue an atomic.
+__global__ void ccl_key_kernel(int h, int w, const int* __restrict__ Lall, int* __restrict__ keymin_all) {
   const int page = blockIdx.y;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   const int hw = h * w;
   if (p >= hw) return;
-  int* L = Lall + size_t(page) * hw;
-  if (L[p] < 0) return;
-  const int r = uf_find(L, p);
-  L[p] = r;  // racing writers all store a valid ancestor; roots are fixed points
+  const int r = Lall[size_t(page) * hw + p];
+  if (r < 0) return;
   const int y = p / w, x = p - y * w;
   if ((y >> 1) == ((r / w) >> 1)) atomicMin(&keymin_all[size_t(page) * hw + r], x >> 1);
 }
@@ -528,9 +542,9 @@ __global__ void __launch_bounds__(256) ccl_scan_seg_kernel(int h, int w, int* __
   }
   if (threadIdx.x == 255) segsum[page * nseg + seg] = woff + incl;
 }
-// Pass 5b: exclusive scan of the segment totals, n_labels.  Chunks of 4096 segments (4 consecutive entries per thread,
+// Pass 5b: exclusive scan of the segment totals.  Chunks of 4096 segments (4 consecutive entries per thread,
 // block scan of the per-thread sums) with a running carry, so any segment count works: a 2^28-pixel image has 32768.
-__global__ void __launch_bounds__(1024) ccl_scan_top_kernel(int* __restrict__ segsum, int nseg, int* __restrict__ n_labels) {
+__global__ void __launch_bounds__(1024) ccl_scan_top_kernel(int* __restrict__ segsum, int nseg) {
   __shared__ int part[1024];
   const int page = blockIdx.x;
   int* sgs = segsum + size_t(page) * nseg;
@@ -562,7 +576,6 @@ __global__ void __launch_bounds__(1024) ccl_scan_top_kernel(int* __restrict__ se
     carry += part[1023];
     __syncthreads();   // every thread has read part[1023] before the next chunk overwrites it
   }
-  if (threadIdx.x == 0) n_labels[page] = carry + 1;
 }
 
 __global__ void ccl_relabel_kernel(int h, int w, const int* __restrict__ Lall, const int* __restrict__ keymin_all,
@@ -583,9 +596,20 @@ __global__ void ccl_relabel_kernel(int h, int w, const int* __restrict__ Lall, c
   labels[o + p] = lab;
 }
 
-// scratch: 3 * n*h*w ints (L, keymin, bflag/rank); segment sums live at the tail of the bflag area
-cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* labels, int32_t* scratch, int32_t* n_labels,
-                       cudaStream_t s) {
+// scratch: 3 * n*h*w ints (L, keymin, bflag/rank); ccl_launch uses the first n*h*w
+cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* scratch, int32_t* n_labels, cudaStream_t s) {
+  const int hw = h * w;
+  int* L = scratch;
+  dim3 tgrid((w + kCclTile - 1) / kCclTile, (h + kCclTile - 1) / kCclTile, n);
+  ccl_local_kernel<<<tgrid, 1024, 0, s>>>(img, h, w, L, n_labels);
+  const int nborder = ((w - 1) / kCclTile) * h + ((h - 1) / kCclTile) * w;
+  if (nborder > 0) ccl_border_kernel<<<dim3((nborder + 255) / 256, n), 256, 0, s>>>(h, w, L);
+  ccl_flatten_kernel<<<dim3((hw + 255) / 256, n), 256, 0, s>>>(h, w, L, n_labels);
+  return cudaGetLastError();
+}
+
+// segment sums live at the tail of the bflag area
+cudaError_t ccl_number_launch(int n, int h, int w, int32_t* scratch, int32_t* labels, cudaStream_t s) {
   const int hw = h * w;
   int* L = scratch;
   int* keymin = scratch + size_t(n) * hw;
@@ -595,17 +619,16 @@ cudaError_t ccl_launch(const uint8_t* img, int n, int h, int w, int32_t* labels,
   // per page the bflag area has hw ints but only nb (<= hw/4 + ..) are used: keep segsum after them
   int* segsum = bflag + size_t(n - 1) * hw + nb;  // n*nseg ints, fits: nseg*n <= hw - nb for sane shapes
   if (size_t(n) * nseg > size_t(hw - nb)) return cudaErrorInvalidValue;
-  cudaError_t e = cudaMemset2DAsync(bflag, size_t(hw) * sizeof(int), 0, size_t(nb) * sizeof(int), n, s);
+  // 0x7f7f7f7f: above every block column; every root's own pixel lowers its key
+  cudaError_t e = cudaMemsetAsync(keymin, 0x7f, size_t(n) * hw * sizeof(int), s);
   if (e != cudaSuccess) return e;
-  dim3 tgrid((w + kCclTile - 1) / kCclTile, (h + kCclTile - 1) / kCclTile, n);
-  ccl_local_kernel<<<tgrid, 1024, 0, s>>>(img, h, w, L, keymin);
-  const int nborder = ((w - 1) / kCclTile) * h + ((h - 1) / kCclTile) * w;
-  if (nborder > 0) ccl_border_kernel<<<dim3((nborder + 255) / 256, n), 256, 0, s>>>(h, w, L);
+  e = cudaMemset2DAsync(bflag, size_t(hw) * sizeof(int), 0, size_t(nb) * sizeof(int), n, s);
+  if (e != cudaSuccess) return e;
   dim3 grid((hw + 255) / 256, n);
-  ccl_flatten_key_kernel<<<grid, 256, 0, s>>>(h, w, L, keymin);
+  ccl_key_kernel<<<grid, 256, 0, s>>>(h, w, L, keymin);
   ccl_markfirst_kernel<<<grid, 256, 0, s>>>(h, w, L, keymin, bflag);
   ccl_scan_seg_kernel<<<dim3(nseg, n), 256, 0, s>>>(h, w, bflag, segsum, nseg);
-  ccl_scan_top_kernel<<<n, 1024, 0, s>>>(segsum, nseg, n_labels);
+  ccl_scan_top_kernel<<<n, 1024, 0, s>>>(segsum, nseg);
   ccl_relabel_kernel<<<grid, 256, 0, s>>>(h, w, L, keymin, bflag, segsum, nseg, labels);
   return cudaGetLastError();
 }

@@ -94,13 +94,16 @@ __global__ void bg_border_kernel(int h, int w, int* __restrict__ Lall) {
     if (L[p] >= 0 && L[p - w] >= 0) uf_union_g(L, p, p - w);
   }
 }
-__global__ void bg_flatten_kernel(int h, int w, int* __restrict__ Lall) {
+// flatten; every root marks its parent "not decided" (-1)
+__global__ void bg_flatten_kernel(int h, int w, int* __restrict__ Lall, int* __restrict__ parent_all) {
   const int page = blockIdx.y;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= h * w) return;
   int* L = Lall + size_t(page) * h * w;
   if (L[p] < 0) return;
-  L[p] = uf_find_g(L, p);
+  const int r = uf_find_g(L, p);
+  L[p] = r;
+  if (r == p) parent_all[size_t(page) * h * w + p] = -1;
 }
 
 // ---- component tree ---------------------------------------------------------------------------
@@ -108,9 +111,15 @@ __global__ void bg_flatten_kernel(int h, int w, int* __restrict__ Lall) {
 constexpr int kFrame = -2;
 
 // bg components touching the frame are "outside": mark their roots
-__global__ void mark_outside_kernel(int h, int w, const int* __restrict__ Lb_all, int* __restrict__ parent_all) {
+// (and reset the contours' y ranges)
+__global__ void mark_outside_kernel(int h, int w, const int* __restrict__ Lb_all, int* __restrict__ parent_all,
+                                    int* __restrict__ c_yrange, int max_cand) {
   const int page = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < max_cand) {
+    c_yrange[(page * max_cand + i) * 2] = INT_MAX;
+    c_yrange[(page * max_cand + i) * 2 + 1] = -1;
+  }
   const int per = 2 * w + 2 * h;
   if (i >= per) return;
   int x, y;
@@ -123,75 +132,77 @@ __global__ void mark_outside_kernel(int h, int w, const int* __restrict__ Lb_all
   if (r >= 0) parent_all[o + r] = kFrame;
 }
 
-// per pixel: roots get their parent, zeroed accumulators and a discovery flag
-__global__ void roots_kernel(int h, int w, const int* __restrict__ Lf_all, const int* __restrict__ Lb_all,
-                             int* __restrict__ parent_all, int* __restrict__ flag_all, double* __restrict__ own_sum,
-                             int* __restrict__ own_cnt, double* __restrict__ tot_sum, int* __restrict__ tot_cnt,
-                             double* __restrict__ ring_sum, int* __restrict__ ring_cnt) {
-  const int page = blockIdx.y;
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  const int hw = h * w;
-  if (p >= hw) return;
-  const size_t o = size_t(page) * hw;
-  const int lf = Lf_all[o + p], lb = Lb_all[o + p];
-  int flag = 0;
-  if (lf == p) {
-    const int x = p % w;
-    int par = kFrame;
-    if (x > 0) {
-      const int q = Lb_all[o + p - 1];  // bg (p is the component's first raster pixel)
-      par = (q >= 0 && parent_all[o + q] != kFrame) ? q : kFrame;
-    }
-    parent_all[o + p] = par;
-    flag = 1;
-  } else if (lb == p) {
-    if (parent_all[o + p] != kFrame) {  // a hole: its left neighbour is foreground
-      parent_all[o + p] = Lf_all[o + p - 1];
-      flag = 1;
-    }
+// ---- discovery order -> contour ids (OpenCV returns the reverse discovery order) ----------------
+// The roots of a page are numbered in raster order.  A 256-thread CTA owns a segment of kSeg pixels and sweeps it in
+// kSeg / 256 coalesced steps; roots_kernel counts the segment's roots, flag_scan_top scans the counts, and
+// assign_cid_kernel ranks each root inside its segment.
+constexpr int kSeg = 2048;
+
+// a CTA-wide exclusive prefix of one flag per thread (raster order = thread order); returns the CTA's total
+__device__ __forceinline__ int cta_flag_prefix(bool flag, int* excl, int* wsum) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned b = __ballot_sync(0xffffffffu, flag);
+  __syncthreads();   // wsum of the previous call has been read
+  if (lane == 0) wsum[warp] = __popc(b);
+  __syncthreads();
+  int off = 0, tot = 0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    off += k < warp ? wsum[k] : 0;
+    tot += wsum[k];
   }
-  if (lf == p || lb == p) {
-    own_sum[o + p] = 0.0; own_cnt[o + p] = 0;
-    tot_sum[o + p] = 0.0; tot_cnt[o + p] = 0;
-    ring_sum[o + p] = 0.0; ring_cnt[o + p] = 0;
-  }
-  flag_all[o + p] = flag;
+  *excl = off + __popc(b & ((1u << lane) - 1u));
+  return tot;
 }
 
-// ---- discovery order -> contour ids (OpenCV returns the reverse discovery order) ----------------
-constexpr int kSeg = 2048;
-__global__ void __launch_bounds__(256) flag_scan_seg_kernel(int hw, int* __restrict__ flag_all, int* __restrict__ segsum, int nseg) {
+// per pixel: roots get their parent and zeroed accumulators; per segment: the count of discovery points (the first
+// pixels of foreground components and of holes)
+__global__ void __launch_bounds__(256) roots_kernel(int h, int w, const int* __restrict__ Lf_all, const int* __restrict__ Lb_all,
+                                                    int* __restrict__ parent_all, double* __restrict__ own_sum,
+                                                    int* __restrict__ own_cnt, double* __restrict__ tot_sum,
+                                                    int* __restrict__ tot_cnt, double* __restrict__ ring_sum,
+                                                    int* __restrict__ ring_cnt, int* __restrict__ segsum, int nseg) {
   __shared__ int wsum[8];
   const int page = blockIdx.y, seg = blockIdx.x;
-  int* f = flag_all + size_t(page) * hw + size_t(seg) * kSeg;
-  const int base = seg * kSeg;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int v[8], t = 0;
-  const int i0 = threadIdx.x * 8;
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    v[e] = (base + i0 + e < hw) ? f[i0 + e] : 0;
-    t += v[e];
+  const int hw = h * w;
+  const size_t o = size_t(page) * hw;
+  int cnt = 0;
+  for (int e = 0; e < kSeg / 256; ++e) {
+    const int p = seg * kSeg + e * 256 + threadIdx.x;
+    if (p >= hw) break;
+    const int lf = Lf_all[o + p], lb = Lb_all[o + p];
+    if (lf == p) {
+      const int x = p % w;
+      int par = kFrame;
+      if (x > 0) {
+        const int q = Lb_all[o + p - 1];  // bg (p is the component's first raster pixel)
+        par = (q >= 0 && parent_all[o + q] != kFrame) ? q : kFrame;
+      }
+      parent_all[o + p] = par;
+      ++cnt;
+    } else if (lb == p) {
+      if (parent_all[o + p] != kFrame) {  // a hole: its left neighbour is foreground
+        parent_all[o + p] = Lf_all[o + p - 1];
+        ++cnt;
+      }
+    }
+    if (lf == p || lb == p) {
+      own_sum[o + p] = 0.0; own_cnt[o + p] = 0;
+      tot_sum[o + p] = 0.0; tot_cnt[o + p] = 0;
+      ring_sum[o + p] = 0.0; ring_cnt[o + p] = 0;
+    }
   }
-  int incl = t;
 #pragma unroll
-  for (int off = 1; off < 32; off <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, incl, off);
-    if (lane >= off) incl += u;
-  }
-  if (lane == 31) wsum[warp] = incl;
+  for (int off = 16; off > 0; off >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, off);
+  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = cnt;
   __syncthreads();
-  int woff = 0;
-  for (int k = 0; k < warp; ++k) woff += wsum[k];
-  int run = woff + incl - t;
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    // keep the flag in bit 30 so that the next kernel still knows which pixels are discovery points
-    if (base + i0 + e < hw) f[i0 + e] = run | (v[e] << 30);
-    run += v[e];
+  if (threadIdx.x == 0) {
+    int t = 0;
+    for (int k = 0; k < 8; ++k) t += wsum[k];
+    segsum[page * nseg + seg] = t;
   }
-  if (threadIdx.x == 255) segsum[page * nseg + seg] = woff + incl;
 }
+
 __global__ void __launch_bounds__(1024) flag_scan_top_kernel(int* __restrict__ segsum, int nseg, int* __restrict__ total) {
   // exclusive scan of up to 4096 segment sums: 4 consecutive entries per thread, block scan of the per-thread sums
   __shared__ int part[1024];
@@ -222,40 +233,53 @@ __global__ void __launch_bounds__(1024) flag_scan_top_kernel(int* __restrict__ s
   }
   if (threadIdx.x == 1023) total[page] = part[1023];
 }
-// cid[root pixel] = position in OpenCV's list if < max_candidates else -1; contour table
-__global__ void assign_cid_kernel(int h, int w, const int* __restrict__ Lf_all, int* __restrict__ flag_all,
-                                  const int* __restrict__ segoff, int nseg, const int* __restrict__ total, int max_cand,
-                                  int* __restrict__ c_root, int* __restrict__ rowmin, int* __restrict__ rowmax) {
-  const int page = blockIdx.y;
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+// each discovery point (a root whose parent roots_kernel decided: every foreground root, and the background roots that
+// are not outside) gets its discovery rank; cid[root] = its position in OpenCV's list if < max_candidates else -1,
+// written at roots only; the contour table; the list of roots in discovery order, for tree_kernel
+__global__ void __launch_bounds__(256) assign_cid_kernel(int h, int w, const int* __restrict__ Lf_all,
+                                                         const int* __restrict__ Lb_all, const int* __restrict__ parent_all,
+                                                         const int* __restrict__ segoff, int nseg, const int* __restrict__ total,
+                                                         int max_cand, int* __restrict__ cid_all, int* __restrict__ c_root,
+                                                         int* __restrict__ root_list) {
+  __shared__ int wsum[8];
+  const int page = blockIdx.y, seg = blockIdx.x;
   const int hw = h * w;
-  if (p >= hw) return;
   const size_t o = size_t(page) * hw;
-  const int f = flag_all[o + p];
-  int cid = -1;
-  if (f & (1 << 30)) {
-    const int rank = segoff[page * nseg + p / kSeg] + (f & ((1 << 30) - 1));
-    const int c = total[page] - 1 - rank;
-    if (c < max_cand) {
-      cid = c;
-      // bit 31 of the table entry: 1 = hole contour
-      c_root[page * max_cand + c] = (Lf_all[o + p] == p) ? p : (p | int(0x80000000u));
+  int base = segoff[page * nseg + seg];
+  for (int e = 0; e < kSeg / 256; ++e) {
+    const int p = seg * kSeg + e * 256 + threadIdx.x;
+    if (seg * kSeg + e * 256 >= hw) break;   // CTA-uniform
+    bool fg_root = false, flag = false;
+    if (p < hw) {
+      fg_root = Lf_all[o + p] == p;
+      flag = fg_root || (Lb_all[o + p] == p && parent_all[o + p] != kFrame);
     }
+    int excl;
+    const int tot = cta_flag_prefix(flag, &excl, wsum);
+    if (flag) {
+      const int rank = base + excl;
+      root_list[o + rank] = p;
+      const int c = total[page] - 1 - rank;
+      int cid = -1;
+      if (c < max_cand) {
+        cid = c;
+        // bit 31 of the table entry: 1 = hole contour
+        c_root[page * max_cand + c] = fg_root ? p : (p | int(0x80000000u));
+      }
+      cid_all[o + p] = cid;
+    }
+    base += tot;
   }
-  flag_all[o + p] = cid;  // the flag array now holds contour ids at root pixels
-  (void)rowmin; (void)rowmax;
 }
-__global__ void rows_init_kernel(int* __restrict__ rowmin, int* __restrict__ rowmax, size_t n, int* __restrict__ c_yrange,
-                                 size_t ncont) {
-  const size_t i = blockIdx.x * size_t(blockDim.x) + threadIdx.x;
-  if (i < n) {
-    rowmin[i] = INT_MAX;
-    rowmax[i] = -1;
-  }
-  if (i < ncont) {
-    c_yrange[2 * i] = INT_MAX;
-    c_yrange[2 * i + 1] = -1;
-  }
+// Every row a contour's pixels reach lies in its y range: reset those rows to all ones (min 0xffffffff as unsigned,
+// max -1), so that the next launch finds the whole rows area reset without clearing n x max_cand x h entries.
+__global__ void rows_clear_kernel(int h, int max_cand, const int* __restrict__ total, const int* __restrict__ c_yrange,
+                                  int2* __restrict__ rows) {
+  const int page = blockIdx.y, c = blockIdx.x;
+  if (c >= total[page]) return;
+  const int y0 = c_yrange[(page * max_cand + c) * 2], y1 = c_yrange[(page * max_cand + c) * 2 + 1];
+  int2* r = rows + (size_t(page) * max_cand + c) * h;
+  for (int y = y0 + int(threadIdx.x); y <= y1; y += blockDim.x) r[y] = make_int2(-1, -1);
 }
 
 // ---- per-pixel accumulation ----------------------------------------------------------------------
@@ -265,8 +289,8 @@ __global__ void accumulate_kernel(int h, int w, const float* __restrict__ pred_a
                                   const int* __restrict__ Lf_all, const int* __restrict__ Lb_all,
                                   const int* __restrict__ parent_all, const int* __restrict__ cid_all,
                                   double* __restrict__ own_sum, int* __restrict__ own_cnt, double* __restrict__ ring_sum,
-                                  int* __restrict__ ring_cnt, int* __restrict__ rowmin, int* __restrict__ rowmax,
-                                  int* __restrict__ c_yrange, int max_cand) {
+                                  int* __restrict__ ring_cnt, int2* __restrict__ rows, int* __restrict__ c_yrange,
+                                  int max_cand) {
   const int page = blockIdx.y;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   const int hw = h * w;
@@ -315,8 +339,8 @@ __global__ void accumulate_kernel(int h, int w, const float* __restrict__ pred_a
       if (cid >= 0) {
         const int last = 31 - __clz(peers);
         const size_t ro = (size_t(page) * max_cand + cid) * h + y;
-        atomicMin(&rowmin[ro], x);                  // the leader is the left-most peer
-        atomicMax(&rowmax[ro], x + (last - lane));
+        atomicMin(reinterpret_cast<unsigned*>(&rows[ro].x), unsigned(x));   // the leader is the left-most peer
+        atomicMax(&rows[ro].y, x + (last - lane));
         atomicMin(&c_yrange[(page * max_cand + cid) * 2], y);
         atomicMax(&c_yrange[(page * max_cand + cid) * 2 + 1], y);
       }
@@ -345,8 +369,8 @@ __global__ void accumulate_kernel(int h, int w, const float* __restrict__ pred_a
       const int c2 = cid_all[o + q];
       if (c2 >= 0) {
         const size_t ro = (size_t(page) * max_cand + c2) * h + y;
-        atomicMin(&rowmin[ro], x);
-        atomicMax(&rowmax[ro], x);
+        atomicMin(reinterpret_cast<unsigned*>(&rows[ro].x), unsigned(x));
+        atomicMax(&rows[ro].y, x);
         atomicMin(&c_yrange[(page * max_cand + c2) * 2], y);
         atomicMax(&c_yrange[(page * max_cand + c2) * 2 + 1], y);
       }
@@ -354,17 +378,15 @@ __global__ void accumulate_kernel(int h, int w, const float* __restrict__ pred_a
   }
 }
 
-// every node adds its own sums to itself and to all its ancestors
-__global__ void tree_kernel(int h, int w, const int* __restrict__ Lf_all, const int* __restrict__ Lb_all,
+// every node (a root of root_list) adds its own sums to itself and to all its ancestors
+__global__ void tree_kernel(int h, int w, const int* __restrict__ root_list, const int* __restrict__ total,
                             const int* __restrict__ parent_all, const double* __restrict__ own_sum,
                             const int* __restrict__ own_cnt, double* __restrict__ tot_sum, int* __restrict__ tot_cnt) {
   const int page = blockIdx.y;
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  const int hw = h * w;
-  if (p >= hw) return;
-  const size_t o = size_t(page) * hw;
-  const bool root = Lf_all[o + p] == p || (Lb_all[o + p] == p && parent_all[o + p] != kFrame);
-  if (!root) return;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total[page]) return;
+  const size_t o = size_t(page) * h * w;
+  const int p = root_list[o + i];
   const double s = own_sum[o + p];
   const int c = own_cnt[o + p];
   int a = p;
@@ -480,8 +502,8 @@ __global__ void __launch_bounds__(1024) contour_order_kernel(int max_cand, const
 constexpr int kContourWarps = 4;
 template <int CAP>
 __global__ void __launch_bounds__(32 * kContourWarps) contour_kernel(int h, int w, int max_cand, const int* __restrict__ total,
-                                                     const int* __restrict__ c_root, const int* __restrict__ rowmin,
-                                                     const int* __restrict__ rowmax, const int* __restrict__ c_yrange,
+                                                     const int* __restrict__ c_root, const int2* __restrict__ rows,
+                                                     const int* __restrict__ c_yrange,
                                                      const double* __restrict__ tot_sum,
                                                      const int* __restrict__ tot_cnt, const double* __restrict__ ring_sum,
                                                      const int* __restrict__ ring_cnt, ContourScratch* __restrict__ scratch,
@@ -520,8 +542,7 @@ __global__ void __launch_bounds__(32 * kContourWarps) contour_kernel(int h, int 
   const bool is_hole = entry < 0;
   const int root = entry & 0x7fffffff;
   const size_t o = size_t(page) * h * w;
-  const int* rmin = rowmin + (size_t(page) * max_cand + c) * h;
-  const int* rmax = rowmax + (size_t(page) * max_cand + c) * h;
+  const int2* rr = rows + (size_t(page) * max_cand + c) * h;
   // monotone chain over the row extremes; rows are sorted by y, so the chain runs in the transposed
   // plane (x' = y, y' = x) and the result is transposed back (which mirrors the orientation -> reversed).
   // The rows are prefetched 64 at a time by the whole warp (coalesced) and consumed by lane 0.
@@ -532,8 +553,8 @@ __global__ void __launch_bounds__(32 * kContourWarps) contour_kernel(int h, int 
   for (int y0 = y_lo; y0 <= y_hi; y0 += 64) {
     for (int e = lane; e < 64; e += 32) {
       const int y = y0 + e;
-      rbuf[e] = y <= y_hi ? rmin[y] : INT_MAX;
-      rbuf[64 + e] = y <= y_hi ? rmax[y] : -1;
+      rbuf[e] = y <= y_hi ? rr[y].x : INT_MAX;
+      rbuf[64 + e] = y <= y_hi ? rr[y].y : -1;
     }
     __syncwarp();
     if (lane == 0 && !overflow) {
@@ -555,8 +576,8 @@ __global__ void __launch_bounds__(32 * kContourWarps) contour_kernel(int h, int 
   for (int y1 = y_hi; y1 >= y_lo; y1 -= 64) {
     for (int e = lane; e < 64; e += 32) {
       const int y = y1 - e;
-      rbuf[e] = y >= y_lo ? rmin[y] : INT_MAX;
-      rbuf[64 + e] = y >= y_lo ? rmax[y] : -1;
+      rbuf[e] = y >= y_lo ? rr[y].x : INT_MAX;
+      rbuf[64 + e] = y >= y_lo ? rr[y].y : -1;
     }
     __syncwarp();
     if (lane == 0 && !overflow) {
@@ -660,32 +681,30 @@ cudaError_t binarize_launch(const float* pred, size_t count, float thresh, uint8
 
 size_t segrep_scratch_bytes(int n, int h, int w, int max_cand) {
   const size_t hw = size_t(n) * h * w;
-  return hw * 4 * 4            // Lb, parent, flag/cid, own_cnt
+  return hw * 4 * 5            // Lb, parent, cid, root_list, own_cnt
          + hw * 4 * 2          // tot_cnt, ring_cnt
          + hw * 8 * 3          // own_sum, tot_sum, ring_sum
-         + size_t(n) * max_cand * h * 4 * 2   // rowmin, rowmax
          + size_t(n) * max_cand * 20          // c_root, c_yrange, perm, overflow list
          + size_t(n) * 8192 * 4               // segsum (<= 4096 per page) + totals
          + 65536;                             // 256-byte alignment slack of the 17 sub-arrays
 }
 
 cudaError_t segrep_launch(const uint8_t* bitmap, const float* pred, size_t pred_page_stride, const int* Lf, int n, int h,
-                          int w, int max_cand, float unclip_ratio, void* scratch, int16_t* boxes, float* scores,
-                          int* n_contours, cudaStream_t s) {
+                          int w, int max_cand, float unclip_ratio, void* scratch, int2* rows, int16_t* boxes,
+                          float* scores, int* n_contours, cudaStream_t s) {
   const size_t hw = size_t(h) * w, nhw = size_t(n) * hw;
   char* p = static_cast<char*>(scratch);
   auto take = [&](size_t bytes) { char* r = p; p += (bytes + 255) / 256 * 256; return r; };
   int* Lb = reinterpret_cast<int*>(take(nhw * 4));
   int* parent = reinterpret_cast<int*>(take(nhw * 4));
-  int* flag = reinterpret_cast<int*>(take(nhw * 4));
+  int* cid = reinterpret_cast<int*>(take(nhw * 4));
+  int* root_list = reinterpret_cast<int*>(take(nhw * 4));
   int* own_cnt = reinterpret_cast<int*>(take(nhw * 4));
   int* tot_cnt = reinterpret_cast<int*>(take(nhw * 4));
   int* ring_cnt = reinterpret_cast<int*>(take(nhw * 4));
   double* own_sum = reinterpret_cast<double*>(take(nhw * 8));
   double* tot_sum = reinterpret_cast<double*>(take(nhw * 8));
   double* ring_sum = reinterpret_cast<double*>(take(nhw * 8));
-  int* rowmin = reinterpret_cast<int*>(take(size_t(n) * max_cand * h * 4));
-  int* rowmax = reinterpret_cast<int*>(take(size_t(n) * max_cand * h * 4));
   int* c_root = reinterpret_cast<int*>(take(size_t(n) * max_cand * 4));
   int* c_yrange = reinterpret_cast<int*>(take(size_t(n) * max_cand * 8));
   int* perm = reinterpret_cast<int*>(take(size_t(n) * max_cand * 4));
@@ -696,42 +715,39 @@ cudaError_t segrep_launch(const uint8_t* bitmap, const float* pred, size_t pred_
   ContourScratch* cs = nullptr;
   const int nseg = int((hw + kSeg - 1) / kSeg);
   if (nseg > 4096) return cudaErrorInvalidValue;
+  if (max_cand > 1024) return cudaErrorInvalidValue;
 
   dim3 tgrid((w + 31) / 32, (h + 31) / 32, n);
   dim3 grid(unsigned((hw + 255) / 256), n);
-  cudaError_t e = cudaMemsetAsync(parent, 0xff, nhw * 4, s);  // -1 = "not decided"
-  if (e != cudaSuccess) return e;
+  dim3 sgrid(unsigned(nseg), n);
   bg_local_kernel<<<tgrid, 1024, 0, s>>>(bitmap, h, w, Lb);
   const int nborder = ((w - 1) / 32) * h + ((h - 1) / 32) * w;
   if (nborder > 0) bg_border_kernel<<<dim3((nborder + 255) / 256, n), 256, 0, s>>>(h, w, Lb);
-  bg_flatten_kernel<<<grid, 256, 0, s>>>(h, w, Lb);
-  mark_outside_kernel<<<dim3((2 * w + 2 * h + 255) / 256, n), 256, 0, s>>>(h, w, Lb, parent);
-  roots_kernel<<<grid, 256, 0, s>>>(h, w, Lf, Lb, parent, flag, own_sum, own_cnt, tot_sum, tot_cnt, ring_sum, ring_cnt);
-  flag_scan_seg_kernel<<<dim3(nseg, n), 256, 0, s>>>(int(hw), flag, segsum, nseg);
+  bg_flatten_kernel<<<grid, 256, 0, s>>>(h, w, Lb, parent);
+  mark_outside_kernel<<<dim3((max(2 * w + 2 * h, max_cand) + 255) / 256, n), 256, 0, s>>>(h, w, Lb, parent, c_yrange,
+                                                                                          max_cand);
+  roots_kernel<<<sgrid, 256, 0, s>>>(h, w, Lf, Lb, parent, own_sum, own_cnt, tot_sum, tot_cnt, ring_sum, ring_cnt, segsum,
+                                     nseg);
   flag_scan_top_kernel<<<n, 1024, 0, s>>>(segsum, nseg, total);
-  {
-    const size_t nr = size_t(n) * max_cand * h;
-    rows_init_kernel<<<unsigned((nr + 255) / 256), 256, 0, s>>>(rowmin, rowmax, nr, c_yrange, size_t(n) * max_cand);
-  }
-  assign_cid_kernel<<<grid, 256, 0, s>>>(h, w, Lf, flag, segsum, nseg, total, max_cand, c_root, rowmin, rowmax);
-  accumulate_kernel<<<grid, 256, 0, s>>>(h, w, pred, pred_page_stride, Lf, Lb, parent, flag, own_sum, own_cnt, ring_sum,
-                                         ring_cnt, rowmin, rowmax, c_yrange, max_cand);
-  tree_kernel<<<grid, 256, 0, s>>>(h, w, Lf, Lb, parent, own_sum, own_cnt, tot_sum, tot_cnt);
+  assign_cid_kernel<<<sgrid, 256, 0, s>>>(h, w, Lf, Lb, parent, segsum, nseg, total, max_cand, cid, c_root, root_list);
+  accumulate_kernel<<<grid, 256, 0, s>>>(h, w, pred, pred_page_stride, Lf, Lb, parent, cid, own_sum, own_cnt, ring_sum,
+                                         ring_cnt, rows, c_yrange, max_cand);
+  tree_kernel<<<grid, 256, 0, s>>>(h, w, root_list, total, parent, own_sum, own_cnt, tot_sum, tot_cnt);
   constexpr int kCapSmall = 128, kCapLarge = ctdgeom::kMaxHull;
   const size_t sm_small = sizeof(ContourScratchT<kCapSmall>) * kContourWarps, sm_large = sizeof(ContourScratchT<kCapLarge>) * kContourWarps;
   // per device, so set on every launch (cheap; a process may own engines on several GPUs)
   cudaFuncSetAttribute(contour_kernel<kCapLarge>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(sm_large));
-  if (max_cand > 1024) return cudaErrorInvalidValue;
   contour_order_kernel<<<n, 1024, 0, s>>>(max_cand, total, c_yrange, perm);
-  e = cudaMemsetAsync(ovf_count, 0, size_t(n) * 4, s);
+  cudaError_t e = cudaMemsetAsync(ovf_count, 0, size_t(n) * 4, s);
   if (e != cudaSuccess) return e;
   const unsigned cgrid = unsigned((max_cand + kContourWarps - 1) / kContourWarps) * unsigned(n);
   contour_kernel<kCapSmall><<<cgrid, 32 * kContourWarps, sm_small, s>>>(
-      h, w, max_cand, total, c_root, rowmin, rowmax, c_yrange, tot_sum, tot_cnt, ring_sum, ring_cnt, cs, boxes, scores,
+      h, w, max_cand, total, c_root, rows, c_yrange, tot_sum, tot_cnt, ring_sum, ring_cnt, cs, boxes, scores,
       n_contours, w, h, unclip_ratio, perm, n, ovf_count, ovf_list, 0);
   contour_kernel<kCapLarge><<<cgrid, 32 * kContourWarps, sm_large, s>>>(
-      h, w, max_cand, total, c_root, rowmin, rowmax, c_yrange, tot_sum, tot_cnt, ring_sum, ring_cnt, cs, boxes, scores,
+      h, w, max_cand, total, c_root, rows, c_yrange, tot_sum, tot_cnt, ring_sum, ring_cnt, cs, boxes, scores,
       n_contours, w, h, unclip_ratio, perm, n, ovf_count, ovf_list, 1);
+  rows_clear_kernel<<<dim3(max_cand, n), 128, 0, s>>>(h, max_cand, total, c_yrange, rows);
   return cudaGetLastError();
 }
 

@@ -187,7 +187,8 @@ CTD_API int ctd_get_nms_status(ctd_handle* h, int32_t* cand_total, int32_t* cap)
  * (db_utils.py:71-72 and the labelling findContours/connectedComponents imply):
  * bitmap u8 [n][h][w] (0/1), labels i32 [n][h][w] numbered like
  * cv2.connectedComponents(connectivity=8) (0 = background), n_labels i32 [n] (incl. bg).
- * Any pointer may be NULL.                                                                 */
+ * Any pointer may be NULL.  The forward counts the components; the label plane is numbered
+ * by this call, on the engine's stream, only when `labels` is given.                       */
 CTD_API int ctd_get_db_components(ctd_handle* h, uint8_t* bitmap, int32_t* labels, int32_t* n_labels);
 
 /* `SegDetectorRepresenter.__call__` -> `boxes_from_bitmap` (db_utils.py:40-69,123-166) on the shrink map of
