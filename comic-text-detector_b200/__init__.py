@@ -6,7 +6,7 @@ from .binding import Engine, CtdError, load_library, LIB_PATH  # noqa: F401
 from . import binding, multigpu, onnx_model, textblock  # noqa: F401
 from .inference import TextDetector, REFINEMASK_INPAINT, REFINEMASK_ANNOTATION  # noqa: F401
 from .basemodel import TextDetBase  # noqa: F401
-from .jpeg import JpegDecoder, jpeg_probe  # noqa: F401
+from .jpeg import JpegDecoder, JpegEncoder, jpeg_probe  # noqa: F401
 from .png import PngDecoder, PngEncoder, png_probe  # noqa: F401
 from .textmask import MaskRefiner, refine_mask, refine_undetected_mask  # noqa: F401
 from .regions import RegionCropper  # noqa: F401

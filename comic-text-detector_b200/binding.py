@@ -82,6 +82,12 @@ class CtdPngImage(C.Structure):
                 ("stride_c", C.c_int64), ("event", C.c_void_p)]
 
 
+class CtdJpegParams(C.Structure):
+    """ctypes mirror of `ctd_jpeg_params` (include/ctd_b200.h)"""
+    _fields_ = [("quality", C.c_int32), ("sampling", C.c_int32), ("optimize", C.c_int32),
+                ("restart_interval", C.c_int32)]
+
+
 class CtdDevicePage(C.Structure):
     """ctypes mirror of `ctd_device_page` (include/ctd_b200.h)"""
     _fields_ = [("data", C.c_void_p), ("stride_h", C.c_int64), ("stride_w", C.c_int64), ("stride_c", C.c_int64),
@@ -109,7 +115,8 @@ EXPORTS = ["ctd_create", "ctd_destroy", "ctd_last_error", "ctd_forward", "ctd_ge
            "ctd_png_encoder_create", "ctd_png_encoder_destroy", "ctd_png_encode", "ctd_png_probe",
            "ctd_png_decoder_create", "ctd_png_decoder_destroy", "ctd_png_decode", "ctd_png_decoder_stats",
            "ctd_refine_plan", "ctd_submit_refine", "ctd_submit_regions", "ctd_debug_read_slot", "ctd_submit_outputs",
-           "ctd_preprocess_pages", "ctd_submit_outputs_dtype", "ctd_forward_tensor_f16", "ctd_nms_dtype"]
+           "ctd_preprocess_pages", "ctd_submit_outputs_dtype", "ctd_forward_tensor_f16", "ctd_nms_dtype",
+           "ctd_jpeg_encoder_create", "ctd_jpeg_encoder_destroy", "ctd_jpeg_encode"]
 PRE_F32_NCHW, PRE_F16_NCHW, PRE_U8_NHWC = 0, 1, 2   # ctd_pre_format
 DTYPE_F32, DTYPE_F16 = 0, 1   # ctd_dtype
 
@@ -209,6 +216,10 @@ def load_library():
     lib.ctd_png_encoder_destroy.argtypes = [vp]
     lib.ctd_png_encode.argtypes = [vp, C.POINTER(CtdPngImage), i32, vp, vp]
     lib.ctd_png_encoder_destroy.restype = None
+    lib.ctd_jpeg_encoder_create.argtypes = [i32, C.POINTER(vp)]
+    lib.ctd_jpeg_encoder_destroy.argtypes = [vp]
+    lib.ctd_jpeg_encode.argtypes = [vp, C.POINTER(CtdPngImage), C.POINTER(CtdJpegParams), i32, vp, vp]
+    lib.ctd_jpeg_encoder_destroy.restype = None
     lib.ctd_png_probe.argtypes = [vp, C.c_size_t, C.POINTER(CtdPngInfo)]
     lib.ctd_png_decoder_create.argtypes = [i32, i32, C.POINTER(vp)]
     lib.ctd_png_decoder_destroy.argtypes = [vp]

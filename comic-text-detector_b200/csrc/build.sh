@@ -10,7 +10,7 @@ OBJ=${CTD_BUILD_DIR:-_obj}
 OUT=${CTD_BUILD_DIR:-..}/libctd_b200.so
 mkdir -p "$OBJ"
 pids=()
-for f in engine pipeline conv_tc conv_ends simt postproc segrep refine_mk resize gather group region_plan region jpeg_plan jpeg png png_plan png_dec; do
+for f in engine pipeline conv_tc conv_ends simt postproc segrep refine_mk resize gather group region_plan region jpeg_plan jpeg jpeg_enc png png_plan png_dec; do
   [ -f $f.cu ] || [ -f $f.cpp ] || continue
   src=$f.cu; [ -f $src ] || src=$f.cpp
   extra=""

@@ -6,13 +6,24 @@ page for each; every other file (PNG, progressive JPEG, CMYK, a corrupt scan, ..
 host, so each result is exactly what cv2 returns, a numpy page or None.  (PNG files have a GPU decoder of their own,
 png.PngDecoder; TextDetector sends each encoded page to the decoder of its format.)  `jpeg_probe(buf)` is the host marker walk that
 decides which files the GPU takes.
+
+`JpegEncoder.encode(imgs, params)` (csrc/jpeg_enc.cu) writes JPEG files on the GPU, byte for byte what the reference's
+`io_utils.imwrite(path, img, '.jpg')` writes: `cv2.imencode('.jpg', img, params)[1]`, for u8 grey [h][w] or BGR
+[h][w][3] images, numpy arrays or torch.uint8 CUDA tensors of any strides, many in one call.
 """
 import ctypes as C
 import os
 
 import numpy as np
 
-from .binding import CtdError, CtdJpegInfo, load_library
+from .binding import CtdError, CtdJpegInfo, CtdJpegParams, load_library
+
+# cv2.IMWRITE_JPEG_* keys and the IMWRITE_JPEG_SAMPLING_FACTOR_* values
+JPEG_QUALITY, JPEG_PROGRESSIVE, JPEG_OPTIMIZE, JPEG_RST_INTERVAL, JPEG_LUMA_QUALITY, JPEG_CHROMA_QUALITY, \
+    JPEG_SAMPLING_FACTOR = 1, 2, 3, 4, 5, 6, 7
+JPEG_SAMPLINGS = (0x411111, 0x221111, 0x211111, 0x121111, 0x111111)
+_JPEG_KEY_NAMES = {JPEG_PROGRESSIVE: "IMWRITE_JPEG_PROGRESSIVE", JPEG_LUMA_QUALITY: "IMWRITE_JPEG_LUMA_QUALITY",
+                   JPEG_CHROMA_QUALITY: "IMWRITE_JPEG_CHROMA_QUALITY"}
 
 # ctd_jpeg_status (include/ctd_b200.h)
 JPEG_STATUS = ["ok", "not_jpeg", "truncated", "progressive", "arithmetic", "precision", "lossless", "sampling", "color",
@@ -125,3 +136,79 @@ def read_encoded(page):
     if isinstance(page, (str, os.PathLike)):
         return np.fromfile(page, dtype=np.uint8), os.fspath(page)
     return as_buffer(page), None
+
+
+def jpeg_params(i, params):
+    """cv2.imencode's reading of image i's flat [key, value, ...] list, as a CtdJpegParams: quality clamped to
+    [0, 100] (default 95), a sampling value other than the five IMWRITE_JPEG_SAMPLING_FACTOR_* constants taken as 4:2:0
+    (the default), OPTIMIZE clamped to [0, 1], the restart interval clamped to [0, 65535].  PROGRESSIVE,
+    LUMA_QUALITY, CHROMA_QUALITY and every other key raise ValueError naming the image and the key."""
+    p = CtdJpegParams(95, 0x221111, 0, 0)
+    params = list(params)
+    if len(params) % 2:
+        raise ValueError("image %d: JPEG params must be [key, value, ...] pairs, got %d values" % (i, len(params)))
+    for k, v in zip(params[0::2], params[1::2]):
+        k, v = int(k), int(v)
+        if k == JPEG_QUALITY:
+            p.quality = min(max(v, 0), 100)
+        elif k == JPEG_SAMPLING_FACTOR:
+            p.sampling = v if v in JPEG_SAMPLINGS else 0x221111
+        elif k == JPEG_OPTIMIZE:
+            p.optimize = int(v > 0)
+        elif k == JPEG_RST_INTERVAL:
+            p.restart_interval = min(max(v, 0), 65535)
+        else:
+            raise ValueError("image %d: JPEG parameter %s is not supported by the GPU encoder"
+                             % (i, _JPEG_KEY_NAMES.get(k, "key %d" % k)))
+    return p
+
+
+class JpegEncoder:
+    """A GPU JPEG encoder on cuda:device_index with a stream and buffers of its own."""
+
+    def __init__(self, device_index=0):
+        self.lib = load_library()
+        self.device_index = int(device_index)
+        self.h = C.c_void_p()
+        rc = self.lib.ctd_jpeg_encoder_create(self.device_index, C.byref(self.h))
+        if rc != 0:
+            raise CtdError("ctd_jpeg_encoder_create failed (%d): %s" % (rc, self.lib.ctd_last_error(None).decode()))
+
+    def close(self):
+        if getattr(self, "h", None):
+            self.lib.ctd_jpeg_encoder_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def encode(self, imgs, params=None):
+        """imgs: a list of u8 images, each a numpy [h][w] / [h][w][3] array or a torch.uint8 CUDA tensor of those
+        shapes on this encoder's device (any strides: a crop, `chw.permute(1, 2, 0)`).  A CUDA tensor is read after
+        the work already queued on its device's current stream.  params: None, one cv2-style flat list
+        ([cv2.IMWRITE_JPEG_QUALITY, 90, ...]) for every image, or a list of such lists, one per image.  Returns one
+        1-D np.uint8 array per image, equal to `cv2.imencode('.jpg', img, params)[1]`.  Any other input, a side above
+        65500 or an unsupported parameter raises ValueError naming its index, before any GPU work."""
+        from .png import files_from, image_descs
+        n = len(imgs)
+        if params is None:
+            params = []
+        if len(params) and isinstance(params[0], (list, tuple, np.ndarray)):
+            per = list(params)
+            if len(per) != n:
+                raise ValueError("%d parameter lists for %d images" % (len(per), n))
+        else:
+            per = [params] * n
+        prm = (CtdJpegParams * max(n, 1))(*[jpeg_params(i, p) for i, p in enumerate(per)])
+        if n == 0:
+            return []
+        descs, _keep = image_descs(imgs, self.device_index, "JPEG", max_side=65500)
+        files = (C.c_void_p * n)()
+        sizes = (C.c_int64 * n)()
+        rc = self.lib.ctd_jpeg_encode(self.h, descs, prm, n, files, sizes)
+        if rc != 0:
+            raise CtdError("ctd_jpeg_encode failed (%d): %s" % (rc, self.lib.ctd_last_error(None).decode()))
+        return files_from(files, sizes, n)

@@ -23,13 +23,64 @@ PNG_STATUS = ["ok", "not_png", "truncated", "header", "interlaced", "apng", "chu
 PNG_SIGNATURE = b"\x89PNG\r\n\x1a\n"
 
 
-def _check(i, shape, dtype_ok):
+def _check(i, shape, dtype_ok, fmt, max_side):
     if not dtype_ok:
-        raise ValueError("image %d: a PNG image must be uint8" % i)
+        raise ValueError("image %d: a %s image must be uint8" % (i, fmt))
     if len(shape) not in (2, 3) or (len(shape) == 3 and shape[2] != 3):
-        raise ValueError("image %d: a PNG image must be [h][w] or [h][w][3], got shape %s" % (i, tuple(shape)))
+        raise ValueError("image %d: a %s image must be [h][w] or [h][w][3], got shape %s" % (i, fmt, tuple(shape)))
     if 0 in tuple(shape):
-        raise ValueError("image %d: a PNG image must not be empty, got shape %s" % (i, tuple(shape)))
+        raise ValueError("image %d: a %s image must not be empty, got shape %s" % (i, fmt, tuple(shape)))
+    if max_side and max(shape[0], shape[1]) > max_side:
+        raise ValueError("image %d: a %s image has sides of at most %d, got shape %s" % (i, fmt, max_side, tuple(shape)))
+
+
+def image_descs(imgs, device_index, fmt, max_side=None):
+    """`ctd_png_image` descriptors of u8 images for the encoders (PNG and JPEG): numpy arrays, or torch.uint8 CUDA
+    tensors on cuda:device_index of any strides, each tensor with an event recorded on its device's current stream.
+    max_side (None: no limit) bounds both sides.  Returns (descs, keep): `keep` holds what the descriptors point to
+    (and the events) until the call returns.  Any other input raises ValueError naming its index, before an event is
+    recorded."""
+    n = len(imgs)
+    descs = (CtdPngImage * n)()
+    keep = []
+    torch = None
+    for i, img in enumerate(imgs):
+        d = descs[i]
+        if isinstance(img, np.ndarray):
+            _check(i, img.shape, img.dtype == np.uint8, fmt, max_side)
+            a = np.ascontiguousarray(img)
+            keep.append(a)
+            d.data = a.ctypes.data
+            d.on_device = 0
+        else:
+            if torch is None:
+                import torch
+            if not isinstance(img, torch.Tensor):
+                raise ValueError("image %d: expected a numpy array or a torch CUDA tensor, got %s" % (i, type(img)))
+            if not img.is_cuda or img.device.index != device_index:
+                raise ValueError("image %d: a tensor must be on cuda:%d, got %s" % (i, device_index, img.device))
+            _check(i, img.shape, img.dtype == torch.uint8, fmt, max_side)
+            keep.append(img)
+            d.data = img.data_ptr()
+            d.on_device = 1
+            st = img.stride()
+            d.stride_h, d.stride_w = st[0], st[1]
+            d.stride_c = st[2] if img.dim() == 3 else 0
+        d.height, d.width = img.shape[0], img.shape[1]
+        d.channels = 3 if len(img.shape) == 3 else 1
+        d.bit_depth = 8
+    for i, img in enumerate(imgs):
+        if descs[i].on_device:
+            ev = torch.cuda.Event()
+            ev.record(torch.cuda.current_stream(img.device))
+            keep.append(ev)
+            descs[i].event = ev.cuda_event
+    return descs, keep
+
+
+def files_from(files, sizes, n):
+    """copies of the n files an encoder left in its pinned output"""
+    return [np.ctypeslib.as_array(C.cast(files[i], C.POINTER(C.c_uint8)), (sizes[i],)).copy() for i in range(n)]
 
 
 class PngEncoder:
@@ -62,46 +113,13 @@ class PngEncoder:
         n = len(imgs)
         if n == 0:
             return []
-        descs = (CtdPngImage * n)()
-        keep, events = [], []
-        torch = None
-        for i, img in enumerate(imgs):
-            d = descs[i]
-            if isinstance(img, np.ndarray):
-                _check(i, img.shape, img.dtype == np.uint8)
-                a = np.ascontiguousarray(img)
-                keep.append(a)
-                d.data = a.ctypes.data
-                d.on_device = 0
-            else:
-                if torch is None:
-                    import torch
-                if not isinstance(img, torch.Tensor):
-                    raise ValueError("image %d: expected a numpy array or a torch CUDA tensor, got %s" % (i, type(img)))
-                if not img.is_cuda or img.device.index != self.device_index:
-                    raise ValueError("image %d: a tensor must be on cuda:%d, got %s" % (i, self.device_index, img.device))
-                _check(i, img.shape, img.dtype == torch.uint8)
-                keep.append(img)
-                d.data = img.data_ptr()
-                d.on_device = 1
-                st = img.stride()
-                d.stride_h, d.stride_w = st[0], st[1]
-                d.stride_c = st[2] if img.dim() == 3 else 0
-            d.height, d.width = img.shape[0], img.shape[1]
-            d.channels = 3 if len(img.shape) == 3 else 1
-            d.bit_depth = 8
-        for i, img in enumerate(imgs):
-            if descs[i].on_device:
-                ev = torch.cuda.Event()
-                ev.record(torch.cuda.current_stream(img.device))
-                events.append(ev)
-                descs[i].event = ev.cuda_event
+        descs, _keep = image_descs(imgs, self.device_index, "PNG")
         files = (C.c_void_p * n)()
         sizes = (C.c_int64 * n)()
         rc = self.lib.ctd_png_encode(self.h, descs, n, files, sizes)
         if rc != 0:
             raise CtdError("ctd_png_encode failed (%d): %s" % (rc, self.lib.ctd_last_error(None).decode()))
-        return [np.ctypeslib.as_array(C.cast(files[i], C.POINTER(C.c_uint8)), (sizes[i],)).copy() for i in range(n)]
+        return files_from(files, sizes, n)
 
 
 def png_probe(buf):

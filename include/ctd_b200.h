@@ -800,6 +800,35 @@ CTD_API void ctd_png_encoder_destroy(ctd_png_encoder* enc);
 CTD_API int ctd_png_encode(ctd_png_encoder* enc, const ctd_png_image* images, int32_t n, const uint8_t** files,
                            int64_t* sizes);
 
+/* ---- JPEG files encoded on the GPU ------------------------------------------------------
+ * io_utils.imwrite(path, img, '.jpg') writes cv2.imencode('.jpg', img, params).  These entry points encode u8 images
+ * on the GPU to exactly the baseline file cv2.imencode('.jpg', img, params) gives with the libjpeg-turbo OpenCV 4.13
+ * bundles (3.1): BGR input converted by jccolor.c, jcsample.c's downsampling, jpeg_fdct_islow, the reciprocal
+ * quantiser, Annex K.3 or per-image optimal Huffman tables, SOI / APP0 JFIF 1.01 / DQT / SOF0 / DHT / DRI / SOS / EOI
+ * (csrc/jpeg_enc.cu, oracle/jpeg_enc_ref.py).  Images are described by ctd_png_image (channels 1: one grey component;
+ * channels 3: BGR, coded as YCbCr).
+ *
+ * ctd_jpeg_params holds one image's parameters, as cv2 leaves them after clamping: quality 0..100 (0 codes as 1),
+ * sampling one of cv2's IMWRITE_JPEG_SAMPLING_FACTOR_* values (0x411111, 0x221111, 0x211111, 0x121111, 0x111111: the
+ * luma factors H and V in 0xHV1111; a grey image is always 1x1), optimize 0 / nonzero, restart_interval 0..65535 MCUs
+ * (0: none).                                                                                                        */
+typedef struct ctd_jpeg_params {
+  int32_t quality, sampling, optimize, restart_interval;
+} ctd_jpeg_params;
+typedef struct ctd_jpeg_encoder ctd_jpeg_encoder;
+/* An encoder bound to one GPU and one stream of its own; staging, scratch and output buffers grow on demand.  Not
+ * thread-safe; errors via ctd_last_error(NULL).                                                                     */
+CTD_API int ctd_jpeg_encoder_create(int32_t device, ctd_jpeg_encoder** out);
+CTD_API void ctd_jpeg_encoder_destroy(ctd_jpeg_encoder* enc);
+/* Encodes n images at once, image i with params[i].  files[i] / sizes[i] get image i's complete JPEG file in pinned
+ * host memory owned by the encoder, valid until its next call.  Synchronises with the host once, at the end.
+ * CTD_E_INVALID, before any GPU work, for a side < 1 or > 65500, channels other than 1 or 3, bit_depth other than 8,
+ * a parameter out of range, a negative stride or a device image that is not memory of the encoder's GPU;
+ * CTD_E_CAPACITY when the files' worst case (2048 header bytes and 418 bytes per 8x8 block, MCU padding included, per
+ * image) reaches 2^31 bytes in one call.  The output buffer is sized at that worst case.                          */
+CTD_API int ctd_jpeg_encode(ctd_jpeg_encoder* enc, const ctd_png_image* images, const ctd_jpeg_params* params,
+                            int32_t n, const uint8_t** files, int64_t* sizes);
+
 #ifdef __cplusplus
 }
 #endif
